@@ -1,4 +1,4 @@
-// autospeed.cu — the AutoSpeed detector (SURVEY.md 8f rank 4) on the B200 engine pieces, behind the C-ABI of
+// autospeed.cu — the AutoSpeed detector (SURVEY.md 8f rank 4) on the H100 engine pieces, behind the C-ABI of
 // include/vp_b200_autospeed.h.
 //
 // Reference being replaced (paths relative to the reference repo):
@@ -10,7 +10,7 @@
 //             PSABlock, C2PSA, DFL)
 //   C++ twin  VisionPilot/production_release/src/inference/autospeed/tensorrt_engine.cpp (same graph through TensorRT)
 //
-// Every dense contraction runs on the tcgen05 implicit-GEMM convolution of conv_gemm.cu: 3x3 stride 1 / stride 2
+// Every dense contraction runs on the wgmma implicit-GEMM convolution of conv_gemm.cu: 3x3 stride 1 / stride 2
 // (the stride is the tensor map's traversal stride), 1x1, and the PSA attention's two contractions expressed as 1x1
 // "convolutions" whose weight operand is an activation slice (S = Q K^T: weights = the K rows of the qkv tensor;
 // O = P V^T: weights = the transposed V block).  torch.cat / chunk never copy: producers write channel slices of
@@ -399,7 +399,7 @@ struct vp_autospeed {
   }
   void op(const std::string& name, std::function<int(cudaStream_t)> fn) { ops.push_back(std::move(fn)); op_names.push_back(name); }
 
-  // one tcgen05 convolution: in (slice) -> out (slice); w [taps][Cout][Cin] 16-bit (or an activation slice with ldw)
+  // one wgmma convolution: in (slice) -> out (slice); w [taps][Cout][Cin] 16-bit (or an activation slice with ldw)
   int conv(const std::string& name, const ASTens& in, const ASTens& out, int Cout, int taps, int stride, const void* w,
            const float* bias, int act, int mode = VPB_EPI_STORE, const ASTens* res = nullptr, int act2 = ACT_NONE,
            int ldw = 0, int cin = 0) {
@@ -522,7 +522,7 @@ struct ASBuilder {
       e.flops += 2.0 * HW * co * 9;
       e.op(p + ".ctx0", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, nullptr, 0, st, ACT_SILU); });
     }
-    // ctx1: SiLU(conv) * x + x, then SiLU (:224-232) — one tcgen05 conv with the MULADD epilogue and a post activation
+    // ctx1: SiLU(conv) * x + x, then SiLU (:224-232) — one wgmma conv with the MULADD epilogue and a post activation
     ASTens c4 = e.talloc(H, W, C);
     plain(p + ".ctx1", c2, c4, C, 3, ACT_SILU, VPB_EPI_MULADD, &x, ACT_SILU);
     plain(p + ".ctx2", c4, out, cout, 3, ACT_NONE);
@@ -814,7 +814,7 @@ extern "C" int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtyp
   DeviceGuard guard(gpu_id);
   cudaDeviceProp prop;
   VPB_CUDA_OK(cudaGetDeviceProperties(&prop, gpu_id));
-  if (prop.major != 10) { vpb_set_error("vp_autospeed_create: device %d is sm_%d%d; built for sm_100a only", gpu_id, prop.major, prop.minor); return VPB_ERR_CUDA; }
+  if (prop.major != 9 || prop.minor != 0) { vpb_set_error("vp_autospeed_create: device %d is sm_%d%d; built for sm_90a only", gpu_id, prop.major, prop.minor); return VPB_ERR_CUDA; }
   std::unique_ptr<vp_autospeed> e(new vp_autospeed());
   e->gpu_id = gpu_id; e->dtype = dtype == VPB_BF16 ? VPB_BF16 : VPB_F16;
   if (stream) e->stream = static_cast<cudaStream_t>(stream);

@@ -1,6 +1,6 @@
-// common.cuh — sm_100a device-side primitives shared by the vision-pilot kernels.
+// common.cuh — sm_90a device-side primitives shared by the vision-pilot kernels.
 //
-// Thin inline-PTX wrappers only (mbarrier, TMA, tcgen05/TMEM) plus 16-bit
+// Thin inline-PTX wrappers only (mbarrier, TMA, wgmma) plus 16-bit
 // pack/unpack helpers.  Nothing here is generic: every wrapper is the exact
 // form the kernels in this directory issue.
 #pragma once
@@ -16,7 +16,7 @@ namespace vpb {
 
 // ----------------------------------------------------------------------------
 // Element type tags for the 16-bit activation/weight storage.
-// kind::f16 tcgen05.mma accepts both at the same rate; fp16 is the default
+// wgmma accepts both at the same rate; fp16 is the default
 // because its 10-bit mantissa keeps the class maps closer to the fp32 oracle.
 // ----------------------------------------------------------------------------
 struct F16 { using T = __half; static constexpr int kUmmaFmt = 0; };
@@ -72,31 +72,13 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// Packed fp32x2 arithmetic (Blackwell FFMA2 / FMUL2 / FADD2): two elements per instruction.  The
-// epilogue of the convolution kernels is instruction-issue bound (profiles/r1_conv_v6_ncu.md), so the
-// activation polynomial runs on register pairs.
+// fp32 pairs: the activation polynomial is written on register pairs so that the two elements of a
+// pair form independent instruction chains the scheduler can interleave.
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)),
-        "l"(*reinterpret_cast<unsigned long long*>(&c)));
-  return *reinterpret_cast<float2*>(&d);
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  unsigned long long d;
-  asm("mul.rn.f32x2 %0, %1, %2;"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&d);
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  unsigned long long d;
-  asm("add.rn.f32x2 %0, %1, %2;"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&d);
-}
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float2 splat2(float v) { return make_float2(v, v); }
 // Exact-erf GELU, branch-free, on a register pair.
 //   gelu(x) = max(x,0) - q,   q = 0.5*|x|*erfc(|x|/sqrt2)
@@ -179,6 +161,13 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// Same without the printf: a function call anywhere in a kernel that issues wgmma makes ptxas serialise them.
+__device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity))
+    if (++spins > VPB_MBAR_SPIN_LIMIT) __trap();
+}
+
 // ----------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor) tile loads.  OOB coordinates are legal and zero-fill,
 // which is how the 3x3 convolution gets its padding for free.
@@ -222,200 +211,66 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// TMA tile STORE shared -> global (bulk async group).  The source box in shared memory uses the same
-// 128-byte swizzle as the loads; rows / channels outside the tensor are clipped by the TMA unit.
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-      ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-      ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all earlier bulk groups of this thread have finished READING shared memory (the buffer may be rewritten)
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// ... have completed entirely (writes performed)
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint4 v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
 
 // ----------------------------------------------------------------------------
-// tcgen05 / TMEM
+// Hopper warpgroup MMA (wgmma): D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp32 accumulators in registers,
+// both operands K-major in shared memory.
 // ----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16/fp16 operands, fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma has retired.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------
-// CTA pair (cta_group::2): two CTAs of a 2-cluster (one TPC) run ONE tcgen05.mma of M = 256.  Each CTA
-// stages its own 128 A rows and HALF of the B tile (N/2 rows) at the same shared-memory offsets; the
-// leader (cluster rank 0) issues the MMA and both accumulate into their own TMEM.  Halves the weight
-// bytes staged and read per SM, which is what bounds the 1-CTA kernel (profiles/r1_tma_ring_microbench.md).
-// ----------------------------------------------------------------------------
-static constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2cta(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once all earlier MMAs of the pair retired) on the barrier at this offset in BOTH CTAs.
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-// Pair loads: data lands in the issuing CTA's shared memory, the byte count is signalled on the
-// LEADER's barrier (`bar` already masked with kPeerBitMask).
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_pair(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
-                                                 int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
-                                                 int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_pair(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
-                                                 int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-// mbarrier.arrive on the barrier at the same offset in CTA `cta` of the cluster.
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar), "r"(cta)
-      : "memory");
-}
-
-// 16-byte load from the shared memory of CTA `cta` of the cluster, same offset as local address `addr`
-__device__ __forceinline__ float4 ld_dsmem_f4(uint32_t addr, uint32_t cta) {
-  float4 v;
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %4, %5;\n\t"
-      "ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [ra];\n\t}"
-      : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-      : "r"(addr), "r"(cta)
-      : "memory");
-  return v;
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle:
-// rows are 128 B apart inside an 8-row (1024 B) swizzle atom, atoms are SBO apart.
-//   [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major) | [32,46) SBO>>4
-//   [46,48) version=1 (sm_100) | [61,64) layout (2 = SWIZZLE_128B)
-// `base_offset` ([49,52)) = (start_address >> 7) & 7 when the start address is not aligned to the
-// 1024-byte swizzle repeat (used for the row-shifted tap views of the halo kernel).
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr, uint32_t base_offset = 0) {
-  uint64_t d = static_cast<uint64_t>(base_offset & 7u) << 49;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows are 128 B apart inside an
+// 8-row (1024 B) swizzle atom, atoms are SBO apart.
+//   [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major) | [32,46) SBO>>4 | [62,64) layout (1 = SWIZZLE_128B)
+// One k16 step (32 B) inside the 128-B swizzle row is +2 in the encoded start address.
+__device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t smem_addr) {
+  uint64_t d = static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;               // LBO (ignored) — canonical value 1
   d |= static_cast<uint64_t>(1024 >> 4) << 32;       // SBO = 1024 B
-  d |= static_cast<uint64_t>(1) << 46;               // descriptor version
-  d |= static_cast<uint64_t>(2) << 61;               // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;               // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16: fp32 accumulate, both operands K-major.
-__host__ __device__ constexpr uint32_t umma_idesc(int fmt /*0 f16, 1 bf16*/, int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(fmt) << 7) | (static_cast<uint32_t>(fmt) << 10) |
-         (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// m64nNk16, fp32 accumulate; acc == 0 overwrites D.  d[] is the standard accumulator fragment: register
+// 4j + {0,1} holds row (warp%4)*16 + lane/4, columns 8j + 2*(lane%4) + {0,1}; 4j + {2,3} the same 8 rows below.
+template <class E, int N> struct Wgmma;
+#define VPB_WGMMA(E, TY, N, DREGS, ...)                                                                     \
+  template <> struct Wgmma<E, N> {                                                                          \
+    __device__ __forceinline__ static void mma(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {    \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\twgmma.mma_async.sync.aligned.m64n" #N     \
+                   "k16.f32." TY "." TY " {" DREGS "}, %0, %1, p, 1, 1, 0, 0;\n\t}"                             \
+                   : "+l"(a), "+l"(b), "+r"(acc), __VA_ARGS__);                                             \
+    }                                                                                                       \
+  };
+#define VPB_D16 "%3, %4, %5, %6, %7, %8, %9, %10"
+#define VPB_C16 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+#define VPB_D32 "%3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18"
+#define VPB_C32 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+#define VPB_D64 "%3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34"
+#define VPB_C64 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+#define VPB_D128 "%3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66"
+#define VPB_C128 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+VPB_WGMMA(F16, "f16", 16, VPB_D16, VPB_C16)
+VPB_WGMMA(F16, "f16", 32, VPB_D32, VPB_C32)
+VPB_WGMMA(F16, "f16", 64, VPB_D64, VPB_C64)
+VPB_WGMMA(F16, "f16", 128, VPB_D128, VPB_C128)
+VPB_WGMMA(BF16, "bf16", 16, VPB_D16, VPB_C16)
+VPB_WGMMA(BF16, "bf16", 32, VPB_D32, VPB_C32)
+VPB_WGMMA(BF16, "bf16", 64, VPB_D64, VPB_C64)
+VPB_WGMMA(BF16, "bf16", 128, VPB_D128, VPB_C128)
+#undef VPB_D16
+#undef VPB_C16
+#undef VPB_D32
+#undef VPB_C32
+#undef VPB_D64
+#undef VPB_C64
+#undef VPB_D128
+#undef VPB_C128
+#undef VPB_WGMMA
+
 
 // Programmatic dependent launch (PDL): a kernel launched with the programmatic-stream-serialization
 // attribute may start while its predecessor is still running; it must not touch the predecessor's

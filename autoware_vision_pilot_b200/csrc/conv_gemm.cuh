@@ -1,4 +1,4 @@
-// conv_gemm.cuh — host-side plan object for the tcgen05 implicit-GEMM convolution.
+// conv_gemm.cuh — host-side plan object for the wgmma implicit-GEMM convolution.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -12,35 +12,23 @@ struct ConvKParams {
   int H, W, Cin, Cout;
   int taps, phases;
   int TH, TW, tw_shift;          // spatial tile (TH*TW == 128), log2(TW)
-  int BN;                        // N tile (multiple of 16, <= 256)
+  int BN;                        // N tile: 16, 32, 64 or 128 (the kernel's template parameter)
   int tiles_h, tiles_w, tiles_n; // tile grid
   int total_tiles;
   int kchunks;                   // ceil(Cin / 64)
-  int Cin2, kchunks2;            // tile kernel: fused second 1x1 input (skip link), 0 = none
-  int stages;                    // smem pipeline depth (tile kernel)
-  int lin;                       // 1 = linear-padded 3x3 kernel
-  int fuse4;                     // tile kernel, ConvTranspose: all 4 phases per CTA tile
-  int wstat;                     // weight-stationary ConvTranspose kernel (convt_ws_kernel): a CTA keeps ONE (phase, N tile)
-                                 // weight set resident in shared memory and streams pixel tiles through it
-  int upc;                       // upconv_pair_kernel: fused ConvTranspose2d(k2,s2) [+ 1x1 skip] -> Conv3x3 (taps = 4 low-res taps per output
-                                 // phase, taps2 = 9 skip taps, bias = [9 border classes][Cout])
-  int taps2;
-  int tma_store;                 // tile kernel: epilogue stages the tile in shared memory and writes it with TMA stores
+  int Cin2, kchunks2;            // fused second 1x1 input (skip link), 0 = none
+  int stages;                    // shared-memory operand ring depth
+  int lin;                       // VPB_ALGO_LINEAR with a padded output: the border is written as zeros after the GEMM
+  int upc;                       // fused ConvTranspose2d(k2,s2) [+ 1x1 skip] -> Conv3x3 (taps = 4 low-res taps per output
+                                 // phase, 9 skip taps, bias = [9 border classes][Cout])
   int nlim;                      // channels of an output row that may be written: ldo, or round8(Cout) for a channel SLICE
-  int stride;                    // tile kernel: 1 | 2 (input sampled through the tensor map's traversal stride)
+  int stride;                    // 1 | 2 (input sampled through the tensor map's traversal stride)
   int act2;                      // activation after the residual step (ADD / MULADD), ACT_NONE = off
-  int split;                     // tile kernel: split-fp16 mode, 3 K segments (A_hi W_hi, A_lo W_hi, A_hi W_lo), hi/lo outputs
+  int split;                     // split-fp16 mode, 3 K segments (A_hi W_hi, A_lo W_hi, A_hi W_lo), hi/lo outputs
   void* out_lo;                  // split mode: low halves of out / res (same layout as the hi tensors)
   const void* res_lo;
-  int na, nb;                    // linear kernel: activation-segment / weight-slot ring depths
-  int gb;                        // linear kernel: weight tiles per slot (3 = one kernel row per barrier)
-  int ms;                        // linear kernel: M sub-tiles (of 128 pixels) per CTA tile, 1, 2 or 4
-  int pair;                      // linear kernel: 1 = CTA-pair kernel (cta_group::2), tiles are pair tiles
-  int splitk;                    // linear kernel: > 1 = split-K kernel, K chunks divided over a cluster of `splitk` CTAs
-  int NP, WP, tiles_m;           // linear kernel: padded pixel count, padded width, M tiles
   int in_pad, out_pad, res_pad;  // 1 = that tensor is a zero-bordered image [(H+2)*(W+2)][C]
-  uint32_t mg_tn, mg_tw, mg_tpp, mg_wp;  // magic reciprocals (fast_div) of tiles_n, tiles_w, tiles per phase, WP
-  int desc_bo;                   // 1 = set the smem-descriptor base_offset for shifted tap views
+  uint32_t mg_tn, mg_tw, mg_tpp; // magic reciprocals (fast_div) of tiles_n, tiles_w, tiles per phase
   int act, mode, final_kind;
   const float* bias;
   void* out;
@@ -49,21 +37,18 @@ struct ConvKParams {
   int ldr;
   float* out_f32;
   uint8_t* out_cls;
-  unsigned long long* trace;     // experiment hook (tile kernel): clock64() stamps of CTA 0, [16 tiles][16]
 };
 
-// Tensor maps of the tile kernel, passed as ONE __grid_constant__ parameter (TMA reads them from param space).
+// Tensor maps of the kernel, passed as ONE __grid_constant__ parameter (TMA reads them from param space).
 struct ConvMaps {
   CUtensorMap A, B;              // activations / weights
   CUtensorMap A2, B2;            // second 1x1 input and its weights (copies of A / B when unused)
-  CUtensorMap O;                 // output view [h][a][w][b][c] for the TMA-store epilogue (copy of A when unused)
   CUtensorMap Alo, Blo, A2lo, B2lo;   // split-fp16 mode: the low halves (copies of the hi maps when unused)
 };
 
 struct ConvPlan {
   CUtensorMap mapA, mapB;
   CUtensorMap mapA2, mapB2;      // second 1x1 input and its weights (copies of mapA/mapB when unused)
-  CUtensorMap mapO;              // output view [h][a][w][b][c] for the TMA-store epilogue (copy of mapA when unused)
   CUtensorMap mapAlo, mapBlo, mapA2lo, mapB2lo;
   ConvKParams p;
   int dtype;

@@ -3,7 +3,7 @@
 // Reference: torchvision.models.efficientnet_b0(...).features as used by
 // Models/model_components/backbone.py:9-22 (third-party; architecture in SURVEY.md Appendix A),
 // Models/model_components/scene_context.py:25-57, backbone_feature_fusion.py:13-38.
-// The dense 1x1 convolutions of the encoder run on the tcgen05 GEMM (conv_gemm.cu); what is here
+// The dense 1x1 convolutions of the encoder run on the wgmma GEMM (conv_gemm.cu); what is here
 // is byte-moving SIMT work: stem conv (3 input channels), depthwise convs with the
 // squeeze-excitation average pool fused in, the SE gate (folded into the projection weights),
 // global average pool, the context MLP (GEMV), the 1->128 conv on the 10x20 map and the max-pool
@@ -87,7 +87,7 @@ DwGeom dw_geometry(int H, int W, int C, int k, int stride) {
   const int nitems = g.Ho * ((g.Wo + kXT - 1) / kXT);   // (row, group of kXT columns)
   // ~2 blocks per SM, each block a contiguous item range (multiple of PPB); few blocks keep the
   // number of pooling atomics (and their contention on a handful of cache lines) low
-  int ppb = (nitems + 148 * 2 - 1) / (148 * 2);
+  int ppb = (nitems + 132 * 2 - 1) / (132 * 2);
   ppb = (ppb + g.PPB - 1) / g.PPB * g.PPB;
   g.pix_per_block = std::max(ppb, g.PPB);
   g.nblocks = (nitems + g.pix_per_block - 1) / g.pix_per_block;
@@ -545,9 +545,9 @@ int vpb::se_scale_x(int dtype, const long long* gap_acc, int HW, int C, int sq, 
   const size_t smem = (2 * static_cast<size_t>(C) + sq) * sizeof(float);
   if ((C & 7) || C > 1152 || sq > 48 || !act) { vpb_set_error("se_scale: unsupported C=%d sq=%d", C, sq); return VPB_ERR_ARG; }
   // every block recomputes the gate (reads w1 + w2: 8*C*sq bytes), so the grid follows the activation bytes: one block
-  // per 64 KB, at most two waves; the late blocks (C = 1152 on 10x20 pixels) get 7 blocks, the first (96 on 160x320) 148+
+  // per 64 KB, at most two waves; the late blocks (C = 1152 on 10x20 pixels) get 7 blocks, the first (96 on 160x320) two waves on 132 SMs
   const int n8 = HW * (C / 8);
-  const int grid = std::max(1, std::min(296, (n8 * 16 + 65535) / 65536));
+  const int grid = std::max(1, std::min(264, (n8 * 16 + 65535) / 65536));
   if (dtype == VPB_BF16)
     VPB_CUDA_OK(launch_k(se_scale_kernel<BF16>, dim3(grid), dim3(512), smem, st, gap_acc, 1.0f / HW, C, sq, w1, b1, w2, b2,
                          static_cast<uint4*>(act), static_cast<uint4*>(act_lo), n8, scale_out));

@@ -1,4 +1,4 @@
-// engine.cu — host side of the B200 camera-perception engine (C++; owns weights, buffers, the
+// engine.cu — host side of the H100 camera-perception engine (C++; owns weights, buffers, the
 // per-frame launch list and its CUDA graph) behind the C-ABI of include/vp_b200.h.
 //
 // Reference composition being replaced (paths relative to the reference repo):
@@ -277,8 +277,8 @@ struct vp_engine {
     ConvPlan* pp = plan.get();
     plans.push_back(std::move(plan));
     OpRec op; op.name = name; op.flops = pp->flops; op.gemm = true; op.lane = cur_lane;
-    op.kind = pp->p.lin ? (pp->p.pair ? 3 : 2) : 1;
-    op.kname = pp->p.upc ? "upconv_pair_kernel" : pp->p.wstat ? "convt_ws_kernel" : !pp->p.lin ? "conv_gemm_kernel" : pp->p.splitk ? "conv3x3_splitk_kernel" : pp->p.pair ? "conv3x3_pair_kernel" : "conv3x3_lin_kernel";
+    op.kind = a.algo == VPB_ALGO_LINEAR ? 2 : 1;
+    op.kname = "conv_wgmma_kernel";
     op.launch = [pp](cudaStream_t s) { return conv_plan_launch(pp, s); };
     ops.push_back(std::move(op));
     return VPB_OK;
@@ -390,7 +390,7 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
       const std::string nm = tag + "mb" + std::to_string(si + 1) + "." + std::to_string(r) + ".";
       int bi = 0;
       Tens cur = x;
-      if (exp != 1) {  // 1x1 expand + BN + SiLU -> tcgen05 GEMM
+      if (exp != 1) {  // 1x1 expand + BN + SiLU -> wgmma GEMM
         const HostTensor* ew = find_w_shaped(w, bp + "0.0.weight", {ce, ci, 1, 1});
         if (!ew || !bn_fold(w, bp + "0.1.", ce, s, t)) return VPB_ERR_IO;
         void* dw_ = e.upload_16(pack_conv(*ew, &s));
@@ -486,7 +486,7 @@ static int up_skip(vp_engine& e, const WeightMap& w, const std::string& p, int i
     return e.add_conv(tag + "up" + std::to_string(i), in, Cout, 1, 4, dw_, e.upload_f32(ub->f), ACT_NONE,
                       VPB_EPI_STORE, out, nullptr);
   // the skip link's 1x1 conv is a second K segment of the same GEMM: both layers accumulate in the
-  // fp32 TMEM accumulator and the sum is rounded and written once (no intermediate tensor)
+  // fp32 accumulator and the sum is rounded and written once (no intermediate tensor)
   const std::string sk = p + "skip_link_layer_" + std::to_string(i);
   const HostTensor *st = find_w_shaped(w, sk + ".weight", {Cout, -1, 1, 1}), *sb = find_w_shaped(w, sk + ".bias", {Cout});
   if (!st || !sb) return VPB_ERR_IO;
@@ -883,8 +883,8 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
   DeviceGuard guard(cfg->gpu_id);
   cudaDeviceProp prop;
   VPB_CUDA_OK(cudaGetDeviceProperties(&prop, cfg->gpu_id));
-  if (prop.major != 10) {
-    vpb_set_error("vp_engine_create: device %d is sm_%d%d; this library is built for sm_100a only", cfg->gpu_id, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    vpb_set_error("vp_engine_create: device %d is sm_%d%d; this library is built for sm_90a only", cfg->gpu_id, prop.major, prop.minor);
     return VPB_ERR_CUDA;
   }
   std::unique_ptr<vp_engine> e(new vp_engine());

@@ -228,7 +228,7 @@ extern "C" int vp_multicam_step(vp_multicam* mc, const void* feat_dev, const dou
   if (reinterpret_cast<uintptr_t>(feat_dev) & 15) { vpb_set_error("vp_multicam_step: features must be 16-byte aligned"); return VPB_ERR_ARG; }
   DeviceGuard g(mc->gpu_id);
   uint8_t* slot = mc->d_gather + static_cast<size_t>(mc->rank) * VP_MC_PAYLOAD_BYTES;
-  pack_payload_kernel<<<148, 256, 0, mc->stream>>>(static_cast<const uint4*>(feat_dev), meas_dev, slot);
+  pack_payload_kernel<<<132, 256, 0, mc->stream>>>(static_cast<const uint4*>(feat_dev), meas_dev, slot);
   VPB_CUDA_OK(cudaGetLastError());
   int rc = multicam_allgather(mc);
   if (rc) return rc;

@@ -12,7 +12,7 @@
 //   bias9[cy,cx]   = b3 + sum over the 3x3 taps inside the image of  W3[dy,dx] . (bt + bs)
 // (x and s are zero outside the image — Conv2d's zero padding of `up` — which the consumer gets from TMA out-of-bounds
 // fill; only the constant term needs the nine border classes.)  Verified in fp64 against conv_transpose2d + conv2d by
-// tests/test_upconv_gpu.py; consumed by upconv_pair_kernel (conv_gemm.cu).
+// tests/test_upconv_gpu.py; consumed by conv_wgmma_kernel (conv_gemm.cu).
 // All arithmetic here is fp32 on the device (SIMT SGEMM, runs once per engine construction).
 #include "common.cuh"
 #include "ops_internal.h"
@@ -129,7 +129,7 @@ extern "C" int vpb_f32_to_16(int dtype, const float* src, void* dst, long long n
   if (!src || !dst || n < 0 || (dtype != VPB_F16 && dtype != VPB_BF16)) { vpb_set_error("f32_to_16: bad arguments"); return VPB_ERR_ARG; }
   if (n == 0) return VPB_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int blocks = static_cast<int>(std::min<long long>((n + 255) / 256, 148 * 16));
+  const int blocks = static_cast<int>(std::min<long long>((n + 255) / 256, 132 * 16));
   if (dtype == VPB_BF16) f32_to_16_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>(src, static_cast<__nv_bfloat16*>(dst), n);
   else f32_to_16_kernel<__half><<<blocks, 256, 0, st>>>(src, static_cast<__half*>(dst), n);
   VPB_CUDA_OK(cudaGetLastError());

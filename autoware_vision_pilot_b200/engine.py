@@ -183,12 +183,12 @@ class Engine:
         cnt = C.c_int()
         gemm = (C.c_int * n)()
         L.check(self._lib.vp_engine_profile(self._h, n, ms, fl, names, gemm, C.byref(cnt)), "vp_engine_profile")
-        kern = {1: "conv_gemm_kernel", 2: "conv3x3_lin_kernel", 3: "conv3x3_pair_kernel"}
+        kern = {1: "conv_wgmma_kernel", 2: "conv_wgmma_kernel"}
         return [{"name": names[i].decode(), "ms": ms[i], "flops": fl[i], "gemm": bool(gemm[i]),
                  "kernel": kern.get(gemm[i])} for i in range(cnt.value)]
 
     def time_kernel(self, kind: int, reps: int = 10) -> dict:
-        """Back-to-back device time of every launch of one convolution kernel (1 tile, 2 lin, 3 pair)."""
+        """Back-to-back device time of every convolution launch of one kind (1 tile layout, 2 3x3 on a padded input)."""
         ms, fl, n = C.c_float(), C.c_double(), C.c_int()
         self._lib.vp_engine_time_kind.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float),
                                                   C.POINTER(C.c_double), C.POINTER(C.c_int)]

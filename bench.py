@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py — camera frames/s @1080p multi-task on B200 (BASELINE.json metric), one JSON line.
+"""bench.py — camera frames/s @1080p multi-task on H100 (BASELINE.json metric), one JSON line.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python bench.py --autospeed ...      # row f.4: the AutoSpeed detector, 1080p frame -> boxes
     python bench.py --config5 ...        # row e: multi-camera all-gather + fusion, one rank per camera (torchrun)
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
@@ -20,14 +20,17 @@ Lines printed by rank 0:
   roofline   the dominant kernel (the tensor-core kernel with the most device time per frame): ALGORITHMIC 2*MAC per
              launch (SURVEY.md 8d: of the reference graph's layers the launch computes) / mean launch duration, all its
              launches of the frame issued back to back for >= 2 s between one CUDA-event pair (vp_engine_time_kernel),
-             against the measured SUSTAINED cuBLAS bf16 peak; achieved_executed / frac_executed = the same with the MACs
+             against the H100 SXM data-sheet dense bf16 peak; achieved_executed / frac_executed = the same with the MACs
              the kernel actually executes (the composed ConvTranspose->Conv3x3 GEMM runs 44 % of the reference's);
-             roofline.stages = one entry per kernel of the frame (HBM-bound ones against the measured copy peak);
+             roofline.stages = one entry per kernel of the frame (HBM-bound ones against the data-sheet HBM3 bandwidth);
   cpu_baseline  the oracle (CPU fp32 port of the reference's PyTorch path: PIL resize -> 4 networks
              -> post-process) on the host cores, a bounded sample, N=1 only.
   --impl reference  times that CPU path alone with all host threads (the reference's own
-             implementation of the path is PyTorch-on-CPU; /root/reference is not on the GPU box,
-             so the port in oracle/ — validated bit-equal against it — is what runs).
+             implementation of the path is PyTorch-on-CPU; the port in oracle/ — validated bit-equal
+             against it — is what runs).
+  --dump-outputs DIR  after the timed steps, the outputs of the last timed step (per network: raw fp32 maps and
+             the class map as float32) are written as DIR/<network>_{raw,cls}.npy; inputs are seeded, so two
+             builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -48,34 +51,16 @@ sys.path.insert(0, ROOT)
 H_IN, W_IN = 1080, 1920
 MODELS = ("scene_seg", "scene_3d", "domain_seg", "ego_lanes")
 GFLOP_MT = 1153.25      # SURVEY.md §8d: algorithmic GFLOP / frame, shared-encoder multi-task
-POOL_FRAMES = 24        # 24 x 6.22 MB = 149 MB > 126 MB L2
+POOL_FRAMES = 24        # 24 x 6.22 MB = 149 MB > 50 MB L2
 
 
 def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return {"tflops_burst": d.get("bf16_tflops"), "tflops_sustained": d.get("bf16_tflops_sustained"),
-                "hbm_gbs": d.get("hbm_gbs"), "src": "measured"}
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "src": "fallback"}
+    """NVIDIA's H100 SXM data sheet (700 W card): dense bf16 989 TFLOP/s, HBM3 3.35 TB/s.  Denominators only —
+    a power-limited card runs below them (the clocks block of the line shows what this one ran at)."""
+    return {"tflops_burst": 989.0, "tflops_sustained": 989.0, "hbm_gbs": 3350.0, "src": "H100 SXM data sheet"}
 
 
-def load_traffic(kernel):
-    """Average DRAM bytes per launch of the dominant kernel from the newest committed ncu capture of THAT kernel
-    (profiles/r*_traffic*.json, produced by scripts/ncu_conv_traffic.sh).  STATIC: read from the committed file, not
-    measured in this run (ncu cannot run inside a timed bench)."""
-    import glob
-    for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "r*traffic*.json")), reverse=True):
-        with open(path) as f:
-            d = json.load(f)
-        if d.get("kernel") == kernel:
-            return d.get("avg_dram_bytes"), os.path.relpath(path, ROOT)
-    return None, None
-
-
-TENSOR_KERNELS = ("conv_gemm_kernel", "conv3x3_lin_kernel", "conv3x3_pair_kernel", "conv3x3_splitk_kernel",
-                  "convt_ws_kernel", "upconv_pair_kernel")
+TENSOR_KERNELS = ("conv_wgmma_kernel",)
 
 
 def stage_rooflines(eng, peaks):
@@ -86,7 +71,7 @@ def stage_rooflines(eng, peaks):
     composed ConvTranspose->Conv3x3 GEMM executes fewer MACs than the reference layers it replaces: its row carries
     both figures (achieved = algorithmic, achieved_executed = what the tensor pipe actually does)."""
     st = eng.stats()
-    extra_ref = max(0.0, st["reference_flops"] - st["total_flops"])      # per frame, all of it in upconv_pair_kernel
+    extra_ref = max(0.0, st["reference_flops"] - st["total_flops"])      # per frame, all of it in conv_wgmma_kernel
     rows, total_us = [], 0.0
     for k in eng.kernel_names():
         r = eng.time_kernel_name(k, reps=20)
@@ -98,14 +83,14 @@ def stage_rooflines(eng, peaks):
         ach_exec = None
         if tensor:
             ach_exec = r["flops"] / (r["ms"] / 1e3) / 1e12
-            fl = r["flops"] + (20 * extra_ref if k == "upconv_pair_kernel" else 0.0)
+            fl = r["flops"] + 20 * extra_ref
             ach, peak, unit = fl / (r["ms"] / 1e3) / 1e12, peaks["tflops_burst"], "TFLOP/s"
         else:
             ach, peak, unit = r["bytes"] / (r["ms"] / 1e3) / 1e9, peaks["hbm_gbs"], "GB/s"
         row = {"kernel": k, "bound": "tensor" if tensor else "hbm", "launches_per_frame": r["launches"] // 20,
                "us_per_frame": us_frame, "achieved": ach, "peak": peak, "unit": unit,
                "frac": ach / peak if peak else None}
-        if k == "upconv_pair_kernel":
+        if tensor:
             row["achieved_executed"] = ach_exec
             row["frac_executed"] = ach_exec / peak if peak else None
         rows.append(row)
@@ -301,17 +286,7 @@ def run_config5(args, rank, local_rank, world):
     for i in range(max(args.warmup, 3)):
         step(i)
     torch.cuda.synchronize()
-    t_est = time.time()
-    for i in range(args.steps):
-        step(i)
-    torch.cuda.synchronize()
-    t_est = time.time() - t_est
-    blocks = max(1, int(np.ceil(args.min_seconds / max(t_est, 1e-4))))
-    if world > 1:
-        tb = torch.tensor([blocks], device=dev)
-        dist.all_reduce(tb, op=dist.ReduceOp.MAX)
-        blocks = int(tb.item())
-    timed_steps = blocks * args.steps
+    timed_steps = args.steps
     sampler = ClockSampler(local_rank)
     sampler.start()
     barrier()
@@ -382,16 +357,7 @@ def run_autospeed(args, rank, local_rank, world):
     for i in range(max(args.warmup, 3)):
         step(i)
     torch.cuda.synchronize()
-    t_est = time.time()
-    for i in range(args.steps):
-        step(i)
-    torch.cuda.synchronize()
-    blocks = max(1, int(np.ceil(args.min_seconds / max(time.time() - t_est, 1e-4))))
-    if world > 1:
-        tb = torch.tensor([blocks], device=dev)
-        dist.all_reduce(tb, op=dist.ReduceOp.MAX)
-        blocks = int(tb.item())
-    timed_steps = blocks * args.steps
+    timed_steps = args.steps
     sampler = ClockSampler(local_rank)
     sampler.start()
     barrier()
@@ -446,6 +412,18 @@ def run_autospeed(args, rank, local_rank, world):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(eng, out_dir):
+    """What a caller of the timed path receives for the last frame: per network the raw output maps (fp32
+    [C, H, W]) and, where the network has one, the class map (as float32)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for i, m in enumerate(MODELS):
+        eng.fetch_raw(i)
+        np.save(os.path.join(out_dir, f"{m}_raw.npy"), np.array(eng.raw(i), dtype=np.float32))
+        cls = eng.cls(i)
+        if cls is not None:
+            np.save(os.path.join(out_dir, f"{m}_cls.npy"), cls.astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -459,8 +437,8 @@ def main():
                     help="BASELINE configs[4]: per rank EgoLanes + device lateral post-process, ONE ncclAllGather of the "
                          "fused features + PathFinder measurements (C++, vp_b200_multicam.h), Estimator fusion")
     ap.add_argument("--autospeed", action="store_true", help="SURVEY 8f.4: the AutoSpeed detector instead of the 4-task frame")
-    ap.add_argument("--min-seconds", type=float, default=1.0,
-                    help="the K-step block is repeated inside the timed region until it lasts at least this long")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     ap.add_argument("--inflight", type=int, default=4,
                     help="camera frames in flight per GPU (engine replicas on separate streams; the next "
                          "frame's latency-bound encoder overlaps the current frame's decoders)")
@@ -525,19 +503,7 @@ def main():
     for i in range(max(args.warmup, 2 * n_eng)):
         step(i)
     torch.cuda.synchronize()
-    # minimum timed duration: one untimed K-step block gives the estimate, the timed region then repeats the
-    # K-step block `blocks` times back to back (a 20-step region is 33 ms — too short to be a measurement)
-    t_est = time.time()
-    for i in range(args.steps):
-        step(i)
-    torch.cuda.synchronize()
-    t_est = time.time() - t_est
-    blocks = max(1, int(np.ceil(args.min_seconds / max(t_est, 1e-4))))
-    if world > 1:
-        tb = torch.tensor([blocks], device="cuda")
-        dist.all_reduce(tb, op=dist.ReduceOp.MAX)
-        blocks = int(tb.item())
-    timed_steps = blocks * args.steps
+    timed_steps = args.steps
 
     sampler = ClockSampler(local_rank)
     sampler.start()
@@ -557,6 +523,8 @@ def main():
     ms = elapsed_all(e0, ends)
     ms = multicam.max_over_ranks(ms, torch.device("cuda", local_rank))
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(engs[(timed_steps - 1) % n_eng], args.dump_outputs)
 
     # ---- end to end through the C-ABI with pinned host frames (H2D + kernels + D2H per step)
     # (a) latency: one engine, synchronous per frame
@@ -631,9 +599,8 @@ def main():
     e2e_fps = world * n_e2e_frames / (e2e_ms / 1e3)
     executed = gemm_fl / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
     peak = peaks["tflops_sustained"]
-    traffic, traffic_src = load_traffic(dom)
     # FLOPs the reference's layer-by-layer graph spends on what the fused ConvTranspose->Conv3x3 launches compute
-    extra_ref = max(0.0, stats["reference_flops"] - stats["total_flops"]) if dom == "upconv_pair_kernel" else 0.0
+    extra_ref = max(0.0, stats["reference_flops"] - stats["total_flops"]) if dom in TENSOR_KERNELS else 0.0
     dom_per_frame = next(r["launches_per_frame"] for r in stages if r["kernel"] == dom)
     # SURVEY.md 8d: roofline.achieved counts the ALGORITHMIC FLOPs of the reference graph's layers these launches compute
     achieved = (gemm_fl + extra_ref * n_gemm / max(dom_per_frame, 1)) / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
@@ -641,8 +608,7 @@ def main():
         "metric": "camera frames/sec @1080p multi-task", "value": fps, "unit": "frames/s", "n_gpus": world,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / timed_steps, "higher_is_better": True,
         "timed_steps": timed_steps, "timed_region_s": ms / 1e3,
-        "timing": f"the {args.steps}-step block repeated {blocks}x back to back inside ONE device-timed region "
-                  f"(>= {args.min_seconds} s), max over ranks",
+        "timing": f"{timed_steps} steps back to back inside ONE device-timed region, max over ranks",
         "scaling": "weak", "vs_baseline": None, "dtype": "f16" if args.dtype == "fp16" else "bf16",
         "data": "synthetic",
         "config": {"workload": "1080p multi-task: SceneSeg+Scene3D+DomainSeg+EgoLanes, shared encoder "
@@ -664,7 +630,7 @@ def main():
         "gpu_launches": stats["n_launches"] * timed_steps,
         "launches_per_frame": stats["n_launches"],
         "tensor_tflops_whole_step": GFLOP_MT * fps / world / 1e3,
-        "roofline": {"bound": "tensor", "kernel": f"{dom} (tcgen05 implicit-GEMM convolution)",
+        "roofline": {"bound": "tensor", "kernel": f"{dom} (wgmma implicit-GEMM convolution)",
                      "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak if peak else None,
                      "flops_counted": "achieved / frac: ALGORITHMIC 2*MAC of the reference graph's layers these launches compute "
                                       "(SURVEY.md 8d); achieved_executed / frac_executed: the 2*MAC the kernel actually "
@@ -672,14 +638,12 @@ def main():
                                       "layers' MACs for the same outputs, DESIGN.md 3e) = the tensor-pipe utilisation",
                      "achieved_executed": executed,
                      "frac_executed": executed / peak if peak else None,
-                     "peak_src": f"{peaks['src']} bf16 cuBLAS, SUSTAINED: the kernel is timed over {gemm_ms / 1e3:.1f} s of "
+                     "peak_src": f"{peaks['src']} dense bf16; the kernel is timed over {gemm_ms / 1e3:.1f} s of "
                                  "back-to-back launches",
                      "frac_vs_burst_peak": achieved / peaks["tflops_burst"] if peaks["tflops_burst"] else None,
                      "burst_peak": peaks["tflops_burst"],
                      "launches_timed": n_gemm,
                      "share_of_kernel_time": next(r["share_of_kernel_time"] for r in stages if r["kernel"] == dom),
-                     "traffic": traffic, "traffic_src": f"STATIC, {traffic_src} (ncu --set full of an earlier run of this "
-                                                        "kernel; not measured in this run)" if traffic_src else None,
                      "flop_per_launch": achieved * 1e12 * (gemm_ms / 1e3) / max(n_gemm, 1),
                      "flop_per_launch_executed": gemm_fl / max(n_gemm, 1), "us_per_launch": 1e3 * gemm_ms / max(n_gemm, 1),
                      "all_tensor_kernels": {"achieved_executed": all_fl / (all_us / 1e6) / 1e12 if all_us else None,

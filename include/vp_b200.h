@@ -62,7 +62,7 @@ typedef struct {
                                        (tensorrt_engine.hpp:53); VP_PREC_SPLIT: split-fp16 "fp32-grade" mode for the
                                        reference's precision="fp32" engines (tensorrt_backend.cpp:129-131,
                                        run_model_node.cpp:29-36): every tensor is a (hi, lo) fp16 pair (~22 bits), the
-                                       tcgen05 GEMMs accumulate A_hi W_hi + A_lo W_hi + A_hi W_lo in fp32 — about
+                                       wgmma GEMMs accumulate A_hi W_hi + A_lo W_hi + A_hi W_lo in fp32 — about
                                        3x the tensor work, results within ~1e-5 sigma of the fp32 CPU path */
 } vp_engine_config;
 
@@ -106,7 +106,7 @@ uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes);
 /* Introspection for the benchmark / roofline report. */
 typedef struct {
   int n_launches;        /* kernels launched per frame                                           */
-  int n_gemm_launches;   /* of which tcgen05 implicit-GEMM convolutions                          */
+  int n_gemm_launches;   /* of which wgmma implicit-GEMM convolutions                          */
   double gemm_flops;     /* algorithmic 2*MAC of those convolutions per frame                    */
   double total_flops;    /* 2*MAC per frame actually EXECUTED (shared parts once; the fused ConvTranspose->Conv3x3
                             layers run fewer MACs than the reference's two layers)                */
@@ -119,7 +119,7 @@ typedef struct {
 } vp_engine_stats;
 int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s);
 /* Eagerly run one frame with a CUDA-event pair around every kernel; returns the per-kernel
- * device times (ms) in launch order; is_gemm[i] != 0 for the tcgen05 convolution launches
+ * device times (ms) in launch order; is_gemm[i] != 0 for the wgmma convolution launches
  * (1 = conv_gemm_kernel, 2 = conv3x3_lin_kernel, 3 = conv3x3_pair_kernel), 0 otherwise.
  * names[i] point into engine-owned storage. */
 int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* flops, const char** names,

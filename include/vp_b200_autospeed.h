@@ -12,9 +12,9 @@
  *   vp_autospeed_raw          the network's raw prediction tensor [1, 4 + nc, 10752] (auto_speed_head.py:63)
  *
  * The checkpoint is a .vpw file holding the module's state_dict (python -m autoware_vision_pilot_b200.convert);
- * BatchNorm (eps 1e-3) is folded at load.  16-bit operands on the tcgen05 tensor cores, fp32 accumulation, exactly
+ * BatchNorm (eps 1e-3) is folded at load.  16-bit operands on the wgmma tensor cores, fp32 accumulation, exactly
  * like the reference helper's own half-precision inference (auto_speed_infer.py:50 `.half()`).
- * No CPU fallback: creation fails with VPB_ERR_CUDA without an sm_100 device.
+ * No CPU fallback: creation fails with VPB_ERR_CUDA without an sm_90 device.
  */
 #ifndef VP_B200_AUTOSPEED_H_
 #define VP_B200_AUTOSPEED_H_

@@ -1,6 +1,6 @@
 /* vp_b200_ops.h — op-level C-ABI of libvp_b200.so (device pointers in, device pointers out).
  *
- * These are the individual sm_100a kernels the engine (vp_b200.h) strings together.
+ * These are the individual sm_90a kernels the engine (vp_b200.h) strings together.
  * They are exported so that the parity tests can check every stage against the
  * oracle in isolation, and so that a host written in another language can build its
  * own graph.  All pointers are DEVICE pointers unless a name ends in _host.
@@ -45,7 +45,7 @@ enum { VPB_ALGO_TILE = 0, VPB_ALGO_LINEAR = 1 };
 const char* vpb_last_error(void);
 void vpb_set_error(const char* fmt, ...);
 
-/* Implicit-GEMM convolution on tcgen05 tensor cores.
+/* Implicit-GEMM convolution on wgmma tensor cores.
  *   taps = 9 : Conv2d 3x3 stride 1 pad 1   (scene_neck.py:13-24, scene_seg_head.py:13-19, ...)
  *   taps = 1 : Conv2d 1x1                  (skip links scene_neck.py:12, EfficientNet pointwise)
  *   phases = 4, taps = 1: ConvTranspose2d k2 s2 (scene_neck.py:11); phase p=(a*2+b)
@@ -73,13 +73,11 @@ typedef struct {
   /* Zero-bordered ("padded") image layout: tensor stored as [(H+2)*(W+2)][ld] with a one-pixel zero
    * border; flags say which of in / out / res use it (out/res dims are those of the OUTPUT image). */
   int in_pad, out_pad, res_pad;
-  int algo;               /* VPB_ALGO_TILE (default) | VPB_ALGO_LINEAR (3x3 on a padded input:
-                             one TMA segment per kernel row serves the three dx taps) */
-  int dbg_ms;             /* experiment hook: force 1 or 2 M sub-tiles per CTA in the LINEAR kernel (0 = auto) */
-  int dbg_gb;             /* experiment hook: 1 = one weight tile per pipeline stage in the LINEAR kernel; 2 = ConvTranspose
-                             with the direct-store epilogue; 3 = upconv with the staged TMA-store epilogue */
-  int dbg_base_offset;    /* experiment hook: also set the descriptor base_offset = dx in the LINEAR
-                             kernel (measured WRONG on B200; default 0 is the correct setting) */
+  int algo;               /* VPB_ALGO_TILE (default) | VPB_ALGO_LINEAR (3x3 on a padded input; the layer also writes
+                             the zero border of a padded output, so the result is a valid input for the next layer) */
+  int dbg_ms;             /* unused (kept for ABI compatibility) */
+  int dbg_gb;             /* unused (kept for ABI compatibility) */
+  int dbg_base_offset;    /* unused (kept for ABI compatibility) */
   /* Optional second 1x1 input accumulated into the same fp32 accumulator before the epilogue
    * (TILE algorithm, taps == 1): the neck's skip link  out = ConvT(in) + Conv1x1(in2)
    * (scene_neck.py:30-32) in ONE pass — in2 lives at the OUTPUT resolution [Ho][Wo][ld2]
@@ -88,16 +86,13 @@ typedef struct {
   const void* in2;
   const void* w2;
   int Cin2, ld2, in2_pad;
-  int dbg_pair;           /* experiment hook, LINEAR kernel: 1 = force the CTA-pair (cta_group::2) kernel,
-                             -1 = never use it, 0 = auto */
-  int dbg_splitk;         /* experiment hook, LINEAR kernel: k >= 2 = force the split-K cluster kernel with k CTAs per
-                             tile, -1 = never use it, 0 = auto (small-M layers) */
-  unsigned long long* dbg_trace; /* experiment hook, TILE kernel: device buffer [16 tiles][16] of clock64() stamps
-                             written by CTA 0 (scripts/trace_tile.py decodes it); NULL = off */
+  int dbg_pair;           /* unused (kept for ABI compatibility) */
+  int dbg_splitk;         /* unused (kept for ABI compatibility) */
+  unsigned long long* dbg_trace; /* unused (kept for ABI compatibility) */
   /* Split-fp16 ("fp32-grade") mode, selected by in_lo != NULL (TILE algorithm; the reference's precision="fp32",
    * tensorrt_backend.cpp:129-131): every 16-bit tensor x is the pair (x_hi = fp16(x), x_lo = fp16(x - x_hi)), ~22
    * significant bits.  The GEMM accumulates  A_hi*W_hi + A_lo*W_hi + A_hi*W_lo  as three K segments into the same
-   * fp32 TMEM accumulator (the dropped A_lo*W_lo term is 2^-22 relative) and the epilogue writes (out, out_lo).
+   * fp32 accumulator (the dropped A_lo*W_lo term is 2^-22 relative) and the epilogue writes (out, out_lo).
    * All *_lo tensors have exactly the layout of their hi partner; res_lo / in2_lo / w2_lo are required iff the hi
    * partner is given. */
   /* Widening for the AutoSpeed detector (SURVEY.md 8f.4), TILE algorithm:

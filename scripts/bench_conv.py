@@ -1,4 +1,4 @@
-"""Per-layer timing of the tcgen05 conv on the SceneSeg decoder shapes (SURVEY Appendix B).
+"""Per-layer timing of the wgmma conv on the SceneSeg decoder shapes (SURVEY Appendix B).
 Run on the GPU box:  python scripts/bench_conv.py [bn_override]"""
 import ctypes as C
 import json

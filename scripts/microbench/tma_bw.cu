@@ -1,7 +1,7 @@
 // tma_bw.cu — microbenchmark: how many bytes per clock per SM can TMA pull from L2 into shared memory
 // with the box shape the convolution kernels use (64 channels x R rows, 128-B swizzle), with all SMs
 // active — unicast vs 2-CTA-cluster multicast.  Decides whether weight multicast is worth building.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tma_bw tma_bw.cu && ./tma_bw
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_bw tma_bw.cu && ./tma_bw
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdio>

@@ -1,4 +1,4 @@
-"""AutoSpeed detector (SURVEY.md §8f.4) on the B200 engine against the fp32 CPU oracle (oracle/autospeed.py, pinned
+"""AutoSpeed detector (SURVEY.md §8f.4) on the H100 engine against the fp32 CPU oracle (oracle/autospeed.py, pinned
 against the unmodified reference module + helper) on the same frames and the seeded synthetic checkpoint.
 
 Gates (16-bit operands, like the reference helper's own `.half()` inference):

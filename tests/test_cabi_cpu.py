@@ -147,7 +147,7 @@ def test_write_vpw_is_atomic_under_concurrent_writers(tmp_path):
 
 
 def test_engine_create_fails_loudly_without_gpu(tmp_path):
-    """No CPU fallback: on a box without a B200 the engine must refuse, not degrade."""
+    """No CPU fallback: on a box without a H100 the engine must refuse, not degrade."""
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present")

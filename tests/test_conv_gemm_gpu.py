@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 implicit-GEMM convolution against torch fp32 (GPU, TF32 off) on the
+"""Parity of the wgmma implicit-GEMM convolution against torch fp32 (GPU, TF32 off) on the
 same 16-bit-rounded operands.  Accumulation is fp32 on both sides, so the only differences are
 summation order and the final rounding to the 16-bit storage type."""
 import pytest

@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 engine against the oracle (fp32 CPU restatement of the reference
+"""End-to-end parity of the H100 engine against the oracle (fp32 CPU restatement of the reference
 networks) through the reference-facing entry points: the Models/inference drop-in classes and the
 C-ABI engine.
 

@@ -724,7 +724,7 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
 }
 
 static int as_launch_all(vp_autospeed& e, const uint8_t* src, int stride, cudaStream_t st) {
-  int rc = e.pre.launch(src, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr, st);
+  int rc = e.pre.launch(&src, 1, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr, st);
   if (rc) return rc;
   for (auto& op : e.ops) { rc = op(st); if (rc) return rc; }
   PostParams pp{};
@@ -761,7 +761,7 @@ static int as_enqueue(vp_autospeed& e, const uint8_t* src, int h, int w, int str
   if (rc) return rc;
   if (e.gexec && e.g_stride == stride && e.g_src != src && e.g_pre_node) {
     // same geometry, another frame buffer: re-point the letterbox node instead of re-capturing
-    rc = e.pre.update_graph_node(e.gexec, e.g_pre_node, src, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
+    rc = e.pre.update_graph_node(e.gexec, e.g_pre_node, &src, 1, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
     if (rc) return rc;
     e.g_src = src;
   }

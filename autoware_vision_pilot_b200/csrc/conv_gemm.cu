@@ -14,8 +14,10 @@
 // unit, which IS the convolution's zero padding (and channels past Cin are zero in both operands, so every
 // K chunk runs four full k16 steps).
 //   ConvTranspose = 4 phase GEMMs (output pixel (2h+a, 2w+b)); the neck's skip link ConvT(in) + Conv1x1(skip)
-//   is ONE GEMM: the skip tensor is a second K segment read at output resolution through a 5-D TMA view
-//   [h][a][w][b][c] into the same accumulator.
+//   is ONE GEMM: the skip tensor is a second K segment read at output resolution through a TMA box with
+//   element stride 2 (every second pixel = one phase) into the same accumulator.
+//   Batch: both activation maps are 4-D [image][row][column][channel]; the tile index is image-major, no tile
+//   straddles two images, and the weight tiles are the same for every image.
 //   "upconv": ConvTranspose2d(k2,s2) [+ Conv1x1 skip] and the Conv3x3 that follows, composed at load time into
 //   ONE GEMM over the low-resolution tensor (weights from upconv_compose.cu): four 2x2 taps per output phase +
 //   nine skip taps, and a bias that depends on which 3x3 taps fall inside the image (9 border classes).
@@ -71,7 +73,8 @@ struct EpiPix {
   bool zero;      // store zeros instead (border pixel of a padded output)
   uint32_t ooff;  // element offset of the pixel in the output tensor   (pixel * ldo; < 2^31, checked by the plan)
   uint32_t roff;  // element offset of the pixel in the residual tensor (pixel * ldr)
-  uint32_t fpix;  // pixel index in the planar fp32 / class outputs (FINAL)
+  uint32_t fpix;  // pixel index in the planar fp32 / class outputs (FINAL), within the image
+  uint32_t img;   // image of the batch (FINAL: selects the [Cout][H][W] / [H][W] planes)
 };
 
 // NC = 16-column chunks handled per loop iteration (only NC = 1 is instantiated).
@@ -124,9 +127,10 @@ __device__ __forceinline__ void epilogue_chunks(const ConvKParams& p, uint32_t t
     if (p.mode == VPB_EPI_FINAL) {
       if (px.ok && chunk0 == 0) {
         const uint32_t plane = static_cast<uint32_t>(p.H * p.W);
+        float* of = p.out_f32 + px.img * static_cast<uint32_t>(p.Cout) * plane;
 #pragma unroll
         for (int i = 0; i < 16; ++i)
-          if (i < p.Cout) p.out_f32[i * plane + px.fpix] = v[0][i];
+          if (i < p.Cout) of[i * plane + px.fpix] = v[0][i];
         if (p.out_cls) {
           uint8_t cls = 0;
           if (p.final_kind == VPB_FINAL_ARGMAX) {
@@ -139,7 +143,7 @@ __device__ __forceinline__ void epilogue_chunks(const ConvKParams& p, uint32_t t
           } else if (p.final_kind == VPB_FINAL_EGOLANES) {
             cls = (v[0][2] > 0.f) ? 2 : (v[0][1] > 0.f) ? 1 : (v[0][0] > 0.f) ? 0 : 255;
           }
-          p.out_cls[px.fpix] = cls;
+          p.out_cls[px.img * plane + px.fpix] = cls;
         }
       }
     } else if (px.ok) {
@@ -352,8 +356,10 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
     uint32_t phase = 0;
     auto next = [&]() { if (++stage == p.stages) { stage = 0; phase ^= 1u; } };
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int ph = static_cast<int>(fast_div(tile, p.mg_tpp));
-      const int r = tile - ph * tiles_per_phase;
+      const int img = static_cast<int>(fast_div(tile, p.mg_ti));
+      const int ti = tile - img * p.tiles_img;
+      const int ph = static_cast<int>(fast_div(ti, p.mg_tpp));
+      const int r = ti - ph * tiles_per_phase;
       const int rn = static_cast<int>(fast_div(r, p.mg_tn));
       const int nt = r - rn * p.tiles_n;
       const int thi = static_cast<int>(fast_div(rn, p.mg_tw));
@@ -370,15 +376,16 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
               const uint32_t full = smem_u32(&bar_full[stage]);
               const uint32_t sa = smem_base + stage * kStageBytes;
               mbar_arrive_expect_tx(full, kStageBytes);
-              tma_load_4d(sa, &mapA, full, c * 64, w0 + ox, h0 + oy, 0);
+              tma_load_4d(sa, &mapA, full, c * 64, w0 + ox, h0 + oy, img);
               tma_load_3d(sa + kATileBytes, &mapB, full, c * 64, n0, ph * 4 + t);
             }
             __syncwarp();
             next();
           }
         }
-        // the nine taps of the skip tensor (output resolution, [h][a][w][b][c] view): hi-res row 2h + a + dy - 1 is
-        // low-res row h + floor(u / 2) of row phase u & 1, u = a + dy - 1; rows / columns outside the image are zero-filled
+        // the nine taps of the skip tensor (output resolution, traversed with element stride 2): output pixel
+        // (2h + a, 2w + b) reads hi-res row 2h + a + dy - 1 = 2 h0 + u (+ 2 lh) and column 2 w0 + v (+ 2 lw);
+        // rows / columns outside the image (of this image: the batch is the map's 4th dimension) are zero-filled
         for (int t2 = 0; t2 < (p.kchunks2 ? 9 : 0); ++t2) {
           const int dy = t2 / 3, dx = t2 - dy * 3;
           const int u = pa + dy - 1, v = pb + dx - 1;
@@ -388,7 +395,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
               const uint32_t full = smem_u32(&bar_full[stage]);
               const uint32_t sa = smem_base + stage * kStageBytes;
               mbar_arrive_expect_tx(full, kStageBytes);
-              tma_load_5d(sa, &mapA2, full, c2 * 64, v & 1, w0 + (v >> 1), u & 1, h0 + (u >> 1));
+              tma_load_4d(sa, &mapA2, full, c2 * 64, 2 * w0 + v, 2 * h0 + u, img);
               tma_load_3d(sa + kATileBytes, &mapB2, full, c2 * 64, n0, t2);
             }
             __syncwarp();
@@ -410,7 +417,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
               const uint32_t full = smem_u32(&bar_full[stage]);
               const uint32_t sa = smem_base + stage * kStageBytes;
               mbar_arrive_expect_tx(full, kStageBytes);
-              tma_load_4d(sa, mA, full, c * 64, w0 * p.stride + dx, h0 * p.stride + dy, 0);
+              tma_load_4d(sa, mA, full, c * 64, w0 * p.stride + dx, h0 * p.stride + dy, img);
               tma_load_3d(sa + kATileBytes, mB, full, c * 64, n0, wsel);
             }
             __syncwarp();
@@ -419,8 +426,9 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
         }
       }
       // fused skip link: the same output pixels seen in the second input (at output resolution);
-      // for a ConvTranspose phase (a,b) that is the pixel set (2h+a, 2w+b), addressed through a
-      // 5-D view [h][a][w][b][c] of the tensor so a plain tiled box picks every second pixel
+      // for a ConvTranspose phase (a,b) that is the pixel set (2h+a, 2w+b), which the second map's
+      // element stride 2 picks from a box starting at (2 h0 + a, 2 w0 + b)
+      const int s2 = p.phases > 1 ? 2 : 1;
       for (int c2 = 0; c2 < p.kchunks2; ++c2) {
         for (int seg = 0; seg < nseg; ++seg) {
           const CUtensorMap* mA = seg == 1 ? &maps.A2lo : &mapA2;
@@ -430,7 +438,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
             const uint32_t full = smem_u32(&bar_full[stage]);
             const uint32_t sa = smem_base + stage * kStageBytes;
             mbar_arrive_expect_tx(full, kStageBytes);
-            tma_load_5d(sa, mA, full, c2 * 64, ph & 1, w0, ph >> 1, h0);
+            tma_load_4d(sa, mA, full, c2 * 64, s2 * w0 + (ph & 1), s2 * h0 + (ph >> 1), img);
             tma_load_3d(sa + kATileBytes, mB, full, c2 * 64, n0, 0);
           }
           __syncwarp();
@@ -470,15 +478,17 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(smem_u32(&bar_empty[prev]));
 
-      const int ph = static_cast<int>(fast_div(tile, p.mg_tpp));
-      const int r = tile - ph * tiles_per_phase;
+      const int img = static_cast<int>(fast_div(tile, p.mg_ti));
+      const int ti = tile - img * p.tiles_img;
+      const int ph = static_cast<int>(fast_div(ti, p.mg_tpp));
+      const int r = ti - ph * tiles_per_phase;
       const int rn = static_cast<int>(fast_div(r, p.mg_tn));
       const int nt = r - rn * p.tiles_n;
       const int thi = static_cast<int>(fast_div(rn, p.mg_tw));
       const int twi = rn - thi * p.tiles_w;
       const int h = thi * p.TH + lh, w = twi * p.TW + lw, n0 = nt * p.BN;
 
-      named_bar_sync(1, kConsumers);         // the previous tile's epilogue is done with the staged accumulator and bias
+      named_bar_sync(1, kConsumers);        // the previous tile's epilogue is done with the staged accumulator and bias
       {
         const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
         float* a0 = acc_s + r0 * kPitch + 2 * (lane & 3);
@@ -506,8 +516,8 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
         EpiPix px;
         px.ok = (h < p.H) && (w < p.W);
         px.zero = false;
-        px.ooff = static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
-        px.roff = 0; px.fpix = 0;
+        px.ooff = img * p.out_img + static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
+        px.roff = 0; px.fpix = 0; px.img = 0;
         if (p.act == ACT_GELU) epilogue_store_fast<E, ACT_GELU, false, true>(p, t_row, n0, s_bias, part, px, gb);
         else epilogue_store_fast<E, ACT_NONE, false, true>(p, t_row, n0, s_bias, part, px, gb);
         continue;
@@ -517,9 +527,10 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
       EpiPix px;
       px.ok = (h < p.H) && (w < p.W);
       px.zero = false;
-      px.ooff = static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
-      px.roff = static_cast<uint32_t>((oh + p.res_pad) * (Wo + 2 * p.res_pad) + (ow + p.res_pad)) * p.ldr;
+      px.ooff = img * p.out_img + static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
+      px.roff = img * p.res_img + static_cast<uint32_t>((oh + p.res_pad) * (Wo + 2 * p.res_pad) + (ow + p.res_pad)) * p.ldr;
       px.fpix = static_cast<uint32_t>(h * p.W + w);
+      px.img = static_cast<uint32_t>(img);
       epilogue_tile<E>(p, t_row, n0, s_bias, part, px);
     }
   }
@@ -527,9 +538,10 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
 
 // Zero border of a zero-bordered [(H+2)][(W+2)][ldo] output (the first nlim channels of each border pixel): the
 // VPB_ALGO_LINEAR contract is that the layer writes the whole padded image, so its output is a valid input for the
-// next 3x3 layer whatever the buffer held before.
+// next 3x3 layer whatever the buffer held before.  blockIdx.y = image of the batch.
 __global__ void zero_border_kernel(uint4* out, int H, int W, int ldo, int nlim) {
   pdl_wait();                // complete only after the convolution before it (the next kernel waits on this one)
+  out += (static_cast<size_t>(blockIdx.y) * (H + 2) * (W + 2) * ldo) >> 3;
   const int per = nlim >> 3, nb = 2 * (W + 2) + 2 * H;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nb * per; i += gridDim.x * blockDim.x) {
     const int pix = i / per, v = i - pix * per;
@@ -645,10 +657,12 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
       return VPB_ERR_ARG;
     }
   }
+  if (a->batch < 0) { vpb_set_error("conv: batch %d", a->batch); return VPB_ERR_ARG; }
+  const int batch = a->batch > 0 ? a->batch : 1;
   {
-    // the epilogue addresses pixels with 32-bit element offsets
+    // the epilogue addresses pixels with 32-bit element offsets, across the whole batch
     const long ho = a->phases == 4 ? 2L * a->H + 2 : a->H + 2, wo = a->phases == 4 ? 2L * a->W + 2 : a->W + 2;
-    if (ho * wo * std::max(a->ldo, a->ldr) >= (1L << 31) || static_cast<long>(a->H) * a->W * 16 >= (1L << 31)) {
+    if (ho * wo * std::max(a->ldo, a->ldr) * batch >= (1L << 31) || static_cast<long>(a->H) * a->W * 16 * batch >= (1L << 31)) {
       vpb_set_error("conv: tensor too large for 32-bit element offsets");
       return VPB_ERR_ARG;
     }
@@ -693,7 +707,14 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
   p.tw_shift = 0; while ((1 << p.tw_shift) < p.TW) ++p.tw_shift;
   p.tiles_h = (a->H + p.TH - 1) / p.TH;
   p.tiles_w = (a->W + p.TW - 1) / p.TW;
-  p.total_tiles = p.tiles_h * p.tiles_w * p.tiles_n * p.phases;
+  p.tiles_img = p.tiles_h * p.tiles_w * p.tiles_n * p.phases;
+  p.total_tiles = p.tiles_img * batch;
+  p.mg_ti = fast_div_magic(p.tiles_img);
+  {
+    const long ho = a->phases == 4 ? 2L * a->H : a->H, wo = a->phases == 4 ? 2L * a->W : a->W;
+    p.out_img = static_cast<uint32_t>((ho + 2 * p.out_pad) * (wo + 2 * p.out_pad) * a->ldo);
+    p.res_img = static_cast<uint32_t>((ho + 2 * p.res_pad) * (wo + 2 * p.res_pad) * a->ldr);
+  }
   const size_t stage_bytes = kATileBytes + static_cast<size_t>(p.BN) * 128;
   p.stages = static_cast<int>(std::min<size_t>(kMaxStages, (kMaxDynSmem - 1024 - acc_bytes(p.BN)) / stage_bytes));
   if (p.stages < 2) { vpb_set_error("conv: no room for the operand ring (BN %d)", p.BN); return VPB_ERR_ARG; }
@@ -705,7 +726,7 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
   p.out_f32 = a->out_f32; p.out_cls = a->out_cls;
   plan->dtype = a->dtype;
   plan->grid = std::min(p.total_tiles, device_sm_count());
-  plan->flops = 2.0 * a->H * a->W * static_cast<double>(a->Cout) * a->phases * (a->Cin * a->taps + p.Cin2 * (upc ? 9 : 1));
+  plan->flops = 2.0 * batch * a->H * a->W * static_cast<double>(a->Cout) * a->phases * (a->Cin * a->taps + p.Cin2 * (upc ? 9 : 1));
 
   const CUtensorMapDataType dt =
       a->dtype == VPB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
@@ -718,7 +739,7 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
       const size_t pitch = static_cast<size_t>(Win + 2 * pad) * a->ldi * 2;
       const uint8_t* base = static_cast<const uint8_t*>(ptr) + pad * pitch + static_cast<size_t>(pad) * a->ldi * 2;
       cuuint64_t dims[4] = {static_cast<cuuint64_t>(a->Cin), static_cast<cuuint64_t>(Win),
-                            static_cast<cuuint64_t>(Hin), 1};
+                            static_cast<cuuint64_t>(Hin), static_cast<cuuint64_t>(batch)};
       cuuint64_t strides[3] = {static_cast<cuuint64_t>(a->ldi) * 2, pitch, pitch * (Hin + 2 * pad)};
       // stride 2: the box spans 2*TW x 2*TH input pixels and is traversed with element stride 2 (TW x TH loaded)
       cuuint32_t box[4] = {64, static_cast<cuuint32_t>(p.TW * cstride), static_cast<cuuint32_t>(p.TH * cstride), 1};
@@ -759,21 +780,22 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
   plan->mapA2lo = plan->mapAlo;
   plan->mapB2lo = plan->mapBlo;
   if (a->in2) {
-    // second input at output resolution, viewed as [h][a][w][b][c] (s = 2 for a ConvTranspose,
-    // a = b = 0 and s = 1 otherwise); box = one pixel tile of one phase
+    // second input at output resolution [batch][s*H][s*W][ld2] (s = 2 for a ConvTranspose, 1 otherwise), addressed
+    // like the first input through its interior; the box spans s*TW x s*TH pixels traversed with element stride s,
+    // so a tile loads the TW x TH pixels of one phase, and rows / columns outside an image (the upconv's skip taps
+    // at hi-res row -1 and 2H) are the TMA unit's zero fill, per image
     auto encA2 = [&](const void* ptr, CUtensorMap* m) {
       const int s2 = a->phases == 4 ? 2 : 1;
       const int pad = a->in2_pad ? 1 : 0;
       const size_t px = static_cast<size_t>(a->ld2) * 2;                       // bytes per pixel
       const size_t pitch = static_cast<size_t>(a->W * s2 + 2 * pad) * px;      // bytes per image row
       const uint8_t* base = static_cast<const uint8_t*>(ptr) + pad * pitch + pad * px;
-      cuuint64_t dims[5] = {static_cast<cuuint64_t>(a->Cin2), static_cast<cuuint64_t>(s2),
-                            static_cast<cuuint64_t>(a->W), static_cast<cuuint64_t>(s2),
-                            static_cast<cuuint64_t>(a->H)};
-      cuuint64_t strides[4] = {px, px * s2, pitch, pitch * s2};
-      cuuint32_t box[5] = {64, 1, static_cast<cuuint32_t>(p.TW), 1, static_cast<cuuint32_t>(p.TH)};
-      cuuint32_t es[5] = {1, 1, 1, 1, 1};
-      return enc(m, dt, 5, const_cast<uint8_t*>(base), dims, strides, box, es,
+      cuuint64_t dims[4] = {static_cast<cuuint64_t>(a->Cin2), static_cast<cuuint64_t>(a->W * s2),
+                            static_cast<cuuint64_t>(a->H * s2), static_cast<cuuint64_t>(batch)};
+      cuuint64_t strides[3] = {px, pitch, pitch * (a->H * s2 + 2 * pad)};
+      cuuint32_t box[4] = {64, static_cast<cuuint32_t>(p.TW * s2), static_cast<cuuint32_t>(p.TH * s2), 1};
+      cuuint32_t es[4] = {1, static_cast<cuuint32_t>(s2), static_cast<cuuint32_t>(s2), 1};
+      return enc(m, dt, 4, const_cast<uint8_t*>(base), dims, strides, box, es,
                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     };
@@ -839,7 +861,7 @@ int conv_plan_launch(const ConvPlan* plan, cudaStream_t stream) {
   if (plan->p.lin) {
     const ConvKParams& p = plan->p;
     const int n = (2 * (p.W + 2) + 2 * p.H) * (p.nlim >> 3);
-    VPB_CUDA_OK(launch_k(zero_border_kernel, dim3(std::min((n + 255) / 256, 256)), dim3(256), 0, stream,
+    VPB_CUDA_OK(launch_k(zero_border_kernel, dim3(std::min((n + 255) / 256, 256), p.total_tiles / p.tiles_img), dim3(256), 0, stream,
                          static_cast<uint4*>(p.out), p.H, p.W, p.ldo, p.nlim));
   }
   return VPB_OK;

@@ -14,7 +14,10 @@ struct ConvKParams {
   int TH, TW, tw_shift;          // spatial tile (TH*TW == 128), log2(TW)
   int BN;                        // N tile: 16, 32, 64 or 128 (the kernel's template parameter)
   int tiles_h, tiles_w, tiles_n; // tile grid
-  int total_tiles;
+  int total_tiles;               // tiles_img * batch: image index outermost, no tile straddles two images
+  int tiles_img;                 // tiles of one image (tiles_n * tiles_h * tiles_w * phases)
+  uint32_t mg_ti;                // magic reciprocal (fast_div) of tiles_img
+  uint32_t out_img, res_img;     // elements between consecutive images of out / res (< 2^31 with the whole batch)
   int kchunks;                   // ceil(Cin / 64)
   int Cin2, kchunks2;            // fused second 1x1 input (skip link), 0 = none
   int stages;                    // shared-memory operand ring depth

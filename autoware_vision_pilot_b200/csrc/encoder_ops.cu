@@ -24,6 +24,11 @@ __global__ void __launch_bounds__(128) stem_conv_kernel(const uint2* __restrict_
                                                          int Ho, int Wo) {
   pdl_launch_dependents();
   pdl_wait();
+  {  // blockIdx.y = image of the batch (split-fp16 tensors are never batched)
+    const size_t img = blockIdx.y;
+    in += img * H * W;
+    out += img * Ho * Wo * 4;
+  }
   __shared__ float sw[27 * 32];
   __shared__ float sb[32];
   for (int i = threadIdx.x; i < 27 * 32; i += blockDim.x) sw[i] = w[i];
@@ -94,7 +99,9 @@ DwGeom dw_geometry(int H, int W, int C, int k, int stride) {
   return g;
 }
 
-template <class E, int K, int S, bool SP>
+// MB: batched launch (blockIdx.y = image); the batch-1 instantiation keeps the single-image code, which the
+// register allocation of this kernel is sensitive to
+template <class E, int K, int S, bool SP, bool MB>
 __global__ void __launch_bounds__(256) depthwise_kernel(const uint4* __restrict__ in, const uint4* __restrict__ in_lo,
                                                          int H, int W,
                                                          int C, const float* __restrict__ w,
@@ -106,6 +113,13 @@ __global__ void __launch_bounds__(256) depthwise_kernel(const uint4* __restrict_
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float red[];  // [PPB][C]
+  // blockIdx.y = image of the batch: its tensors and (below) its own pooling accumulators (split-fp16 tensors are never
+  // batched)
+  if (MB) {
+    in += blockIdx.y * (H * W * G);
+    out += blockIdx.y * (Ho * Wo * G);
+    gap_acc += blockIdx.y * kGapReplicas * C;
+  }
   constexpr int PAD = (K - 1) / 2;
   constexpr int COLS = (kXT - 1) * S + K;   // input columns feeding kXT outputs
   const int cg = threadIdx.x % G, pl = threadIdx.x / G;
@@ -223,6 +237,12 @@ __global__ void __launch_bounds__(512) se_scale_kernel(const long long* __restri
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float sm[];
+  {  // blockIdx.y = image of the batch (split-fp16 tensors are never batched)
+    const size_t img = blockIdx.y;
+    gap_acc += img * kGapReplicas * C;
+    act += img * n8;
+    if (scale_out) scale_out += img * C;
+  }
   float* mean = sm;        // [C]
   float* hid = sm + C;     // [sq]
   float* gate = hid + sq;  // [C]
@@ -312,6 +332,8 @@ __global__ void __launch_bounds__(256) gap_kernel(const typename E::T* __restric
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float part[8][256];
+  in += static_cast<size_t>(blockIdx.y) * HW * ld;    // blockIdx.y = image of the batch
+  out += static_cast<size_t>(blockIdx.y) * C;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c0 = blockIdx.x * 256 + lane * 8;
   float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -356,6 +378,9 @@ __global__ void __launch_bounds__(256) gap_kernel(const typename E::T* __restric
 }
 
 // ------------------------------------------------------------------ GEMV: one warp per output
+// NB input vectors x [NB][in_f] -> y [NB][out_f]: each weight row is read once for all of them, and each vector's
+// dot product is summed in the same order whatever NB is (bit-identical to NB = 1).
+template <int NB>
 __global__ void __launch_bounds__(256) linear_kernel(const float* __restrict__ x,
                                                       const float* __restrict__ w,
                                                       const float* __restrict__ b, int in_f, int out_f,
@@ -366,20 +391,31 @@ __global__ void __launch_bounds__(256) linear_kernel(const float* __restrict__ x
   const int lane = threadIdx.x & 31;
   if (o >= out_f) return;
   const float* wr = w + static_cast<size_t>(o) * in_f;
-  float s = 0.f;
-  for (int i = lane; i < in_f; i += 32) s = fmaf(__ldg(wr + i), __ldg(x + i), s);
+  float s[NB];
 #pragma unroll
-  for (int k = 16; k > 0; k >>= 1) s += __shfl_xor_sync(0xffffffffu, s, k);
+  for (int n = 0; n < NB; ++n) s[n] = 0.f;
+  for (int i = lane; i < in_f; i += 32) {
+    const float wv = __ldg(wr + i);
+#pragma unroll
+    for (int n = 0; n < NB; ++n) s[n] = fmaf(wv, __ldg(x + static_cast<size_t>(n) * in_f + i), s[n]);
+  }
+#pragma unroll
+  for (int n = 0; n < NB; ++n)
+#pragma unroll
+    for (int k = 16; k > 0; k >>= 1) s[n] += __shfl_xor_sync(0xffffffffu, s[n], k);
   if (lane == 0) {
-    s += b[o];
-    if (act == ACT_GELU) s = act_gelu(s);
-    else if (act == ACT_SIGMOID) s = 1.0f / (1.0f + expf(-s));
-    else if (act == ACT_SILU) s = s / (1.0f + expf(-s));
-    else if (act == 4 /* VPB_ACT_SILU2: SiLU(SiLU(x)), CTX block common_layers.py:218-221 */) {
-      s = s / (1.0f + expf(-s));
-      s = s / (1.0f + expf(-s));
+#pragma unroll
+    for (int n = 0; n < NB; ++n) {
+      float v = s[n] + b[o];
+      if (act == ACT_GELU) v = act_gelu(v);
+      else if (act == ACT_SIGMOID) v = 1.0f / (1.0f + expf(-v));
+      else if (act == ACT_SILU) v = v / (1.0f + expf(-v));
+      else if (act == 4 /* VPB_ACT_SILU2: SiLU(SiLU(x)), CTX block common_layers.py:218-221 */) {
+        v = v / (1.0f + expf(-v));
+        v = v / (1.0f + expf(-v));
+      }
+      y[static_cast<size_t>(n) * out_f + o] = v;
     }
-    y[o] = s;
   }
 }
 
@@ -391,6 +427,8 @@ __global__ void ctx_conv1_kernel(const float* __restrict__ in, int H, int W,
                                  int act) {
   pdl_launch_dependents();
   pdl_wait();
+  in += static_cast<size_t>(blockIdx.y) * H * W;     // blockIdx.y = image of the batch (split-fp16: never batched)
+  out += static_cast<size_t>(blockIdx.y) * (H + 2 * out_pad) * (W + 2 * out_pad) * Cout;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= H * W * Cout) return;
   const int co = idx % Cout, pix = idx / Cout;
@@ -413,7 +451,7 @@ __global__ void ctx_conv1_kernel(const float* __restrict__ in, int H, int W,
 // ------------------------------------------------------------------ max-pool feature fusion
 // One warp per (output pixel, source tensor, 8-channel group): lanes split the pooling window,
 // then a shuffle max.  Window = 2^n x 2^n (n successive MaxPool2d(2,2)).
-template <class E>
+template <class E, bool MB>   // MB: batched launch (blockIdx.y = image), as depthwise_kernel
 __global__ void __launch_bounds__(256) fuse_pool_kernel(const uint4* __restrict__ f0,
                                                          const uint4* __restrict__ f1,
                                                          const uint4* __restrict__ f2,
@@ -440,6 +478,10 @@ __global__ void __launch_bounds__(256) fuse_pool_kernel(const uint4* __restrict_
   else if (g < 22) { src = f3; win = 2; G = 10; cg = g - 12; lo_off = lo3; }
   else { src = f4; win = 1; G = 160; cg = g - 22; lo_off = lo4; }
   const int Ws = W4 * win;
+  if (MB) {     // blockIdx.y = image of the batch (split-fp16: never batched)
+    src += static_cast<size_t>(blockIdx.y) * (H4 * win) * Ws * G;
+    out += static_cast<size_t>(blockIdx.y) * H4 * W4 * kGroups;
+  }
   float m[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) m[i] = -INFINITY;
@@ -480,10 +522,10 @@ using namespace vpb;
 
 // `*_lo` arguments of the *_x launchers: the low halves of split-fp16 tensors (NULL = plain 16-bit mode).
 int vpb::stem_conv_x(int dtype, const void* in, const void* in_lo, int H, int W, const float* w, const float* bias,
-                     void* out, void* out_lo, cudaStream_t st) {
+                     void* out, void* out_lo, cudaStream_t st, int batch) {
   const int Ho = H / 2, Wo = W / 2;
   const int n = Ho * Wo;
-  const dim3 g((n + 127) / 128), b(128);
+  const dim3 g((n + 127) / 128, batch), b(128);
   if (dtype == VPB_BF16)
     VPB_CUDA_OK(launch_k(stem_conv_kernel<BF16>, g, b, 0, st, static_cast<const uint2*>(in), static_cast<const uint2*>(in_lo), H, W, w, bias, static_cast<uint4*>(out), static_cast<uint4*>(out_lo), Ho, Wo));
   else
@@ -502,7 +544,7 @@ extern "C" int vpb_depthwise(int dtype, const void* in, int H, int W, int C, int
 }
 int vpb::depthwise_x(int dtype, const void* in, const void* in_lo, int H, int W, int C, int k, int stride,
                      const float* w, const float* bias, void* out, void* out_lo, long long* gap_acc,
-                     cudaStream_t st, int act) {
+                     cudaStream_t st, int act, int batch) {
   if ((C & 7) || (k != 3 && k != 5) || (stride != 1 && stride != 2) || C > 2048) {
     vpb_set_error("depthwise: unsupported C=%d k=%d stride=%d", C, k, stride);
     return VPB_ERR_ARG;
@@ -517,9 +559,11 @@ int vpb::depthwise_x(int dtype, const void* in, const void* in_lo, int H, int W,
   if (sp && !out_lo) { vpb_set_error("depthwise: split mode needs out_lo"); return VPB_ERR_ARG; }
 #define DW_LAUNCH(E, K, S)                                                                             \
   do {                                                                                                 \
-    if (sp) VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, true>, dim3(g.nblocks), dim3(g.threads), smem, st, i4, i4l, H, W, C, \
+    if (sp) VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, true, false>, dim3(g.nblocks), dim3(g.threads), smem, st, i4, i4l, H, W, C, \
                                  w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, act));  \
-    else VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, false>, dim3(g.nblocks), dim3(g.threads), smem, st, i4, i4l, H, W, C, \
+    else if (batch > 1) VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, false, true>, dim3(g.nblocks, batch), dim3(g.threads), smem, st, \
+                              i4, i4l, H, W, C, w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, act)); \
+    else VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, false, false>, dim3(g.nblocks), dim3(g.threads), smem, st, i4, i4l, H, W, C, \
                               w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, act));     \
   } while (0)
 #define DW_DISPATCH(E)                                            \
@@ -541,7 +585,8 @@ extern "C" int vpb_se_scale(int dtype, const long long* gap_acc, int HW, int C, 
   return vpb::se_scale_x(dtype, gap_acc, HW, C, sq, w1, b1, w2, b2, act, nullptr, scale_out, static_cast<cudaStream_t>(stream));
 }
 int vpb::se_scale_x(int dtype, const long long* gap_acc, int HW, int C, int sq, const float* w1, const float* b1,
-                    const float* w2, const float* b2, void* act, void* act_lo, float* scale_out, cudaStream_t st) {
+                    const float* w2, const float* b2, void* act, void* act_lo, float* scale_out, cudaStream_t st,
+                    int batch) {
   const size_t smem = (2 * static_cast<size_t>(C) + sq) * sizeof(float);
   if ((C & 7) || C > 1152 || sq > 48 || !act) { vpb_set_error("se_scale: unsupported C=%d sq=%d", C, sq); return VPB_ERR_ARG; }
   // every block recomputes the gate (reads w1 + w2: 8*C*sq bytes), so the grid follows the activation bytes: one block
@@ -549,10 +594,10 @@ int vpb::se_scale_x(int dtype, const long long* gap_acc, int HW, int C, int sq, 
   const int n8 = HW * (C / 8);
   const int grid = std::max(1, std::min(264, (n8 * 16 + 65535) / 65536));
   if (dtype == VPB_BF16)
-    VPB_CUDA_OK(launch_k(se_scale_kernel<BF16>, dim3(grid), dim3(512), smem, st, gap_acc, 1.0f / HW, C, sq, w1, b1, w2, b2,
+    VPB_CUDA_OK(launch_k(se_scale_kernel<BF16>, dim3(grid, batch), dim3(512), smem, st, gap_acc, 1.0f / HW, C, sq, w1, b1, w2, b2,
                          static_cast<uint4*>(act), static_cast<uint4*>(act_lo), n8, scale_out));
   else
-    VPB_CUDA_OK(launch_k(se_scale_kernel<F16>, dim3(grid), dim3(512), smem, st, gap_acc, 1.0f / HW, C, sq, w1, b1, w2, b2,
+    VPB_CUDA_OK(launch_k(se_scale_kernel<F16>, dim3(grid, batch), dim3(512), smem, st, gap_acc, 1.0f / HW, C, sq, w1, b1, w2, b2,
                          static_cast<uint4*>(act), static_cast<uint4*>(act_lo), n8, scale_out));
   return VPB_OK;
 }
@@ -560,17 +605,32 @@ int vpb::se_scale_x(int dtype, const long long* gap_acc, int HW, int C, int sq, 
 extern "C" int vpb_gap(int dtype, const void* in, int HW, int C, int ld, float* out, void* stream) {
   return vpb::gap_x(dtype, in, nullptr, HW, C, ld, out, static_cast<cudaStream_t>(stream));
 }
-int vpb::gap_x(int dtype, const void* in, const void* in_lo, int HW, int C, int ld, float* out, cudaStream_t st) {
+int vpb::gap_x(int dtype, const void* in, const void* in_lo, int HW, int C, int ld, float* out, cudaStream_t st, int batch) {
   if (dtype == VPB_BF16)
-    VPB_CUDA_OK(launch_k(gap_kernel<BF16>, dim3((C + 255) / 256), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(in), static_cast<const __nv_bfloat16*>(in_lo), HW, C, ld, out));
+    VPB_CUDA_OK(launch_k(gap_kernel<BF16>, dim3((C + 255) / 256, batch), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(in), static_cast<const __nv_bfloat16*>(in_lo), HW, C, ld, out));
   else
-    VPB_CUDA_OK(launch_k(gap_kernel<F16>, dim3((C + 255) / 256), dim3(256), 0, st, static_cast<const __half*>(in), static_cast<const __half*>(in_lo), HW, C, ld, out));
+    VPB_CUDA_OK(launch_k(gap_kernel<F16>, dim3((C + 255) / 256, batch), dim3(256), 0, st, static_cast<const __half*>(in), static_cast<const __half*>(in_lo), HW, C, ld, out));
   return VPB_OK;
 }
 
 extern "C" int vpb_linear(const float* x, const float* w, const float* b, int in_f, int out_f, int act,
                           float* y, void* stream) {
-  VPB_CUDA_OK(launch_k(linear_kernel, dim3((out_f + 7) / 8), dim3(256), 0, static_cast<cudaStream_t>(stream), x, w, b, in_f, out_f, act, y));
+  return vpb::linear_x(x, w, b, in_f, out_f, act, y, static_cast<cudaStream_t>(stream), 1);
+}
+int vpb::linear_x(const float* x, const float* w, const float* b, int in_f, int out_f, int act, float* y, cudaStream_t st,
+                  int batch) {
+  const dim3 g((out_f + 7) / 8), blk(256);
+  switch (batch) {
+    case 1: VPB_CUDA_OK(launch_k(linear_kernel<1>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
+    case 2: VPB_CUDA_OK(launch_k(linear_kernel<2>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
+    case 3: VPB_CUDA_OK(launch_k(linear_kernel<3>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
+    case 4: VPB_CUDA_OK(launch_k(linear_kernel<4>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
+    case 5: VPB_CUDA_OK(launch_k(linear_kernel<5>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
+    case 6: VPB_CUDA_OK(launch_k(linear_kernel<6>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
+    case 7: VPB_CUDA_OK(launch_k(linear_kernel<7>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
+    case 8: VPB_CUDA_OK(launch_k(linear_kernel<8>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
+    default: vpb_set_error("linear: batch %d (1..%d)", batch, kMaxBatch); return VPB_ERR_ARG;
+  }
   return VPB_OK;
 }
 
@@ -579,12 +639,12 @@ extern "C" int vpb_ctx_conv1(int dtype, const float* in, int H, int W, const flo
   return vpb::ctx_conv1_x(dtype, in, H, W, w, b, Cout, out, nullptr, out_pad, static_cast<cudaStream_t>(stream));
 }
 int vpb::ctx_conv1_x(int dtype, const float* in, int H, int W, const float* w, const float* b, int Cout, void* out,
-                     void* out_lo, int out_pad, cudaStream_t st, int act) {
+                     void* out_lo, int out_pad, cudaStream_t st, int act, int batch) {
   const int n = H * W * Cout;
   if (dtype == VPB_BF16)
-    VPB_CUDA_OK(launch_k(ctx_conv1_kernel<BF16>, dim3((n + 255) / 256), dim3(256), 0, st, in, H, W, w, b, Cout, static_cast<__nv_bfloat16*>(out), static_cast<__nv_bfloat16*>(out_lo), out_pad, act));
+    VPB_CUDA_OK(launch_k(ctx_conv1_kernel<BF16>, dim3((n + 255) / 256, batch), dim3(256), 0, st, in, H, W, w, b, Cout, static_cast<__nv_bfloat16*>(out), static_cast<__nv_bfloat16*>(out_lo), out_pad, act));
   else
-    VPB_CUDA_OK(launch_k(ctx_conv1_kernel<F16>, dim3((n + 255) / 256), dim3(256), 0, st, in, H, W, w, b, Cout, static_cast<__half*>(out), static_cast<__half*>(out_lo), out_pad, act));
+    VPB_CUDA_OK(launch_k(ctx_conv1_kernel<F16>, dim3((n + 255) / 256, batch), dim3(256), 0, st, in, H, W, w, b, Cout, static_cast<__half*>(out), static_cast<__half*>(out_lo), out_pad, act));
   return VPB_OK;
 }
 
@@ -595,14 +655,19 @@ extern "C" int vpb_fuse_pool_concat(int dtype, const void* f0, const void* f1, c
   return vpb::fuse_pool_x(dtype, f0, f1, f2, f3, f4, z, H4, W4, out, nullptr, static_cast<cudaStream_t>(stream));
 }
 int vpb::fuse_pool_x(int dtype, const void* f0, const void* f1, const void* f2, const void* f3, const void* f4,
-                     const size_t lo_off[5], int H4, int W4, void* out, void* out_lo, cudaStream_t st) {
+                     const size_t lo_off[5], int H4, int W4, void* out, void* out_lo, cudaStream_t st, int batch) {
   const long warps = static_cast<long>(H4) * W4 * 182;
   const int blocks = static_cast<int>((warps * 32 + 255) / 256);
 #define FP_ARGS static_cast<const uint4*>(f0), static_cast<const uint4*>(f1), static_cast<const uint4*>(f2), \
                 static_cast<const uint4*>(f3), static_cast<const uint4*>(f4), H4, W4, static_cast<uint4*>(out), \
                 lo_off[0], lo_off[1], lo_off[2], lo_off[3], lo_off[4], static_cast<uint4*>(out_lo)
-  if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(fuse_pool_kernel<BF16>, dim3(blocks), dim3(256), 0, st, FP_ARGS));
-  else VPB_CUDA_OK(launch_k(fuse_pool_kernel<F16>, dim3(blocks), dim3(256), 0, st, FP_ARGS));
+  if (batch > 1) {
+    if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(fuse_pool_kernel<BF16, true>, dim3(blocks, batch), dim3(256), 0, st, FP_ARGS));
+    else VPB_CUDA_OK(launch_k(fuse_pool_kernel<F16, true>, dim3(blocks, batch), dim3(256), 0, st, FP_ARGS));
+  } else {
+    if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(fuse_pool_kernel<BF16, false>, dim3(blocks), dim3(256), 0, st, FP_ARGS));
+    else VPB_CUDA_OK(launch_k(fuse_pool_kernel<F16, false>, dim3(blocks), dim3(256), 0, st, FP_ARGS));
+  }
 #undef FP_ARGS
   return VPB_OK;
 }

@@ -14,6 +14,7 @@
 #include "../../include/vp_b200.h"
 #include "engine_internal.h"
 
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -139,6 +140,9 @@ struct vp_engine {
   void* lo(const void* hi) const { auto it = lo_of.find(hi); return it == lo_of.end() ? nullptr : it->second; }
   void* d_pre_lo = nullptr;
   int dtype = VPB_F16;
+  // frames per call (vp_engine_config.batch): every activation, the pre-process output and the model outputs hold
+  // `batch` samples back to back (batch outermost); weights, the launch list and the graph are those of one call
+  int batch = 1;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   std::vector<void*> dev_allocs;
@@ -155,13 +159,14 @@ struct vp_engine {
   std::vector<ModelOut> outs;
   std::map<std::string, Tens> taps;
   int shared_encoders = 0, shared_trunks = 0;
-  // SE pooling accumulators of every MBConv block: one arena, zeroed by one memset per frame
+  // SE pooling accumulators of every MBConv block: one arena, zeroed by one memset per frame; one accumulator set per
+  // sample of the batch
   long long* d_gap = nullptr; size_t gap_used = 0;
-  static constexpr size_t kGapCap = 512 * 1024;  // int64 slots (16 blocks x <=1152 ch x 8 replicas per encoder)
+  static constexpr size_t kGapCap = 512 * 1024;  // int64 slots per sample (16 blocks x <=1152 ch x 8 replicas per encoder)
   long long* gap_alloc(int C) {
-    if (!d_gap) d_gap = static_cast<long long*>(dalloc(kGapCap * 8, false));
-    const size_t need = static_cast<size_t>(C) * kGapReplicas;
-    if (gap_used + need > kGapCap) return nullptr;
+    if (!d_gap) d_gap = static_cast<long long*>(dalloc(kGapCap * batch * 8, false));
+    const size_t need = static_cast<size_t>(C) * kGapReplicas * batch;
+    if (gap_used + need > kGapCap * batch) return nullptr;
     long long* p = d_gap + gap_used;
     gap_used += (need + 31) / 32 * 32;
     return p;
@@ -169,7 +174,8 @@ struct vp_engine {
   // graph
   cudaGraphExec_t gexec = nullptr;
   cudaGraph_t graph = nullptr;           // kept alive: g_pre_node is a handle into it
-  int g_h = 0, g_w = 0, g_stride = 0; const uint8_t* g_src = nullptr;
+  int g_h = 0, g_w = 0, g_stride = 0;
+  std::array<const uint8_t*, kMaxBatch> g_src{};   // frames of the captured / last call ([0] == NULL: none yet)
   cudaGraphNode_t g_pre_node = nullptr;  // the captured pre-process kernel node (re-pointed per frame)
   // module caches for sharing
   struct EncOut { Tens f[5]; };
@@ -219,7 +225,7 @@ struct vp_engine {
   }
   Tens act_alloc(int H, int W, int C, int pad = 0) {
     Tens a; a.H = H; a.W = W; a.C = C; a.pad = pad;
-    a.p = dalloc(a.bytes() * (split ? 2 : 1), false);
+    a.p = dalloc(a.bytes() * batch * (split ? 2 : 1), false);
     if (split && a.p) a.lo = static_cast<uint8_t*>(a.p) + a.bytes();
     return a;
   }
@@ -254,6 +260,7 @@ struct vp_engine {
                int final_kind = 0, float* out_f32 = nullptr, uint8_t* out_cls = nullptr,
                const Tens* in2 = nullptr, const void* w2 = nullptr, int taps2 = 0) {
     vpb_conv_args a{};
+    a.batch = batch;
     a.dtype = dtype; a.H = in.H; a.W = in.W; a.Cin = in.C; a.ldi = in.C;
     a.Cout = Cout; a.taps = taps; a.phases = phases; a.act = act; a.mode = mode;
     a.final_kind = final_kind; a.in = in.p; a.w = w; a.bias = bias;
@@ -283,9 +290,10 @@ struct vp_engine {
     ops.push_back(std::move(op));
     return VPB_OK;
   }
+  // flops: per sample (counted for the whole batch); bytes: per launch
   void add_op(const std::string& name, const char* kname, std::function<int(cudaStream_t)> fn, double flops = 0,
               double bytes = 0) {
-    OpRec op; op.name = name; op.kname = kname; op.launch = std::move(fn); op.flops = flops; op.bytes = bytes; op.lane = cur_lane;
+    OpRec op; op.name = name; op.kname = kname; op.launch = std::move(fn); op.flops = flops * batch; op.bytes = bytes; op.lane = cur_lane;
     ops.push_back(std::move(op));
   }
 };
@@ -361,7 +369,7 @@ static const int kStages[7][6] = {  // expand, kernel, stride, cin, cout, repeat
 // ---------------------------------------------------------------- encoder (backbone.py:11-22)
 static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p, const std::string& tag,
                          vp_engine::EncOut& out) {
-  const int dt = e.dtype;
+  const int dt = e.dtype, nb = e.batch;
   std::vector<float> s, t;
   // stem
   const HostTensor* sw = find_w_shaped(w, p + "0.0.weight", {32, 3, 3, 3});
@@ -376,8 +384,8 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
   {
     const void* in = e.d_pre; void* o = x.p;
     const void* in_lo = e.d_pre_lo; void* o_lo = x.lo;
-    e.add_op(tag + "stem", "stem_conv_kernel", [=](cudaStream_t st) { return stem_conv_x(dt, in, in_lo, kNetH, kNetW, d_stem, d_stem_b, o, o_lo, st); },
-             2.0 * x.H * x.W * 32 * 27, 2.0 * kNetH * kNetW * 4 + 2.0 * x.H * x.W * 32);
+    e.add_op(tag + "stem", "stem_conv_kernel", [=](cudaStream_t st) { return stem_conv_x(dt, in, in_lo, kNetH, kNetW, d_stem, d_stem_b, o, o_lo, st, nb); },
+             2.0 * x.H * x.W * 32 * 27, nb * (2.0 * kNetH * kNetW * 4 + 2.0 * x.H * x.W * 32));
   }
   Tens stage_out[9];
   stage_out[0] = x;
@@ -414,8 +422,8 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
       {
         const void* in = cur.p; void* o = dwo.p; const int H = cur.H, W = cur.W;
         const void* in_lo = cur.lo; void* o_lo = dwo.lo;
-        e.add_op(nm + "dw", "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, in, in_lo, H, W, ce, k, s_, d_dw, d_dwb, o, o_lo, d_part, st); },
-                 2.0 * g.Ho * g.Wo * ce * k * k, 2.0 * H * W * ce + 2.0 * g.Ho * g.Wo * ce);
+        e.add_op(nm + "dw", "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, in, in_lo, H, W, ce, k, s_, d_dw, d_dwb, o, o_lo, d_part, st, 1, nb); },
+                 2.0 * g.Ho * g.Wo * ce * k * k, nb * (2.0 * H * W * ce + 2.0 * g.Ho * g.Wo * ce));
       }
       // SE gate applied to the depthwise output in place (where the reference graph applies it), then a plain 1x1
       const std::string sp = bp + std::to_string(bi + 1) + ".";
@@ -434,8 +442,8 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
         const int HW = g.Ho * g.Wo;
         void* act = dwo.p; void* act_lo = dwo.lo;
         e.add_op(nm + "se", "se_scale_kernel", [=](cudaStream_t st) {
-          return se_scale_x(dt, d_part, HW, ce, sq, d_f1, d_b1, d_f2, d_b2, act, act_lo, nullptr, st);
-        }, 2.0 * (2.0 * ce * sq), 8.0 * ce * kGapReplicas + 8.0 * ce * sq + 4.0 * HW * ce);
+          return se_scale_x(dt, d_part, HW, ce, sq, d_f1, d_b1, d_f2, d_b2, act, act_lo, nullptr, st, nb);
+        }, 2.0 * (2.0 * ce * sq), nb * (8.0 * ce * kGapReplicas + 4.0 * HW * ce) + 8.0 * ce * sq);
       }
       // 1x1 project + BN (+ residual; StochasticDepth is identity in eval)
       const bool residual = (s_ == 1 && ci == cout);
@@ -574,18 +582,18 @@ static int upconv_layer(vp_engine& e, const WeightMap& w, const std::string& p, 
   rc = e.add_conv(tag + "up" + std::to_string(i) + "dec" + std::to_string(dec), in, Cout, 4, 4, d_wf16, d_b9, ACT_GELU,
                   VPB_EPI_STORE, out, nullptr, 0, nullptr, nullptr, skip, d_w216, C2 ? 9 : 0);
   if (rc == VPB_OK)   // what the reference's three layers cost: ConvTranspose + skip 1x1 at 4 phases, then the 3x3 at 2H x 2W
-    e.ops.back().flops_ref = 2.0 * in.H * in.W * 4.0 * Cmid * (Cin + C2) + 2.0 * (4.0 * in.H * in.W) * Cout * 9.0 * Cmid;
+    e.ops.back().flops_ref = e.batch * (2.0 * in.H * in.W * 4.0 * Cmid * (Cin + C2) + 2.0 * (4.0 * in.H * in.W) * Cout * 9.0 * Cmid);
   return rc;
 }
 
 // SceneContext / DepthContext / AutoSteerContext (scene_context.py:25-57)
 static int build_context(vp_engine& e, const WeightMap& w, const std::string& p, const std::string& tag,
                          const Tens& feat, Tens* ctx) {
-  const int dt = e.dtype, C = feat.C, HW = feat.H * feat.W;
-  float* d_v = static_cast<float*>(e.dalloc(C * 4, false));
+  const int dt = e.dtype, C = feat.C, HW = feat.H * feat.W, nb = e.batch;
+  float* d_v = static_cast<float*>(e.dalloc(static_cast<size_t>(C) * 4 * nb, false));   // [batch][C]: per-sample context vectors
   {
     const void* in = feat.p; const void* in_lo = feat.lo;
-    e.add_op(tag + "gap", "gap_kernel", [=](cudaStream_t st) { return gap_x(dt, in, in_lo, HW, C, C, d_v, st); }, 0.0, 2.0 * HW * C);
+    e.add_op(tag + "gap", "gap_kernel", [=](cudaStream_t st) { return gap_x(dt, in, in_lo, HW, C, C, d_v, st, nb); }, 0.0, nb * 2.0 * HW * C);
   }
   const int dims[4] = {C, 800, 800, 200};
   const int acts[3] = {ACT_GELU, ACT_GELU, ACT_SIGMOID};
@@ -595,10 +603,10 @@ static int build_context(vp_engine& e, const WeightMap& w, const std::string& p,
     const HostTensor *wt = find_w_shaped(w, k + ".weight", {dims[i + 1], dims[i]}), *bt = find_w_shaped(w, k + ".bias", {dims[i + 1]});
     if (!wt || !bt) return VPB_ERR_IO;
     float *dw_ = e.upload_f32(wt->f), *db = e.upload_f32(bt->f);
-    float* y = static_cast<float*>(e.dalloc(dims[i + 1] * 4, false));
+    float* y = static_cast<float*>(e.dalloc(static_cast<size_t>(dims[i + 1]) * 4 * nb, false));
     const int in_f = dims[i], out_f = dims[i + 1], a = acts[i];
     const float* xin = cur;
-    e.add_op(tag + "mlp" + std::to_string(i), "linear_kernel", [=](cudaStream_t st) { return vpb_linear(xin, dw_, db, in_f, out_f, a, y, st); },
+    e.add_op(tag + "mlp" + std::to_string(i), "linear_kernel", [=](cudaStream_t st) { return linear_x(xin, dw_, db, in_f, out_f, a, y, st, nb); },
              2.0 * in_f * out_f, 4.0 * in_f * out_f);
     cur = y;
   }
@@ -608,8 +616,8 @@ static int build_context(vp_engine& e, const WeightMap& w, const std::string& p,
   Tens c4 = e.act_alloc(feat.H, feat.W, 128, /*pad=*/1);
   {
     const float* xin = cur; void* o = c4.p; void* o_lo = c4.lo; const int H = feat.H, W = feat.W;
-    e.add_op(tag + "ctx3", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, xin, H, W, d_w3, d_b3, 128, o, o_lo, 1, st); },
-             2.0 * HW * 128 * 9, 2.0 * (H + 2) * (W + 2) * 128);
+    e.add_op(tag + "ctx3", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, xin, H, W, d_w3, d_b3, 128, o, o_lo, 1, st, 1, nb); },
+             2.0 * HW * 128 * 9, nb * 2.0 * (H + 2) * (W + 2) * 128);
   }
   Tens c5, c6;
   int rc = conv_layer(e, w, p + "context_layer_4", tag + "ctx4", c4, 9, ACT_GELU, VPB_EPI_STORE, &c5, nullptr);
@@ -655,14 +663,15 @@ static int final_conv(vp_engine& e, const WeightMap& w, const std::string& key, 
   float* db = e.upload_f32(bt->f);
   mo.C = Cout; mo.H = in.H; mo.W = in.W;
   const size_t n = static_cast<size_t>(Cout) * in.H * in.W;
-  mo.d_raw = static_cast<float*>(e.dalloc(n * 4, false));
+  const size_t nb = e.batch;     // [batch][C][H][W] fp32 and [batch][H][W] uint8
+  mo.d_raw = static_cast<float*>(e.dalloc(n * 4 * nb, false));
   mo.has_cls = final_kind != VPB_FINAL_NONE;
-  if (mo.has_cls) mo.d_cls = static_cast<uint8_t*>(e.dalloc(static_cast<size_t>(in.H) * in.W, false));
+  if (mo.has_cls) mo.d_cls = static_cast<uint8_t*>(e.dalloc(static_cast<size_t>(in.H) * in.W * nb, false));
   void* hp = nullptr;
-  if (cudaMallocHost(&hp, n * 4) != cudaSuccess) { vpb_set_error("cudaMallocHost failed"); return VPB_ERR_CUDA; }
+  if (cudaMallocHost(&hp, n * 4 * nb) != cudaSuccess) { vpb_set_error("cudaMallocHost failed"); return VPB_ERR_CUDA; }
   e.host_allocs.push_back(hp); mo.h_raw = static_cast<float*>(hp);
   if (mo.has_cls) {
-    if (cudaMallocHost(&hp, static_cast<size_t>(in.H) * in.W) != cudaSuccess) { vpb_set_error("cudaMallocHost failed"); return VPB_ERR_CUDA; }
+    if (cudaMallocHost(&hp, static_cast<size_t>(in.H) * in.W * nb) != cudaSuccess) { vpb_set_error("cudaMallocHost failed"); return VPB_ERR_CUDA; }
     e.host_allocs.push_back(hp); mo.h_cls = static_cast<uint8_t*>(hp);
   }
   return e.add_conv(name, in, Cout, 9, 1, dw_, db, ACT_NONE, VPB_EPI_FINAL, nullptr, nullptr, final_kind, mo.d_raw, mo.d_cls);
@@ -726,8 +735,9 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
       struct LoOff { size_t v[5]; } lo{};
       for (int i = 0; i < 5; ++i)
         lo.v[i] = enc.f[i].lo ? static_cast<size_t>(static_cast<const uint8_t*>(enc.f[i].lo) - static_cast<const uint8_t*>(enc.f[i].p)) : 0;
-      e.add_op(tag + "fuse", "fuse_pool_kernel", [=](cudaStream_t st) { return fuse_pool_x(dt, f0, f1, f2, f3, f4, lo.v, H4, W4, o, o_lo, st); },
-               0.0, 2.0 * (160.0 * 320 * 32 + 80.0 * 160 * 24 + 40.0 * 80 * 40 + 20.0 * 40 * 80 + 200.0 * 1280 + 200.0 * 1456));
+      const int nb = e.batch;
+      e.add_op(tag + "fuse", "fuse_pool_kernel", [=](cudaStream_t st) { return fuse_pool_x(dt, f0, f1, f2, f3, f4, lo.v, H4, W4, o, o_lo, st, nb); },
+               0.0, nb * 2.0 * (160.0 * 320 * 32 + 80.0 * 160 * 24 + 40.0 * 80 * 40 + 20.0 * 40 * 80 + 200.0 * 1280 + 200.0 * 1456));
       e.taps[tag + "fused"] = feat;
     }
     Tens ctx;
@@ -777,13 +787,13 @@ static int prepare_lanes(vp_engine& e) {
   return VPB_OK;
 }
 
-static int launch_all(vp_engine& e, const uint8_t* src_dev, int stride, cudaStream_t st) {
+static int launch_all(vp_engine& e, const uint8_t* const* srcs, int stride, cudaStream_t st) {
   int rc = prepare_lanes(e);
   if (rc) return rc;
   const size_t nl = e.lane_dep.size();
   const bool multi = nl > 1 && e.cfg.single_stream == 0;
   if (e.d_gap) VPB_CUDA_OK(cudaMemsetAsync(e.d_gap, 0, e.gap_used * 8, st));
-  rc = e.pre.launch(src_dev, stride, e.cfg.convention, e.dtype, e.d_pre, e.d_resized, st);
+  rc = e.pre.launch(srcs, e.batch, stride, e.cfg.convention, e.dtype, e.d_pre, e.d_resized, st);
   if (rc) return rc;
   if (!multi) {
     for (auto& op : e.ops) { rc = op.launch(st); if (rc) return rc; }
@@ -811,27 +821,30 @@ static int launch_all(vp_engine& e, const uint8_t* src_dev, int stride, cudaStre
   return VPB_OK;
 }
 
-// Enqueue one frame's kernels (graph replay when enabled and the geometry is unchanged).
-static int enqueue_frame(vp_engine& e, const uint8_t* src_dev, int h, int w, int stride) {
+// Enqueue one call's kernels for the e.batch frames srcs[0 .. batch-1] (graph replay when enabled and the geometry
+// is unchanged).
+static int enqueue_frame(vp_engine& e, const uint8_t* const* srcs, int h, int w, int stride) {
   int rc = e.pre.configure(h, w, e.cfg.resize_mode);
   if (rc) return rc;
-  if (!e.cfg.use_graph) return launch_all(e, src_dev, stride, e.stream);
-  if (e.gexec && e.g_h == h && e.g_w == w && e.g_stride == stride && e.g_src != src_dev && e.g_pre_node) {
-    // same geometry, different frame buffer: re-point the pre-process node instead of re-capturing
-    rc = e.pre.update_graph_node(e.gexec, e.g_pre_node, src_dev, stride, e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
+  std::array<const uint8_t*, kMaxBatch> src{};
+  std::copy(srcs, srcs + e.batch, src.begin());
+  if (!e.cfg.use_graph) return launch_all(e, src.data(), stride, e.stream);
+  if (e.gexec && e.g_h == h && e.g_w == w && e.g_stride == stride && e.g_src != src && e.g_pre_node) {
+    // same geometry, different frame buffers: re-point the pre-process node instead of re-capturing
+    rc = e.pre.update_graph_node(e.gexec, e.g_pre_node, src.data(), e.batch, stride, e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
     if (rc) return rc;
-    e.g_src = src_dev;
+    e.g_src = src;
   }
-  if (!e.gexec || e.g_h != h || e.g_w != w || e.g_stride != stride || e.g_src != src_dev) {
+  if (!e.gexec || e.g_h != h || e.g_w != w || e.g_stride != stride || e.g_src != src) {
     if (e.gexec) { cudaGraphExecDestroy(e.gexec); e.gexec = nullptr; }
     e.g_pre_node = nullptr;
     // warm (sets function attributes outside capture), then capture
-    rc = launch_all(e, src_dev, stride, e.stream);
+    rc = launch_all(e, src.data(), stride, e.stream);
     if (rc) return rc;
     VPB_CUDA_OK(cudaStreamSynchronize(e.stream));
     cudaGraph_t g = nullptr;
     VPB_CUDA_OK(cudaStreamBeginCapture(e.stream, cudaStreamCaptureModeThreadLocal));
-    rc = launch_all(e, src_dev, stride, e.stream);
+    rc = launch_all(e, src.data(), stride, e.stream);
     cudaError_t ce = cudaStreamEndCapture(e.stream, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
     if (ce != cudaSuccess) { vpb_set_error("graph capture failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
@@ -854,7 +867,7 @@ static int enqueue_frame(vp_engine& e, const uint8_t* src_dev, int h, int w, int
     if (e.graph) cudaGraphDestroy(e.graph);
     e.graph = g;
     if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    e.g_h = h; e.g_w = w; e.g_stride = stride; e.g_src = src_dev;
+    e.g_h = h; e.g_w = w; e.g_stride = stride; e.g_src = src;
   }
   VPB_CUDA_OK(cudaGraphLaunch(e.gexec, e.stream));
   return VPB_OK;
@@ -896,12 +909,22 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
     return VPB_ERR_ARG;
   }
   e->split = cfg->precision == VP_PREC_SPLIT;
+  static_assert(kMaxBatch == VP_MAX_BATCH, "ops_internal.h kMaxBatch mirrors VP_MAX_BATCH");
+  if (cfg->batch < 0 || cfg->batch > VP_MAX_BATCH) {
+    vpb_set_error("vp_engine_create: batch %d out of range (0..%d)", cfg->batch, VP_MAX_BATCH);
+    return VPB_ERR_ARG;
+  }
+  e->batch = cfg->batch > 1 ? cfg->batch : 1;
+  if (e->batch > 1 && e->split) {
+    vpb_set_error("vp_engine_create: batch > 1 needs the 16-bit precision (the split-fp16 mode runs one frame per call)");
+    return VPB_ERR_ARG;
+  }
   if (cfg->stream) e->stream = static_cast<cudaStream_t>(cfg->stream);
   else { VPB_CUDA_OK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking)); e->own_stream = true; }
-  e->d_pre = e->dalloc(static_cast<size_t>(kNetH) * kNetW * 4 * 2 * (e->split ? 2 : 1), false);
+  e->d_pre = e->dalloc(static_cast<size_t>(kNetH) * kNetW * 4 * 2 * e->batch * (e->split ? 2 : 1), false);
   if (e->split && e->d_pre) e->d_pre_lo = static_cast<uint8_t*>(e->d_pre) + static_cast<size_t>(kNetH) * kNetW * 4 * 2;
   e->pre.out_lo = e->d_pre_lo;
-  e->d_resized = static_cast<uint8_t*>(e->dalloc(static_cast<size_t>(kNetH) * kNetW * 3, false));
+  e->d_resized = static_cast<uint8_t*>(e->dalloc(static_cast<size_t>(kNetH) * kNetW * 3 * e->batch, false));
   {
     Tens pre; pre.p = e->d_pre; pre.lo = e->d_pre_lo; pre.H = kNetH; pre.W = kNetW; pre.C = 4;
     e->taps["pre"] = pre;
@@ -941,10 +964,27 @@ extern "C" uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes) {
   return e->h_frame;
 }
 
-extern "C" int vp_engine_infer_device(vp_engine* e, const uint8_t* frame_dev, int h, int w, int stride) {
-  if (!e || !frame_dev || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("vp_engine_infer_device: bad arguments"); return VPB_ERR_ARG; }
+// n frames of one geometry, n == the engine's batch
+static bool frames_ok(const vp_engine* e, const uint8_t* const* frames, int n, int h, int w, int stride, const char* who) {
+  if (!e || !frames || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("%s: bad arguments", who); return false; }
+  if (n != e->batch) {
+    vpb_set_error("%s: %d frame(s) for an engine of batch %d%s", who, n, e->batch,
+                  n == 1 ? " (use the *_batch calls)" : "");
+    return false;
+  }
+  for (int k = 0; k < n; ++k)
+    if (!frames[k]) { vpb_set_error("%s: frame %d is NULL", who, k); return false; }
+  return true;
+}
+
+extern "C" int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev, int n, int h, int w, int stride) {
+  if (!frames_ok(e, frames_dev, n, h, w, stride, "vp_engine_infer_device")) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  return enqueue_frame(*e, frame_dev, h, w, stride);
+  return enqueue_frame(*e, frames_dev, h, w, stride);
+}
+
+extern "C" int vp_engine_infer_device(vp_engine* e, const uint8_t* frame_dev, int h, int w, int stride) {
+  return vp_engine_infer_device_batch(e, &frame_dev, 1, h, w, stride);
 }
 
 extern "C" int vp_engine_sync(vp_engine* e) {
@@ -954,58 +994,74 @@ extern "C" int vp_engine_sync(vp_engine* e) {
   return VPB_OK;
 }
 
-static int submit_host_frame(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride, bool sync);
-
-extern "C" int vp_engine_infer(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride) {
-  return submit_host_frame(e, frame_host, h, w, stride, true);
-}
-
-extern "C" int vp_engine_submit(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride) {
-  return submit_host_frame(e, frame_host, h, w, stride, false);
-}
-
-static int submit_host_frame(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride, bool sync) {
-  if (!e || !frame_host || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("vp_engine_infer: bad arguments"); return VPB_ERR_ARG; }
+static int submit_host_frames(vp_engine* e, const uint8_t* const* frames, int n, int h, int w, int stride, bool sync) {
+  if (!frames_ok(e, frames, n, h, w, stride, sync ? "vp_engine_infer" : "vp_engine_submit")) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
   // The device copy is tightly packed (pitch w*3): only the w*3 valid bytes of every row are read from the
   // caller's buffer, so a cv::Mat ROI / strided view is never read past its last row's end.
   const int dpitch = w * 3;
   const size_t bytes = static_cast<size_t>(h) * dpitch;
-  int rc = ensure_frame_buffers(*e, bytes);
+  int rc = ensure_frame_buffers(*e, bytes * n);
   if (rc) return rc;
-  if (stride == dpitch) VPB_CUDA_OK(cudaMemcpyAsync(e->d_frame, frame_host, bytes, cudaMemcpyHostToDevice, e->stream));
-  else VPB_CUDA_OK(cudaMemcpy2DAsync(e->d_frame, dpitch, frame_host, stride, dpitch, h, cudaMemcpyHostToDevice, e->stream));
-  rc = enqueue_frame(*e, e->d_frame, h, w, dpitch);
+  std::array<const uint8_t*, kMaxBatch> dev{};
+  for (int k = 0; k < n; ++k) {
+    uint8_t* d = e->d_frame + bytes * k;
+    dev[k] = d;
+    if (stride == dpitch) VPB_CUDA_OK(cudaMemcpyAsync(d, frames[k], bytes, cudaMemcpyHostToDevice, e->stream));
+    else VPB_CUDA_OK(cudaMemcpy2DAsync(d, dpitch, frames[k], stride, dpitch, h, cudaMemcpyHostToDevice, e->stream));
+  }
+  rc = enqueue_frame(*e, dev.data(), h, w, dpitch);
   if (rc) return rc;
   for (auto& mo : e->outs) {
     if (mo.has_cls)
-      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, static_cast<size_t>(mo.H) * mo.W, cudaMemcpyDeviceToHost, e->stream));
+      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, static_cast<size_t>(mo.H) * mo.W * n, cudaMemcpyDeviceToHost, e->stream));
     if (e->cfg.fetch_raw || !mo.has_cls || mo.kind == VP_EGO_LANES)
-      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4, cudaMemcpyDeviceToHost, e->stream));
+      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4 * n, cudaMemcpyDeviceToHost, e->stream));
   }
   if (sync) VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   return VPB_OK;
+}
+
+extern "C" int vp_engine_infer(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride) {
+  return submit_host_frames(e, &frame_host, 1, h, w, stride, true);
+}
+
+extern "C" int vp_engine_submit(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride) {
+  return submit_host_frames(e, &frame_host, 1, h, w, stride, false);
+}
+
+extern "C" int vp_engine_infer_batch(vp_engine* e, const uint8_t* const* frames_host, int n, int h, int w, int stride) {
+  return submit_host_frames(e, frames_host, n, h, w, stride, true);
+}
+
+extern "C" int vp_engine_submit_batch(vp_engine* e, const uint8_t* const* frames_host, int n, int h, int w, int stride) {
+  return submit_host_frames(e, frames_host, n, h, w, stride, false);
 }
 
 extern "C" int vp_engine_fetch_raw(vp_engine* e, int idx) {
   if (!e || idx < 0 || idx >= static_cast<int>(e->outs.size())) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
   auto& mo = e->outs[idx];
-  VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4, cudaMemcpyDeviceToHost, e->stream));
+  const size_t nb = e->batch;
+  VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4 * nb, cudaMemcpyDeviceToHost, e->stream));
   if (mo.has_cls)
-    VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, static_cast<size_t>(mo.H) * mo.W, cudaMemcpyDeviceToHost, e->stream));
+    VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, static_cast<size_t>(mo.H) * mo.W * nb, cudaMemcpyDeviceToHost, e->stream));
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   return VPB_OK;
 }
 
-extern "C" int vp_engine_output(vp_engine* e, int idx, vp_output* o) {
+extern "C" int vp_engine_output_at(vp_engine* e, int idx, int sample, vp_output* o) {
   if (!e || !o || idx < 0 || idx >= static_cast<int>(e->outs.size())) { vpb_set_error("vp_engine_output: bad index"); return VPB_ERR_ARG; }
+  if (sample < 0 || sample >= e->batch) { vpb_set_error("vp_engine_output: sample %d of a batch of %d", sample, e->batch); return VPB_ERR_ARG; }
   const auto& mo = e->outs[idx];
+  const size_t plane = static_cast<size_t>(mo.H) * mo.W, raw = plane * mo.C * sample, cls = plane * sample;
   o->kind = mo.kind; o->channels = mo.C; o->height = mo.H; o->width = mo.W;
-  o->raw_host = mo.h_raw; o->cls_host = mo.has_cls ? mo.h_cls : nullptr;
-  o->raw_dev = mo.d_raw; o->cls_dev = mo.has_cls ? mo.d_cls : nullptr;
+  o->raw_host = mo.h_raw + raw; o->cls_host = mo.has_cls ? mo.h_cls + cls : nullptr;
+  o->raw_dev = mo.d_raw + raw; o->cls_dev = mo.has_cls ? mo.d_cls + cls : nullptr;
   return VPB_OK;
 }
+
+extern "C" int vp_engine_output(vp_engine* e, int idx, vp_output* o) { return vp_engine_output_at(e, idx, 0, o); }
 
 extern "C" int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s) {
   if (!e || !s) return VPB_ERR_ARG;
@@ -1023,7 +1079,7 @@ extern "C" int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s) {
 
 extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* flops, const char** names, int* is_gemm, int* n_ops) {
   if (!e || !ms || !n_ops) return VPB_ERR_ARG;
-  if (!e->g_src) { vpb_set_error("vp_engine_profile: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->g_src[0]) { vpb_set_error("vp_engine_profile: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   const int n = static_cast<int>(e->ops.size()) + 1;
   *n_ops = n;
@@ -1032,7 +1088,7 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
   for (auto& x : ev) VPB_CUDA_OK(cudaEventCreate(&x));
   if (e->d_gap) VPB_CUDA_OK(cudaMemsetAsync(e->d_gap, 0, e->gap_used * 8, e->stream));
   VPB_CUDA_OK(cudaEventRecord(ev[0], e->stream));
-  int rc = e->pre.launch(e->g_src, e->g_stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
+  int rc = e->pre.launch(e->g_src.data(), e->batch, e->g_stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
   if (rc) return rc;
   VPB_CUDA_OK(cudaEventRecord(ev[1], e->stream));
   for (int i = 0; i < n - 1; ++i) {
@@ -1054,7 +1110,7 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
 
 extern "C" int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flops, int* launches) {
   if (!e || !ms || reps <= 0) return VPB_ERR_ARG;
-  if (!e->g_src) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->g_src[0]) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   cudaEvent_t a, b;
   VPB_CUDA_OK(cudaEventCreate(&a));
@@ -1099,12 +1155,33 @@ template <class T> __global__ void tap_to_f32_nchw(const T* in, const T* in_lo, 
 }
 }  // namespace vpb
 
+// Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
+static bool find_tap(const vp_engine* e, const char* name, Tens* out, std::string* base) {
+  std::string nm(name);
+  int k = 0;
+  const size_t at = nm.find('@');
+  if (at != std::string::npos) {
+    const std::string ks = nm.substr(at + 1);
+    char* end = nullptr;
+    const long v = ks.empty() ? -1 : strtol(ks.c_str(), &end, 10);
+    if (v < 0 || v >= e->batch || *end) { vpb_set_error("tap '%s': sample out of range (batch %d)", name, e->batch); return false; }
+    k = static_cast<int>(v);
+    nm.resize(at);
+  }
+  auto it = e->taps.find(nm);
+  if (it == e->taps.end()) { vpb_set_error("no tap '%s'", name); return false; }
+  *out = it->second;
+  out->p = static_cast<uint8_t*>(out->p) + out->bytes() * k;    // split-fp16 engines (lo != NULL) have batch 1
+  *base = nm;
+  return true;
+}
+
 extern "C" long vp_engine_read_tap(vp_engine* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {
   if (!e || !name) return VPB_ERR_ARG;
-  auto it = e->taps.find(name);
-  if (it == e->taps.end()) { vpb_set_error("no tap '%s'", name); return VPB_ERR_ARG; }
-  const Tens& a = it->second;
-  const int Cv = (strcmp(name, "pre") == 0) ? 3 : a.C;
+  Tens a;
+  std::string base;
+  if (!find_tap(e, name, &a, &base)) return VPB_ERR_ARG;
+  const int Cv = base == "pre" ? 3 : a.C;
   const long n = static_cast<long>(a.H) * a.W * Cv;
   if (c) *c = Cv; if (h) *h = a.H; if (w) *w = a.W;
   if (!dst) return n;
@@ -1127,9 +1204,9 @@ extern "C" long vp_engine_read_tap(vp_engine* e, const char* name, float* dst, l
 
 extern "C" int vp_engine_tap_dev(vp_engine* e, const char* name, vp_tap_view* v) {
   if (!e || !name || !v) return VPB_ERR_ARG;
-  auto it = e->taps.find(name);
-  if (it == e->taps.end()) { vpb_set_error("no tap '%s'", name); return VPB_ERR_ARG; }
-  const Tens& a = it->second;
+  Tens a;
+  std::string base;
+  if (!find_tap(e, name, &a, &base)) return VPB_ERR_ARG;
   v->data = a.p; v->height = a.H; v->width = a.W; v->channels = a.C; v->ld = a.C; v->pad = a.pad;
   v->dtype = e->dtype;
   return VPB_OK;
@@ -1155,7 +1232,7 @@ extern "C" int vp_engine_kernel_names(vp_engine* e, const char** names, int cap,
 extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, float* ms, double* flops,
                                      double* bytes, int* launches) {
   if (!e || !kname || !ms || reps <= 0) return VPB_ERR_ARG;
-  if (!e->g_src) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->g_src[0]) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   const bool is_pre = strcmp(kname, "preprocess") == 0;
   cudaEvent_t a, b;
@@ -1166,10 +1243,10 @@ extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, 
   for (int r = -1; r < reps; ++r) {            // r = -1: untimed warm-up pass
     if (r == 0) VPB_CUDA_OK(cudaEventRecord(a, e->stream));
     if (is_pre) {
-      const int rc = e->pre.launch(e->g_src, e->g_stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
+      const int rc = e->pre.launch(e->g_src.data(), e->batch, e->g_stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
       if (rc) return rc;
-      // SURVEY.md 8d: frame read + 3 x 320 x 640 16-bit tensor written
-      if (r >= 0) { by += 3.0 * e->g_h * e->g_w + 2.0 * 3 * kNetH * kNetW; ++n; }
+      // SURVEY.md 8d: frame read + 3 x 320 x 640 16-bit tensor written, per sample
+      if (r >= 0) { by += e->batch * (3.0 * e->g_h * e->g_w + 2.0 * 3 * kNetH * kNetW); ++n; }
       continue;
     }
     for (auto& op : e->ops) {

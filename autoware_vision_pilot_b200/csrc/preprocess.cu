@@ -102,7 +102,7 @@ void resize_tables_host(int mode, int in_size, int out_size, std::vector<int>& b
 
 // ---------------------------------------------------------------- device
 struct PreParams {
-  const uint8_t* src;   // [h][stride] bytes, 3 interleaved channels
+  const uint8_t* src[kMaxBatch];   // per image of the batch (blockIdx.z): [h][stride] bytes, 3 interleaved channels
   int h, w, stride;
   int mode;             // VPB_RESIZE_*
   int swap_rb;          // 1: tensor channel c = source channel 2-c
@@ -115,10 +115,12 @@ struct PreParams {
   int out_pitch, out_x0, out_y0, out_c;   // output canvas: pixels per row, paste offset, channels per pixel (4 | 8)
   uint8_t* out_u8;      // optional [OH][OW][3] resized image in tensor channel order
   int OH, OW;
+  size_t out_img;       // elements between the images of out (out_lo); out_u8 images are OH * OW * 3 bytes apart
 };
 
 template <class E>
-__device__ __forceinline__ void emit_pixel(const PreParams& p, int oy, int ox, const int (&u)[3]) {
+__device__ __forceinline__ void emit_pixel(const PreParams& p, int img, int oy, int ox, const int (&u)[3]) {
+  uint8_t* out_u8 = p.out_u8 ? p.out_u8 + static_cast<size_t>(img) * p.OH * p.OW * 3 : nullptr;
   float v[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
@@ -126,13 +128,13 @@ __device__ __forceinline__ void emit_pixel(const PreParams& p, int oy, int ox, c
     float x = static_cast<float>(s);
     x = p.mul_inv255 ? x * (1.0f / 255.0f) : __fdiv_rn(x, 255.0f);
     v[c] = __fdiv_rn(x - p.mean[c], p.stdv[c]);
-    if (p.out_u8) p.out_u8[(static_cast<size_t>(oy) * p.OW + ox) * 3 + c] = static_cast<uint8_t>(s);
+    if (out_u8) out_u8[(static_cast<size_t>(oy) * p.OW + ox) * 3 + c] = static_cast<uint8_t>(s);
   }
   uint2 o, l;
   split2<E>(v[0], v[1], o.x, l.x);
   split2<E>(v[2], 0.f, o.y, l.y);
   const size_t pix = static_cast<size_t>(oy + p.out_y0) * p.out_pitch + (ox + p.out_x0);
-  reinterpret_cast<uint2*>(p.out)[pix * (p.out_c >> 2)] = o;
+  reinterpret_cast<uint2*>(static_cast<typename E::T*>(p.out) + img * p.out_img)[pix * (p.out_c >> 2)] = o;
   if (p.out_lo) reinterpret_cast<uint2*>(p.out_lo)[pix * (p.out_c >> 2)] = l;
 }
 
@@ -162,6 +164,7 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
   __shared__ int s_yb[kTYMax];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ox0 = blockIdx.x * kTX, oy0 = blockIdx.y * TY;
+  const int img = blockIdx.z;                                      // image of the batch
   const int ox1 = min(ox0 + kTX, p.OW) - 1, oy1 = min(oy0 + TY, p.OH) - 1;
   // bounds are monotone non-decreasing: first / last output coordinate give the tile's input extent
   const int x_lo = p.xb[ox0];
@@ -176,7 +179,7 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
   if (tid < TY) s_yb[tid] = (oy0 + tid <= oy1) ? p.yb[oy0 + tid] - y_lo : 0;
 
   // ---- phase 1: stage (coalesced aligned words)
-  const uintptr_t base = reinterpret_cast<uintptr_t>(p.src) + static_cast<size_t>(x_lo) * 3;
+  const uintptr_t base = reinterpret_cast<uintptr_t>(p.src[img]) + static_cast<size_t>(x_lo) * 3;
   for (int r = warp; r < rows; r += kPreThreads / 32) {
     const uintptr_t a = base + static_cast<size_t>(y_lo + r) * p.stride;
     const uint32_t* w0 = reinterpret_cast<const uint32_t*>(a & ~static_cast<uintptr_t>(3));
@@ -214,7 +217,8 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
 
   // ---- phase 3: vertical pass on 32-bit byte columns + normalise + store
   const uint32_t* interw = reinterpret_cast<const uint32_t*>(inter);
-  typename E::T* outp = reinterpret_cast<typename E::T*>(p.out);
+  typename E::T* outp = reinterpret_cast<typename E::T*>(p.out) + img * p.out_img;
+  uint8_t* out_u8 = p.out_u8 ? p.out_u8 + static_cast<size_t>(img) * p.OH * p.OW * 3 : nullptr;
   for (int i = tid; i < TY * (kRowBytes / 4); i += kPreThreads) {
     const int yo = i / (kRowBytes / 4), j = i - yo * (kRowBytes / 4);
     const int oy = oy0 + yo;
@@ -256,7 +260,7 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
         if (tc == 2) reinterpret_cast<uint32_t*>(lop)[ei >> 1] = pack2<E>(lo, 0.f);
         else lop[ei] = from_f32<E>(lo);
       }
-      if (p.out_u8) p.out_u8[(static_cast<size_t>(oy) * p.OW + ox) * 3 + tc] = static_cast<uint8_t>(u[b]);
+      if (out_u8) out_u8[(static_cast<size_t>(oy) * p.OW + ox) * 3 + tc] = static_cast<uint8_t>(u[b]);
     }
   }
 }
@@ -267,19 +271,20 @@ __global__ void __launch_bounds__(256) preprocess_direct_kernel(const PreParams 
   pdl_launch_dependents();
   pdl_wait();
   const int ox = blockIdx.x * blockDim.x + threadIdx.x;
-  const int oy = blockIdx.y;
+  const int oy = blockIdx.y, img = blockIdx.z;
   if (ox >= p.OW) return;
+  const uint8_t* src = p.src[img];
   int u[3];
   if (p.mode == VPB_RESIZE_NONE) {
-    const uint8_t* s = p.src + static_cast<size_t>(oy) * p.stride + ox * 3;
+    const uint8_t* s = src + static_cast<size_t>(oy) * p.stride + ox * 3;
     u[0] = s[0]; u[1] = s[1]; u[2] = s[2];
   } else {
     const int sx = p.xb[ox], sy = p.yb[oy];
     const int sx1 = min(sx + 1, p.w - 1), sy1 = min(sy + 1, p.h - 1);
     const int a0 = p.xk[2 * ox], a1 = p.xk[2 * ox + 1];
     const int b0 = p.yk[2 * oy], b1 = p.yk[2 * oy + 1];
-    const uint8_t* r0 = p.src + static_cast<size_t>(sy) * p.stride;
-    const uint8_t* r1 = p.src + static_cast<size_t>(sy1) * p.stride;
+    const uint8_t* r0 = src + static_cast<size_t>(sy) * p.stride;
+    const uint8_t* r1 = src + static_cast<size_t>(sy1) * p.stride;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const int h0 = r0[sx * 3 + c] * a0 + r0[sx1 * 3 + c] * a1;
@@ -287,7 +292,7 @@ __global__ void __launch_bounds__(256) preprocess_direct_kernel(const PreParams 
       u[c] = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
     }
   }
-  emit_pixel<E>(p, oy, ox, u);
+  emit_pixel<E>(p, img, oy, ox, u);
 }
 
 // ---------------------------------------------------------------- host: plan
@@ -367,12 +372,18 @@ PreprocessPlan::~PreprocessPlan() {
   if (d_tables) cudaFree(d_tables);
 }
 
-static void fill_params(const PreprocessPlan& pl, const uint8_t* src, int stride, int convention,
-                        void* out, uint8_t* out_u8, PreParams& p) {
+static int fill_params(const PreprocessPlan& pl, const uint8_t* const* srcs, int batch, int stride, int convention,
+                       void* out, uint8_t* out_u8, PreParams& p) {
+  if (batch < 1 || batch > kMaxBatch || (batch > 1 && (pl.out_lo || pl.out_pitch > 0 || pl.out_x0 || pl.out_y0))) {
+    vpb_set_error("preprocess: batch %d (1..%d, 16-bit network-sized output only)", batch, kMaxBatch);
+    return VPB_ERR_ARG;
+  }
   p.out_lo = pl.out_lo;
   p.out_pitch = pl.out_pitch > 0 ? pl.out_pitch : pl.OW; p.out_x0 = pl.out_x0; p.out_y0 = pl.out_y0;
   p.out_c = pl.out_c;
-  p.src = src; p.h = pl.h; p.w = pl.w; p.stride = stride; p.mode = pl.mode;
+  for (int i = 0; i < kMaxBatch; ++i) p.src[i] = srcs[i < batch ? i : 0];
+  p.h = pl.h; p.w = pl.w; p.stride = stride; p.mode = pl.mode;
+  p.out_img = static_cast<size_t>(pl.OH) * pl.OW * pl.out_c;
   // conventions: see include/vp_b200_ops.h
   static const float kMeanRGB[3] = {0.485f, 0.456f, 0.406f}, kStdRGB[3] = {0.229f, 0.224f, 0.225f};
   p.swap_rb = convention == VPB_CONV_BGR_SWAP ? 1 : 0;
@@ -385,6 +396,7 @@ static void fill_params(const PreprocessPlan& pl, const uint8_t* src, int stride
   p.xb = pl.d_tables + pl.off_xb; p.xk = pl.d_tables + pl.off_xk; p.xks = pl.xks;
   p.yb = pl.d_tables + pl.off_yb; p.yk = pl.d_tables + pl.off_yk; p.yks = pl.yks;
   p.out = out; p.out_u8 = out_u8; p.OH = pl.OH; p.OW = pl.OW;
+  return VPB_OK;
 }
 
 static const void* kernel_func(int mode, int dtype, int xt) {
@@ -403,11 +415,12 @@ bool PreprocessPlan::owns_kernel(const void* func, int dtype) const { return fun
 
 // Re-point the captured pre-process node at another source frame (same geometry): lets the frame
 // graph be replayed on any device buffer without re-capturing.
-int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const uint8_t* src,
-                                      int stride, int convention, int dtype, void* out,
+int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const uint8_t* const* srcs,
+                                      int batch, int stride, int convention, int dtype, void* out,
                                       uint8_t* out_u8) const {
   PreParams p;
-  fill_params(*this, src, stride, convention, out, out_u8, p);
+  const int rc = fill_params(*this, srcs, batch, stride, convention, out, out_u8, p);
+  if (rc) return rc;
   int rc_ = rows_cap, pitch_ = pitch, ty_ = TY;
   void* args[4] = {&p, &rc_, &pitch_, &ty_};
   cudaKernelNodeParams kp{};
@@ -415,11 +428,11 @@ int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node
   kp.kernelParams = args;
   kp.extra = nullptr;
   if (is_pil(mode)) {
-    kp.gridDim = dim3((OW + kTX - 1) / kTX, (OH + TY - 1) / TY);
+    kp.gridDim = dim3((OW + kTX - 1) / kTX, (OH + TY - 1) / TY, batch);
     kp.blockDim = dim3(kPreThreads);
     kp.sharedMemBytes = static_cast<unsigned>(smem_bytes);
   } else {
-    kp.gridDim = dim3((OW + 255) / 256, OH);
+    kp.gridDim = dim3((OW + 255) / 256, OH, batch);
     kp.blockDim = dim3(256);
     kp.sharedMemBytes = 0;
   }
@@ -427,12 +440,13 @@ int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node
   return VPB_OK;
 }
 
-int PreprocessPlan::launch(const uint8_t* src, int stride, int convention, int dtype, void* out,
+int PreprocessPlan::launch(const uint8_t* const* srcs, int batch, int stride, int convention, int dtype, void* out,
                            uint8_t* out_u8, cudaStream_t stream) const {
   PreParams p;
-  fill_params(*this, src, stride, convention, out, out_u8, p);
+  const int rc = fill_params(*this, srcs, batch, stride, convention, out, out_u8, p);
+  if (rc) return rc;
   if (is_pil(mode)) {
-    dim3 grid((OW + kTX - 1) / kTX, (OH + TY - 1) / TY);
+    dim3 grid((OW + kTX - 1) / kTX, (OH + TY - 1) / TY, batch);
     {
       std::lock_guard<std::mutex> g(init_mutex());
       bool* done = device_flag(kInitPreprocess);
@@ -453,7 +467,7 @@ int PreprocessPlan::launch(const uint8_t* src, int stride, int convention, int d
       else VPB_CUDA_OK(launch_k(preprocess_pil_kernel<F16, 32>, grid, blk, smem_bytes, stream, p, rows_cap, pitch, TY));
     }
   } else {
-    dim3 grid((OW + 255) / 256, OH);
+    dim3 grid((OW + 255) / 256, OH, batch);
     if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(preprocess_direct_kernel<BF16>, grid, dim3(256), 0, stream, p));
     else VPB_CUDA_OK(launch_k(preprocess_direct_kernel<F16>, grid, dim3(256), 0, stream, p));
   }
@@ -489,6 +503,6 @@ extern "C" int vpb_preprocess(const uint8_t* src_dev, int h, int w, int stride, 
   static thread_local vpb::PreprocessPlan plan;
   int rc = plan.configure(h, w, resize_mode);
   if (rc != VPB_OK) return rc;
-  return plan.launch(src_dev, stride, convention, dtype, out_dev, out_u8_dev,
+  return plan.launch(&src_dev, 1, stride, convention, dtype, out_dev, out_u8_dev,
                      static_cast<cudaStream_t>(stream));
 }

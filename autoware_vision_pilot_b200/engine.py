@@ -15,13 +15,14 @@ CONV_RGB, CONV_BGR_NOSWAP, CONV_BGR_SWAP = 0, 1, 2
 RESIZE_BY_NAME = {"none": RESIZE_NONE, "pil_bicubic": RESIZE_PIL_BICUBIC, "cv_linear": RESIZE_CV_LINEAR}
 DTYPE_BY_NAME = {"fp16": L.VPB_F16, "bf16": L.VPB_BF16, "fp32": L.VPB_F16}
 PREC_16, PREC_SPLIT = 0, 1
+MAX_BATCH = 8   # VP_MAX_BATCH
 
 
 class _Config(C.Structure):
     _fields_ = [("gpu_id", C.c_int), ("dtype", C.c_int), ("resize_mode", C.c_int), ("convention", C.c_int),
                 ("n_models", C.c_int), ("kinds", C.c_int * 4), ("weights", C.c_char_p * 4),
                 ("fetch_raw", C.c_int), ("use_graph", C.c_int), ("stream", C.c_void_p),
-                ("single_stream", C.c_int), ("precision", C.c_int)]
+                ("single_stream", C.c_int), ("precision", C.c_int), ("batch", C.c_int)]
 
 
 class _Output(C.Structure):
@@ -56,6 +57,10 @@ def _bind():
     lib.vp_engine_infer.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     lib.vp_engine_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     lib.vp_engine_infer_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    lib.vp_engine_infer_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.vp_engine_submit_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.vp_engine_infer_device_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.vp_engine_output_at.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(_Output)]
     lib.vp_engine_sync.argtypes = [C.c_void_p]
     lib.vp_engine_fetch_raw.argtypes = [C.c_void_p, C.c_int]
     lib.vp_engine_output.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Output)]
@@ -82,9 +87,11 @@ class Engine:
     def __init__(self, kinds: Sequence[int], weights: Sequence[str], *, gpu_id: int = 0, dtype: str = "fp16",
                  resize_mode: int = RESIZE_NONE, convention: int = CONV_RGB, fetch_raw: bool = True,
                  use_graph: bool = True, stream: Optional[int] = None, single_stream: bool = False,
-                 precision: Optional[int] = None):
+                 precision: Optional[int] = None, batch: int = 1):
         """dtype "fp16" | "bf16": 16-bit operands; dtype "fp32" (the reference's precision="fp32") selects the
-        split-fp16 fp32-grade mode (precision=PREC_SPLIT on fp16 pairs)."""
+        split-fp16 fp32-grade mode (precision=PREC_SPLIT on fp16 pairs).  batch > 1 (16-bit only): every call takes
+        exactly `batch` frames of one geometry (infer_batch / submit_batch / infer_device_batch); sample k's outputs
+        are raw(idx, k) / cls(idx, k)."""
         self._lib = _bind()
         cfg = _Config()
         cfg.gpu_id, cfg.dtype = gpu_id, DTYPE_BY_NAME[dtype]
@@ -97,9 +104,11 @@ class Engine:
         cfg.stream = stream
         cfg.single_stream = int(single_stream)
         cfg.precision = (PREC_SPLIT if dtype == "fp32" else PREC_16) if precision is None else precision
+        cfg.batch = batch
         self._h = C.c_void_p()
         L.check(self._lib.vp_engine_create(C.byref(cfg), C.byref(self._h)), "vp_engine_create")
         self.kinds = list(kinds)
+        self.batch = max(1, batch)
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -136,37 +145,78 @@ class Engine:
     def infer_device(self, dev_ptr: int, h: int, w: int, stride: int) -> None:
         L.check(self._lib.vp_engine_infer_device(self._h, dev_ptr, h, w, stride), "vp_engine_infer_device")
 
+    def _check_batch(self, frames: Sequence[np.ndarray], allow_copy: bool) -> List[np.ndarray]:
+        """`batch` frames of one shape and one row stride (checked here, before the C call)."""
+        frames = list(frames)
+        if len(frames) != self.batch:
+            raise ValueError(f"{len(frames)} frame(s) for an engine of batch {self.batch}")
+        frames = [self._check_frame(f, allow_copy) for f in frames]
+        if len({f.shape for f in frames}) != 1:
+            raise ValueError(f"frames of one call must share one shape, got {sorted({f.shape for f in frames})}")
+        if len({f.strides[0] for f in frames}) != 1:
+            if not allow_copy:
+                raise ValueError("submit_batch() needs frames with one row stride")
+            frames = [np.ascontiguousarray(f) for f in frames]
+        return frames
+
+    @staticmethod
+    def _ptrs(ptrs: Sequence[int]):
+        return (C.c_void_p * len(ptrs))(*ptrs)
+
+    def infer_batch(self, frames: Sequence[np.ndarray]) -> None:
+        """`batch` uint8 [h, w, 3] host frames of one shape in one call; outputs of frame k are sample k."""
+        frames = self._check_batch(frames, allow_copy=True)
+        h, w, _ = frames[0].shape
+        L.check(self._lib.vp_engine_infer_batch(self._h, self._ptrs([f.ctypes.data for f in frames]), len(frames), h, w,
+                                                frames[0].strides[0]), "vp_engine_infer_batch")
+
+    def submit_batch(self, frames: Sequence[np.ndarray]) -> None:
+        """Asynchronous infer_batch() (pinned frames: slices of pinned_frame(h, w, n)); sync() completes it."""
+        frames = self._check_batch(frames, allow_copy=False)
+        h, w, _ = frames[0].shape
+        L.check(self._lib.vp_engine_submit_batch(self._h, self._ptrs([f.ctypes.data for f in frames]), len(frames), h, w,
+                                                 frames[0].strides[0]), "vp_engine_submit_batch")
+
+    def infer_device_batch(self, dev_ptrs: Sequence[int], h: int, w: int, stride: int) -> None:
+        """`batch` device frames (uint8, h x w x 3, `stride` bytes per row) in one asynchronous call."""
+        if len(dev_ptrs) != self.batch:
+            raise ValueError(f"{len(dev_ptrs)} frame(s) for an engine of batch {self.batch}")
+        L.check(self._lib.vp_engine_infer_device_batch(self._h, self._ptrs(dev_ptrs), len(dev_ptrs), h, w, stride),
+                "vp_engine_infer_device_batch")
+
     def sync(self) -> None:
         L.check(self._lib.vp_engine_sync(self._h), "vp_engine_sync")
 
     def fetch_raw(self, idx: int) -> None:
         L.check(self._lib.vp_engine_fetch_raw(self._h, idx), "vp_engine_fetch_raw")
 
-    def pinned_frame(self, h: int, w: int) -> np.ndarray:
-        n = h * w * 3
-        p = self._lib.vp_engine_pinned_frame(self._h, n)
+    def pinned_frame(self, h: int, w: int, n: Optional[int] = None) -> np.ndarray:
+        """Engine-owned pinned host buffer: [h, w, 3], or [n, h, w, 3] for n frames (submit_batch(list(buf)))."""
+        size = h * w * 3 * (1 if n is None else n)
+        p = self._lib.vp_engine_pinned_frame(self._h, size)
         if not p:
             raise RuntimeError(L.last_error())
-        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(n,)).reshape(h, w, 3)
+        a = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(size,))
+        return a.reshape(h, w, 3) if n is None else a.reshape(n, h, w, 3)
 
     # ---- outputs (views into engine-owned host buffers: copy if kept past the next infer)
-    def _out(self, idx: int) -> _Output:
+    def _out(self, idx: int, sample: int = 0) -> _Output:
         o = _Output()
-        L.check(self._lib.vp_engine_output(self._h, idx, C.byref(o)), "vp_engine_output")
+        L.check(self._lib.vp_engine_output_at(self._h, idx, sample, C.byref(o)), "vp_engine_output_at")
         return o
 
-    def raw(self, idx: int) -> np.ndarray:
-        o = self._out(idx)
+    def raw(self, idx: int, sample: int = 0) -> np.ndarray:
+        o = self._out(idx, sample)
         return np.ctypeslib.as_array(o.raw_host, shape=(o.channels, o.height, o.width))
 
-    def cls(self, idx: int) -> Optional[np.ndarray]:
-        o = self._out(idx)
+    def cls(self, idx: int, sample: int = 0) -> Optional[np.ndarray]:
+        o = self._out(idx, sample)
         if not o.cls_host:
             return None
         return np.ctypeslib.as_array(o.cls_host, shape=(o.height, o.width))
 
-    def out_dev(self, idx: int):
-        o = self._out(idx)
+    def out_dev(self, idx: int, sample: int = 0):
+        o = self._out(idx, sample)
         return o.raw_dev, o.cls_dev, (o.channels, o.height, o.width)
 
     # ---- introspection

@@ -26,7 +26,12 @@
  * turn them back into std::runtime_error / `false` exactly where the reference throws / returns).
  *
  * There is no CPU fallback: every entry point that computes requires a CUDA device of compute
- * capability 10.x and fails with VPB_ERR_CUDA otherwise.
+ * capability 9.0 (H100, the library is built for sm_90a) and fails with VPB_ERR_CUDA otherwise.
+ *
+ * Batched engines (vp_engine_config.batch = N > 1) evaluate N frames of one geometry per call through
+ * the same launch list: one weight copy, one graph replay, activations and outputs for N samples.
+ * They take the *_batch entry points only; sample k of the outputs is vp_engine_output_at(.., k, ..)
+ * and tap "<name>@k".  Sample k's outputs are bit-identical to a batch-1 engine's on frame k.
  */
 #ifndef VP_B200_H_
 #define VP_B200_H_
@@ -39,6 +44,7 @@ extern "C" {
 #endif
 
 #define VP_MAX_MODELS 4
+#define VP_MAX_BATCH 8
 
 /* network kinds (the four Models/model_components network modules, e.g. scene_seg_network.py) */
 enum { VP_SCENE_SEG = 0, VP_SCENE_3D = 1, VP_DOMAIN_SEG = 2, VP_EGO_LANES = 3 };
@@ -64,6 +70,9 @@ typedef struct {
                                        run_model_node.cpp:29-36): every tensor is a (hi, lo) fp16 pair (~22 bits), the
                                        wgmma GEMMs accumulate A_hi W_hi + A_lo W_hi + A_hi W_lo in fp32 — about
                                        3x the tensor work, results within ~1e-5 sigma of the fp32 CPU path */
+  int batch;                        /* frames per call: 0 or 1 = one frame (vp_engine_infer ...); 2..VP_MAX_BATCH =
+                                       the *_batch entry points with exactly `batch` frames (16-bit mode only:
+                                       VP_PREC_SPLIT with batch > 1 fails with VPB_ERR_ARG) */
 } vp_engine_config;
 
 typedef struct {
@@ -93,17 +102,30 @@ int vp_engine_submit(vp_engine* e, const uint8_t* frame_host, int h, int w, int 
  * stay on the device (vp_output.raw_dev / cls_dev); call vp_engine_sync before reading them. */
 int vp_engine_infer_device(vp_engine* e, const uint8_t* frame_dev, int h, int w, int stride);
 int vp_engine_sync(vp_engine* e);
+
+/* Batched forms of the three calls above, for an engine created with batch = n > 1 (the single-frame calls
+ * return VPB_ERR_ARG on such an engine, and these on a batch-1 engine unless n == 1).  frames[k] is frame k;
+ * all n frames share h, w and stride, and each row copy reads exactly w*3 bytes.  vp_engine_submit_batch
+ * reads its frames asynchronously: give it pinned memory (vp_engine_pinned_frame(e, n * bytes) sliced into
+ * n frames). */
+int vp_engine_infer_batch(vp_engine* e, const uint8_t* const* frames_host, int n, int h, int w, int stride);
+int vp_engine_submit_batch(vp_engine* e, const uint8_t* const* frames_host, int n, int h, int w, int stride);
+int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev, int n, int h, int w, int stride);
 /* Copy the raw fp32 tensor of one model to its host buffer (after a device/async inference). */
 int vp_engine_fetch_raw(vp_engine* e, int model_idx);
 
 int vp_engine_output(vp_engine* e, int model_idx, vp_output* out);
+/* Sample `sample` (0 .. batch-1) of a batched engine's outputs: per model the buffers are [batch][C][H][W] fp32
+ * and [batch][H][W] uint8, and the pointers returned address sample `sample`.  vp_engine_output is sample 0. */
+int vp_engine_output_at(vp_engine* e, int model_idx, int sample, vp_output* out);
 int vp_engine_num_models(const vp_engine* e);
 
 /* A pinned host buffer owned by the engine that a caller may fill directly (capture threads):
  * vp_engine_infer recognises the pointer and skips the staging copy. */
 uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes);
 
-/* Introspection for the benchmark / roofline report. */
+/* Introspection for the benchmark / roofline report.  Per call: on a batched engine the FLOP counts cover all
+ * `batch` frames, while launches and weight bytes are those of one call (they do not grow with the batch). */
 typedef struct {
   int n_launches;        /* kernels launched per frame                                           */
   int n_gemm_launches;   /* of which wgmma implicit-GEMM convolutions                          */
@@ -141,7 +163,8 @@ int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, float* ms, 
                           int* launches);
 
 /* Intermediate activations for the per-tap parity tests: copies tensor `name`
- * ("<model_idx>/f0".."f4", "context", "neck", "pre") to host as fp32 NCHW. Returns element count. */
+ * ("<model_idx>/f0".."f4", "context", "neck", "pre") to host as fp32 NCHW. Returns element count.
+ * A suffix "@k" selects sample k of a batched engine ("0/neck@3"); without it, sample 0. */
 long vp_engine_read_tap(vp_engine* e, const char* name, float* dst, long cap, int* c, int* h, int* w);
 
 /* Device view of an intermediate tensor (same names as vp_engine_read_tap): lets a host chain further

@@ -124,6 +124,11 @@ typedef struct {
    *         ConvTranspose bias only passes through the 3x3 taps that lie inside the image)
    * vpb_upconv_compose builds w / w2 / bias from the three layers' parameters.  mode STORE, act NONE | GELU. */
   int taps2;
+  /* Images per call (0 = 1).  in / out / res / in2 (and the split-mode low halves) hold `batch` images back to back,
+   * each with the layout the fields above describe (zero-bordered or not); FINAL outputs are out_f32
+   * [batch][Cout][H][W] and out_cls [batch][H][W].  Every image sees the same weights, and its outputs are
+   * bit-identical to a call on that image alone. */
+  int batch;
 } vpb_conv_args;
 int vpb_conv_gemm(const vpb_conv_args* a, void* stream);
 /* Composition of the upconv operands on the device (all pointers device fp32, outputs may be NULL to skip):

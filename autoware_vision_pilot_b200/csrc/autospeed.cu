@@ -24,9 +24,7 @@
 #include "../../include/vp_b200_autospeed.h"
 
 #include <cmath>
-#include <cstring>
 #include <functional>
-#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -307,101 +305,35 @@ __global__ void fill_canvas_kernel(typename E::T* __restrict__ x, int npix) {
   for (int c = 0; c < 8; ++c) x[static_cast<size_t>(i) * 8 + c] = c < 3 ? g : z;
 }
 
-template <class T> __global__ void tap_slice_to_f32(const T* in, int H, int W, int C, int ld, float* out) {
-  const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<long>(H) * W * C) return;
-  const int c = static_cast<int>(i / (static_cast<long>(H) * W));
-  const long pix = i - static_cast<long>(c) * H * W;
-  out[i] = static_cast<float>(in[pix * ld + c]);
-}
-
 }  // namespace vpb
 
 using namespace vpb;
 
 // ====================================================================== engine
-struct ASTens {   // NHWC 16-bit view: base pointer (already offset to the slice's first channel), row stride ld
-  void* p = nullptr; int H = 0, W = 0, C = 0, ld = 0;
-  ASTens slice(int c0, int c) const { ASTens t = *this; t.p = static_cast<uint8_t*>(p) + static_cast<size_t>(c0) * 2; t.C = c; return t; }
-};
-
-struct vp_autospeed {
-  int gpu_id = 0, dtype = VPB_F16;
-  cudaStream_t stream = nullptr; bool own_stream = false;
-  std::vector<void*> dev_allocs, host_allocs;
-  bool oom = false;
-  std::vector<std::unique_ptr<ConvPlan>> plans;
-  std::vector<std::function<int(cudaStream_t)>> ops;
-  std::vector<std::string> op_names;
-  std::map<std::string, ASTens> taps;
-  double flops = 0;
+struct vp_autospeed : EngineRuntime {
   PreprocessPlan pre;
-  uint8_t* d_frame = nullptr; size_t d_frame_cap = 0;
   void* d_canvas = nullptr;
   float* d_raw = nullptr; float* h_raw = nullptr;
   float* d_cand = nullptr; int* d_order = nullptr; float* d_det = nullptr; int* d_counts = nullptr;
   float* h_det = nullptr; int* h_counts = nullptr;
   long long* d_gap_scratch = nullptr;
-  float* d_tap_scratch = nullptr; size_t tap_cap = 0;
   int src_w = 0, src_h = 0; float scale = 1.f; int pad_x = 0, pad_y = 0, new_w = 0, new_h = 0;
   float conf = 0.6f, iou = 0.45f;
   static constexpr int kMaxCand = 4096, kMaxDet = 1024;
-  cudaGraphExec_t gexec = nullptr; cudaGraph_t graph = nullptr;
-  const uint8_t* g_src = nullptr; int g_stride = 0;
-  cudaGraphNode_t g_pre_node = nullptr;      // the captured letterbox kernel node (re-pointed per frame)
 
-  ~vp_autospeed() {
-    DeviceGuard g(gpu_id);
-    if (gexec) cudaGraphExecDestroy(gexec);
-    if (graph) cudaGraphDestroy(graph);
-    if (d_tap_scratch) cudaFree(d_tap_scratch);
-    for (void* p : dev_allocs) cudaFree(p);
-    for (void* p : host_allocs) cudaFreeHost(p);
-    if (own_stream && stream) cudaStreamDestroy(stream);
-  }
-  void* dalloc(size_t bytes) {
-    void* p = nullptr;
-    const cudaError_t ce = cudaMalloc(&p, std::max<size_t>(bytes, 256));
-    if (ce != cudaSuccess || !p) {
-      if (!oom) vpb_set_error("cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(ce));
-      oom = true; cudaGetLastError();
-      return nullptr;
-    }
-    cudaMemset(p, 0, std::max<size_t>(bytes, 256));
-    dev_allocs.push_back(p);
-    return p;
-  }
-  void* halloc(size_t bytes) {
-    void* p = nullptr;
-    if (cudaMallocHost(&p, std::max<size_t>(bytes, 64)) != cudaSuccess) { oom = true; vpb_set_error("cudaMallocHost failed"); return nullptr; }
-    host_allocs.push_back(p);
-    return p;
-  }
-  ASTens talloc(int H, int W, int C) {
-    ASTens t; t.H = H; t.W = W; t.C = C; t.ld = C;
+  Tens talloc(int H, int W, int C) {
+    Tens t; t.H = H; t.W = W; t.C = C; t.ld = C;
     t.p = dalloc(static_cast<size_t>(H) * W * C * 2);
     return t;
   }
-  float* up_f32(const std::vector<float>& v) {
-    float* p = static_cast<float*>(dalloc(v.size() * 4));
-    if (p) cudaMemcpy(p, v.data(), v.size() * 4, cudaMemcpyHostToDevice);
-    return p;
+  void op(const std::string& name, std::function<int(cudaStream_t)> fn, double flops = 0) {
+    OpRec r; r.name = name; r.launch = std::move(fn); r.flops = flops;
+    ops.push_back(std::move(r));
   }
-  void* up_16(const std::vector<float>& v) {
-    std::vector<uint16_t> h(v.size());
-    for (size_t i = 0; i < v.size(); ++i) {
-      if (dtype == VPB_BF16) { __nv_bfloat16 b = __float2bfloat16_rn(v[i]); memcpy(&h[i], &b, 2); }
-      else { __half b = __float2half_rn(v[i]); memcpy(&h[i], &b, 2); }
-    }
-    void* p = dalloc(h.size() * 2);
-    if (p) cudaMemcpy(p, h.data(), h.size() * 2, cudaMemcpyHostToDevice);
-    return p;
-  }
-  void op(const std::string& name, std::function<int(cudaStream_t)> fn) { ops.push_back(std::move(fn)); op_names.push_back(name); }
 
   // one wgmma convolution: in (slice) -> out (slice); w [taps][Cout][Cin] 16-bit (or an activation slice with ldw)
-  int conv(const std::string& name, const ASTens& in, const ASTens& out, int Cout, int taps, int stride, const void* w,
-           const float* bias, int act, int mode = VPB_EPI_STORE, const ASTens* res = nullptr, int act2 = ACT_NONE,
+  int conv(const std::string& name, const Tens& in, const Tens& out, int Cout, int taps, int stride, const void* w,
+           const float* bias, int act, int mode = VPB_EPI_STORE, const Tens* res = nullptr, int act2 = ACT_NONE,
            int ldw = 0, int cin = 0) {
     vpb_conv_args a{};
     a.dtype = dtype; a.H = out.H; a.W = out.W; a.Cin = cin > 0 ? cin : in.C; a.ldi = in.ld;
@@ -412,14 +344,7 @@ struct vp_autospeed {
     a.algo = VPB_ALGO_TILE;
     a.stride = stride; a.in_h = in.H; a.in_w = in.W;
     a.act2 = act2; a.ldw = ldw;
-    auto plan = std::make_unique<ConvPlan>();
-    int rc = conv_plan_build(&a, plan.get());
-    if (rc != VPB_OK) { std::string e = vpb_last_error(); vpb_set_error("%s: %s", name.c_str(), e.c_str()); return rc; }
-    ConvPlan* pp = plan.get();
-    plans.push_back(std::move(plan));
-    flops += pp->flops;
-    op(name, [pp](cudaStream_t s) { return conv_plan_launch(pp, s); });
-    return VPB_OK;
+    return append_conv(name, a);
   }
 };
 
@@ -458,36 +383,36 @@ struct ASBuilder {
         for (int ci = 0; ci < cin; ++ci) o[(static_cast<size_t>(t) * cout + co) * cin_pad + ci] = wt[(static_cast<size_t>(t) * cout + co) * cin + ci];
     return o;
   }
-  void cbs(const std::string& p, const ASTens& in, const ASTens& out, int cout, int k, int stride, bool act, int cin_pad = 0,
-           int mode = VPB_EPI_STORE, const ASTens* res = nullptr) {
+  void cbs(const std::string& p, const Tens& in, const Tens& out, int cout, int k, int stride, bool act, int cin_pad = 0,
+           int mode = VPB_EPI_STORE, const Tens* res = nullptr) {
     if (!ok()) return;
     const int cin = cin_pad ? 3 : in.C;
     std::vector<float> wt, bias;
     if (!fold(p, cout, cin, k, wt, bias, false)) return;
     if (cin_pad) wt = pad_cin(wt, k * k, cout, cin, cin_pad);
-    rc = e.conv(p, in, out, cout, k * k, stride, e.up_16(wt), e.up_f32(bias), act ? ACT_SILU : ACT_NONE, mode, res);
+    rc = e.conv(p, in, out, cout, k * k, stride, e.upload_16(wt), e.upload_f32(bias), act ? ACT_SILU : ACT_NONE, mode, res);
   }
   // plain nn.Conv2d with bias (CTX convs, head output convs)
-  void plain(const std::string& p, const ASTens& in, const ASTens& out, int cout, int k, int act, int mode = VPB_EPI_STORE,
-             const ASTens* res = nullptr, int act2 = ACT_NONE) {
+  void plain(const std::string& p, const Tens& in, const Tens& out, int cout, int k, int act, int mode = VPB_EPI_STORE,
+             const Tens* res = nullptr, int act2 = ACT_NONE) {
     if (!ok()) return;
     const HostTensor* cw = find_w_shaped(w, p + ".weight", {cout, in.C, k, k});
     const HostTensor* cb = find_w_shaped(w, p + ".bias", {cout});
     if (!cw || !cb) { rc = VPB_ERR_IO; return; }
-    rc = e.conv(p, in, out, cout, k * k, 1, e.up_16(pack_conv(*cw, nullptr)), e.up_f32(cb->f), act, mode, res, act2);
+    rc = e.conv(p, in, out, cout, k * k, 1, e.upload_16(pack_conv(*cw, nullptr)), e.upload_f32(cb->f), act, mode, res, act2);
   }
-  void dw(const std::string& p, const ASTens& in, const ASTens& out, bool act) {
+  void dw(const std::string& p, const Tens& in, const Tens& out, bool act) {
     if (!ok()) return;
     std::vector<float> wt, bias;
     if (!fold(p, in.C, 1, 3, wt, bias, true)) return;
-    float *dwt = e.up_f32(wt), *db = e.up_f32(bias);
+    float *dwt = e.upload_f32(wt), *db = e.upload_f32(bias);
     const int dt = e.dtype, H = in.H, W = in.W, C = in.C;
     const void* ip = in.p; void* op_ = out.p; long long* gap = e.d_gap_scratch;
-    e.flops += 2.0 * H * W * C * 9;
-    e.op(p, [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? 1 : 0); });
+    e.op(p, [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? 1 : 0); },
+         2.0 * H * W * C * 9);
   }
   // CTX (common_layers.py:194-239): x [h][w][C] -> out [h][w][Cout]
-  void ctx(const std::string& p, const ASTens& x, const ASTens& out, int cout) {
+  void ctx(const std::string& p, const Tens& x, const Tens& out, int cout) {
     if (!ok()) return;
     const int C = x.C, H = x.H, W = x.W, HW = H * W, dt = e.dtype;
     const HostTensor *ew = find_w_shaped(w, p + ".exp0.weight", {HW, C, 3}), *eb = find_w_shaped(w, p + ".exp0.bias", {HW});
@@ -510,41 +435,41 @@ struct ASBuilder {
     std::vector<float> lw(static_cast<size_t>(HW) * C);
     for (int o = 0; o < HW; ++o)
       for (int c = 0; c < C; ++c) lw[static_cast<size_t>(o) * C + c] = ew->f[(static_cast<size_t>(o) * C + c) * 3 + 1];
-    float *d_lw = e.up_f32(lw), *d_lb = e.up_f32(eb->f);
+    float *d_lw = e.upload_f32(lw), *d_lb = e.upload_f32(eb->f);
     float* d_map = static_cast<float*>(e.dalloc(static_cast<size_t>(HW) * 4));
-    e.flops += 2.0 * HW * C;
-    e.op(p + ".exp0", [=](cudaStream_t st) { return vpb_linear(d_mean, d_lw, d_lb, C, HW, VPB_ACT_SILU2, d_map, st); });
+    e.op(p + ".exp0", [=](cudaStream_t st) { return vpb_linear(d_mean, d_lw, d_lb, C, HW, VPB_ACT_SILU2, d_map, st); },
+         2.0 * HW * C);
     // ctx0: Conv2d(1 -> C/2, 3x3) + SiLU
-    ASTens c2 = e.talloc(H, W, C / 2);
-    float *d_c0w = e.up_f32(c0w->f), *d_c0b = e.up_f32(c0b->f);
+    Tens c2 = e.talloc(H, W, C / 2);
+    float *d_c0w = e.upload_f32(c0w->f), *d_c0b = e.upload_f32(c0b->f);
     {
       void* op_ = c2.p; const int co = C / 2;
-      e.flops += 2.0 * HW * co * 9;
-      e.op(p + ".ctx0", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, nullptr, 0, st, ACT_SILU); });
+      e.op(p + ".ctx0", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, nullptr, 0, st, ACT_SILU); },
+           2.0 * HW * co * 9);
     }
     // ctx1: SiLU(conv) * x + x, then SiLU (:224-232) — one wgmma conv with the MULADD epilogue and a post activation
-    ASTens c4 = e.talloc(H, W, C);
+    Tens c4 = e.talloc(H, W, C);
     plain(p + ".ctx1", c2, c4, C, 3, ACT_SILU, VPB_EPI_MULADD, &x, ACT_SILU);
     plain(p + ".ctx2", c4, out, cout, 3, ACT_NONE);
   }
-  void residual(const std::string& p, const ASTens& x, const ASTens& out, int mid) {   // out = x + conv2(conv1(x)); out may alias x
-    ASTens t = e.talloc(x.H, x.W, mid);
+  void residual(const std::string& p, const Tens& x, const Tens& out, int mid) {   // out = x + conv2(conv1(x)); out may alias x
+    Tens t = e.talloc(x.H, x.W, mid);
     cbs(p + ".conv1", x, t, mid, 3, 1, true);
     cbs(p + ".conv2", t, out, x.C, 3, 1, true, 0, VPB_EPI_ADD, &x);
   }
   // C3K2 (n = 1): cat buffer [3c]: conv1 -> [0, 2c), residual / C3K on [c, 2c) -> [2c, 3c), conv2 over all 3c
-  void c3k2(const std::string& p, const ASTens& in, const ASTens& out, int cout, bool csp) {
+  void c3k2(const std::string& p, const Tens& in, const Tens& out, int cout, bool csp) {
     if (!ok()) return;
     const int c = cout / 2;
-    ASTens cat = e.talloc(in.H, in.W, 3 * c);
+    Tens cat = e.talloc(in.H, in.W, 3 * c);
     cbs(p + ".conv1", in, cat.slice(0, 2 * c), 2 * c, 1, 1, true);
-    ASTens y1 = cat.slice(c, c), y2 = cat.slice(2 * c, c);
+    Tens y1 = cat.slice(c, c), y2 = cat.slice(2 * c, c);
     if (!csp) {
       residual(p + ".res_m.0", y1, y2, c / 2);
     } else {                                                   // C3K (common_layers.py:158-173)
       const std::string q = p + ".res_m.0";
-      ASTens k = e.talloc(in.H, in.W, c);                      // cat(res_m(conv1(y1)), conv2(y1))
-      ASTens k1 = k.slice(0, c / 2);
+      Tens k = e.talloc(in.H, in.W, c);                      // cat(res_m(conv1(y1)), conv2(y1))
+      Tens k1 = k.slice(0, c / 2);
       cbs(q + ".conv1", y1, k1, c / 2, 1, 1, true);
       cbs(q + ".conv2", y1, k.slice(c / 2, c / 2), c / 2, 1, 1, true);
       residual(q + ".res_m.0", k1, k1, c / 2);
@@ -553,7 +478,7 @@ struct ASBuilder {
     }
     cbs(p + ".conv2", cat, out, cout, 1, 1, true);
   }
-  void upsample(const std::string& name, const ASTens& in, const ASTens& out) {
+  void upsample(const std::string& name, const Tens& in, const Tens& out) {
     const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, li = in.ld / 8, lo = out.ld / 8;
     const void* ip = in.p; void* op_ = out.p;
     const long n = 4L * H * W * C8;
@@ -564,7 +489,7 @@ struct ASBuilder {
       return VPB_OK;
     });
   }
-  void maxpool(const std::string& name, const ASTens& in, const ASTens& out) {
+  void maxpool(const std::string& name, const Tens& in, const Tens& out) {
     const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, ld8 = in.ld / 8;
     const void* ip = in.p; void* op_ = out.p;
     e.op(name, [=](cudaStream_t st) {
@@ -575,12 +500,12 @@ struct ASBuilder {
     });
   }
   // PSABlock on y (in place): y += attention(y); y += ffn(y)   (common_layers.py:77-118)
-  void psablock(const std::string& p, const ASTens& y, int nh) {
+  void psablock(const std::string& p, const Tens& y, int nh) {
     if (!ok()) return;
     const int C = y.C, T = y.H * y.W, dh = C / nh, dk = dh / 2, per = 2 * dk + dh, dt = e.dtype;
-    ASTens qkv = e.talloc(y.H, y.W, nh * per);
+    Tens qkv = e.talloc(y.H, y.W, nh * per);
     cbs(p + ".conv1.qkv", y, qkv, nh * per, 1, 1, false);
-    ASTens vc = e.talloc(y.H, y.W, C);
+    Tens vc = e.talloc(y.H, y.W, C);
     void* vt = e.dalloc(static_cast<size_t>(nh) * dh * T * 2);
     {
       const void* q = qkv.p; void* vcp = vc.p;
@@ -591,15 +516,15 @@ struct ASBuilder {
         return VPB_OK;
       });
     }
-    ASTens dwv = e.talloc(y.H, y.W, C);
+    Tens dwv = e.talloc(y.H, y.W, C);
     dw(p + ".conv1.conv1", vc, dwv, false);                     // positional term: depthwise 3x3 on v, no activation
-    ASTens att = e.talloc(y.H, y.W, C);
+    Tens att = e.talloc(y.H, y.W, C);
     const float scale = 1.0f / std::sqrt(static_cast<float>(dk));
     for (int h = 0; h < nh && ok(); ++h) {
       // S = Q K^T: pixels = query tokens, Cin = dk (q channels of head h), "weights" = the k channels of every token
-      ASTens s = e.talloc(1, T, T), pm = e.talloc(1, T, T);
-      ASTens q = qkv.slice(h * per, dk);
-      ASTens qv = q; qv.H = 1; qv.W = T;
+      Tens s = e.talloc(1, T, T), pm = e.talloc(1, T, T);
+      Tens q = qkv.slice(h * per, dk);
+      Tens qv = q; qv.H = 1; qv.W = T;
       const void* kmat = static_cast<const uint8_t*>(qkv.p) + static_cast<size_t>(h * per + dk) * 2;
       rc = e.conv(p + ".attn.qk" + std::to_string(h), qv, s, T, 1, 1, kmat, nullptr, ACT_NONE, VPB_EPI_STORE, nullptr, ACT_NONE,
                   /*ldw=*/qkv.ld);
@@ -614,13 +539,13 @@ struct ASBuilder {
         });
       }
       // O = P V^T (+ depthwise term): Cin = key tokens, "weights" = Vt[h] [dh][T]
-      ASTens o = att.slice(h * dh, dh); o.H = 1; o.W = T;
-      ASTens r = dwv.slice(h * dh, dh); r.H = 1; r.W = T;
+      Tens o = att.slice(h * dh, dh); o.H = 1; o.W = T;
+      Tens r = dwv.slice(h * dh, dh); r.H = 1; r.W = T;
       rc = e.conv(p + ".attn.pv" + std::to_string(h), pm, o, dh, 1, 1, static_cast<const uint8_t*>(vt) + static_cast<size_t>(h) * dh * T * 2,
                   nullptr, ACT_NONE, VPB_EPI_ADD, &r, ACT_NONE, /*ldw=*/T);
     }
     cbs(p + ".conv1.conv2", att, y, C, 1, 1, false, 0, VPB_EPI_ADD, &y);          // y = y + proj(attention)
-    ASTens f = e.talloc(y.H, y.W, 2 * C);
+    Tens f = e.talloc(y.H, y.W, 2 * C);
     cbs(p + ".conv2.0", y, f, 2 * C, 1, 1, true);
     cbs(p + ".conv2.1", f, y, C, 1, 1, false, 0, VPB_EPI_ADD, &y);                // y = y + ffn(y)
   }
@@ -630,69 +555,69 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   ASBuilder b{e, w};
   const int W0 = kASW, H0 = kASH;
   e.d_gap_scratch = static_cast<long long*>(e.dalloc(static_cast<size_t>(kGapReplicas) * 256 * 8 + 64));
-  ASTens x0; x0.p = e.d_canvas; x0.H = H0; x0.W = W0; x0.C = 8; x0.ld = 8;
+  Tens x0; x0.p = e.d_canvas; x0.H = H0; x0.W = W0; x0.C = 8; x0.ld = 8;
   // ---- backbone (auto_speed_backbone.py:9-48)
-  ASTens p1 = e.talloc(H0 / 2, W0 / 2, 16);
+  Tens p1 = e.talloc(H0 / 2, W0 / 2, 16);
   b.cbs("net.p1", x0, p1, 16, 3, 2, true, /*cin_pad=*/8);
-  ASTens a2 = e.talloc(H0 / 4, W0 / 4, 32);
+  Tens a2 = e.talloc(H0 / 4, W0 / 4, 32);
   b.cbs("net.p2.0", p1, a2, 32, 3, 2, true);
-  ASTens p2 = e.talloc(H0 / 4, W0 / 4, 64);
+  Tens p2 = e.talloc(H0 / 4, W0 / 4, 64);
   b.ctx("net.p2.1", a2, p2, 64);
-  ASTens a3 = e.talloc(H0 / 8, W0 / 8, 64);
+  Tens a3 = e.talloc(H0 / 8, W0 / 8, 64);
   b.cbs("net.p3.0", p2, a3, 64, 3, 2, true);
-  ASTens h2cat = e.talloc(H0 / 8, W0 / 8, 256);                // cat(up(p4'), p3)
-  ASTens p3 = h2cat.slice(128, 128);
+  Tens h2cat = e.talloc(H0 / 8, W0 / 8, 256);                // cat(up(p4'), p3)
+  Tens p3 = h2cat.slice(128, 128);
   b.ctx("net.p3.1", a3, p3, 128);
-  ASTens a4 = e.talloc(H0 / 16, W0 / 16, 128);
+  Tens a4 = e.talloc(H0 / 16, W0 / 16, 128);
   b.cbs("net.p4.0", p3, a4, 128, 3, 2, true);
-  ASTens h1cat = e.talloc(H0 / 16, W0 / 16, 384);              // cat(up(p5), p4)
-  ASTens p4 = h1cat.slice(256, 128);
+  Tens h1cat = e.talloc(H0 / 16, W0 / 16, 384);              // cat(up(p5), p4)
+  Tens p4 = h1cat.slice(256, 128);
   b.ctx("net.p4.1", a4, p4, 128);
-  ASTens a5 = e.talloc(H0 / 32, W0 / 32, 256);
+  Tens a5 = e.talloc(H0 / 32, W0 / 32, 256);
   b.cbs("net.p5.0", p4, a5, 256, 3, 2, true);
-  ASTens q5 = e.talloc(H0 / 32, W0 / 32, 256);
+  Tens q5 = e.talloc(H0 / 32, W0 / 32, 256);
   b.ctx("net.p5.1", a5, q5, 256);
-  ASTens sp = e.talloc(H0 / 32, W0 / 32, 512);                 // SPPF cat (common_layers.py:242-254)
+  Tens sp = e.talloc(H0 / 32, W0 / 32, 512);                 // SPPF cat (common_layers.py:242-254)
   b.cbs("net.p5.2.cv1", q5, sp.slice(0, 128), 128, 1, 1, true);
   if (b.ok()) {
     b.maxpool("net.p5.2.pool1", sp.slice(0, 128), sp.slice(128, 128));
     b.maxpool("net.p5.2.pool2", sp.slice(128, 128), sp.slice(256, 128));
     b.maxpool("net.p5.2.pool3", sp.slice(256, 128), sp.slice(384, 128));
   }
-  ASTens s5 = e.talloc(H0 / 32, W0 / 32, 256);
+  Tens s5 = e.talloc(H0 / 32, W0 / 32, 256);
   b.cbs("net.p5.2.cv2", sp, s5, 256, 1, 1, true);
-  ASTens cp = e.talloc(H0 / 32, W0 / 32, 256);                 // C2PSA cat (common_layers.py:257-269)
+  Tens cp = e.talloc(H0 / 32, W0 / 32, 256);                 // C2PSA cat (common_layers.py:257-269)
   b.cbs("net.p5.3.cv1", s5, cp, 256, 1, 1, true);
   b.psablock("net.p5.3.middle_block", cp.slice(128, 128), 2);
-  ASTens h6cat = e.talloc(H0 / 32, W0 / 32, 384);              // cat(h5(p4''), p5)
-  ASTens p5 = h6cat.slice(128, 256);
+  Tens h6cat = e.talloc(H0 / 32, W0 / 32, 384);              // cat(h5(p4''), p5)
+  Tens p5 = h6cat.slice(128, 256);
   b.cbs("net.p5.3.cv2", cp, p5, 256, 1, 1, true);
   // ---- neck (auto_speed_neck.py:17-24)
   if (b.ok()) b.upsample("fpn.up_p5", p5, h1cat.slice(0, 256));
-  ASTens h4cat = e.talloc(H0 / 16, W0 / 16, 192);              // cat(h3(p3'), p4')
-  ASTens p4n = h4cat.slice(64, 128);
+  Tens h4cat = e.talloc(H0 / 16, W0 / 16, 192);              // cat(h3(p3'), p4')
+  Tens p4n = h4cat.slice(64, 128);
   b.c3k2("fpn.h1", h1cat, p4n, 128, false);
   if (b.ok()) b.upsample("fpn.up_p4", p4n, h2cat.slice(0, 128));
-  ASTens n3 = e.talloc(H0 / 8, W0 / 8, 64);
+  Tens n3 = e.talloc(H0 / 8, W0 / 8, 64);
   b.c3k2("fpn.h2", h2cat, n3, 64, false);
   b.cbs("fpn.h3", n3, h4cat.slice(0, 64), 64, 3, 2, true);
-  ASTens n4 = e.talloc(H0 / 16, W0 / 16, 128);
+  Tens n4 = e.talloc(H0 / 16, W0 / 16, 128);
   b.c3k2("fpn.h4", h4cat, n4, 128, false);
   b.cbs("fpn.h5", n4, h6cat.slice(0, 128), 128, 3, 2, true);
-  ASTens n5 = e.talloc(H0 / 32, W0 / 32, 256);
+  Tens n5 = e.talloc(H0 / 32, W0 / 32, 256);
   b.c3k2("fpn.h6", h6cat, n5, 256, true);
   // ---- head (auto_speed_head.py:36-49): per level [hw][72]: 64 box logits | 4 class logits | 4 zero
-  const ASTens feats[3] = {n3, n4, n5};
-  ASTens lv[3];
+  const Tens feats[3] = {n3, n4, n5};
+  Tens lv[3];
   for (int i = 0; i < 3 && b.ok(); ++i) {
-    const ASTens& f = feats[i];
+    const Tens& f = feats[i];
     const std::string bi = "head.box." + std::to_string(i), ci = "head.cls." + std::to_string(i);
     lv[i] = e.talloc(f.H, f.W, 72);
-    ASTens b1 = e.talloc(f.H, f.W, 64), b2 = e.talloc(f.H, f.W, 64);
+    Tens b1 = e.talloc(f.H, f.W, 64), b2 = e.talloc(f.H, f.W, 64);
     b.cbs(bi + ".0", f, b1, 64, 3, 1, true);
     b.cbs(bi + ".1", b1, b2, 64, 3, 1, true);
     b.plain(bi + ".2", b2, lv[i].slice(0, 64), 64, 1, ACT_NONE);
-    ASTens c1 = e.talloc(f.H, f.W, f.C), c2 = e.talloc(f.H, f.W, 80), c3 = e.talloc(f.H, f.W, 80), c4 = e.talloc(f.H, f.W, 80);
+    Tens c1 = e.talloc(f.H, f.W, f.C), c2 = e.talloc(f.H, f.W, 80), c3 = e.talloc(f.H, f.W, 80), c4 = e.talloc(f.H, f.W, 80);
     b.dw(ci + ".0", f, c1, true);
     b.cbs(ci + ".1", c1, c2, 80, 1, 1, true);
     b.dw(ci + ".2", c2, c3, true);
@@ -716,17 +641,17 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
       a0 += h * wd;
     }
   }
-  e.taps["p1"] = p1; e.taps["p2"] = p2; e.taps["p3"] = p3; e.taps["p4"] = p4; e.taps["p5_ctx"] = q5; e.taps["p5_sppf"] = s5;
-  e.taps["p5"] = p5; e.taps["n3"] = n3; e.taps["n4"] = n4; e.taps["n5"] = n5;
-  e.taps["head0"] = lv[0]; e.taps["head1"] = lv[1]; e.taps["head2"] = lv[2];
-  e.taps["canvas"] = x0;
+  e.tap("p1", p1); e.tap("p2", p2); e.tap("p3", p3); e.tap("p4", p4); e.tap("p5_ctx", q5); e.tap("p5_sppf", s5);
+  e.tap("p5", p5); e.tap("n3", n3); e.tap("n4", n4); e.tap("n5", n5);
+  for (int i = 0; i < 3; ++i) e.tap("head" + std::to_string(i), lv[i], 4 * kDfl + kNC);   // box | class logits, no padding
+  e.tap("canvas", x0, 3);                                                                  // RGB of the 8-channel canvas
   return VPB_OK;
 }
 
 static int as_launch_all(vp_autospeed& e, const uint8_t* src, int stride, cudaStream_t st) {
   int rc = e.pre.launch(&src, 1, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr, st);
   if (rc) return rc;
-  for (auto& op : e.ops) { rc = op(st); if (rc) return rc; }
+  for (auto& op : e.ops) { rc = op.launch(st); if (rc) return rc; }
   PostParams pp{};
   pp.raw = e.d_raw; pp.NA = kNA; pp.conf = e.conf; pp.iou = e.iou; pp.scale = e.scale; pp.pad_x = e.pad_x; pp.pad_y = e.pad_y;
   pp.orig_w = e.src_w; pp.orig_h = e.src_h; pp.max_cand = vp_autospeed::kMaxCand; pp.max_det = vp_autospeed::kMaxDet;
@@ -752,51 +677,17 @@ static int as_configure(vp_autospeed& e, int h, int w) {
   else fill_canvas_kernel<F16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__half*>(e.d_canvas), npix);
   VPB_CUDA_OK(cudaGetLastError());
   e.src_h = h; e.src_w = w;
-  if (e.gexec) { cudaGraphExecDestroy(e.gexec); e.gexec = nullptr; }
   return VPB_OK;
 }
 
 static int as_enqueue(vp_autospeed& e, const uint8_t* src, int h, int w, int stride) {
   int rc = as_configure(e, h, w);
   if (rc) return rc;
-  if (e.gexec && e.g_stride == stride && e.g_src != src && e.g_pre_node) {
-    // same geometry, another frame buffer: re-point the letterbox node instead of re-capturing
-    rc = e.pre.update_graph_node(e.gexec, e.g_pre_node, &src, 1, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
-    if (rc) return rc;
-    e.g_src = src;
-  }
-  if (!e.gexec || e.g_src != src || e.g_stride != stride) {
-    if (e.gexec) { cudaGraphExecDestroy(e.gexec); e.gexec = nullptr; }
-    e.g_pre_node = nullptr;
-    rc = as_launch_all(e, src, stride, e.stream);             // warm (function attributes) + correct results
-    if (rc) return rc;
-    VPB_CUDA_OK(cudaStreamSynchronize(e.stream));
-    cudaGraph_t g = nullptr;
-    VPB_CUDA_OK(cudaStreamBeginCapture(e.stream, cudaStreamCaptureModeThreadLocal));
-    rc = as_launch_all(e, src, stride, e.stream);
-    const cudaError_t ce = cudaStreamEndCapture(e.stream, &g);
-    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
-    if (ce != cudaSuccess) { vpb_set_error("autospeed: graph capture failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    {
-      size_t nn = 0;
-      cudaGraphGetNodes(g, nullptr, &nn);
-      std::vector<cudaGraphNode_t> nodes(nn);
-      cudaGraphGetNodes(g, nodes.data(), &nn);
-      for (size_t i = 0; i < nn; ++i) {
-        cudaGraphNodeType ty;
-        if (cudaGraphNodeGetType(nodes[i], &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
-        cudaKernelNodeParams kp{};
-        if (cudaGraphKernelNodeGetParams(nodes[i], &kp) == cudaSuccess && e.pre.owns_kernel(kp.func, e.dtype)) { e.g_pre_node = nodes[i]; break; }
-      }
-    }
-    const cudaError_t ci = cudaGraphInstantiate(&e.gexec, g, 0);
-    if (e.graph) cudaGraphDestroy(e.graph);
-    e.graph = g;
-    if (ci != cudaSuccess) { vpb_set_error("autospeed: graph instantiate failed: %s", cudaGetErrorString(ci)); return VPB_ERR_CUDA; }
-    e.g_src = src; e.g_stride = stride;
-  }
-  VPB_CUDA_OK(cudaGraphLaunch(e.gexec, e.stream));
-  return VPB_OK;
+  return e.frame_graph.run(
+      e.stream, e.pre, e.dtype, h, w, stride, FrameSrcs{src}, [&](cudaStream_t st) { return as_launch_all(e, src, stride, st); },
+      [&](cudaGraphExec_t x, cudaGraphNode_t n) {
+        return e.pre.update_graph_node(x, n, &src, 1, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
+      });
 }
 
 }  // namespace vpb
@@ -806,19 +697,11 @@ extern "C" int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtyp
   if (!out) return VPB_ERR_ARG;
   *out = nullptr;
   if (!weights_vpw || !weights_vpw[0]) { vpb_set_error("vp_autospeed_create: no checkpoint path"); return VPB_ERR_ARG; }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || gpu_id < 0 || gpu_id >= ndev) {
-    vpb_set_error("vp_autospeed_create: no CUDA device %d (this engine has no CPU fallback)", gpu_id);
-    return VPB_ERR_CUDA;
-  }
-  DeviceGuard guard(gpu_id);
-  cudaDeviceProp prop;
-  VPB_CUDA_OK(cudaGetDeviceProperties(&prop, gpu_id));
-  if (prop.major != 9 || prop.minor != 0) { vpb_set_error("vp_autospeed_create: device %d is sm_%d%d; built for sm_90a only", gpu_id, prop.major, prop.minor); return VPB_ERR_CUDA; }
   std::unique_ptr<vp_autospeed> e(new vp_autospeed());
-  e->gpu_id = gpu_id; e->dtype = dtype == VPB_BF16 ? VPB_BF16 : VPB_F16;
-  if (stream) e->stream = static_cast<cudaStream_t>(stream);
-  else { VPB_CUDA_OK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking)); e->own_stream = true; }
+  int rc = e->open("vp_autospeed_create", gpu_id, stream);
+  if (rc) return rc;
+  DeviceGuard guard(gpu_id);
+  e->dtype = dtype == VPB_BF16 ? VPB_BF16 : VPB_F16;
   e->d_canvas = e->dalloc(static_cast<size_t>(kASW) * kASH * 8 * 2);
   e->d_raw = static_cast<float*>(e->dalloc(static_cast<size_t>(8) * kNA * 4));
   e->h_raw = static_cast<float*>(e->halloc(static_cast<size_t>(8) * kNA * 4));
@@ -828,9 +711,9 @@ extern "C" int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtyp
   e->d_counts = static_cast<int*>(e->dalloc(64));
   e->h_det = static_cast<float*>(e->halloc(static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4));
   e->h_counts = static_cast<int*>(e->halloc(64));
-  if (e->oom) return VPB_ERR_CUDA;
+  if (e->oom || !e->h_raw || !e->h_det || !e->h_counts) return VPB_ERR_CUDA;
   WeightMap w;
-  int rc = load_vpw(weights_vpw, w);
+  rc = load_vpw(weights_vpw, w);
   if (rc) return rc;
   rc = as_build(*e, w);
   if (e->oom) return VPB_ERR_CUDA;
@@ -845,7 +728,8 @@ extern "C" void vp_autospeed_destroy(vp_autospeed* e) { delete e; }
 extern "C" int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float iou) {
   if (!e) return VPB_ERR_ARG;
   e->conf = conf; e->iou = iou;
-  if (e->gexec) { DeviceGuard g(e->gpu_id); cudaGraphExecDestroy(e->gexec); e->gexec = nullptr; }
+  DeviceGuard g(e->gpu_id);
+  e->frame_graph.invalidate();           // the thresholds are arguments of the captured NMS kernel
   return VPB_OK;
 }
 
@@ -859,17 +743,10 @@ static int as_fetch(vp_autospeed* e, bool raw) {
 extern "C" int vp_autospeed_infer(vp_autospeed* e, const uint8_t* frame_host, int h, int w, int stride, int fetch_raw) {
   if (!e || !frame_host || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("vp_autospeed_infer: bad arguments"); return VPB_ERR_ARG; }
   DeviceGuard guard(e->gpu_id);
-  const int dpitch = w * 3;
-  const size_t bytes = static_cast<size_t>(h) * dpitch;
-  if (bytes > e->d_frame_cap) {
-    void* p = e->dalloc(bytes + 256);
-    if (!p) return VPB_ERR_CUDA;
-    e->d_frame = static_cast<uint8_t*>(p); e->d_frame_cap = bytes;
-    if (e->gexec) { cudaGraphExecDestroy(e->gexec); e->gexec = nullptr; }
-  }
-  if (stride == dpitch) VPB_CUDA_OK(cudaMemcpyAsync(e->d_frame, frame_host, bytes, cudaMemcpyHostToDevice, e->stream));
-  else VPB_CUDA_OK(cudaMemcpy2DAsync(e->d_frame, dpitch, frame_host, stride, dpitch, h, cudaMemcpyHostToDevice, e->stream));
-  int rc = as_enqueue(*e, e->d_frame, h, w, dpitch);
+  FrameSrcs dev;
+  int rc = e->upload_frames(&frame_host, 1, h, w, stride, dev);
+  if (rc) return rc;
+  rc = as_enqueue(*e, dev[0], h, w, w * 3);
   if (rc) return rc;
   rc = as_fetch(e, fetch_raw != 0);
   if (rc) return rc;
@@ -910,7 +787,11 @@ extern "C" int vp_autospeed_raw(vp_autospeed* e, const float** raw_host, const f
 extern "C" int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flops) {
   if (!e) return VPB_ERR_ARG;
   if (n_launches) *n_launches = static_cast<int>(e->ops.size()) + 2;
-  if (flops) *flops = e->flops;
+  if (flops) {
+    double f = 0;
+    for (const auto& op : e->ops) f += op.flops;       // build order: the same sum as accumulated while building
+    *flops = f;
+  }
   return VPB_OK;
 }
 
@@ -918,23 +799,5 @@ extern "C" long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* 
   if (!e || !name) return VPB_ERR_ARG;
   auto it = e->taps.find(name);
   if (it == e->taps.end()) { vpb_set_error("no tap '%s'", name); return VPB_ERR_ARG; }
-  const ASTens& a = it->second;
-  const int Cv = strcmp(name, "canvas") == 0 ? 3 : (strncmp(name, "head", 4) == 0 ? 68 : a.C);
-  const long n = static_cast<long>(a.H) * a.W * Cv;
-  if (c) *c = Cv; if (h) *h = a.H; if (w) *w = a.W;
-  if (!dst) return n;
-  if (cap < n) { vpb_set_error("tap buffer too small"); return VPB_ERR_ARG; }
-  DeviceGuard guard(e->gpu_id);
-  if (static_cast<size_t>(n) > e->tap_cap) {
-    if (e->d_tap_scratch) { cudaFree(e->d_tap_scratch); e->d_tap_scratch = nullptr; e->tap_cap = 0; }
-    VPB_CUDA_OK(cudaMalloc(&e->d_tap_scratch, static_cast<size_t>(n) * 4));
-    e->tap_cap = static_cast<size_t>(n);
-  }
-  const int blocks = static_cast<int>((n + 255) / 256);
-  if (e->dtype == VPB_BF16) tap_slice_to_f32<<<blocks, 256, 0, e->stream>>>(static_cast<const __nv_bfloat16*>(a.p), a.H, a.W, Cv, a.ld, e->d_tap_scratch);
-  else tap_slice_to_f32<<<blocks, 256, 0, e->stream>>>(static_cast<const __half*>(a.p), a.H, a.W, Cv, a.ld, e->d_tap_scratch);
-  cudaError_t ce = cudaMemcpyAsync(dst, e->d_tap_scratch, n * 4, cudaMemcpyDeviceToHost, e->stream);
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
-  if (ce != cudaSuccess) { vpb_set_error("read_tap: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-  return n;
+  return e->read_tap(it->second.t, it->second.channels, dst, cap, c, h, w);
 }

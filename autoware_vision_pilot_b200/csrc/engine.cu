@@ -14,64 +14,15 @@
 #include "../../include/vp_b200.h"
 #include "engine_internal.h"
 
-#include <array>
 #include <cmath>
-#include <cstdio>
 #include <cstring>
 #include <functional>
 #include <map>
 #include <memory>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 namespace vpb {
-
-// =============================================================== weight file (.vpw)
-// magic "VPW1", u32 n; per tensor: u32 name_len, name, u32 dtype (0 f32, 1 i64), u32 ndim,
-// u32 dims[ndim], u64 nbytes, raw little-endian data.  Written by
-// autoware_vision_pilot_b200/weights.py from the reference's .pth state_dict (SURVEY App. C).
-int load_vpw(const char* path, WeightMap& out) {
-  FILE* fp = fopen(path, "rb");
-  if (!fp) { vpb_set_error("cannot open weight file '%s'", path); return VPB_ERR_IO; }
-  auto fail = [&](const char* why) { fclose(fp); vpb_set_error("%s: %s", path, why); return VPB_ERR_IO; };
-  if (fseek(fp, 0, SEEK_END) != 0) return fail("cannot seek");
-  const long file_size = ftell(fp);
-  rewind(fp);
-  char magic[4]; uint32_t n = 0;
-  if (fread(magic, 1, 4, fp) != 4 || memcmp(magic, "VPW1", 4) != 0) return fail("not a VPW1 file");
-  if (fread(&n, 4, 1, fp) != 1 || n > 100000) return fail("bad tensor count");
-  for (uint32_t i = 0; i < n; ++i) {
-    uint32_t nl = 0, dt = 0, nd = 0; uint64_t nb = 0;
-    if (fread(&nl, 4, 1, fp) != 1 || nl > 4096) return fail("bad name length");
-    std::string name(nl, '\0');
-    if (fread(&name[0], 1, nl, fp) != nl) return fail("truncated name");
-    if (fread(&dt, 4, 1, fp) != 1 || fread(&nd, 4, 1, fp) != 1 || nd > 8) return fail("bad header");
-    HostTensor t; t.dims.resize(nd);
-    for (uint32_t d = 0; d < nd; ++d) { uint32_t v; if (fread(&v, 4, 1, fp) != 1) return fail("bad dims"); t.dims[d] = static_cast<int>(v); }
-    if (fread(&nb, 8, 1, fp) != 1) return fail("bad size");
-    size_t ne = 1;
-    bool dims_ok = true;
-    for (int d : t.dims) {                                   // bounded: no overflow, no absurd allocation
-      if (d < 0 || (d > 0 && ne > (static_cast<size_t>(1) << 31) / static_cast<size_t>(d))) { dims_ok = false; break; }
-      ne *= static_cast<size_t>(d);
-    }
-    if (!dims_ok) return fail("tensor dims out of range");
-    if (dt == 0) {
-      if (nb != ne * 4) return fail("f32 size mismatch");
-      t.f.resize(ne);
-      if (ne && fread(t.f.data(), 4, ne, fp) != ne) return fail("truncated data");
-    } else {
-      // num_batches_tracked (int64 scalar): skipped, but the payload must really be there
-      const long here = ftell(fp);
-      if (here < 0 || nb > static_cast<uint64_t>(file_size - here) || fseek(fp, static_cast<long>(nb), SEEK_CUR) != 0)
-        return fail("truncated data");
-    }
-    out[name] = std::move(t);
-  }
-  fclose(fp);
-  return VPB_OK;
-}
 
 static uint64_t fnv1a(uint64_t h, const void* p, size_t n) {
   const uint8_t* b = static_cast<const uint8_t*>(p);
@@ -90,24 +41,6 @@ static uint64_t hash_prefix(const WeightMap& w, const std::string& pfx) {
 }
 
 // =============================================================== engine
-struct Tens {  // NHWC 16-bit activation, channel stride == C; pad = 1: zero-bordered [(H+2)*(W+2)][C]
-  void* p = nullptr; int H = 0, W = 0, C = 0, pad = 0;
-  void* lo = nullptr;   // split-fp16 mode: the low half (same layout), NULL otherwise
-  size_t bytes() const { return static_cast<size_t>(H + 2 * pad) * (W + 2 * pad) * C * 2; }
-};
-
-struct OpRec {
-  std::string name;
-  std::function<int(cudaStream_t)> launch;
-  double flops = 0;     // 2*MAC this launch executes
-  double flops_ref = -1; // 2*MAC of the reference's layers this op stands for (< 0: same as flops)
-  double bytes = 0;     // algorithmic HBM bytes per launch (HBM-bound stages; SURVEY.md 8d definitions)
-  std::string kname;    // kernel the op launches (roofline report groups launches by kernel)
-  bool gemm = false;
-  int kind = 0;   // 0 = not a convolution GEMM, 1 = conv_gemm_kernel, 2 = conv3x3_lin_kernel, 3 = conv3x3_pair_kernel
-  int lane = 0;   // execution lane (= index of the model that owns the op); lanes run concurrently
-};
-
 struct ModelOut {
   int kind = 0, C = 0, H = 0, W = 0;
   float* d_raw = nullptr; uint8_t* d_cls = nullptr;
@@ -129,35 +62,17 @@ static Prefixes prefixes_for(int kind) {
 
 using namespace vpb;
 
-using vpb::DeviceGuard;
-
-struct vp_engine {
+struct vp_engine : EngineRuntime {
   vp_engine_config cfg{};
-  int gpu_id = 0;
-  bool oom = false;                       // a device / pinned allocation failed during construction
-  bool split = false;                     // VP_PREC_SPLIT: every 16-bit tensor is a (hi, lo) pair, GEMMs run 3 K segments
-  std::unordered_map<const void*, void*> lo_of;   // 16-bit weight buffer -> its low half (split mode)
-  void* lo(const void* hi) const { auto it = lo_of.find(hi); return it == lo_of.end() ? nullptr : it->second; }
   void* d_pre_lo = nullptr;
-  int dtype = VPB_F16;
   // frames per call (vp_engine_config.batch): every activation, the pre-process output and the model outputs hold
   // `batch` samples back to back (batch outermost); weights, the launch list and the graph are those of one call
   int batch = 1;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
-  std::vector<void*> dev_allocs;
-  std::vector<void*> host_allocs;
-  size_t weight_bytes = 0, act_bytes = 0;
-  std::vector<OpRec> ops;                 // network ops (after the pre-process)
-  std::vector<std::unique_ptr<ConvPlan>> plans;
   PreprocessPlan pre;
-  uint8_t* d_frame = nullptr; size_t d_frame_cap = 0;
   uint8_t* h_frame = nullptr; size_t h_frame_cap = 0;
   void* d_pre = nullptr;                  // [320][640][4]
   uint8_t* d_resized = nullptr;           // optional uint8 resized image (tap "resized")
-  float* d_tap_scratch = nullptr; size_t tap_scratch_cap = 0;   // vp_engine_read_tap staging (grown on demand)
   std::vector<ModelOut> outs;
-  std::map<std::string, Tens> taps;
   int shared_encoders = 0, shared_trunks = 0;
   // SE pooling accumulators of every MBConv block: one arena, zeroed by one memset per frame; one accumulator set per
   // sample of the batch
@@ -171,12 +86,6 @@ struct vp_engine {
     gap_used += (need + 31) / 32 * 32;
     return p;
   }
-  // graph
-  cudaGraphExec_t gexec = nullptr;
-  cudaGraph_t graph = nullptr;           // kept alive: g_pre_node is a handle into it
-  int g_h = 0, g_w = 0, g_stride = 0;
-  std::array<const uint8_t*, kMaxBatch> g_src{};   // frames of the captured / last call ([0] == NULL: none yet)
-  cudaGraphNode_t g_pre_node = nullptr;  // the captured pre-process kernel node (re-pointed per frame)
   // module caches for sharing
   struct EncOut { Tens f[5]; };
   std::map<uint64_t, EncOut> enc_cache;
@@ -195,63 +104,17 @@ struct vp_engine {
 
   ~vp_engine() {
     DeviceGuard guard(gpu_id);
-    if (d_tap_scratch) cudaFree(d_tap_scratch);
-    if (gexec) cudaGraphExecDestroy(gexec);
-    if (graph) cudaGraphDestroy(graph);
     for (size_t i = 1; i < lane_streams.size(); ++i) if (lane_streams[i]) cudaStreamDestroy(lane_streams[i]);
     for (auto ev : op_events) if (ev) cudaEventDestroy(ev);
     for (auto ev : lane_done) if (ev) cudaEventDestroy(ev);
     if (ev_pre) cudaEventDestroy(ev_pre);
-    for (void* p : dev_allocs) cudaFree(p);
-    for (void* p : host_allocs) cudaFreeHost(p);
-    if (own_stream && stream) cudaStreamDestroy(stream);
   }
 
-  // ---------------------------------------------------------- allocation / upload helpers
-  void* dalloc(size_t bytes, bool is_weight) {
-    void* p = nullptr;
-    const cudaError_t ce = cudaMalloc(&p, std::max<size_t>(bytes, 256));
-    if (ce != cudaSuccess || !p) {
-      // sticky: vp_engine_create reports it (uploads below skip NULL, nothing is launched during construction)
-      if (!oom) vpb_set_error("cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(ce));
-      oom = true;
-      cudaGetLastError();
-      return nullptr;
-    }
-    cudaMemset(p, 0, std::max<size_t>(bytes, 256));
-    dev_allocs.push_back(p);
-    (is_weight ? weight_bytes : act_bytes) += bytes;
-    return p;
-  }
   Tens act_alloc(int H, int W, int C, int pad = 0) {
-    Tens a; a.H = H; a.W = W; a.C = C; a.pad = pad;
+    Tens a; a.H = H; a.W = W; a.C = C; a.ld = C; a.pad = pad;
     a.p = dalloc(a.bytes() * batch * (split ? 2 : 1), false);
     if (split && a.p) a.lo = static_cast<uint8_t*>(a.p) + a.bytes();
     return a;
-  }
-  float* upload_f32(const std::vector<float>& v) {
-    float* p = static_cast<float*>(dalloc(v.size() * 4, true));
-    if (p) cudaMemcpy(p, v.data(), v.size() * 4, cudaMemcpyHostToDevice);
-    return p;
-  }
-  void* upload_16(const std::vector<float>& v) {
-    const size_t n = v.size();
-    std::vector<uint16_t> h(split ? 2 * n : n);     // split mode: [hi | lo], lo = round16(v - hi)
-    for (size_t i = 0; i < n; ++i) {
-      if (dtype == VPB_BF16) {
-        __nv_bfloat16 b = __float2bfloat16_rn(v[i]); memcpy(&h[i], &b, 2);
-        if (split) { __nv_bfloat16 l = __float2bfloat16_rn(v[i] - __bfloat162float(b)); memcpy(&h[n + i], &l, 2); }
-      } else {
-        __half b = __float2half_rn(v[i]); memcpy(&h[i], &b, 2);
-        if (split) { __half l = __float2half_rn(v[i] - __half2float(b)); memcpy(&h[n + i], &l, 2); }
-      }
-    }
-    void* p = dalloc(h.size() * 2, true);
-    if (p) {
-      cudaMemcpy(p, h.data(), h.size() * 2, cudaMemcpyHostToDevice);
-      if (split) lo_of[p] = static_cast<uint8_t*>(p) + n * 2;
-    }
-    return p;
   }
 
   // ---------------------------------------------------------- op emitters
@@ -261,12 +124,12 @@ struct vp_engine {
                const Tens* in2 = nullptr, const void* w2 = nullptr, int taps2 = 0) {
     vpb_conv_args a{};
     a.batch = batch;
-    a.dtype = dtype; a.H = in.H; a.W = in.W; a.Cin = in.C; a.ldi = in.C;
+    a.dtype = dtype; a.H = in.H; a.W = in.W; a.Cin = in.C; a.ldi = in.ld;
     a.Cout = Cout; a.taps = taps; a.phases = phases; a.act = act; a.mode = mode;
     a.final_kind = final_kind; a.in = in.p; a.w = w; a.bias = bias;
     a.in_pad = in.pad;
-    if (out) { a.out = out->p; a.ldo = out->C; a.out_pad = out->pad; }
-    if (res) { a.res = res->p; a.ldr = res->C; a.res_pad = res->pad; }
+    if (out) { a.out = out->p; a.ldo = out->ld; a.out_pad = out->pad; }
+    if (res) { a.res = res->p; a.ldr = res->ld; a.res_pad = res->pad; }
     // 3x3 on a zero-bordered input -> linear-padded kernel (one TMA segment per kernel row); the split-fp16 mode
     // runs everything on the tile kernel (three K segments per chunk)
     a.algo = (taps == 9 && in.pad && !split) ? VPB_ALGO_LINEAR : VPB_ALGO_TILE;
@@ -277,18 +140,8 @@ struct vp_engine {
       if (in2) { a.in2_lo = in2->lo; a.w2_lo = lo(w2); }
     }
     a.out_f32 = out_f32; a.out_cls = out_cls;
-    if (in2) { a.in2 = in2->p; a.w2 = w2; a.Cin2 = in2->C; a.ld2 = in2->C; a.in2_pad = in2->pad; a.taps2 = taps2; }
-    auto plan = std::make_unique<ConvPlan>();
-    int rc = conv_plan_build(&a, plan.get());
-    if (rc != VPB_OK) return rc;
-    ConvPlan* pp = plan.get();
-    plans.push_back(std::move(plan));
-    OpRec op; op.name = name; op.flops = pp->flops; op.gemm = true; op.lane = cur_lane;
-    op.kind = a.algo == VPB_ALGO_LINEAR ? 2 : 1;
-    op.kname = "conv_wgmma_kernel";
-    op.launch = [pp](cudaStream_t s) { return conv_plan_launch(pp, s); };
-    ops.push_back(std::move(op));
-    return VPB_OK;
+    if (in2) { a.in2 = in2->p; a.w2 = w2; a.Cin2 = in2->C; a.ld2 = in2->ld; a.in2_pad = in2->pad; a.taps2 = taps2; }
+    return append_conv(name, a, cur_lane);
   }
   // flops: per sample (counted for the whole batch); bytes: per launch
   void add_op(const std::string& name, const char* kname, std::function<int(cudaStream_t)> fn, double flops = 0,
@@ -299,33 +152,6 @@ struct vp_engine {
 };
 
 namespace vpb {
-
-#define NEED(w, key)                                                             \
-  auto it_##__LINE__ = (w).find(key);                                            \
-  if (it_##__LINE__ == (w).end()) { vpb_set_error("weight '%s' missing", std::string(key).c_str()); return VPB_ERR_IO; }
-
-const HostTensor* find_w(const WeightMap& w, const std::string& key) {
-  auto it = w.find(key);
-  if (it == w.end()) { vpb_set_error("weight '%s' missing from checkpoint", key.c_str()); return nullptr; }
-  return &it->second;
-}
-
-// Every tensor's shape is checked against what the architecture expects before it is indexed: a checkpoint
-// of another variant, or a truncated / corrupt file, fails with VPB_ERR_IO instead of reading out of bounds.
-const HostTensor* find_w_shaped(const WeightMap& w, const std::string& key, std::initializer_list<int> dims) {
-  const HostTensor* t = find_w(w, key);
-  if (!t) return nullptr;
-  bool ok = t->dims.size() == dims.size() && t->f.size() == t->numel();
-  if (ok) { size_t i = 0; for (int d : dims) { if (d >= 0 && t->dims[i] != d) ok = false; ++i; } }
-  if (!ok) {
-    std::string got, want;
-    for (int d : t->dims) got += std::to_string(d) + ",";
-    for (int d : dims) want += (d < 0 ? std::string("*") : std::to_string(d)) + ",";
-    vpb_set_error("weight '%s' has shape [%s] but this architecture needs [%s]", key.c_str(), got.c_str(), want.c_str());
-    return nullptr;
-  }
-  return t;
-}
 
 // BatchNorm folding (eval mode, eps 1e-5 — torchvision EfficientNet-B0): y = conv(x)*s + t
 static bool bn_fold(const WeightMap& w, const std::string& p, int C, std::vector<float>& s, std::vector<float>& t) {
@@ -340,17 +166,6 @@ static bool bn_fold(const WeightMap& w, const std::string& p, int C, std::vector
   return true;
 }
 
-// Conv2d weight [Cout][Cin][k][k] -> [k*k][Cout][Cin] (optionally scaled per Cout)
-std::vector<float> pack_conv(const HostTensor& t, const std::vector<float>* scale) {
-  const int Cout = t.dims[0], Cin = t.dims[1], k = t.dims[2];
-  std::vector<float> o(t.f.size());
-  for (int co = 0; co < Cout; ++co)
-    for (int ci = 0; ci < Cin; ++ci)
-      for (int tt = 0; tt < k * k; ++tt)
-        o[(static_cast<size_t>(tt) * Cout + co) * Cin + ci] =
-            t.f[(static_cast<size_t>(co) * Cin + ci) * k * k + tt] * (scale ? (*scale)[co] : 1.0f);
-  return o;
-}
 // ConvTranspose2d weight [Cin][Cout][2][2] -> [a*2+b][Cout][Cin]
 static std::vector<float> pack_convT(const HostTensor& t) {
   const int Cin = t.dims[0], Cout = t.dims[1];
@@ -667,13 +482,9 @@ static int final_conv(vp_engine& e, const WeightMap& w, const std::string& key, 
   mo.d_raw = static_cast<float*>(e.dalloc(n * 4 * nb, false));
   mo.has_cls = final_kind != VPB_FINAL_NONE;
   if (mo.has_cls) mo.d_cls = static_cast<uint8_t*>(e.dalloc(static_cast<size_t>(in.H) * in.W * nb, false));
-  void* hp = nullptr;
-  if (cudaMallocHost(&hp, n * 4 * nb) != cudaSuccess) { vpb_set_error("cudaMallocHost failed"); return VPB_ERR_CUDA; }
-  e.host_allocs.push_back(hp); mo.h_raw = static_cast<float*>(hp);
-  if (mo.has_cls) {
-    if (cudaMallocHost(&hp, static_cast<size_t>(in.H) * in.W * nb) != cudaSuccess) { vpb_set_error("cudaMallocHost failed"); return VPB_ERR_CUDA; }
-    e.host_allocs.push_back(hp); mo.h_cls = static_cast<uint8_t*>(hp);
-  }
+  mo.h_raw = static_cast<float*>(e.halloc(n * 4 * nb));
+  if (mo.has_cls) mo.h_cls = static_cast<uint8_t*>(e.halloc(static_cast<size_t>(in.H) * in.W * nb));
+  if (!mo.h_raw || (mo.has_cls && !mo.h_cls)) return VPB_ERR_CUDA;
   return e.add_conv(name, in, Cout, 9, 1, dw_, db, ACT_NONE, VPB_EPI_FINAL, nullptr, nullptr, final_kind, mo.d_raw, mo.d_cls);
 }
 
@@ -700,7 +511,7 @@ static int build_head(vp_engine& e, const WeightMap& w, const std::string& p, co
     rc = conv_layer(e, w, p + "decode_layer_8", tag + "dec8", u4, 9, ACT_GELU, VPB_EPI_STORE, &c, nullptr); if (rc) return rc;
   }
   rc = conv_layer(e, w, p + "decode_layer_9", tag + "dec9", c, 9, ACT_GELU, VPB_EPI_STORE, &d, nullptr); if (rc) return rc;
-  e.taps[tag + "d9"] = d;
+  e.tap(tag + "d9", d);
   const int fk = kind == VP_SCENE_SEG ? VPB_FINAL_ARGMAX : kind == VP_DOMAIN_SEG ? VPB_FINAL_THRESH : VPB_FINAL_NONE;
   return final_conv(e, w, p + "decode_layer_10", tag + "dec10", d, fk, mo);
 }
@@ -720,7 +531,7 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
     e.enc_cache[h_enc] = enc;
     e.enc_last_op[h_enc] = static_cast<int>(e.ops.size()) - 1;
   }
-  for (int i = 0; i < 5; ++i) e.taps[tag + "f" + std::to_string(i)] = enc.f[i];
+  for (int i = 0; i < 5; ++i) e.tap(tag + "f" + std::to_string(i), enc.f[i]);
   uint64_t h_trunk = h_enc;
   { const uint64_t a = hash_prefix(w, pf.ctx), b = hash_prefix(w, pf.neck); h_trunk = fnv1a(fnv1a(h_trunk, &a, 8), &b, 8); }
   Tens neck;
@@ -738,12 +549,12 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
       const int nb = e.batch;
       e.add_op(tag + "fuse", "fuse_pool_kernel", [=](cudaStream_t st) { return fuse_pool_x(dt, f0, f1, f2, f3, f4, lo.v, H4, W4, o, o_lo, st, nb); },
                0.0, nb * 2.0 * (160.0 * 320 * 32 + 80.0 * 160 * 24 + 40.0 * 80 * 40 + 20.0 * 40 * 80 + 200.0 * 1280 + 200.0 * 1456));
-      e.taps[tag + "fused"] = feat;
+      e.tap(tag + "fused", feat);
     }
     Tens ctx;
     int rc = build_context(e, w, pf.ctx, tag, feat, &ctx);
     if (rc) return rc;
-    e.taps[tag + "context"] = ctx;
+    e.tap(tag + "context", ctx);
     rc = build_neck(e, w, pf.neck, tag, ctx, enc, &neck);
     if (rc) return rc;
     e.trunk_cache[h_trunk] = neck;
@@ -751,21 +562,11 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
   }
   e.lane_dep.resize(idx + 1, -1);
   e.lane_dep[idx] = dep;
-  e.taps[tag + "neck"] = neck;
+  e.tap(tag + "neck", neck);
   ModelOut mo; mo.kind = kind;
   int rc = build_head(e, w, pf.head, tag, kind, neck, enc, mo);
   if (rc) return rc;
   e.outs.push_back(mo);
-  return VPB_OK;
-}
-
-static int ensure_frame_buffers(vp_engine& e, size_t bytes) {
-  if (bytes <= e.d_frame_cap) return VPB_OK;
-  if (e.gexec) { cudaGraphExecDestroy(e.gexec); e.gexec = nullptr; }
-  void* p = nullptr;
-  VPB_CUDA_OK(cudaMalloc(&p, bytes + 256));
-  e.dev_allocs.push_back(p);
-  e.d_frame = static_cast<uint8_t*>(p); e.d_frame_cap = bytes;
   return VPB_OK;
 }
 
@@ -826,51 +627,14 @@ static int launch_all(vp_engine& e, const uint8_t* const* srcs, int stride, cuda
 static int enqueue_frame(vp_engine& e, const uint8_t* const* srcs, int h, int w, int stride) {
   int rc = e.pre.configure(h, w, e.cfg.resize_mode);
   if (rc) return rc;
-  std::array<const uint8_t*, kMaxBatch> src{};
+  FrameSrcs src{};
   std::copy(srcs, srcs + e.batch, src.begin());
   if (!e.cfg.use_graph) return launch_all(e, src.data(), stride, e.stream);
-  if (e.gexec && e.g_h == h && e.g_w == w && e.g_stride == stride && e.g_src != src && e.g_pre_node) {
-    // same geometry, different frame buffers: re-point the pre-process node instead of re-capturing
-    rc = e.pre.update_graph_node(e.gexec, e.g_pre_node, src.data(), e.batch, stride, e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
-    if (rc) return rc;
-    e.g_src = src;
-  }
-  if (!e.gexec || e.g_h != h || e.g_w != w || e.g_stride != stride || e.g_src != src) {
-    if (e.gexec) { cudaGraphExecDestroy(e.gexec); e.gexec = nullptr; }
-    e.g_pre_node = nullptr;
-    // warm (sets function attributes outside capture), then capture
-    rc = launch_all(e, src.data(), stride, e.stream);
-    if (rc) return rc;
-    VPB_CUDA_OK(cudaStreamSynchronize(e.stream));
-    cudaGraph_t g = nullptr;
-    VPB_CUDA_OK(cudaStreamBeginCapture(e.stream, cudaStreamCaptureModeThreadLocal));
-    rc = launch_all(e, src.data(), stride, e.stream);
-    cudaError_t ce = cudaStreamEndCapture(e.stream, &g);
-    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
-    if (ce != cudaSuccess) { vpb_set_error("graph capture failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    {  // locate the pre-process kernel node
-      size_t nn = 0;
-      cudaGraphGetNodes(g, nullptr, &nn);
-      std::vector<cudaGraphNode_t> nodes(nn);
-      cudaGraphGetNodes(g, nodes.data(), &nn);
-      for (size_t i = 0; i < nn; ++i) {
-        cudaGraphNodeType ty;
-        if (cudaGraphNodeGetType(nodes[i], &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
-        cudaKernelNodeParams kp{};
-        if (cudaGraphKernelNodeGetParams(nodes[i], &kp) == cudaSuccess && e.pre.owns_kernel(kp.func, e.dtype)) {
-          e.g_pre_node = nodes[i];
-          break;
-        }
-      }
-    }
-    ce = cudaGraphInstantiate(&e.gexec, g, 0);
-    if (e.graph) cudaGraphDestroy(e.graph);
-    e.graph = g;
-    if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    e.g_h = h; e.g_w = w; e.g_stride = stride; e.g_src = src;
-  }
-  VPB_CUDA_OK(cudaGraphLaunch(e.gexec, e.stream));
-  return VPB_OK;
+  return e.frame_graph.run(
+      e.stream, e.pre, e.dtype, h, w, stride, src, [&](cudaStream_t st) { return launch_all(e, src.data(), stride, st); },
+      [&](cudaGraphExec_t x, cudaGraphNode_t n) {
+        return e.pre.update_graph_node(x, n, src.data(), e.batch, stride, e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
+      });
 }
 
 }  // namespace vpb
@@ -884,25 +648,11 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
     return VPB_ERR_ARG;
   }
   *out = nullptr;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-    vpb_set_error("vp_engine_create: no CUDA device (this engine has no CPU fallback)");
-    return VPB_ERR_CUDA;
-  }
-  if (cfg->gpu_id < 0 || cfg->gpu_id >= ndev) {
-    vpb_set_error("vp_engine_create: gpu_id %d out of range (%d devices)", cfg->gpu_id, ndev);
-    return VPB_ERR_ARG;
-  }
-  DeviceGuard guard(cfg->gpu_id);
-  cudaDeviceProp prop;
-  VPB_CUDA_OK(cudaGetDeviceProperties(&prop, cfg->gpu_id));
-  if (prop.major != 9 || prop.minor != 0) {
-    vpb_set_error("vp_engine_create: device %d is sm_%d%d; this library is built for sm_90a only", cfg->gpu_id, prop.major, prop.minor);
-    return VPB_ERR_CUDA;
-  }
   std::unique_ptr<vp_engine> e(new vp_engine());
+  int rc = e->open("vp_engine_create", cfg->gpu_id, cfg->stream);
+  if (rc) return rc;
+  DeviceGuard guard(cfg->gpu_id);
   e->cfg = *cfg;
-  e->gpu_id = cfg->gpu_id;
   e->dtype = cfg->dtype == VPB_BF16 ? VPB_BF16 : VPB_F16;
   if (cfg->precision != VP_PREC_16 && cfg->precision != VP_PREC_SPLIT) {
     vpb_set_error("vp_engine_create: unknown precision %d", cfg->precision);
@@ -919,15 +669,13 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
     vpb_set_error("vp_engine_create: batch > 1 needs the 16-bit precision (the split-fp16 mode runs one frame per call)");
     return VPB_ERR_ARG;
   }
-  if (cfg->stream) e->stream = static_cast<cudaStream_t>(cfg->stream);
-  else { VPB_CUDA_OK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking)); e->own_stream = true; }
   e->d_pre = e->dalloc(static_cast<size_t>(kNetH) * kNetW * 4 * 2 * e->batch * (e->split ? 2 : 1), false);
   if (e->split && e->d_pre) e->d_pre_lo = static_cast<uint8_t*>(e->d_pre) + static_cast<size_t>(kNetH) * kNetW * 4 * 2;
   e->pre.out_lo = e->d_pre_lo;
   e->d_resized = static_cast<uint8_t*>(e->dalloc(static_cast<size_t>(kNetH) * kNetW * 3 * e->batch, false));
   {
-    Tens pre; pre.p = e->d_pre; pre.lo = e->d_pre_lo; pre.H = kNetH; pre.W = kNetW; pre.C = 4;
-    e->taps["pre"] = pre;
+    Tens pre; pre.p = e->d_pre; pre.lo = e->d_pre_lo; pre.H = kNetH; pre.W = kNetW; pre.C = 4; pre.ld = 4;
+    e->tap("pre", pre, 3);                 // RGB of the [320][640][4] network input
   }
   for (int i = 0; i < cfg->n_models; ++i) {
     if (!cfg->weights[i] || !cfg->weights[i][0]) {
@@ -936,7 +684,7 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
       return VPB_ERR_ARG;
     }
     WeightMap w;
-    int rc = load_vpw(cfg->weights[i], w);
+    rc = load_vpw(cfg->weights[i], w);
     if (rc) return rc;
     rc = build_model(*e, i, cfg->kinds[i], w);
     if (e->oom) return VPB_ERR_CUDA;       // message set by the failing allocation
@@ -956,9 +704,8 @@ extern "C" uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes) {
   if (!e) return nullptr;
   DeviceGuard guard(e->gpu_id);
   if (bytes > e->h_frame_cap) {
-    void* p = nullptr;
-    if (cudaMallocHost(&p, bytes) != cudaSuccess) { vpb_set_error("cudaMallocHost(%zu) failed", bytes); return nullptr; }
-    e->host_allocs.push_back(p);
+    void* p = e->halloc(bytes);
+    if (!p) return nullptr;
     e->h_frame = static_cast<uint8_t*>(p); e->h_frame_cap = bytes;
   }
   return e->h_frame;
@@ -997,20 +744,10 @@ extern "C" int vp_engine_sync(vp_engine* e) {
 static int submit_host_frames(vp_engine* e, const uint8_t* const* frames, int n, int h, int w, int stride, bool sync) {
   if (!frames_ok(e, frames, n, h, w, stride, sync ? "vp_engine_infer" : "vp_engine_submit")) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  // The device copy is tightly packed (pitch w*3): only the w*3 valid bytes of every row are read from the
-  // caller's buffer, so a cv::Mat ROI / strided view is never read past its last row's end.
-  const int dpitch = w * 3;
-  const size_t bytes = static_cast<size_t>(h) * dpitch;
-  int rc = ensure_frame_buffers(*e, bytes * n);
+  FrameSrcs dev;
+  int rc = e->upload_frames(frames, n, h, w, stride, dev);
   if (rc) return rc;
-  std::array<const uint8_t*, kMaxBatch> dev{};
-  for (int k = 0; k < n; ++k) {
-    uint8_t* d = e->d_frame + bytes * k;
-    dev[k] = d;
-    if (stride == dpitch) VPB_CUDA_OK(cudaMemcpyAsync(d, frames[k], bytes, cudaMemcpyHostToDevice, e->stream));
-    else VPB_CUDA_OK(cudaMemcpy2DAsync(d, dpitch, frames[k], stride, dpitch, h, cudaMemcpyHostToDevice, e->stream));
-  }
-  rc = enqueue_frame(*e, dev.data(), h, w, dpitch);
+  rc = enqueue_frame(*e, dev.data(), h, w, w * 3);
   if (rc) return rc;
   for (auto& mo : e->outs) {
     if (mo.has_cls)
@@ -1079,7 +816,7 @@ extern "C" int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s) {
 
 extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* flops, const char** names, int* is_gemm, int* n_ops) {
   if (!e || !ms || !n_ops) return VPB_ERR_ARG;
-  if (!e->g_src[0]) { vpb_set_error("vp_engine_profile: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->frame_graph.src[0]) { vpb_set_error("vp_engine_profile: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   const int n = static_cast<int>(e->ops.size()) + 1;
   *n_ops = n;
@@ -1088,7 +825,7 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
   for (auto& x : ev) VPB_CUDA_OK(cudaEventCreate(&x));
   if (e->d_gap) VPB_CUDA_OK(cudaMemsetAsync(e->d_gap, 0, e->gap_used * 8, e->stream));
   VPB_CUDA_OK(cudaEventRecord(ev[0], e->stream));
-  int rc = e->pre.launch(e->g_src.data(), e->batch, e->g_stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
+  int rc = e->pre.launch(e->frame_graph.src.data(), e->batch, e->frame_graph.stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
   if (rc) return rc;
   VPB_CUDA_OK(cudaEventRecord(ev[1], e->stream));
   for (int i = 0; i < n - 1; ++i) {
@@ -1110,7 +847,7 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
 
 extern "C" int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flops, int* launches) {
   if (!e || !ms || reps <= 0) return VPB_ERR_ARG;
-  if (!e->g_src[0]) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->frame_graph.src[0]) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   cudaEvent_t a, b;
   VPB_CUDA_OK(cudaEventCreate(&a));
@@ -1143,20 +880,8 @@ extern "C" int vp_engine_read_resized(vp_engine* e, uint8_t* dst) {
   return VPB_OK;
 }
 
-namespace vpb {
-template <class T> __global__ void tap_to_f32_nchw(const T* in, const T* in_lo, int H, int W, int C, int Cvalid, int pad, float* out) {
-  const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<long>(H) * W * Cvalid) return;
-  const int c = static_cast<int>(i / (static_cast<long>(H) * W));
-  const long pix = i - static_cast<long>(c) * H * W;
-  const long y = pix / W, x = pix - y * W;
-  const long si = ((y + pad) * (W + 2 * pad) + (x + pad)) * C + c;
-  out[i] = static_cast<float>(in[si]) + (in_lo ? static_cast<float>(in_lo[si]) : 0.f);
-}
-}  // namespace vpb
-
 // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
-static bool find_tap(const vp_engine* e, const char* name, Tens* out, std::string* base) {
+static bool find_tap(const vp_engine* e, const char* name, Tap* out) {
   std::string nm(name);
   int k = 0;
   const size_t at = nm.find('@');
@@ -1171,43 +896,22 @@ static bool find_tap(const vp_engine* e, const char* name, Tens* out, std::strin
   auto it = e->taps.find(nm);
   if (it == e->taps.end()) { vpb_set_error("no tap '%s'", name); return false; }
   *out = it->second;
-  out->p = static_cast<uint8_t*>(out->p) + out->bytes() * k;    // split-fp16 engines (lo != NULL) have batch 1
-  *base = nm;
+  out->t.p = static_cast<uint8_t*>(out->t.p) + out->t.bytes() * k;    // split-fp16 engines (lo != NULL) have batch 1
   return true;
 }
 
 extern "C" long vp_engine_read_tap(vp_engine* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {
   if (!e || !name) return VPB_ERR_ARG;
-  Tens a;
-  std::string base;
-  if (!find_tap(e, name, &a, &base)) return VPB_ERR_ARG;
-  const int Cv = base == "pre" ? 3 : a.C;
-  const long n = static_cast<long>(a.H) * a.W * Cv;
-  if (c) *c = Cv; if (h) *h = a.H; if (w) *w = a.W;
-  if (!dst) return n;
-  if (cap < n) { vpb_set_error("tap buffer too small"); return VPB_ERR_ARG; }
-  DeviceGuard guard(e->gpu_id);
-  if (static_cast<size_t>(n) > e->tap_scratch_cap) {       // staging buffer kept by the engine, grown on demand
-    if (e->d_tap_scratch) { cudaFree(e->d_tap_scratch); e->d_tap_scratch = nullptr; e->tap_scratch_cap = 0; }
-    VPB_CUDA_OK(cudaMalloc(&e->d_tap_scratch, static_cast<size_t>(n) * 4));
-    e->tap_scratch_cap = static_cast<size_t>(n);
-  }
-  float* d = e->d_tap_scratch;
-  const int blocks = static_cast<int>((n + 255) / 256);
-  if (e->dtype == VPB_BF16) tap_to_f32_nchw<<<blocks, 256, 0, e->stream>>>(static_cast<const __nv_bfloat16*>(a.p), static_cast<const __nv_bfloat16*>(a.lo), a.H, a.W, a.C, Cv, a.pad, d);
-  else tap_to_f32_nchw<<<blocks, 256, 0, e->stream>>>(static_cast<const __half*>(a.p), static_cast<const __half*>(a.lo), a.H, a.W, a.C, Cv, a.pad, d);
-  cudaError_t ce = cudaMemcpyAsync(dst, d, n * 4, cudaMemcpyDeviceToHost, e->stream);
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
-  if (ce != cudaSuccess) { vpb_set_error("read_tap: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-  return n;
+  Tap a;
+  if (!find_tap(e, name, &a)) return VPB_ERR_ARG;
+  return e->read_tap(a.t, a.channels, dst, cap, c, h, w);
 }
 
 extern "C" int vp_engine_tap_dev(vp_engine* e, const char* name, vp_tap_view* v) {
   if (!e || !name || !v) return VPB_ERR_ARG;
-  Tens a;
-  std::string base;
-  if (!find_tap(e, name, &a, &base)) return VPB_ERR_ARG;
-  v->data = a.p; v->height = a.H; v->width = a.W; v->channels = a.C; v->ld = a.C; v->pad = a.pad;
+  Tap a;
+  if (!find_tap(e, name, &a)) return VPB_ERR_ARG;
+  v->data = a.t.p; v->height = a.t.H; v->width = a.t.W; v->channels = a.t.C; v->ld = a.t.ld; v->pad = a.t.pad;
   v->dtype = e->dtype;
   return VPB_OK;
 }
@@ -1232,7 +936,7 @@ extern "C" int vp_engine_kernel_names(vp_engine* e, const char** names, int cap,
 extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, float* ms, double* flops,
                                      double* bytes, int* launches) {
   if (!e || !kname || !ms || reps <= 0) return VPB_ERR_ARG;
-  if (!e->g_src[0]) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->frame_graph.src[0]) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   const bool is_pre = strcmp(kname, "preprocess") == 0;
   cudaEvent_t a, b;
@@ -1243,10 +947,10 @@ extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, 
   for (int r = -1; r < reps; ++r) {            // r = -1: untimed warm-up pass
     if (r == 0) VPB_CUDA_OK(cudaEventRecord(a, e->stream));
     if (is_pre) {
-      const int rc = e->pre.launch(e->g_src.data(), e->batch, e->g_stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
+      const int rc = e->pre.launch(e->frame_graph.src.data(), e->batch, e->frame_graph.stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
       if (rc) return rc;
       // SURVEY.md 8d: frame read + 3 x 320 x 640 16-bit tensor written, per sample
-      if (r >= 0) { by += e->batch * (3.0 * e->g_h * e->g_w + 2.0 * 3 * kNetH * kNetW); ++n; }
+      if (r >= 0) { by += e->batch * (3.0 * e->frame_graph.h * e->frame_graph.w + 2.0 * 3 * kNetH * kNetW); ++n; }
       continue;
     }
     for (auto& op : e->ops) {

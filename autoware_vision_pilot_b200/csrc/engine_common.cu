@@ -1,0 +1,303 @@
+// engine_common.cu — host runtime shared by the engines (declarations and roles in engine_internal.h).
+#include "common.cuh"
+#include "conv_gemm.cuh"
+#include "engine_internal.h"
+
+#include <cstdio>
+#include <cstring>
+
+namespace vpb {
+
+// =============================================================== weight file (.vpw)
+// magic "VPW1", u32 n; per tensor: u32 name_len, name, u32 dtype (0 f32, 1 i64), u32 ndim,
+// u32 dims[ndim], u64 nbytes, raw little-endian data.  Written by
+// autoware_vision_pilot_b200/weights.py from the reference's .pth state_dict (SURVEY App. C).
+int load_vpw(const char* path, WeightMap& out) {
+  FILE* fp = fopen(path, "rb");
+  if (!fp) { vpb_set_error("cannot open weight file '%s'", path); return VPB_ERR_IO; }
+  auto fail = [&](const char* why) { fclose(fp); vpb_set_error("%s: %s", path, why); return VPB_ERR_IO; };
+  if (fseek(fp, 0, SEEK_END) != 0) return fail("cannot seek");
+  const long file_size = ftell(fp);
+  rewind(fp);
+  char magic[4]; uint32_t n = 0;
+  if (fread(magic, 1, 4, fp) != 4 || memcmp(magic, "VPW1", 4) != 0) return fail("not a VPW1 file");
+  if (fread(&n, 4, 1, fp) != 1 || n > 100000) return fail("bad tensor count");
+  for (uint32_t i = 0; i < n; ++i) {
+    uint32_t nl = 0, dt = 0, nd = 0; uint64_t nb = 0;
+    if (fread(&nl, 4, 1, fp) != 1 || nl > 4096) return fail("bad name length");
+    std::string name(nl, '\0');
+    if (fread(&name[0], 1, nl, fp) != nl) return fail("truncated name");
+    if (fread(&dt, 4, 1, fp) != 1 || fread(&nd, 4, 1, fp) != 1 || nd > 8) return fail("bad header");
+    HostTensor t; t.dims.resize(nd);
+    for (uint32_t d = 0; d < nd; ++d) { uint32_t v; if (fread(&v, 4, 1, fp) != 1) return fail("bad dims"); t.dims[d] = static_cast<int>(v); }
+    if (fread(&nb, 8, 1, fp) != 1) return fail("bad size");
+    size_t ne = 1;
+    bool dims_ok = true;
+    for (int d : t.dims) {                                   // bounded: no overflow, no absurd allocation
+      if (d < 0 || (d > 0 && ne > (static_cast<size_t>(1) << 31) / static_cast<size_t>(d))) { dims_ok = false; break; }
+      ne *= static_cast<size_t>(d);
+    }
+    if (!dims_ok) return fail("tensor dims out of range");
+    if (dt == 0) {
+      if (nb != ne * 4) return fail("f32 size mismatch");
+      t.f.resize(ne);
+      if (ne && fread(t.f.data(), 4, ne, fp) != ne) return fail("truncated data");
+    } else {
+      // num_batches_tracked (int64 scalar): skipped, but the payload must really be there
+      const long here = ftell(fp);
+      if (here < 0 || nb > static_cast<uint64_t>(file_size - here) || fseek(fp, static_cast<long>(nb), SEEK_CUR) != 0)
+        return fail("truncated data");
+    }
+    out[name] = std::move(t);
+  }
+  fclose(fp);
+  return VPB_OK;
+}
+
+const HostTensor* find_w(const WeightMap& w, const std::string& key) {
+  auto it = w.find(key);
+  if (it == w.end()) { vpb_set_error("weight '%s' missing from checkpoint", key.c_str()); return nullptr; }
+  return &it->second;
+}
+
+// Every tensor's shape is checked against what the architecture expects before it is indexed: a checkpoint
+// of another variant, or a truncated / corrupt file, fails with VPB_ERR_IO instead of reading out of bounds.
+const HostTensor* find_w_shaped(const WeightMap& w, const std::string& key, std::initializer_list<int> dims) {
+  const HostTensor* t = find_w(w, key);
+  if (!t) return nullptr;
+  bool ok = t->dims.size() == dims.size() && t->f.size() == t->numel();
+  if (ok) { size_t i = 0; for (int d : dims) { if (d >= 0 && t->dims[i] != d) ok = false; ++i; } }
+  if (!ok) {
+    std::string got, want;
+    for (int d : t->dims) got += std::to_string(d) + ",";
+    for (int d : dims) want += (d < 0 ? std::string("*") : std::to_string(d)) + ",";
+    vpb_set_error("weight '%s' has shape [%s] but this architecture needs [%s]", key.c_str(), got.c_str(), want.c_str());
+    return nullptr;
+  }
+  return t;
+}
+
+std::vector<float> pack_conv(const HostTensor& t, const std::vector<float>* scale) {
+  const int Cout = t.dims[0], Cin = t.dims[1], k = t.dims[2];
+  std::vector<float> o(t.f.size());
+  for (int co = 0; co < Cout; ++co)
+    for (int ci = 0; ci < Cin; ++ci)
+      for (int tt = 0; tt < k * k; ++tt)
+        o[(static_cast<size_t>(tt) * Cout + co) * Cin + ci] =
+            t.f[(static_cast<size_t>(co) * Cin + ci) * k * k + tt] * (scale ? (*scale)[co] : 1.0f);
+  return o;
+}
+
+// =============================================================== frame graph
+int FrameGraph::run(cudaStream_t st, const PreprocessPlan& pre, int dtype, int h_, int w_, int stride_,
+                    const FrameSrcs& src_, const std::function<int(cudaStream_t)>& launch,
+                    const std::function<int(cudaGraphExec_t, cudaGraphNode_t)>& repoint) {
+  const bool same_geometry = exec && h == h_ && w == w_ && stride == stride_;
+  if (same_geometry && src != src_ && pre_node) {
+    const int rc = repoint(exec, pre_node);
+    if (rc) return rc;
+    src = src_;
+  }
+  if (!same_geometry || src != src_) {
+    invalidate();
+    pre_node = nullptr;
+    int rc = launch(st);
+    if (rc) return rc;
+    VPB_CUDA_OK(cudaStreamSynchronize(st));
+    cudaGraph_t g = nullptr;
+    VPB_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    rc = launch(st);
+    cudaError_t ce = cudaStreamEndCapture(st, &g);
+    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+    if (ce != cudaSuccess) { vpb_set_error("graph capture failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
+    size_t nn = 0;
+    cudaGraphGetNodes(g, nullptr, &nn);
+    std::vector<cudaGraphNode_t> nodes(nn);
+    cudaGraphGetNodes(g, nodes.data(), &nn);
+    for (size_t i = 0; i < nn; ++i) {
+      cudaGraphNodeType ty;
+      if (cudaGraphNodeGetType(nodes[i], &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
+      cudaKernelNodeParams kp{};
+      if (cudaGraphKernelNodeGetParams(nodes[i], &kp) == cudaSuccess && pre.owns_kernel(kp.func, dtype)) {
+        pre_node = nodes[i];
+        break;
+      }
+    }
+    ce = cudaGraphInstantiate(&exec, g, 0);
+    if (graph) cudaGraphDestroy(graph);
+    graph = g;
+    if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
+    h = h_; w = w_; stride = stride_; src = src_;
+  }
+  VPB_CUDA_OK(cudaGraphLaunch(exec, st));
+  return VPB_OK;
+}
+
+void FrameGraph::invalidate() {
+  if (exec) { cudaGraphExecDestroy(exec); exec = nullptr; }
+}
+
+void FrameGraph::release() {
+  invalidate();
+  if (graph) { cudaGraphDestroy(graph); graph = nullptr; }
+}
+
+// =============================================================== engine runtime
+EngineRuntime::~EngineRuntime() {
+  DeviceGuard guard(gpu_id);
+  frame_graph.release();
+  if (d_tap_scratch) cudaFree(d_tap_scratch);
+  for (void* p : dev_allocs) cudaFree(p);
+  for (void* p : host_allocs) cudaFreeHost(p);
+  if (own_stream && stream) cudaStreamDestroy(stream);
+}
+
+int EngineRuntime::open(const char* who, int gpu, void* user_stream) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
+    vpb_set_error("%s: no CUDA device (this engine has no CPU fallback)", who);
+    return VPB_ERR_CUDA;
+  }
+  if (gpu < 0 || gpu >= ndev) {
+    vpb_set_error("%s: gpu_id %d out of range (%d devices)", who, gpu, ndev);
+    return VPB_ERR_ARG;
+  }
+  DeviceGuard guard(gpu);
+  cudaDeviceProp prop;
+  VPB_CUDA_OK(cudaGetDeviceProperties(&prop, gpu));
+  if (prop.major != 9 || prop.minor != 0) {
+    vpb_set_error("%s: device %d is sm_%d%d; this library is built for sm_90a only", who, gpu, prop.major, prop.minor);
+    return VPB_ERR_CUDA;
+  }
+  gpu_id = gpu;
+  if (user_stream) stream = static_cast<cudaStream_t>(user_stream);
+  else { VPB_CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking)); own_stream = true; }
+  return VPB_OK;
+}
+
+void* EngineRuntime::dalloc(size_t bytes, bool is_weight) {
+  void* p = nullptr;
+  const cudaError_t ce = cudaMalloc(&p, std::max<size_t>(bytes, 256));
+  if (ce != cudaSuccess || !p) {
+    // sticky: the create call reports it (uploads skip NULL, nothing is launched during construction)
+    if (!oom) vpb_set_error("cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(ce));
+    oom = true;
+    cudaGetLastError();
+    return nullptr;
+  }
+  cudaMemset(p, 0, std::max<size_t>(bytes, 256));
+  dev_allocs.push_back(p);
+  (is_weight ? weight_bytes : act_bytes) += bytes;
+  return p;
+}
+
+void* EngineRuntime::halloc(size_t bytes) {
+  void* p = nullptr;
+  const cudaError_t ce = cudaMallocHost(&p, std::max<size_t>(bytes, 64));
+  if (ce != cudaSuccess) {
+    vpb_set_error("pinned host allocation of %zu bytes failed: %s", bytes, cudaGetErrorString(ce));
+    cudaGetLastError();
+    return nullptr;
+  }
+  host_allocs.push_back(p);
+  return p;
+}
+
+float* EngineRuntime::upload_f32(const std::vector<float>& v) {
+  float* p = static_cast<float*>(dalloc(v.size() * 4, true));
+  if (p) cudaMemcpy(p, v.data(), v.size() * 4, cudaMemcpyHostToDevice);
+  return p;
+}
+
+void* EngineRuntime::upload_16(const std::vector<float>& v) {
+  const size_t n = v.size();
+  std::vector<uint16_t> h(split ? 2 * n : n);
+  for (size_t i = 0; i < n; ++i) {
+    if (dtype == VPB_BF16) {
+      __nv_bfloat16 b = __float2bfloat16_rn(v[i]); memcpy(&h[i], &b, 2);
+      if (split) { __nv_bfloat16 l = __float2bfloat16_rn(v[i] - __bfloat162float(b)); memcpy(&h[n + i], &l, 2); }
+    } else {
+      __half b = __float2half_rn(v[i]); memcpy(&h[i], &b, 2);
+      if (split) { __half l = __float2half_rn(v[i] - __half2float(b)); memcpy(&h[n + i], &l, 2); }
+    }
+  }
+  void* p = dalloc(h.size() * 2, true);
+  if (p) {
+    cudaMemcpy(p, h.data(), h.size() * 2, cudaMemcpyHostToDevice);
+    if (split) lo_of[p] = static_cast<uint8_t*>(p) + n * 2;
+  }
+  return p;
+}
+
+int EngineRuntime::append_conv(const std::string& name, const vpb_conv_args& a, int lane) {
+  auto plan = std::make_unique<ConvPlan>();
+  const int rc = conv_plan_build(&a, plan.get());
+  if (rc != VPB_OK) { const std::string e = vpb_last_error(); vpb_set_error("%s: %s", name.c_str(), e.c_str()); return rc; }
+  ConvPlan* pp = plan.get();
+  plans.push_back(std::move(plan));
+  OpRec op; op.name = name; op.flops = pp->flops; op.gemm = true; op.lane = lane;
+  op.kind = a.algo == VPB_ALGO_LINEAR ? 2 : 1;
+  op.kname = "conv_wgmma_kernel";
+  op.launch = [pp](cudaStream_t s) { return conv_plan_launch(pp, s); };
+  ops.push_back(std::move(op));
+  return VPB_OK;
+}
+
+int EngineRuntime::upload_frames(const uint8_t* const* frames, int n, int h, int w, int stride, FrameSrcs& dev) {
+  const int dpitch = w * 3;
+  const size_t bytes = static_cast<size_t>(h) * dpitch;
+  if (bytes * n > d_frame_cap) {
+    frame_graph.invalidate();
+    void* p = nullptr;
+    VPB_CUDA_OK(cudaMalloc(&p, bytes * n + 256));
+    dev_allocs.push_back(p);
+    d_frame = static_cast<uint8_t*>(p); d_frame_cap = bytes * n;
+  }
+  dev = {};
+  for (int k = 0; k < n; ++k) {
+    uint8_t* d = d_frame + bytes * k;
+    dev[k] = d;
+    if (stride == dpitch) VPB_CUDA_OK(cudaMemcpyAsync(d, frames[k], bytes, cudaMemcpyHostToDevice, stream));
+    else VPB_CUDA_OK(cudaMemcpy2DAsync(d, dpitch, frames[k], stride, dpitch, h, cudaMemcpyHostToDevice, stream));
+  }
+  return VPB_OK;
+}
+
+// [C][H][W] fp32 from the first C channels of a view with channel stride ld and border pad (+ the split-fp16 low half)
+template <class T>
+__global__ void tap_to_f32_nchw(const T* in, const T* in_lo, int H, int W, int C, int ld, int pad, float* out) {
+  const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long>(H) * W * C) return;
+  const int c = static_cast<int>(i / (static_cast<long>(H) * W));
+  const long pix = i - static_cast<long>(c) * H * W;
+  const long y = pix / W, x = pix - y * W;
+  const long si = ((y + pad) * (W + 2 * pad) + (x + pad)) * ld + c;
+  const float v = static_cast<float>(in[si]);
+  out[i] = in_lo ? v + static_cast<float>(in_lo[si]) : v;
+}
+
+long EngineRuntime::read_tap(const Tens& t, int channels, float* dst, long cap, int* c, int* h, int* w) {
+  const long n = static_cast<long>(t.H) * t.W * channels;
+  if (c) *c = channels; if (h) *h = t.H; if (w) *w = t.W;
+  if (!dst) return n;
+  if (cap < n) { vpb_set_error("tap buffer too small"); return VPB_ERR_ARG; }
+  DeviceGuard guard(gpu_id);
+  if (static_cast<size_t>(n) > tap_scratch_cap) {
+    if (d_tap_scratch) { cudaFree(d_tap_scratch); d_tap_scratch = nullptr; tap_scratch_cap = 0; }
+    VPB_CUDA_OK(cudaMalloc(&d_tap_scratch, static_cast<size_t>(n) * 4));
+    tap_scratch_cap = static_cast<size_t>(n);
+  }
+  const int blocks = static_cast<int>((n + 255) / 256);
+  if (dtype == VPB_BF16)
+    tap_to_f32_nchw<<<blocks, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(t.p), static_cast<const __nv_bfloat16*>(t.lo),
+                                               t.H, t.W, channels, t.ld, t.pad, d_tap_scratch);
+  else
+    tap_to_f32_nchw<<<blocks, 256, 0, stream>>>(static_cast<const __half*>(t.p), static_cast<const __half*>(t.lo),
+                                               t.H, t.W, channels, t.ld, t.pad, d_tap_scratch);
+  cudaError_t ce = cudaMemcpyAsync(dst, d_tap_scratch, n * 4, cudaMemcpyDeviceToHost, stream);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream);
+  if (ce != cudaSuccess) { vpb_set_error("read_tap: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
+  return n;
+}
+
+}  // namespace vpb

@@ -1,12 +1,18 @@
-// engine_internal.h — host-side pieces shared by the engines (engine.cu: the four segmentation / depth / lane
-// networks; autospeed.cu: the AutoSpeed detector): the .vpw weight-file reader, shape-checked lookups, K-major
-// repacking, the device guard.
+// engine_internal.h — host-side runtime shared by the engines (engine.cu: the four segmentation / depth / lane
+// networks; autospeed.cu: the AutoSpeed detector), defined in engine_common.cu: the .vpw weight-file reader,
+// shape-checked lookups, K-major repacking, the device guard, and EngineRuntime (device and stream set-up, device /
+// pinned allocations, weight uploads, the op list, the frame graph, host frame upload, tap read-back).
 #pragma once
 #include <cuda_runtime.h>
+#include <array>
+#include <functional>
 #include <initializer_list>
 #include <map>
+#include <memory>
 #include <string>
+#include <unordered_map>
 #include <vector>
+#include "ops_internal.h"
 
 namespace vpb {
 
@@ -30,6 +36,99 @@ struct DeviceGuard {
   int prev = -1; bool changed = false;
   explicit DeviceGuard(int d) { if (cudaGetDevice(&prev) == cudaSuccess && prev != d) changed = cudaSetDevice(d) == cudaSuccess; }
   ~DeviceGuard() { if (changed) cudaSetDevice(prev); }
+};
+
+// NHWC 16-bit activation view.  p points at the first channel of the view; ld = channel stride of a pixel;
+// pad = 1: zero-bordered [(H+2)*(W+2)][ld]; lo: split-fp16 low half (same layout), NULL otherwise.
+struct Tens {
+  void* p = nullptr; void* lo = nullptr;
+  int H = 0, W = 0, C = 0, ld = 0, pad = 0;
+  size_t bytes() const { return static_cast<size_t>(H + 2 * pad) * (W + 2 * pad) * ld * 2; }
+  Tens slice(int c0, int c) const {
+    Tens t = *this;
+    t.p = static_cast<uint8_t*>(p) + static_cast<size_t>(c0) * 2;
+    if (lo) t.lo = static_cast<uint8_t*>(lo) + static_cast<size_t>(c0) * 2;
+    t.C = c;
+    return t;
+  }
+};
+
+// A named intermediate tensor readable as fp32: the leading `channels` channels of t are reported (the rest is padding).
+struct Tap { Tens t; int channels = 0; };
+
+struct OpRec {
+  std::string name;
+  std::function<int(cudaStream_t)> launch;
+  double flops = 0;     // 2*MAC this launch executes
+  double flops_ref = -1; // 2*MAC of the reference's layers this op stands for (< 0: same as flops)
+  double bytes = 0;     // algorithmic HBM bytes per launch (HBM-bound stages; SURVEY.md 8d definitions)
+  std::string kname;    // kernel the op launches (roofline report groups launches by kernel)
+  bool gemm = false;
+  int kind = 0;   // 0 = not a convolution GEMM; conv_wgmma_kernel with 1 = VPB_ALGO_TILE, 2 = VPB_ALGO_LINEAR
+  int lane = 0;   // execution lane (= index of the model that owns the op); lanes run concurrently
+};
+
+using FrameSrcs = std::array<const uint8_t*, kMaxBatch>;
+
+// The CUDA graph of one call, keyed on (h, w, stride, frame pointers).  A frame of the captured geometry in another
+// buffer only re-points the captured pre-process node.
+struct FrameGraph {
+  cudaGraph_t graph = nullptr;           // kept alive: pre_node is a handle into it
+  cudaGraphExec_t exec = nullptr;
+  cudaGraphNode_t pre_node = nullptr;    // the captured pre-process kernel node (re-pointed per frame)
+  int h = 0, w = 0, stride = 0;
+  FrameSrcs src{};                       // frames of the captured / last call ([0] == NULL: none yet)
+
+  // Launch the graph for frames src_ on st.  When the key differs in more than the frame pointers: launch(st) once
+  // outside capture (sets function attributes; its results are correct), capture launch(st), find the node of `pre`
+  // and instantiate.  When only the pointers differ: repoint(exec, pre_node).
+  int run(cudaStream_t st, const PreprocessPlan& pre, int dtype, int h_, int w_, int stride_, const FrameSrcs& src_,
+          const std::function<int(cudaStream_t)>& launch,
+          const std::function<int(cudaGraphExec_t, cudaGraphNode_t)>& repoint);
+  void invalidate();                     // the next run() captures again
+  void release();
+};
+
+struct ConvPlan;
+
+// What every engine owns: its device and stream, device / pinned allocations, the op list and the frame graph.
+struct EngineRuntime {
+  int gpu_id = 0, dtype = VPB_F16;
+  cudaStream_t stream = nullptr; bool own_stream = false;
+  bool oom = false;                       // a device allocation failed during construction (the create call reports it)
+  bool split = false;                     // VP_PREC_SPLIT: every 16-bit tensor is a (hi, lo) pair, GEMMs run 3 K segments
+  std::unordered_map<const void*, void*> lo_of;   // 16-bit weight buffer -> its low half (split mode)
+  std::vector<void*> dev_allocs, host_allocs;
+  size_t weight_bytes = 0, act_bytes = 0;
+  std::vector<std::unique_ptr<ConvPlan>> plans;
+  std::vector<OpRec> ops;                 // network ops (after the pre-process)
+  std::map<std::string, Tap> taps;
+  FrameGraph frame_graph;
+  uint8_t* d_frame = nullptr; size_t d_frame_cap = 0;           // device copy of the host frames
+  float* d_tap_scratch = nullptr; size_t tap_scratch_cap = 0;   // read_tap staging (grown on demand)
+
+  EngineRuntime() = default;
+  EngineRuntime(const EngineRuntime&) = delete;
+  EngineRuntime& operator=(const EngineRuntime&) = delete;
+  ~EngineRuntime();
+
+  // Device gpu exists and is an sm_90 part; then borrow user_stream or create a non-blocking stream.  Errors name `who`.
+  int open(const char* who, int gpu, void* user_stream);
+  // zeroed device memory (legacy-stream memset: construction time only, followed by a device synchronise); NULL and
+  // the sticky oom flag on failure
+  void* dalloc(size_t bytes, bool is_weight = false);
+  void* halloc(size_t bytes);             // pinned host memory; NULL (error set) on failure
+  float* upload_f32(const std::vector<float>& v);
+  void* upload_16(const std::vector<float>& v);   // split mode: [hi | lo], lo = round16(v - hi)
+  void* lo(const void* hi) const { auto it = lo_of.find(hi); return it == lo_of.end() ? nullptr : it->second; }
+  // build the plan of one wgmma convolution, keep it, append its launch (errors are prefixed with name)
+  int append_conv(const std::string& name, const vpb_conv_args& a, int lane = 0);
+  void tap(const std::string& name, const Tens& t, int channels = 0) { taps[name] = Tap{t, channels > 0 ? channels : t.C}; }
+  // Copy n host frames of one geometry to d_frame (grown on demand), packed with pitch w*3: only the w*3 valid bytes
+  // of every row are read from the caller's buffer, so a cv::Mat ROI / strided view is never read past its last row.
+  int upload_frames(const uint8_t* const* frames, int n, int h, int w, int stride, FrameSrcs& dev);
+  // the first `channels` channels of t as fp32 [channels][H][W] into dst (NULL: size query); element count or < 0
+  long read_tap(const Tens& t, int channels, float* dst, long cap, int* c, int* h, int* w);
 };
 
 }  // namespace vpb

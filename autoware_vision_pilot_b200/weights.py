@@ -1,5 +1,5 @@
 """Checkpoint conversion: the reference's `.pth` state_dict -> `.vpw` (the flat file the C++ engine
-reads; csrc/engine.cu load_vpw).
+reads; csrc/engine_common.cu load_vpw).
 
 The reference loads `torch.load(path, weights_only=True)` into the nn.Module
 (Models/inference/scene_seg_infer.py:30-31); its C++ side never reads a .pth either — it consumes a

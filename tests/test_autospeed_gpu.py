@@ -105,6 +105,29 @@ def test_drop_in_helper_and_other_frame_sizes(ckpt, tmp_path):
     assert out2 == out
 
 
+def test_infer_device_repoints_the_frame_graph(ckpt):
+    """infer_device on device buffers A, B, A (one geometry: the captured letterbox node is re-pointed), C (another
+    geometry: captured again), then A: raw predictions and detections equal infer() on the same host frame bit for bit."""
+    _, vpw = ckpt
+    eng = AS.AutoSpeedEngine(vpw)
+    frames = {"A": synth.synth_frame(0), "B": synth.synth_frame(1),
+              "C": np.ascontiguousarray(synth.synth_frame(2)[:400, :1600])}
+    assert frames["A"].shape == frames["B"].shape != frames["C"].shape
+    ref = {}
+    for k, f in frames.items():
+        det = eng.infer(f, fetch_raw=True)
+        ref[k] = (eng.raw(), det)
+    dev = {k: torch.from_numpy(f).cuda() for k, f in frames.items()}
+    torch.cuda.synchronize()
+    for k in ("A", "B", "A", "C", "A"):
+        t = dev[k]
+        eng.infer_device(t.data_ptr(), t.shape[0], t.shape[1], t.stride(0))
+        eng.sync(2)
+        raw, det = ref[k]
+        assert np.array_equal(eng.raw().view(np.uint32), raw.view(np.uint32)), k
+        assert np.array_equal(eng.detections().view(np.uint32), det.view(np.uint32)), k
+
+
 def test_conv_stride2_and_weight_stride_ops():
     """The two conv features AutoSpeed adds, in isolation against torch: stride-2 3x3 through the tensor map's
     traversal stride, and a 1x1 conv whose weight operand is a strided activation slice (attention's Q K^T)."""

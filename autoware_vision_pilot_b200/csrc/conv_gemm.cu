@@ -25,12 +25,15 @@
 //
 // Operands land in shared memory in the 128-byte-swizzled K-major layout wgmma reads through descriptors,
 // through a ring of `stages` TMA stages guarded by mbarriers.  Persistent grid, warp-specialised:
-//   warps 0..7   two consumer warpgroups: warpgroup g issues m64nBNk16 wgmma for accumulator rows
-//                64g..64g+63 (fp32 in registers), then the accumulator is staged in shared memory
-//                (row-major fp32) and all 256 threads run the epilogue on it, two threads per row:
+//   warps 0..7   two MMA warpgroups: warpgroup g issues m64nBNk16 wgmma for accumulator rows 64g..64g+63
+//                (fp32 in registers), then stages the accumulator in shared memory (row-major fp32) and
+//                goes straight on to the next tile's K loop.
+//   warps 8..11  the epilogue warpgroup runs the epilogue on the staged accumulator, one thread per row:
 //                +bias -> activation -> residual -> 16-bit NHWC stores (or fp32 planar logits + class
-//                map for the heads' last conv).
-//   warp 8       TMA producer (one elected lane); it runs ahead into the next tile during the epilogue.
+//                map for the heads' last conv), while the tensor cores work on the next tile.
+//   warp 12      TMA producer (one elected lane); it runs up to `stages` K chunks ahead of the MMAs.
+// The staging buffer is handed between the two roles through the acc_full / acc_empty mbarriers, so the
+// MMA warps of tile t+1 wait only if the epilogue of tile t is still reading it when they finish.
 #include "common.cuh"
 #include "conv_gemm.cuh"
 #include "ops_internal.h"
@@ -40,9 +43,12 @@
 
 namespace vpb {
 
-static constexpr int kConsumers = 256;                // two consumer warpgroups
-static constexpr int kThreads = kConsumers + 32;      // + the TMA producer warp
-static constexpr int kParts = kConsumers / 128;       // epilogue threads per accumulator row
+static constexpr int kMma = 256;                     // two MMA warpgroups
+// one epilogue warpgroup: with two (kParts = 2) the 544-thread launch caps the kernel at 96 registers and it measured
+// no faster on the H100
+static constexpr int kEpilogue = 128;
+static constexpr int kThreads = kMma + kEpilogue + 32;   // + the TMA producer warp
+static constexpr int kParts = kEpilogue / 128;        // epilogue threads per accumulator row
 static constexpr int kMaxStages = 8;
 static constexpr int kATileBytes = 128 * 128;  // 128 pixels x 64 ch x 2 B
 // 227 KB opt-in limit covers static + dynamic shared memory; keep 4 KB for the static part.
@@ -320,7 +326,9 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[kMaxStages];
   __shared__ __align__(8) uint64_t bar_empty[kMaxStages];
-  __shared__ __align__(16) float s_bias[BN];
+  __shared__ __align__(8) uint64_t acc_full;      // the MMA warps have staged a tile's accumulator
+  __shared__ __align__(8) uint64_t acc_empty;     // the epilogue warps are done reading it
+  __shared__ __align__(16) float s_bias[BN];      // epilogue warps only
 
   constexpr uint32_t kBTileBytes = static_cast<uint32_t>(BN) * 128u;
   constexpr uint32_t kStageBytes = kATileBytes + kBTileBytes;      // a multiple of 1024 (swizzle atoms stay aligned)
@@ -330,15 +338,17 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t acc_base = smem_base + static_cast<uint32_t>(p.stages) * kStageBytes;
 
-  if (threadIdx.x == kConsumers) {
+  if (threadIdx.x == kMma + kEpilogue) {
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
     if (p.kchunks2) { tma_prefetch_desc(&mapA2); tma_prefetch_desc(&mapB2); }
     if (p.split) { tma_prefetch_desc(&maps.Alo); tma_prefetch_desc(&maps.Blo); }
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), kConsumers / 32);     // one arrival per consumer warp
+      mbar_init(smem_u32(&bar_empty[s]), kMma / 32);     // one arrival per MMA warp
     }
+    mbar_init(smem_u32(&acc_full), kMma);               // one arrival per thread: each stages its own registers
+    mbar_init(smem_u32(&acc_empty), kEpilogue);
     fence_mbar_init();
   }
   __syncthreads();
@@ -350,7 +360,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
   const int kiters_all = p.upc ? 4 * p.kchunks + 9 * p.kchunks2 : (p.taps * p.kchunks + p.kchunks2) * nseg;
   const int tiles_per_phase = p.tiles_n * p.tiles_h * p.tiles_w;
 
-  if (warp == kConsumers / 32) {
+  if (warp == (kMma + kEpilogue) / 32) {
     // ------------------------------------------------------------ TMA producer (converged warp, elected lane)
     int stage = 0;
     uint32_t phase = 0;
@@ -446,19 +456,13 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
         }
       }
     }
-  } else {
-    // ------------------------------------------------------------ consumers: wgmma main loop, then the epilogue
+  } else if (warp < kMma / 32) {
+    // ------------------------------------------------------------ MMA warpgroups: wgmma main loop, then stage the accumulator
     const int wg = warp >> 2;                 // accumulator rows 64*wg .. 64*wg + 63
-    const int row = threadIdx.x & 127;        // epilogue: accumulator row == pixel within the tile
-    const int part = threadIdx.x >> 7;
-    const int lh = row >> p.tw_shift;
-    const int lw = row & (p.TW - 1);
-    const int Wo = (p.phases > 1) ? 2 * p.W : p.W;
     float* acc_s = reinterpret_cast<float*>(smem_raw + (acc_base - smem_u32(smem_raw)));
-    const uint32_t t_row = (acc_base >> 2) + static_cast<uint32_t>(row * kPitch);
     float acc[BN / 2];
     int stage = 0, prev = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, acc_phase = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       for (int k = 0; k < kiters_all; ++k) {
         mbar_wait_quiet(smem_u32(&bar_full[stage]), phase);
@@ -478,6 +482,30 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(smem_u32(&bar_empty[prev]));
 
+      mbar_wait_quiet(smem_u32(&acc_empty), acc_phase ^ 1u);   // the previous tile's epilogue is done with the staging buffer
+      {
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        float* a0 = acc_s + r0 * kPitch + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(a0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(a0 + 8 * kPitch + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      mbar_arrive(smem_u32(&acc_full));
+      acc_phase ^= 1u;
+    }
+  } else {
+    // ------------------------------------------------------------ epilogue warps: one tile behind the MMA warps
+    const int et = threadIdx.x - kMma;
+    const int row = et & 127;                 // accumulator row == pixel within the tile
+    const int part = et >> 7;
+    const int lh = row >> p.tw_shift;
+    const int lw = row & (p.TW - 1);
+    const int Wo = (p.phases > 1) ? 2 * p.W : p.W;
+    const uint32_t t_row = (acc_base >> 2) + static_cast<uint32_t>(row * kPitch);
+    uint32_t acc_phase = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const int img = static_cast<int>(fast_div(tile, p.mg_ti));
       const int ti = tile - img * p.tiles_img;
       const int ph = static_cast<int>(fast_div(ti, p.mg_tpp));
@@ -488,22 +516,14 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
       const int twi = rn - thi * p.tiles_w;
       const int h = thi * p.TH + lh, w = twi * p.TW + lw, n0 = nt * p.BN;
 
-      named_bar_sync(1, kConsumers);        // the previous tile's epilogue is done with the staged accumulator and bias
-      {
-        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-        float* a0 = acc_s + r0 * kPitch + 2 * (lane & 3);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          *reinterpret_cast<float2*>(a0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(a0 + 8 * kPitch + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-      }
-      if (threadIdx.x < BN) {
-        const int nn = n0 + threadIdx.x;
+      named_bar_sync(1, kEpilogue);         // the previous tile's epilogue is done with the bias row
+      if (et < BN) {
+        const int nn = n0 + et;
         // upconv: the interior bias row (class 4); border pixels read theirs from global memory
-        s_bias[threadIdx.x] = (p.bias && nn < p.Cout) ? __ldg(p.bias + (p.upc ? 4 * p.Cout : 0) + nn) : 0.f;
+        s_bias[et] = (p.bias && nn < p.Cout) ? __ldg(p.bias + (p.upc ? 4 * p.Cout : 0) + nn) : 0.f;
       }
-      named_bar_sync(1, kConsumers);
+      named_bar_sync(1, kEpilogue);
+      mbar_wait_quiet(smem_u32(&acc_full), acc_phase);
 
       if (p.upc) {
         const int pa = ph >> 1, pb = ph & 1;
@@ -520,18 +540,20 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
         px.roff = 0; px.fpix = 0; px.img = 0;
         if (p.act == ACT_GELU) epilogue_store_fast<E, ACT_GELU, false, true>(p, t_row, n0, s_bias, part, px, gb);
         else epilogue_store_fast<E, ACT_NONE, false, true>(p, t_row, n0, s_bias, part, px, gb);
-        continue;
+      } else {
+        const int oh = (p.phases > 1) ? 2 * h + (ph >> 1) : h;
+        const int ow = (p.phases > 1) ? 2 * w + (ph & 1) : w;
+        EpiPix px;
+        px.ok = (h < p.H) && (w < p.W);
+        px.zero = false;
+        px.ooff = img * p.out_img + static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
+        px.roff = img * p.res_img + static_cast<uint32_t>((oh + p.res_pad) * (Wo + 2 * p.res_pad) + (ow + p.res_pad)) * p.ldr;
+        px.fpix = static_cast<uint32_t>(h * p.W + w);
+        px.img = static_cast<uint32_t>(img);
+        epilogue_tile<E>(p, t_row, n0, s_bias, part, px);
       }
-      const int oh = (p.phases > 1) ? 2 * h + (ph >> 1) : h;
-      const int ow = (p.phases > 1) ? 2 * w + (ph & 1) : w;
-      EpiPix px;
-      px.ok = (h < p.H) && (w < p.W);
-      px.zero = false;
-      px.ooff = img * p.out_img + static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
-      px.roff = img * p.res_img + static_cast<uint32_t>((oh + p.res_pad) * (Wo + 2 * p.res_pad) + (ow + p.res_pad)) * p.ldr;
-      px.fpix = static_cast<uint32_t>(h * p.W + w);
-      px.img = static_cast<uint32_t>(img);
-      epilogue_tile<E>(p, t_row, n0, s_bias, part, px);
+      mbar_arrive(smem_u32(&acc_empty));     // this thread's reads of the staged accumulator are done
+      acc_phase ^= 1u;
     }
   }
 }

@@ -408,7 +408,7 @@ struct ASBuilder {
     float *dwt = e.upload_f32(wt), *db = e.upload_f32(bias);
     const int dt = e.dtype, H = in.H, W = in.W, C = in.C;
     const void* ip = in.p; void* op_ = out.p; long long* gap = e.d_gap_scratch;
-    e.op(p, [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? 1 : 0); },
+    e.op(p, [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? VPB_ACT_SILU : VPB_ACT_NONE); },
          2.0 * H * W * C * 9);
   }
   // CTX (common_layers.py:194-239): x [h][w][C] -> out [h][w][Cout]

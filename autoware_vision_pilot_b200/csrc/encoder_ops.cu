@@ -5,7 +5,7 @@
 // Models/model_components/scene_context.py:25-57, backbone_feature_fusion.py:13-38.
 // The dense 1x1 convolutions of the encoder run on the wgmma GEMM (conv_gemm.cu); what is here
 // is byte-moving SIMT work: stem conv (3 input channels), depthwise convs with the
-// squeeze-excitation average pool fused in, the SE gate (folded into the projection weights),
+// squeeze-excitation average pool fused in, the SE gate (applied in place to the depthwise output),
 // global average pool, the context MLP (GEMV), the 1->128 conv on the 10x20 map and the max-pool
 // feature fusion.  All kernels read/write NHWC 16-bit with 16-byte vectors, accumulate in fp32.
 #include "common.cuh"
@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(128) stem_conv_kernel(const uint2* __restrict_
 // ------------------------------------------------------------------ depthwise + SiLU + SE pool
 // Register-tiled along x: one thread owns 8 channels of kXT consecutive output pixels, slides the
 // K-wide input window through registers (each activation vector is loaded once per kernel row and
-// each weight vector once per kXT outputs) and does the MACs with packed FFMA2.
+// each weight vector once per kXT outputs) and does the MACs as scalar fmaf on channel pairs (ffma2).
 static constexpr int kXT = 4;
 
 DwGeom dw_geometry(int H, int W, int C, int k, int stride) {
@@ -521,8 +521,18 @@ using namespace vpb;
   } while (0)
 
 // `*_lo` arguments of the *_x launchers: the low halves of split-fp16 tensors (NULL = plain 16-bit mode).
+// The kernels offset only the hi tensors by the image index, so split-fp16 tensors cannot be batched.
+static int check_batch(const char* op, int batch, bool split) {
+  if (batch < 1 || batch > kMaxBatch) { vpb_set_error("%s: batch %d (1..%d)", op, batch, kMaxBatch); return VPB_ERR_ARG; }
+  if (batch > 1 && split) { vpb_set_error("%s: split-fp16 tensors cannot be batched (batch %d)", op, batch); return VPB_ERR_ARG; }
+  return VPB_OK;
+}
+
 int vpb::stem_conv_x(int dtype, const void* in, const void* in_lo, int H, int W, const float* w, const float* bias,
                      void* out, void* out_lo, cudaStream_t st, int batch) {
+  if (const int rc = check_batch("stem", batch, in_lo || out_lo)) return rc;
+  // Ho = H/2 is the 3x3 s2 p1 output size only for even H (PyTorch gives ceil(H/2)); the network input is always even
+  if (H < 2 || W < 2 || (H & 1) || (W & 1)) { vpb_set_error("stem: H=%d W=%d must be even and >= 2", H, W); return VPB_ERR_ARG; }
   const int Ho = H / 2, Wo = W / 2;
   const int n = Ho * Wo;
   const dim3 g((n + 127) / 128, batch), b(128);
@@ -536,19 +546,32 @@ extern "C" int vpb_stem_conv(int dtype, const void* in, int H, int W, const floa
                              const float* bias, void* out, void* stream) {
   return vpb::stem_conv_x(dtype, in, nullptr, H, W, w, bias, out, nullptr, static_cast<cudaStream_t>(stream));
 }
+extern "C" int vpb_stem_conv_ex(int dtype, const void* in, const void* in_lo, int H, int W, const float* w,
+                                const float* bias, void* out, void* out_lo, int batch, void* stream) {
+  return vpb::stem_conv_x(dtype, in, in_lo, H, W, w, bias, out, out_lo, static_cast<cudaStream_t>(stream), batch);
+}
 
 extern "C" int vpb_depthwise(int dtype, const void* in, int H, int W, int C, int k, int stride,
                              const float* w, const float* bias, void* out, long long* gap_acc,
                              void* stream) {
   return vpb::depthwise_x(dtype, in, nullptr, H, W, C, k, stride, w, bias, out, nullptr, gap_acc, static_cast<cudaStream_t>(stream));
 }
+extern "C" int vpb_depthwise_ex(int dtype, const void* in, const void* in_lo, int H, int W, int C, int k, int stride,
+                                const float* w, const float* bias, void* out, void* out_lo, long long* gap_acc, int act,
+                                int batch, void* stream) {
+  return vpb::depthwise_x(dtype, in, in_lo, H, W, C, k, stride, w, bias, out, out_lo, gap_acc,
+                          static_cast<cudaStream_t>(stream), act, batch);
+}
 int vpb::depthwise_x(int dtype, const void* in, const void* in_lo, int H, int W, int C, int k, int stride,
                      const float* w, const float* bias, void* out, void* out_lo, long long* gap_acc,
                      cudaStream_t st, int act, int batch) {
-  if ((C & 7) || (k != 3 && k != 5) || (stride != 1 && stride != 2) || C > 2048) {
+  if (C < 8 || (C & 7) || (k != 3 && k != 5) || (stride != 1 && stride != 2) || C > 2048) {
     vpb_set_error("depthwise: unsupported C=%d k=%d stride=%d", C, k, stride);
     return VPB_ERR_ARG;
   }
+  if (act != VPB_ACT_NONE && act != VPB_ACT_SILU) { vpb_set_error("depthwise: act %d (NONE or SILU)", act); return VPB_ERR_ARG; }
+  if (const int rc = check_batch("depthwise", batch, in_lo || out_lo)) return rc;
+  const int silu = act == VPB_ACT_SILU;   // the kernel takes a 0/1 flag
   const DwGeom g = dw_geometry(H, W, C, k, stride);
   const size_t smem = static_cast<size_t>(g.PPB) * C * sizeof(float);
   const uint4* i4 = static_cast<const uint4*>(in);
@@ -556,15 +579,15 @@ int vpb::depthwise_x(int dtype, const void* in, const void* in_lo, int H, int W,
   uint4* o4 = static_cast<uint4*>(out);
   uint4* o4l = static_cast<uint4*>(out_lo);
   const bool sp = in_lo != nullptr;
-  if (sp && !out_lo) { vpb_set_error("depthwise: split mode needs out_lo"); return VPB_ERR_ARG; }
+  if (sp != (out_lo != nullptr)) { vpb_set_error("depthwise: split mode needs both in_lo and out_lo"); return VPB_ERR_ARG; }
 #define DW_LAUNCH(E, K, S)                                                                             \
   do {                                                                                                 \
     if (sp) VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, true, false>, dim3(g.nblocks), dim3(g.threads), smem, st, i4, i4l, H, W, C, \
-                                 w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, act));  \
+                                 w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, silu));  \
     else if (batch > 1) VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, false, true>, dim3(g.nblocks, batch), dim3(g.threads), smem, st, \
-                              i4, i4l, H, W, C, w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, act)); \
+                              i4, i4l, H, W, C, w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, silu)); \
     else VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, false, false>, dim3(g.nblocks), dim3(g.threads), smem, st, i4, i4l, H, W, C, \
-                              w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, act));     \
+                              w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, silu));     \
   } while (0)
 #define DW_DISPATCH(E)                                            \
   do {                                                            \
@@ -584,11 +607,18 @@ extern "C" int vpb_se_scale(int dtype, const long long* gap_acc, int HW, int C, 
                             void* act, float* scale_out, void* stream) {
   return vpb::se_scale_x(dtype, gap_acc, HW, C, sq, w1, b1, w2, b2, act, nullptr, scale_out, static_cast<cudaStream_t>(stream));
 }
+extern "C" int vpb_se_scale_ex(int dtype, const long long* gap_acc, int HW, int C, int sq, const float* w1,
+                               const float* b1, const float* w2, const float* b2, void* act, void* act_lo,
+                               float* scale_out, int batch, void* stream) {
+  return vpb::se_scale_x(dtype, gap_acc, HW, C, sq, w1, b1, w2, b2, act, act_lo, scale_out, static_cast<cudaStream_t>(stream),
+                         batch);
+}
 int vpb::se_scale_x(int dtype, const long long* gap_acc, int HW, int C, int sq, const float* w1, const float* b1,
                     const float* w2, const float* b2, void* act, void* act_lo, float* scale_out, cudaStream_t st,
                     int batch) {
   const size_t smem = (2 * static_cast<size_t>(C) + sq) * sizeof(float);
   if ((C & 7) || C > 1152 || sq > 48 || !act) { vpb_set_error("se_scale: unsupported C=%d sq=%d", C, sq); return VPB_ERR_ARG; }
+  if (const int rc = check_batch("se_scale", batch, act_lo != nullptr)) return rc;
   // every block recomputes the gate (reads w1 + w2: 8*C*sq bytes), so the grid follows the activation bytes: one block
   // per 64 KB, at most two waves; the late blocks (C = 1152 on 10x20 pixels) get 7 blocks, the first (96 on 160x320) two waves on 132 SMs
   const int n8 = HW * (C / 8);
@@ -605,7 +635,13 @@ int vpb::se_scale_x(int dtype, const long long* gap_acc, int HW, int C, int sq, 
 extern "C" int vpb_gap(int dtype, const void* in, int HW, int C, int ld, float* out, void* stream) {
   return vpb::gap_x(dtype, in, nullptr, HW, C, ld, out, static_cast<cudaStream_t>(stream));
 }
+extern "C" int vpb_gap_ex(int dtype, const void* in, const void* in_lo, int HW, int C, int ld, float* out, int batch,
+                          void* stream) {
+  return vpb::gap_x(dtype, in, in_lo, HW, C, ld, out, static_cast<cudaStream_t>(stream), batch);
+}
 int vpb::gap_x(int dtype, const void* in, const void* in_lo, int HW, int C, int ld, float* out, cudaStream_t st, int batch) {
+  if (ld < C) { vpb_set_error("gap: ld=%d < C=%d", ld, C); return VPB_ERR_ARG; }
+  if (const int rc = check_batch("gap", batch, in_lo != nullptr)) return rc;
   if (dtype == VPB_BF16)
     VPB_CUDA_OK(launch_k(gap_kernel<BF16>, dim3((C + 255) / 256, batch), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(in), static_cast<const __nv_bfloat16*>(in_lo), HW, C, ld, out));
   else
@@ -617,8 +653,13 @@ extern "C" int vpb_linear(const float* x, const float* w, const float* b, int in
                           float* y, void* stream) {
   return vpb::linear_x(x, w, b, in_f, out_f, act, y, static_cast<cudaStream_t>(stream), 1);
 }
+extern "C" int vpb_linear_ex(const float* x, const float* w, const float* b, int in_f, int out_f, int act, float* y,
+                             int batch, void* stream) {
+  return vpb::linear_x(x, w, b, in_f, out_f, act, y, static_cast<cudaStream_t>(stream), batch);
+}
 int vpb::linear_x(const float* x, const float* w, const float* b, int in_f, int out_f, int act, float* y, cudaStream_t st,
                   int batch) {
+  if (act < VPB_ACT_NONE || act > VPB_ACT_SILU2) { vpb_set_error("linear: act %d", act); return VPB_ERR_ARG; }
   const dim3 g((out_f + 7) / 8), blk(256);
   switch (batch) {
     case 1: VPB_CUDA_OK(launch_k(linear_kernel<1>, g, blk, 0, st, x, w, b, in_f, out_f, act, y)); break;
@@ -638,8 +679,14 @@ extern "C" int vpb_ctx_conv1(int dtype, const float* in, int H, int W, const flo
                              int Cout, void* out, int out_pad, void* stream) {
   return vpb::ctx_conv1_x(dtype, in, H, W, w, b, Cout, out, nullptr, out_pad, static_cast<cudaStream_t>(stream));
 }
+extern "C" int vpb_ctx_conv1_ex(int dtype, const float* in, int H, int W, const float* w, const float* b, int Cout,
+                                void* out, void* out_lo, int out_pad, int act, int batch, void* stream) {
+  return vpb::ctx_conv1_x(dtype, in, H, W, w, b, Cout, out, out_lo, out_pad, static_cast<cudaStream_t>(stream), act, batch);
+}
 int vpb::ctx_conv1_x(int dtype, const float* in, int H, int W, const float* w, const float* b, int Cout, void* out,
                      void* out_lo, int out_pad, cudaStream_t st, int act, int batch) {
+  if (act != VPB_ACT_GELU && act != VPB_ACT_SILU) { vpb_set_error("ctx_conv1: act %d (GELU or SILU)", act); return VPB_ERR_ARG; }
+  if (const int rc = check_batch("ctx_conv1", batch, out_lo != nullptr)) return rc;
   const int n = H * W * Cout;
   if (dtype == VPB_BF16)
     VPB_CUDA_OK(launch_k(ctx_conv1_kernel<BF16>, dim3((n + 255) / 256, batch), dim3(256), 0, st, in, H, W, w, b, Cout, static_cast<__nv_bfloat16*>(out), static_cast<__nv_bfloat16*>(out_lo), out_pad, act));
@@ -654,8 +701,26 @@ extern "C" int vpb_fuse_pool_concat(int dtype, const void* f0, const void* f1, c
   const size_t z[5] = {0, 0, 0, 0, 0};
   return vpb::fuse_pool_x(dtype, f0, f1, f2, f3, f4, z, H4, W4, out, nullptr, static_cast<cudaStream_t>(stream));
 }
+extern "C" int vpb_fuse_pool_concat_ex(int dtype, const void* f0, const void* f1, const void* f2, const void* f3,
+                                       const void* f4, const void* f0_lo, const void* f1_lo, const void* f2_lo,
+                                       const void* f3_lo, const void* f4_lo, int H4, int W4, void* out, void* out_lo,
+                                       int batch, void* stream) {
+  const void* hi[5] = {f0, f1, f2, f3, f4};
+  const void* lo[5] = {f0_lo, f1_lo, f2_lo, f3_lo, f4_lo};
+  size_t off[5] = {0, 0, 0, 0, 0};
+  for (int i = 0; i < 5; ++i) {
+    if ((lo[i] != nullptr) != (out_lo != nullptr)) {
+      vpb_set_error("fuse_pool_concat: split mode needs all five input low halves and out_lo");
+      return VPB_ERR_ARG;
+    }
+    // the kernel reaches each low half at a byte offset from its hi tensor (unsigned wrap-around for lo < hi)
+    if (lo[i]) off[i] = reinterpret_cast<uintptr_t>(lo[i]) - reinterpret_cast<uintptr_t>(hi[i]);
+  }
+  return vpb::fuse_pool_x(dtype, f0, f1, f2, f3, f4, off, H4, W4, out, out_lo, static_cast<cudaStream_t>(stream), batch);
+}
 int vpb::fuse_pool_x(int dtype, const void* f0, const void* f1, const void* f2, const void* f3, const void* f4,
                      const size_t lo_off[5], int H4, int W4, void* out, void* out_lo, cudaStream_t st, int batch) {
+  if (const int rc = check_batch("fuse_pool_concat", batch, out_lo != nullptr)) return rc;
   const long warps = static_cast<long>(H4) * W4 * 182;
   const int blocks = static_cast<int>((warps * 32 + 255) / 256);
 #define FP_ARGS static_cast<const uint4*>(f0), static_cast<const uint4*>(f1), static_cast<const uint4*>(f2), \

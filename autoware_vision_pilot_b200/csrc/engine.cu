@@ -237,7 +237,7 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
       {
         const void* in = cur.p; void* o = dwo.p; const int H = cur.H, W = cur.W;
         const void* in_lo = cur.lo; void* o_lo = dwo.lo;
-        e.add_op(nm + "dw", "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, in, in_lo, H, W, ce, k, s_, d_dw, d_dwb, o, o_lo, d_part, st, 1, nb); },
+        e.add_op(nm + "dw", "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, in, in_lo, H, W, ce, k, s_, d_dw, d_dwb, o, o_lo, d_part, st, VPB_ACT_SILU, nb); },
                  2.0 * g.Ho * g.Wo * ce * k * k, nb * (2.0 * H * W * ce + 2.0 * g.Ho * g.Wo * ce));
       }
       // SE gate applied to the depthwise output in place (where the reference graph applies it), then a plain 1x1
@@ -431,7 +431,7 @@ static int build_context(vp_engine& e, const WeightMap& w, const std::string& p,
   Tens c4 = e.act_alloc(feat.H, feat.W, 128, /*pad=*/1);
   {
     const float* xin = cur; void* o = c4.p; void* o_lo = c4.lo; const int H = feat.H, W = feat.W;
-    e.add_op(tag + "ctx3", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, xin, H, W, d_w3, d_b3, 128, o, o_lo, 1, st, 1, nb); },
+    e.add_op(tag + "ctx3", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, xin, H, W, d_w3, d_b3, 128, o, o_lo, 1, st, VPB_ACT_GELU, nb); },
              2.0 * HW * 128 * 9, nb * 2.0 * (H + 2) * (W + 2) * 128);
   }
   Tens c5, c6;

@@ -48,21 +48,22 @@ struct DwGeom {
 DwGeom dw_geometry(int H, int W, int C, int k, int stride);
 
 // Launchers with the optional low halves of split-fp16 tensors (NULL / 0 = plain 16-bit mode); the extern "C"
-// entry points of vp_b200_ops.h forward to these.  `batch` images (1..kMaxBatch, 16-bit mode only) are stored back
-// to back in every tensor argument (gap_acc: one [kGapReplicas][C] accumulator set per image; linear: x [batch][in_f],
-// y [batch][out_f]); each image's result is bit-identical to a batch-1 call on it.
+// entry points of vp_b200_ops.h forward to these.  `batch` images (1..kMaxBatch, 16-bit mode only: VPB_ERR_ARG
+// otherwise) are stored back to back in every tensor argument (gap_acc: one [kGapReplicas][C] accumulator set per
+// image; linear: x [batch][in_f], y [batch][out_f]); each image's result is bit-identical to a batch-1 call on it.
+// `act` takes VPB_ACT_* values.
 int stem_conv_x(int dtype, const void* in, const void* in_lo, int H, int W, const float* w, const float* bias,
                 void* out, void* out_lo, cudaStream_t st, int batch = 1);
 int depthwise_x(int dtype, const void* in, const void* in_lo, int H, int W, int C, int k, int stride, const float* w,
-                const float* bias, void* out, void* out_lo, long long* gap_acc, cudaStream_t st, int act = 1 /* SiLU; 0 = none */,
-                int batch = 1);
+                const float* bias, void* out, void* out_lo, long long* gap_acc, cudaStream_t st,
+                int act = VPB_ACT_SILU /* or VPB_ACT_NONE */, int batch = 1);
 int se_scale_x(int dtype, const long long* gap_acc, int HW, int C, int sq, const float* w1, const float* b1,
                const float* w2, const float* b2, void* act, void* act_lo, float* scale_out, cudaStream_t st, int batch = 1);
 int gap_x(int dtype, const void* in, const void* in_lo, int HW, int C, int ld, float* out, cudaStream_t st, int batch = 1);
 int linear_x(const float* x, const float* w, const float* b, int in_f, int out_f, int act, float* y, cudaStream_t st,
              int batch);
 int ctx_conv1_x(int dtype, const float* in, int H, int W, const float* w, const float* b, int Cout, void* out,
-                void* out_lo, int out_pad, cudaStream_t st, int act = 1 /* ACT_GELU; 2 = ACT_SILU */, int batch = 1);
+                void* out_lo, int out_pad, cudaStream_t st, int act = VPB_ACT_GELU /* or VPB_ACT_SILU */, int batch = 1);
 int fuse_pool_x(int dtype, const void* f0, const void* f1, const void* f2, const void* f3, const void* f4,
                 const size_t lo_off[5], int H4, int W4, void* out, void* out_lo, cudaStream_t st, int batch = 1);
 

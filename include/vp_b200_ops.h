@@ -166,38 +166,69 @@ int vpb_resize_tables_host(int mode, int in_size, int out_size, int* bounds, int
 
 /* ---- EfficientNet-B0 encoder pieces (torchvision efficientnet_b0().features, reached through
  *      Models/model_components/backbone.py:9-22; BatchNorm folded at load) ---- */
-/* stem: Conv3x3 s2 p1 (3->32) + BN + SiLU.  in [H][W][4] 16-bit -> out [H/2][W/2][32].
+/* stem: Conv3x3 s2 p1 (3->32) + BN + SiLU.  in [H][W][4] 16-bit (channel 3 is never read) -> out [H/2][W/2][32];
+ * H and W must be even and >= 2 (VPB_ERR_ARG otherwise).
  * w: fp32 [27][32] (tap-major ky,kx,c), bias fp32 [32]. */
 int vpb_stem_conv(int dtype, const void* in, int H, int W, const float* w, const float* bias,
                   void* out, void* stream);
 /* depthwise k x k (k = 3 or 5), stride 1 or 2, pad (k-1)/2, + bias + SiLU; also accumulates the
- * squeeze-excitation average pool: gap_acc[8][C] int64 (8 replicas that the SE kernel sums),
- * 2^-24 fixed point, must be zero on entry (integer atomics => the pooled sum is
- * bit-reproducible regardless of block order).
- * in [H][W][C] -> out [Ho][Wo][C]; w fp32 [k*k][C]. */
+ * squeeze-excitation average pool of the fp32 outputs before 16-bit rounding: gap_acc[8][C] int64
+ * (8 replicas that the SE kernel sums), 2^-24 fixed point, must be zero on entry (integer atomics =>
+ * the pooled sum is bit-reproducible regardless of block order).
+ * in [H][W][C] -> out [Ho][Wo][C]; w fp32 [k*k][C]; C a multiple of 8 in 8..2048. */
 int vpb_depthwise(int dtype, const void* in, int H, int W, int C, int k, int stride, const float* w,
                   const float* bias, void* out, long long* gap_acc, void* stream);
 /* squeeze-excitation (torchvision SqueezeExcitation): mean = gap_acc * 2^-24 / HW; s = sigmoid(W2 silu(W1 mean + b1) + b2);
  * then act[p][c] *= s[c] IN PLACE on the depthwise output [HW][C] 16-bit — where the reference graph applies the gate.
  * (Round 1 folded s into the 16-bit projection weights instead; measured 3-8x less accurate off the calibration frame.)
- * w1 fp32 [sq][C], w2 fp32 TRANSPOSED [sq][C]; scale_out (optional) fp32 [C]. */
+ * w1 fp32 [sq][C], w2 fp32 TRANSPOSED [sq][C]; scale_out (optional) fp32 [C]; C a multiple of 8 <= 1152, sq <= 48. */
 int vpb_se_scale(int dtype, const long long* gap_acc, int HW, int C, int sq, const float* w1,
                  const float* b1, const float* w2, const float* b2, void* act, float* scale_out, void* stream);
 
 /* ---- context block pieces (scene_context.py:25-57 / auto_steer_context.py:28-60) ---- */
-/* global average pool over [HW][C] 16-bit -> fp32 [C] (scene_context.py:27) */
+/* global average pool over [HW][ld] 16-bit (ld >= C) -> fp32 [C] (scene_context.py:27) */
 int vpb_gap(int dtype, const void* in, int HW, int C, int ld, float* out, void* stream);
-/* y = act(W x + b), fp32, W [out][in] (scene_context.py:30-38) */
+/* y = act(W x + b), fp32, W [out][in] (scene_context.py:30-38); act VPB_ACT_NONE .. VPB_ACT_SILU2 */
 int vpb_linear(const float* x, const float* w, const float* b, int in_f, int out_f, int act, float* y,
                void* stream);
 /* context_layer_3: Conv3x3 1->128 + GELU on the 10x20 map (scene_context.py:41-47).
- * in fp32 [H][W], w fp32 [Cout][9], out [H][W][Cout] 16-bit (zero-bordered image if out_pad) */
+ * in fp32 [H][W], w fp32 [Cout][9], out [H][W][Cout] 16-bit.  With out_pad = 1, out is the
+ * [(H+2)][(W+2)][Cout] zero-bordered image: only its interior is written, the border is left as the
+ * caller stored it. */
 int vpb_ctx_conv1(int dtype, const float* in, int H, int W, const float* w, const float* b, int Cout,
                   void* out, int out_pad, void* stream);
 /* BackboneFeatureFusion (backbone_feature_fusion.py:13-38): 4/3/2/1 x MaxPool2x2 of f0..f3,
  * concatenated with f4 -> [H4][W4][32+24+40+80+1280]. */
 int vpb_fuse_pool_concat(int dtype, const void* f0, const void* f1, const void* f2, const void* f3,
                          const void* f4, int H4, int W4, void* out, void* stream);
+
+/* ---- the same encoder / context ops with every variant the engines launch ----
+ * Each *_ex entry takes, in addition to the arguments of the entry above:
+ *   *_lo    the low halves of split-fp16 tensors (the layout of their hi partner; NULL = 16-bit mode): the op
+ *           reads hi + lo and writes the result as (hi, lo) = (round16(r), round16(r - round16(r)));
+ *   act     where the kernel has a choice of activation;
+ *   batch   1..8 images stored back to back in every tensor (gap_acc: one [8][C] set per image; linear: x [batch][in_f],
+ *           y [batch][out_f]; se_scale: scale_out [batch][C]); each image's result is bit-identical to a batch-1 call on
+ *           it.  Split-fp16 tensors cannot be batched.
+ * Arguments outside these contracts return VPB_ERR_ARG before any device work. */
+int vpb_stem_conv_ex(int dtype, const void* in, const void* in_lo, int H, int W, const float* w, const float* bias,
+                     void* out, void* out_lo, int batch, void* stream);
+/* act: VPB_ACT_SILU (EfficientNet) or VPB_ACT_NONE (AutoSpeed); in_lo and out_lo both or neither */
+int vpb_depthwise_ex(int dtype, const void* in, const void* in_lo, int H, int W, int C, int k, int stride,
+                     const float* w, const float* bias, void* out, void* out_lo, long long* gap_acc, int act, int batch,
+                     void* stream);
+int vpb_se_scale_ex(int dtype, const long long* gap_acc, int HW, int C, int sq, const float* w1, const float* b1,
+                    const float* w2, const float* b2, void* act, void* act_lo, float* scale_out, int batch, void* stream);
+int vpb_gap_ex(int dtype, const void* in, const void* in_lo, int HW, int C, int ld, float* out, int batch, void* stream);
+int vpb_linear_ex(const float* x, const float* w, const float* b, int in_f, int out_f, int act, float* y, int batch,
+                  void* stream);
+/* act: VPB_ACT_GELU (scene context) or VPB_ACT_SILU (AutoSpeed CTX block) */
+int vpb_ctx_conv1_ex(int dtype, const float* in, int H, int W, const float* w, const float* b, int Cout, void* out,
+                     void* out_lo, int out_pad, int act, int batch, void* stream);
+/* f*_lo: all five and out_lo, or none */
+int vpb_fuse_pool_concat_ex(int dtype, const void* f0, const void* f1, const void* f2, const void* f3, const void* f4,
+                            const void* f0_lo, const void* f1_lo, const void* f2_lo, const void* f3_lo,
+                            const void* f4_lo, int H4, int W4, void* out, void* out_lo, int batch, void* stream);
 
 /* ---- output side (all device-resident) ---- */
 /* createMaskKernel (cuda_visualization_kernels.cu:13-42; CPU twin run_model_node.cpp:148-172):

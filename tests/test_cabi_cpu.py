@@ -83,6 +83,77 @@ def test_conv_rejects_bad_arguments_without_a_gpu():
     assert lib.vpb_upconv_compose(None, None, None, None, None, None, 8, 8, 8, 0, None, None, None, None) == -1
 
 
+def test_encoder_ops_reject_bad_arguments_without_a_gpu():
+    """Every contract violation of the encoder / context op entry points returns VPB_ERR_ARG with a message before
+    any device work (so no GPU is needed to see it)."""
+    lib = L.lib()
+    vp, i = C.c_void_p, C.c_int
+    lib.vpb_stem_conv_ex.argtypes = [i, vp, vp, i, i, vp, vp, vp, vp, i, vp]
+    lib.vpb_depthwise.argtypes = [i, vp, i, i, i, i, i, vp, vp, vp, vp, vp]
+    lib.vpb_depthwise_ex.argtypes = [i, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp, i, i, vp]
+    lib.vpb_se_scale_ex.argtypes = [i, vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, i, vp]
+    lib.vpb_gap_ex.argtypes = [i, vp, vp, i, i, i, vp, i, vp]
+    lib.vpb_linear_ex.argtypes = [vp, vp, vp, i, i, i, vp, i, vp]
+    lib.vpb_ctx_conv1_ex.argtypes = [i, vp, i, i, vp, vp, i, vp, vp, i, i, i, vp]
+    lib.vpb_fuse_pool_concat_ex.argtypes = [i] + [vp] * 10 + [i, i, vp, vp, i, vp]
+    buf = (C.c_float * 64)()
+    p = C.addressof(buf)           # never dereferenced: every call below must fail validation first
+
+    def stem(H=8, W=8, lo=None, out_lo=None, batch=1):
+        return lib.vpb_stem_conv_ex(0, p, lo, H, W, p, p, p, out_lo, batch, None)
+
+    def dw(C_=32, k=3, s=1, lo=None, out_lo=None, act=L.ACT_SILU, batch=1):
+        return lib.vpb_depthwise_ex(0, p, lo, 8, 8, C_, k, s, p, p, p, out_lo, p, act, batch, None)
+
+    def se(C_=32, sq=8, act_lo=None, batch=1):
+        return lib.vpb_se_scale_ex(0, p, 64, C_, sq, p, p, p, p, p, act_lo, None, batch, None)
+
+    def gap(C_=32, ld=32, lo=None, batch=1):
+        return lib.vpb_gap_ex(0, p, lo, 64, C_, ld, p, batch, None)
+
+    def linear(act=L.ACT_NONE, batch=1):
+        return lib.vpb_linear_ex(p, p, p, 32, 8, act, p, batch, None)
+
+    def ctx(act=L.ACT_GELU, out_lo=None, batch=1):
+        return lib.vpb_ctx_conv1_ex(0, p, 10, 20, p, p, 128, p, out_lo, 1, act, batch, None)
+
+    def fuse(lo=(None,) * 5, out_lo=None, batch=1):
+        return lib.vpb_fuse_pool_concat_ex(0, p, p, p, p, p, *lo, 3, 5, p, out_lo, batch, None)
+
+    cases = [
+        ("stem odd H", lambda: stem(H=7), "stem"), ("stem odd W", lambda: stem(W=9), "stem"),
+        ("stem H < 2", lambda: stem(H=0), "stem"), ("stem W = 1", lambda: stem(W=1), "stem"),
+        ("stem batch 0", lambda: stem(batch=0), "batch"), ("stem batch 9", lambda: stem(batch=9), "batch"),
+        ("stem split batch", lambda: stem(lo=p, out_lo=p, batch=2), "split"),
+        ("stem split out batch", lambda: stem(out_lo=p, batch=2), "split"),
+        ("depthwise C 2056", lambda: dw(C_=2056), "depthwise"), ("depthwise C 4", lambda: dw(C_=4), "depthwise"),
+        ("depthwise C 0", lambda: dw(C_=0), "depthwise"), ("depthwise C 12", lambda: dw(C_=12), "depthwise"),
+        ("depthwise k 7", lambda: dw(k=7), "depthwise"), ("depthwise stride 3", lambda: dw(s=3), "depthwise"),
+        ("depthwise act GELU", lambda: dw(act=L.ACT_GELU), "act"),
+        ("depthwise act SIGMOID", lambda: dw(act=L.ACT_SIGMOID), "act"),
+        ("depthwise in_lo only", lambda: dw(lo=p), "split"), ("depthwise out_lo only", lambda: dw(out_lo=p), "split"),
+        ("depthwise batch 9", lambda: dw(batch=9), "batch"),
+        ("depthwise split batch", lambda: dw(lo=p, out_lo=p, batch=3), "split"),
+        ("depthwise legacy C 0", lambda: lib.vpb_depthwise(0, p, 8, 8, 0, 3, 1, p, p, p, p, None), "depthwise"),
+        ("se C 1160", lambda: se(C_=1160), "se_scale"), ("se sq 49", lambda: se(sq=49), "se_scale"),
+        ("se batch 0", lambda: se(batch=0), "batch"), ("se split batch", lambda: se(act_lo=p, batch=2), "split"),
+        ("gap ld < C", lambda: gap(ld=24), "ld"), ("gap batch 9", lambda: gap(batch=9), "batch"),
+        ("gap split batch", lambda: gap(lo=p, batch=2), "split"),
+        ("linear act 5", lambda: linear(act=5), "act"), ("linear act -1", lambda: linear(act=-1), "act"),
+        ("linear batch 0", lambda: linear(batch=0), "batch"), ("linear batch 9", lambda: linear(batch=9), "batch"),
+        ("ctx act NONE", lambda: ctx(act=L.ACT_NONE), "act"), ("ctx act SIGMOID", lambda: ctx(act=L.ACT_SIGMOID), "act"),
+        ("ctx batch 9", lambda: ctx(batch=9), "batch"), ("ctx split batch", lambda: ctx(out_lo=p, batch=2), "split"),
+        ("fuse batch 9", lambda: fuse(batch=9), "batch"),
+        ("fuse split batch", lambda: fuse(lo=(p,) * 5, out_lo=p, batch=2), "split"),
+        ("fuse four low halves", lambda: fuse(lo=(p, p, None, p, p), out_lo=p), "low halves"),
+        ("fuse low halves without out_lo", lambda: fuse(lo=(p,) * 5), "low halves"),
+        ("fuse out_lo without low halves", lambda: fuse(out_lo=p), "low halves"),
+    ]
+    for name, call, msg in cases:
+        assert call() == -1, name
+        assert msg in L.last_error(), (name, L.last_error())
+
+
 def test_vpw_writer_layout(tmp_path):
     sd = {"a.weight": np.arange(24, dtype=np.float32).reshape(2, 3, 2, 2),
           "a.num_batches_tracked": np.array(7, dtype=np.int64)}

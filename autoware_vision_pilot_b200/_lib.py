@@ -40,7 +40,7 @@ class ConvArgs(C.Structure):
         ("stride", C.c_int), ("in_h", C.c_int), ("in_w", C.c_int), ("ldw", C.c_int), ("act2", C.c_int), ("out_slice", C.c_int),
         ("in_lo", C.c_void_p), ("w_lo", C.c_void_p), ("out_lo", C.c_void_p), ("res_lo", C.c_void_p),
         ("in2_lo", C.c_void_p), ("w2_lo", C.c_void_p), ("taps2", C.c_int),
-        ("batch", C.c_int),
+        ("batch", C.c_int), ("w_img", C.c_int),
     ]
 
 

@@ -17,12 +17,18 @@
 // the concatenated tensor (ldo / ldi strides), BatchNorm (eps 1e-3) is folded at load.  The byte-moving pieces are
 // small SIMT kernels in this file (mean over H x W, nearest upsample, 5x5 max-pool, V transpose, softmax, DFL decode,
 // confidence filter + NMS).
+//
+// Batch (vp_autospeed_create_batch): every per-frame buffer holds `batch` samples back to back, sample outermost.  The
+// convolutions take the batch as their tensor maps' image dimension (the attention's activation "weights" through
+// w_img); each SIMT kernel takes the image from blockIdx.y or folds it into its flat index, with the grid of one image
+// unchanged, so every sample is computed in its batch-1 order and equals a batch-1 call bit for bit.
 #include "common.cuh"
 #include "conv_gemm.cuh"
 #include "ops_internal.h"
 #include "engine_internal.h"
 #include "../../include/vp_b200_autospeed.h"
 
+#include <algorithm>
 #include <cmath>
 #include <functional>
 #include <memory>
@@ -36,12 +42,19 @@ static constexpr int kNC = 4, kDfl = 16, kNA = 64 * 128 + 32 * 64 + 16 * 32;   /
 static constexpr float kBnEps = 1e-3f;                        // common_layers.py:10
 
 // ------------------------------------------------------------------ SIMT kernels
-// mean over H*W per channel, two deterministic stages (CTX block, common_layers.py:214)
-template <class E>
+// kB / kBatch = false (batch 1, a grid without images) compiles each kernel to its single-image code: these kernels are
+// latency-bound, and the per-image addressing on the critical path slowed a batch-1 frame by about 1 % on the H100.
+// mean over H*W per channel, two deterministic stages (CTX block, common_layers.py:214); blockIdx.y = image:
+// in [N][HW][ld], part [N][nblk][C], out [N][C]
+template <class E, bool kB>
 __global__ void __launch_bounds__(256) mean_part_kernel(const typename E::T* __restrict__ in, int HW, int C, int ld,
                                                         float* __restrict__ part) {
   pdl_launch_dependents();
   pdl_wait();
+  if (kB) {
+    in += static_cast<size_t>(blockIdx.y) * HW * ld;
+    part += static_cast<size_t>(blockIdx.y) * gridDim.x * C;
+  }
   // block b reduces pixels [b*chunk, (b+1)*chunk); thread t owns channel t % C of pixel lane t / C
   const int ppb = 256 / C;                    // pixels handled in parallel (C <= 256, power of two here)
   const int c = threadIdx.x % C, pl = threadIdx.x / C;
@@ -59,22 +72,31 @@ __global__ void __launch_bounds__(256) mean_part_kernel(const typename E::T* __r
     part[blockIdx.x * C + threadIdx.x] = t;
   }
 }
+template <bool kB>
 __global__ void mean_final_kernel(const float* __restrict__ part, int nblk, int C, float inv_hw, float* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
+  if (kB) {
+    part += static_cast<size_t>(blockIdx.y) * nblk * C;
+    out += static_cast<size_t>(blockIdx.y) * C;
+  }
   float s = 0.f;
   for (int b = 0; b < nblk; ++b) s += part[b * C + c];       // fixed order
   out[c] = s * inv_hw;
 }
 
-// nn.Upsample(scale_factor=2) (nearest, auto_speed_neck.py:10) written straight into a concat slice
-template <class E>
+// nn.Upsample(scale_factor=2) (nearest, auto_speed_neck.py:10) written straight into a concat slice; blockIdx.y = image
+template <class E, bool kB>
 __global__ void upsample2_kernel(const uint4* __restrict__ in, int H, int W, int C8, int ld8_in, uint4* __restrict__ out,
                                  int ld8_out) {
   pdl_launch_dependents();
   pdl_wait();
+  if (kB) {
+    in += static_cast<size_t>(blockIdx.y) * H * W * ld8_in;
+    out += static_cast<size_t>(blockIdx.y) * 4 * H * W * ld8_out;
+  }
   const long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long n = static_cast<long>(4) * H * W * C8;
   if (i >= n) return;
@@ -84,11 +106,15 @@ __global__ void upsample2_kernel(const uint4* __restrict__ in, int H, int W, int
   out[pix * ld8_out + g] = __ldg(in + (static_cast<long>(oy >> 1) * W + (ox >> 1)) * ld8_in + g);
 }
 
-// MaxPool2d(5, stride 1, padding 2) (SPPF, common_layers.py:249), slice in -> slice out
-template <class E>
+// MaxPool2d(5, stride 1, padding 2) (SPPF, common_layers.py:249), slice in -> slice out; blockIdx.y = image
+template <class E, bool kB>
 __global__ void maxpool5_kernel(const uint4* __restrict__ in, int H, int W, int C8, int ld8, uint4* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
+  if (kB) {
+    in += static_cast<size_t>(blockIdx.y) * H * W * ld8;
+    out += static_cast<size_t>(blockIdx.y) * H * W * ld8;
+  }
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= H * W * C8) return;
   const int g = i % C8, pix = i / C8;
@@ -117,12 +143,18 @@ __global__ void maxpool5_kernel(const uint4* __restrict__ in, int H, int W, int 
 }
 
 // qkv [T][nh*(2dk+dh)] -> Vc [T][nh*dh] (token-major, for the depthwise conv on v, common_layers.py:102) and
-// Vt [nh][dh][T] (key-token-major, the K-major "weight" operand of O = P V^T)
-template <class E>
+// Vt [nh][dh][T] (key-token-major, the K-major "weight" operand of O = P V^T); blockIdx.y = image
+template <class E, bool kB>
 __global__ void split_v_kernel(const typename E::T* __restrict__ qkv, int T, int nh, int dk, int dh,
                                typename E::T* __restrict__ vc, typename E::T* __restrict__ vt) {
   pdl_launch_dependents();
   pdl_wait();
+  if (kB) {
+    const size_t img = blockIdx.y;
+    qkv += img * T * nh * (2 * dk + dh);
+    vc += img * T * nh * dh;
+    vt += img * T * nh * dh;
+  }
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= T * nh * dh) return;
   const int d = i % dh, h = (i / dh) % nh, t = i / (dh * nh);
@@ -131,7 +163,8 @@ __global__ void split_v_kernel(const typename E::T* __restrict__ qkv, int T, int
   vt[(static_cast<size_t>(h) * dh + d) * T + t] = v;
 }
 
-// softmax over the key axis of S * scale (common_layers.py:99-100): one warp per query row, fp32 math
+// softmax over the key axis of S * scale (common_layers.py:99-100): one warp per query row, fp32 math (a batch is
+// [N * T] independent rows)
 template <class E>
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const typename E::T* __restrict__ s, int rows, int cols,
                                                            float scale, typename E::T* __restrict__ p) {
@@ -165,12 +198,17 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const typename E::T* 
 
 // AutoSpeedHead decode (auto_speed_head.py:53-63): DFL expectation over 16 bins x 4 sides, anchors, stride,
 // class sigmoid.  lvl [hw][ld] 16-bit: channels 0..63 box logits (side-major: side*16 + bin), 64..67 class logits.
-// out fp32 planar [8][NA]: cx, cy, w, h (pixels of the 1024x512 canvas), 4 class probabilities.
-template <class E>
+// out fp32 planar [8][NA]: cx, cy, w, h (pixels of the 1024x512 canvas), 4 class probabilities.  blockIdx.y = image
+// (lvl [N][hw][ld], out [N][8][NA]).
+template <class E, bool kB>
 __global__ void decode_kernel(const typename E::T* __restrict__ lvl, int h, int w, int ld, float stride, int a0, int NA,
                               float* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
+  if (kB) {
+    lvl += static_cast<size_t>(blockIdx.y) * h * w * ld;
+    out += static_cast<size_t>(blockIdx.y) * 8 * NA;
+  }
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= h * w) return;
   const typename E::T* r = lvl + static_cast<size_t>(i) * ld;
@@ -200,15 +238,26 @@ __global__ void decode_kernel(const typename E::T* __restrict__ lvl, int h, int 
 //   scores = max_c sigmoid(cls) (the SECOND sigmoid, :78), keep scores > conf, xywh -> xyxy, greedy class-agnostic
 //   NMS (torchvision.ops.nms: descending score, stable for ties, suppress IoU > thr), map back to the source frame.
 // det [max_det][6] = x1, y1, x2, y2, score, class;  n_det = number kept (<= max_det; n_cand = candidates seen).
+// One block per image (blockIdx.x): every buffer below is per image, sample outermost; the thresholds are shared.
 struct PostParams {
   const float* raw; int NA; float conf, iou; float scale; int pad_x, pad_y, orig_w, orig_h; int max_cand, max_det;
   float* cand;     // [max_cand][6] scratch (xyxy, score, class)
   int* order;      // [max_cand] scratch
   float* det; int* counts;   // counts[0] = n_det, counts[1] = n_cand
 };
-__global__ void __launch_bounds__(1024) postprocess_kernel(const PostParams p) {
+static PostParams __device__ __forceinline__ post_image(PostParams p, size_t img) {
+  p.raw += img * 8 * p.NA;
+  p.cand += img * p.max_cand * 6;
+  p.order += img * p.max_cand;
+  p.det += img * p.max_det * 6;
+  p.counts += img * 2;
+  return p;
+}
+template <bool kBatch>
+__global__ void __launch_bounds__(1024) postprocess_kernel(const PostParams p_) {
   pdl_launch_dependents();
   pdl_wait();
+  const PostParams p = kBatch ? post_image(p_, blockIdx.x) : p_;
   __shared__ int s_n;
   __shared__ int s_scan[1024];
   const int tid = threadIdx.x;
@@ -295,7 +344,7 @@ __global__ void __launch_bounds__(1024) postprocess_kernel(const PostParams p) {
   if (tid == 0) { p.counts[0] = s_keep_n; p.counts[1] = ncand_all; }
 }
 
-// gray (114, 114, 114) / 255 letterbox canvas with zero channels 3..7 (auto_speed_infer.py:39)
+// gray (114, 114, 114) / 255 letterbox canvas with zero channels 3..7 (auto_speed_infer.py:39); npix covers all canvases
 template <class E>
 __global__ void fill_canvas_kernel(typename E::T* __restrict__ x, int npix) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -310,6 +359,8 @@ __global__ void fill_canvas_kernel(typename E::T* __restrict__ x, int npix) {
 using namespace vpb;
 
 // ====================================================================== engine
+// Per-frame buffers hold `batch` samples (sample outermost): canvas [N][512][1024][8], raw [N][8][kNA], cand / order /
+// det [N][...], counts [N][2], every activation [N][H][W][C].
 struct vp_autospeed : EngineRuntime {
   PreprocessPlan pre;
   void* d_canvas = nullptr;
@@ -323,20 +374,23 @@ struct vp_autospeed : EngineRuntime {
 
   Tens talloc(int H, int W, int C) {
     Tens t; t.H = H; t.W = W; t.C = C; t.ld = C;
-    t.p = dalloc(static_cast<size_t>(H) * W * C * 2);
+    t.p = dalloc(static_cast<size_t>(H) * W * C * 2 * batch);
     return t;
   }
+  // flops: per sample (counted for the whole batch)
   void op(const std::string& name, std::function<int(cudaStream_t)> fn, double flops = 0) {
-    OpRec r; r.name = name; r.launch = std::move(fn); r.flops = flops;
+    OpRec r; r.name = name; r.launch = std::move(fn); r.flops = flops * batch;
     ops.push_back(std::move(r));
   }
 
-  // one wgmma convolution: in (slice) -> out (slice); w [taps][Cout][Cin] 16-bit (or an activation slice with ldw)
+  // one wgmma convolution: in (slice) -> out (slice); w [taps][Cout][Cin] 16-bit (or an activation slice with ldw,
+  // w_img elements apart per sample)
   int conv(const std::string& name, const Tens& in, const Tens& out, int Cout, int taps, int stride, const void* w,
            const float* bias, int act, int mode = VPB_EPI_STORE, const Tens* res = nullptr, int act2 = ACT_NONE,
-           int ldw = 0, int cin = 0) {
+           int ldw = 0, int w_img = 0) {
     vpb_conv_args a{};
-    a.dtype = dtype; a.H = out.H; a.W = out.W; a.Cin = cin > 0 ? cin : in.C; a.ldi = in.ld;
+    a.batch = batch; a.w_img = w_img;
+    a.dtype = dtype; a.H = out.H; a.W = out.W; a.Cin = in.C; a.ldi = in.ld;
     a.Cout = Cout; a.taps = taps; a.phases = 1; a.act = act; a.mode = mode;
     a.in = in.p; a.w = w; a.bias = bias;
     a.out = out.p; a.ldo = out.ld; a.out_slice = 1;
@@ -406,28 +460,28 @@ struct ASBuilder {
     std::vector<float> wt, bias;
     if (!fold(p, in.C, 1, 3, wt, bias, true)) return;
     float *dwt = e.upload_f32(wt), *db = e.upload_f32(bias);
-    const int dt = e.dtype, H = in.H, W = in.W, C = in.C;
+    const int dt = e.dtype, H = in.H, W = in.W, C = in.C, nb = e.batch;
     const void* ip = in.p; void* op_ = out.p; long long* gap = e.d_gap_scratch;
-    e.op(p, [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? VPB_ACT_SILU : VPB_ACT_NONE); },
+    e.op(p, [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? VPB_ACT_SILU : VPB_ACT_NONE, nb); },
          2.0 * H * W * C * 9);
   }
   // CTX (common_layers.py:194-239): x [h][w][C] -> out [h][w][Cout]
   void ctx(const std::string& p, const Tens& x, const Tens& out, int cout) {
     if (!ok()) return;
-    const int C = x.C, H = x.H, W = x.W, HW = H * W, dt = e.dtype;
+    const int C = x.C, H = x.H, W = x.W, HW = H * W, dt = e.dtype, nb = e.batch;
     const HostTensor *ew = find_w_shaped(w, p + ".exp0.weight", {HW, C, 3}), *eb = find_w_shaped(w, p + ".exp0.bias", {HW});
     const HostTensor *c0w = find_w_shaped(w, p + ".ctx0.weight", {C / 2, 1, 3, 3}), *c0b = find_w_shaped(w, p + ".ctx0.bias", {C / 2});
     if (!ew || !eb || !c0w || !c0b) { rc = VPB_ERR_IO; return; }
     // mean over H x W
     const int nblk = std::min(148, std::max(1, HW / 64));
-    float* d_part = static_cast<float*>(e.dalloc(static_cast<size_t>(nblk) * C * 4));
-    float* d_mean = static_cast<float*>(e.dalloc(C * 4));
+    float* d_part = static_cast<float*>(e.dalloc(static_cast<size_t>(nblk) * C * 4 * nb));
+    float* d_mean = static_cast<float*>(e.dalloc(static_cast<size_t>(C) * 4 * nb));
     {
       const void* ip = x.p; const int ld = x.ld;
       e.op(p + ".mean", [=](cudaStream_t st) {
-        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(mean_part_kernel<BF16>, dim3(nblk), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(ip), HW, C, ld, d_part));
-        else VPB_CUDA_OK(launch_k(mean_part_kernel<F16>, dim3(nblk), dim3(256), 0, st, static_cast<const __half*>(ip), HW, C, ld, d_part));
-        VPB_CUDA_OK(launch_k(mean_final_kernel, dim3((C + 127) / 128), dim3(128), 0, st, static_cast<const float*>(d_part), nblk, C, 1.0f / HW, d_mean));
+        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? mean_part_kernel<BF16, true> : mean_part_kernel<BF16, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(ip), HW, C, ld, d_part));
+        else VPB_CUDA_OK(launch_k(nb > 1 ? mean_part_kernel<F16, true> : mean_part_kernel<F16, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const __half*>(ip), HW, C, ld, d_part));
+        VPB_CUDA_OK(launch_k(nb > 1 ? mean_final_kernel<true> : mean_final_kernel<false>, dim3((C + 127) / 128, nb), dim3(128), 0, st, static_cast<const float*>(d_part), nblk, C, 1.0f / HW, d_mean));
         return VPB_OK;
       });
     }
@@ -436,15 +490,15 @@ struct ASBuilder {
     for (int o = 0; o < HW; ++o)
       for (int c = 0; c < C; ++c) lw[static_cast<size_t>(o) * C + c] = ew->f[(static_cast<size_t>(o) * C + c) * 3 + 1];
     float *d_lw = e.upload_f32(lw), *d_lb = e.upload_f32(eb->f);
-    float* d_map = static_cast<float*>(e.dalloc(static_cast<size_t>(HW) * 4));
-    e.op(p + ".exp0", [=](cudaStream_t st) { return vpb_linear(d_mean, d_lw, d_lb, C, HW, VPB_ACT_SILU2, d_map, st); },
+    float* d_map = static_cast<float*>(e.dalloc(static_cast<size_t>(HW) * 4 * nb));
+    e.op(p + ".exp0", [=](cudaStream_t st) { return linear_x(d_mean, d_lw, d_lb, C, HW, VPB_ACT_SILU2, d_map, st, nb); },
          2.0 * HW * C);
     // ctx0: Conv2d(1 -> C/2, 3x3) + SiLU
     Tens c2 = e.talloc(H, W, C / 2);
     float *d_c0w = e.upload_f32(c0w->f), *d_c0b = e.upload_f32(c0b->f);
     {
       void* op_ = c2.p; const int co = C / 2;
-      e.op(p + ".ctx0", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, nullptr, 0, st, ACT_SILU); },
+      e.op(p + ".ctx0", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, nullptr, 0, st, ACT_SILU, nb); },
            2.0 * HW * co * 9);
     }
     // ctx1: SiLU(conv) * x + x, then SiLU (:224-232) — one wgmma conv with the MULADD epilogue and a post activation
@@ -479,40 +533,40 @@ struct ASBuilder {
     cbs(p + ".conv2", cat, out, cout, 1, 1, true);
   }
   void upsample(const std::string& name, const Tens& in, const Tens& out) {
-    const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, li = in.ld / 8, lo = out.ld / 8;
+    const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, li = in.ld / 8, lo = out.ld / 8, nb = e.batch;
     const void* ip = in.p; void* op_ = out.p;
     const long n = 4L * H * W * C8;
     e.op(name, [=](cudaStream_t st) {
-      const dim3 g(static_cast<unsigned>((n + 255) / 256)), b(256);
-      if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(upsample2_kernel<BF16>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, li, static_cast<uint4*>(op_), lo));
-      else VPB_CUDA_OK(launch_k(upsample2_kernel<F16>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, li, static_cast<uint4*>(op_), lo));
+      const dim3 g(static_cast<unsigned>((n + 255) / 256), nb), b(256);
+      if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? upsample2_kernel<BF16, true> : upsample2_kernel<BF16, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, li, static_cast<uint4*>(op_), lo));
+      else VPB_CUDA_OK(launch_k(nb > 1 ? upsample2_kernel<F16, true> : upsample2_kernel<F16, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, li, static_cast<uint4*>(op_), lo));
       return VPB_OK;
     });
   }
   void maxpool(const std::string& name, const Tens& in, const Tens& out) {
-    const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, ld8 = in.ld / 8;
+    const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, ld8 = in.ld / 8, nb = e.batch;
     const void* ip = in.p; void* op_ = out.p;
     e.op(name, [=](cudaStream_t st) {
-      const dim3 g((H * W * C8 + 255) / 256), b(256);
-      if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(maxpool5_kernel<BF16>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, ld8, static_cast<uint4*>(op_)));
-      else VPB_CUDA_OK(launch_k(maxpool5_kernel<F16>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, ld8, static_cast<uint4*>(op_)));
+      const dim3 g((H * W * C8 + 255) / 256, nb), b(256);
+      if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? maxpool5_kernel<BF16, true> : maxpool5_kernel<BF16, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, ld8, static_cast<uint4*>(op_)));
+      else VPB_CUDA_OK(launch_k(nb > 1 ? maxpool5_kernel<F16, true> : maxpool5_kernel<F16, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, ld8, static_cast<uint4*>(op_)));
       return VPB_OK;
     });
   }
   // PSABlock on y (in place): y += attention(y); y += ffn(y)   (common_layers.py:77-118)
   void psablock(const std::string& p, const Tens& y, int nh) {
     if (!ok()) return;
-    const int C = y.C, T = y.H * y.W, dh = C / nh, dk = dh / 2, per = 2 * dk + dh, dt = e.dtype;
+    const int C = y.C, T = y.H * y.W, dh = C / nh, dk = dh / 2, per = 2 * dk + dh, dt = e.dtype, nb = e.batch;
     Tens qkv = e.talloc(y.H, y.W, nh * per);
     cbs(p + ".conv1.qkv", y, qkv, nh * per, 1, 1, false);
     Tens vc = e.talloc(y.H, y.W, C);
-    void* vt = e.dalloc(static_cast<size_t>(nh) * dh * T * 2);
+    void* vt = e.dalloc(static_cast<size_t>(nh) * dh * T * 2 * nb);          // [N][nh][dh][T]
     {
       const void* q = qkv.p; void* vcp = vc.p;
       e.op(p + ".split_v", [=](cudaStream_t st) {
-        const dim3 g((T * nh * dh + 255) / 256), b(256);
-        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(split_v_kernel<BF16>, g, b, 0, st, static_cast<const __nv_bfloat16*>(q), T, nh, dk, dh, static_cast<__nv_bfloat16*>(vcp), static_cast<__nv_bfloat16*>(vt)));
-        else VPB_CUDA_OK(launch_k(split_v_kernel<F16>, g, b, 0, st, static_cast<const __half*>(q), T, nh, dk, dh, static_cast<__half*>(vcp), static_cast<__half*>(vt)));
+        const dim3 g((T * nh * dh + 255) / 256, nb), b(256);
+        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? split_v_kernel<BF16, true> : split_v_kernel<BF16, false>, g, b, 0, st, static_cast<const __nv_bfloat16*>(q), T, nh, dk, dh, static_cast<__nv_bfloat16*>(vcp), static_cast<__nv_bfloat16*>(vt)));
+        else VPB_CUDA_OK(launch_k(nb > 1 ? split_v_kernel<F16, true> : split_v_kernel<F16, false>, g, b, 0, st, static_cast<const __half*>(q), T, nh, dk, dh, static_cast<__half*>(vcp), static_cast<__half*>(vt)));
         return VPB_OK;
       });
     }
@@ -522,27 +576,28 @@ struct ASBuilder {
     const float scale = 1.0f / std::sqrt(static_cast<float>(dk));
     for (int h = 0; h < nh && ok(); ++h) {
       // S = Q K^T: pixels = query tokens, Cin = dk (q channels of head h), "weights" = the k channels of every token
+      // of the same sample
       Tens s = e.talloc(1, T, T), pm = e.talloc(1, T, T);
       Tens q = qkv.slice(h * per, dk);
       Tens qv = q; qv.H = 1; qv.W = T;
       const void* kmat = static_cast<const uint8_t*>(qkv.p) + static_cast<size_t>(h * per + dk) * 2;
       rc = e.conv(p + ".attn.qk" + std::to_string(h), qv, s, T, 1, 1, kmat, nullptr, ACT_NONE, VPB_EPI_STORE, nullptr, ACT_NONE,
-                  /*ldw=*/qkv.ld);
+                  /*ldw=*/qkv.ld, /*w_img=*/T * qkv.ld);
       if (!ok()) return;
       {
         const void* sp = s.p; void* pp = pm.p;
         e.op(p + ".attn.softmax" + std::to_string(h), [=](cudaStream_t st) {
-          const dim3 g((T + 7) / 8), b(256);
-          if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(softmax_rows_kernel<BF16>, g, b, 0, st, static_cast<const __nv_bfloat16*>(sp), T, T, scale, static_cast<__nv_bfloat16*>(pp)));
-          else VPB_CUDA_OK(launch_k(softmax_rows_kernel<F16>, g, b, 0, st, static_cast<const __half*>(sp), T, T, scale, static_cast<__half*>(pp)));
+          const dim3 g((nb * T + 7) / 8), b(256);
+          if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(softmax_rows_kernel<BF16>, g, b, 0, st, static_cast<const __nv_bfloat16*>(sp), nb * T, T, scale, static_cast<__nv_bfloat16*>(pp)));
+          else VPB_CUDA_OK(launch_k(softmax_rows_kernel<F16>, g, b, 0, st, static_cast<const __half*>(sp), nb * T, T, scale, static_cast<__half*>(pp)));
           return VPB_OK;
         });
       }
-      // O = P V^T (+ depthwise term): Cin = key tokens, "weights" = Vt[h] [dh][T]
+      // O = P V^T (+ depthwise term): Cin = key tokens, "weights" = Vt[h] [dh][T] of the same sample
       Tens o = att.slice(h * dh, dh); o.H = 1; o.W = T;
       Tens r = dwv.slice(h * dh, dh); r.H = 1; r.W = T;
       rc = e.conv(p + ".attn.pv" + std::to_string(h), pm, o, dh, 1, 1, static_cast<const uint8_t*>(vt) + static_cast<size_t>(h) * dh * T * 2,
-                  nullptr, ACT_NONE, VPB_EPI_ADD, &r, ACT_NONE, /*ldw=*/T);
+                  nullptr, ACT_NONE, VPB_EPI_ADD, &r, ACT_NONE, /*ldw=*/T, /*w_img=*/nh * dh * T);
     }
     cbs(p + ".conv1.conv2", att, y, C, 1, 1, false, 0, VPB_EPI_ADD, &y);          // y = y + proj(attention)
     Tens f = e.talloc(y.H, y.W, 2 * C);
@@ -554,7 +609,7 @@ struct ASBuilder {
 static int as_build(vp_autospeed& e, const WeightMap& w) {
   ASBuilder b{e, w};
   const int W0 = kASW, H0 = kASH;
-  e.d_gap_scratch = static_cast<long long*>(e.dalloc(static_cast<size_t>(kGapReplicas) * 256 * 8 + 64));
+  e.d_gap_scratch = static_cast<long long*>(e.dalloc(static_cast<size_t>(kGapReplicas) * 256 * 8 * e.batch + 64));
   Tens x0; x0.p = e.d_canvas; x0.H = H0; x0.W = W0; x0.C = 8; x0.ld = 8;
   // ---- backbone (auto_speed_backbone.py:9-48)
   Tens p1 = e.talloc(H0 / 2, W0 / 2, 16);
@@ -627,15 +682,15 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   if (!b.ok()) return b.rc != VPB_OK ? b.rc : VPB_ERR_CUDA;
   // ---- decode (auto_speed_head.py:53-63)
   {
-    const int dt = e.dtype; float* raw = e.d_raw;
+    const int dt = e.dtype, nb = e.batch; float* raw = e.d_raw;
     int a0 = 0;
     const float strides[3] = {8.f, 16.f, 32.f};
     for (int i = 0; i < 3; ++i) {
       const void* lp = lv[i].p; const int h = lv[i].H, wd = lv[i].W, ld = lv[i].ld, off = a0; const float st_ = strides[i];
       e.op("head.decode" + std::to_string(i), [=](cudaStream_t st) {
-        const dim3 g((h * wd + 127) / 128), bb(128);
-        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(decode_kernel<BF16>, g, bb, 0, st, static_cast<const __nv_bfloat16*>(lp), h, wd, ld, st_, off, kNA, raw));
-        else VPB_CUDA_OK(launch_k(decode_kernel<F16>, g, bb, 0, st, static_cast<const __half*>(lp), h, wd, ld, st_, off, kNA, raw));
+        const dim3 g((h * wd + 127) / 128, nb), bb(128);
+        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? decode_kernel<BF16, true> : decode_kernel<BF16, false>, g, bb, 0, st, static_cast<const __nv_bfloat16*>(lp), h, wd, ld, st_, off, kNA, raw));
+        else VPB_CUDA_OK(launch_k(nb > 1 ? decode_kernel<F16, true> : decode_kernel<F16, false>, g, bb, 0, st, static_cast<const __half*>(lp), h, wd, ld, st_, off, kNA, raw));
         return VPB_OK;
       });
       a0 += h * wd;
@@ -648,31 +703,34 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   return VPB_OK;
 }
 
-static int as_launch_all(vp_autospeed& e, const uint8_t* src, int stride, cudaStream_t st) {
-  int rc = e.pre.launch(&src, 1, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr, st);
+static int as_launch_all(vp_autospeed& e, const uint8_t* const* srcs, int stride, cudaStream_t st) {
+  int rc = e.pre.launch(srcs, e.batch, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr, st);
   if (rc) return rc;
   for (auto& op : e.ops) { rc = op.launch(st); if (rc) return rc; }
   PostParams pp{};
   pp.raw = e.d_raw; pp.NA = kNA; pp.conf = e.conf; pp.iou = e.iou; pp.scale = e.scale; pp.pad_x = e.pad_x; pp.pad_y = e.pad_y;
   pp.orig_w = e.src_w; pp.orig_h = e.src_h; pp.max_cand = vp_autospeed::kMaxCand; pp.max_det = vp_autospeed::kMaxDet;
   pp.cand = e.d_cand; pp.order = e.d_order; pp.det = e.d_det; pp.counts = e.d_counts;
-  VPB_CUDA_OK(launch_k(postprocess_kernel, dim3(1), dim3(1024), static_cast<size_t>(vp_autospeed::kMaxCand), st, pp));
+  const size_t smem = vp_autospeed::kMaxCand;
+  if (e.batch > 1) VPB_CUDA_OK(launch_k(postprocess_kernel<true>, dim3(e.batch), dim3(1024), smem, st, pp));
+  else VPB_CUDA_OK(launch_k(postprocess_kernel<false>, dim3(1), dim3(1024), smem, st, pp));
   return VPB_OK;
 }
 
-// letterbox geometry (auto_speed_infer.py:31-43)
+// letterbox geometry (auto_speed_infer.py:31-43), shared by every sample of a call
 static int as_configure(vp_autospeed& e, int h, int w) {
   if (h == e.src_h && w == e.src_w) return VPB_OK;
   const double sc = std::min(static_cast<double>(kASW) / w, static_cast<double>(kASH) / h);
   const int nw = static_cast<int>(w * sc), nh = static_cast<int>(h * sc);
   if (nw < 1 || nh < 1) { vpb_set_error("autospeed: frame %dx%d too small", w, h); return VPB_ERR_ARG; }
   e.scale = static_cast<float>(sc); e.new_w = nw; e.new_h = nh; e.pad_x = (kASW - nw) / 2; e.pad_y = (kASH - nh) / 2;
-  e.pre.OW = nw; e.pre.OH = nh; e.pre.out_pitch = kASW; e.pre.out_x0 = e.pad_x; e.pre.out_y0 = e.pad_y; e.pre.out_c = 8;
+  e.pre.OW = nw; e.pre.OH = nh; e.pre.out_pitch = kASW; e.pre.out_rows = kASH; e.pre.out_x0 = e.pad_x; e.pre.out_y0 = e.pad_y;
+  e.pre.out_c = 8;
   e.pre.h = -1;                                                // force a table rebuild
   int rc = e.pre.configure(h, w, VPB_RESIZE_PIL_BILINEAR);
   if (rc) return rc;
-  // the canvas border is constant per geometry: gray everywhere, the pre-process overwrites the pasted region
-  const int npix = kASW * kASH;
+  // the canvas border is constant per geometry: gray everywhere (all samples), the pre-process overwrites the pasted region
+  const int npix = kASW * kASH * e.batch;
   if (e.dtype == VPB_BF16) fill_canvas_kernel<BF16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__nv_bfloat16*>(e.d_canvas), npix);
   else fill_canvas_kernel<F16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__half*>(e.d_canvas), npix);
   VPB_CUDA_OK(cudaGetLastError());
@@ -680,37 +738,41 @@ static int as_configure(vp_autospeed& e, int h, int w) {
   return VPB_OK;
 }
 
-static int as_enqueue(vp_autospeed& e, const uint8_t* src, int h, int w, int stride) {
+// Enqueue one call for the e.batch frames srcs[0 .. batch-1] (one geometry).
+static int as_enqueue(vp_autospeed& e, const uint8_t* const* srcs, int h, int w, int stride) {
   int rc = as_configure(e, h, w);
   if (rc) return rc;
+  FrameSrcs src{};
+  std::copy(srcs, srcs + e.batch, src.begin());
   return e.frame_graph.run(
-      e.stream, e.pre, e.dtype, h, w, stride, FrameSrcs{src}, [&](cudaStream_t st) { return as_launch_all(e, src, stride, st); },
+      e.stream, e.pre, e.dtype, h, w, stride, src, [&](cudaStream_t st) { return as_launch_all(e, src.data(), stride, st); },
       [&](cudaGraphExec_t x, cudaGraphNode_t n) {
-        return e.pre.update_graph_node(x, n, &src, 1, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
+        return e.pre.update_graph_node(x, n, src.data(), e.batch, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
       });
 }
 
-}  // namespace vpb
-
-// ====================================================================== C-ABI
-extern "C" int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtype, void* stream, vp_autospeed** out) {
+static int as_create(const char* who, const char* weights_vpw, int gpu_id, int dtype, void* stream, int batch,
+                     vp_autospeed** out) {
   if (!out) return VPB_ERR_ARG;
   *out = nullptr;
-  if (!weights_vpw || !weights_vpw[0]) { vpb_set_error("vp_autospeed_create: no checkpoint path"); return VPB_ERR_ARG; }
+  if (batch < 1 || batch > kMaxBatch) { vpb_set_error("%s: batch %d out of range (1..%d)", who, batch, kMaxBatch); return VPB_ERR_ARG; }
+  if (!weights_vpw || !weights_vpw[0]) { vpb_set_error("%s: no checkpoint path", who); return VPB_ERR_ARG; }
   std::unique_ptr<vp_autospeed> e(new vp_autospeed());
-  int rc = e->open("vp_autospeed_create", gpu_id, stream);
+  int rc = e->open(who, gpu_id, stream);
   if (rc) return rc;
   DeviceGuard guard(gpu_id);
   e->dtype = dtype == VPB_BF16 ? VPB_BF16 : VPB_F16;
-  e->d_canvas = e->dalloc(static_cast<size_t>(kASW) * kASH * 8 * 2);
-  e->d_raw = static_cast<float*>(e->dalloc(static_cast<size_t>(8) * kNA * 4));
-  e->h_raw = static_cast<float*>(e->halloc(static_cast<size_t>(8) * kNA * 4));
-  e->d_cand = static_cast<float*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxCand) * 6 * 4));
-  e->d_order = static_cast<int*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxCand) * 4));
-  e->d_det = static_cast<float*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4));
-  e->d_counts = static_cast<int*>(e->dalloc(64));
-  e->h_det = static_cast<float*>(e->halloc(static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4));
-  e->h_counts = static_cast<int*>(e->halloc(64));
+  e->batch = batch;
+  const size_t nb = batch;
+  e->d_canvas = e->dalloc(static_cast<size_t>(kASW) * kASH * 8 * 2 * nb);
+  e->d_raw = static_cast<float*>(e->dalloc(static_cast<size_t>(8) * kNA * 4 * nb));
+  e->h_raw = static_cast<float*>(e->halloc(static_cast<size_t>(8) * kNA * 4 * nb));
+  e->d_cand = static_cast<float*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxCand) * 6 * 4 * nb));
+  e->d_order = static_cast<int*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxCand) * 4 * nb));
+  e->d_det = static_cast<float*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4 * nb));
+  e->d_counts = static_cast<int*>(e->dalloc(64 * nb));
+  e->h_det = static_cast<float*>(e->halloc(static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4 * nb));
+  e->h_counts = static_cast<int*>(e->halloc(64 * nb));
   if (e->oom || !e->h_raw || !e->h_det || !e->h_counts) return VPB_ERR_CUDA;
   WeightMap w;
   rc = load_vpw(weights_vpw, w);
@@ -723,6 +785,48 @@ extern "C" int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtyp
   return VPB_OK;
 }
 
+// detections (and with raw the raw tensors) of every sample to the host buffers
+static int as_fetch(vp_autospeed* e, bool raw) {
+  const size_t nb = e->batch;
+  VPB_CUDA_OK(cudaMemcpyAsync(e->h_counts, e->d_counts, 8 * nb, cudaMemcpyDeviceToHost, e->stream));
+  VPB_CUDA_OK(cudaMemcpyAsync(e->h_det, e->d_det, static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4 * nb, cudaMemcpyDeviceToHost, e->stream));
+  if (raw) VPB_CUDA_OK(cudaMemcpyAsync(e->h_raw, e->d_raw, static_cast<size_t>(8) * kNA * 4 * nb, cudaMemcpyDeviceToHost, e->stream));
+  return VPB_OK;
+}
+
+static int as_infer_host(vp_autospeed* e, const uint8_t* const* frames, int n, int h, int w, int stride, int fetch_raw,
+                         const char* who) {
+  if (!frames_ok(e, frames, n, h, w, stride, who)) return VPB_ERR_ARG;
+  DeviceGuard guard(e->gpu_id);
+  FrameSrcs dev;
+  int rc = e->upload_frames(frames, n, h, w, stride, dev);
+  if (rc) return rc;
+  rc = as_enqueue(*e, dev.data(), h, w, w * 3);
+  if (rc) return rc;
+  rc = as_fetch(e, fetch_raw != 0);
+  if (rc) return rc;
+  VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
+  return VPB_OK;
+}
+
+static bool sample_ok(const vp_autospeed* e, int sample, const char* who) {
+  if (sample >= 0 && sample < e->batch) return true;
+  vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch);
+  return false;
+}
+
+}  // namespace vpb
+
+// ====================================================================== C-ABI
+extern "C" int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtype, void* stream, vp_autospeed** out) {
+  return as_create("vp_autospeed_create", weights_vpw, gpu_id, dtype, stream, 1, out);
+}
+
+extern "C" int vp_autospeed_create_batch(const char* weights_vpw, int gpu_id, int dtype, void* stream, int batch,
+                                         vp_autospeed** out) {
+  return as_create("vp_autospeed_create_batch", weights_vpw, gpu_id, dtype, stream, batch, out);
+}
+
 extern "C" void vp_autospeed_destroy(vp_autospeed* e) { delete e; }
 
 extern "C" int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float iou) {
@@ -733,31 +837,24 @@ extern "C" int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float io
   return VPB_OK;
 }
 
-static int as_fetch(vp_autospeed* e, bool raw) {
-  VPB_CUDA_OK(cudaMemcpyAsync(e->h_counts, e->d_counts, 8, cudaMemcpyDeviceToHost, e->stream));
-  VPB_CUDA_OK(cudaMemcpyAsync(e->h_det, e->d_det, static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4, cudaMemcpyDeviceToHost, e->stream));
-  if (raw) VPB_CUDA_OK(cudaMemcpyAsync(e->h_raw, e->d_raw, static_cast<size_t>(8) * kNA * 4, cudaMemcpyDeviceToHost, e->stream));
-  return VPB_OK;
+extern "C" int vp_autospeed_infer(vp_autospeed* e, const uint8_t* frame_host, int h, int w, int stride, int fetch_raw) {
+  return as_infer_host(e, &frame_host, 1, h, w, stride, fetch_raw, "vp_autospeed_infer");
 }
 
-extern "C" int vp_autospeed_infer(vp_autospeed* e, const uint8_t* frame_host, int h, int w, int stride, int fetch_raw) {
-  if (!e || !frame_host || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("vp_autospeed_infer: bad arguments"); return VPB_ERR_ARG; }
+extern "C" int vp_autospeed_infer_batch(vp_autospeed* e, const uint8_t* const* frames_host, int n, int h, int w, int stride,
+                                        int fetch_raw) {
+  return as_infer_host(e, frames_host, n, h, w, stride, fetch_raw, "vp_autospeed_infer_batch");
+}
+
+extern "C" int vp_autospeed_infer_device_batch(vp_autospeed* e, const uint8_t* const* frames_dev, int n, int h, int w,
+                                               int stride) {
+  if (!frames_ok(e, frames_dev, n, h, w, stride, "vp_autospeed_infer_device")) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  FrameSrcs dev;
-  int rc = e->upload_frames(&frame_host, 1, h, w, stride, dev);
-  if (rc) return rc;
-  rc = as_enqueue(*e, dev[0], h, w, w * 3);
-  if (rc) return rc;
-  rc = as_fetch(e, fetch_raw != 0);
-  if (rc) return rc;
-  VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return VPB_OK;
+  return as_enqueue(*e, frames_dev, h, w, stride);
 }
 
 extern "C" int vp_autospeed_infer_device(vp_autospeed* e, const uint8_t* frame_dev, int h, int w, int stride) {
-  if (!e || !frame_dev || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("vp_autospeed_infer_device: bad arguments"); return VPB_ERR_ARG; }
-  DeviceGuard guard(e->gpu_id);
-  return as_enqueue(*e, frame_dev, h, w, stride);
+  return vp_autospeed_infer_device_batch(e, &frame_dev, 1, h, w, stride);
 }
 
 extern "C" int vp_autospeed_sync(vp_autospeed* e, int fetch) {
@@ -768,25 +865,37 @@ extern "C" int vp_autospeed_sync(vp_autospeed* e, int fetch) {
   return VPB_OK;
 }
 
-extern "C" int vp_autospeed_detections(vp_autospeed* e, const float** det, int* n, int* n_candidates) {
+extern "C" int vp_autospeed_detections_at(vp_autospeed* e, int sample, const float** det, int* n, int* n_candidates) {
   if (!e || !det || !n) return VPB_ERR_ARG;
-  *det = e->h_det; *n = e->h_counts[0];
-  if (n_candidates) *n_candidates = e->h_counts[1];
+  if (!sample_ok(e, sample, "vp_autospeed_detections")) return VPB_ERR_ARG;
+  *det = e->h_det + static_cast<size_t>(sample) * vp_autospeed::kMaxDet * 6; *n = e->h_counts[2 * sample];
+  if (n_candidates) *n_candidates = e->h_counts[2 * sample + 1];
   return VPB_OK;
 }
 
-extern "C" int vp_autospeed_raw(vp_autospeed* e, const float** raw_host, const float** raw_dev, int* channels, int* anchors) {
+extern "C" int vp_autospeed_detections(vp_autospeed* e, const float** det, int* n, int* n_candidates) {
+  return vp_autospeed_detections_at(e, 0, det, n, n_candidates);
+}
+
+extern "C" int vp_autospeed_raw_at(vp_autospeed* e, int sample, const float** raw_host, const float** raw_dev, int* channels,
+                                   int* anchors) {
   if (!e) return VPB_ERR_ARG;
-  if (raw_host) *raw_host = e->h_raw;
-  if (raw_dev) *raw_dev = e->d_raw;
+  if (!sample_ok(e, sample, "vp_autospeed_raw")) return VPB_ERR_ARG;
+  const size_t off = static_cast<size_t>(sample) * 8 * kNA;
+  if (raw_host) *raw_host = e->h_raw + off;
+  if (raw_dev) *raw_dev = e->d_raw + off;
   if (channels) *channels = 4 + kNC;
   if (anchors) *anchors = kNA;
   return VPB_OK;
 }
 
+extern "C" int vp_autospeed_raw(vp_autospeed* e, const float** raw_host, const float** raw_dev, int* channels, int* anchors) {
+  return vp_autospeed_raw_at(e, 0, raw_host, raw_dev, channels, anchors);
+}
+
 extern "C" int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flops) {
   if (!e) return VPB_ERR_ARG;
-  if (n_launches) *n_launches = static_cast<int>(e->ops.size()) + 2;
+  if (n_launches) *n_launches = static_cast<int>(e->ops.size()) + 2;     // per call, whatever the batch
   if (flops) {
     double f = 0;
     for (const auto& op : e->ops) f += op.flops;       // build order: the same sum as accumulated while building
@@ -797,7 +906,7 @@ extern "C" int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flop
 
 extern "C" long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {
   if (!e || !name) return VPB_ERR_ARG;
-  auto it = e->taps.find(name);
-  if (it == e->taps.end()) { vpb_set_error("no tap '%s'", name); return VPB_ERR_ARG; }
-  return e->read_tap(it->second.t, it->second.channels, dst, cap, c, h, w);
+  Tap a;
+  if (!e->find_tap(name, &a)) return VPB_ERR_ARG;
+  return e->read_tap(a.t, a.channels, dst, cap, c, h, w);
 }

@@ -17,7 +17,8 @@
 //   is ONE GEMM: the skip tensor is a second K segment read at output resolution through a TMA box with
 //   element stride 2 (every second pixel = one phase) into the same accumulator.
 //   Batch: both activation maps are 4-D [image][row][column][channel]; the tile index is image-major, no tile
-//   straddles two images, and the weight tiles are the same for every image.
+//   straddles two images, and the weight tiles are the same for every image (w_img: the weight map's third
+//   dimension is the image, for attention operands that are activations).
 //   "upconv": ConvTranspose2d(k2,s2) [+ Conv1x1 skip] and the Conv3x3 that follows, composed at load time into
 //   ONE GEMM over the low-resolution tensor (weights from upconv_compose.cu): four 2x2 taps per output phase +
 //   nine skip taps, and a bias that depends on which 3x3 taps fall inside the image (9 border classes).
@@ -417,7 +418,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
       for (int t = 0; t < p.taps; ++t) {
         const int dy = (p.taps == 9) ? (t / 3 - 1) : 0;
         const int dx = (p.taps == 9) ? (t % 3 - 1) : 0;
-        const int wsel = (p.phases > 1) ? ph : t;
+        const int wsel = p.w_img ? img : (p.phases > 1) ? ph : t;
         for (int c = 0; c < p.kchunks; ++c) {
           for (int seg = 0; seg < nseg; ++seg) {
             const CUtensorMap* mA = seg == 1 ? &maps.Alo : &mapA;
@@ -681,6 +682,17 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
   }
   if (a->batch < 0) { vpb_set_error("conv: batch %d", a->batch); return VPB_ERR_ARG; }
   const int batch = a->batch > 0 ? a->batch : 1;
+  if (a->w_img != 0) {
+    const long ldw = a->ldw > 0 ? a->ldw : a->Cin;
+    const char* why = a->algo == VPB_ALGO_LINEAR ? "the LINEAR algorithm has one weight operand"
+                      : a->taps * a->phases != 1 ? "taps * phases must be 1"
+                      : a->in2 ? "no second input"
+                      : a->in_lo ? "no split-fp16 mode"
+                      : (a->w_img & 7) ? "w_img must be a multiple of 8"
+                      : a->w_img < ldw * a->Cout ? "w_img < ldw * Cout: the images' weight operands overlap"
+                      : nullptr;
+    if (why) { vpb_set_error("conv: per-image weights (w_img=%d): %s", a->w_img, why); return VPB_ERR_ARG; }
+  }
   {
     // the epilogue addresses pixels with 32-bit element offsets, across the whole batch
     const long ho = a->phases == 4 ? 2L * a->H + 2 : a->H + 2, wo = a->phases == 4 ? 2L * a->W + 2 : a->W + 2;
@@ -702,6 +714,7 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
   p.in_pad = a->in_pad ? 1 : 0; p.out_pad = a->out_pad ? 1 : 0; p.res_pad = a->res_pad ? 1 : 0;
   p.lin = (lin && a->out_pad && a->mode != VPB_EPI_FINAL) ? 1 : 0;
   p.split = split ? 1 : 0;
+  p.w_img = a->w_img != 0 ? 1 : 0;
   p.stride = cstride; p.act2 = a->act2;
   p.nlim = a->out_slice ? std::min(a->ldo, (a->Cout + 7) / 8 * 8) : a->ldo;
   p.out_lo = a->out_lo; p.res_lo = a->res_lo;
@@ -779,10 +792,12 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
   }
   {
     auto encB = [&](const void* ptr, CUtensorMap* m) {
+      // w_img != 0: the third dimension is the image instead of the tap / phase
       const size_t ldw = a->ldw > 0 ? a->ldw : a->Cin;
       cuuint64_t dims[3] = {static_cast<cuuint64_t>(a->Cin), static_cast<cuuint64_t>(a->Cout),
-                            static_cast<cuuint64_t>(a->taps * a->phases)};
-      cuuint64_t strides[2] = {static_cast<cuuint64_t>(ldw) * 2, static_cast<cuuint64_t>(ldw) * 2 * a->Cout};
+                            static_cast<cuuint64_t>(a->w_img ? batch : a->taps * a->phases)};
+      cuuint64_t strides[2] = {static_cast<cuuint64_t>(ldw) * 2,
+                               a->w_img ? static_cast<cuuint64_t>(a->w_img) * 2 : static_cast<cuuint64_t>(ldw) * 2 * a->Cout};
       cuuint32_t box[3] = {64, static_cast<cuuint32_t>(p.BN), 1};
       cuuint32_t es[3] = {1, 1, 1};
       return enc(m, dt, 3, const_cast<void*>(ptr), dims, strides, box, es,

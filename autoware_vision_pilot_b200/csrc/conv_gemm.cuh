@@ -40,6 +40,7 @@ struct ConvKParams {
   int ldr;
   float* out_f32;
   uint8_t* out_cls;
+  int w_img;                     // 1: the weight map's third dimension is the image (a weight operand per image)
 };
 
 // Tensor maps of the kernel, passed as ONE __grid_constant__ parameter (TMA reads them from param space).

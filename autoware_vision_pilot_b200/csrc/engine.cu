@@ -65,9 +65,6 @@ using namespace vpb;
 struct vp_engine : EngineRuntime {
   vp_engine_config cfg{};
   void* d_pre_lo = nullptr;
-  // frames per call (vp_engine_config.batch): every activation, the pre-process output and the model outputs hold
-  // `batch` samples back to back (batch outermost); weights, the launch list and the graph are those of one call
-  int batch = 1;
   PreprocessPlan pre;
   uint8_t* h_frame = nullptr; size_t h_frame_cap = 0;
   void* d_pre = nullptr;                  // [320][640][4]
@@ -711,19 +708,6 @@ extern "C" uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes) {
   return e->h_frame;
 }
 
-// n frames of one geometry, n == the engine's batch
-static bool frames_ok(const vp_engine* e, const uint8_t* const* frames, int n, int h, int w, int stride, const char* who) {
-  if (!e || !frames || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("%s: bad arguments", who); return false; }
-  if (n != e->batch) {
-    vpb_set_error("%s: %d frame(s) for an engine of batch %d%s", who, n, e->batch,
-                  n == 1 ? " (use the *_batch calls)" : "");
-    return false;
-  }
-  for (int k = 0; k < n; ++k)
-    if (!frames[k]) { vpb_set_error("%s: frame %d is NULL", who, k); return false; }
-  return true;
-}
-
 extern "C" int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev, int n, int h, int w, int stride) {
   if (!frames_ok(e, frames_dev, n, h, w, stride, "vp_engine_infer_device")) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
@@ -880,37 +864,17 @@ extern "C" int vp_engine_read_resized(vp_engine* e, uint8_t* dst) {
   return VPB_OK;
 }
 
-// Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
-static bool find_tap(const vp_engine* e, const char* name, Tap* out) {
-  std::string nm(name);
-  int k = 0;
-  const size_t at = nm.find('@');
-  if (at != std::string::npos) {
-    const std::string ks = nm.substr(at + 1);
-    char* end = nullptr;
-    const long v = ks.empty() ? -1 : strtol(ks.c_str(), &end, 10);
-    if (v < 0 || v >= e->batch || *end) { vpb_set_error("tap '%s': sample out of range (batch %d)", name, e->batch); return false; }
-    k = static_cast<int>(v);
-    nm.resize(at);
-  }
-  auto it = e->taps.find(nm);
-  if (it == e->taps.end()) { vpb_set_error("no tap '%s'", name); return false; }
-  *out = it->second;
-  out->t.p = static_cast<uint8_t*>(out->t.p) + out->t.bytes() * k;    // split-fp16 engines (lo != NULL) have batch 1
-  return true;
-}
-
 extern "C" long vp_engine_read_tap(vp_engine* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {
   if (!e || !name) return VPB_ERR_ARG;
   Tap a;
-  if (!find_tap(e, name, &a)) return VPB_ERR_ARG;
+  if (!e->find_tap(name, &a)) return VPB_ERR_ARG;
   return e->read_tap(a.t, a.channels, dst, cap, c, h, w);
 }
 
 extern "C" int vp_engine_tap_dev(vp_engine* e, const char* name, vp_tap_view* v) {
   if (!e || !name || !v) return VPB_ERR_ARG;
   Tap a;
-  if (!find_tap(e, name, &a)) return VPB_ERR_ARG;
+  if (!e->find_tap(name, &a)) return VPB_ERR_ARG;
   v->data = a.t.p; v->height = a.t.H; v->width = a.t.W; v->channels = a.t.C; v->ld = a.t.ld; v->pad = a.t.pad;
   v->dtype = e->dtype;
   return VPB_OK;

@@ -4,6 +4,7 @@
 #include "engine_internal.h"
 
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 
 namespace vpb {
@@ -243,6 +244,18 @@ int EngineRuntime::append_conv(const std::string& name, const vpb_conv_args& a, 
   return VPB_OK;
 }
 
+bool frames_ok(const EngineRuntime* e, const uint8_t* const* frames, int n, int h, int w, int stride, const char* who) {
+  if (!e || !frames || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("%s: bad arguments", who); return false; }
+  if (n != e->batch) {
+    vpb_set_error("%s: %d frame(s) for an engine of batch %d%s", who, n, e->batch,
+                  n == 1 ? " (use the *_batch calls)" : "");
+    return false;
+  }
+  for (int k = 0; k < n; ++k)
+    if (!frames[k]) { vpb_set_error("%s: frame %d is NULL", who, k); return false; }
+  return true;
+}
+
 int EngineRuntime::upload_frames(const uint8_t* const* frames, int n, int h, int w, int stride, FrameSrcs& dev) {
   const int dpitch = w * 3;
   const size_t bytes = static_cast<size_t>(h) * dpitch;
@@ -298,6 +311,25 @@ long EngineRuntime::read_tap(const Tens& t, int channels, float* dst, long cap, 
   if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream);
   if (ce != cudaSuccess) { vpb_set_error("read_tap: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
   return n;
+}
+
+bool EngineRuntime::find_tap(const char* name, Tap* out) const {
+  std::string nm(name);
+  int k = 0;
+  const size_t at = nm.find('@');
+  if (at != std::string::npos) {
+    const std::string ks = nm.substr(at + 1);
+    char* end = nullptr;
+    const long v = ks.empty() ? -1 : strtol(ks.c_str(), &end, 10);
+    if (v < 0 || v >= batch || *end) { vpb_set_error("tap '%s': sample out of range (batch %d)", name, batch); return false; }
+    k = static_cast<int>(v);
+    nm.resize(at);
+  }
+  auto it = taps.find(nm);
+  if (it == taps.end()) { vpb_set_error("no tap '%s'", name); return false; }
+  *out = it->second;
+  out->t.p = static_cast<uint8_t*>(out->t.p) + out->t.bytes() * k;    // split-fp16 engines (lo != NULL) have batch 1
+  return true;
 }
 
 }  // namespace vpb

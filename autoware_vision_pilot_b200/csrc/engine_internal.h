@@ -94,6 +94,9 @@ struct ConvPlan;
 // What every engine owns: its device and stream, device / pinned allocations, the op list and the frame graph.
 struct EngineRuntime {
   int gpu_id = 0, dtype = VPB_F16;
+  // frames per call: every per-frame buffer holds `batch` samples back to back (sample outermost); weights, the launch
+  // list and the graph are those of one call
+  int batch = 1;
   cudaStream_t stream = nullptr; bool own_stream = false;
   bool oom = false;                       // a device allocation failed during construction (the create call reports it)
   bool split = false;                     // VP_PREC_SPLIT: every 16-bit tensor is a (hi, lo) pair, GEMMs run 3 K segments
@@ -129,6 +132,11 @@ struct EngineRuntime {
   int upload_frames(const uint8_t* const* frames, int n, int h, int w, int stride, FrameSrcs& dev);
   // the first `channels` channels of t as fp32 [channels][H][W] into dst (NULL: size query); element count or < 0
   long read_tap(const Tens& t, int channels, float* dst, long cap, int* c, int* h, int* w);
+  // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
+  bool find_tap(const char* name, Tap* out) const;
 };
+
+// n frames of one geometry, n == e's batch (who names the call in the error message)
+bool frames_ok(const EngineRuntime* e, const uint8_t* const* frames, int n, int h, int w, int stride, const char* who);
 
 }  // namespace vpb

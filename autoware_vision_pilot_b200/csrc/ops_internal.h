@@ -25,14 +25,14 @@ struct PreprocessPlan {
   int device = -1;                   // device that owns d_tables
   void* out_lo = nullptr;            // split-fp16 mode: low half of the output tensor (set once by the engine)
   // output canvas (letterbox, auto_speed_infer.py:24-45): the OW x OH resized image is pasted at (out_x0, out_y0) of a
-  // canvas with out_pitch pixels per row (0 = OW) and out_c channels per pixel (4 | 8)
-  int out_pitch = 0, out_x0 = 0, out_y0 = 0, out_c = 4;
+  // canvas of out_rows rows (0 = OH) with out_pitch pixels per row (0 = OW) and out_c channels per pixel (4 | 8); a batch
+  // holds whole canvases back to back
+  int out_pitch = 0, out_x0 = 0, out_y0 = 0, out_c = 4, out_rows = 0;
   size_t smem_bytes = 0;
   int* d_tables = nullptr;
   size_t off_xb = 0, off_xk = 0, off_yb = 0, off_yk = 0;
   int configure(int in_h, int in_w, int mode);
-  // srcs[0 .. batch-1]: one frame each, same geometry; out / out_u8 hold `batch` images back to back (network-sized
-  // canvases: out_pitch = 0, no paste offset)
+  // srcs[0 .. batch-1]: one frame each, same geometry; out / out_u8 hold `batch` images back to back (16-bit mode only)
   int launch(const uint8_t* const* srcs, int batch, int stride, int convention, int dtype, void* out, uint8_t* out_u8,
              cudaStream_t stream) const;
   bool owns_kernel(const void* func, int dtype) const;

@@ -374,8 +374,8 @@ PreprocessPlan::~PreprocessPlan() {
 
 static int fill_params(const PreprocessPlan& pl, const uint8_t* const* srcs, int batch, int stride, int convention,
                        void* out, uint8_t* out_u8, PreParams& p) {
-  if (batch < 1 || batch > kMaxBatch || (batch > 1 && (pl.out_lo || pl.out_pitch > 0 || pl.out_x0 || pl.out_y0))) {
-    vpb_set_error("preprocess: batch %d (1..%d, 16-bit network-sized output only)", batch, kMaxBatch);
+  if (batch < 1 || batch > kMaxBatch || (batch > 1 && pl.out_lo)) {
+    vpb_set_error("preprocess: batch %d (1..%d, 16-bit output only)", batch, kMaxBatch);
     return VPB_ERR_ARG;
   }
   p.out_lo = pl.out_lo;
@@ -383,7 +383,7 @@ static int fill_params(const PreprocessPlan& pl, const uint8_t* const* srcs, int
   p.out_c = pl.out_c;
   for (int i = 0; i < kMaxBatch; ++i) p.src[i] = srcs[i < batch ? i : 0];
   p.h = pl.h; p.w = pl.w; p.stride = stride; p.mode = pl.mode;
-  p.out_img = static_cast<size_t>(pl.OH) * pl.OW * pl.out_c;
+  p.out_img = static_cast<size_t>(pl.out_rows > 0 ? pl.out_rows : pl.OH) * p.out_pitch * pl.out_c;   // whole canvases
   // conventions: see include/vp_b200_ops.h
   static const float kMeanRGB[3] = {0.485f, 0.456f, 0.406f}, kStdRGB[3] = {0.229f, 0.224f, 0.225f};
   p.swap_rb = convention == VPB_CONV_BGR_SWAP ? 1 : 0;

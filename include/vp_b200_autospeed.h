@@ -10,6 +10,15 @@
  *                             un-letterbox + clamp (:100-106)
  *   vp_autospeed_detections   the list the helper returns: [[x1, y1, x2, y2, score, class], ...] in source-frame pixels
  *   vp_autospeed_raw          the network's raw prediction tensor [1, 4 + nc, 10752] (auto_speed_head.py:63)
+ *   vp_autospeed_*_batch, *_at  N calls of the helper's inference (the reference has no batch call); the batch-N forward
+ *                             of the network [N, 4 + nc, 10752], whose samples the module computes independently
+ *
+ * Batch contract: vp_autospeed_create_batch(..., batch = N) builds an engine that evaluates exactly N frames of one
+ * geometry per call, through one launch list, one weight copy and one graph replay (the launch count per call does not
+ * depend on N).  Every per-frame buffer holds N samples, sample outermost; sample k's raw tensor, detections and taps
+ * are bit-identical to a batch-1 engine's on frame k.  Batched engines take the *_batch calls only; the single-frame
+ * calls, a frame count other than N and a sample outside 0..N-1 return VPB_ERR_ARG.  vp_autospeed_create is batch 1.
+ * The thresholds are shared by all samples.
  *
  * The checkpoint is a .vpw file holding the module's state_dict (python -m autoware_vision_pilot_b200.convert);
  * BatchNorm (eps 1e-3) is folded at load.  16-bit operands on the wgmma tensor cores, fp32 accumulation, exactly
@@ -30,6 +39,8 @@ typedef struct vp_autospeed vp_autospeed;
 
 int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtype /* VPB_F16 | VPB_BF16 */, void* stream,
                         vp_autospeed** out);
+/* batch 1..VP_MAX_BATCH (vp_b200.h) frames per call; VPB_ERR_ARG otherwise, before the device is opened */
+int vp_autospeed_create_batch(const char* weights_vpw, int gpu_id, int dtype, void* stream, int batch, vp_autospeed** out);
 void vp_autospeed_destroy(vp_autospeed* e);
 /* conf_thres / iou_thres of post_process_predictions (defaults 0.6 / 0.45, auto_speed_infer.py:71) */
 int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float iou);
@@ -39,7 +50,11 @@ int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float iou);
 int vp_autospeed_infer(vp_autospeed* e, const uint8_t* frame_host_rgb, int h, int w, int stride, int fetch_raw);
 /* Same work for a frame already in device memory, only enqueued on the engine's stream. */
 int vp_autospeed_infer_device(vp_autospeed* e, const uint8_t* frame_dev_rgb, int h, int w, int stride);
-/* Drain the stream; fetch: 0 nothing, 1 detections, 2 detections + raw tensor to the host buffers. */
+/* The same two calls for n == batch frames of one geometry (h, w, stride); frame k becomes sample k. */
+int vp_autospeed_infer_batch(vp_autospeed* e, const uint8_t* const* frames_host_rgb, int n, int h, int w, int stride,
+                             int fetch_raw);
+int vp_autospeed_infer_device_batch(vp_autospeed* e, const uint8_t* const* frames_dev_rgb, int n, int h, int w, int stride);
+/* Drain the stream; fetch: 0 nothing, 1 detections, 2 detections + raw tensor to the host buffers (all samples). */
 int vp_autospeed_sync(vp_autospeed* e, int fetch);
 
 /* det: engine-owned host buffer [n][6] = x1, y1, x2, y2, score, class (descending score, as torchvision.ops.nms
@@ -47,9 +62,14 @@ int vp_autospeed_sync(vp_autospeed* e, int fetch);
 int vp_autospeed_detections(vp_autospeed* e, const float** det, int* n, int* n_candidates);
 /* raw prediction tensor, fp32 planar [channels = 8][anchors = 10752]: cx, cy, w, h (canvas pixels), 4 class scores */
 int vp_autospeed_raw(vp_autospeed* e, const float** raw_host, const float** raw_dev, int* channels, int* anchors);
+/* the same for sample 0..batch-1 (the two calls above return sample 0) */
+int vp_autospeed_detections_at(vp_autospeed* e, int sample, const float** det, int* n, int* n_candidates);
+int vp_autospeed_raw_at(vp_autospeed* e, int sample, const float** raw_host, const float** raw_dev, int* channels,
+                        int* anchors);
+/* launches per call (any batch) and the FLOPs of all samples of a call */
 int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flops);
-/* intermediate tensors for the parity tests ("canvas", "p1".."p5", "p5_ctx", "p5_sppf", "n3".."n5", "head0".."head2")
- * as fp32 NCHW; returns the element count (dst == NULL: size query) */
+/* intermediate tensors for the parity tests ("canvas", "p1".."p5", "p5_ctx", "p5_sppf", "n3".."n5", "head0".."head2";
+ * "<name>@k" = sample k, default 0) as fp32 NCHW; returns the element count (dst == NULL: size query) */
 long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* dst, long cap, int* c, int* h, int* w);
 
 #ifdef __cplusplus

@@ -126,9 +126,14 @@ typedef struct {
   int taps2;
   /* Images per call (0 = 1).  in / out / res / in2 (and the split-mode low halves) hold `batch` images back to back,
    * each with the layout the fields above describe (zero-bordered or not); FINAL outputs are out_f32
-   * [batch][Cout][H][W] and out_cls [batch][H][W].  Every image sees the same weights, and its outputs are
-   * bit-identical to a call on that image alone. */
+   * [batch][Cout][H][W] and out_cls [batch][H][W].  Every image sees the same weights (unless w_img), and its outputs
+   * are bit-identical to a call on that image alone. */
   int batch;
+  /* Elements between consecutive images' weight operands (0 = every image shares w).  Non-zero: image k of the batch
+   * reads its weights at w + k * w_img (ldw still separates output-channel rows), so a per-image activation can act
+   * as the weight matrix (the detector's batched attention: S = Q K^T, O = P V^T).  Needs taps * phases == 1, the
+   * TILE algorithm, no in2, no split mode, a multiple of 8 and w_img >= ldw * Cout (images may not overlap). */
+  int w_img;
 } vpb_conv_args;
 int vpb_conv_gemm(const vpb_conv_args* a, void* stream);
 /* Composition of the upconv operands on the device (all pointers device fp32, outputs may be NULL to skip):

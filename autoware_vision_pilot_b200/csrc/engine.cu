@@ -696,6 +696,7 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
 extern "C" void vp_engine_destroy(vp_engine* e) { delete e; }   // ~vp_engine switches to the engine's device
 
 extern "C" int vp_engine_num_models(const vp_engine* e) { return e ? static_cast<int>(e->outs.size()) : 0; }
+int vpb_engine_batch(const vp_engine* e) { return e ? e->batch : 0; }
 
 extern "C" uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes) {
   if (!e) return nullptr;

@@ -140,3 +140,7 @@ struct EngineRuntime {
 bool frames_ok(const EngineRuntime* e, const uint8_t* const* frames, int n, int h, int w, int stride, const char* who);
 
 }  // namespace vpb
+
+// frames per call of a segmentation engine (engine.cu), for callers that see vp_engine only as an opaque type
+struct vp_engine;
+int vpb_engine_batch(const vp_engine* e);

@@ -8,6 +8,8 @@
 //   fuse_kernel           Estimator predict (estimator.cpp:15-22) + Estimator::update (estimator.cpp:24-74)
 //                         with every camera's measurement in rank order
 // NCCL is resolved with dlopen at first use so that the library has no link-time NCCL dependency.
+// Local mode (vp_multicam_create_local): n cameras on one GPU.  The pack launch fills all n slots (blockIdx.y =
+// camera) in the same gathered layout, there is no collective, and the same fuse kernel runs with world = n.
 #include "common.cuh"
 #include "ops_internal.h"
 #include "engine_internal.h"
@@ -69,14 +71,21 @@ static NcclApi* nccl_api() {
     }                                                                                   \
   } while (0)
 
-// one 16-byte word per thread; the measurement rides at the end of the same launch
-__global__ void pack_payload_kernel(const uint4* __restrict__ feat, const double* __restrict__ meas,
-                                    uint8_t* __restrict__ slot) {
+struct PackFeats { const uint4* p[kMaxBatch]; };   // per-camera feature maps, by value
+
+// Camera k = blockIdx.y: its features into slot k, one 16-byte word per thread, and its measurement (meas +
+// k * meas_stride doubles) at the end of the slot in the same launch.  One camera (gridDim.y = 1) is the NCCL mode's
+// pack into the rank's own slot.
+__global__ void pack_payload_kernel(const __grid_constant__ PackFeats feats, const double* __restrict__ meas,
+                                    size_t meas_stride, uint8_t* __restrict__ slots) {
+  const int k = blockIdx.y;
+  const uint4* __restrict__ feat = feats.p[k];
+  uint8_t* slot = slots + static_cast<size_t>(k) * VP_MC_PAYLOAD_BYTES;
   const int n16 = VP_MC_FEAT_BYTES / 16;
   uint4* dst = reinterpret_cast<uint4*>(slot);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += gridDim.x * blockDim.x) dst[i] = feat[i];
   if (blockIdx.x == 0 && threadIdx.x < VP_MC_STATE_DIM * 2)
-    reinterpret_cast<double*>(slot + VP_MC_FEAT_BYTES)[threadIdx.x] = meas[threadIdx.x];
+    reinterpret_cast<double*>(slot + VP_MC_FEAT_BYTES)[threadIdx.x] = meas[k * meas_stride + threadIdx.x];
 }
 
 // Estimator::predict (variance += process-noise variance, estimator.cpp:15-22; PathFinder uses
@@ -122,6 +131,7 @@ using namespace vpb;
 
 struct vp_multicam {
   int rank = 0, world = 1, gpu_id = 0;
+  bool local = false;              // vp_multicam_create_local: world = cameras on this GPU, no communicator
   ncclComm_t_ comm = nullptr;
   bool own_comm = false;
   cudaStream_t stream = nullptr;
@@ -202,6 +212,26 @@ static int multicam_create_common(void* comm, const uint8_t* id128, int rank, in
 extern "C" int vp_multicam_create(const uint8_t* id128, int rank, int world, int gpu_id, void* stream, vp_multicam** out) {
   return multicam_create_common(nullptr, id128, rank, world, gpu_id, stream, out);
 }
+extern "C" int vp_multicam_create_local(int n_cameras, int gpu_id, void* stream, vp_multicam** out) {
+  if (!out || n_cameras < 1 || n_cameras > kMaxBatch) {
+    vpb_set_error("vp_multicam_create_local: %d cameras (1..%d)%s", n_cameras, kMaxBatch, out ? "" : ", NULL out");
+    return VPB_ERR_ARG;
+  }
+  *out = nullptr;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || gpu_id < 0 || gpu_id >= ndev) {
+    vpb_set_error("vp_multicam_create_local: no CUDA device %d (there is no CPU fallback)", gpu_id);
+    return VPB_ERR_CUDA;
+  }
+  DeviceGuard g(gpu_id);
+  vp_multicam* mc = new vp_multicam();
+  mc->rank = 0; mc->world = n_cameras; mc->gpu_id = gpu_id; mc->local = true;
+  int rc = multicam_alloc(mc, stream);
+  if (rc) { vp_multicam_destroy(mc); return rc; }
+  *out = mc;
+  return VPB_OK;
+}
+
 extern "C" int vp_multicam_create_with_comm(void* nccl_comm, int rank, int world, int gpu_id, void* stream, vp_multicam** out) {
   if (!nccl_comm) { vpb_set_error("vp_multicam_create_with_comm: NULL communicator"); return VPB_ERR_ARG; }
   return multicam_create_common(nccl_comm, nullptr, rank, world, gpu_id, stream, out);
@@ -223,33 +253,65 @@ static int multicam_allgather(vp_multicam* mc) {
   return VPB_OK;
 }
 
-extern "C" int vp_multicam_step(vp_multicam* mc, const void* feat_dev, const double* meas_dev, int predict) {
-  if (!mc || !feat_dev || !meas_dev) { vpb_set_error("vp_multicam_step: bad arguments"); return VPB_ERR_ARG; }
-  if (reinterpret_cast<uintptr_t>(feat_dev) & 15) { vpb_set_error("vp_multicam_step: features must be 16-byte aligned"); return VPB_ERR_ARG; }
+// pack -> [all-gather] -> fuse.  Camera k's features are feats.p[k] (16-byte aligned), its measurement
+// meas + k * meas_stride doubles.
+static int multicam_pack_fuse(vp_multicam* mc, const PackFeats& feats, const double* meas, size_t meas_stride,
+                              int predict, const char* who) {
+  for (int k = 0; k < (mc->local ? mc->world : 1); ++k)
+    if (reinterpret_cast<uintptr_t>(feats.p[k]) & 15) {
+      vpb_set_error("%s: features must be 16-byte aligned", who);
+      return VPB_ERR_ARG;
+    }
   DeviceGuard g(mc->gpu_id);
-  uint8_t* slot = mc->d_gather + static_cast<size_t>(mc->rank) * VP_MC_PAYLOAD_BYTES;
-  pack_payload_kernel<<<132, 256, 0, mc->stream>>>(static_cast<const uint4*>(feat_dev), meas_dev, slot);
-  VPB_CUDA_OK(cudaGetLastError());
-  int rc = multicam_allgather(mc);
-  if (rc) return rc;
+  if (mc->local) {
+    pack_payload_kernel<<<dim3(132, mc->world), 256, 0, mc->stream>>>(feats, meas, meas_stride, mc->d_gather);
+    VPB_CUDA_OK(cudaGetLastError());
+  } else {
+    uint8_t* slot = mc->d_gather + static_cast<size_t>(mc->rank) * VP_MC_PAYLOAD_BYTES;
+    pack_payload_kernel<<<132, 256, 0, mc->stream>>>(feats, meas, meas_stride, slot);
+    VPB_CUDA_OK(cudaGetLastError());
+    int rc = multicam_allgather(mc);
+    if (rc) return rc;
+  }
   multicam_fuse_kernel<<<1, 32, 0, mc->stream>>>(mc->d_state, mc->d_gather, VP_MC_PAYLOAD_BYTES, mc->world, predict);
   VPB_CUDA_OK(cudaGetLastError());
   return VPB_OK;
 }
 
+extern "C" int vp_multicam_step(vp_multicam* mc, const void* feat_dev, const double* meas_dev, int predict) {
+  if (!mc || !feat_dev || !meas_dev) { vpb_set_error("vp_multicam_step: bad arguments"); return VPB_ERR_ARG; }
+  PackFeats feats{};
+  for (int k = 0; k < (mc->local ? mc->world : 1); ++k)     // local mode: the n feature maps back to back
+    feats.p[k] = reinterpret_cast<const uint4*>(static_cast<const uint8_t*>(feat_dev) +
+                                                static_cast<size_t>(k) * VP_MC_FEAT_BYTES);
+  return multicam_pack_fuse(mc, feats, meas_dev, VP_MC_STATE_DIM * 2, predict, "vp_multicam_step");
+}
+
 extern "C" int vp_multicam_step_engine(vp_multicam* mc, vp_engine* e, int model_idx, const vpb_lateral_out* lat,
                                        int predict) {
   if (!mc || !e || !lat) { vpb_set_error("vp_multicam_step_engine: bad arguments"); return VPB_ERR_ARG; }
-  char name[32];
-  snprintf(name, sizeof(name), "%d/fused", model_idx);
-  vp_tap_view tv;
-  int rc = vp_engine_tap_dev(e, name, &tv);
-  if (rc) return rc;
-  if (tv.pad || static_cast<size_t>(tv.height) * tv.width * tv.ld * 2 != VP_MC_FEAT_BYTES) {
-    vpb_set_error("vp_multicam_step_engine: tensor '%s' is not the [10][20][1456] fused feature map", name);
+  if (mc->local && vpb_engine_batch(e) != mc->world) {
+    vpb_set_error("vp_multicam_step_engine: engine of batch %d for %d cameras", vpb_engine_batch(e), mc->world);
     return VPB_ERR_ARG;
   }
-  return vp_multicam_step(mc, tv.data, &lat->pf_meas[0][0], predict);
+  PackFeats feats{};
+  for (int k = 0; k < (mc->local ? mc->world : 1); ++k) {   // NCCL mode: "<idx>/fused" of the rank's single frame
+    char name[32];
+    if (mc->local) snprintf(name, sizeof(name), "%d/fused@%d", model_idx, k);
+    else snprintf(name, sizeof(name), "%d/fused", model_idx);
+    vp_tap_view tv;
+    int rc = vp_engine_tap_dev(e, name, &tv);
+    if (rc) return rc;
+    if (tv.pad || static_cast<size_t>(tv.height) * tv.width * tv.ld * 2 != VP_MC_FEAT_BYTES) {
+      vpb_set_error("vp_multicam_step_engine: tensor '%s' is not the [10][20][1456] fused feature map", name);
+      return VPB_ERR_ARG;
+    }
+    feats.p[k] = static_cast<const uint4*>(tv.data);
+  }
+  // camera k's measurement is the pf_meas of record k: records are sizeof(vpb_lateral_out) bytes apart
+  static_assert(sizeof(vpb_lateral_out) % sizeof(double) == 0, "vpb_lateral_out is a whole number of doubles");
+  return multicam_pack_fuse(mc, feats, &lat->pf_meas[0][0], sizeof(vpb_lateral_out) / sizeof(double), predict,
+                            "vp_multicam_step_engine");
 }
 
 extern "C" int vp_multicam_sync(vp_multicam* mc) {
@@ -282,6 +344,10 @@ extern "C" int vp_multicam_read(vp_multicam* mc, void* feats_host, double* meas_
 
 extern "C" int vp_multicam_time_allgather(vp_multicam* mc, int reps, float* ms_total) {
   if (!mc || reps <= 0 || !ms_total) return VPB_ERR_ARG;
+  if (mc->local) {
+    vpb_set_error("vp_multicam_time_allgather: a local (single-GPU) vp_multicam has no all-gather");
+    return VPB_ERR_STATE;
+  }
   DeviceGuard g(mc->gpu_id);
   cudaEvent_t a, b;
   VPB_CUDA_OK(cudaEventCreate(&a));

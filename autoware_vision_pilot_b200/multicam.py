@@ -14,6 +14,9 @@ below is its ctypes face — pack kernel -> ncclAllGather -> Estimator::update k
 the NCCL communicator created in C++ from a 128-byte unique id.  torch.distributed is plumbing only: it
 carries that id between the ranks (and the max-over-ranks of the benchmark timings); the pure-Python
 `all_gather_cameras` mirrors the payload layout for the gloo / CPU tests of the host logic.
+
+`MultiCamera.local(n)` is the same fusion for n cameras on ONE GPU (a batched EgoLanes engine and
+`lateral.BatchedLateralPostProcess`): one pack launch fills all n slots, no collective, fusion in camera order.
 """
 from __future__ import annotations
 
@@ -99,6 +102,7 @@ def _bind():
         return lib
     lib.vp_multicam_unique_id.argtypes = [C.c_void_p]
     lib.vp_multicam_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
+    lib.vp_multicam_create_local.argtypes = [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
     lib.vp_multicam_create_with_comm.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
     lib.vp_multicam_destroy.argtypes = [C.c_void_p]
     lib.vp_multicam_destroy.restype = None
@@ -141,6 +145,17 @@ class MultiCamera:
         L.check(self._lib.vp_multicam_create(idb, rank, world, gpu_id, stream, C.byref(self._h)), "vp_multicam_create")
         self.rank, self.world = rank, world
 
+    @classmethod
+    def local(cls, cameras: int, gpu_id: int = 0, stream: Optional[int] = None) -> "MultiCamera":
+        """n cameras on one GPU, no NCCL (vp_multicam_create_local): step() takes n feature maps back to back and
+        [n,14,2] measurements, step_engine() an engine of batch n and the n records of a BatchedLateralPostProcess."""
+        self = cls.__new__(cls)
+        self._lib = _bind()
+        self._h = C.c_void_p()
+        L.check(self._lib.vp_multicam_create_local(cameras, gpu_id, stream, C.byref(self._h)), "vp_multicam_create_local")
+        self.rank, self.world = 0, cameras
+        return self
+
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
             self._lib.vp_multicam_destroy(self._h)
@@ -173,7 +188,7 @@ class MultiCamera:
         return feats, meas, state
 
     def time_allgather(self, reps: int = 100) -> float:
-        """Mean device time (us) of one ncclAllGather of the payloads, `reps` back to back."""
+        """Mean device time (us) of one ncclAllGather of the payloads, `reps` back to back (raises in local mode)."""
         ms = C.c_float()
         L.check(self._lib.vp_multicam_time_allgather(self._h, reps, C.byref(ms)), "vp_multicam_time_allgather")
         return 1e3 * ms.value / reps

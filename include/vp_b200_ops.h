@@ -321,6 +321,18 @@ int vpb_lateral_init(vpb_lateral_state* state_dev, void* stream);
 int vpb_lateral_update(const float* masks, int H, int W, int img_w, int img_h, float smoothing,
                        const double* homography, double autosteer_steering_rad,
                        vpb_lateral_state* state_dev, vpb_lateral_out* out_dev, void* stream);
+/* n cameras (1..VP_MAX_BATCH, vp_b200.h) in ONE launch, one CTA per camera.  Camera k reads masks + k*3*H*W (device
+ * float [n][3][H][W], i.e. vpb_lane_masks over a batched EgoLanes raw tensor), updates states_dev[k] and writes
+ * outs_dev[k] (both device arrays of n records; initialise the states with one vpb_lateral_init each).
+ * homographies: host, n*9 doubles (camera k's orig -> BEV matrix), or NULL = the reference matrix for every camera.
+ * steering_rad: host, n doubles, or NULL = 0.  All cameras share H, W, img_w, img_h and smoothing.
+ * Camera k's state and record are byte-identical to vpb_lateral_update on the same inputs.  The per-camera
+ * parameters travel by value in the launch (no copy), so the call can be captured in a CUDA graph.
+ * VPB_ERR_ARG before any device work: n outside 1..VP_MAX_BATCH, H outside 41..128, W outside 2..256, a NULL
+ * device pointer, or a non-positive image size. */
+int vpb_lateral_update_batch(const float* masks, int n, int H, int W, int img_w, int img_h, float smoothing,
+                             const double* homographies, const double* steering_rad,
+                             vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream);
 
 /* ---- AutoSteer boundary (SURVEY.md 8f rank 2) ----
  * The AutoSteer v1 network itself (ONNX [1,6,80,160] -> 2 x [1,61]) is not in the reference repository

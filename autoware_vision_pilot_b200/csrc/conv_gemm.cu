@@ -71,6 +71,23 @@ __device__ __forceinline__ void acc_ld16(uint32_t t, uint32_t (&r)[16]) {
                  : "memory");
 }
 
+// Class-map rule of a head's output layer (VPB_FINAL_*) on one pixel's logits v[0 .. Cout-1]; v[i] == 0 for
+// i >= Cout.  Shared by the FINAL epilogue and final_tapsum_kernel.
+__device__ __forceinline__ uint8_t final_class(int kind, const float (&v)[16], int Cout) {
+  uint8_t cls = 0;
+  if (kind == VPB_FINAL_ARGMAX) {
+    float best = v[0];
+#pragma unroll
+    for (int i = 1; i < 16; ++i)
+      if (i < Cout && v[i] > best) { best = v[i]; cls = static_cast<uint8_t>(i); }
+  } else if (kind == VPB_FINAL_THRESH) {
+    cls = v[0] > 0.f ? 1 : 0;
+  } else if (kind == VPB_FINAL_EGOLANES) {
+    cls = (v[2] > 0.f) ? 2 : (v[1] > 0.f) ? 1 : (v[0] > 0.f) ? 0 : 255;
+  }
+  return cls;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Epilogue: one accumulator row (BN fp32 columns) per pixel -> outputs.  `part` selects the interleaved set
 // of 16-column chunks (part, part + kParts, ...) this thread handles.
@@ -132,26 +149,15 @@ __device__ __forceinline__ void epilogue_chunks(const ConvKParams& p, uint32_t t
         for (int i = 0; i < 16; ++i) v[c][i] = (n0 + (chunk0 + kParts * c) * 16 + i < p.Cout) ? act_sigmoid(v[c][i]) : 0.f;
     }
     if (p.mode == VPB_EPI_FINAL) {
-      if (px.ok && chunk0 == 0) {
+      if (px.ok) {
         const uint32_t plane = static_cast<uint32_t>(p.H * p.W);
-        float* of = p.out_f32 + px.img * static_cast<uint32_t>(p.Cout) * plane;
+        const int c0 = n0 + chunk0 * 16;
+        float* of = p.out_f32 + (px.img * static_cast<uint32_t>(p.Cout) + c0) * plane;
 #pragma unroll
         for (int i = 0; i < 16; ++i)
-          if (i < p.Cout) of[i * plane + px.fpix] = v[0][i];
-        if (p.out_cls) {
-          uint8_t cls = 0;
-          if (p.final_kind == VPB_FINAL_ARGMAX) {
-            float best = v[0][0];
-#pragma unroll
-            for (int i = 1; i < 16; ++i)
-              if (i < p.Cout && v[0][i] > best) { best = v[0][i]; cls = static_cast<uint8_t>(i); }
-          } else if (p.final_kind == VPB_FINAL_THRESH) {
-            cls = v[0][0] > 0.f ? 1 : 0;
-          } else if (p.final_kind == VPB_FINAL_EGOLANES) {
-            cls = (v[0][2] > 0.f) ? 2 : (v[0][1] > 0.f) ? 1 : (v[0][0] > 0.f) ? 0 : 255;
-          }
-          p.out_cls[px.img * plane + px.fpix] = cls;
-        }
+          if (c0 + i < p.Cout) of[i * plane + px.fpix] = v[0][i];
+        // the plan allows a class map only for Cout <= 16: every logit is in chunk 0 of the one N tile
+        if (p.out_cls && c0 == 0) p.out_cls[px.img * plane + px.fpix] = final_class(p.final_kind, v[0], p.Cout);
       }
     } else if (px.ok) {
       if (p.mode == VPB_EPI_ADD || p.mode == VPB_EPI_MULADD) {
@@ -576,7 +582,65 @@ __global__ void zero_border_kernel(uint4* out, int H, int W, int ldo, int nlim) 
   }
 }
 
-// ------------------------------------------------------------------ host side
+// Second half of a 3x3 convolution to few channels run as a tap-stacked GEMM (vpb_final_tapsum): P holds the products
+// of each tap, P[t*Cout + o] = sum_c W[o][c][dy][dx] * In[c] (t = 3 dy + dx), and
+//   out[o][y][x] = (sum_{t = 0..8} P[t*Cout + o][y + dy - 1][x + dx - 1]) + bias[o]     (0 outside the image)
+// in that order, then the class map.  Plane t is read at one shift only, so P is streamed once.  One thread per pixel,
+// consecutive pixels on consecutive lanes: each shifted plane is read in contiguous runs.  blockIdx.y = image.
+// Cout <= 3: the FINAL epilogue writes at most 32 columns, 9 * 3 tap products.
+static constexpr int kTapsumMaxC = 3;
+__global__ void __launch_bounds__(256) final_tapsum_kernel(const float* __restrict__ P, const float* __restrict__ bias,
+                                                           int Cout, int H, int W, int kind, float* __restrict__ out,
+                                                           uint8_t* __restrict__ cls) {
+  pdl_launch_dependents();
+  pdl_wait();                // P is the output of the GEMM launched just before
+  const int HW = H * W;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= HW) return;
+  const int y = pix / W, x = pix - y * W;
+  const float* pi = P + static_cast<size_t>(blockIdx.y) * 9 * Cout * HW;
+  // element offset of tap t's term within the image (< 2^31, checked by the launcher), and which taps are inside
+  int off[9];
+  uint32_t inside = 0;
+#pragma unroll
+  for (int t = 0; t < 9; ++t) {
+    const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
+    off[t] = t * Cout * HW + yy * W + xx;
+    if (yy >= 0 && yy < H && xx >= 0 && xx < W) inside |= 1u << t;
+  }
+  // all 9 * Cout loads in flight before the first add (small images are latency-bound)
+  float p[9][kTapsumMaxC];
+#pragma unroll
+  for (int t = 0; t < 9; ++t)
+#pragma unroll
+    for (int o = 0; o < kTapsumMaxC; ++o)
+      p[t][o] = (o < Cout && (inside & (1u << t))) ? __ldg(pi + (off[t] + o * HW)) : 0.f;
+  float v[16] = {};
+#pragma unroll
+  for (int o = 0; o < kTapsumMaxC; ++o) {
+    if (o >= Cout) continue;
+#pragma unroll
+    for (int t = 0; t < 9; ++t)
+      if (inside & (1u << t)) v[o] += p[t][o];
+    if (bias) v[o] += __ldg(bias + o);
+    out[(static_cast<size_t>(blockIdx.y) * Cout + o) * HW + pix] = v[o];
+  }
+  if (cls) cls[static_cast<size_t>(blockIdx.y) * HW + pix] = final_class(kind, v, Cout);
+}
+
+int final_tapsum_x(const float* P, const float* bias, int Cout, int H, int W, int final_kind, float* out, uint8_t* cls,
+                   cudaStream_t st, int batch) {
+  if (!P || !out || Cout < 1 || Cout > kTapsumMaxC || H < 1 || W < 1 || batch < 1 || batch > kMaxBatch ||
+      final_kind < VPB_FINAL_NONE || final_kind > VPB_FINAL_EGOLANES) {
+    vpb_set_error("final_tapsum: bad arguments (Cout %d must be 1..%d, batch %d 1..%d, H %d, W %d, final_kind %d)", Cout,
+                  kTapsumMaxC, batch, kMaxBatch, H, W, final_kind);
+    return VPB_ERR_ARG;
+  }
+  if (static_cast<long>(H) * W * 9 * kTapsumMaxC >= (1L << 31)) { vpb_set_error("final_tapsum: image too large"); return VPB_ERR_ARG; }
+  const dim3 grid((H * W + 255) / 256, batch);
+  VPB_CUDA_OK(launch_k(final_tapsum_kernel, grid, dim3(256), 0, st, P, bias, Cout, H, W, final_kind, out, cls));
+  return VPB_OK;
+}
 
 // ------------------------------------------------------------------ host side
 
@@ -651,8 +715,8 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
     return VPB_ERR_ARG;
   }
   if (a->mode == VPB_EPI_FINAL) {
-    if (a->Cout > 16 || !a->out_f32) {
-      vpb_set_error("conv: FINAL mode needs Cout<=16 and out_f32");
+    if (a->Cout > 32 || (a->out_cls && a->Cout > 16) || !a->out_f32) {
+      vpb_set_error("conv: FINAL mode needs Cout<=32 (<=16 with a class map) and out_f32");
       return VPB_ERR_ARG;
     }
   } else {
@@ -696,7 +760,7 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
   {
     // the epilogue addresses pixels with 32-bit element offsets, across the whole batch
     const long ho = a->phases == 4 ? 2L * a->H + 2 : a->H + 2, wo = a->phases == 4 ? 2L * a->W + 2 : a->W + 2;
-    if (ho * wo * std::max(a->ldo, a->ldr) * batch >= (1L << 31) || static_cast<long>(a->H) * a->W * 16 * batch >= (1L << 31)) {
+    if (ho * wo * std::max(a->ldo, a->ldr) * batch >= (1L << 31) || static_cast<long>(a->H) * a->W * (a->mode == VPB_EPI_FINAL ? std::max(a->Cout, 16) : 16) * batch >= (1L << 31)) {
       vpb_set_error("conv: tensor too large for 32-bit element offsets");
       return VPB_ERR_ARG;
     }
@@ -912,4 +976,9 @@ extern "C" int vpb_conv_gemm(const vpb_conv_args* a, void* stream) {
   int rc = vpb::conv_plan_build(a, &plan);
   if (rc != VPB_OK) return rc;
   return vpb::conv_plan_launch(&plan, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_final_tapsum(const float* P, const float* bias, int Cout, int H, int W, int final_kind, float* out,
+                                uint8_t* cls, int batch, void* stream) {
+  return vpb::final_tapsum_x(P, bias, Cout, H, W, final_kind, out, cls, static_cast<cudaStream_t>(stream), batch);
 }

@@ -465,24 +465,35 @@ static int build_neck(vp_engine& e, const WeightMap& w, const std::string& p, co
   return VPB_OK;
 }
 
+// A head's output layer (3x3 to Cout <= 3 channels) as two ops (DESIGN.md §3f): a 1x1 GEMM onto the 9*Cout tap
+// products P — the activation tensor is read once instead of once per tap — and the nine-point shifted sum + bias +
+// class map (final_tapsum_kernel).
 static int final_conv(vp_engine& e, const WeightMap& w, const std::string& key, const std::string& name,
                       const Tens& in, int final_kind, ModelOut& mo) {
   const HostTensor* wt = find_w_shaped(w, key + ".weight", {-1, in.C, 3, 3});
   const HostTensor* bt = wt ? find_w_shaped(w, key + ".bias", {wt->dims[0]}) : nullptr;
   if (!wt || !bt) return VPB_ERR_IO;
-  const int Cout = wt->dims[0];
-  void* dw_ = e.upload_16(pack_conv(*wt, nullptr));
+  const int Cout = wt->dims[0], H = in.H, W = in.W, nb = e.batch;
+  void* dw_ = e.upload_16(pack_conv(*wt, nullptr));     // [9][Cout][Cin] == [9*Cout][Cin], row t*Cout + o
   float* db = e.upload_f32(bt->f);
-  mo.C = Cout; mo.H = in.H; mo.W = in.W;
-  const size_t n = static_cast<size_t>(Cout) * in.H * in.W;
-  const size_t nb = e.batch;     // [batch][C][H][W] fp32 and [batch][H][W] uint8
-  mo.d_raw = static_cast<float*>(e.dalloc(n * 4 * nb, false));
+  mo.C = Cout; mo.H = H; mo.W = W;
+  const size_t plane = static_cast<size_t>(H) * W;
+  // [batch][C][H][W] fp32 and [batch][H][W] uint8
+  mo.d_raw = static_cast<float*>(e.dalloc(plane * Cout * 4 * nb, false));
   mo.has_cls = final_kind != VPB_FINAL_NONE;
-  if (mo.has_cls) mo.d_cls = static_cast<uint8_t*>(e.dalloc(static_cast<size_t>(in.H) * in.W * nb, false));
-  mo.h_raw = static_cast<float*>(e.halloc(n * 4 * nb));
-  if (mo.has_cls) mo.h_cls = static_cast<uint8_t*>(e.halloc(static_cast<size_t>(in.H) * in.W * nb));
+  if (mo.has_cls) mo.d_cls = static_cast<uint8_t*>(e.dalloc(plane * nb, false));
+  mo.h_raw = static_cast<float*>(e.halloc(plane * Cout * 4 * nb));
+  if (mo.has_cls) mo.h_cls = static_cast<uint8_t*>(e.halloc(plane * nb));
   if (!mo.h_raw || (mo.has_cls && !mo.h_cls)) return VPB_ERR_CUDA;
-  return e.add_conv(name, in, Cout, 9, 1, dw_, db, ACT_NONE, VPB_EPI_FINAL, nullptr, nullptr, final_kind, mo.d_raw, mo.d_cls);
+  float* d_taps = static_cast<float*>(e.dalloc(plane * 9 * Cout * 4 * nb, false));   // P [batch][9*Cout][H][W]
+  int rc = e.add_conv(name + "taps", in, 9 * Cout, 1, 1, dw_, nullptr, ACT_NONE, VPB_EPI_FINAL, nullptr, nullptr,
+                      VPB_FINAL_NONE, d_taps);
+  if (rc) return rc;
+  float* raw = mo.d_raw; uint8_t* cls = mo.d_cls;
+  e.add_op(name + "sum", "final_tapsum_kernel",
+           [=](cudaStream_t st) { return final_tapsum_x(d_taps, db, Cout, H, W, final_kind, raw, cls, st, nb); },
+           0.0, nb * (4.0 * 10 * Cout * plane + (cls ? plane : 0)));
+  return VPB_OK;
 }
 
 // SceneSegHead / Scene3DHead / DomainSegHead (scene_seg_head.py:21-44) and EgoLanesHead

@@ -89,6 +89,21 @@ std::vector<float> pack_conv(const HostTensor& t, const std::vector<float>* scal
   return o;
 }
 
+}  // namespace vpb
+
+// The GEMM operand of a heads' output layer: pack_conv's [9][Cout][Cin] is the [9*Cout][Cin] matrix with row t*Cout + o.
+extern "C" int vpb_final_conv_weights_host(const float* w, int Cout, int Cin, float* out) {
+  if (!w || !out || Cout < 1 || Cin < 1) { vpb_set_error("final_conv_weights: bad arguments"); return VPB_ERR_ARG; }
+  vpb::HostTensor t;
+  t.dims = {Cout, Cin, 3, 3};
+  t.f.assign(w, w + t.numel());
+  const std::vector<float> o = vpb::pack_conv(t, nullptr);
+  memcpy(out, o.data(), o.size() * sizeof(float));
+  return VPB_OK;
+}
+
+namespace vpb {
+
 // =============================================================== frame graph
 int FrameGraph::run(cudaStream_t st, const PreprocessPlan& pre, int dtype, int h_, int w_, int stride_,
                     const FrameSrcs& src_, const std::function<int(cudaStream_t)>& launch,

@@ -66,6 +66,9 @@ int ctx_conv1_x(int dtype, const float* in, int H, int W, const float* w, const 
                 void* out_lo, int out_pad, cudaStream_t st, int act = VPB_ACT_GELU /* or VPB_ACT_SILU */, int batch = 1);
 int fuse_pool_x(int dtype, const void* f0, const void* f1, const void* f2, const void* f3, const void* f4,
                 const size_t lo_off[5], int H4, int W4, void* out, void* out_lo, cudaStream_t st, int batch = 1);
+// vpb_final_tapsum (conv_gemm.cu)
+int final_tapsum_x(const float* P, const float* bias, int Cout, int H, int W, int final_kind, float* out, uint8_t* cls,
+                   cudaStream_t st, int batch = 1);
 
 // One-time per-DEVICE initialisation (function attributes, constant tables): engines for several GPUs may
 // live in one process, and entry points may be called from several threads.

@@ -53,7 +53,7 @@ void vpb_set_error(const char* fmt, ...);
  *   w      : [taps*phases][Cout][Cin] 16-bit,   bias: fp32 [Cout] or NULL
  *   in     : [H][W][ldi]  (Cin valid channels, ldi >= Cin, both multiples of 8)
  *   out    : [Ho][Wo][ldo], res (modes ADD/MULADD): [Ho][Wo][ldr]
- *   FINAL  : out_f32 planar [Cout][H][W] fp32, out_cls [H][W] uint8 (may be NULL)
+ *   FINAL  : out_f32 planar [Cout][H][W] fp32 (Cout <= 32), out_cls [H][W] uint8 (may be NULL; needs Cout <= 16)
  */
 typedef struct {
   int dtype;
@@ -136,6 +136,19 @@ typedef struct {
   int w_img;
 } vpb_conv_args;
 int vpb_conv_gemm(const vpb_conv_args* a, void* stream);
+/* A heads' output layer (Conv2d 3x3 pad 1 to Cout <= 3 channels, scene_seg_head.py:44, ego_lanes_head.py:26) as a
+ * tap-stacked GEMM and a nine-point sum, the way the engine runs it:
+ *   1. vpb_conv_gemm with taps = 1, Cout' = 9*Cout, mode FINAL, no bias, no class map, w = the [9*Cout][Cin] matrix of
+ *      vpb_final_conv_weights_host:  P[t*Cout + o][y][x] = sum_c W[o][c][dy][dx] * in[y][x][c]   (t = 3*dy + dx);
+ *   2. vpb_final_tapsum: out[o][y][x] = (sum_{t=0..8} P[t*Cout + o][y+dy-1][x+dx-1]) + bias[o], the sum in this tap
+ *      order with terms outside the image left out, and the class map of VPB_EPI_FINAL.
+ * P fp32 [batch][9*Cout][H][W], bias fp32 [Cout] or NULL, out fp32 [batch][Cout][H][W], cls uint8 [batch][H][W] or
+ * NULL (final_kind VPB_FINAL_*); Cout 1..3 (9*Cout tap products fit FINAL's 32 columns), batch 1..8; each image's
+ * result is bit-identical to a batch-1 call. */
+int vpb_final_tapsum(const float* P, const float* bias, int Cout, int H, int W, int final_kind, float* out,
+                     uint8_t* cls, int batch, void* stream);
+/* Host-only: w fp32 [Cout][Cin][3][3] -> out fp32 [9*Cout][Cin], out[(t*Cout + o)*Cin + c] = w[o][c][t/3][t%3] */
+int vpb_final_conv_weights_host(const float* w, int Cout, int Cin, float* out);
 /* Composition of the upconv operands on the device (all pointers device fp32, outputs may be NULL to skip):
  *   w3 [Cout][Cmid][3][3], b3 [Cout]          Conv2d 3x3            (e.g. decode_layer_0, scene_neck.py:13)
  *   wt [Cin][Cmid][2][2],  bt [Cmid]          ConvTranspose2d k2 s2 (upsample_layer_0, scene_neck.py:11)

@@ -45,11 +45,10 @@
 namespace vpb {
 
 static constexpr int kMma = 256;                     // two MMA warpgroups
-// one epilogue warpgroup: with two (kParts = 2) the 544-thread launch caps the kernel at 96 registers and it measured
-// no faster on the H100
+// one epilogue warpgroup, one thread per accumulator row: with two the 544-thread launch caps the kernel at 96
+// registers and it measured no faster on the H100
 static constexpr int kEpilogue = 128;
 static constexpr int kThreads = kMma + kEpilogue + 32;   // + the TMA producer warp
-static constexpr int kParts = kEpilogue / 128;        // epilogue threads per accumulator row
 static constexpr int kMaxStages = 8;
 static constexpr int kATileBytes = 128 * 128;  // 128 pixels x 64 ch x 2 B
 // 227 KB opt-in limit covers static + dynamic shared memory; keep 4 KB for the static part.
@@ -89,151 +88,116 @@ __device__ __forceinline__ uint8_t final_class(int kind, const float (&v)[16], i
 }
 
 // ------------------------------------------------------------------------------------------------
-// Epilogue: one accumulator row (BN fp32 columns) per pixel -> outputs.  `part` selects the interleaved set
-// of 16-column chunks (part, part + kParts, ...) this thread handles.
+// Epilogue: one accumulator row (BN fp32 columns) per pixel -> outputs, one epilogue thread per row.
 // ------------------------------------------------------------------------------------------------
 struct EpiPix {
   bool ok;        // compute and store this row
-  bool zero;      // store zeros instead (border pixel of a padded output)
   uint32_t ooff;  // element offset of the pixel in the output tensor   (pixel * ldo; < 2^31, checked by the plan)
   uint32_t roff;  // element offset of the pixel in the residual tensor (pixel * ldr)
   uint32_t fpix;  // pixel index in the planar fp32 / class outputs (FINAL), within the image
   uint32_t img;   // image of the batch (FINAL: selects the [Cout][H][W] / [H][W] planes)
 };
 
-// NC = 16-column chunks handled per loop iteration (only NC = 1 is instantiated).
-template <class E, int NC, bool TILEK>
+// General form: every mode, activation, post-residual activation and split-fp16 output, with per-store channel
+// predicates; one 16-column chunk per iteration.
+template <class E>
 __device__ __forceinline__ void epilogue_chunks(const ConvKParams& p, uint32_t t_row, int n0,
-                                                const float* sbias, int part, const EpiPix& px) {
-  const bool split = TILEK && p.split;       // split-fp16 mode and the post-residual activation exist in the tile kernel only
+                                                const float* sbias, const EpiPix& px) {
   const int nchunks = p.BN >> 4;
   typename E::T* out = reinterpret_cast<typename E::T*>(p.out);
   const typename E::T* res = reinterpret_cast<const typename E::T*>(p.res);
   typename E::T* out_lo = reinterpret_cast<typename E::T*>(p.out_lo);                // split-fp16 mode only
   const typename E::T* res_lo = reinterpret_cast<const typename E::T*>(p.res_lo);
-  for (int chunk0 = part; chunk0 < nchunks; chunk0 += kParts * NC) {
-    uint32_t rr[NC][16];
+  for (int chunk = 0; chunk < nchunks; ++chunk) {
+    const int n = n0 + chunk * 16;
+    uint32_t rr[16];
+    acc_ld16(t_row + chunk * 16, rr);
+    float v[16];
+    const float4* sb4 = reinterpret_cast<const float4*>(sbias + chunk * 16);   // 4 x LDS.128
 #pragma unroll
-    for (int c = 0; c < NC; ++c) acc_ld16(t_row + (chunk0 + kParts * c) * 16, rr[c]);
-    float v[NC][16];
-#pragma unroll
-    for (int c = 0; c < NC; ++c) {
-      const float4* sb4 = reinterpret_cast<const float4*>(sbias + (chunk0 + kParts * c) * 16);   // 4 x LDS.128
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float4 b4 = sb4[i];
-        const float2 lo = fadd2(make_float2(__uint_as_float(rr[c][4 * i]), __uint_as_float(rr[c][4 * i + 1])), make_float2(b4.x, b4.y));
-        const float2 hi = fadd2(make_float2(__uint_as_float(rr[c][4 * i + 2]), __uint_as_float(rr[c][4 * i + 3])), make_float2(b4.z, b4.w));
-        v[c][4 * i] = lo.x; v[c][4 * i + 1] = lo.y; v[c][4 * i + 2] = hi.x; v[c][4 * i + 3] = hi.y;
-      }
+    for (int i = 0; i < 4; ++i) {
+      const float4 b4 = sb4[i];
+      const float2 lo = fadd2(make_float2(__uint_as_float(rr[4 * i]), __uint_as_float(rr[4 * i + 1])), make_float2(b4.x, b4.y));
+      const float2 hi = fadd2(make_float2(__uint_as_float(rr[4 * i + 2]), __uint_as_float(rr[4 * i + 3])), make_float2(b4.z, b4.w));
+      v[4 * i] = lo.x; v[4 * i + 1] = lo.y; v[4 * i + 2] = hi.x; v[4 * i + 3] = hi.y;
     }
     // activation switch hoisted out of the element loop (act(0) == 0 for GELU/SiLU keeps the
     // channel padding zero; sigmoid is masked explicitly)
     if (p.act == ACT_GELU) {
 #pragma unroll
-      for (int c = 0; c < NC; ++c)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {   // packed fp32x2: two elements per FFMA2 / FMUL2
-          const float2 g = act_gelu2(make_float2(v[c][2 * i], v[c][2 * i + 1]));
-          v[c][2 * i] = g.x; v[c][2 * i + 1] = g.y;
-        }
+      for (int i = 0; i < 8; ++i) {   // packed fp32x2: two elements per FFMA2 / FMUL2
+        const float2 g = act_gelu2(make_float2(v[2 * i], v[2 * i + 1]));
+        v[2 * i] = g.x; v[2 * i + 1] = g.y;
+      }
     } else if (p.act == ACT_SILU) {
 #pragma unroll
-      for (int c = 0; c < NC; ++c)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[c][i] = act_silu(v[c][i]);
+      for (int i = 0; i < 16; ++i) v[i] = act_silu(v[i]);
     } else if (p.act == ACT_SIGMOID) {
 #pragma unroll
-      for (int c = 0; c < NC; ++c)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[c][i] = (n0 + (chunk0 + kParts * c) * 16 + i < p.Cout) ? act_sigmoid(v[c][i]) : 0.f;
+      for (int i = 0; i < 16; ++i) v[i] = (n + i < p.Cout) ? act_sigmoid(v[i]) : 0.f;
     }
+    if (!px.ok) continue;
     if (p.mode == VPB_EPI_FINAL) {
-      if (px.ok) {
-        const uint32_t plane = static_cast<uint32_t>(p.H * p.W);
-        const int c0 = n0 + chunk0 * 16;
-        float* of = p.out_f32 + (px.img * static_cast<uint32_t>(p.Cout) + c0) * plane;
+      const uint32_t plane = static_cast<uint32_t>(p.H * p.W);
+      float* of = p.out_f32 + (px.img * static_cast<uint32_t>(p.Cout) + n) * plane;
 #pragma unroll
-        for (int i = 0; i < 16; ++i)
-          if (c0 + i < p.Cout) of[i * plane + px.fpix] = v[0][i];
-        // the plan allows a class map only for Cout <= 16: every logit is in chunk 0 of the one N tile
-        if (p.out_cls && c0 == 0) p.out_cls[px.img * plane + px.fpix] = final_class(p.final_kind, v[0], p.Cout);
+      for (int i = 0; i < 16; ++i)
+        if (n + i < p.Cout) of[i * plane + px.fpix] = v[i];
+      // the plan allows a class map only for Cout <= 16: every logit is in chunk 0 of the one N tile
+      if (p.out_cls && n == 0) p.out_cls[px.img * plane + px.fpix] = final_class(p.final_kind, v, p.Cout);
+      continue;
+    }
+    if (p.mode == VPB_EPI_ADD || p.mode == VPB_EPI_MULADD) {
+      // all residual loads in flight before the first use
+      const typename E::T* rp = res + (px.roff + n);
+      uint4 rv[2];
+      bool rok[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        rok[j] = (n + 8 * j < p.ldr) && (n + 8 * j < p.nlim);
+        rv[j] = rok[j] ? *reinterpret_cast<const uint4*>(rp + 8 * j) : make_uint4(0, 0, 0, 0);
       }
-    } else if (px.ok) {
-      if (p.mode == VPB_EPI_ADD || p.mode == VPB_EPI_MULADD) {
-        uint4 rv[NC][2];
-        bool rok[NC][2];
+      uint4 rl[2];
 #pragma unroll
-        for (int c = 0; c < NC; ++c) {          // all residual loads in flight before the first use
-          const int n = n0 + (chunk0 + kParts * c) * 16;
-          const typename E::T* rp = res + (px.roff + n);
+      for (int j = 0; j < 2; ++j)
+        rl[j] = (p.split && rok[j]) ? *reinterpret_cast<const uint4*>(res_lo + (px.roff + n) + 8 * j) : make_uint4(0, 0, 0, 0);
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            rok[c][j] = (n + 8 * j < p.ldr) && (n + 8 * j < p.nlim);
-            rv[c][j] = rok[c][j] ? *reinterpret_cast<const uint4*>(rp + 8 * j) : make_uint4(0, 0, 0, 0);
-          }
-        }
-        uint4 rl[NC][2];
+      for (int j = 0; j < 2; ++j) {
+        if (!rok[j]) continue;
+        const uint32_t rw[4] = {rv[j].x, rv[j].y, rv[j].z, rv[j].w};
+        const uint32_t rwl[4] = {rl[j].x, rl[j].y, rl[j].z, rl[j].w};
 #pragma unroll
-        for (int c = 0; c < NC; ++c)
-#pragma unroll
-          for (int j = 0; j < 2; ++j)
-            rl[c][j] = (split && rok[c][j])
-                           ? *reinterpret_cast<const uint4*>(res_lo + (px.roff + n0 + (chunk0 + kParts * c) * 16) + 8 * j)
-                           : make_uint4(0, 0, 0, 0);
-#pragma unroll
-        for (int c = 0; c < NC; ++c)
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            if (!rok[c][j]) continue;
-            const uint32_t rw[4] = {rv[c][j].x, rv[c][j].y, rv[c][j].z, rv[c][j].w};
-            const uint32_t rwl[4] = {rl[c][j].x, rl[c][j].y, rl[c][j].z, rl[c][j].w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              float2 f = unpack2<E>(rw[i]);
-              if (split) { const float2 fl = unpack2<E>(rwl[i]); f.x += fl.x; f.y += fl.y; }
-              float& a = v[c][8 * j + 2 * i];
-              float& b = v[c][8 * j + 2 * i + 1];
-              if (p.mode == VPB_EPI_ADD) { a += f.x; b += f.y; }
-              else { a = fmaf(a, f.x, f.x); b = fmaf(b, f.y, f.y); }
-              if (TILEK && p.act2 == ACT_SILU) { a = act_silu(a); b = act_silu(b); }
-            }
-          }
-      }
-#pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        const int n = n0 + (chunk0 + kParts * c) * 16;
-        typename E::T* op = out + (px.ooff + n);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          if (n + 8 * j < p.nlim) {
-            uint4 o;
-            o.x = pack2<E>(v[c][8 * j + 0], v[c][8 * j + 1]);
-            o.y = pack2<E>(v[c][8 * j + 2], v[c][8 * j + 3]);
-            o.z = pack2<E>(v[c][8 * j + 4], v[c][8 * j + 5]);
-            o.w = pack2<E>(v[c][8 * j + 6], v[c][8 * j + 7]);
-            *reinterpret_cast<uint4*>(op + 8 * j) = o;
-            if (split) {          // low half: what the 16-bit rounding of the high half lost
-              const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
-              uint32_t lw[4];
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float2 h = unpack2<E>(ow[i]);
-                lw[i] = pack2<E>(v[c][8 * j + 2 * i] - h.x, v[c][8 * j + 2 * i + 1] - h.y);
-              }
-              *reinterpret_cast<uint4*>(out_lo + (px.ooff + n) + 8 * j) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-            }
-          }
+        for (int i = 0; i < 4; ++i) {
+          float2 f = unpack2<E>(rw[i]);
+          if (p.split) { const float2 fl = unpack2<E>(rwl[i]); f.x += fl.x; f.y += fl.y; }
+          float& a = v[8 * j + 2 * i];
+          float& b = v[8 * j + 2 * i + 1];
+          if (p.mode == VPB_EPI_ADD) { a += f.x; b += f.y; }
+          else { a = fmaf(a, f.x, f.x); b = fmaf(b, f.y, f.y); }
+          if (p.act2 == ACT_SILU) { a = act_silu(a); b = act_silu(b); }
         }
       }
-    } else if (px.zero) {
+    }
+    typename E::T* op = out + (px.ooff + n);
 #pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        const int n = n0 + (chunk0 + kParts * c) * 16;
-        typename E::T* op = out + (px.ooff + n);
+    for (int j = 0; j < 2; ++j) {
+      if (n + 8 * j < p.nlim) {
+        uint4 o;
+        o.x = pack2<E>(v[8 * j + 0], v[8 * j + 1]);
+        o.y = pack2<E>(v[8 * j + 2], v[8 * j + 3]);
+        o.z = pack2<E>(v[8 * j + 4], v[8 * j + 5]);
+        o.w = pack2<E>(v[8 * j + 6], v[8 * j + 7]);
+        *reinterpret_cast<uint4*>(op + 8 * j) = o;
+        if (p.split) {          // low half: what the 16-bit rounding of the high half lost
+          const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
+          uint32_t lw[4];
 #pragma unroll
-        for (int j = 0; j < 2; ++j)
-          if (n + 8 * j < p.nlim) *reinterpret_cast<uint4*>(op + 8 * j) = make_uint4(0, 0, 0, 0);
+          for (int i = 0; i < 4; ++i) {
+            const float2 h = unpack2<E>(ow[i]);
+            lw[i] = pack2<E>(v[8 * j + 2 * i] - h.x, v[8 * j + 2 * i + 1] - h.y);
+          }
+          *reinterpret_cast<uint4*>(out_lo + (px.ooff + n) + 8 * j) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+        }
       }
     }
   }
@@ -248,15 +212,15 @@ __device__ __forceinline__ void epilogue_chunks(const ConvKParams& p, uint32_t t
 // 3x3 taps, and its bias row comes from global memory instead of the staged interior row.
 template <class E, int ACT, bool ADD = false, bool CLS = false>
 __device__ __forceinline__ void epilogue_store_fast(const ConvKParams& p, uint32_t t_row, int n0,
-                                                    const float* sbias, int part, const EpiPix& px,
+                                                    const float* sbias, const EpiPix& px,
                                                     const float* gb = nullptr) {
   const int nchunks = p.BN >> 4;
-  typename E::T* op = reinterpret_cast<typename E::T*>(p.out) + (px.ooff + n0 + part * 16);
-  const typename E::T* rp = ADD ? reinterpret_cast<const typename E::T*>(p.res) + (px.roff + n0 + part * 16) : nullptr;
-  const float4* sb4 = reinterpret_cast<const float4*>(sbias + part * 16);
-  const float4* gb4 = (CLS && gb) ? reinterpret_cast<const float4*>(gb + part * 16) : nullptr;
-  uint32_t ta = t_row + part * 16;
-  const bool ok = px.ok, zero = px.zero;
+  typename E::T* op = reinterpret_cast<typename E::T*>(p.out) + (px.ooff + n0);
+  const typename E::T* rp = ADD ? reinterpret_cast<const typename E::T*>(p.res) + (px.roff + n0) : nullptr;
+  const float4* sb4 = reinterpret_cast<const float4*>(sbias);
+  const float4* gb4 = (CLS && gb) ? reinterpret_cast<const float4*>(gb) : nullptr;
+  uint32_t ta = t_row;
+  const bool ok = px.ok;
   auto finish = [&](const uint32_t (&rr)[16], const float4* sb, typename E::T* o, const typename E::T* r, int goff = 0) {
     uint4 r0 = make_uint4(0, 0, 0, 0), r1 = r0;
     if (ADD && ok) { r0 = reinterpret_cast<const uint4*>(r)[0]; r1 = reinterpret_cast<const uint4*>(r)[1]; }   // in flight early
@@ -284,22 +248,21 @@ __device__ __forceinline__ void epilogue_store_fast(const ConvKParams& p, uint32
     uint4 o0, o1;
     o0.x = pack2<E>(v[0].x, v[0].y); o0.y = pack2<E>(v[1].x, v[1].y); o0.z = pack2<E>(v[2].x, v[2].y); o0.w = pack2<E>(v[3].x, v[3].y);
     o1.x = pack2<E>(v[4].x, v[4].y); o1.y = pack2<E>(v[5].x, v[5].y); o1.z = pack2<E>(v[6].x, v[6].y); o1.w = pack2<E>(v[7].x, v[7].y);
-    if (zero) { o0 = make_uint4(0, 0, 0, 0); o1 = o0; }
-    if (ok || zero) {
+    if (ok) {
       reinterpret_cast<uint4*>(o)[0] = o0;
       reinterpret_cast<uint4*>(o)[1] = o1;
     }
   };
-  int chunk = part;
+  int chunk = 0;
   // two chunks per iteration while at least two remain (two independent chains), then the odd one
-  for (; chunk + kParts < nchunks; chunk += 2 * kParts, op += 32 * kParts, sb4 += 8 * kParts, ta += 32 * kParts) {
+  for (; chunk + 1 < nchunks; chunk += 2, op += 32, sb4 += 8, ta += 32) {
     uint32_t ra[16], rb[16];
     acc_ld16(ta, ra);
-    acc_ld16(ta + 16 * kParts, rb);
+    acc_ld16(ta + 16, rb);
     finish(ra, sb4, op, rp);
-    finish(rb, sb4 + 4 * kParts, op + 16 * kParts, rp + 16 * kParts, 4 * kParts);
-    if (ADD) rp += 32 * kParts;
-    if (CLS && gb4) gb4 += 8 * kParts;
+    finish(rb, sb4 + 4, op + 16, rp + 16, 4);
+    if (ADD) rp += 32;
+    if (CLS && gb4) gb4 += 8;
   }
   if (chunk < nchunks) {
     uint32_t ra[16];
@@ -308,15 +271,34 @@ __device__ __forceinline__ void epilogue_store_fast(const ConvKParams& p, uint32
   }
 }
 
-template <class E, bool TILEK = true>
+template <class E>
 __device__ __forceinline__ void epilogue_tile(const ConvKParams& p, uint32_t t_row, int n0,
-                                              const float* sbias, int part, const EpiPix& px) {
+                                              const float* sbias, const EpiPix& px) {
   const bool whole = !p.split && n0 + p.BN <= p.nlim && p.act2 == ACT_NONE;
-  if (whole && p.mode == VPB_EPI_STORE && p.act == ACT_GELU) epilogue_store_fast<E, ACT_GELU>(p, t_row, n0, sbias, part, px);
-  else if (whole && p.mode == VPB_EPI_STORE && p.act == ACT_NONE) epilogue_store_fast<E, ACT_NONE>(p, t_row, n0, sbias, part, px);
-  else if (TILEK && whole && p.mode == VPB_EPI_STORE && p.act == ACT_SILU) epilogue_store_fast<E, ACT_SILU>(p, t_row, n0, sbias, part, px);
-  else if (TILEK && whole && p.mode == VPB_EPI_ADD && p.act == ACT_NONE && n0 + p.BN <= p.ldr) epilogue_store_fast<E, ACT_NONE, true>(p, t_row, n0, sbias, part, px);
-  else epilogue_chunks<E, 1, TILEK>(p, t_row, n0, sbias, part, px);
+  if (whole && p.mode == VPB_EPI_STORE && p.act == ACT_GELU) epilogue_store_fast<E, ACT_GELU>(p, t_row, n0, sbias, px);
+  else if (whole && p.mode == VPB_EPI_STORE && p.act == ACT_NONE) epilogue_store_fast<E, ACT_NONE>(p, t_row, n0, sbias, px);
+  else if (whole && p.mode == VPB_EPI_STORE && p.act == ACT_SILU) epilogue_store_fast<E, ACT_SILU>(p, t_row, n0, sbias, px);
+  else if (whole && p.mode == VPB_EPI_ADD && p.act == ACT_NONE && n0 + p.BN <= p.ldr) epilogue_store_fast<E, ACT_NONE, true>(p, t_row, n0, sbias, px);
+  else epilogue_chunks<E>(p, t_row, n0, sbias, px);
+}
+
+// Coordinates of one output tile: image of the batch, ConvTranspose / upconv phase, first output channel and first
+// pixel (row h0, column w0, at the GEMM's input resolution).  Tiles are numbered image-major, then phase, then pixel
+// tile (row-major), with the N tile innermost.
+struct TileCoord { int img, ph, n0, h0, w0; };
+
+__device__ __forceinline__ TileCoord decode_tile(const ConvKParams& p, int tile) {
+  TileCoord c;
+  c.img = static_cast<int>(fast_div(tile, p.mg_ti));
+  const int ti = tile - c.img * p.tiles_img;
+  c.ph = static_cast<int>(fast_div(ti, p.mg_tpp));
+  const int r = ti - c.ph * (p.tiles_n * p.tiles_h * p.tiles_w);
+  const int rn = static_cast<int>(fast_div(r, p.mg_tn));
+  const int thi = static_cast<int>(fast_div(rn, p.mg_tw));
+  c.n0 = (r - rn * p.tiles_n) * p.BN;
+  c.h0 = thi * p.TH;
+  c.w0 = (rn - thi * p.tiles_w) * p.TW;
+  return c;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -326,10 +308,6 @@ __device__ __forceinline__ void epilogue_tile(const ConvKParams& p, uint32_t t_r
 template <class E, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
-  const CUtensorMap& mapA = maps.A;
-  const CUtensorMap& mapB = maps.B;
-  const CUtensorMap& mapA2 = maps.A2;
-  const CUtensorMap& mapB2 = maps.B2;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[kMaxStages];
   __shared__ __align__(8) uint64_t bar_empty[kMaxStages];
@@ -346,9 +324,9 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
   const uint32_t acc_base = smem_base + static_cast<uint32_t>(p.stages) * kStageBytes;
 
   if (threadIdx.x == kMma + kEpilogue) {
-    tma_prefetch_desc(&mapA);
-    tma_prefetch_desc(&mapB);
-    if (p.kchunks2) { tma_prefetch_desc(&mapA2); tma_prefetch_desc(&mapB2); }
+    tma_prefetch_desc(&maps.A);
+    tma_prefetch_desc(&maps.B);
+    if (p.kchunks2) { tma_prefetch_desc(&maps.A2); tma_prefetch_desc(&maps.B2); }
     if (p.split) { tma_prefetch_desc(&maps.Alo); tma_prefetch_desc(&maps.Blo); }
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
@@ -365,40 +343,35 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
   // split-fp16 mode: every K chunk is walked three times (A_hi W_hi, A_lo W_hi, A_hi W_lo) into the same accumulator
   const int nseg = p.split ? 3 : 1;
   const int kiters_all = p.upc ? 4 * p.kchunks + 9 * p.kchunks2 : (p.taps * p.kchunks + p.kchunks2) * nseg;
-  const int tiles_per_phase = p.tiles_n * p.tiles_h * p.tiles_w;
 
   if (warp == (kMma + kEpilogue) / 32) {
     // ------------------------------------------------------------ TMA producer (converged warp, elected lane)
     int stage = 0;
     uint32_t phase = 0;
-    auto next = [&]() { if (++stage == p.stages) { stage = 0; phase ^= 1u; } };
+    // One K chunk into the next ring stage, once the MMA warps have released it: the activation box of map mA at
+    // {channel, column, row, image} and the weight box of map mB at {channel, output channel, third dimension}.
+    auto load_stage = [&](const CUtensorMap* mA, int a0, int a1, int a2, int a3,
+                          const CUtensorMap* mB, int b0, int b1, int b2) {
+      mbar_wait_quiet(smem_u32(&bar_empty[stage]), phase ^ 1u);
+      if (elect_one()) {
+        const uint32_t full = smem_u32(&bar_full[stage]);
+        const uint32_t sa = smem_base + stage * kStageBytes;
+        mbar_arrive_expect_tx(full, kStageBytes);
+        tma_load_4d(sa, mA, full, a0, a1, a2, a3);
+        tma_load_3d(sa + kATileBytes, mB, full, b0, b1, b2);
+      }
+      __syncwarp();
+      if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+    };
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int img = static_cast<int>(fast_div(tile, p.mg_ti));
-      const int ti = tile - img * p.tiles_img;
-      const int ph = static_cast<int>(fast_div(ti, p.mg_tpp));
-      const int r = ti - ph * tiles_per_phase;
-      const int rn = static_cast<int>(fast_div(r, p.mg_tn));
-      const int nt = r - rn * p.tiles_n;
-      const int thi = static_cast<int>(fast_div(rn, p.mg_tw));
-      const int twi = rn - thi * p.tiles_w;
-      const int h0 = thi * p.TH, w0 = twi * p.TW, n0 = nt * p.BN;
+      const auto [img, ph, n0, h0, w0] = decode_tile(p, tile);
       if (p.upc) {
         const int pa = ph >> 1, pb = ph & 1;
         // the four low-resolution taps of this phase: offsets (ty - 1 + a, tx - 1 + b)
         for (int t = 0; t < 4; ++t) {
           const int oy = (t >> 1) - 1 + pa, ox = (t & 1) - 1 + pb;
-          for (int c = 0; c < p.kchunks; ++c) {
-            mbar_wait_quiet(smem_u32(&bar_empty[stage]), phase ^ 1u);
-            if (elect_one()) {
-              const uint32_t full = smem_u32(&bar_full[stage]);
-              const uint32_t sa = smem_base + stage * kStageBytes;
-              mbar_arrive_expect_tx(full, kStageBytes);
-              tma_load_4d(sa, &mapA, full, c * 64, w0 + ox, h0 + oy, img);
-              tma_load_3d(sa + kATileBytes, &mapB, full, c * 64, n0, ph * 4 + t);
-            }
-            __syncwarp();
-            next();
-          }
+          for (int c = 0; c < p.kchunks; ++c)
+            load_stage(&maps.A, c * 64, w0 + ox, h0 + oy, img, &maps.B, c * 64, n0, ph * 4 + t);
         }
         // the nine taps of the skip tensor (output resolution, traversed with element stride 2): output pixel
         // (2h + a, 2w + b) reads hi-res row 2h + a + dy - 1 = 2 h0 + u (+ 2 lh) and column 2 w0 + v (+ 2 lw);
@@ -406,18 +379,8 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
         for (int t2 = 0; t2 < (p.kchunks2 ? 9 : 0); ++t2) {
           const int dy = t2 / 3, dx = t2 - dy * 3;
           const int u = pa + dy - 1, v = pb + dx - 1;
-          for (int c2 = 0; c2 < p.kchunks2; ++c2) {
-            mbar_wait_quiet(smem_u32(&bar_empty[stage]), phase ^ 1u);
-            if (elect_one()) {
-              const uint32_t full = smem_u32(&bar_full[stage]);
-              const uint32_t sa = smem_base + stage * kStageBytes;
-              mbar_arrive_expect_tx(full, kStageBytes);
-              tma_load_4d(sa, &mapA2, full, c2 * 64, 2 * w0 + v, 2 * h0 + u, img);
-              tma_load_3d(sa + kATileBytes, &mapB2, full, c2 * 64, n0, t2);
-            }
-            __syncwarp();
-            next();
-          }
+          for (int c2 = 0; c2 < p.kchunks2; ++c2)
+            load_stage(&maps.A2, c2 * 64, 2 * w0 + v, 2 * h0 + u, img, &maps.B2, c2 * 64, n0, t2);
         }
         continue;
       }
@@ -425,43 +388,19 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
         const int dy = (p.taps == 9) ? (t / 3 - 1) : 0;
         const int dx = (p.taps == 9) ? (t % 3 - 1) : 0;
         const int wsel = p.w_img ? img : (p.phases > 1) ? ph : t;
-        for (int c = 0; c < p.kchunks; ++c) {
-          for (int seg = 0; seg < nseg; ++seg) {
-            const CUtensorMap* mA = seg == 1 ? &maps.Alo : &mapA;
-            const CUtensorMap* mB = seg == 2 ? &maps.Blo : &mapB;
-            mbar_wait_quiet(smem_u32(&bar_empty[stage]), phase ^ 1u);
-            if (elect_one()) {
-              const uint32_t full = smem_u32(&bar_full[stage]);
-              const uint32_t sa = smem_base + stage * kStageBytes;
-              mbar_arrive_expect_tx(full, kStageBytes);
-              tma_load_4d(sa, mA, full, c * 64, w0 * p.stride + dx, h0 * p.stride + dy, img);
-              tma_load_3d(sa + kATileBytes, mB, full, c * 64, n0, wsel);
-            }
-            __syncwarp();
-            next();
-          }
-        }
+        for (int c = 0; c < p.kchunks; ++c)
+          for (int seg = 0; seg < nseg; ++seg)
+            load_stage(seg == 1 ? &maps.Alo : &maps.A, c * 64, w0 * p.stride + dx, h0 * p.stride + dy, img,
+                       seg == 2 ? &maps.Blo : &maps.B, c * 64, n0, wsel);
       }
       // fused skip link: the same output pixels seen in the second input (at output resolution);
       // for a ConvTranspose phase (a,b) that is the pixel set (2h+a, 2w+b), which the second map's
       // element stride 2 picks from a box starting at (2 h0 + a, 2 w0 + b)
       const int s2 = p.phases > 1 ? 2 : 1;
-      for (int c2 = 0; c2 < p.kchunks2; ++c2) {
-        for (int seg = 0; seg < nseg; ++seg) {
-          const CUtensorMap* mA = seg == 1 ? &maps.A2lo : &mapA2;
-          const CUtensorMap* mB = seg == 2 ? &maps.B2lo : &mapB2;
-          mbar_wait_quiet(smem_u32(&bar_empty[stage]), phase ^ 1u);
-          if (elect_one()) {
-            const uint32_t full = smem_u32(&bar_full[stage]);
-            const uint32_t sa = smem_base + stage * kStageBytes;
-            mbar_arrive_expect_tx(full, kStageBytes);
-            tma_load_4d(sa, mA, full, c2 * 64, s2 * w0 + (ph & 1), s2 * h0 + (ph >> 1), img);
-            tma_load_3d(sa + kATileBytes, mB, full, c2 * 64, n0, 0);
-          }
-          __syncwarp();
-          next();
-        }
-      }
+      for (int c2 = 0; c2 < p.kchunks2; ++c2)
+        for (int seg = 0; seg < nseg; ++seg)
+          load_stage(seg == 1 ? &maps.A2lo : &maps.A2, c2 * 64, s2 * w0 + (ph & 1), s2 * h0 + (ph >> 1), img,
+                     seg == 2 ? &maps.B2lo : &maps.B2, c2 * 64, n0, 0);
     }
   } else if (warp < kMma / 32) {
     // ------------------------------------------------------------ MMA warpgroups: wgmma main loop, then stage the accumulator
@@ -504,34 +443,34 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
     }
   } else {
     // ------------------------------------------------------------ epilogue warps: one tile behind the MMA warps
-    const int et = threadIdx.x - kMma;
-    const int row = et & 127;                 // accumulator row == pixel within the tile
-    const int part = et >> 7;
+    const int row = threadIdx.x - kMma;       // accumulator row == pixel within the tile
     const int lh = row >> p.tw_shift;
     const int lw = row & (p.TW - 1);
     const int Wo = (p.phases > 1) ? 2 * p.W : p.W;
     const uint32_t t_row = (acc_base >> 2) + static_cast<uint32_t>(row * kPitch);
     uint32_t acc_phase = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int img = static_cast<int>(fast_div(tile, p.mg_ti));
-      const int ti = tile - img * p.tiles_img;
-      const int ph = static_cast<int>(fast_div(ti, p.mg_tpp));
-      const int r = ti - ph * tiles_per_phase;
-      const int rn = static_cast<int>(fast_div(r, p.mg_tn));
-      const int nt = r - rn * p.tiles_n;
-      const int thi = static_cast<int>(fast_div(rn, p.mg_tw));
-      const int twi = rn - thi * p.tiles_w;
-      const int h = thi * p.TH + lh, w = twi * p.TW + lw, n0 = nt * p.BN;
+      const auto [img, ph, n0, h0, w0] = decode_tile(p, tile);
+      const int h = h0 + lh, w = w0 + lw;
 
       named_bar_sync(1, kEpilogue);         // the previous tile's epilogue is done with the bias row
-      if (et < BN) {
-        const int nn = n0 + et;
+      if (row < BN) {
+        const int nn = n0 + row;
         // upconv: the interior bias row (class 4); border pixels read theirs from global memory
-        s_bias[et] = (p.bias && nn < p.Cout) ? __ldg(p.bias + (p.upc ? 4 * p.Cout : 0) + nn) : 0.f;
+        s_bias[row] = (p.bias && nn < p.Cout) ? __ldg(p.bias + (p.upc ? 4 * p.Cout : 0) + nn) : 0.f;
       }
       named_bar_sync(1, kEpilogue);
       mbar_wait_quiet(smem_u32(&acc_full), acc_phase);
 
+      // output pixel of this row; ConvTranspose and upconv phase (a, b) writes pixel (2h + a, 2w + b)
+      const int oh = (p.phases > 1) ? 2 * h + (ph >> 1) : h;
+      const int ow = (p.phases > 1) ? 2 * w + (ph & 1) : w;
+      EpiPix px;
+      px.ok = (h < p.H) && (w < p.W);
+      px.ooff = img * p.out_img + static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
+      px.roff = img * p.res_img + static_cast<uint32_t>((oh + p.res_pad) * (Wo + 2 * p.res_pad) + (ow + p.res_pad)) * p.ldr;
+      px.fpix = static_cast<uint32_t>(h * p.W + w);
+      px.img = static_cast<uint32_t>(img);
       if (p.upc) {
         const int pa = ph >> 1, pb = ph & 1;
         // border class of this row's output pixel (2h + a, 2w + b): first / interior / last row and column
@@ -539,25 +478,10 @@ conv_wgmma_kernel(const __grid_constant__ ConvMaps maps, const ConvKParams p) {
         const int cx = (pb == 0 && w == 0) ? 0 : (pb == 1 && w == p.W - 1) ? 2 : 1;
         const int cls = cy * 3 + cx;
         const float* gb = cls != 4 ? p.bias + cls * p.Cout + n0 : nullptr;
-        const int oh = 2 * h + pa, ow = 2 * w + pb;
-        EpiPix px;
-        px.ok = (h < p.H) && (w < p.W);
-        px.zero = false;
-        px.ooff = img * p.out_img + static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
-        px.roff = 0; px.fpix = 0; px.img = 0;
-        if (p.act == ACT_GELU) epilogue_store_fast<E, ACT_GELU, false, true>(p, t_row, n0, s_bias, part, px, gb);
-        else epilogue_store_fast<E, ACT_NONE, false, true>(p, t_row, n0, s_bias, part, px, gb);
+        if (p.act == ACT_GELU) epilogue_store_fast<E, ACT_GELU, false, true>(p, t_row, n0, s_bias, px, gb);
+        else epilogue_store_fast<E, ACT_NONE, false, true>(p, t_row, n0, s_bias, px, gb);
       } else {
-        const int oh = (p.phases > 1) ? 2 * h + (ph >> 1) : h;
-        const int ow = (p.phases > 1) ? 2 * w + (ph & 1) : w;
-        EpiPix px;
-        px.ok = (h < p.H) && (w < p.W);
-        px.zero = false;
-        px.ooff = img * p.out_img + static_cast<uint32_t>((oh + p.out_pad) * (Wo + 2 * p.out_pad) + (ow + p.out_pad)) * p.ldo;
-        px.roff = img * p.res_img + static_cast<uint32_t>((oh + p.res_pad) * (Wo + 2 * p.res_pad) + (ow + p.res_pad)) * p.ldr;
-        px.fpix = static_cast<uint32_t>(h * p.W + w);
-        px.img = static_cast<uint32_t>(img);
-        epilogue_tile<E>(p, t_row, n0, s_bias, part, px);
+        epilogue_tile<E>(p, t_row, n0, s_bias, px);
       }
       mbar_arrive(smem_u32(&acc_empty));     // this thread's reads of the staged accumulator are done
       acc_phase ^= 1u;
@@ -660,6 +584,19 @@ static EncodeTiledFn get_encode_fn() {
       fn = reinterpret_cast<EncodeTiledFn>(p);
   }
   return fn;
+}
+
+// One 128-byte-swizzled operand map of the kernel (elements outside `dims` load as zeros); `name` identifies the map
+// in the error message.
+static int encode_map(CUtensorMap* m, const char* name, CUtensorMapDataType dt, int rank, const void* base,
+                      const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* es,
+                      CUtensorMapL2promotion l2) {
+  const CUresult r = get_encode_fn()(m, dt, rank, const_cast<void*>(base), dims, strides, box, es,
+                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, l2,
+                                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r == CUDA_SUCCESS) return VPB_OK;
+  vpb_set_error("conv: cuTensorMapEncodeTiled(%s) failed: %d", name, static_cast<int>(r));
+  return VPB_ERR_CUDA;
 }
 
 int device_sm_count() {
@@ -765,8 +702,7 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
       return VPB_ERR_ARG;
     }
   }
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) {
+  if (!get_encode_fn()) {
     vpb_set_error("conv: cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
     return VPB_ERR_CUDA;
   }
@@ -829,138 +765,95 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
 
   const CUtensorMapDataType dt =
       a->dtype == VPB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  CUresult r;
+  ConvMaps& m = plan->maps;
+  int rc;
   {
     // a zero-bordered input is addressed through its interior: base at pixel (1,1), padded pitch
-    auto encA = [&](const void* ptr, CUtensorMap* m) {
-      const int pad = p.in_pad;
-      const int Hin = (cstride == 2 && a->in_h > 0) ? a->in_h : a->H, Win = (cstride == 2 && a->in_w > 0) ? a->in_w : a->W;
-      const size_t pitch = static_cast<size_t>(Win + 2 * pad) * a->ldi * 2;
-      const uint8_t* base = static_cast<const uint8_t*>(ptr) + pad * pitch + static_cast<size_t>(pad) * a->ldi * 2;
-      cuuint64_t dims[4] = {static_cast<cuuint64_t>(a->Cin), static_cast<cuuint64_t>(Win),
-                            static_cast<cuuint64_t>(Hin), static_cast<cuuint64_t>(batch)};
-      cuuint64_t strides[3] = {static_cast<cuuint64_t>(a->ldi) * 2, pitch, pitch * (Hin + 2 * pad)};
-      // stride 2: the box spans 2*TW x 2*TH input pixels and is traversed with element stride 2 (TW x TH loaded)
-      cuuint32_t box[4] = {64, static_cast<cuuint32_t>(p.TW * cstride), static_cast<cuuint32_t>(p.TH * cstride), 1};
-      cuuint32_t es[4] = {1, static_cast<cuuint32_t>(cstride), static_cast<cuuint32_t>(cstride), 1};
-      return enc(m, dt, 4, const_cast<uint8_t*>(base), dims, strides, box, es,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    };
-    r = encA(a->in, &plan->mapA);
-    if (r == CUDA_SUCCESS && split) r = encA(a->in_lo, &plan->mapAlo);
-  }
-  if (r != CUDA_SUCCESS) {
-    vpb_set_error("conv: cuTensorMapEncodeTiled(A) failed: %d", static_cast<int>(r));
-    return VPB_ERR_CUDA;
+    const int pad = p.in_pad;
+    const int Hin = (cstride == 2 && a->in_h > 0) ? a->in_h : a->H, Win = (cstride == 2 && a->in_w > 0) ? a->in_w : a->W;
+    const size_t pitch = static_cast<size_t>(Win + 2 * pad) * a->ldi * 2;
+    const size_t skip = pad * pitch + static_cast<size_t>(pad) * a->ldi * 2;
+    const cuuint64_t dims[4] = {static_cast<cuuint64_t>(a->Cin), static_cast<cuuint64_t>(Win),
+                                static_cast<cuuint64_t>(Hin), static_cast<cuuint64_t>(batch)};
+    const cuuint64_t strides[3] = {static_cast<cuuint64_t>(a->ldi) * 2, pitch, pitch * (Hin + 2 * pad)};
+    // stride 2: the box spans 2*TW x 2*TH input pixels and is traversed with element stride 2 (TW x TH loaded)
+    const cuuint32_t box[4] = {64, static_cast<cuuint32_t>(p.TW * cstride), static_cast<cuuint32_t>(p.TH * cstride), 1};
+    const cuuint32_t es[4] = {1, static_cast<cuuint32_t>(cstride), static_cast<cuuint32_t>(cstride), 1};
+    if ((rc = encode_map(&m.A, "A", dt, 4, static_cast<const uint8_t*>(a->in) + skip, dims, strides, box, es,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B)))
+      return rc;
+    if (split && (rc = encode_map(&m.Alo, "Alo", dt, 4, static_cast<const uint8_t*>(a->in_lo) + skip, dims, strides, box,
+                                  es, CU_TENSOR_MAP_L2_PROMOTION_L2_128B)))
+      return rc;
   }
   {
-    auto encB = [&](const void* ptr, CUtensorMap* m) {
-      // w_img != 0: the third dimension is the image instead of the tap / phase
-      const size_t ldw = a->ldw > 0 ? a->ldw : a->Cin;
-      cuuint64_t dims[3] = {static_cast<cuuint64_t>(a->Cin), static_cast<cuuint64_t>(a->Cout),
-                            static_cast<cuuint64_t>(a->w_img ? batch : a->taps * a->phases)};
-      cuuint64_t strides[2] = {static_cast<cuuint64_t>(ldw) * 2,
-                               a->w_img ? static_cast<cuuint64_t>(a->w_img) * 2 : static_cast<cuuint64_t>(ldw) * 2 * a->Cout};
-      cuuint32_t box[3] = {64, static_cast<cuuint32_t>(p.BN), 1};
-      cuuint32_t es[3] = {1, 1, 1};
-      return enc(m, dt, 3, const_cast<void*>(ptr), dims, strides, box, es,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    };
-    r = encB(a->w, &plan->mapB);
-    if (r == CUDA_SUCCESS && split) r = encB(a->w_lo, &plan->mapBlo);
-    if (r != CUDA_SUCCESS) {
-      vpb_set_error("conv: cuTensorMapEncodeTiled(B) failed: %d", static_cast<int>(r));
-      return VPB_ERR_CUDA;
-    }
+    // w_img != 0: the third dimension is the image instead of the tap / phase
+    const size_t ldw = a->ldw > 0 ? a->ldw : a->Cin;
+    const cuuint64_t dims[3] = {static_cast<cuuint64_t>(a->Cin), static_cast<cuuint64_t>(a->Cout),
+                                static_cast<cuuint64_t>(a->w_img ? batch : a->taps * a->phases)};
+    const cuuint64_t strides[2] = {static_cast<cuuint64_t>(ldw) * 2,
+                                   a->w_img ? static_cast<cuuint64_t>(a->w_img) * 2 : static_cast<cuuint64_t>(ldw) * 2 * a->Cout};
+    const cuuint32_t box[3] = {64, static_cast<cuuint32_t>(p.BN), 1};
+    const cuuint32_t es[3] = {1, 1, 1};
+    if ((rc = encode_map(&m.B, "B", dt, 3, a->w, dims, strides, box, es, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if (split && (rc = encode_map(&m.Blo, "Blo", dt, 3, a->w_lo, dims, strides, box, es, CU_TENSOR_MAP_L2_PROMOTION_L2_256B)))
+      return rc;
   }
-  plan->mapA2 = plan->mapA;
-  plan->mapB2 = plan->mapB;
-  if (!split) { plan->mapAlo = plan->mapA; plan->mapBlo = plan->mapB; }
-  plan->mapA2lo = plan->mapAlo;
-  plan->mapB2lo = plan->mapBlo;
+  // the maps a layer does not use are copies of the first input's (the kernel reads only the ones it uses)
+  if (!split) { m.Alo = m.A; m.Blo = m.B; }
+  m.A2 = m.A; m.B2 = m.B; m.A2lo = m.Alo; m.B2lo = m.Blo;
   if (a->in2) {
     // second input at output resolution [batch][s*H][s*W][ld2] (s = 2 for a ConvTranspose, 1 otherwise), addressed
     // like the first input through its interior; the box spans s*TW x s*TH pixels traversed with element stride s,
     // so a tile loads the TW x TH pixels of one phase, and rows / columns outside an image (the upconv's skip taps
     // at hi-res row -1 and 2H) are the TMA unit's zero fill, per image
-    auto encA2 = [&](const void* ptr, CUtensorMap* m) {
-      const int s2 = a->phases == 4 ? 2 : 1;
-      const int pad = a->in2_pad ? 1 : 0;
-      const size_t px = static_cast<size_t>(a->ld2) * 2;                       // bytes per pixel
-      const size_t pitch = static_cast<size_t>(a->W * s2 + 2 * pad) * px;      // bytes per image row
-      const uint8_t* base = static_cast<const uint8_t*>(ptr) + pad * pitch + pad * px;
-      cuuint64_t dims[4] = {static_cast<cuuint64_t>(a->Cin2), static_cast<cuuint64_t>(a->W * s2),
-                            static_cast<cuuint64_t>(a->H * s2), static_cast<cuuint64_t>(batch)};
-      cuuint64_t strides[3] = {px, pitch, pitch * (a->H * s2 + 2 * pad)};
-      cuuint32_t box[4] = {64, static_cast<cuuint32_t>(p.TW * s2), static_cast<cuuint32_t>(p.TH * s2), 1};
-      cuuint32_t es[4] = {1, static_cast<cuuint32_t>(s2), static_cast<cuuint32_t>(s2), 1};
-      return enc(m, dt, 4, const_cast<uint8_t*>(base), dims, strides, box, es,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    };
-    r = encA2(a->in2, &plan->mapA2);
-    if (r == CUDA_SUCCESS && split) r = encA2(a->in2_lo, &plan->mapA2lo);
-    if (r != CUDA_SUCCESS) {
-      vpb_set_error("conv: cuTensorMapEncodeTiled(A2) failed: %d", static_cast<int>(r));
-      return VPB_ERR_CUDA;
-    }
-    auto encB2 = [&](const void* ptr, CUtensorMap* m) {
-      cuuint64_t bd[3] = {static_cast<cuuint64_t>(a->Cin2), static_cast<cuuint64_t>(a->Cout), static_cast<cuuint64_t>(p.upc ? 9 : 1)};
-      cuuint64_t bs[2] = {static_cast<cuuint64_t>(a->Cin2) * 2, static_cast<cuuint64_t>(a->Cin2) * 2 * a->Cout};
-      cuuint32_t bb[3] = {64, static_cast<cuuint32_t>(p.BN), 1};
-      cuuint32_t be[3] = {1, 1, 1};
-      return enc(m, dt, 3, const_cast<void*>(ptr), bd, bs, bb, be,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    };
-    r = encB2(a->w2, &plan->mapB2);
-    if (r == CUDA_SUCCESS && split) r = encB2(a->w2_lo, &plan->mapB2lo);
-    if (r != CUDA_SUCCESS) {
-      vpb_set_error("conv: cuTensorMapEncodeTiled(B2) failed: %d", static_cast<int>(r));
-      return VPB_ERR_CUDA;
-    }
+    const int s2 = a->phases == 4 ? 2 : 1;
+    const int pad = a->in2_pad ? 1 : 0;
+    const size_t px = static_cast<size_t>(a->ld2) * 2;                       // bytes per pixel
+    const size_t pitch = static_cast<size_t>(a->W * s2 + 2 * pad) * px;      // bytes per image row
+    const size_t skip = pad * pitch + pad * px;
+    const cuuint64_t dims[4] = {static_cast<cuuint64_t>(a->Cin2), static_cast<cuuint64_t>(a->W * s2),
+                                static_cast<cuuint64_t>(a->H * s2), static_cast<cuuint64_t>(batch)};
+    const cuuint64_t strides[3] = {px, pitch, pitch * (a->H * s2 + 2 * pad)};
+    const cuuint32_t box[4] = {64, static_cast<cuuint32_t>(p.TW * s2), static_cast<cuuint32_t>(p.TH * s2), 1};
+    const cuuint32_t es[4] = {1, static_cast<cuuint32_t>(s2), static_cast<cuuint32_t>(s2), 1};
+    if ((rc = encode_map(&m.A2, "A2", dt, 4, static_cast<const uint8_t*>(a->in2) + skip, dims, strides, box, es,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B)))
+      return rc;
+    if (split && (rc = encode_map(&m.A2lo, "A2lo", dt, 4, static_cast<const uint8_t*>(a->in2_lo) + skip, dims, strides,
+                                  box, es, CU_TENSOR_MAP_L2_PROMOTION_L2_128B)))
+      return rc;
+    const cuuint64_t bd[3] = {static_cast<cuuint64_t>(a->Cin2), static_cast<cuuint64_t>(a->Cout), static_cast<cuuint64_t>(p.upc ? 9 : 1)};
+    const cuuint64_t bs[2] = {static_cast<cuuint64_t>(a->Cin2) * 2, static_cast<cuuint64_t>(a->Cin2) * 2 * a->Cout};
+    const cuuint32_t bb[3] = {64, static_cast<cuuint32_t>(p.BN), 1};
+    const cuuint32_t be[3] = {1, 1, 1};
+    if ((rc = encode_map(&m.B2, "B2", dt, 3, a->w2, bd, bs, bb, be, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if (split && (rc = encode_map(&m.B2lo, "B2lo", dt, 3, a->w2_lo, bd, bs, bb, be, CU_TENSOR_MAP_L2_PROMOTION_L2_256B)))
+      return rc;
   }
-  return VPB_OK;
   return VPB_OK;
 }
 
-template <class E, int BN>
-static cudaError_t set_smem_attr() {
-  return cudaFuncSetAttribute(conv_wgmma_kernel<E, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
-}
-
-template <class E>
-static cudaError_t launch_conv(const ConvPlan* plan, const ConvMaps& maps, cudaStream_t stream) {
-  const dim3 g(plan->grid), b(kThreads);
-  switch (plan->p.BN) {
-    case 16: return launch_k(conv_wgmma_kernel<E, 16>, g, b, plan->smem_bytes, stream, maps, plan->p);
-    case 32: return launch_k(conv_wgmma_kernel<E, 32>, g, b, plan->smem_bytes, stream, maps, plan->p);
-    case 64: return launch_k(conv_wgmma_kernel<E, 64>, g, b, plan->smem_bytes, stream, maps, plan->p);
-    default: return launch_k(conv_wgmma_kernel<E, 128>, g, b, plan->smem_bytes, stream, maps, plan->p);
-  }
-}
+// Every instantiation of the kernel, [dtype == VPB_BF16][log2(BN / 16)]
+static void (*const kConvKernels[2][4])(ConvMaps, ConvKParams) = {
+    {conv_wgmma_kernel<F16, 16>, conv_wgmma_kernel<F16, 32>, conv_wgmma_kernel<F16, 64>, conv_wgmma_kernel<F16, 128>},
+    {conv_wgmma_kernel<BF16, 16>, conv_wgmma_kernel<BF16, 32>, conv_wgmma_kernel<BF16, 64>, conv_wgmma_kernel<BF16, 128>},
+};
 
 int conv_plan_launch(const ConvPlan* plan, cudaStream_t stream) {
   {
     std::lock_guard<std::mutex> g(init_mutex());
     bool* done = device_flag(kInitConv);
     if (!*done) {
-      VPB_CUDA_OK((set_smem_attr<F16, 16>())); VPB_CUDA_OK((set_smem_attr<F16, 32>()));
-      VPB_CUDA_OK((set_smem_attr<F16, 64>())); VPB_CUDA_OK((set_smem_attr<F16, 128>()));
-      VPB_CUDA_OK((set_smem_attr<BF16, 16>())); VPB_CUDA_OK((set_smem_attr<BF16, 32>()));
-      VPB_CUDA_OK((set_smem_attr<BF16, 64>())); VPB_CUDA_OK((set_smem_attr<BF16, 128>()));
+      for (const auto& by_bn : kConvKernels)
+        for (const auto k : by_bn) VPB_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
       *done = true;
     }
   }
-  ConvMaps maps;
-  maps.A = plan->mapA; maps.B = plan->mapB; maps.A2 = plan->mapA2; maps.B2 = plan->mapB2;
-  maps.Alo = plan->mapAlo; maps.Blo = plan->mapBlo; maps.A2lo = plan->mapA2lo; maps.B2lo = plan->mapB2lo;
-  if (plan->dtype == VPB_BF16) VPB_CUDA_OK(launch_conv<BF16>(plan, maps, stream));
-  else VPB_CUDA_OK(launch_conv<F16>(plan, maps, stream));
-  if (plan->p.lin) {
-    const ConvKParams& p = plan->p;
+  const ConvKParams& p = plan->p;
+  const auto kernel = kConvKernels[plan->dtype == VPB_BF16][__builtin_ctz(p.BN >> 4)];
+  VPB_CUDA_OK(launch_k(kernel, dim3(plan->grid), dim3(kThreads), plan->smem_bytes, stream, plan->maps, p));
+  if (p.lin) {
     const int n = (2 * (p.W + 2) + 2 * p.H) * (p.nlim >> 3);
     VPB_CUDA_OK(launch_k(zero_border_kernel, dim3(std::min((n + 255) / 256, 256), p.total_tiles / p.tiles_img), dim3(256), 0, stream,
                          static_cast<uint4*>(p.out), p.H, p.W, p.ldo, p.nlim));

@@ -51,9 +51,7 @@ struct ConvMaps {
 };
 
 struct ConvPlan {
-  CUtensorMap mapA, mapB;
-  CUtensorMap mapA2, mapB2;      // second 1x1 input and its weights (copies of mapA/mapB when unused)
-  CUtensorMap mapAlo, mapBlo, mapA2lo, mapB2lo;
+  ConvMaps maps;
   ConvKParams p;
   int dtype;
   int grid;

@@ -127,8 +127,8 @@ struct vp_engine : EngineRuntime {
     a.in_pad = in.pad;
     if (out) { a.out = out->p; a.ldo = out->ld; a.out_pad = out->pad; }
     if (res) { a.res = res->p; a.ldr = res->ld; a.res_pad = res->pad; }
-    // 3x3 on a zero-bordered input -> linear-padded kernel (one TMA segment per kernel row); the split-fp16 mode
-    // runs everything on the tile kernel (three K segments per chunk)
+    // 3x3 on a zero-bordered input -> LINEAR: the layer also writes its output's zero border, so the next 3x3 layer
+    // reads it as it stands; the split-fp16 mode runs everything as TILE (three K segments per chunk)
     a.algo = (taps == 9 && in.pad && !split) ? VPB_ALGO_LINEAR : VPB_ALGO_TILE;
     if (split) {
       a.in_lo = in.lo; a.w_lo = lo(w);

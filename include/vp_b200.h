@@ -141,8 +141,9 @@ typedef struct {
 } vp_engine_stats;
 int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s);
 /* Eagerly run one frame with a CUDA-event pair around every kernel; returns the per-kernel
- * device times (ms) in launch order; is_gemm[i] != 0 for the wgmma convolution launches
- * (1 = conv_gemm_kernel, 2 = conv3x3_lin_kernel, 3 = conv3x3_pair_kernel), 0 otherwise.
+ * device times (ms) in launch order; is_gemm[i] != 0 for the convolution launches, all of which run
+ * conv_wgmma_kernel: 1 = the TILE algorithm, 2 = LINEAR (TILE plus the zero-border pass of a padded
+ * output), 0 otherwise.
  * names[i] point into engine-owned storage. */
 int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* flops, const char** names,
                       int* is_gemm, int* n_ops);
@@ -153,7 +154,7 @@ int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* flops, const
  * more memory than L2 holds. */
 int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flops, int* launches);
 /* Per-kernel form of the above for the roofline report: the distinct kernel names of the frame
- * ("preprocess", "stem_conv_kernel", "depthwise_kernel", "se_scale_kernel", "conv3x3_pair_kernel", ...), and
+ * ("preprocess", "stem_conv_kernel", "depthwise_kernel", "se_scale_kernel", "conv_wgmma_kernel", ...), and
  * all launches of one of them issued back to back `reps` times between ONE CUDA-event pair (after an untimed
  * pass).  flops = algorithmic 2*MAC, bytes = algorithmic HBM bytes (SURVEY.md 8d definitions: tensors in +
  * out of the stage) of the timed launches.  A large `reps` (seconds of device time) makes it a sustained

@@ -20,8 +20,8 @@ def pad_img(x):
 
 def conv_gemm(x_nhwc, w_tnc, bias, *, taps, phases=1, act=L.ACT_NONE, mode=L.EPI_STORE,
               res=None, final_kind=L.FINAL_NONE, cout=None, ldo=None, bn=0, dtype=L.VPB_F16,
-              cin=None, in_pad=0, out_pad=0, res_pad=0, algo=L.ALGO_TILE, set_bo=0, ms=0, gb=0,
-              in2=None, w2=None, in2_pad=0, pair=0, splitk=0, taps2=0):
+              cin=None, in_pad=0, out_pad=0, res_pad=0, algo=L.ALGO_TILE,
+              in2=None, w2=None, in2_pad=0, taps2=0):
     """x_nhwc [H,W,ldi] 16-bit cuda (or zero-bordered [H+2,W+2,ldi] with in_pad=1), w_tnc
     [taps*phases,Cout,Cin] 16-bit cuda, bias fp32 or None.  With out_pad=1 the returned tensor is the
     zero-bordered [(Ho+2),(Wo+2),ldo] image (pre-filled with NaN for the LINEAR algorithm, which must
@@ -41,8 +41,7 @@ def conv_gemm(x_nhwc, w_tnc, bias, *, taps, phases=1, act=L.ACT_NONE, mode=L.EPI
     a.inp, a.w = x_nhwc.data_ptr(), w_tnc.data_ptr()
     a.bias = bias.data_ptr() if bias is not None else None
     a.bn = bn
-    a.in_pad, a.out_pad, a.res_pad, a.algo, a.dbg_base_offset = in_pad, out_pad, res_pad, algo, set_bo
-    a.dbg_ms, a.dbg_gb, a.dbg_pair, a.dbg_splitk = ms, gb, pair, splitk
+    a.in_pad, a.out_pad, a.res_pad, a.algo = in_pad, out_pad, res_pad, algo
     if in2 is not None:   # fused second 1x1 input at output resolution: [Ho(+2),Wo(+2),ld2], w2 [Cout,Cin2]
         a.in2, a.w2 = in2.data_ptr(), w2.data_ptr()
         a.Cin2, a.ld2, a.in2_pad = w2.shape[-1], in2.shape[2], in2_pad

@@ -129,10 +129,10 @@ def test_conv_transpose_phases(H, W, Cin, Cout):
     (10, 20, 128, 128, 112, 0, 1),     # neck block 0 shape class: skip = f3 (112 ch, K tail 64+48)
     (20, 40, 96, 72, 40, 0, 0),        # K tails on both inputs, N tail
     (40, 80, 64, 256, 24, 1, 1),       # zero-bordered skip tensor
-    (80, 160, 256, 256, 16, 0, 1),     # up3 of the SceneSeg head at full size (skip = f0, 16 ch): weight-stationary pair kernel, N tile 256
-    (40, 80, 512, 512, 24, 0, 1),      # upsample_layer_2 of the neck (skip = f1): 9 K chunks x 13 tile pairs -> stays on the tile kernel (plan heuristic)
-    (80, 160, 256, 200, 32, 1, 1),     # weight-stationary kernel with an N tail and a zero-bordered skip tensor
-    (20, 40, 768, 768, 40, 0, 1),      # upsample_layer_1 (7 pixel tiles: an odd count, the last pair is half empty)
+    (80, 160, 256, 256, 16, 0, 1),     # up3 of the SceneSeg head at full size (skip = f0, 16 ch)
+    (40, 80, 512, 512, 24, 0, 1),      # upsample_layer_2 of the neck (skip = f1)
+    (80, 160, 256, 200, 32, 1, 1),     # N tail and a zero-bordered skip tensor
+    (20, 40, 768, 768, 40, 0, 1),      # upsample_layer_1 (7 pixel tiles)
     (36, 52, 128, 128, 16, 0, 0),      # ragged pixel tiles
 ])
 def test_conv_transpose_with_fused_skip_link(H, W, Cin, Cout, C2, pad2, out_pad):

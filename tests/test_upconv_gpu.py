@@ -1,5 +1,5 @@
-"""Fused ConvTranspose2d(k2,s2) [+ Conv1x1 skip] -> Conv3x3 + bias + GELU ("upconv", upconv_pair_kernel) against the
-reference's two-layer form (scene_neck.py:30-37, scene_seg_head.py:25-33) computed by torch in fp32 / fp64.
+"""Fused ConvTranspose2d(k2,s2) [+ Conv1x1 skip] -> Conv3x3 + bias [+ GELU] ("upconv", one composed GEMM on
+conv_wgmma_kernel) against the reference's two-layer form (scene_neck.py:30-37, scene_seg_head.py:25-33) computed by torch in fp32 / fp64.
 
 Three gates: (1) vpb_upconv_compose's weights and 9-class bias against an fp64 composition written here from the
 layer definitions, (2) the kernel against an fp32 emulation that uses the SAME 16-bit composed operands (tight: only
@@ -100,19 +100,20 @@ def _emulate(x, s, wf16, w2f16, b9, act):
     return out.permute(1, 2, 0)
 
 
-@pytest.mark.parametrize("gb", [0, 3], ids=["direct_store", "tma_store"])
-@pytest.mark.parametrize("H,W,Cin,Cmid,Cout,C2,bn,pads,dtype,act", [
-    (10, 20, 128, 128, 128, 0, 0, 0, L.VPB_F16, L.ACT_GELU),
-    (20, 40, 256, 256, 256, 32, 0, 0, L.VPB_F16, L.ACT_GELU),      # skip link, N tile 256
-    (12, 20, 64, 96, 64, 24, 0, 0, L.VPB_F16, L.ACT_GELU),         # ragged tiles, C2 = 24 (half-empty K chunk), N tile 64
-    (40, 80, 128, 128, 128, 0, 0, 1, L.VPB_F16, L.ACT_GELU),       # zero-bordered input and output (the engine's layout)
-    (20, 40, 192, 128, 256, 40, 128, 1, L.VPB_F16, L.ACT_NONE),    # K tail (192 = 3 chunks), forced N tile 128, no activation
-    (9, 17, 64, 64, 128, 0, 64, 0, L.VPB_F16, L.ACT_GELU),         # odd sizes: odd number of pixel tiles in a pair
-    (20, 40, 128, 128, 128, 32, 0, 0, L.VPB_BF16, L.ACT_GELU),
-    (10, 20, 72, 64, 64, 80, 0, 1, L.VPB_F16, L.ACT_GELU),         # K tails on both inputs: Cin = 64 + 8, C2 = 64 + 16 (f3 of the encoder)
-    (10, 20, 320, 256, 768, 80, 0, 1, L.VPB_F16, L.ACT_GELU),      # three N tiles of 256 (decode_layer_0 has Cout = 768), one pixel-tile pair
+# the upconv epilogue has one variant per activation: GELU (the neck and heads) and none
+@pytest.mark.parametrize("act", [L.ACT_GELU, L.ACT_NONE], ids=["gelu", "no_act"])
+@pytest.mark.parametrize("H,W,Cin,Cmid,Cout,C2,bn,pads,dtype", [
+    (10, 20, 128, 128, 128, 0, 0, 0, L.VPB_F16),
+    (20, 40, 256, 256, 256, 32, 0, 0, L.VPB_F16),      # skip link, N tile 128 (two N tiles)
+    (12, 20, 64, 96, 64, 24, 0, 0, L.VPB_F16),         # ragged tiles, C2 = 24 (half-empty K chunk), N tile 64
+    (40, 80, 128, 128, 128, 0, 0, 1, L.VPB_F16),       # zero-bordered input and output (the engine's layout)
+    (20, 40, 192, 128, 256, 40, 128, 1, L.VPB_F16),    # K tail (192 = 3 chunks), forced N tile 128
+    (9, 17, 64, 64, 128, 0, 64, 0, L.VPB_F16),         # odd sizes, forced N tile 64
+    (20, 40, 128, 128, 128, 32, 0, 0, L.VPB_BF16),
+    (10, 20, 72, 64, 64, 80, 0, 1, L.VPB_F16),         # K tails on both inputs: Cin = 64 + 8, C2 = 64 + 16 (f3 of the encoder)
+    (10, 20, 320, 256, 768, 80, 0, 1, L.VPB_F16),      # six N tiles of 128 (decode_layer_0 has Cout = 768)
 ])
-def test_upconv_matches_two_layer_reference(H, W, Cin, Cmid, Cout, C2, bn, pads, dtype, act, gb):
+def test_upconv_matches_two_layer_reference(H, W, Cin, Cmid, Cout, C2, bn, pads, dtype, act):
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     from tests.gpu_util import conv_gemm, pad_img, tdtype
@@ -137,7 +138,7 @@ def test_upconv_matches_two_layer_reference(H, W, Cin, Cmid, Cout, C2, bn, pads,
     w2f16 = w2f.to(td) if C2 else None
     _, _, out = conv_gemm(pad_img(x) if pads else x, wf16, b9, taps=4, phases=4, act=act, dtype=dtype, bn=bn,
                           in_pad=pads, out_pad=pads, in2=(pad_img(s) if pads else s) if C2 else None, w2=w2f16,
-                          in2_pad=pads, taps2=9 if C2 else 0, gb=gb)
+                          in2_pad=pads, taps2=9 if C2 else 0)
     if pads:
         assert (out[0].float() == 0).all() and (out[-1].float() == 0).all()
         assert (out[:, 0].float() == 0).all() and (out[:, -1].float() == 0).all()

@@ -44,6 +44,27 @@ class ConvArgs(C.Structure):
     ]
 
 
+class Frame(C.Structure):
+    """Mirror of vpb_frame (include/vp_b200_ops.h): uint8 HWC, 3 channels, `stride` bytes per row."""
+
+    _fields_ = [("data", C.c_void_p), ("h", C.c_int), ("w", C.c_int), ("stride", C.c_int)]
+
+
+def frame_descs(descs) -> "C.Array":
+    """(data_ptr, h, w, stride) tuples as a vpb_frame array; ValueError for a malformed one (before any C call)."""
+    descs = list(descs)
+    arr = (Frame * max(len(descs), 1))()
+    for k, d in enumerate(descs):
+        if len(d) != 4:
+            raise ValueError(f"frame {k}: need (data_ptr, h, w, stride), got {d!r}")
+        ptr, h, w, stride = (int(v) for v in d)
+        if not ptr or h <= 0 or w <= 0 or stride < 3 * w:
+            raise ValueError(f"frame {k}: bad descriptor (ptr {ptr:#x}, h {h}, w {w}, stride {stride}): need a non-NULL "
+                             "pointer, h, w > 0 and stride >= 3*w")
+        arr[k] = Frame(ptr, h, w, stride)
+    return arr
+
+
 class LateralState(C.Structure):
     """Mirror of vpb_lateral_state (device-resident, persistent)."""
 

@@ -27,6 +27,8 @@ def _bind():
     lib.vp_autospeed_infer_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     lib.vp_autospeed_infer_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     lib.vp_autospeed_infer_device_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.vp_autospeed_infer_frames.argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int, C.c_int]
+    lib.vp_autospeed_infer_device_frames.argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int]
     lib.vp_autospeed_sync.argtypes = [C.c_void_p, C.c_int]
     lib.vp_autospeed_detections.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.vp_autospeed_raw.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
@@ -116,6 +118,25 @@ class AutoSpeedEngine:
         ptrs = (C.c_void_p * len(dev_ptrs))(*dev_ptrs)
         L.check(self._lib.vp_autospeed_infer_device_batch(self._h, ptrs, len(dev_ptrs), h, w, stride),
                 "vp_autospeed_infer_device_batch")
+
+    def infer_frames(self, frames: Sequence[np.ndarray], fetch_raw: bool = False) -> List[np.ndarray]:
+        """`batch` uint8 [h_k, w_k, 3] RGB frames, each of its own size, in one call (each gets its own letterbox)
+        -> detections of frame k, in frame k's pixels, at index k."""
+        frames = list(frames)
+        self._check_count(len(frames))
+        frames = [self._check_frame(f) for f in frames]
+        descs = L.frame_descs([(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames])
+        L.check(self._lib.vp_autospeed_infer_frames(self._h, descs, len(frames), int(fetch_raw)),
+                "vp_autospeed_infer_frames")
+        return [self.detections(k) for k in range(self.batch)]
+
+    def infer_device_frames(self, descs: Sequence[Sequence[int]]) -> None:
+        """`batch` device frames as (data_ptr, h, w, stride) tuples, each of its own geometry, enqueued as one call;
+        sync() completes it."""
+        descs = list(descs)
+        self._check_count(len(descs))
+        L.check(self._lib.vp_autospeed_infer_device_frames(self._h, L.frame_descs(descs), len(descs)),
+                "vp_autospeed_infer_device_frames")
 
     def sync(self, fetch: int = 1) -> None:
         L.check(self._lib.vp_autospeed_sync(self._h, fetch), "vp_autospeed_sync")

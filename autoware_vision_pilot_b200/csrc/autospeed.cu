@@ -238,26 +238,35 @@ __global__ void decode_kernel(const typename E::T* __restrict__ lvl, int h, int 
 //   scores = max_c sigmoid(cls) (the SECOND sigmoid, :78), keep scores > conf, xywh -> xyxy, greedy class-agnostic
 //   NMS (torchvision.ops.nms: descending score, stable for ties, suppress IoU > thr), map back to the source frame.
 // det [max_det][6] = x1, y1, x2, y2, score, class;  n_det = number kept (<= max_det; n_cand = candidates seen).
-// One block per image (blockIdx.x): every buffer below is per image, sample outermost; the thresholds are shared.
-struct PostParams {
+// One block per image (blockIdx.x): every buffer below is per image, sample outermost; the thresholds are shared and
+// the letterbox (scale, padding, source size) is the image's own.
+struct PostImage {
   const float* raw; int NA; float conf, iou; float scale; int pad_x, pad_y, orig_w, orig_h; int max_cand, max_det;
   float* cand;     // [max_cand][6] scratch (xyxy, score, class)
   int* order;      // [max_cand] scratch
   float* det; int* counts;   // counts[0] = n_det, counts[1] = n_cand
 };
-static PostParams __device__ __forceinline__ post_image(PostParams p, size_t img) {
-  p.raw += img * 8 * p.NA;
-  p.cand += img * p.max_cand * 6;
-  p.order += img * p.max_cand;
-  p.det += img * p.max_det * 6;
-  p.counts += img * 2;
-  return p;
+struct PostParams {  // by value: the buffers of image 0 and the letterbox of every image
+  const float* raw; int NA; float conf, iou; int max_cand, max_det;
+  float* cand; int* order; float* det; int* counts;
+  float scale[kMaxBatch]; int pad_x[kMaxBatch], pad_y[kMaxBatch], orig_w[kMaxBatch], orig_h[kMaxBatch];
+};
+static PostImage __device__ __forceinline__ post_image(const PostParams& p, int img) {
+  PostImage q;
+  q.raw = p.raw + static_cast<size_t>(img) * 8 * p.NA; q.NA = p.NA; q.conf = p.conf; q.iou = p.iou;
+  q.scale = p.scale[img]; q.pad_x = p.pad_x[img]; q.pad_y = p.pad_y[img]; q.orig_w = p.orig_w[img]; q.orig_h = p.orig_h[img];
+  q.max_cand = p.max_cand; q.max_det = p.max_det;
+  q.cand = p.cand + static_cast<size_t>(img) * p.max_cand * 6;
+  q.order = p.order + static_cast<size_t>(img) * p.max_cand;
+  q.det = p.det + static_cast<size_t>(img) * p.max_det * 6;
+  q.counts = p.counts + static_cast<size_t>(img) * 2;
+  return q;
 }
 template <bool kBatch>
-__global__ void __launch_bounds__(1024) postprocess_kernel(const PostParams p_) {
+__global__ void __launch_bounds__(1024) postprocess_kernel(const __grid_constant__ PostParams p_) {
   pdl_launch_dependents();
   pdl_wait();
-  const PostParams p = kBatch ? post_image(p_, blockIdx.x) : p_;
+  const PostImage p = post_image(p_, kBatch ? static_cast<int>(blockIdx.x) : 0);
   __shared__ int s_n;
   __shared__ int s_scan[1024];
   const int tid = threadIdx.x;
@@ -368,7 +377,8 @@ struct vp_autospeed : EngineRuntime {
   float* d_cand = nullptr; int* d_order = nullptr; float* d_det = nullptr; int* d_counts = nullptr;
   float* h_det = nullptr; int* h_counts = nullptr;
   long long* d_gap_scratch = nullptr;
-  int src_w = 0, src_h = 0; float scale = 1.f; int pad_x = 0, pad_y = 0, new_w = 0, new_h = 0;
+  float scale[kMaxBatch] = {};             // letterbox of each sample of the last call (geometry in pre.geom)
+  PreGeom canvas_geom[kMaxBatch];          // the letterbox each sample's canvas border was last filled for
   float conf = 0.6f, iou = 0.45f;
   static constexpr int kMaxCand = 4096, kMaxDet = 1024;
 
@@ -703,13 +713,17 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   return VPB_OK;
 }
 
-static int as_launch_all(vp_autospeed& e, const uint8_t* const* srcs, int stride, cudaStream_t st) {
-  int rc = e.pre.launch(srcs, e.batch, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr, st);
+static int as_launch_all(vp_autospeed& e, const vpb_frame* frames, cudaStream_t st) {
+  int rc = e.pre.launch(frames, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr, st);
   if (rc) return rc;
   for (auto& op : e.ops) { rc = op.launch(st); if (rc) return rc; }
   PostParams pp{};
-  pp.raw = e.d_raw; pp.NA = kNA; pp.conf = e.conf; pp.iou = e.iou; pp.scale = e.scale; pp.pad_x = e.pad_x; pp.pad_y = e.pad_y;
-  pp.orig_w = e.src_w; pp.orig_h = e.src_h; pp.max_cand = vp_autospeed::kMaxCand; pp.max_det = vp_autospeed::kMaxDet;
+  pp.raw = e.d_raw; pp.NA = kNA; pp.conf = e.conf; pp.iou = e.iou;
+  for (int k = 0; k < e.batch; ++k) {
+    const PreGeom& g = e.pre.geom[k];
+    pp.scale[k] = e.scale[k]; pp.pad_x[k] = g.x0; pp.pad_y[k] = g.y0; pp.orig_w[k] = g.w; pp.orig_h[k] = g.h;
+  }
+  pp.max_cand = vp_autospeed::kMaxCand; pp.max_det = vp_autospeed::kMaxDet;
   pp.cand = e.d_cand; pp.order = e.d_order; pp.det = e.d_det; pp.counts = e.d_counts;
   const size_t smem = vp_autospeed::kMaxCand;
   if (e.batch > 1) VPB_CUDA_OK(launch_k(postprocess_kernel<true>, dim3(e.batch), dim3(1024), smem, st, pp));
@@ -717,37 +731,51 @@ static int as_launch_all(vp_autospeed& e, const uint8_t* const* srcs, int stride
   return VPB_OK;
 }
 
-// letterbox geometry (auto_speed_infer.py:31-43), shared by every sample of a call
-static int as_configure(vp_autospeed& e, int h, int w) {
-  if (h == e.src_h && w == e.src_w) return VPB_OK;
+// letterbox geometry (auto_speed_infer.py:31-43) of an h x w frame; VPB_ERR_ARG (naming `who` and frame k) if it
+// cannot be resized.  Host-only.
+static int as_letterbox(int h, int w, const char* who, int k, PreGeom* g, float* scale) {
   const double sc = std::min(static_cast<double>(kASW) / w, static_cast<double>(kASH) / h);
   const int nw = static_cast<int>(w * sc), nh = static_cast<int>(h * sc);
-  if (nw < 1 || nh < 1) { vpb_set_error("autospeed: frame %dx%d too small", w, h); return VPB_ERR_ARG; }
-  e.scale = static_cast<float>(sc); e.new_w = nw; e.new_h = nh; e.pad_x = (kASW - nw) / 2; e.pad_y = (kASH - nh) / 2;
-  e.pre.OW = nw; e.pre.OH = nh; e.pre.out_pitch = kASW; e.pre.out_rows = kASH; e.pre.out_x0 = e.pad_x; e.pre.out_y0 = e.pad_y;
-  e.pre.out_c = 8;
-  e.pre.h = -1;                                                // force a table rebuild
-  int rc = e.pre.configure(h, w, VPB_RESIZE_PIL_BILINEAR);
-  if (rc) return rc;
-  // the canvas border is constant per geometry: gray everywhere (all samples), the pre-process overwrites the pasted region
-  const int npix = kASW * kASH * e.batch;
-  if (e.dtype == VPB_BF16) fill_canvas_kernel<BF16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__nv_bfloat16*>(e.d_canvas), npix);
-  else fill_canvas_kernel<F16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__half*>(e.d_canvas), npix);
-  VPB_CUDA_OK(cudaGetLastError());
-  e.src_h = h; e.src_w = w;
+  if (nw < 1 || nh < 1) { vpb_set_error("%s: frame %d: %dx%d too small", who, k, w, h); return VPB_ERR_ARG; }
+  g->h = h; g->w = w; g->OW = nw; g->OH = nh; g->x0 = (kASW - nw) / 2; g->y0 = (kASH - nh) / 2;
+  *scale = static_cast<float>(sc);
+  return PreprocessPlan::check(*g, VPB_RESIZE_PIL_BILINEAR, who, k);
+}
+
+static int as_geoms(const vp_autospeed& e, const vpb_frame* frames, const char* who, PreGeom* g, float* scale) {
+  for (int k = 0; k < e.batch; ++k) {
+    const int rc = as_letterbox(frames[k].h, frames[k].w, who, k, &g[k], &scale[k]);
+    if (rc) return rc;
+  }
   return VPB_OK;
 }
 
-// Enqueue one call for the e.batch frames srcs[0 .. batch-1] (one geometry).
-static int as_enqueue(vp_autospeed& e, const uint8_t* const* srcs, int h, int w, int stride) {
-  int rc = as_configure(e, h, w);
+// Tables for the call's letterboxes; the gray border of a sample's canvas is refilled only when its letterbox changed
+// (the pre-process overwrites the pasted region on every call).
+static int as_configure(vp_autospeed& e, const PreGeom* g, const float* scale) {
+  int rc = e.pre.configure(g, e.batch, VPB_RESIZE_PIL_BILINEAR);
   if (rc) return rc;
-  FrameSrcs src{};
-  std::copy(srcs, srcs + e.batch, src.begin());
+  const int npix = kASW * kASH;
+  for (int k = 0; k < e.batch; ++k) {
+    e.scale[k] = scale[k];
+    if (e.canvas_geom[k] == g[k]) continue;
+    void* c = static_cast<uint8_t*>(e.d_canvas) + static_cast<size_t>(npix) * 8 * 2 * k;
+    if (e.dtype == VPB_BF16) fill_canvas_kernel<BF16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__nv_bfloat16*>(c), npix);
+    else fill_canvas_kernel<F16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__half*>(c), npix);
+    VPB_CUDA_OK(cudaGetLastError());
+    e.canvas_geom[k] = g[k];
+  }
+  return VPB_OK;
+}
+
+// Enqueue one call for the e.batch frames f[0 .. batch-1].
+static int as_enqueue(vp_autospeed& e, const Frames& f, const PreGeom* g, const float* scale) {
+  int rc = as_configure(e, g, scale);
+  if (rc) return rc;
   return e.frame_graph.run(
-      e.stream, e.pre, e.dtype, h, w, stride, src, [&](cudaStream_t st) { return as_launch_all(e, src.data(), stride, st); },
+      e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return as_launch_all(e, f.data(), st); },
       [&](cudaGraphExec_t x, cudaGraphNode_t n) {
-        return e.pre.update_graph_node(x, n, src.data(), e.batch, stride, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
+        return e.pre.update_graph_node(x, n, f.data(), VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
       });
 }
 
@@ -765,6 +793,8 @@ static int as_create(const char* who, const char* weights_vpw, int gpu_id, int d
   e->batch = batch;
   const size_t nb = batch;
   e->d_canvas = e->dalloc(static_cast<size_t>(kASW) * kASH * 8 * 2 * nb);
+  e->pre.out_pitch = kASW; e->pre.out_rows = kASH; e->pre.out_c = 8;
+  for (int k = 0; k < batch; ++k) e->canvas_geom[k].h = -1;   // no border filled yet
   e->d_raw = static_cast<float*>(e->dalloc(static_cast<size_t>(8) * kNA * 4 * nb));
   e->h_raw = static_cast<float*>(e->halloc(static_cast<size_t>(8) * kNA * 4 * nb));
   e->d_cand = static_cast<float*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxCand) * 6 * 4 * nb));
@@ -794,19 +824,39 @@ static int as_fetch(vp_autospeed* e, bool raw) {
   return VPB_OK;
 }
 
-static int as_infer_host(vp_autospeed* e, const uint8_t* const* frames, int n, int h, int w, int stride, int fetch_raw,
-                         const char* who) {
-  if (!frames_ok(e, frames, n, h, w, stride, who)) return VPB_ERR_ARG;
+static int as_infer_host(vp_autospeed* e, const vpb_frame* frames, int n, int fetch_raw, const char* who) {
+  if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
+  PreGeom g[kMaxBatch];
+  float scale[kMaxBatch];
+  if (as_geoms(*e, frames, who, g, scale)) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  FrameSrcs dev;
-  int rc = e->upload_frames(frames, n, h, w, stride, dev);
+  Frames dev;
+  int rc = e->upload_frames(frames, n, dev);
   if (rc) return rc;
-  rc = as_enqueue(*e, dev.data(), h, w, w * 3);
+  rc = as_enqueue(*e, dev, g, scale);
   if (rc) return rc;
   rc = as_fetch(e, fetch_raw != 0);
   if (rc) return rc;
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   return VPB_OK;
+}
+
+static int as_infer_host_batch(vp_autospeed* e, const uint8_t* const* frames, int n, int h, int w, int stride,
+                               int fetch_raw, const char* who) {
+  Frames f;
+  if (!batch_frames(e, frames, n, h, w, stride, who, f)) return VPB_ERR_ARG;
+  return as_infer_host(e, f.data(), n, fetch_raw, who);
+}
+
+static int as_infer_device(vp_autospeed* e, const vpb_frame* frames, int n, const char* who) {
+  if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
+  PreGeom g[kMaxBatch];
+  float scale[kMaxBatch];
+  if (as_geoms(*e, frames, who, g, scale)) return VPB_ERR_ARG;
+  Frames f{};
+  std::copy(frames, frames + n, f.begin());
+  DeviceGuard guard(e->gpu_id);
+  return as_enqueue(*e, f, g, scale);
 }
 
 static bool sample_ok(const vp_autospeed* e, int sample, const char* who) {
@@ -838,19 +888,27 @@ extern "C" int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float io
 }
 
 extern "C" int vp_autospeed_infer(vp_autospeed* e, const uint8_t* frame_host, int h, int w, int stride, int fetch_raw) {
-  return as_infer_host(e, &frame_host, 1, h, w, stride, fetch_raw, "vp_autospeed_infer");
+  return as_infer_host_batch(e, &frame_host, 1, h, w, stride, fetch_raw, "vp_autospeed_infer");
 }
 
 extern "C" int vp_autospeed_infer_batch(vp_autospeed* e, const uint8_t* const* frames_host, int n, int h, int w, int stride,
                                         int fetch_raw) {
-  return as_infer_host(e, frames_host, n, h, w, stride, fetch_raw, "vp_autospeed_infer_batch");
+  return as_infer_host_batch(e, frames_host, n, h, w, stride, fetch_raw, "vp_autospeed_infer_batch");
+}
+
+extern "C" int vp_autospeed_infer_frames(vp_autospeed* e, const vpb_frame* frames_host, int n, int fetch_raw) {
+  return as_infer_host(e, frames_host, n, fetch_raw, "vp_autospeed_infer_frames");
 }
 
 extern "C" int vp_autospeed_infer_device_batch(vp_autospeed* e, const uint8_t* const* frames_dev, int n, int h, int w,
                                                int stride) {
-  if (!frames_ok(e, frames_dev, n, h, w, stride, "vp_autospeed_infer_device")) return VPB_ERR_ARG;
-  DeviceGuard guard(e->gpu_id);
-  return as_enqueue(*e, frames_dev, h, w, stride);
+  Frames f;
+  if (!batch_frames(e, frames_dev, n, h, w, stride, "vp_autospeed_infer_device", f)) return VPB_ERR_ARG;
+  return as_infer_device(e, f.data(), n, "vp_autospeed_infer_device");
+}
+
+extern "C" int vp_autospeed_infer_device_frames(vp_autospeed* e, const vpb_frame* frames_dev, int n) {
+  return as_infer_device(e, frames_dev, n, "vp_autospeed_infer_device_frames");
 }
 
 extern "C" int vp_autospeed_infer_device(vp_autospeed* e, const uint8_t* frame_dev, int h, int w, int stride) {

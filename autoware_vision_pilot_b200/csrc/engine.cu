@@ -596,13 +596,13 @@ static int prepare_lanes(vp_engine& e) {
   return VPB_OK;
 }
 
-static int launch_all(vp_engine& e, const uint8_t* const* srcs, int stride, cudaStream_t st) {
+static int launch_all(vp_engine& e, const vpb_frame* frames, cudaStream_t st) {
   int rc = prepare_lanes(e);
   if (rc) return rc;
   const size_t nl = e.lane_dep.size();
   const bool multi = nl > 1 && e.cfg.single_stream == 0;
   if (e.d_gap) VPB_CUDA_OK(cudaMemsetAsync(e.d_gap, 0, e.gap_used * 8, st));
-  rc = e.pre.launch(srcs, e.batch, stride, e.cfg.convention, e.dtype, e.d_pre, e.d_resized, st);
+  rc = e.pre.launch(frames, e.cfg.convention, e.dtype, e.d_pre, e.d_resized, st);
   if (rc) return rc;
   if (!multi) {
     for (auto& op : e.ops) { rc = op.launch(st); if (rc) return rc; }
@@ -630,18 +630,28 @@ static int launch_all(vp_engine& e, const uint8_t* const* srcs, int stride, cuda
   return VPB_OK;
 }
 
-// Enqueue one call's kernels for the e.batch frames srcs[0 .. batch-1] (graph replay when enabled and the geometry
-// is unchanged).
-static int enqueue_frame(vp_engine& e, const uint8_t* const* srcs, int h, int w, int stride) {
-  int rc = e.pre.configure(h, w, e.cfg.resize_mode);
+// Every frame resizes to the 640 x 320 network input: VPB_ERR_ARG (naming `who` and the frame) if one cannot in the
+// engine's resize mode.  Host-only: callers run it before any device work.
+static int engine_geoms(const vp_engine& e, const vpb_frame* frames, const char* who, PreGeom* g) {
+  for (int k = 0; k < e.batch; ++k) {
+    g[k] = PreGeom{};
+    g[k].h = frames[k].h; g[k].w = frames[k].w;
+    const int rc = PreprocessPlan::check(g[k], e.cfg.resize_mode, who, k);
+    if (rc) return rc;
+  }
+  return VPB_OK;
+}
+
+// Enqueue one call's kernels for the e.batch frames f[0 .. batch-1] (graph replay when enabled and the geometries are
+// unchanged).
+static int enqueue_frames(vp_engine& e, const Frames& f, const PreGeom* g) {
+  int rc = e.pre.configure(g, e.batch, e.cfg.resize_mode);
   if (rc) return rc;
-  FrameSrcs src{};
-  std::copy(srcs, srcs + e.batch, src.begin());
-  if (!e.cfg.use_graph) return launch_all(e, src.data(), stride, e.stream);
+  if (!e.cfg.use_graph) return launch_all(e, f.data(), e.stream);
   return e.frame_graph.run(
-      e.stream, e.pre, e.dtype, h, w, stride, src, [&](cudaStream_t st) { return launch_all(e, src.data(), stride, st); },
+      e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return launch_all(e, f.data(), st); },
       [&](cudaGraphExec_t x, cudaGraphNode_t n) {
-        return e.pre.update_graph_node(x, n, src.data(), e.batch, stride, e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
+        return e.pre.update_graph_node(x, n, f.data(), e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
       });
 }
 
@@ -720,10 +730,26 @@ extern "C" uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes) {
   return e->h_frame;
 }
 
-extern "C" int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev, int n, int h, int w, int stride) {
-  if (!frames_ok(e, frames_dev, n, h, w, stride, "vp_engine_infer_device")) return VPB_ERR_ARG;
+static int infer_device_frames(vp_engine* e, const Frames& f, int n, const char* who) {
+  if (!frames_ok(e, f.data(), n, who)) return VPB_ERR_ARG;
+  PreGeom g[kMaxBatch];
+  if (engine_geoms(*e, f.data(), who, g)) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  return enqueue_frame(*e, frames_dev, h, w, stride);
+  return enqueue_frames(*e, f, g);
+}
+
+extern "C" int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev, int n, int h, int w, int stride) {
+  Frames f;
+  if (!batch_frames(e, frames_dev, n, h, w, stride, "vp_engine_infer_device", f)) return VPB_ERR_ARG;
+  return infer_device_frames(e, f, n, "vp_engine_infer_device");
+}
+
+extern "C" int vp_engine_infer_device_frames(vp_engine* e, const vpb_frame* frames_dev, int n) {
+  const char* who = "vp_engine_infer_device_frames";
+  if (!frames_ok(e, frames_dev, n, who)) return VPB_ERR_ARG;
+  Frames f{};
+  std::copy(frames_dev, frames_dev + n, f.begin());
+  return infer_device_frames(e, f, n, who);
 }
 
 extern "C" int vp_engine_infer_device(vp_engine* e, const uint8_t* frame_dev, int h, int w, int stride) {
@@ -737,13 +763,15 @@ extern "C" int vp_engine_sync(vp_engine* e) {
   return VPB_OK;
 }
 
-static int submit_host_frames(vp_engine* e, const uint8_t* const* frames, int n, int h, int w, int stride, bool sync) {
-  if (!frames_ok(e, frames, n, h, w, stride, sync ? "vp_engine_infer" : "vp_engine_submit")) return VPB_ERR_ARG;
+static int submit_host_frames(vp_engine* e, const vpb_frame* frames, int n, bool sync, const char* who) {
+  if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
+  PreGeom g[kMaxBatch];
+  if (engine_geoms(*e, frames, who, g)) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  FrameSrcs dev;
-  int rc = e->upload_frames(frames, n, h, w, stride, dev);
+  Frames dev;
+  int rc = e->upload_frames(frames, n, dev);
   if (rc) return rc;
-  rc = enqueue_frame(*e, dev.data(), h, w, w * 3);
+  rc = enqueue_frames(*e, dev, g);
   if (rc) return rc;
   for (auto& mo : e->outs) {
     if (mo.has_cls)
@@ -755,20 +783,35 @@ static int submit_host_frames(vp_engine* e, const uint8_t* const* frames, int n,
   return VPB_OK;
 }
 
+static int submit_host_batch(vp_engine* e, const uint8_t* const* frames, int n, int h, int w, int stride, bool sync) {
+  const char* who = sync ? "vp_engine_infer" : "vp_engine_submit";
+  Frames f;
+  if (!batch_frames(e, frames, n, h, w, stride, who, f)) return VPB_ERR_ARG;
+  return submit_host_frames(e, f.data(), n, sync, who);
+}
+
 extern "C" int vp_engine_infer(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride) {
-  return submit_host_frames(e, &frame_host, 1, h, w, stride, true);
+  return submit_host_batch(e, &frame_host, 1, h, w, stride, true);
 }
 
 extern "C" int vp_engine_submit(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride) {
-  return submit_host_frames(e, &frame_host, 1, h, w, stride, false);
+  return submit_host_batch(e, &frame_host, 1, h, w, stride, false);
 }
 
 extern "C" int vp_engine_infer_batch(vp_engine* e, const uint8_t* const* frames_host, int n, int h, int w, int stride) {
-  return submit_host_frames(e, frames_host, n, h, w, stride, true);
+  return submit_host_batch(e, frames_host, n, h, w, stride, true);
 }
 
 extern "C" int vp_engine_submit_batch(vp_engine* e, const uint8_t* const* frames_host, int n, int h, int w, int stride) {
-  return submit_host_frames(e, frames_host, n, h, w, stride, false);
+  return submit_host_batch(e, frames_host, n, h, w, stride, false);
+}
+
+extern "C" int vp_engine_infer_frames(vp_engine* e, const vpb_frame* frames_host, int n) {
+  return submit_host_frames(e, frames_host, n, true, "vp_engine_infer_frames");
+}
+
+extern "C" int vp_engine_submit_frames(vp_engine* e, const vpb_frame* frames_host, int n) {
+  return submit_host_frames(e, frames_host, n, false, "vp_engine_submit_frames");
 }
 
 extern "C" int vp_engine_fetch_raw(vp_engine* e, int idx) {
@@ -812,7 +855,7 @@ extern "C" int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s) {
 
 extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* flops, const char** names, int* is_gemm, int* n_ops) {
   if (!e || !ms || !n_ops) return VPB_ERR_ARG;
-  if (!e->frame_graph.src[0]) { vpb_set_error("vp_engine_profile: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->frame_graph.n) { vpb_set_error("vp_engine_profile: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   const int n = static_cast<int>(e->ops.size()) + 1;
   *n_ops = n;
@@ -821,7 +864,7 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
   for (auto& x : ev) VPB_CUDA_OK(cudaEventCreate(&x));
   if (e->d_gap) VPB_CUDA_OK(cudaMemsetAsync(e->d_gap, 0, e->gap_used * 8, e->stream));
   VPB_CUDA_OK(cudaEventRecord(ev[0], e->stream));
-  int rc = e->pre.launch(e->frame_graph.src.data(), e->batch, e->frame_graph.stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
+  int rc = e->pre.launch(e->frame_graph.frames.data(), e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
   if (rc) return rc;
   VPB_CUDA_OK(cudaEventRecord(ev[1], e->stream));
   for (int i = 0; i < n - 1; ++i) {
@@ -843,7 +886,7 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
 
 extern "C" int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flops, int* launches) {
   if (!e || !ms || reps <= 0) return VPB_ERR_ARG;
-  if (!e->frame_graph.src[0]) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->frame_graph.n) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   cudaEvent_t a, b;
   VPB_CUDA_OK(cudaEventCreate(&a));
@@ -868,10 +911,14 @@ extern "C" int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, 
   return VPB_OK;
 }
 
-extern "C" int vp_engine_read_resized(vp_engine* e, uint8_t* dst) {
+extern "C" int vp_engine_read_resized(vp_engine* e, uint8_t* dst) { return vp_engine_read_resized_at(e, 0, dst); }
+
+extern "C" int vp_engine_read_resized_at(vp_engine* e, int sample, uint8_t* dst) {
   if (!e || !dst) return VPB_ERR_ARG;
+  if (sample < 0 || sample >= e->batch) { vpb_set_error("vp_engine_read_resized: sample %d of a batch of %d", sample, e->batch); return VPB_ERR_ARG; }
   DeviceGuard guard(e->gpu_id);
-  VPB_CUDA_OK(cudaMemcpyAsync(dst, e->d_resized, static_cast<size_t>(kNetH) * kNetW * 3, cudaMemcpyDeviceToHost, e->stream));
+  const size_t bytes = static_cast<size_t>(kNetH) * kNetW * 3;
+  VPB_CUDA_OK(cudaMemcpyAsync(dst, e->d_resized + bytes * sample, bytes, cudaMemcpyDeviceToHost, e->stream));
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   return VPB_OK;
 }
@@ -912,7 +959,7 @@ extern "C" int vp_engine_kernel_names(vp_engine* e, const char** names, int cap,
 extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, float* ms, double* flops,
                                      double* bytes, int* launches) {
   if (!e || !kname || !ms || reps <= 0) return VPB_ERR_ARG;
-  if (!e->frame_graph.src[0]) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->frame_graph.n) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
   const bool is_pre = strcmp(kname, "preprocess") == 0;
   cudaEvent_t a, b;
@@ -923,10 +970,14 @@ extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, 
   for (int r = -1; r < reps; ++r) {            // r = -1: untimed warm-up pass
     if (r == 0) VPB_CUDA_OK(cudaEventRecord(a, e->stream));
     if (is_pre) {
-      const int rc = e->pre.launch(e->frame_graph.src.data(), e->batch, e->frame_graph.stride, e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
+      const int rc = e->pre.launch(e->frame_graph.frames.data(), e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
       if (rc) return rc;
       // SURVEY.md 8d: frame read + 3 x 320 x 640 16-bit tensor written, per sample
-      if (r >= 0) { by += e->batch * (3.0 * e->frame_graph.h * e->frame_graph.w + 2.0 * 3 * kNetH * kNetW); ++n; }
+      if (r >= 0) {
+        for (int k = 0; k < e->batch; ++k)
+          by += 3.0 * e->frame_graph.frames[k].h * e->frame_graph.frames[k].w + 2.0 * 3 * kNetH * kNetW;
+        ++n;
+      }
       continue;
     }
     for (auto& op : e->ops) {

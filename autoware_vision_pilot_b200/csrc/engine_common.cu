@@ -105,18 +105,24 @@ extern "C" int vpb_final_conv_weights_host(const float* w, int Cout, int Cin, fl
 namespace vpb {
 
 // =============================================================== frame graph
-int FrameGraph::run(cudaStream_t st, const PreprocessPlan& pre, int dtype, int h_, int w_, int stride_,
-                    const FrameSrcs& src_, const std::function<int(cudaStream_t)>& launch,
+static bool same_geometry(const vpb_frame& a, const vpb_frame& b) { return a.h == b.h && a.w == b.w && a.stride == b.stride; }
+
+int FrameGraph::run(cudaStream_t st, const PreprocessPlan& pre, int dtype, const Frames& f, int n_,
+                    const std::function<int(cudaStream_t)>& launch,
                     const std::function<int(cudaGraphExec_t, cudaGraphNode_t)>& repoint) {
-  const bool same_geometry = exec && h == h_ && w == w_ && stride == stride_;
-  if (same_geometry && src != src_ && pre_node) {
+  bool same_geom = exec && n == n_, same_src = n == n_;
+  for (int k = 0; k < n_ && same_geom; ++k) same_geom = same_geometry(frames[k], f[k]);
+  for (int k = 0; k < n_ && same_src; ++k) same_src = frames[k].data == f[k].data;
+  if (same_geom && !same_src && pre_node) {
     const int rc = repoint(exec, pre_node);
     if (rc) return rc;
-    src = src_;
+    frames = f;
+    same_src = true;
   }
-  if (!same_geometry || src != src_) {
+  if (!same_geom || !same_src) {
     invalidate();
     pre_node = nullptr;
+    n = 0;
     int rc = launch(st);
     if (rc) return rc;
     VPB_CUDA_OK(cudaStreamSynchronize(st));
@@ -143,7 +149,7 @@ int FrameGraph::run(cudaStream_t st, const PreprocessPlan& pre, int dtype, int h
     if (graph) cudaGraphDestroy(graph);
     graph = g;
     if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    h = h_; w = w_; stride = stride_; src = src_;
+    frames = f; n = n_;
   }
   VPB_CUDA_OK(cudaGraphLaunch(exec, st));
   return VPB_OK;
@@ -259,34 +265,53 @@ int EngineRuntime::append_conv(const std::string& name, const vpb_conv_args& a, 
   return VPB_OK;
 }
 
-bool frames_ok(const EngineRuntime* e, const uint8_t* const* frames, int n, int h, int w, int stride, const char* who) {
-  if (!e || !frames || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("%s: bad arguments", who); return false; }
+bool frames_ok(const EngineRuntime* e, const vpb_frame* frames, int n, const char* who) {
+  if (!e || !frames) { vpb_set_error("%s: bad arguments", who); return false; }
   if (n != e->batch) {
     vpb_set_error("%s: %d frame(s) for an engine of batch %d%s", who, n, e->batch,
                   n == 1 ? " (use the *_batch calls)" : "");
     return false;
   }
-  for (int k = 0; k < n; ++k)
-    if (!frames[k]) { vpb_set_error("%s: frame %d is NULL", who, k); return false; }
+  for (int k = 0; k < n; ++k) {
+    const vpb_frame& f = frames[k];
+    if (!f.data) { vpb_set_error("%s: frame %d is NULL", who, k); return false; }
+    if (f.h <= 0 || f.w <= 0 || f.stride < 3 * f.w) {
+      vpb_set_error("%s: frame %d: bad geometry h %d, w %d, stride %d (need h, w > 0 and stride >= 3*w)", who, k, f.h,
+                    f.w, f.stride);
+      return false;
+    }
+  }
   return true;
 }
 
-int EngineRuntime::upload_frames(const uint8_t* const* frames, int n, int h, int w, int stride, FrameSrcs& dev) {
-  const int dpitch = w * 3;
-  const size_t bytes = static_cast<size_t>(h) * dpitch;
-  if (bytes * n > d_frame_cap) {
+bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int h, int w, int stride, const char* who,
+                  Frames& out) {
+  if (!e || !ptrs || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("%s: bad arguments", who); return false; }
+  out = {};
+  for (int k = 0; k < n && k < kMaxBatch; ++k) out[k] = vpb_frame{ptrs[k], h, w, stride};
+  return frames_ok(e, out.data(), n, who);
+}
+
+int EngineRuntime::upload_frames(const vpb_frame* frames, int n, Frames& dev) {
+  size_t total = 0;
+  for (int k = 0; k < n; ++k) total += static_cast<size_t>(frames[k].h) * frames[k].w * 3;
+  if (total > d_frame_cap) {
     frame_graph.invalidate();
     void* p = nullptr;
-    VPB_CUDA_OK(cudaMalloc(&p, bytes * n + 256));
+    VPB_CUDA_OK(cudaMalloc(&p, total + 256));
     dev_allocs.push_back(p);
-    d_frame = static_cast<uint8_t*>(p); d_frame_cap = bytes * n;
+    d_frame = static_cast<uint8_t*>(p); d_frame_cap = total;
   }
   dev = {};
+  size_t off = 0;
   for (int k = 0; k < n; ++k) {
-    uint8_t* d = d_frame + bytes * k;
-    dev[k] = d;
-    if (stride == dpitch) VPB_CUDA_OK(cudaMemcpyAsync(d, frames[k], bytes, cudaMemcpyHostToDevice, stream));
-    else VPB_CUDA_OK(cudaMemcpy2DAsync(d, dpitch, frames[k], stride, dpitch, h, cudaMemcpyHostToDevice, stream));
+    const vpb_frame& f = frames[k];
+    const int dpitch = f.w * 3;
+    uint8_t* d = d_frame + off;
+    dev[k] = vpb_frame{d, f.h, f.w, dpitch};
+    if (f.stride == dpitch) VPB_CUDA_OK(cudaMemcpyAsync(d, f.data, static_cast<size_t>(f.h) * dpitch, cudaMemcpyHostToDevice, stream));
+    else VPB_CUDA_OK(cudaMemcpy2DAsync(d, dpitch, f.data, f.stride, dpitch, f.h, cudaMemcpyHostToDevice, stream));
+    off += static_cast<size_t>(f.h) * dpitch;
   }
   return VPB_OK;
 }

@@ -68,21 +68,22 @@ struct OpRec {
   int lane = 0;   // execution lane (= index of the model that owns the op); lanes run concurrently
 };
 
-using FrameSrcs = std::array<const uint8_t*, kMaxBatch>;
+// The frames of one call: descriptor k is sample k (entries past the batch are unused).
+using Frames = std::array<vpb_frame, kMaxBatch>;
 
-// The CUDA graph of one call, keyed on (h, w, stride, frame pointers).  A frame of the captured geometry in another
-// buffer only re-points the captured pre-process node.
+// The CUDA graph of one call, keyed on the n (h, w, stride) triples and the frame pointers.  Frames of the captured
+// geometries in other buffers only re-point the captured pre-process node.
 struct FrameGraph {
   cudaGraph_t graph = nullptr;           // kept alive: pre_node is a handle into it
   cudaGraphExec_t exec = nullptr;
-  cudaGraphNode_t pre_node = nullptr;    // the captured pre-process kernel node (re-pointed per frame)
-  int h = 0, w = 0, stride = 0;
-  FrameSrcs src{};                       // frames of the captured / last call ([0] == NULL: none yet)
+  cudaGraphNode_t pre_node = nullptr;    // the captured pre-process kernel node (re-pointed per call)
+  int n = 0;                             // frames of the captured / last call (0: none yet)
+  Frames frames{};
 
-  // Launch the graph for frames src_ on st.  When the key differs in more than the frame pointers: launch(st) once
-  // outside capture (sets function attributes; its results are correct), capture launch(st), find the node of `pre`
-  // and instantiate.  When only the pointers differ: repoint(exec, pre_node).
-  int run(cudaStream_t st, const PreprocessPlan& pre, int dtype, int h_, int w_, int stride_, const FrameSrcs& src_,
+  // Launch the graph for frames f[0 .. n_-1] on st.  When the key differs in more than the frame pointers: launch(st)
+  // once outside capture (sets function attributes; its results are correct), capture launch(st), find the node of
+  // `pre` and instantiate.  When only the pointers differ: repoint(exec, pre_node).
+  int run(cudaStream_t st, const PreprocessPlan& pre, int dtype, const Frames& f, int n_,
           const std::function<int(cudaStream_t)>& launch,
           const std::function<int(cudaGraphExec_t, cudaGraphNode_t)>& repoint);
   void invalidate();                     // the next run() captures again
@@ -127,17 +128,22 @@ struct EngineRuntime {
   // build the plan of one wgmma convolution, keep it, append its launch (errors are prefixed with name)
   int append_conv(const std::string& name, const vpb_conv_args& a, int lane = 0);
   void tap(const std::string& name, const Tens& t, int channels = 0) { taps[name] = Tap{t, channels > 0 ? channels : t.C}; }
-  // Copy n host frames of one geometry to d_frame (grown on demand), packed with pitch w*3: only the w*3 valid bytes
+  // Copy n host frames to d_frame (grown on demand), back to back, frame k with pitch w_k*3: only the w_k*3 valid bytes
   // of every row are read from the caller's buffer, so a cv::Mat ROI / strided view is never read past its last row.
-  int upload_frames(const uint8_t* const* frames, int n, int h, int w, int stride, FrameSrcs& dev);
+  // dev[k] describes the device copy of frame k.
+  int upload_frames(const vpb_frame* frames, int n, Frames& dev);
   // the first `channels` channels of t as fp32 [channels][H][W] into dst (NULL: size query); element count or < 0
   long read_tap(const Tens& t, int channels, float* dst, long cap, int* c, int* h, int* w);
   // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
   bool find_tap(const char* name, Tap* out) const;
 };
 
-// n frames of one geometry, n == e's batch (who names the call in the error message)
-bool frames_ok(const EngineRuntime* e, const uint8_t* const* frames, int n, int h, int w, int stride, const char* who);
+// n == e's batch descriptors, each with non-NULL data, h, w > 0 and stride >= 3*w (who names the call and the message
+// the frame index)
+bool frames_ok(const EngineRuntime* e, const vpb_frame* frames, int n, const char* who);
+// n frames of one geometry (the *_batch calls) as descriptors; false (error set as frames_ok does) on bad arguments
+bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int h, int w, int stride, const char* who,
+                  Frames& out);
 
 }  // namespace vpb
 

@@ -240,10 +240,10 @@ __device__ int sliding_search(const LatShared& s, uint8_t* px, uint8_t* py, int 
 struct LatCam {               // what differs between the cameras of one launch
   double Hm[9], Hi[9];      // orig -> BEV homography and its inverse
   double steering;          // AutoSteer steering angle handed to PathFinder (main.cpp:577)
+  double sx, sy;            // image / model scale (each camera has its own source size)
 };
-struct LatParams {          // by value: 1.25 KB at kMaxBatch cameras, under the 4 KB kernel-parameter limit
+struct LatParams {          // by value: 1.4 KB at kMaxBatch cameras, under the 4 KB kernel-parameter limit
   int H, W;
-  double sx, sy;            // image / model scale
   float smoothing;
   LatCam cam[kMaxBatch];    // camera k = blockIdx.x
 };
@@ -262,15 +262,15 @@ __device__ __forceinline__ void warp_pt(const double* m, float x, float y, float
 }
 
 // genPointsFromCoeffs on the upscaled coefficients + warp to BEV; returns the point count.
-__device__ int gen_and_warp(const double c6[6], const LatParams& p, const LatCam& cam, float* ox, float* oy) {
+__device__ int gen_and_warp(const double c6[6], const LatCam& cam, float* ox, float* oy) {
   const int lane = threadIdx.x & 31;
   double up[6];
   up[0] = 0.0;
-  up[1] = c6[1] * p.sx / (p.sy * p.sy);
-  up[2] = c6[2] * p.sx / p.sy;
-  up[3] = c6[3] * p.sx;
-  up[4] = c6[4] * p.sy;
-  up[5] = c6[5] * p.sy;
+  up[1] = c6[1] * cam.sx / (cam.sy * cam.sy);
+  up[2] = c6[2] * cam.sx / cam.sy;
+  up[3] = c6[3] * cam.sx;
+  up[4] = c6[4] * cam.sy;
+  up[5] = c6[5] * cam.sy;
   // y = min_y + 5k (the reference accumulates y += 5 in double: exact for these magnitudes)
   int n = 0;
   if (up[5] >= up[4]) n = static_cast<int>(floor((up[5] - up[4]) / 5.0)) + 1;
@@ -397,8 +397,8 @@ __global__ void __launch_bounds__(256, 1) lateral_kernel(const float* __restrict
   double left6[6], right6[6];
   for (int k = 0; k < 6; ++k) { left6[k] = valid[0] ? fit[0][k] : 0.0; right6[k] = valid[1] ? fit[1][k] : 0.0; }
   bool out_left = valid[0], out_right = valid[1];
-  int nl = valid[0] ? gen_and_warp(fit[0], p, cam, s.ax, s.ay) : 0;
-  int nr = valid[1] ? gen_and_warp(fit[1], p, cam, s.bx, s.by) : 0;
+  int nl = valid[0] ? gen_and_warp(fit[0], cam, s.ax, s.ay) : 0;
+  int nr = valid[1] ? gen_and_warp(fit[1], cam, s.bx, s.by) : 0;
   double width = st->last_valid_bev_width;
   int has_width = st->has_valid_width_history;
   if (valid[0] && valid[1]) {
@@ -422,8 +422,8 @@ __global__ void __launch_bounds__(256, 1) lateral_kernel(const float* __restrict
       dsty[k] = srcy[k];
       float ox, oy;
       warp_pt(cam.Hi, dstx[k], dsty[k], &ox, &oy);
-      s.cx[k] = static_cast<float>(static_cast<double>(ox) / p.sx);
-      s.cy[k] = static_cast<float>(static_cast<double>(oy) / p.sy);
+      s.cx[k] = static_cast<float>(static_cast<double>(ox) / cam.sx);
+      s.cy[k] = static_cast<float>(static_cast<double>(oy) / cam.sy);
     }
     __syncwarp();
     if (miss_left) { nl = n; fit2_to6(s.cx, s.cy, n, left6); out_left = true; }
@@ -567,46 +567,73 @@ extern "C" int vpb_lateral_init(vpb_lateral_state* state, void* stream) {
   return VPB_OK;
 }
 
-// n cameras of one geometry in one launch (vpb_lateral_update is n = 1).  Everything is checked before device work.
-static int lateral_launch(const char* who, const float* masks, int n, int H, int W, int img_w, int img_h, float smoothing,
-                          const double* homographies, const double* steering, vpb_lateral_state* states,
-                          vpb_lateral_out* outs, void* stream) {
+// n cameras in one launch, camera k with source size img_w[k] x img_h[k] (vpb_lateral_update is n = 1,
+// vpb_lateral_update_batch n equal sizes).  Everything is checked before device work.
+static int lateral_launch(const char* who, const float* masks, int n, int H, int W, const int* img_w, const int* img_h,
+                          float smoothing, const double* homographies, const double* steering,
+                          vpb_lateral_state* states, vpb_lateral_out* outs, void* stream) {
   if (n < 1 || n > vpb::kMaxBatch) {
     vpb_set_error("%s: %d cameras (1..%d)", who, n, vpb::kMaxBatch);
     return VPB_ERR_ARG;
   }
-  if (!masks || !states || !outs || H < 41 || H > vpb::kMaxH || W < 2 || W > vpb::kMaxWords * 32 || img_w <= 0 || img_h <= 0) {
-    vpb_set_error("%s: need masks [3][H<=128][W<=256] (H >= 41), state and out", who);
+  static const char* kNeed = "need masks [3][H<=128][W<=256] (H >= 41), state and out";
+  if (!masks || !states || !outs || H < 41 || H > vpb::kMaxH || W < 2 || W > vpb::kMaxWords * 32) {
+    vpb_set_error("%s: %s", who, kNeed);
     return VPB_ERR_ARG;
   }
+  if (!img_w || !img_h) {
+    vpb_set_error("%s: %s, and img_w / img_h arrays (NULL)", who, kNeed);
+    return VPB_ERR_ARG;
+  }
+  for (int c = 0; c < n; ++c)
+    if (img_w[c] <= 0 || img_h[c] <= 0) {
+      vpb_set_error("%s: %s; camera %d: image size %dx%d is not positive", who, kNeed, c, img_w[c], img_h[c]);
+      return VPB_ERR_ARG;
+    }
   // lane_tracking.hpp:75-79 (hard-coded in the reference; overridable here)
   static const double kH[9] = {-1.79887412e-01, -6.05811422e-01, 6.02998251e+02,
                                1.85824549e-14,  -1.28170839e+00, 8.63871455e+02,
                                2.95628463e-17,  -1.76125061e-03, 1.00000000e+00};
   vpb::LatParams p;
   p.H = H; p.W = W; p.smoothing = smoothing;
-  p.sx = static_cast<double>(img_w) / W; p.sy = static_cast<double>(img_h) / H;
   for (int c = 0; c < n; ++c) {
     vpb::LatCam& cam = p.cam[c];
     for (int k = 0; k < 9; ++k) cam.Hm[k] = homographies ? homographies[9 * c + k] : kH[k];
     vpb::inv3(cam.Hm, cam.Hi);
     cam.steering = steering ? steering[c] : 0.0;
+    cam.sx = static_cast<double>(img_w[c]) / W; cam.sy = static_cast<double>(img_h[c]) / H;
   }
   vpb::lateral_kernel<<<n, 256, 0, static_cast<cudaStream_t>(stream)>>>(masks, p, states, outs);
   VPB_CUDA_OK(cudaGetLastError());
   return VPB_OK;
 }
 
+// One source size for all n cameras (n is checked by the launcher before the arrays are read).
+static int lateral_launch_one_size(const char* who, const float* masks, int n, int H, int W, int img_w, int img_h,
+                                   float smoothing, const double* homographies, const double* steering,
+                                   vpb_lateral_state* states, vpb_lateral_out* outs, void* stream) {
+  int ws[vpb::kMaxBatch], hs[vpb::kMaxBatch];
+  for (int c = 0; c < vpb::kMaxBatch; ++c) { ws[c] = img_w; hs[c] = img_h; }
+  return lateral_launch(who, masks, n, H, W, ws, hs, smoothing, homographies, steering, states, outs, stream);
+}
+
 extern "C" int vpb_lateral_update(const float* masks, int H, int W, int img_w, int img_h, float smoothing,
                                   const double* homography, double autosteer_steering_rad,
                                   vpb_lateral_state* state, vpb_lateral_out* out, void* stream) {
-  return lateral_launch("lateral", masks, 1, H, W, img_w, img_h, smoothing, homography, &autosteer_steering_rad, state,
-                        out, stream);
+  return lateral_launch_one_size("lateral", masks, 1, H, W, img_w, img_h, smoothing, homography, &autosteer_steering_rad,
+                                 state, out, stream);
 }
 
 extern "C" int vpb_lateral_update_batch(const float* masks, int n, int H, int W, int img_w, int img_h, float smoothing,
                                         const double* homographies, const double* steering_rad,
                                         vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream) {
-  return lateral_launch("vpb_lateral_update_batch", masks, n, H, W, img_w, img_h, smoothing, homographies, steering_rad,
-                        states_dev, outs_dev, stream);
+  return lateral_launch_one_size("vpb_lateral_update_batch", masks, n, H, W, img_w, img_h, smoothing, homographies,
+                                 steering_rad, states_dev, outs_dev, stream);
+}
+
+extern "C" int vpb_lateral_update_cameras(const float* masks, int n, int H, int W, const int* img_w, const int* img_h,
+                                          float smoothing, const double* homographies, const double* steering_rad,
+                                          vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream) {
+  return lateral_launch("vpb_lateral_update_cameras", masks, n, H, W, img_w, img_h, smoothing, homographies,
+                        steering_rad, states_dev, outs_dev, stream);
 }

@@ -15,29 +15,41 @@ static constexpr int kMaxBatch = 8;              // VP_MAX_BATCH (vp_b200.h): fr
 void resize_tables_host(int mode, int in_size, int out_size, std::vector<int>& bounds,
                         std::vector<int>& coeffs, int& ksize);
 
-// Pre-process plan: coefficient tables resident on the device for one (input size, mode).
+// Geometry of one image of a pre-process call: its h x w source is resized to OW x OH and pasted at (x0, y0) of its
+// output canvas (the letterbox, auto_speed_infer.py:24-45; the segmentation engine pastes 640 x 320 at (0, 0)).
+struct PreGeom {
+  int h = 0, w = 0, OH = kNetH, OW = kNetW, x0 = 0, y0 = 0;
+  bool operator==(const PreGeom& o) const { return h == o.h && w == o.w && OH == o.OH && OW == o.OW && x0 == o.x0 && y0 == o.y0; }
+  bool operator!=(const PreGeom& o) const { return !(*this == o); }
+};
+
+// Pre-process plan: coefficient tables resident on the device for the images of one call (one table set per distinct
+// geometry, one allocation) and one mode; the launch shape (XT, TY, shared memory) covers every image.
 struct PreprocessPlan {
-  int h = 0, w = 0, mode = -1;
-  int OH = kNetH, OW = kNetW;
-  int xks = 0, yks = 0;
-  int rows_cap = 0, patch_w_cap = 0;
+  int mode = -1, n = 0;
+  PreGeom geom[kMaxBatch];           // per image of the call
+  struct Tables { size_t xb, xk, yb, yk; int xks, yks; };
+  Tables tab[kMaxBatch];             // per image: offsets into d_tables, filter lengths
+  int OHmax = 0, OWmax = 0;          // the grid covers the largest output
+  int rows_cap = 0;
   int TY = 20, pitch = 0, xt = 16;   // Pillow kernel: output rows per block, smem row pitch (bytes), tap capacity (16 | 32)
   int device = -1;                   // device that owns d_tables
   void* out_lo = nullptr;            // split-fp16 mode: low half of the output tensor (set once by the engine)
-  // output canvas (letterbox, auto_speed_infer.py:24-45): the OW x OH resized image is pasted at (out_x0, out_y0) of a
-  // canvas of out_rows rows (0 = OH) with out_pitch pixels per row (0 = OW) and out_c channels per pixel (4 | 8); a batch
-  // holds whole canvases back to back
-  int out_pitch = 0, out_x0 = 0, out_y0 = 0, out_c = 4, out_rows = 0;
+  // output canvas: out_rows rows of out_pitch pixels with out_c channels per pixel (4 | 8); a batch holds whole
+  // canvases back to back
+  int out_pitch = kNetW, out_c = 4, out_rows = kNetH;
   size_t smem_bytes = 0;
   int* d_tables = nullptr;
-  size_t off_xb = 0, off_xk = 0, off_yb = 0, off_yk = 0;
-  int configure(int in_h, int in_w, int mode);
-  // srcs[0 .. batch-1]: one frame each, same geometry; out / out_u8 hold `batch` images back to back (16-bit mode only)
-  int launch(const uint8_t* const* srcs, int batch, int stride, int convention, int dtype, void* out, uint8_t* out_u8,
-             cudaStream_t stream) const;
+  // VPB_OK if an image of geometry g can be resized in `mode`; otherwise VPB_ERR_ARG with "<who>: frame <k>: ..." set
+  static int check(const PreGeom& g, int mode, const char* who, int k);
+  // n images (1..kMaxBatch); rebuilds the tables only when a geometry or the mode changed
+  int configure(const PreGeom* g, int n, int mode);
+  // frames[0 .. n-1]: image k reads frames[k].data with frames[k].stride (its h, w are geom[k]'s); out / out_u8 hold
+  // n images back to back (16-bit mode only for n > 1)
+  int launch(const vpb_frame* frames, int convention, int dtype, void* out, uint8_t* out_u8, cudaStream_t stream) const;
   bool owns_kernel(const void* func, int dtype) const;
-  int update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const uint8_t* const* srcs, int batch, int stride,
-                        int convention, int dtype, void* out, uint8_t* out_u8) const;
+  int update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame* frames, int convention, int dtype,
+                        void* out, uint8_t* out_u8) const;
   ~PreprocessPlan();
 };
 

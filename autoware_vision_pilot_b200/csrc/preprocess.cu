@@ -101,26 +101,30 @@ void resize_tables_host(int mode, int in_size, int out_size, std::vector<int>& b
 }
 
 // ---------------------------------------------------------------- device
-struct PreParams {
-  const uint8_t* src[kMaxBatch];   // per image of the batch (blockIdx.z): [h][stride] bytes, 3 interleaved channels
-  int h, w, stride;
+struct PreImg {          // one image of the call (blockIdx.z); images of one call may differ in every field
+  const uint8_t* src;   // [h][stride] bytes, 3 interleaved channels
+  const int* xb; const int* xk;   // horizontal bounds / coeffs (xks per output column)
+  const int* yb; const int* yk;   // vertical
+  int h, w, stride, xks, yks;
+  int OH, OW, out_x0, out_y0;     // resized size and its paste offset in the output canvas
+};
+struct PreParams {      // by value (__grid_constant__): under 0.8 KB at kMaxBatch images
+  PreImg im[kMaxBatch];
   int mode;             // VPB_RESIZE_*
   int swap_rb;          // 1: tensor channel c = source channel 2-c
   int mul_inv255;       // 1: x * (1/255) (OpenCV convertTo), 0: x / 255 (ToTensor)
   float mean[3], stdv[3];
-  const int* xb; const int* xk; int xks;   // horizontal bounds / coeffs / ksize
-  const int* yb; const int* yk; int yks;   // vertical
-  void* out;            // [OH][OW][4] 16-bit
+  void* out;            // [out_rows][out_pitch][out_c] 16-bit canvases
   void* out_lo;         // split-fp16 mode: low half of the normalised tensor (NULL otherwise)
-  int out_pitch, out_x0, out_y0, out_c;   // output canvas: pixels per row, paste offset, channels per pixel (4 | 8)
-  uint8_t* out_u8;      // optional [OH][OW][3] resized image in tensor channel order
-  int OH, OW;
-  size_t out_img;       // elements between the images of out (out_lo); out_u8 images are OH * OW * 3 bytes apart
+  int out_pitch, out_c; // output canvas: pixels per row, channels per pixel (4 | 8)
+  uint8_t* out_u8;      // optional resized image in tensor channel order, [out_rows][out_pitch][3] per image
+  size_t out_img;       // elements between the canvases of out (out_lo); out_u8 images are out_img / out_c * 3 bytes apart
 };
 
 template <class E>
-__device__ __forceinline__ void emit_pixel(const PreParams& p, int img, int oy, int ox, const int (&u)[3]) {
-  uint8_t* out_u8 = p.out_u8 ? p.out_u8 + static_cast<size_t>(img) * p.OH * p.OW * 3 : nullptr;
+__device__ __forceinline__ void emit_pixel(const PreParams& p, const PreImg& im, int img, int oy, int ox, const int (&u)[3]) {
+  const size_t pix = static_cast<size_t>(oy + im.out_y0) * p.out_pitch + (ox + im.out_x0);
+  uint8_t* out_u8 = p.out_u8 ? p.out_u8 + static_cast<size_t>(img) * (p.out_img / p.out_c) * 3 : nullptr;
   float v[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
@@ -128,12 +132,11 @@ __device__ __forceinline__ void emit_pixel(const PreParams& p, int img, int oy, 
     float x = static_cast<float>(s);
     x = p.mul_inv255 ? x * (1.0f / 255.0f) : __fdiv_rn(x, 255.0f);
     v[c] = __fdiv_rn(x - p.mean[c], p.stdv[c]);
-    if (out_u8) out_u8[(static_cast<size_t>(oy) * p.OW + ox) * 3 + c] = static_cast<uint8_t>(s);
+    if (out_u8) out_u8[pix * 3 + c] = static_cast<uint8_t>(s);
   }
   uint2 o, l;
   split2<E>(v[0], v[1], o.x, l.x);
   split2<E>(v[2], 0.f, o.y, l.y);
-  const size_t pix = static_cast<size_t>(oy + p.out_y0) * p.out_pitch + (ox + p.out_x0);
   reinterpret_cast<uint2*>(static_cast<typename E::T*>(p.out) + img * p.out_img)[pix * (p.out_c >> 2)] = o;
   if (p.out_lo) reinterpret_cast<uint2*>(p.out_lo)[pix * (p.out_c >> 2)] = l;
 }
@@ -153,8 +156,11 @@ static constexpr int kRowBytes = kTX * 3;     // 96
 //             neighbouring bytes, one aligned word load per tap; then /255, (x-mean)/std, 16-bit NHWC4 store.
 // Round 1's kernel (byte gathers with 11-way bank-conflicted coefficient reads, 8-row tiles whose vertical halo
 // re-staged every input row 1.75x) took 50 us per 1080p frame = 2 % of the HBM roofline.
+// A call may mix geometries: the grid covers the largest output, and a block outside its own image's output returns
+// (as a whole block, before the first barrier).
 template <class E, int XT>
-__global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PreParams p, int rows_cap, int pitch, int TY) {
+__global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __grid_constant__ PreParams p, int rows_cap,
+                                                                     int pitch, int TY) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ __align__(16) uint8_t sm[];
@@ -165,23 +171,26 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ox0 = blockIdx.x * kTX, oy0 = blockIdx.y * TY;
   const int img = blockIdx.z;                                      // image of the batch
-  const int ox1 = min(ox0 + kTX, p.OW) - 1, oy1 = min(oy0 + TY, p.OH) - 1;
+  const PreImg im = p.im[img];                                      // this image's fields, loaded once
+  if (ox0 >= im.OW || oy0 >= im.OH) return;
+  const int ox1 = min(ox0 + kTX, im.OW) - 1, oy1 = min(oy0 + TY, im.OH) - 1;
   // bounds are monotone non-decreasing: first / last output coordinate give the tile's input extent
-  const int x_lo = p.xb[ox0];
-  const int x_hi = min(p.xb[ox1] + p.xks, p.w);
-  const int y_lo = p.yb[oy0];
-  const int y_hi = min(p.yb[oy1] + p.yks, p.h);
+  const int x_lo = im.xb[ox0];
+  const int x_hi = min(im.xb[ox1] + im.xks, im.w);
+  const int y_lo = im.yb[oy0];
+  const int y_hi = min(im.yb[oy1] + im.yks, im.h);
   const int rows = y_hi - y_lo, pwb = (x_hi - x_lo) * 3;
   for (int i = tid; i < TY * 32; i += kPreThreads) {
     const int yo = i >> 5, t = i & 31;
-    s_yk[i] = (oy0 + yo <= oy1 && t < p.yks) ? p.yk[static_cast<size_t>(oy0 + yo) * p.yks + t] : 0;
+    s_yk[i] = (oy0 + yo <= oy1 && t < im.yks) ? im.yk[static_cast<size_t>(oy0 + yo) * im.yks + t] : 0;
   }
-  if (tid < TY) s_yb[tid] = (oy0 + tid <= oy1) ? p.yb[oy0 + tid] - y_lo : 0;
+  if (tid < TY) s_yb[tid] = (oy0 + tid <= oy1) ? im.yb[oy0 + tid] - y_lo : 0;
 
   // ---- phase 1: stage (coalesced aligned words)
-  const uintptr_t base = reinterpret_cast<uintptr_t>(p.src[img]) + static_cast<size_t>(x_lo) * 3;
+  const uintptr_t base = reinterpret_cast<uintptr_t>(im.src) + static_cast<size_t>(x_lo) * 3;
+  const int stride = im.stride;
   for (int r = warp; r < rows; r += kPreThreads / 32) {
-    const uintptr_t a = base + static_cast<size_t>(y_lo + r) * p.stride;
+    const uintptr_t a = base + static_cast<size_t>(y_lo + r) * stride;
     const uint32_t* w0 = reinterpret_cast<const uint32_t*>(a & ~static_cast<uintptr_t>(3));
     const int words = (static_cast<int>(a & 3) + pwb + 3) >> 2;
     uint32_t* dst = reinterpret_cast<uint32_t*>(patch + r * pitch);
@@ -193,9 +202,9 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
   const bool col_ok = ox0 + xo <= ox1;
   int K[XT];
 #pragma unroll
-  for (int t = 0; t < XT; ++t) K[t] = (col_ok && t < p.xks) ? __ldg(p.xk + static_cast<size_t>(ox0 + xo) * p.xks + t) : 0;
-  const int boff = col_ok ? (p.xb[ox0 + xo] - x_lo) * 3 + c : 0;  // byte offset of tap 0 inside the staged row
-  const int mis0 = static_cast<int>(base & 3), smis = p.stride & 3;
+  for (int t = 0; t < XT; ++t) K[t] = (col_ok && t < im.xks) ? __ldg(im.xk + static_cast<size_t>(ox0 + xo) * im.xks + t) : 0;
+  const int boff = col_ok ? (im.xb[ox0 + xo] - x_lo) * 3 + c : 0;  // byte offset of tap 0 inside the staged row
+  const int mis0 = static_cast<int>(base & 3), smis = stride & 3;
   __syncthreads();
 
   // ---- phase 2: horizontal pass (taps beyond the filter multiply staged bytes by 0: the row pitch covers XT taps)
@@ -218,14 +227,15 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
   // ---- phase 3: vertical pass on 32-bit byte columns + normalise + store
   const uint32_t* interw = reinterpret_cast<const uint32_t*>(inter);
   typename E::T* outp = reinterpret_cast<typename E::T*>(p.out) + img * p.out_img;
-  uint8_t* out_u8 = p.out_u8 ? p.out_u8 + static_cast<size_t>(img) * p.OH * p.OW * 3 : nullptr;
+  uint8_t* out_u8 = p.out_u8 ? p.out_u8 + static_cast<size_t>(img) * (p.out_img / p.out_c) * 3 : nullptr;
+  const int yks = im.yks, out_x0 = im.out_x0, out_y0 = im.out_y0;
   for (int i = tid; i < TY * (kRowBytes / 4); i += kPreThreads) {
     const int yo = i / (kRowBytes / 4), j = i - yo * (kRowBytes / 4);
     const int oy = oy0 + yo;
     if (oy > oy1) break;
     const int* k = s_yk + yo * 32;
     const int yb = s_yb[yo];
-    const int n = min(p.yks, rows - yb);
+    const int n = min(yks, rows - yb);
     int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21, a3 = 1 << 21;
     for (int t = 0; t < n; ++t) {
       const uint32_t wv = interw[(yb + t) * (kRowBytes / 4) + j];
@@ -249,7 +259,7 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
       const float mean = tc == 0 ? p.mean[0] : tc == 1 ? p.mean[1] : p.mean[2];     // selects, not a dynamic
       const float stdv = tc == 0 ? p.stdv[0] : tc == 1 ? p.stdv[1] : p.stdv[2];     // index into the params
       const float v = __fdiv_rn(x - mean, stdv);
-      const size_t pix = static_cast<size_t>(oy + p.out_y0) * p.out_pitch + (ox + p.out_x0);
+      const size_t pix = static_cast<size_t>(oy + out_y0) * p.out_pitch + (ox + out_x0);
       const size_t ei = pix * p.out_c + tc;                  // element index (out_c is even: ei is even for tc == 2)
       const typename E::T hi = from_f32<E>(v);
       if (tc == 2) reinterpret_cast<uint32_t*>(outp)[ei >> 1] = pack2<E>(v, 0.f);   // (channel 2, zero pad)
@@ -260,31 +270,32 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const PrePa
         if (tc == 2) reinterpret_cast<uint32_t*>(lop)[ei >> 1] = pack2<E>(lo, 0.f);
         else lop[ei] = from_f32<E>(lo);
       }
-      if (out_u8) out_u8[(static_cast<size_t>(oy) * p.OW + ox) * 3 + tc] = static_cast<uint8_t>(u[b]);
+      if (out_u8) out_u8[pix * 3 + tc] = static_cast<uint8_t>(u[b]);
     }
   }
 }
 
 // OpenCV path (and the no-resize path): one thread per output pixel, gather from global.
 template <class E>
-__global__ void __launch_bounds__(256) preprocess_direct_kernel(const PreParams p) {
+__global__ void __launch_bounds__(256) preprocess_direct_kernel(const __grid_constant__ PreParams p) {
   pdl_launch_dependents();
   pdl_wait();
   const int ox = blockIdx.x * blockDim.x + threadIdx.x;
   const int oy = blockIdx.y, img = blockIdx.z;
-  if (ox >= p.OW) return;
-  const uint8_t* src = p.src[img];
+  const PreImg im = p.im[img];                                      // this image's fields, loaded once
+  if (ox >= im.OW || oy >= im.OH) return;
+  const uint8_t* src = im.src;
   int u[3];
   if (p.mode == VPB_RESIZE_NONE) {
-    const uint8_t* s = src + static_cast<size_t>(oy) * p.stride + ox * 3;
+    const uint8_t* s = src + static_cast<size_t>(oy) * im.stride + ox * 3;
     u[0] = s[0]; u[1] = s[1]; u[2] = s[2];
   } else {
-    const int sx = p.xb[ox], sy = p.yb[oy];
-    const int sx1 = min(sx + 1, p.w - 1), sy1 = min(sy + 1, p.h - 1);
-    const int a0 = p.xk[2 * ox], a1 = p.xk[2 * ox + 1];
-    const int b0 = p.yk[2 * oy], b1 = p.yk[2 * oy + 1];
-    const uint8_t* r0 = src + static_cast<size_t>(sy) * p.stride;
-    const uint8_t* r1 = src + static_cast<size_t>(sy1) * p.stride;
+    const int sx = im.xb[ox], sy = im.yb[oy];
+    const int sx1 = min(sx + 1, im.w - 1), sy1 = min(sy + 1, im.h - 1);
+    const int a0 = im.xk[2 * ox], a1 = im.xk[2 * ox + 1];
+    const int b0 = im.yk[2 * oy], b1 = im.yk[2 * oy + 1];
+    const uint8_t* r0 = src + static_cast<size_t>(sy) * im.stride;
+    const uint8_t* r1 = src + static_cast<size_t>(sy1) * im.stride;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const int h0 = r0[sx * 3 + c] * a0 + r0[sx1 * 3 + c] * a1;
@@ -292,78 +303,128 @@ __global__ void __launch_bounds__(256) preprocess_direct_kernel(const PreParams 
       u[c] = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
     }
   }
-  emit_pixel<E>(p, img, oy, ox, u);
+  emit_pixel<E>(p, im, img, oy, ox, u);
 }
 
 // ---------------------------------------------------------------- host: plan
-int PreprocessPlan::configure(int in_h, int in_w, int mode_) {
+// Filter length of one axis (the ksize of resize_tables_host), without building the tables.
+static int axis_taps(int mode, int in_size, int out_size) {
+  if (!is_pil(mode)) return 2;
+  const double scale = static_cast<double>(in_size) / out_size;
+  const double support = (mode == VPB_RESIZE_PIL_BILINEAR ? 1.0 : 2.0) * (scale < 1.0 ? 1.0 : scale);
+  return static_cast<int>(std::ceil(support)) * 2 + 1;
+}
+
+int PreprocessPlan::check(const PreGeom& g, int mode_, const char* who, int k) {
+  if (mode_ == VPB_RESIZE_NONE && (g.h != g.OH || g.w != g.OW)) {
+    vpb_set_error("%s: frame %d: resize mode 'none' needs a %dx%d input, got %dx%d", who, k, g.OW, g.OH, g.w, g.h);
+    return VPB_ERR_ARG;
+  }
+  if (mode_ != VPB_RESIZE_NONE) {
+    const int taps = std::max(axis_taps(mode_, g.w, g.OW), axis_taps(mode_, g.h, g.OH));
+    if (is_pil(mode_) && taps > 32) {
+      vpb_set_error("%s: frame %d: %dx%d -> %dx%d needs %d-tap filters (max 32: input at most ~7x the network size)",
+                    who, k, g.w, g.h, g.OW, g.OH, taps);
+      return VPB_ERR_ARG;
+    }
+  }
+  return VPB_OK;
+}
+
+// Worst-case input extent of the tiles of one axis: the largest (last input coordinate + 1 - first) over tiles of
+// `tile` outputs.
+static int tile_extent(const std::vector<int>& bounds, int ks, int in_size, int tile) {
+  const int out = static_cast<int>(bounds.size());
+  int cap = 0;
+  for (int o0 = 0; o0 < out; o0 += tile) {
+    int hi = 0;
+    for (int o = o0; o < std::min(o0 + tile, out); ++o) hi = std::max(hi, std::min(bounds[o] + ks, in_size));
+    cap = std::max(cap, hi - bounds[o0]);
+  }
+  return cap;
+}
+
+int PreprocessPlan::configure(const PreGeom* g, int n_, int mode_) {
   int cur = -1;
   cudaGetDevice(&cur);
-  if (in_h == h && in_w == w && mode_ == mode && d_tables && cur == device) return VPB_OK;
+  if (n_ < 1 || n_ > kMaxBatch) { vpb_set_error("preprocess: %d images (1..%d)", n_, kMaxBatch); return VPB_ERR_ARG; }
+  if (n_ == n && mode_ == mode && d_tables && cur == device && std::equal(g, g + n_, geom)) return VPB_OK;
   if (d_tables && cur != device) {   // the plan's tables live on another device (thread_local plan of vpb_preprocess)
     int keep = cur;
     cudaSetDevice(device); cudaFree(d_tables); cudaSetDevice(keep);
     d_tables = nullptr;
   }
-  if (mode_ == VPB_RESIZE_NONE && (in_h != OH || in_w != OW)) {
-    vpb_set_error("preprocess: resize mode 'none' needs a %dx%d input, got %dx%d", OW, OH, in_w, in_h);
-    return VPB_ERR_ARG;
+  for (int k = 0; k < n_; ++k) {
+    const int rc = check(g[k], mode_, "preprocess", k);
+    if (rc) return rc;
   }
-  h = in_h; w = in_w; mode = mode_;
-  std::vector<int> xb, xk, yb, yk;
-  if (mode == VPB_RESIZE_NONE) {
-    xks = yks = 0;
-    xb.assign(OW, 0); yb.assign(OH, 0); xk.assign(1, 0); yk.assign(1, 0);
-  } else {
-    resize_tables_host(mode, w, OW, xb, xk, xks);
-    resize_tables_host(mode, h, OH, yb, yk, yks);
-  }
-  if (is_pil(mode) && (xks > 32 || yks > 32)) {
-    vpb_set_error("preprocess: %dx%d -> %dx%d needs %d-tap filters (max 32: input at most ~7x the network size)", w, h, OW, OH, std::max(xks, yks));
-    return VPB_ERR_ARG;
-  }
-  if (is_pil(mode)) {
-    // worst-case tile extents for the shared-memory staging; the row tile TY shrinks until two blocks fit an SM
-    // (very large inputs: until one does)
-    patch_w_cap = 0;
-    for (int x0 = 0; x0 < OW; x0 += kTX) {
-      int hi = 0;
-      for (int x = x0; x < std::min(x0 + kTX, OW); ++x) hi = std::max(hi, std::min(xb[x] + xks, w));
-      patch_w_cap = std::max(patch_w_cap, hi - xb[x0]);
+  // one table set per distinct geometry, all in one allocation
+  struct Set { PreGeom g; std::vector<int> xb, xk, yb, yk; int xks = 0, yks = 0; size_t off = 0; };
+  std::vector<Set> sets;
+  int set_of[kMaxBatch];
+  for (int k = 0; k < n_; ++k) {
+    int j = 0;
+    while (j < static_cast<int>(sets.size()) && sets[j].g != g[k]) ++j;
+    if (j == static_cast<int>(sets.size())) {
+      Set st; st.g = g[k];
+      if (mode_ == VPB_RESIZE_NONE) {
+        st.xb.assign(g[k].OW, 0); st.yb.assign(g[k].OH, 0); st.xk.assign(1, 0); st.yk.assign(1, 0);
+      } else {
+        resize_tables_host(mode_, g[k].w, g[k].OW, st.xb, st.xk, st.xks);
+        resize_tables_host(mode_, g[k].h, g[k].OH, st.yb, st.yk, st.yks);
+      }
+      sets.push_back(std::move(st));
     }
-    xt = xks <= 16 ? 16 : 32;
-    pitch = ((patch_w_cap + xt) * 3 + 3 + 3) & ~3;     // + misalignment, + the zero-weight taps past the filter
+    set_of[k] = j;
+  }
+  if (is_pil(mode_)) {
+    // one tap capacity and one row tile TY for the call: the staging of the worst tile of any image must fit; TY
+    // shrinks until two blocks fit an SM (very large inputs: until one does)
+    xt = 16;
+    for (const Set& st : sets) if (st.xks > 16) xt = 32;
+    pitch = 0;
+    for (const Set& st : sets) {
+      const int patch_w_cap = tile_extent(st.xb, st.xks, st.g.w, kTX);
+      pitch = std::max(pitch, ((patch_w_cap + xt) * 3 + 3 + 3) & ~3);   // + misalignment, + the zero-weight taps
+    }
     bool fits = false;
     for (int ty : {kTYMax, 16, 10, 8, 5, 4, 2, 1}) {
       rows_cap = 0;
-      for (int y0 = 0; y0 < OH; y0 += ty) {
-        int hi = 0;
-        for (int y = y0; y < std::min(y0 + ty, OH); ++y) hi = std::max(hi, std::min(yb[y] + yks, h));
-        rows_cap = std::max(rows_cap, hi - yb[y0]);
-      }
+      for (const Set& st : sets) rows_cap = std::max(rows_cap, tile_extent(st.yb, st.yks, st.g.h, ty));
       smem_bytes = static_cast<size_t>(rows_cap) * pitch + static_cast<size_t>(rows_cap) * kRowBytes + 16;
       TY = ty;
       if (smem_bytes <= (ty > 4 ? 100u : 200u) * 1024) { fits = true; break; }
     }
     if (!fits) {
-      vpb_set_error("preprocess: %dx%d -> %dx%d needs %zu B of shared memory per tile (input too large)",
-                    w, h, OW, OH, smem_bytes);
+      vpb_set_error("preprocess: %d image(s) need %zu B of shared memory per tile (input too large)", n_, smem_bytes);
       return VPB_ERR_ARG;
     }
   }
-  const size_t n = xb.size() + xk.size() + yb.size() + yk.size();
-  if (d_tables) cudaFree(d_tables);
-  VPB_CUDA_OK(cudaMalloc(&d_tables, n * sizeof(int)));
   std::vector<int> all;
-  all.reserve(n);
-  off_xb = 0; all.insert(all.end(), xb.begin(), xb.end());
-  off_xk = all.size(); all.insert(all.end(), xk.begin(), xk.end());
-  off_yb = all.size(); all.insert(all.end(), yb.begin(), yb.end());
-  off_yk = all.size(); all.insert(all.end(), yk.begin(), yk.end());
-  VPB_CUDA_OK(cudaMemcpy(d_tables, all.data(), n * sizeof(int), cudaMemcpyHostToDevice));
+  for (Set& st : sets) {
+    st.off = all.size();
+    all.insert(all.end(), st.xb.begin(), st.xb.end());
+    all.insert(all.end(), st.xk.begin(), st.xk.end());
+    all.insert(all.end(), st.yb.begin(), st.yb.end());
+    all.insert(all.end(), st.yk.begin(), st.yk.end());
+  }
+  if (d_tables) { cudaFree(d_tables); d_tables = nullptr; }
+  n = 0;                                 // invalid until the tables are resident
+  VPB_CUDA_OK(cudaMalloc(&d_tables, all.size() * sizeof(int)));
+  VPB_CUDA_OK(cudaMemcpy(d_tables, all.data(), all.size() * sizeof(int), cudaMemcpyHostToDevice));
   // a pageable H2D copy may return once the data is staged: the consuming kernel runs on a non-blocking stream
-  // that is NOT ordered after the legacy default stream, so drain the device once per (size, mode)
+  // that is NOT ordered after the legacy default stream, so drain the device once per geometry set and mode
   VPB_CUDA_OK(cudaDeviceSynchronize());
+  OHmax = OWmax = 0;
+  for (int k = 0; k < n_; ++k) {
+    const Set& st = sets[set_of[k]];
+    geom[k] = g[k];
+    tab[k].xb = st.off; tab[k].xk = tab[k].xb + st.xb.size();
+    tab[k].yb = tab[k].xk + st.xk.size(); tab[k].yk = tab[k].yb + st.yb.size();
+    tab[k].xks = st.xks; tab[k].yks = st.yks;
+    OHmax = std::max(OHmax, g[k].OH); OWmax = std::max(OWmax, g[k].OW);
+  }
+  n = n_; mode = mode_;
   cudaGetDevice(&device);
   return VPB_OK;
 }
@@ -372,18 +433,26 @@ PreprocessPlan::~PreprocessPlan() {
   if (d_tables) cudaFree(d_tables);
 }
 
-static int fill_params(const PreprocessPlan& pl, const uint8_t* const* srcs, int batch, int stride, int convention,
-                       void* out, uint8_t* out_u8, PreParams& p) {
-  if (batch < 1 || batch > kMaxBatch || (batch > 1 && pl.out_lo)) {
-    vpb_set_error("preprocess: batch %d (1..%d, 16-bit output only)", batch, kMaxBatch);
+static int fill_params(const PreprocessPlan& pl, const vpb_frame* frames, int convention, void* out, uint8_t* out_u8,
+                       PreParams& p) {
+  if (pl.n < 1 || (pl.n > 1 && pl.out_lo)) {
+    vpb_set_error("preprocess: batch %d (1..%d, 16-bit output only)", pl.n, kMaxBatch);
     return VPB_ERR_ARG;
   }
   p.out_lo = pl.out_lo;
-  p.out_pitch = pl.out_pitch > 0 ? pl.out_pitch : pl.OW; p.out_x0 = pl.out_x0; p.out_y0 = pl.out_y0;
-  p.out_c = pl.out_c;
-  for (int i = 0; i < kMaxBatch; ++i) p.src[i] = srcs[i < batch ? i : 0];
-  p.h = pl.h; p.w = pl.w; p.stride = stride; p.mode = pl.mode;
-  p.out_img = static_cast<size_t>(pl.out_rows > 0 ? pl.out_rows : pl.OH) * p.out_pitch * pl.out_c;   // whole canvases
+  p.out_pitch = pl.out_pitch; p.out_c = pl.out_c;
+  for (int i = 0; i < kMaxBatch; ++i) {
+    const int k = i < pl.n ? i : 0;
+    PreImg& im = p.im[i];
+    const PreGeom& g = pl.geom[k];
+    const PreprocessPlan::Tables& t = pl.tab[k];
+    im.src = frames[k].data; im.stride = frames[k].stride;
+    im.h = g.h; im.w = g.w; im.OH = g.OH; im.OW = g.OW; im.out_x0 = g.x0; im.out_y0 = g.y0;
+    im.xb = pl.d_tables + t.xb; im.xk = pl.d_tables + t.xk; im.xks = t.xks;
+    im.yb = pl.d_tables + t.yb; im.yk = pl.d_tables + t.yk; im.yks = t.yks;
+  }
+  p.mode = pl.mode;
+  p.out_img = static_cast<size_t>(pl.out_rows) * p.out_pitch * pl.out_c;   // whole canvases
   // conventions: see include/vp_b200_ops.h
   static const float kMeanRGB[3] = {0.485f, 0.456f, 0.406f}, kStdRGB[3] = {0.229f, 0.224f, 0.225f};
   p.swap_rb = convention == VPB_CONV_BGR_SWAP ? 1 : 0;
@@ -393,9 +462,7 @@ static int fill_params(const PreprocessPlan& pl, const uint8_t* const* srcs, int
     p.mean[c] = convention == VPB_CONV_RGB_UNIT ? 0.f : kMeanRGB[s];   // ToTensor only (auto_speed_infer.py:50)
     p.stdv[c] = convention == VPB_CONV_RGB_UNIT ? 1.f : kStdRGB[s];
   }
-  p.xb = pl.d_tables + pl.off_xb; p.xk = pl.d_tables + pl.off_xk; p.xks = pl.xks;
-  p.yb = pl.d_tables + pl.off_yb; p.yk = pl.d_tables + pl.off_yk; p.yks = pl.yks;
-  p.out = out; p.out_u8 = out_u8; p.OH = pl.OH; p.OW = pl.OW;
+  p.out = out; p.out_u8 = out_u8;
   return VPB_OK;
 }
 
@@ -413,13 +480,12 @@ static const void* kernel_func(int mode, int dtype, int xt) {
 
 bool PreprocessPlan::owns_kernel(const void* func, int dtype) const { return func == kernel_func(mode, dtype, xt); }
 
-// Re-point the captured pre-process node at another source frame (same geometry): lets the frame
-// graph be replayed on any device buffer without re-capturing.
-int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const uint8_t* const* srcs,
-                                      int batch, int stride, int convention, int dtype, void* out,
-                                      uint8_t* out_u8) const {
+// Re-point the captured pre-process node at other source frames (same geometries): lets the frame graph be replayed
+// on any device buffers without re-capturing.
+int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame* frames,
+                                      int convention, int dtype, void* out, uint8_t* out_u8) const {
   PreParams p;
-  const int rc = fill_params(*this, srcs, batch, stride, convention, out, out_u8, p);
+  const int rc = fill_params(*this, frames, convention, out, out_u8, p);
   if (rc) return rc;
   int rc_ = rows_cap, pitch_ = pitch, ty_ = TY;
   void* args[4] = {&p, &rc_, &pitch_, &ty_};
@@ -428,11 +494,11 @@ int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node
   kp.kernelParams = args;
   kp.extra = nullptr;
   if (is_pil(mode)) {
-    kp.gridDim = dim3((OW + kTX - 1) / kTX, (OH + TY - 1) / TY, batch);
+    kp.gridDim = dim3((OWmax + kTX - 1) / kTX, (OHmax + TY - 1) / TY, n);
     kp.blockDim = dim3(kPreThreads);
     kp.sharedMemBytes = static_cast<unsigned>(smem_bytes);
   } else {
-    kp.gridDim = dim3((OW + 255) / 256, OH, batch);
+    kp.gridDim = dim3((OWmax + 255) / 256, OHmax, n);
     kp.blockDim = dim3(256);
     kp.sharedMemBytes = 0;
   }
@@ -440,13 +506,13 @@ int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node
   return VPB_OK;
 }
 
-int PreprocessPlan::launch(const uint8_t* const* srcs, int batch, int stride, int convention, int dtype, void* out,
-                           uint8_t* out_u8, cudaStream_t stream) const {
+int PreprocessPlan::launch(const vpb_frame* frames, int convention, int dtype, void* out, uint8_t* out_u8,
+                           cudaStream_t stream) const {
   PreParams p;
-  const int rc = fill_params(*this, srcs, batch, stride, convention, out, out_u8, p);
+  const int rc = fill_params(*this, frames, convention, out, out_u8, p);
   if (rc) return rc;
   if (is_pil(mode)) {
-    dim3 grid((OW + kTX - 1) / kTX, (OH + TY - 1) / TY, batch);
+    dim3 grid((OWmax + kTX - 1) / kTX, (OHmax + TY - 1) / TY, n);
     {
       std::lock_guard<std::mutex> g(init_mutex());
       bool* done = device_flag(kInitPreprocess);
@@ -467,7 +533,7 @@ int PreprocessPlan::launch(const uint8_t* const* srcs, int batch, int stride, in
       else VPB_CUDA_OK(launch_k(preprocess_pil_kernel<F16, 32>, grid, blk, smem_bytes, stream, p, rows_cap, pitch, TY));
     }
   } else {
-    dim3 grid((OW + 255) / 256, OH, batch);
+    dim3 grid((OWmax + 255) / 256, OHmax, n);
     if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(preprocess_direct_kernel<BF16>, grid, dim3(256), 0, stream, p));
     else VPB_CUDA_OK(launch_k(preprocess_direct_kernel<F16>, grid, dim3(256), 0, stream, p));
   }
@@ -501,8 +567,10 @@ extern "C" int vpb_preprocess(const uint8_t* src_dev, int h, int w, int stride, 
                               int convention, int dtype, void* out_dev, uint8_t* out_u8_dev,
                               void* stream) {
   static thread_local vpb::PreprocessPlan plan;
-  int rc = plan.configure(h, w, resize_mode);
+  vpb::PreGeom g;
+  g.h = h; g.w = w;
+  int rc = plan.configure(&g, 1, resize_mode);
   if (rc != VPB_OK) return rc;
-  return plan.launch(&src_dev, 1, stride, convention, dtype, out_dev, out_u8_dev,
-                     static_cast<cudaStream_t>(stream));
+  const vpb_frame f{src_dev, h, w, stride};
+  return plan.launch(&f, convention, dtype, out_dev, out_u8_dev, static_cast<cudaStream_t>(stream));
 }

@@ -74,6 +74,9 @@ def _bind():
                                        C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.vp_engine_read_tap.restype = C.c_long
     lib.vp_engine_read_resized.argtypes = [C.c_void_p, C.c_void_p]
+    lib.vp_engine_read_resized_at.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    for fn in ("vp_engine_infer_frames", "vp_engine_submit_frames", "vp_engine_infer_device_frames"):
+        getattr(lib, fn).argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int]
     lib.vp_engine_tap_dev.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(_TapView)]
     lib.vp_engine_stream.argtypes = [C.c_void_p]
     lib.vp_engine_stream.restype = C.c_void_p
@@ -90,8 +93,8 @@ class Engine:
                  precision: Optional[int] = None, batch: int = 1):
         """dtype "fp16" | "bf16": 16-bit operands; dtype "fp32" (the reference's precision="fp32") selects the
         split-fp16 fp32-grade mode (precision=PREC_SPLIT on fp16 pairs).  batch > 1 (16-bit only): every call takes
-        exactly `batch` frames of one geometry (infer_batch / submit_batch / infer_device_batch); sample k's outputs
-        are raw(idx, k) / cls(idx, k)."""
+        exactly `batch` frames, of one geometry (infer_batch / submit_batch / infer_device_batch) or each of its own
+        size (infer_frames / submit_frames / infer_device_frames); sample k's outputs are raw(idx, k) / cls(idx, k)."""
         self._lib = _bind()
         cfg = _Config()
         cfg.gpu_id, cfg.dtype = gpu_id, DTYPE_BY_NAME[dtype]
@@ -184,6 +187,37 @@ class Engine:
         L.check(self._lib.vp_engine_infer_device_batch(self._h, self._ptrs(dev_ptrs), len(dev_ptrs), h, w, stride),
                 "vp_engine_infer_device_batch")
 
+    def _check_frames(self, frames: Sequence[np.ndarray], allow_copy: bool) -> List[np.ndarray]:
+        """`batch` frames, each of its own shape and row stride (checked here, before the C call)."""
+        frames = list(frames)
+        if len(frames) != self.batch:
+            raise ValueError(f"{len(frames)} frame(s) for an engine of batch {self.batch}")
+        return [self._check_frame(f, allow_copy) for f in frames]
+
+    @staticmethod
+    def _descs(frames: Sequence[np.ndarray]):
+        return L.frame_descs([(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames])
+
+    def infer_frames(self, frames: Sequence[np.ndarray]) -> None:
+        """`batch` uint8 [h_k, w_k, 3] host frames, each of its own size (a mixed camera rig), in one call; outputs of
+        frame k are sample k."""
+        frames = self._check_frames(frames, allow_copy=True)
+        L.check(self._lib.vp_engine_infer_frames(self._h, self._descs(frames), len(frames)), "vp_engine_infer_frames")
+
+    def submit_frames(self, frames: Sequence[np.ndarray]) -> None:
+        """Asynchronous infer_frames() (pinned frames: pinned_frames(shapes)); sync() completes it."""
+        frames = self._check_frames(frames, allow_copy=False)
+        L.check(self._lib.vp_engine_submit_frames(self._h, self._descs(frames), len(frames)), "vp_engine_submit_frames")
+
+    def infer_device_frames(self, descs: Sequence[Sequence[int]]) -> None:
+        """`batch` device frames as (data_ptr, h, w, stride) tuples, each of its own geometry, in one asynchronous
+        call."""
+        descs = list(descs)
+        if len(descs) != self.batch:
+            raise ValueError(f"{len(descs)} frame(s) for an engine of batch {self.batch}")
+        L.check(self._lib.vp_engine_infer_device_frames(self._h, L.frame_descs(descs), len(descs)),
+                "vp_engine_infer_device_frames")
+
     def sync(self) -> None:
         L.check(self._lib.vp_engine_sync(self._h), "vp_engine_sync")
 
@@ -198,6 +232,23 @@ class Engine:
             raise RuntimeError(L.last_error())
         a = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(size,))
         return a.reshape(h, w, 3) if n is None else a.reshape(n, h, w, 3)
+
+    def pinned_frames(self, shapes: Sequence[Sequence[int]]) -> List[np.ndarray]:
+        """Views [h_k, w_k, 3] into one engine-owned pinned host buffer, one per (h, w) in shapes
+        (submit_frames(views))."""
+        shapes = [(int(h), int(w)) for h, w in shapes]
+        if any(h <= 0 or w <= 0 for h, w in shapes):
+            raise ValueError(f"frame shapes must be positive, got {shapes}")
+        sizes = [h * w * 3 for h, w in shapes]
+        p = self._lib.vp_engine_pinned_frame(self._h, max(sum(sizes), 1))
+        if not p:
+            raise RuntimeError(L.last_error())
+        a = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(max(sum(sizes), 1),))
+        views, off = [], 0
+        for (h, w), n in zip(shapes, sizes):
+            views.append(a[off:off + n].reshape(h, w, 3))
+            off += n
+        return views
 
     # ---- outputs (views into engine-owned host buffers: copy if kept past the next infer)
     def _out(self, idx: int, sample: int = 0) -> _Output:
@@ -272,9 +323,10 @@ class Engine:
     def handle(self) -> C.c_void_p:
         return self._h
 
-    def read_resized(self) -> np.ndarray:
+    def read_resized(self, sample: int = 0) -> np.ndarray:
+        """The 640x320 uint8 image the fused resize produced for sample `sample` of the last call."""
         buf = np.empty((320, 640, 3), dtype=np.uint8)
-        L.check(self._lib.vp_engine_read_resized(self._h, buf.ctypes.data), "vp_engine_read_resized")
+        L.check(self._lib.vp_engine_read_resized_at(self._h, sample, buf.ctypes.data), "vp_engine_read_resized_at")
         return buf
 
     def read_tap(self, name: str) -> np.ndarray:

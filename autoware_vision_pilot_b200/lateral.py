@@ -28,6 +28,9 @@ def _bind():
     lib.vpb_lateral_update_batch.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                              C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p, C.c_void_p,
                                              C.c_void_p]
+    lib.vpb_lateral_update_cameras.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
+                                               C.POINTER(C.c_int), C.c_float, C.POINTER(C.c_double),
+                                               C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p]
     return lib
 
 
@@ -78,20 +81,40 @@ class LateralPostProcess:
         return self.result()
 
 
+def _image_sizes(cameras: int, image_size) -> List[tuple]:
+    """One (w, h) for every camera, or `cameras` (w, h) pairs -> a list of `cameras` positive (w, h) int pairs."""
+    sizes = list(image_size)
+    if len(sizes) == 2 and all(np.isscalar(v) for v in sizes):
+        sizes = [tuple(sizes)] * cameras
+    if len(sizes) != cameras:
+        raise ValueError(f"{len(sizes)} image sizes for {cameras} cameras")
+    out = []
+    for k, s in enumerate(sizes):
+        w, h = (int(v) for v in s)
+        if w <= 0 or h <= 0:
+            raise ValueError(f"camera {k}: image size {w}x{h} is not positive")
+        out.append((w, h))
+    return out
+
+
 class BatchedLateralPostProcess:
-    """n cameras (1..8) of one frame geometry, one launch per frame (vpb_lateral_update_batch): camera k keeps its own
-    state and homography and gets its own steering value.  Camera k's record and state are byte-identical to a
-    `LateralPostProcess` fed camera k's frames alone."""
+    """n cameras (1..8), one launch per frame (vpb_lateral_update_cameras): camera k keeps its own state, homography
+    and source image size and gets its own steering value.  Camera k's record and state are byte-identical to a
+    `LateralPostProcess` of the same image size fed camera k's frames alone."""
 
     def __init__(self, cameras: int, image_size=(1920, 1080), smoothing_factor: float = 0.5,
                  homographies: Optional[Sequence[Sequence[float]]] = None, device: str = "cuda:0"):
-        """homographies: None (the reference matrix for every camera) or one 3x3 / 9-value orig -> BEV matrix per
+        """image_size: one (w, h) for every camera, or one (w, h) per camera (a mixed rig, or a cropped view).
+        homographies: None (the reference matrix for every camera) or one 3x3 / 9-value orig -> BEV matrix per
         camera."""
         if not 1 <= cameras <= MAX_CAMERAS:
             raise ValueError(f"{cameras} cameras (1..{MAX_CAMERAS})")
+        sizes = _image_sizes(cameras, image_size)
         self._lib = _bind()
         self.cameras = cameras
-        self.image_size = tuple(image_size)
+        self.image_sizes = sizes
+        self._img_w = (C.c_int * cameras)(*[w for w, _ in sizes])
+        self._img_h = (C.c_int * cameras)(*[h for _, h in sizes])
         self.smoothing = float(smoothing_factor)
         self._hom = None
         if homographies is not None:
@@ -124,10 +147,10 @@ class BatchedLateralPostProcess:
             if len(steering) != self.cameras:
                 raise ValueError(f"{len(steering)} steering values for {self.cameras} cameras")
             st = (C.c_double * self.cameras)(*[float(v) for v in steering])
-        L.check(self._lib.vpb_lateral_update_batch(masks_ptr, self.cameras, height, width, self.image_size[0],
-                                                   self.image_size[1], self.smoothing, self._hom, st,
-                                                   self._state.data_ptr(), self._out.data_ptr(), stream or None),
-                "vpb_lateral_update_batch")
+        L.check(self._lib.vpb_lateral_update_cameras(masks_ptr, self.cameras, height, width, self._img_w, self._img_h,
+                                                     self.smoothing, self._hom, st, self._state.data_ptr(),
+                                                     self._out.data_ptr(), stream or None),
+                "vpb_lateral_update_cameras")
 
     def results(self) -> List[dict]:
         """Copy the n records to the host (synchronises) and return them as dicts, camera order."""

@@ -28,10 +28,12 @@
  * There is no CPU fallback: every entry point that computes requires a CUDA device of compute
  * capability 9.0 (H100, the library is built for sm_90a) and fails with VPB_ERR_CUDA otherwise.
  *
- * Batched engines (vp_engine_config.batch = N > 1) evaluate N frames of one geometry per call through
- * the same launch list: one weight copy, one graph replay, activations and outputs for N samples.
- * They take the *_batch entry points only; sample k of the outputs is vp_engine_output_at(.., k, ..)
- * and tap "<name>@k".  Sample k's outputs are bit-identical to a batch-1 engine's on frame k.
+ * Batched engines (vp_engine_config.batch = N > 1) evaluate N frames per call through the same launch
+ * list: one weight copy, one graph replay, activations and outputs for N samples.  They take the *_batch
+ * entry points (N frames of one geometry) or the *_frames entry points (N vpb_frame descriptors, each with
+ * its own h, w and stride: cameras of different resolutions in one call).  Sample k of the outputs is
+ * vp_engine_output_at(.., k, ..) and tap "<name>@k".  Sample k's outputs are bit-identical to a batch-1
+ * engine's on frame k.
  */
 #ifndef VP_B200_H_
 #define VP_B200_H_
@@ -111,6 +113,17 @@ int vp_engine_sync(vp_engine* e);
 int vp_engine_infer_batch(vp_engine* e, const uint8_t* const* frames_host, int n, int h, int w, int stride);
 int vp_engine_submit_batch(vp_engine* e, const uint8_t* const* frames_host, int n, int h, int w, int stride);
 int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev, int n, int h, int w, int stride);
+/* The batched calls with one descriptor per frame: frames[k] is frame k with its own h, w and stride (a front
+ * camera at 1920x1080 next to side cameras at 1280x720, or a cropped ROI view), n == the engine's batch.  Every
+ * descriptor is checked before any device work: VPB_ERR_ARG, with a message naming the call and the frame index,
+ * for n != batch, a NULL data pointer, h or w <= 0, stride < 3*w, a frame other than 640x320 under
+ * VPB_RESIZE_NONE, or a frame whose Pillow filter needs more than 32 taps.  Host frames are copied with pitch
+ * 3*w_k each (w_k*3 bytes read per row); vp_engine_submit_frames reads them asynchronously, so give it pinned
+ * memory.  The *_batch calls are the case of n equal descriptors.  The frame graph is keyed on the n (h, w,
+ * stride) triples: new pointers only re-point the captured pre-process node, a new geometry captures again. */
+int vp_engine_infer_frames(vp_engine* e, const vpb_frame* frames_host, int n);
+int vp_engine_submit_frames(vp_engine* e, const vpb_frame* frames_host, int n);
+int vp_engine_infer_device_frames(vp_engine* e, const vpb_frame* frames_dev, int n);
 /* Copy the raw fp32 tensor of one model to its host buffer (after a device/async inference). */
 int vp_engine_fetch_raw(vp_engine* e, int model_idx);
 
@@ -183,6 +196,8 @@ void* vp_engine_stream(vp_engine* e);
 /* The 640x320 uint8 image the fused pre-process produced for the last frame ([320][640][3], tensor
  * channel order) — lets the parity tests check the integer resize stage bit-exactly. */
 int vp_engine_read_resized(vp_engine* e, uint8_t* dst);
+/* The same for sample `sample` (0 .. batch-1) of a batched engine; vp_engine_read_resized is sample 0. */
+int vp_engine_read_resized_at(vp_engine* e, int sample, uint8_t* dst);
 
 #ifdef __cplusplus
 }

@@ -18,6 +18,8 @@
  * depend on N).  Every per-frame buffer holds N samples, sample outermost; sample k's raw tensor, detections and taps
  * are bit-identical to a batch-1 engine's on frame k.  Batched engines take the *_batch calls only; the single-frame
  * calls, a frame count other than N and a sample outside 0..N-1 return VPB_ERR_ARG.  vp_autospeed_create is batch 1.
+ * The *_frames calls take N vpb_frame descriptors of different sizes: the letterbox (scale, resized size, padding)
+ * and its inverse in the NMS are computed per sample.
  * The thresholds are shared by all samples.
  *
  * The checkpoint is a .vpw file holding the module's state_dict (python -m autoware_vision_pilot_b200.convert);
@@ -54,6 +56,11 @@ int vp_autospeed_infer_device(vp_autospeed* e, const uint8_t* frame_dev_rgb, int
 int vp_autospeed_infer_batch(vp_autospeed* e, const uint8_t* const* frames_host_rgb, int n, int h, int w, int stride,
                              int fetch_raw);
 int vp_autospeed_infer_device_batch(vp_autospeed* e, const uint8_t* const* frames_dev_rgb, int n, int h, int w, int stride);
+/* The same two calls with one descriptor per frame (each its own h, w, stride), n == batch.  Every descriptor is checked
+ * before any device work (VPB_ERR_ARG naming the call and the frame index: n != batch, NULL data, h or w <= 0,
+ * stride < 3*w, a letterbox filter of more than 32 taps).  The *_batch calls are the case of n equal descriptors. */
+int vp_autospeed_infer_frames(vp_autospeed* e, const vpb_frame* frames_host_rgb, int n, int fetch_raw);
+int vp_autospeed_infer_device_frames(vp_autospeed* e, const vpb_frame* frames_dev_rgb, int n);
 /* Drain the stream; fetch: 0 nothing, 1 detections, 2 detections + raw tensor to the host buffers (all samples). */
 int vp_autospeed_sync(vp_autospeed* e, int fetch);
 

@@ -42,6 +42,10 @@ enum {
 
 enum { VPB_ALGO_TILE = 0, VPB_ALGO_LINEAR = 1 };
 
+/* One camera frame of a batched call (vp_engine_*_frames, vp_autospeed_*_frames): uint8 HWC, 3 interleaved
+ * channels, `stride` bytes per row (>= 3*w).  Each frame of a call may have its own h, w and stride. */
+typedef struct { const uint8_t* data; int h, w, stride; } vpb_frame;
+
 const char* vpb_last_error(void);
 void vpb_set_error(const char* fmt, ...);
 
@@ -346,6 +350,14 @@ int vpb_lateral_update(const float* masks, int H, int W, int img_w, int img_h, f
 int vpb_lateral_update_batch(const float* masks, int n, int H, int W, int img_w, int img_h, float smoothing,
                              const double* homographies, const double* steering_rad,
                              vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream);
+/* vpb_lateral_update_batch with one source size per camera: camera k's frame is img_w[k] x img_h[k] (host arrays of
+ * n ints), so cameras of different resolutions, or a cropped view next to a full frame, share one launch.  Camera k's
+ * state and record are byte-identical to vpb_lateral_update with img_w[k] x img_h[k].  VPB_ERR_ARG before any device
+ * work as above, and for NULL img_w / img_h or a non-positive size (the message names the camera).
+ * vpb_lateral_update_batch and vpb_lateral_update are the case of n equal sizes. */
+int vpb_lateral_update_cameras(const float* masks, int n, int H, int W, const int* img_w, const int* img_h,
+                               float smoothing, const double* homographies, const double* steering_rad,
+                               vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream);
 
 /* ---- AutoSteer boundary (SURVEY.md 8f rank 2) ----
  * The AutoSteer v1 network itself (ONNX [1,6,80,160] -> 2 x [1,61]) is not in the reference repository

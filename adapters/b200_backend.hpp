@@ -35,8 +35,11 @@ class B200Backend : public InferenceBackend
 {
 public:
   // model_kind: VP_SCENE_SEG / VP_SCENE_3D / VP_DOMAIN_SEG / VP_EGO_LANES
+  // source_outputs: every doInference also makes the result at the input image's own size on the GPU (the resize-back
+  // run_model_node.cpp:96-104,177 does on the CPU): getSourceMask() / getSourceDepth()
   B200Backend(const std::string & model_path, const std::string & precision, int gpu_id,
-              int model_kind = VP_SCENE_SEG)
+              int model_kind = VP_SCENE_SEG, bool source_outputs = false)
+  : source_kind_(source_outputs ? (model_kind == VP_SCENE_3D ? VP_SRC_DEPTH : VP_SRC_MASK) : 0)
   {
     vp_engine_config cfg{};
     cfg.gpu_id = gpu_id;
@@ -53,6 +56,7 @@ public:
     cfg.weights[0] = model_path.c_str();
     cfg.fetch_raw = 1;
     cfg.use_graph = 1;
+    cfg.source_outputs = source_kind_;
     if (vp_engine_create(&cfg, &engine_) != VPB_OK) {
       throw std::runtime_error(std::string("B200Backend: ") + vp_last_error());
     }
@@ -69,6 +73,7 @@ public:
       return false;
     }
     ran_ = true;
+    if (source_kind_ && vp_engine_source_output(engine_, 0, 0, source_kind_, &src_) != VPB_OK) return false;
     return vp_engine_output(engine_, 0, &out_) == VPB_OK;
   }
 
@@ -89,9 +94,24 @@ public:
   // D2H+H2D round trip in the reference).  SceneSeg: class id {0,1,2}; DomainSeg: {0,1}; nullptr for depth.
   const uint8_t * getClassMap() const { return ran_ ? out_.cls_host : nullptr; }
 
+  // Extension (constructed with source_outputs = true): the result at the input image's rows x cols, host memory owned
+  // by the backend and valid until the next doInference.  getSourceMask: SceneSeg / DomainSeg mask 255 / 0 (the
+  // argmax / > 0 rule, run_model_node.cpp:148-172), EgoLanes ids {0,1,2,255}, INTER_NEAREST; getSourceDepth: Scene3D
+  // depth, INTER_LINEAR.  nullptr when that output was not requested or before the first inference.
+  const uint8_t * getSourceMask() const
+  {
+    return ran_ && source_kind_ == VP_SRC_MASK ? static_cast<const uint8_t *>(src_.host) : nullptr;
+  }
+  const float * getSourceDepth() const
+  {
+    return ran_ && source_kind_ == VP_SRC_DEPTH ? static_cast<const float *>(src_.host) : nullptr;
+  }
+
 private:
   vp_engine * engine_{nullptr};
   vp_output out_{};
+  int source_kind_{0};
+  vp_source_output src_{};
   bool ran_{false};
 };
 

@@ -65,6 +65,18 @@ def frame_descs(descs) -> "C.Array":
     return arr
 
 
+SRC_MASK255, SRC_IDS, SRC_DEPTH, SRC_OVERLAY = 0, 1, 2, 3
+VIZ_SCENE, VIZ_DOMAIN, VIZ_EGOLANES = 0, 1, 2
+
+
+class SrcJob(C.Structure):
+    """Mirror of vpb_src_job (include/vp_b200_ops.h): one output image of vpb_source_outputs."""
+
+    _fields_ = [("kind", C.c_int), ("src", C.c_void_p), ("sh", C.c_int), ("sw", C.c_int), ("viz_type", C.c_int),
+                ("frame", C.c_void_p), ("frame_stride", C.c_int), ("dst", C.c_void_p), ("dh", C.c_int),
+                ("dw", C.c_int), ("dst_pitch", C.c_int)]
+
+
 class LateralState(C.Structure):
     """Mirror of vpb_lateral_state (device-resident, persistent)."""
 

@@ -774,7 +774,7 @@ static int as_enqueue(vp_autospeed& e, const Frames& f, const PreGeom* g, const 
   if (rc) return rc;
   return e.frame_graph.run(
       e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return as_launch_all(e, f.data(), st); },
-      [&](cudaGraphExec_t x, cudaGraphNode_t n) {
+      [&](cudaGraphExec_t x, cudaGraphNode_t n, cudaGraphNode_t) {
         return e.pre.update_graph_node(x, n, f.data(), VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
       });
 }

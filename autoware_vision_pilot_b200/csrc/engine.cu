@@ -48,6 +48,15 @@ struct ModelOut {
   bool has_cls = false;
 };
 
+// One source-resolution output (vp_engine_config.source_outputs): model, sample, VP_SRC_* flag and its job for
+// vpb_source_outputs.  src, sh, sw, kind and viz_type are fixed at create; dst, the size, the pitch and the frame are
+// those of the current call.  The device / pinned host buffers are sized to the sample's frame and only grow.
+struct SrcOut {
+  int model = 0, sample = 0, flag = 0;
+  vpb_src_job job{};
+  void* d = nullptr; void* h = nullptr; size_t cap = 0;
+};
+
 struct Prefixes { std::string enc, ctx, neck, head; };
 static Prefixes prefixes_for(int kind) {
   switch (kind) {
@@ -98,6 +107,11 @@ struct vp_engine : EngineRuntime {
   std::vector<cudaEvent_t> op_events;      // [op], only for ops some lane waits on
   cudaEvent_t ev_pre = nullptr;
   std::vector<cudaEvent_t> lane_done;
+  // source-resolution outputs: one entry per (model, sample, flag); src_jobs is the job table of the current call
+  std::vector<SrcOut> src_outs;
+  std::vector<vpb_src_job> src_jobs;
+  bool src_ready = false;                  // a call has run (vp_engine_source_output answers)
+  bool src_host = false;                   // the last call was a host call: the pinned copies are current
 
   ~vp_engine() {
     DeviceGuard guard(gpu_id);
@@ -612,6 +626,7 @@ static int launch_all(vp_engine& e, const vpb_frame* frames, cudaStream_t st) {
   std::vector<char> started(nl, 0);
   for (size_t i = 0; i < e.ops.size(); ++i) {
     auto& op = e.ops[i];
+    if (op.lane < 0) continue;               // after the join
     cudaStream_t s = op.lane == 0 ? st : e.lane_streams[op.lane];
     if (op.lane > 0 && !started[op.lane]) {   // fork: wait for the producer of this lane's input
       const int dep = e.lane_dep[op.lane];
@@ -626,6 +641,11 @@ static int launch_all(vp_engine& e, const vpb_frame* frames, cudaStream_t st) {
     if (!started[l]) continue;
     VPB_CUDA_OK(cudaEventRecord(e.lane_done[l], e.lane_streams[l]));
     VPB_CUDA_OK(cudaStreamWaitEvent(st, e.lane_done[l], 0));
+  }
+  for (auto& op : e.ops) {
+    if (op.lane >= 0) continue;
+    rc = op.launch(st);
+    if (rc) return rc;
   }
   return VPB_OK;
 }
@@ -642,17 +662,113 @@ static int engine_geoms(const vp_engine& e, const vpb_frame* frames, const char*
   return VPB_OK;
 }
 
+// The source-output jobs of frames f: sample k's buffers grown to its frame (outside any capture; a grown buffer drops
+// the captured graph, whose node holds the old pointer), destinations, sizes and frame pointers of this call.
+static int prepare_source(vp_engine& e, const Frames& f) {
+  for (auto& so : e.src_outs) {
+    const vpb_frame& fr = f[so.sample];
+    vpb_src_job& j = so.job;
+    const int el = j.kind == VPB_SRC_DEPTH ? 4 : j.kind == VPB_SRC_OVERLAY ? 3 : 1;
+    const size_t bytes = static_cast<size_t>(fr.h) * fr.w * el;
+    if (bytes > so.cap) {
+      e.frame_graph.invalidate();
+      void* d = nullptr; void* h = nullptr;
+      VPB_CUDA_OK(cudaMalloc(&d, bytes));
+      e.dev_allocs.push_back(d);
+      VPB_CUDA_OK(cudaMallocHost(&h, bytes));
+      e.host_allocs.push_back(h);
+      so.d = d; so.h = h; so.cap = bytes;
+    }
+    j.dst = so.d; j.dh = fr.h; j.dw = fr.w; j.dst_pitch = fr.w * el;
+    j.frame = j.kind == VPB_SRC_OVERLAY ? fr.data : nullptr;
+    j.frame_stride = j.kind == VPB_SRC_OVERLAY ? fr.stride : 0;
+  }
+  e.src_jobs.clear();
+  for (const auto& so : e.src_outs) e.src_jobs.push_back(so.job);
+  e.ops.back().bytes = source_outputs_bytes(e.src_jobs.data(), static_cast<int>(e.src_jobs.size()));
+  return VPB_OK;
+}
+
 // Enqueue one call's kernels for the e.batch frames f[0 .. batch-1] (graph replay when enabled and the geometries are
 // unchanged).
 static int enqueue_frames(vp_engine& e, const Frames& f, const PreGeom* g) {
   int rc = e.pre.configure(g, e.batch, e.cfg.resize_mode);
   if (rc) return rc;
-  if (!e.cfg.use_graph) return launch_all(e, f.data(), e.stream);
-  return e.frame_graph.run(
-      e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return launch_all(e, f.data(), st); },
-      [&](cudaGraphExec_t x, cudaGraphNode_t n) {
-        return e.pre.update_graph_node(x, n, f.data(), e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
-      });
+  if (!e.src_outs.empty()) {
+    rc = prepare_source(e, f);
+    if (rc) return rc;
+  }
+  if (!e.cfg.use_graph) rc = launch_all(e, f.data(), e.stream);
+  else
+    rc = e.frame_graph.run(
+        e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return launch_all(e, f.data(), st); },
+        [&](cudaGraphExec_t x, cudaGraphNode_t pre, cudaGraphNode_t post) {
+          const int r = e.pre.update_graph_node(x, pre, f.data(), e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
+          if (r || !post) return r;
+          return source_outputs_update_node(x, post, e.src_jobs.data(), static_cast<int>(e.src_jobs.size()));
+        });
+  if (rc == VPB_OK) e.src_ready = true;
+  return rc;
+}
+
+// VP_SRC_* flags -> the source-output jobs of every model and sample, and their launch after the lanes' join
+static int build_source_outputs(vp_engine& e) {
+  static const int kFlags[3] = {VP_SRC_MASK, VP_SRC_DEPTH, VP_SRC_OVERLAY};
+  for (int m = 0; m < static_cast<int>(e.outs.size()); ++m) {
+    const ModelOut& mo = e.outs[m];
+    const size_t plane = static_cast<size_t>(mo.H) * mo.W;
+    for (int k = 0; k < e.batch; ++k)
+      for (int flag : kFlags) {
+        if (!(e.cfg.source_outputs & flag)) continue;
+        SrcOut so;
+        so.model = m; so.sample = k; so.flag = flag;
+        vpb_src_job& j = so.job;
+        j.sh = mo.H; j.sw = mo.W;
+        if (mo.kind == VP_SCENE_3D) {
+          if (flag != VP_SRC_DEPTH) continue;
+          if (mo.C != 1) { vpb_set_error("vp_engine_create: depth output with %d channels", mo.C); return VPB_ERR_STATE; }
+          j.kind = VPB_SRC_DEPTH; j.src = mo.d_raw + plane * k;
+        } else {
+          if (flag == VP_SRC_DEPTH || !mo.d_cls) continue;
+          j.src = mo.d_cls + plane * k;
+          j.kind = flag == VP_SRC_OVERLAY ? VPB_SRC_OVERLAY : mo.kind == VP_EGO_LANES ? VPB_SRC_IDS : VPB_SRC_MASK255;
+          j.viz_type = mo.kind == VP_EGO_LANES ? VPB_VIZ_EGOLANES : mo.kind == VP_DOMAIN_SEG ? VPB_VIZ_DOMAIN : VPB_VIZ_SCENE;
+        }
+        e.src_outs.push_back(so);
+      }
+  }
+  if (e.src_outs.empty()) return VPB_OK;
+  const int rc = viz_tables_init();
+  if (rc) return rc;
+  vp_engine* ep = &e;
+  OpRec op;
+  op.name = "source_outputs"; op.kname = "source_outputs_kernel"; op.lane = -1;
+  op.launch = [ep](cudaStream_t st) { return source_outputs_x(ep->src_jobs.data(), static_cast<int>(ep->src_jobs.size()), st); };
+  e.ops.push_back(std::move(op));
+  e.frame_graph.has_post = true;
+  return VPB_OK;
+}
+
+// A flag outside VP_SRC_* or one no model of the engine makes: VPB_ERR_ARG (host-only, before the device is opened)
+static int check_source_flags(const vp_engine_config& c) {
+  const int all = VP_SRC_MASK | VP_SRC_DEPTH | VP_SRC_OVERLAY;
+  if (c.source_outputs & ~all) {
+    vpb_set_error("vp_engine_create: source_outputs 0x%x has bits outside VP_SRC_MASK | VP_SRC_DEPTH | VP_SRC_OVERLAY",
+                  c.source_outputs);
+    return VPB_ERR_ARG;
+  }
+  int can = 0;
+  for (int i = 0; i < c.n_models; ++i) {
+    const int k = c.kinds[i];
+    if (k == VP_SCENE_3D) can |= VP_SRC_DEPTH;
+    else if (k == VP_SCENE_SEG || k == VP_DOMAIN_SEG || k == VP_EGO_LANES) can |= VP_SRC_MASK | VP_SRC_OVERLAY;
+  }
+  if (c.source_outputs & ~can) {
+    vpb_set_error("vp_engine_create: source_outputs 0x%x: no model of this engine makes 0x%x (depth: Scene3D; mask, "
+                  "overlay: SceneSeg, DomainSeg, EgoLanes)", c.source_outputs, c.source_outputs & ~can);
+    return VPB_ERR_ARG;
+  }
+  return VPB_OK;
 }
 
 }  // namespace vpb
@@ -666,8 +782,10 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
     return VPB_ERR_ARG;
   }
   *out = nullptr;
+  int rc = check_source_flags(*cfg);
+  if (rc) return rc;
   std::unique_ptr<vp_engine> e(new vp_engine());
-  int rc = e->open("vp_engine_create", cfg->gpu_id, cfg->stream);
+  rc = e->open("vp_engine_create", cfg->gpu_id, cfg->stream);
   if (rc) return rc;
   DeviceGuard guard(cfg->gpu_id);
   e->cfg = *cfg;
@@ -709,6 +827,8 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
     if (rc) return rc;
   }
   if (e->oom) return VPB_ERR_CUDA;
+  rc = build_source_outputs(*e);
+  if (rc) return rc;
   VPB_CUDA_OK(cudaDeviceSynchronize());
   *out = e.release();
   return VPB_OK;
@@ -735,6 +855,7 @@ static int infer_device_frames(vp_engine* e, const Frames& f, int n, const char*
   PreGeom g[kMaxBatch];
   if (engine_geoms(*e, f.data(), who, g)) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
+  e->src_host = false;
   return enqueue_frames(*e, f, g);
 }
 
@@ -779,6 +900,9 @@ static int submit_host_frames(vp_engine* e, const vpb_frame* frames, int n, bool
     if (e->cfg.fetch_raw || !mo.has_cls || mo.kind == VP_EGO_LANES)
       VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4 * n, cudaMemcpyDeviceToHost, e->stream));
   }
+  for (const auto& so : e->src_outs)
+    VPB_CUDA_OK(cudaMemcpyAsync(so.h, so.d, static_cast<size_t>(so.job.dh) * so.job.dst_pitch, cudaMemcpyDeviceToHost, e->stream));
+  e->src_host = true;
   if (sync) VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   return VPB_OK;
 }
@@ -838,6 +962,27 @@ extern "C" int vp_engine_output_at(vp_engine* e, int idx, int sample, vp_output*
 }
 
 extern "C" int vp_engine_output(vp_engine* e, int idx, vp_output* o) { return vp_engine_output_at(e, idx, 0, o); }
+
+extern "C" int vp_engine_source_output(vp_engine* e, int idx, int sample, int kind, vp_source_output* o) {
+  const char* who = "vp_engine_source_output";
+  if (!e || !o || idx < 0 || idx >= static_cast<int>(e->outs.size())) { vpb_set_error("%s: bad model index", who); return VPB_ERR_ARG; }
+  if (sample < 0 || sample >= e->batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch); return VPB_ERR_ARG; }
+  const SrcOut* so = nullptr;
+  for (const auto& x : e->src_outs)
+    if (x.model == idx && x.sample == sample && x.flag == kind) { so = &x; break; }
+  if (!so) {
+    vpb_set_error("%s: model %d has no source output of kind %d (not requested, or not made by this model)", who, idx, kind);
+    return VPB_ERR_ARG;
+  }
+  if (!e->src_ready) { vpb_set_error("%s: run one call first", who); return VPB_ERR_STATE; }
+  const vpb_src_job& j = so->job;
+  o->kind = kind; o->height = j.dh; o->width = j.dw; o->pitch = j.dst_pitch;
+  o->channels = j.kind == VPB_SRC_OVERLAY ? 3 : 1;
+  o->is_f32 = j.kind == VPB_SRC_DEPTH;
+  o->host = e->src_host ? so->h : nullptr;
+  o->dev = so->d;
+  return VPB_OK;
+}
 
 extern "C" int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s) {
   if (!e || !s) return VPB_ERR_ARG;

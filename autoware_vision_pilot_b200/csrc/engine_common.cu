@@ -109,19 +109,19 @@ static bool same_geometry(const vpb_frame& a, const vpb_frame& b) { return a.h =
 
 int FrameGraph::run(cudaStream_t st, const PreprocessPlan& pre, int dtype, const Frames& f, int n_,
                     const std::function<int(cudaStream_t)>& launch,
-                    const std::function<int(cudaGraphExec_t, cudaGraphNode_t)>& repoint) {
+                    const std::function<int(cudaGraphExec_t, cudaGraphNode_t, cudaGraphNode_t)>& repoint) {
   bool same_geom = exec && n == n_, same_src = n == n_;
   for (int k = 0; k < n_ && same_geom; ++k) same_geom = same_geometry(frames[k], f[k]);
   for (int k = 0; k < n_ && same_src; ++k) same_src = frames[k].data == f[k].data;
-  if (same_geom && !same_src && pre_node) {
-    const int rc = repoint(exec, pre_node);
+  if (same_geom && !same_src && pre_node && (!has_post || post_node)) {
+    const int rc = repoint(exec, pre_node, post_node);
     if (rc) return rc;
     frames = f;
     same_src = true;
   }
   if (!same_geom || !same_src) {
     invalidate();
-    pre_node = nullptr;
+    pre_node = post_node = nullptr;
     n = 0;
     int rc = launch(st);
     if (rc) return rc;
@@ -140,10 +140,9 @@ int FrameGraph::run(cudaStream_t st, const PreprocessPlan& pre, int dtype, const
       cudaGraphNodeType ty;
       if (cudaGraphNodeGetType(nodes[i], &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
       cudaKernelNodeParams kp{};
-      if (cudaGraphKernelNodeGetParams(nodes[i], &kp) == cudaSuccess && pre.owns_kernel(kp.func, dtype)) {
-        pre_node = nodes[i];
-        break;
-      }
+      if (cudaGraphKernelNodeGetParams(nodes[i], &kp) != cudaSuccess) continue;
+      if (!pre_node && pre.owns_kernel(kp.func, dtype)) pre_node = nodes[i];
+      else if (has_post && !post_node && source_outputs_owns(kp.func)) post_node = nodes[i];
     }
     ce = cudaGraphInstantiate(&exec, g, 0);
     if (graph) cudaGraphDestroy(graph);

@@ -65,27 +65,32 @@ struct OpRec {
   std::string kname;    // kernel the op launches (roofline report groups launches by kernel)
   bool gemm = false;
   int kind = 0;   // 0 = not a convolution GEMM; conv_wgmma_kernel with 1 = VPB_ALGO_TILE, 2 = VPB_ALGO_LINEAR
-  int lane = 0;   // execution lane (= index of the model that owns the op); lanes run concurrently
+  int lane = 0;   // execution lane (= index of the model that owns the op); lanes run concurrently; -1: after every
+                  // lane has joined the engine stream
 };
 
 // The frames of one call: descriptor k is sample k (entries past the batch are unused).
 using Frames = std::array<vpb_frame, kMaxBatch>;
 
 // The CUDA graph of one call, keyed on the n (h, w, stride) triples and the frame pointers.  Frames of the captured
-// geometries in other buffers only re-point the captured pre-process node.
+// geometries in other buffers only re-point the captured kernel nodes that read the frames: the pre-process, and the
+// source-output launch when the engine has one.
 struct FrameGraph {
-  cudaGraph_t graph = nullptr;           // kept alive: pre_node is a handle into it
+  cudaGraph_t graph = nullptr;           // kept alive: pre_node / post_node are handles into it
   cudaGraphExec_t exec = nullptr;
   cudaGraphNode_t pre_node = nullptr;    // the captured pre-process kernel node (re-pointed per call)
+  cudaGraphNode_t post_node = nullptr;   // the captured source_outputs_kernel node (re-pointed per call), if any
+  bool has_post = false;                 // the launch list ends with a source-output launch (set by the engine)
   int n = 0;                             // frames of the captured / last call (0: none yet)
   Frames frames{};
 
   // Launch the graph for frames f[0 .. n_-1] on st.  When the key differs in more than the frame pointers: launch(st)
-  // once outside capture (sets function attributes; its results are correct), capture launch(st), find the node of
-  // `pre` and instantiate.  When only the pointers differ: repoint(exec, pre_node).
+  // once outside capture (sets function attributes; its results are correct), capture launch(st), find the nodes of
+  // `pre` (and of the source outputs when has_post) and instantiate.  When only the pointers differ:
+  // repoint(exec, pre_node, post_node); post_node is NULL without source outputs.
   int run(cudaStream_t st, const PreprocessPlan& pre, int dtype, const Frames& f, int n_,
           const std::function<int(cudaStream_t)>& launch,
-          const std::function<int(cudaGraphExec_t, cudaGraphNode_t)>& repoint);
+          const std::function<int(cudaGraphExec_t, cudaGraphNode_t, cudaGraphNode_t)>& repoint);
   void invalidate();                     // the next run() captures again
   void release();
 };

@@ -11,6 +11,7 @@ namespace vpb {
 static constexpr int kNetH = 320, kNetW = 640;   // the only network input size (scene_seg_infer.py:40-42)
 static constexpr int kGapReplicas = 8;           // copies of each SE pooling accumulator (atomic spreading)
 static constexpr int kMaxBatch = 8;              // VP_MAX_BATCH (vp_b200.h): frames per engine call
+static constexpr int kMaxSrcJobs = 64;           // vpb_source_outputs: 8 samples x 4 models x 2 outputs
 
 void resize_tables_host(int mode, int in_size, int out_size, std::vector<int>& bounds,
                         std::vector<int>& coeffs, int& ksize);
@@ -81,6 +82,15 @@ int fuse_pool_x(int dtype, const void* f0, const void* f1, const void* f2, const
 // vpb_final_tapsum (conv_gemm.cu)
 int final_tapsum_x(const float* P, const float* bias, int Cout, int H, int W, int final_kind, float* out, uint8_t* cls,
                    cudaStream_t st, int batch = 1);
+// vpb_source_outputs (post_ops.cu).  source_outputs_owns: func is source_outputs_kernel (finds the captured node);
+// source_outputs_update_node re-points that node at another job table; source_outputs_bytes: algorithmic HBM bytes of
+// one launch (each distinct source map read once, frames read, outputs written); viz_tables_init uploads the palettes
+// once per device (not during a stream capture).
+int source_outputs_x(const vpb_src_job* jobs, int n, cudaStream_t st);
+bool source_outputs_owns(const void* func);
+int source_outputs_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_src_job* jobs, int n);
+double source_outputs_bytes(const vpb_src_job* jobs, int n);
+int viz_tables_init();
 
 // One-time per-DEVICE initialisation (function attributes, constant tables): engines for several GPUs may
 // live in one process, and entry points may be called from several threads.

@@ -16,19 +16,38 @@ RESIZE_BY_NAME = {"none": RESIZE_NONE, "pil_bicubic": RESIZE_PIL_BICUBIC, "cv_li
 DTYPE_BY_NAME = {"fp16": L.VPB_F16, "bf16": L.VPB_BF16, "fp32": L.VPB_F16}
 PREC_16, PREC_SPLIT = 0, 1
 MAX_BATCH = 8   # VP_MAX_BATCH
+SRC_MASK, SRC_DEPTH, SRC_OVERLAY = 1, 2, 4   # VP_SRC_*
+SRC_BY_NAME = {"mask": SRC_MASK, "depth": SRC_DEPTH, "overlay": SRC_OVERLAY}
 
 
 class _Config(C.Structure):
     _fields_ = [("gpu_id", C.c_int), ("dtype", C.c_int), ("resize_mode", C.c_int), ("convention", C.c_int),
                 ("n_models", C.c_int), ("kinds", C.c_int * 4), ("weights", C.c_char_p * 4),
                 ("fetch_raw", C.c_int), ("use_graph", C.c_int), ("stream", C.c_void_p),
-                ("single_stream", C.c_int), ("precision", C.c_int), ("batch", C.c_int)]
+                ("single_stream", C.c_int), ("precision", C.c_int), ("batch", C.c_int), ("source_outputs", C.c_int)]
 
 
 class _Output(C.Structure):
     _fields_ = [("kind", C.c_int), ("channels", C.c_int), ("height", C.c_int), ("width", C.c_int),
                 ("raw_host", C.POINTER(C.c_float)), ("cls_host", C.POINTER(C.c_uint8)),
                 ("raw_dev", C.c_void_p), ("cls_dev", C.c_void_p)]
+
+
+class _SourceOutput(C.Structure):
+    _fields_ = [("kind", C.c_int), ("height", C.c_int), ("width", C.c_int), ("channels", C.c_int), ("pitch", C.c_int),
+                ("is_f32", C.c_int), ("host", C.c_void_p), ("dev", C.c_void_p)]
+
+
+def source_flags(names: Sequence[str]) -> int:
+    """("mask", "depth", "overlay") -> VP_SRC_* bitmask; ValueError for an unknown name."""
+    if isinstance(names, str):
+        names = (names,)
+    flags = 0
+    for n in names:
+        if n not in SRC_BY_NAME:
+            raise ValueError(f"unknown source output {n!r} (one of {sorted(SRC_BY_NAME)})")
+        flags |= SRC_BY_NAME[n]
+    return flags
 
 
 class _Stats(C.Structure):
@@ -80,6 +99,7 @@ def _bind():
     lib.vp_engine_tap_dev.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(_TapView)]
     lib.vp_engine_stream.argtypes = [C.c_void_p]
     lib.vp_engine_stream.restype = C.c_void_p
+    lib.vp_engine_source_output.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_SourceOutput)]
     _bound = True
     return lib
 
@@ -90,11 +110,13 @@ class Engine:
     def __init__(self, kinds: Sequence[int], weights: Sequence[str], *, gpu_id: int = 0, dtype: str = "fp16",
                  resize_mode: int = RESIZE_NONE, convention: int = CONV_RGB, fetch_raw: bool = True,
                  use_graph: bool = True, stream: Optional[int] = None, single_stream: bool = False,
-                 precision: Optional[int] = None, batch: int = 1):
+                 precision: Optional[int] = None, batch: int = 1, source_outputs: Sequence[str] = ()):
         """dtype "fp16" | "bf16": 16-bit operands; dtype "fp32" (the reference's precision="fp32") selects the
         split-fp16 fp32-grade mode (precision=PREC_SPLIT on fp16 pairs).  batch > 1 (16-bit only): every call takes
         exactly `batch` frames, of one geometry (infer_batch / submit_batch / infer_device_batch) or each of its own
-        size (infer_frames / submit_frames / infer_device_frames); sample k's outputs are raw(idx, k) / cls(idx, k)."""
+        size (infer_frames / submit_frames / infer_device_frames); sample k's outputs are raw(idx, k) / cls(idx, k).
+        source_outputs: any of "mask", "depth", "overlay": every call also makes these results at each camera's own
+        resolution (source(idx, kind, k) / source_dev(idx, kind, k)); a kind no model makes is rejected."""
         self._lib = _bind()
         cfg = _Config()
         cfg.gpu_id, cfg.dtype = gpu_id, DTYPE_BY_NAME[dtype]
@@ -108,6 +130,7 @@ class Engine:
         cfg.single_stream = int(single_stream)
         cfg.precision = (PREC_SPLIT if dtype == "fp32" else PREC_16) if precision is None else precision
         cfg.batch = batch
+        cfg.source_outputs = source_flags(source_outputs)
         self._h = C.c_void_p()
         L.check(self._lib.vp_engine_create(C.byref(cfg), C.byref(self._h)), "vp_engine_create")
         self.kinds = list(kinds)
@@ -269,6 +292,31 @@ class Engine:
     def out_dev(self, idx: int, sample: int = 0):
         o = self._out(idx, sample)
         return o.raw_dev, o.cls_dev, (o.channels, o.height, o.width)
+
+    def _source(self, idx: int, kind: str, sample: int) -> _SourceOutput:
+        o = _SourceOutput()
+        L.check(self._lib.vp_engine_source_output(self._h, idx, sample, source_flags(kind), C.byref(o)),
+                "vp_engine_source_output")
+        return o
+
+    def source(self, idx: int, kind: str, sample: int = 0) -> np.ndarray:
+        """Model idx's `kind` ("mask" | "depth" | "overlay") output of sample `sample` at that camera's resolution after
+        a host call: [h, w] uint8 / float32 or [h, w, 3] uint8, a view into an engine-owned buffer (copy it to keep it
+        past the next call).  After a device call the result is on the device only (source_dev)."""
+        o = self._source(idx, kind, sample)
+        if not o.host:
+            raise RuntimeError(f"source output {kind!r} of model {idx}: the last call was a device call, use source_dev()")
+        dt = np.float32 if o.is_f32 else np.uint8
+        a = np.ctypeslib.as_array(C.cast(o.host, C.POINTER(C.c_uint8)), shape=(o.height * o.pitch,))
+        a = a.view(dt).reshape(o.height, o.pitch // np.dtype(dt).itemsize)
+        a = a[:, :o.width * o.channels]
+        return a.reshape(o.height, o.width, 3) if o.channels == 3 else a
+
+    def source_dev(self, idx: int, kind: str, sample: int = 0) -> dict:
+        """Device view of a source output: {data, height, width, channels, pitch (bytes), dtype ("uint8" | "float32")}."""
+        o = self._source(idx, kind, sample)
+        return {"data": o.dev, "height": o.height, "width": o.width, "channels": o.channels, "pitch": o.pitch,
+                "dtype": "float32" if o.is_f32 else "uint8"}
 
     # ---- introspection
     def stats(self) -> dict:

@@ -75,7 +75,19 @@ typedef struct {
   int batch;                        /* frames per call: 0 or 1 = one frame (vp_engine_infer ...); 2..VP_MAX_BATCH =
                                        the *_batch entry points with exactly `batch` frames (16-bit mode only:
                                        VP_PREC_SPLIT with batch > 1 fails with VPB_ERR_ARG) */
+  int source_outputs;               /* 0 (default) or VP_SRC_* flags: results at each camera's own resolution, made in
+                                       the same call (vp_engine_source_output) */
 } vp_engine_config;
+
+/* Source-resolution outputs (vp_engine_config.source_outputs), what each model makes of a flag:
+ *   VP_SRC_MASK     SceneSeg / DomainSeg: uint8 mask 255 / 0 (createMaskKernel's rule); EgoLanes: uint8 ids {0,1,2,255}
+ *                   (createEgoLanesMaskKernel) — both cv::resize INTER_NEAREST to the frame (run_model_node.cpp:148-177)
+ *   VP_SRC_DEPTH    Scene3D: fp32 depth, cv::resize INTER_LINEAR (run_model_node.cpp:96-104)
+ *   VP_SRC_OVERLAY  SceneSeg / DomainSeg / EgoLanes: the mask's colours blended half/half onto the frame, uint8 [h][w][3]
+ *                   (MasksVisualizationEngine::visualize, masks_visualization_engine.cpp:11-38)
+ * Every output of a call is made by ONE launch (vpb_source_outputs) after the networks, inside the frame graph.  A flag
+ * no model of the engine can produce fails vp_engine_create with VPB_ERR_ARG. */
+enum { VP_SRC_MASK = 1, VP_SRC_DEPTH = 2, VP_SRC_OVERLAY = 4 };
 
 typedef struct {
   int kind;
@@ -120,7 +132,8 @@ int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev,
  * VPB_RESIZE_NONE, or a frame whose Pillow filter needs more than 32 taps.  Host frames are copied with pitch
  * 3*w_k each (w_k*3 bytes read per row); vp_engine_submit_frames reads them asynchronously, so give it pinned
  * memory.  The *_batch calls are the case of n equal descriptors.  The frame graph is keyed on the n (h, w,
- * stride) triples: new pointers only re-point the captured pre-process node, a new geometry captures again. */
+ * stride) triples: new pointers only re-point the captured pre-process node (and the source-output node), a new
+ * geometry captures again. */
 int vp_engine_infer_frames(vp_engine* e, const vpb_frame* frames_host, int n);
 int vp_engine_submit_frames(vp_engine* e, const vpb_frame* frames_host, int n);
 int vp_engine_infer_device_frames(vp_engine* e, const vpb_frame* frames_dev, int n);
@@ -132,6 +145,20 @@ int vp_engine_output(vp_engine* e, int model_idx, vp_output* out);
  * and [batch][H][W] uint8, and the pointers returned address sample `sample`.  vp_engine_output is sample 0. */
 int vp_engine_output_at(vp_engine* e, int model_idx, int sample, vp_output* out);
 int vp_engine_num_models(const vp_engine* e);
+
+/* One source-resolution output of sample `sample` of the last call: kind VP_SRC_MASK | VP_SRC_DEPTH | VP_SRC_OVERLAY,
+ * height x width = that sample's frame size, channels 1 or 3, pitch = bytes per row, is_f32 (depth) or uint8.  host: an
+ * engine-owned pinned copy made by the host calls (vp_engine_infer*, vp_engine_submit*: valid after the call / its
+ * vp_engine_sync), NULL after a device call; dev: the device buffer.  Both stay valid until the next call.
+ * VPB_ERR_ARG for a bad model index or sample, or a kind not requested or not made by that model; VPB_ERR_STATE before
+ * the first call. */
+typedef struct {
+  int kind, height, width, channels, pitch;
+  int is_f32;
+  const void* host;
+  const void* dev;
+} vp_source_output;
+int vp_engine_source_output(vp_engine* e, int model_idx, int sample, int kind, vp_source_output* out);
 
 /* A pinned host buffer owned by the engine that a caller may fill directly (capture threads):
  * vp_engine_infer recognises the pointer and skips the staging copy. */

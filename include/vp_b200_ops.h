@@ -274,6 +274,28 @@ int vpb_resize_linear_f32(const float* src, int sh, int sw, float* dst, int dh, 
 enum { VPB_VIZ_SCENE = 0, VPB_VIZ_DOMAIN = 1, VPB_VIZ_EGOLANES = 2 };
 int vpb_visualize_mask(const uint8_t* mask, int mh, int mw, int viz_type, const uint8_t* frame_bgr, int h,
                        int w, int stride, uint8_t* out, int out_stride, void* stream);
+/* All source-resolution outputs of a call in ONE launch (source_outputs_kernel): every job is one output image at a
+ * camera's own size h x w, made from a network-resolution map, with the arithmetic of the single ops above:
+ *   VPB_SRC_MASK255  uint8 class map (VPB_FINAL_ARGMAX / _THRESH) -> class 1 ? 255 : 0, INTER_NEAREST  == vpb_mask255 on
+ *                    the raw tensor (finite logits), then vpb_resize_nearest_u8
+ *   VPB_SRC_IDS      EgoLanes class map (ids {0,1,2,255}) -> ids, INTER_NEAREST  == vpb_egolanes_ids, then
+ *                    vpb_resize_nearest_u8
+ *   VPB_SRC_DEPTH    fp32 map -> fp32, INTER_LINEAR  == vpb_resize_linear_f32
+ *   VPB_SRC_OVERLAY  class map + the camera frame [dh][dw][3] -> uint8 [dh][dw][3]  == the mask rule of the model
+ *                    (SCENE / DOMAIN: MASK255, EGOLANES: IDS), then vpb_visualize_mask with palette viz_type
+ * Pitches and strides are in bytes.  frame / frame_stride / viz_type are read for OVERLAY only.  VPB_ERR_ARG before any
+ * device work, the message naming the job, for n outside 1..64, a NULL pointer, a non-positive size (or dh > 65535),
+ * an unknown kind or viz_type, frame_stride < 3*dw, a pitch smaller than one row, or (DEPTH) fp32 buffers or a pitch
+ * that are not 4-byte aligned. */
+enum { VPB_SRC_MASK255 = 0, VPB_SRC_IDS = 1, VPB_SRC_DEPTH = 2, VPB_SRC_OVERLAY = 3 };
+typedef struct {
+  int kind;                         /* VPB_SRC_* */
+  const void* src; int sh, sw;      /* class map uint8 [sh][sw] (MASK255 / IDS / OVERLAY) or fp32 [sh][sw] (DEPTH) */
+  int viz_type;                     /* OVERLAY: VPB_VIZ_SCENE | _DOMAIN | _EGOLANES */
+  const uint8_t* frame; int frame_stride;   /* OVERLAY: the camera frame [dh][dw][3], stride in bytes */
+  void* dst; int dh, dw, dst_pitch; /* pitch in bytes */
+} vpb_src_job;
+int vpb_source_outputs(const vpb_src_job* jobs, int n, void* stream);
 /* Lane poly-fit least squares, fp64, one warp per point set (set i = points offsets[i]..offsets[i+1]):
  * x = c0*y^order + ... (highest power first), order 1..3 ->  coeffs[set][4] (unused slots 0; NaN if the
  * set has <= order points), yrange[set][2] = (min_y, max_y) (may be NULL).

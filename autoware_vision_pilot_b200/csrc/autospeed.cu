@@ -382,34 +382,9 @@ struct vp_autospeed : EngineRuntime {
   float conf = 0.6f, iou = 0.45f;
   static constexpr int kMaxCand = 4096, kMaxDet = 1024;
 
-  Tens talloc(int H, int W, int C) {
-    Tens t; t.H = H; t.W = W; t.C = C; t.ld = C;
-    t.p = dalloc(static_cast<size_t>(H) * W * C * 2 * batch);
-    return t;
-  }
-  // flops: per sample (counted for the whole batch)
-  void op(const std::string& name, std::function<int(cudaStream_t)> fn, double flops = 0) {
-    OpRec r; r.name = name; r.launch = std::move(fn); r.flops = flops * batch;
-    ops.push_back(std::move(r));
-  }
-
-  // one wgmma convolution: in (slice) -> out (slice); w [taps][Cout][Cin] 16-bit (or an activation slice with ldw,
-  // w_img elements apart per sample)
-  int conv(const std::string& name, const Tens& in, const Tens& out, int Cout, int taps, int stride, const void* w,
-           const float* bias, int act, int mode = VPB_EPI_STORE, const Tens* res = nullptr, int act2 = ACT_NONE,
-           int ldw = 0, int w_img = 0) {
-    vpb_conv_args a{};
-    a.batch = batch; a.w_img = w_img;
-    a.dtype = dtype; a.H = out.H; a.W = out.W; a.Cin = in.C; a.ldi = in.ld;
-    a.Cout = Cout; a.taps = taps; a.phases = 1; a.act = act; a.mode = mode;
-    a.in = in.p; a.w = w; a.bias = bias;
-    a.out = out.p; a.ldo = out.ld; a.out_slice = 1;
-    if (res) { a.res = res->p; a.ldr = res->ld; }
-    a.algo = VPB_ALGO_TILE;
-    a.stride = stride; a.in_h = in.H; a.in_w = in.W;
-    a.act2 = act2; a.ldw = ldw;
-    return append_conv(name, a);
-  }
+  int geoms(const vpb_frame* frames, const char* who, PreGeom* g) override;
+  int enqueue(const Frames& f, const PreGeom* g) override;
+  int fetch(bool raw) override;
 };
 
 namespace vpb {
@@ -419,6 +394,14 @@ struct ASBuilder {
   const WeightMap& w;
   int rc = VPB_OK;
   bool ok() const { return rc == VPB_OK && !e.oom; }
+
+  // vpb_conv_args of one wgmma convolution in -> out, a channel slice; H x W is the output's size (stride 1 or 2)
+  vpb_conv_args conv(const Tens& in, const Tens& out, int cout, int taps, int stride, const void* wt, const float* bias,
+                     int act, int mode, const Tens* res) const {
+    vpb_conv_args a = e.conv_args(in, &out, res, cout, taps, 1, wt, bias, act, mode);
+    a.H = out.H; a.W = out.W; a.stride = stride; a.in_h = in.H; a.in_w = in.W; a.out_slice = 1;
+    return a;
+  }
 
   // Conv = Conv2d(bias=False) + BatchNorm2d(eps 1e-3) [+ SiLU] (common_layers.py:5-17), folded
   bool fold(const std::string& p, int cout, int cin_per_g, int k, std::vector<float>& wt, std::vector<float>& bias,
@@ -454,7 +437,7 @@ struct ASBuilder {
     std::vector<float> wt, bias;
     if (!fold(p, cout, cin, k, wt, bias, false)) return;
     if (cin_pad) wt = pad_cin(wt, k * k, cout, cin, cin_pad);
-    rc = e.conv(p, in, out, cout, k * k, stride, e.upload_16(wt), e.upload_f32(bias), act ? ACT_SILU : ACT_NONE, mode, res);
+    rc = e.append_conv(p, conv(in, out, cout, k * k, stride, e.upload_16(wt), e.upload_f32(bias), act ? ACT_SILU : ACT_NONE, mode, res));
   }
   // plain nn.Conv2d with bias (CTX convs, head output convs)
   void plain(const std::string& p, const Tens& in, const Tens& out, int cout, int k, int act, int mode = VPB_EPI_STORE,
@@ -463,7 +446,9 @@ struct ASBuilder {
     const HostTensor* cw = find_w_shaped(w, p + ".weight", {cout, in.C, k, k});
     const HostTensor* cb = find_w_shaped(w, p + ".bias", {cout});
     if (!cw || !cb) { rc = VPB_ERR_IO; return; }
-    rc = e.conv(p, in, out, cout, k * k, 1, e.upload_16(pack_conv(*cw, nullptr)), e.upload_f32(cb->f), act, mode, res, act2);
+    vpb_conv_args a = conv(in, out, cout, k * k, 1, e.upload_16(pack_conv(*cw, nullptr)), e.upload_f32(cb->f), act, mode, res);
+    a.act2 = act2;
+    rc = e.append_conv(p, a);
   }
   void dw(const std::string& p, const Tens& in, const Tens& out, bool act) {
     if (!ok()) return;
@@ -472,8 +457,8 @@ struct ASBuilder {
     float *dwt = e.upload_f32(wt), *db = e.upload_f32(bias);
     const int dt = e.dtype, H = in.H, W = in.W, C = in.C, nb = e.batch;
     const void* ip = in.p; void* op_ = out.p; long long* gap = e.d_gap_scratch;
-    e.op(p, [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? VPB_ACT_SILU : VPB_ACT_NONE, nb); },
-         2.0 * H * W * C * 9);
+    e.add_op(p, "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? VPB_ACT_SILU : VPB_ACT_NONE, nb); },
+             2.0 * H * W * C * 9, nb * 4.0 * H * W * C);
   }
   // CTX (common_layers.py:194-239): x [h][w][C] -> out [h][w][Cout]
   void ctx(const std::string& p, const Tens& x, const Tens& out, int cout) {
@@ -488,12 +473,15 @@ struct ASBuilder {
     float* d_mean = static_cast<float*>(e.dalloc(static_cast<size_t>(C) * 4 * nb));
     {
       const void* ip = x.p; const int ld = x.ld;
-      e.op(p + ".mean", [=](cudaStream_t st) {
-        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? mean_part_kernel<BF16, true> : mean_part_kernel<BF16, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(ip), HW, C, ld, d_part));
-        else VPB_CUDA_OK(launch_k(nb > 1 ? mean_part_kernel<F16, true> : mean_part_kernel<F16, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const __half*>(ip), HW, C, ld, d_part));
+      // two launches; the partial sums and the means are small next to the activation read
+      e.add_op(p + ".mean", "mean_part_kernel", [=](cudaStream_t st) {
+        VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+          using E = decltype(tag);
+          return launch_k(nb > 1 ? mean_part_kernel<E, true> : mean_part_kernel<E, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const typename E::T*>(ip), HW, C, ld, d_part);
+        }));
         VPB_CUDA_OK(launch_k(nb > 1 ? mean_final_kernel<true> : mean_final_kernel<false>, dim3((C + 127) / 128, nb), dim3(128), 0, st, static_cast<const float*>(d_part), nblk, C, 1.0f / HW, d_mean));
         return VPB_OK;
-      });
+      }, 0.0, nb * 2.0 * HW * C);
     }
     // exp0: Conv1d(k=3, pad 1) on a length-1 sequence == the centre tap as a Linear(C -> h*w); SiLU twice (:218-221)
     std::vector<float> lw(static_cast<size_t>(HW) * C);
@@ -501,23 +489,23 @@ struct ASBuilder {
       for (int c = 0; c < C; ++c) lw[static_cast<size_t>(o) * C + c] = ew->f[(static_cast<size_t>(o) * C + c) * 3 + 1];
     float *d_lw = e.upload_f32(lw), *d_lb = e.upload_f32(eb->f);
     float* d_map = static_cast<float*>(e.dalloc(static_cast<size_t>(HW) * 4 * nb));
-    e.op(p + ".exp0", [=](cudaStream_t st) { return linear_x(d_mean, d_lw, d_lb, C, HW, VPB_ACT_SILU2, d_map, st, nb); },
-         2.0 * HW * C);
+    e.add_op(p + ".exp0", "linear_kernel", [=](cudaStream_t st) { return linear_x(d_mean, d_lw, d_lb, C, HW, VPB_ACT_SILU2, d_map, st, nb); },
+             2.0 * HW * C, 4.0 * HW * C);
     // ctx0: Conv2d(1 -> C/2, 3x3) + SiLU
-    Tens c2 = e.talloc(H, W, C / 2);
+    Tens c2 = e.act_alloc(H, W, C / 2);
     float *d_c0w = e.upload_f32(c0w->f), *d_c0b = e.upload_f32(c0b->f);
     {
       void* op_ = c2.p; const int co = C / 2;
-      e.op(p + ".ctx0", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, nullptr, 0, st, ACT_SILU, nb); },
-           2.0 * HW * co * 9);
+      e.add_op(p + ".ctx0", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, nullptr, 0, st, ACT_SILU, nb); },
+               2.0 * HW * co * 9, nb * 2.0 * HW * co);
     }
     // ctx1: SiLU(conv) * x + x, then SiLU (:224-232) — one wgmma conv with the MULADD epilogue and a post activation
-    Tens c4 = e.talloc(H, W, C);
+    Tens c4 = e.act_alloc(H, W, C);
     plain(p + ".ctx1", c2, c4, C, 3, ACT_SILU, VPB_EPI_MULADD, &x, ACT_SILU);
     plain(p + ".ctx2", c4, out, cout, 3, ACT_NONE);
   }
   void residual(const std::string& p, const Tens& x, const Tens& out, int mid) {   // out = x + conv2(conv1(x)); out may alias x
-    Tens t = e.talloc(x.H, x.W, mid);
+    Tens t = e.act_alloc(x.H, x.W, mid);
     cbs(p + ".conv1", x, t, mid, 3, 1, true);
     cbs(p + ".conv2", t, out, x.C, 3, 1, true, 0, VPB_EPI_ADD, &x);
   }
@@ -525,14 +513,14 @@ struct ASBuilder {
   void c3k2(const std::string& p, const Tens& in, const Tens& out, int cout, bool csp) {
     if (!ok()) return;
     const int c = cout / 2;
-    Tens cat = e.talloc(in.H, in.W, 3 * c);
+    Tens cat = e.act_alloc(in.H, in.W, 3 * c);
     cbs(p + ".conv1", in, cat.slice(0, 2 * c), 2 * c, 1, 1, true);
     Tens y1 = cat.slice(c, c), y2 = cat.slice(2 * c, c);
     if (!csp) {
       residual(p + ".res_m.0", y1, y2, c / 2);
     } else {                                                   // C3K (common_layers.py:158-173)
       const std::string q = p + ".res_m.0";
-      Tens k = e.talloc(in.H, in.W, c);                      // cat(res_m(conv1(y1)), conv2(y1))
+      Tens k = e.act_alloc(in.H, in.W, c);                      // cat(res_m(conv1(y1)), conv2(y1))
       Tens k1 = k.slice(0, c / 2);
       cbs(q + ".conv1", y1, k1, c / 2, 1, 1, true);
       cbs(q + ".conv2", y1, k.slice(c / 2, c / 2), c / 2, 1, 1, true);
@@ -546,71 +534,82 @@ struct ASBuilder {
     const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, li = in.ld / 8, lo = out.ld / 8, nb = e.batch;
     const void* ip = in.p; void* op_ = out.p;
     const long n = 4L * H * W * C8;
-    e.op(name, [=](cudaStream_t st) {
+    e.add_op(name, "upsample2_kernel", [=](cudaStream_t st) {
       const dim3 g(static_cast<unsigned>((n + 255) / 256), nb), b(256);
-      if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? upsample2_kernel<BF16, true> : upsample2_kernel<BF16, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, li, static_cast<uint4*>(op_), lo));
-      else VPB_CUDA_OK(launch_k(nb > 1 ? upsample2_kernel<F16, true> : upsample2_kernel<F16, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, li, static_cast<uint4*>(op_), lo));
+      VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+        using E = decltype(tag);
+        return launch_k(nb > 1 ? upsample2_kernel<E, true> : upsample2_kernel<E, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, li, static_cast<uint4*>(op_), lo);
+      }));
       return VPB_OK;
-    });
+    }, 0.0, nb * 80.0 * H * W * C8);
   }
   void maxpool(const std::string& name, const Tens& in, const Tens& out) {
     const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, ld8 = in.ld / 8, nb = e.batch;
     const void* ip = in.p; void* op_ = out.p;
-    e.op(name, [=](cudaStream_t st) {
+    e.add_op(name, "maxpool5_kernel", [=](cudaStream_t st) {
       const dim3 g((H * W * C8 + 255) / 256, nb), b(256);
-      if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? maxpool5_kernel<BF16, true> : maxpool5_kernel<BF16, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, ld8, static_cast<uint4*>(op_)));
-      else VPB_CUDA_OK(launch_k(nb > 1 ? maxpool5_kernel<F16, true> : maxpool5_kernel<F16, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, ld8, static_cast<uint4*>(op_)));
+      VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+        using E = decltype(tag);
+        return launch_k(nb > 1 ? maxpool5_kernel<E, true> : maxpool5_kernel<E, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, ld8, static_cast<uint4*>(op_));
+      }));
       return VPB_OK;
-    });
+    }, 0.0, nb * 32.0 * H * W * C8);
   }
   // PSABlock on y (in place): y += attention(y); y += ffn(y)   (common_layers.py:77-118)
   void psablock(const std::string& p, const Tens& y, int nh) {
     if (!ok()) return;
     const int C = y.C, T = y.H * y.W, dh = C / nh, dk = dh / 2, per = 2 * dk + dh, dt = e.dtype, nb = e.batch;
-    Tens qkv = e.talloc(y.H, y.W, nh * per);
+    Tens qkv = e.act_alloc(y.H, y.W, nh * per);
     cbs(p + ".conv1.qkv", y, qkv, nh * per, 1, 1, false);
-    Tens vc = e.talloc(y.H, y.W, C);
+    Tens vc = e.act_alloc(y.H, y.W, C);
     void* vt = e.dalloc(static_cast<size_t>(nh) * dh * T * 2 * nb);          // [N][nh][dh][T]
     {
       const void* q = qkv.p; void* vcp = vc.p;
-      e.op(p + ".split_v", [=](cudaStream_t st) {
+      e.add_op(p + ".split_v", "split_v_kernel", [=](cudaStream_t st) {
         const dim3 g((T * nh * dh + 255) / 256, nb), b(256);
-        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? split_v_kernel<BF16, true> : split_v_kernel<BF16, false>, g, b, 0, st, static_cast<const __nv_bfloat16*>(q), T, nh, dk, dh, static_cast<__nv_bfloat16*>(vcp), static_cast<__nv_bfloat16*>(vt)));
-        else VPB_CUDA_OK(launch_k(nb > 1 ? split_v_kernel<F16, true> : split_v_kernel<F16, false>, g, b, 0, st, static_cast<const __half*>(q), T, nh, dk, dh, static_cast<__half*>(vcp), static_cast<__half*>(vt)));
+        VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+          using E = decltype(tag);
+          using T16 = typename E::T;
+          return launch_k(nb > 1 ? split_v_kernel<E, true> : split_v_kernel<E, false>, g, b, 0, st, static_cast<const T16*>(q), T, nh, dk, dh, static_cast<T16*>(vcp), static_cast<T16*>(vt));
+        }));
         return VPB_OK;
-      });
+      }, 0.0, nb * 6.0 * T * nh * dh);
     }
-    Tens dwv = e.talloc(y.H, y.W, C);
+    Tens dwv = e.act_alloc(y.H, y.W, C);
     dw(p + ".conv1.conv1", vc, dwv, false);                     // positional term: depthwise 3x3 on v, no activation
-    Tens att = e.talloc(y.H, y.W, C);
+    Tens att = e.act_alloc(y.H, y.W, C);
     const float scale = 1.0f / std::sqrt(static_cast<float>(dk));
     for (int h = 0; h < nh && ok(); ++h) {
       // S = Q K^T: pixels = query tokens, Cin = dk (q channels of head h), "weights" = the k channels of every token
       // of the same sample
-      Tens s = e.talloc(1, T, T), pm = e.talloc(1, T, T);
+      Tens s = e.act_alloc(1, T, T), pm = e.act_alloc(1, T, T);
       Tens q = qkv.slice(h * per, dk);
       Tens qv = q; qv.H = 1; qv.W = T;
       const void* kmat = static_cast<const uint8_t*>(qkv.p) + static_cast<size_t>(h * per + dk) * 2;
-      rc = e.conv(p + ".attn.qk" + std::to_string(h), qv, s, T, 1, 1, kmat, nullptr, ACT_NONE, VPB_EPI_STORE, nullptr, ACT_NONE,
-                  /*ldw=*/qkv.ld, /*w_img=*/T * qkv.ld);
+      vpb_conv_args a = conv(qv, s, T, 1, 1, kmat, nullptr, ACT_NONE, VPB_EPI_STORE, nullptr);
+      a.ldw = qkv.ld; a.w_img = T * qkv.ld;
+      rc = e.append_conv(p + ".attn.qk" + std::to_string(h), a);
       if (!ok()) return;
       {
         const void* sp = s.p; void* pp = pm.p;
-        e.op(p + ".attn.softmax" + std::to_string(h), [=](cudaStream_t st) {
+        e.add_op(p + ".attn.softmax" + std::to_string(h), "softmax_rows_kernel", [=](cudaStream_t st) {
           const dim3 g((nb * T + 7) / 8), b(256);
-          if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(softmax_rows_kernel<BF16>, g, b, 0, st, static_cast<const __nv_bfloat16*>(sp), nb * T, T, scale, static_cast<__nv_bfloat16*>(pp)));
-          else VPB_CUDA_OK(launch_k(softmax_rows_kernel<F16>, g, b, 0, st, static_cast<const __half*>(sp), nb * T, T, scale, static_cast<__half*>(pp)));
+          VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+            using E = decltype(tag);
+            return launch_k(softmax_rows_kernel<E>, g, b, 0, st, static_cast<const typename E::T*>(sp), nb * T, T, scale, static_cast<typename E::T*>(pp));
+          }));
           return VPB_OK;
-        });
+        }, 0.0, nb * 4.0 * T * T);
       }
       // O = P V^T (+ depthwise term): Cin = key tokens, "weights" = Vt[h] [dh][T] of the same sample
       Tens o = att.slice(h * dh, dh); o.H = 1; o.W = T;
       Tens r = dwv.slice(h * dh, dh); r.H = 1; r.W = T;
-      rc = e.conv(p + ".attn.pv" + std::to_string(h), pm, o, dh, 1, 1, static_cast<const uint8_t*>(vt) + static_cast<size_t>(h) * dh * T * 2,
-                  nullptr, ACT_NONE, VPB_EPI_ADD, &r, ACT_NONE, /*ldw=*/T, /*w_img=*/nh * dh * T);
+      a = conv(pm, o, dh, 1, 1, static_cast<const uint8_t*>(vt) + static_cast<size_t>(h) * dh * T * 2, nullptr, ACT_NONE, VPB_EPI_ADD, &r);
+      a.ldw = T; a.w_img = nh * dh * T;
+      rc = e.append_conv(p + ".attn.pv" + std::to_string(h), a);
     }
     cbs(p + ".conv1.conv2", att, y, C, 1, 1, false, 0, VPB_EPI_ADD, &y);          // y = y + proj(attention)
-    Tens f = e.talloc(y.H, y.W, 2 * C);
+    Tens f = e.act_alloc(y.H, y.W, 2 * C);
     cbs(p + ".conv2.0", y, f, 2 * C, 1, 1, true);
     cbs(p + ".conv2.1", f, y, C, 1, 1, false, 0, VPB_EPI_ADD, &y);                // y = y + ffn(y)
   }
@@ -622,54 +621,54 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   e.d_gap_scratch = static_cast<long long*>(e.dalloc(static_cast<size_t>(kGapReplicas) * 256 * 8 * e.batch + 64));
   Tens x0; x0.p = e.d_canvas; x0.H = H0; x0.W = W0; x0.C = 8; x0.ld = 8;
   // ---- backbone (auto_speed_backbone.py:9-48)
-  Tens p1 = e.talloc(H0 / 2, W0 / 2, 16);
+  Tens p1 = e.act_alloc(H0 / 2, W0 / 2, 16);
   b.cbs("net.p1", x0, p1, 16, 3, 2, true, /*cin_pad=*/8);
-  Tens a2 = e.talloc(H0 / 4, W0 / 4, 32);
+  Tens a2 = e.act_alloc(H0 / 4, W0 / 4, 32);
   b.cbs("net.p2.0", p1, a2, 32, 3, 2, true);
-  Tens p2 = e.talloc(H0 / 4, W0 / 4, 64);
+  Tens p2 = e.act_alloc(H0 / 4, W0 / 4, 64);
   b.ctx("net.p2.1", a2, p2, 64);
-  Tens a3 = e.talloc(H0 / 8, W0 / 8, 64);
+  Tens a3 = e.act_alloc(H0 / 8, W0 / 8, 64);
   b.cbs("net.p3.0", p2, a3, 64, 3, 2, true);
-  Tens h2cat = e.talloc(H0 / 8, W0 / 8, 256);                // cat(up(p4'), p3)
+  Tens h2cat = e.act_alloc(H0 / 8, W0 / 8, 256);                // cat(up(p4'), p3)
   Tens p3 = h2cat.slice(128, 128);
   b.ctx("net.p3.1", a3, p3, 128);
-  Tens a4 = e.talloc(H0 / 16, W0 / 16, 128);
+  Tens a4 = e.act_alloc(H0 / 16, W0 / 16, 128);
   b.cbs("net.p4.0", p3, a4, 128, 3, 2, true);
-  Tens h1cat = e.talloc(H0 / 16, W0 / 16, 384);              // cat(up(p5), p4)
+  Tens h1cat = e.act_alloc(H0 / 16, W0 / 16, 384);              // cat(up(p5), p4)
   Tens p4 = h1cat.slice(256, 128);
   b.ctx("net.p4.1", a4, p4, 128);
-  Tens a5 = e.talloc(H0 / 32, W0 / 32, 256);
+  Tens a5 = e.act_alloc(H0 / 32, W0 / 32, 256);
   b.cbs("net.p5.0", p4, a5, 256, 3, 2, true);
-  Tens q5 = e.talloc(H0 / 32, W0 / 32, 256);
+  Tens q5 = e.act_alloc(H0 / 32, W0 / 32, 256);
   b.ctx("net.p5.1", a5, q5, 256);
-  Tens sp = e.talloc(H0 / 32, W0 / 32, 512);                 // SPPF cat (common_layers.py:242-254)
+  Tens sp = e.act_alloc(H0 / 32, W0 / 32, 512);                 // SPPF cat (common_layers.py:242-254)
   b.cbs("net.p5.2.cv1", q5, sp.slice(0, 128), 128, 1, 1, true);
   if (b.ok()) {
     b.maxpool("net.p5.2.pool1", sp.slice(0, 128), sp.slice(128, 128));
     b.maxpool("net.p5.2.pool2", sp.slice(128, 128), sp.slice(256, 128));
     b.maxpool("net.p5.2.pool3", sp.slice(256, 128), sp.slice(384, 128));
   }
-  Tens s5 = e.talloc(H0 / 32, W0 / 32, 256);
+  Tens s5 = e.act_alloc(H0 / 32, W0 / 32, 256);
   b.cbs("net.p5.2.cv2", sp, s5, 256, 1, 1, true);
-  Tens cp = e.talloc(H0 / 32, W0 / 32, 256);                 // C2PSA cat (common_layers.py:257-269)
+  Tens cp = e.act_alloc(H0 / 32, W0 / 32, 256);                 // C2PSA cat (common_layers.py:257-269)
   b.cbs("net.p5.3.cv1", s5, cp, 256, 1, 1, true);
   b.psablock("net.p5.3.middle_block", cp.slice(128, 128), 2);
-  Tens h6cat = e.talloc(H0 / 32, W0 / 32, 384);              // cat(h5(p4''), p5)
+  Tens h6cat = e.act_alloc(H0 / 32, W0 / 32, 384);              // cat(h5(p4''), p5)
   Tens p5 = h6cat.slice(128, 256);
   b.cbs("net.p5.3.cv2", cp, p5, 256, 1, 1, true);
   // ---- neck (auto_speed_neck.py:17-24)
   if (b.ok()) b.upsample("fpn.up_p5", p5, h1cat.slice(0, 256));
-  Tens h4cat = e.talloc(H0 / 16, W0 / 16, 192);              // cat(h3(p3'), p4')
+  Tens h4cat = e.act_alloc(H0 / 16, W0 / 16, 192);              // cat(h3(p3'), p4')
   Tens p4n = h4cat.slice(64, 128);
   b.c3k2("fpn.h1", h1cat, p4n, 128, false);
   if (b.ok()) b.upsample("fpn.up_p4", p4n, h2cat.slice(0, 128));
-  Tens n3 = e.talloc(H0 / 8, W0 / 8, 64);
+  Tens n3 = e.act_alloc(H0 / 8, W0 / 8, 64);
   b.c3k2("fpn.h2", h2cat, n3, 64, false);
   b.cbs("fpn.h3", n3, h4cat.slice(0, 64), 64, 3, 2, true);
-  Tens n4 = e.talloc(H0 / 16, W0 / 16, 128);
+  Tens n4 = e.act_alloc(H0 / 16, W0 / 16, 128);
   b.c3k2("fpn.h4", h4cat, n4, 128, false);
   b.cbs("fpn.h5", n4, h6cat.slice(0, 128), 128, 3, 2, true);
-  Tens n5 = e.talloc(H0 / 32, W0 / 32, 256);
+  Tens n5 = e.act_alloc(H0 / 32, W0 / 32, 256);
   b.c3k2("fpn.h6", h6cat, n5, 256, true);
   // ---- head (auto_speed_head.py:36-49): per level [hw][72]: 64 box logits | 4 class logits | 4 zero
   const Tens feats[3] = {n3, n4, n5};
@@ -677,12 +676,12 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   for (int i = 0; i < 3 && b.ok(); ++i) {
     const Tens& f = feats[i];
     const std::string bi = "head.box." + std::to_string(i), ci = "head.cls." + std::to_string(i);
-    lv[i] = e.talloc(f.H, f.W, 72);
-    Tens b1 = e.talloc(f.H, f.W, 64), b2 = e.talloc(f.H, f.W, 64);
+    lv[i] = e.act_alloc(f.H, f.W, 72);
+    Tens b1 = e.act_alloc(f.H, f.W, 64), b2 = e.act_alloc(f.H, f.W, 64);
     b.cbs(bi + ".0", f, b1, 64, 3, 1, true);
     b.cbs(bi + ".1", b1, b2, 64, 3, 1, true);
     b.plain(bi + ".2", b2, lv[i].slice(0, 64), 64, 1, ACT_NONE);
-    Tens c1 = e.talloc(f.H, f.W, f.C), c2 = e.talloc(f.H, f.W, 80), c3 = e.talloc(f.H, f.W, 80), c4 = e.talloc(f.H, f.W, 80);
+    Tens c1 = e.act_alloc(f.H, f.W, f.C), c2 = e.act_alloc(f.H, f.W, 80), c3 = e.act_alloc(f.H, f.W, 80), c4 = e.act_alloc(f.H, f.W, 80);
     b.dw(ci + ".0", f, c1, true);
     b.cbs(ci + ".1", c1, c2, 80, 1, 1, true);
     b.dw(ci + ".2", c2, c3, true);
@@ -697,12 +696,15 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
     const float strides[3] = {8.f, 16.f, 32.f};
     for (int i = 0; i < 3; ++i) {
       const void* lp = lv[i].p; const int h = lv[i].H, wd = lv[i].W, ld = lv[i].ld, off = a0; const float st_ = strides[i];
-      e.op("head.decode" + std::to_string(i), [=](cudaStream_t st) {
+      // 4 * kDfl box and kNC class logits read, 8 fp32 written per anchor
+      e.add_op("head.decode" + std::to_string(i), "decode_kernel", [=](cudaStream_t st) {
         const dim3 g((h * wd + 127) / 128, nb), bb(128);
-        if (dt == VPB_BF16) VPB_CUDA_OK(launch_k(nb > 1 ? decode_kernel<BF16, true> : decode_kernel<BF16, false>, g, bb, 0, st, static_cast<const __nv_bfloat16*>(lp), h, wd, ld, st_, off, kNA, raw));
-        else VPB_CUDA_OK(launch_k(nb > 1 ? decode_kernel<F16, true> : decode_kernel<F16, false>, g, bb, 0, st, static_cast<const __half*>(lp), h, wd, ld, st_, off, kNA, raw));
+        VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+          using E = decltype(tag);
+          return launch_k(nb > 1 ? decode_kernel<E, true> : decode_kernel<E, false>, g, bb, 0, st, static_cast<const typename E::T*>(lp), h, wd, ld, st_, off, kNA, raw);
+        }));
         return VPB_OK;
-      });
+      }, 0.0, nb * (2.0 * (4 * kDfl + kNC) + 32.0) * h * wd);
       a0 += h * wd;
     }
   }
@@ -731,53 +733,61 @@ static int as_launch_all(vp_autospeed& e, const vpb_frame* frames, cudaStream_t 
   return VPB_OK;
 }
 
-// letterbox geometry (auto_speed_infer.py:31-43) of an h x w frame; VPB_ERR_ARG (naming `who` and frame k) if it
-// cannot be resized.  Host-only.
-static int as_letterbox(int h, int w, const char* who, int k, PreGeom* g, float* scale) {
-  const double sc = std::min(static_cast<double>(kASW) / w, static_cast<double>(kASH) / h);
-  const int nw = static_cast<int>(w * sc), nh = static_cast<int>(h * sc);
-  if (nw < 1 || nh < 1) { vpb_set_error("%s: frame %d: %dx%d too small", who, k, w, h); return VPB_ERR_ARG; }
-  g->h = h; g->w = w; g->OW = nw; g->OH = nh; g->x0 = (kASW - nw) / 2; g->y0 = (kASH - nh) / 2;
-  *scale = static_cast<float>(sc);
-  return PreprocessPlan::check(*g, VPB_RESIZE_PIL_BILINEAR, who, k);
-}
+// letterbox scale of an h x w frame (auto_speed_infer.py:31-43)
+static double as_scale(int h, int w) { return std::min(static_cast<double>(kASW) / w, static_cast<double>(kASH) / h); }
 
-static int as_geoms(const vp_autospeed& e, const vpb_frame* frames, const char* who, PreGeom* g, float* scale) {
-  for (int k = 0; k < e.batch; ++k) {
-    const int rc = as_letterbox(frames[k].h, frames[k].w, who, k, &g[k], &scale[k]);
+}  // namespace vpb
+
+// letterbox geometry of every frame; VPB_ERR_ARG (naming `who` and the frame) if one cannot be resized.  Host-only.
+int vp_autospeed::geoms(const vpb_frame* frames, const char* who, PreGeom* g) {
+  for (int k = 0; k < batch; ++k) {
+    const int h = frames[k].h, w = frames[k].w;
+    const double sc = as_scale(h, w);
+    const int nw = static_cast<int>(w * sc), nh = static_cast<int>(h * sc);
+    if (nw < 1 || nh < 1) { vpb_set_error("%s: frame %d: %dx%d too small", who, k, w, h); return VPB_ERR_ARG; }
+    g[k] = PreGeom{};
+    g[k].h = h; g[k].w = w; g[k].OW = nw; g[k].OH = nh; g[k].x0 = (kASW - nw) / 2; g[k].y0 = (kASH - nh) / 2;
+    const int rc = PreprocessPlan::check(g[k], VPB_RESIZE_PIL_BILINEAR, who, k);
     if (rc) return rc;
   }
   return VPB_OK;
 }
 
-// Tables for the call's letterboxes; the gray border of a sample's canvas is refilled only when its letterbox changed
-// (the pre-process overwrites the pasted region on every call).
-static int as_configure(vp_autospeed& e, const PreGeom* g, const float* scale) {
-  int rc = e.pre.configure(g, e.batch, VPB_RESIZE_PIL_BILINEAR);
+// Enqueue one call for the batch frames f[0 .. batch-1]: tables for the call's letterboxes; the gray border of a
+// sample's canvas is refilled only when its letterbox changed (the pre-process overwrites the pasted region on every
+// call).
+int vp_autospeed::enqueue(const Frames& f, const PreGeom* g) {
+  int rc = pre.configure(g, batch, VPB_RESIZE_PIL_BILINEAR);
   if (rc) return rc;
   const int npix = kASW * kASH;
-  for (int k = 0; k < e.batch; ++k) {
-    e.scale[k] = scale[k];
-    if (e.canvas_geom[k] == g[k]) continue;
-    void* c = static_cast<uint8_t*>(e.d_canvas) + static_cast<size_t>(npix) * 8 * 2 * k;
-    if (e.dtype == VPB_BF16) fill_canvas_kernel<BF16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__nv_bfloat16*>(c), npix);
-    else fill_canvas_kernel<F16><<<(npix + 255) / 256, 256, 0, e.stream>>>(static_cast<__half*>(c), npix);
+  for (int k = 0; k < batch; ++k) {
+    scale[k] = static_cast<float>(as_scale(g[k].h, g[k].w));
+    if (canvas_geom[k] == g[k]) continue;
+    void* c = static_cast<uint8_t*>(d_canvas) + static_cast<size_t>(npix) * 8 * 2 * k;
+    dispatch_dtype(dtype, [&](auto tag) {
+      using E = decltype(tag);
+      fill_canvas_kernel<E><<<(npix + 255) / 256, 256, 0, stream>>>(static_cast<typename E::T*>(c), npix);
+    });
     VPB_CUDA_OK(cudaGetLastError());
-    e.canvas_geom[k] = g[k];
+    canvas_geom[k] = g[k];
   }
+  return frame_graph.run(
+      stream, pre, dtype, f, batch, [&](cudaStream_t st) { return as_launch_all(*this, f.data(), st); },
+      [&](cudaGraphExec_t x, cudaGraphNode_t n, cudaGraphNode_t) {
+        return pre.update_graph_node(x, n, f.data(), VPB_CONV_RGB_UNIT, dtype, d_canvas, nullptr);
+      });
+}
+
+// detections (and with raw the raw tensors) of every sample to the host buffers
+int vp_autospeed::fetch(bool raw) {
+  const size_t nb = batch;
+  VPB_CUDA_OK(cudaMemcpyAsync(h_counts, d_counts, 8 * nb, cudaMemcpyDeviceToHost, stream));
+  VPB_CUDA_OK(cudaMemcpyAsync(h_det, d_det, static_cast<size_t>(kMaxDet) * 6 * 4 * nb, cudaMemcpyDeviceToHost, stream));
+  if (raw) VPB_CUDA_OK(cudaMemcpyAsync(h_raw, d_raw, static_cast<size_t>(8) * kNA * 4 * nb, cudaMemcpyDeviceToHost, stream));
   return VPB_OK;
 }
 
-// Enqueue one call for the e.batch frames f[0 .. batch-1].
-static int as_enqueue(vp_autospeed& e, const Frames& f, const PreGeom* g, const float* scale) {
-  int rc = as_configure(e, g, scale);
-  if (rc) return rc;
-  return e.frame_graph.run(
-      e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return as_launch_all(e, f.data(), st); },
-      [&](cudaGraphExec_t x, cudaGraphNode_t n, cudaGraphNode_t) {
-        return e.pre.update_graph_node(x, n, f.data(), VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr);
-      });
-}
+namespace vpb {
 
 static int as_create(const char* who, const char* weights_vpw, int gpu_id, int dtype, void* stream, int batch,
                      vp_autospeed** out) {
@@ -815,48 +825,11 @@ static int as_create(const char* who, const char* weights_vpw, int gpu_id, int d
   return VPB_OK;
 }
 
-// detections (and with raw the raw tensors) of every sample to the host buffers
-static int as_fetch(vp_autospeed* e, bool raw) {
-  const size_t nb = e->batch;
-  VPB_CUDA_OK(cudaMemcpyAsync(e->h_counts, e->d_counts, 8 * nb, cudaMemcpyDeviceToHost, e->stream));
-  VPB_CUDA_OK(cudaMemcpyAsync(e->h_det, e->d_det, static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4 * nb, cudaMemcpyDeviceToHost, e->stream));
-  if (raw) VPB_CUDA_OK(cudaMemcpyAsync(e->h_raw, e->d_raw, static_cast<size_t>(8) * kNA * 4 * nb, cudaMemcpyDeviceToHost, e->stream));
-  return VPB_OK;
-}
-
-static int as_infer_host(vp_autospeed* e, const vpb_frame* frames, int n, int fetch_raw, const char* who) {
-  if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
-  PreGeom g[kMaxBatch];
-  float scale[kMaxBatch];
-  if (as_geoms(*e, frames, who, g, scale)) return VPB_ERR_ARG;
-  DeviceGuard guard(e->gpu_id);
-  Frames dev;
-  int rc = e->upload_frames(frames, n, dev);
-  if (rc) return rc;
-  rc = as_enqueue(*e, dev, g, scale);
-  if (rc) return rc;
-  rc = as_fetch(e, fetch_raw != 0);
-  if (rc) return rc;
-  VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return VPB_OK;
-}
-
 static int as_infer_host_batch(vp_autospeed* e, const uint8_t* const* frames, int n, int h, int w, int stride,
                                int fetch_raw, const char* who) {
   Frames f;
   if (!batch_frames(e, frames, n, h, w, stride, who, f)) return VPB_ERR_ARG;
-  return as_infer_host(e, f.data(), n, fetch_raw, who);
-}
-
-static int as_infer_device(vp_autospeed* e, const vpb_frame* frames, int n, const char* who) {
-  if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
-  PreGeom g[kMaxBatch];
-  float scale[kMaxBatch];
-  if (as_geoms(*e, frames, who, g, scale)) return VPB_ERR_ARG;
-  Frames f{};
-  std::copy(frames, frames + n, f.begin());
-  DeviceGuard guard(e->gpu_id);
-  return as_enqueue(*e, f, g, scale);
+  return call_host(e, f.data(), n, true, fetch_raw != 0, who);
 }
 
 static bool sample_ok(const vp_autospeed* e, int sample, const char* who) {
@@ -897,18 +870,18 @@ extern "C" int vp_autospeed_infer_batch(vp_autospeed* e, const uint8_t* const* f
 }
 
 extern "C" int vp_autospeed_infer_frames(vp_autospeed* e, const vpb_frame* frames_host, int n, int fetch_raw) {
-  return as_infer_host(e, frames_host, n, fetch_raw, "vp_autospeed_infer_frames");
+  return call_host(e, frames_host, n, true, fetch_raw != 0, "vp_autospeed_infer_frames");
 }
 
 extern "C" int vp_autospeed_infer_device_batch(vp_autospeed* e, const uint8_t* const* frames_dev, int n, int h, int w,
                                                int stride) {
   Frames f;
   if (!batch_frames(e, frames_dev, n, h, w, stride, "vp_autospeed_infer_device", f)) return VPB_ERR_ARG;
-  return as_infer_device(e, f.data(), n, "vp_autospeed_infer_device");
+  return call_device(e, f.data(), n, "vp_autospeed_infer_device");
 }
 
 extern "C" int vp_autospeed_infer_device_frames(vp_autospeed* e, const vpb_frame* frames_dev, int n) {
-  return as_infer_device(e, frames_dev, n, "vp_autospeed_infer_device_frames");
+  return call_device(e, frames_dev, n, "vp_autospeed_infer_device_frames");
 }
 
 extern "C" int vp_autospeed_infer_device(vp_autospeed* e, const uint8_t* frame_dev, int h, int w, int stride) {
@@ -918,7 +891,7 @@ extern "C" int vp_autospeed_infer_device(vp_autospeed* e, const uint8_t* frame_d
 extern "C" int vp_autospeed_sync(vp_autospeed* e, int fetch) {
   if (!e) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  if (fetch) { int rc = as_fetch(e, fetch > 1); if (rc) return rc; }
+  if (fetch) { int rc = e->fetch(fetch > 1); if (rc) return rc; }
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   return VPB_OK;
 }
@@ -964,7 +937,5 @@ extern "C" int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flop
 
 extern "C" long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {
   if (!e || !name) return VPB_ERR_ARG;
-  Tap a;
-  if (!e->find_tap(name, &a)) return VPB_ERR_ARG;
-  return e->read_tap(a.t, a.channels, dst, cap, c, h, w);
+  return e->read_tap(name, dst, cap, c, h, w);
 }

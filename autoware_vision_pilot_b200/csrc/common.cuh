@@ -11,6 +11,7 @@
 #include <stdint.h>
 #include <cstdio>
 #include <cstdlib>
+#include "../../include/vp_b200_ops.h"
 
 namespace vpb {
 
@@ -21,6 +22,10 @@ namespace vpb {
 // ----------------------------------------------------------------------------
 struct F16 { using T = __half; static constexpr int kUmmaFmt = 0; };
 struct BF16 { using T = __nv_bfloat16; static constexpr int kUmmaFmt = 1; };
+
+// f(BF16{}) for dtype VPB_BF16, f(F16{}) otherwise: a launch site written once for both element types
+// (using E = decltype(tag) inside f).
+template <class Fn> inline auto dispatch_dtype(int dtype, Fn&& f) { return dtype == VPB_BF16 ? f(BF16{}) : f(F16{}); }
 
 template <class E> __device__ __forceinline__ uint32_t pack2(float a, float b);
 template <> __device__ __forceinline__ uint32_t pack2<F16>(float a, float b) {

@@ -514,11 +514,6 @@ __global__ void __launch_bounds__(256) fuse_pool_kernel(const uint4* __restrict_
 
 // ====================================================================== C-ABI launchers
 using namespace vpb;
-#define DISPATCH(dtype, KERNEL, ...)           \
-  do {                                         \
-    if ((dtype) == VPB_BF16) KERNEL<BF16> __VA_ARGS__; \
-    else KERNEL<F16> __VA_ARGS__;              \
-  } while (0)
 
 // `*_lo` arguments of the *_x launchers: the low halves of split-fp16 tensors (NULL = plain 16-bit mode).
 // The kernels offset only the hi tensors by the image index, so split-fp16 tensors cannot be batched.
@@ -536,10 +531,9 @@ int vpb::stem_conv_x(int dtype, const void* in, const void* in_lo, int H, int W,
   const int Ho = H / 2, Wo = W / 2;
   const int n = Ho * Wo;
   const dim3 g((n + 127) / 128, batch), b(128);
-  if (dtype == VPB_BF16)
-    VPB_CUDA_OK(launch_k(stem_conv_kernel<BF16>, g, b, 0, st, static_cast<const uint2*>(in), static_cast<const uint2*>(in_lo), H, W, w, bias, static_cast<uint4*>(out), static_cast<uint4*>(out_lo), Ho, Wo));
-  else
-    VPB_CUDA_OK(launch_k(stem_conv_kernel<F16>, g, b, 0, st, static_cast<const uint2*>(in), static_cast<const uint2*>(in_lo), H, W, w, bias, static_cast<uint4*>(out), static_cast<uint4*>(out_lo), Ho, Wo));
+  VPB_CUDA_OK(dispatch_dtype(dtype, [&](auto tag) {
+    return launch_k(stem_conv_kernel<decltype(tag)>, g, b, 0, st, static_cast<const uint2*>(in), static_cast<const uint2*>(in_lo), H, W, w, bias, static_cast<uint4*>(out), static_cast<uint4*>(out_lo), Ho, Wo);
+  }));
   return VPB_OK;
 }
 extern "C" int vpb_stem_conv(int dtype, const void* in, int H, int W, const float* w,
@@ -580,7 +574,7 @@ int vpb::depthwise_x(int dtype, const void* in, const void* in_lo, int H, int W,
   uint4* o4l = static_cast<uint4*>(out_lo);
   const bool sp = in_lo != nullptr;
   if (sp != (out_lo != nullptr)) { vpb_set_error("depthwise: split mode needs both in_lo and out_lo"); return VPB_ERR_ARG; }
-#define DW_LAUNCH(E, K, S)                                                                             \
+#define DW_LAUNCH(K, S)                                                                                \
   do {                                                                                                 \
     if (sp) VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, true, false>, dim3(g.nblocks), dim3(g.threads), smem, st, i4, i4l, H, W, C, \
                                  w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, silu));  \
@@ -589,17 +583,15 @@ int vpb::depthwise_x(int dtype, const void* in, const void* in_lo, int H, int W,
     else VPB_CUDA_OK(launch_k(depthwise_kernel<E, K, S, false, false>, dim3(g.nblocks), dim3(g.threads), smem, st, i4, i4l, H, W, C, \
                               w, bias, o4, o4l, g.Ho, g.Wo, gap_acc, g.G, g.PPB, g.pix_per_block, silu));     \
   } while (0)
-#define DW_DISPATCH(E)                                            \
-  do {                                                            \
-    if (k == 3 && stride == 1) DW_LAUNCH(E, 3, 1);                \
-    else if (k == 3) DW_LAUNCH(E, 3, 2);                          \
-    else if (stride == 1) DW_LAUNCH(E, 5, 1);                     \
-    else DW_LAUNCH(E, 5, 2);                                      \
-  } while (0)
-  if (dtype == VPB_BF16) DW_DISPATCH(BF16); else DW_DISPATCH(F16);
-#undef DW_DISPATCH
+  return dispatch_dtype(dtype, [&](auto tag) -> int {
+    using E = decltype(tag);
+    if (k == 3 && stride == 1) DW_LAUNCH(3, 1);
+    else if (k == 3) DW_LAUNCH(3, 2);
+    else if (stride == 1) DW_LAUNCH(5, 1);
+    else DW_LAUNCH(5, 2);
+    return VPB_OK;
+  });
 #undef DW_LAUNCH
-  return VPB_OK;
 }
 
 extern "C" int vpb_se_scale(int dtype, const long long* gap_acc, int HW, int C, int sq,
@@ -623,12 +615,9 @@ int vpb::se_scale_x(int dtype, const long long* gap_acc, int HW, int C, int sq, 
   // per 64 KB, at most two waves; the late blocks (C = 1152 on 10x20 pixels) get 7 blocks, the first (96 on 160x320) two waves on 132 SMs
   const int n8 = HW * (C / 8);
   const int grid = std::max(1, std::min(264, (n8 * 16 + 65535) / 65536));
-  if (dtype == VPB_BF16)
-    VPB_CUDA_OK(launch_k(se_scale_kernel<BF16>, dim3(grid, batch), dim3(512), smem, st, gap_acc, 1.0f / HW, C, sq, w1, b1, w2, b2,
-                         static_cast<uint4*>(act), static_cast<uint4*>(act_lo), n8, scale_out));
-  else
-    VPB_CUDA_OK(launch_k(se_scale_kernel<F16>, dim3(grid, batch), dim3(512), smem, st, gap_acc, 1.0f / HW, C, sq, w1, b1, w2, b2,
-                         static_cast<uint4*>(act), static_cast<uint4*>(act_lo), n8, scale_out));
+  VPB_CUDA_OK(dispatch_dtype(dtype, [&](auto tag) {
+    return launch_k(se_scale_kernel<decltype(tag)>, dim3(grid, batch), dim3(512), smem, st, gap_acc, 1.0f / HW, C, sq, w1, b1, w2, b2, static_cast<uint4*>(act), static_cast<uint4*>(act_lo), n8, scale_out);
+  }));
   return VPB_OK;
 }
 
@@ -642,10 +631,10 @@ extern "C" int vpb_gap_ex(int dtype, const void* in, const void* in_lo, int HW, 
 int vpb::gap_x(int dtype, const void* in, const void* in_lo, int HW, int C, int ld, float* out, cudaStream_t st, int batch) {
   if (ld < C) { vpb_set_error("gap: ld=%d < C=%d", ld, C); return VPB_ERR_ARG; }
   if (const int rc = check_batch("gap", batch, in_lo != nullptr)) return rc;
-  if (dtype == VPB_BF16)
-    VPB_CUDA_OK(launch_k(gap_kernel<BF16>, dim3((C + 255) / 256, batch), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(in), static_cast<const __nv_bfloat16*>(in_lo), HW, C, ld, out));
-  else
-    VPB_CUDA_OK(launch_k(gap_kernel<F16>, dim3((C + 255) / 256, batch), dim3(256), 0, st, static_cast<const __half*>(in), static_cast<const __half*>(in_lo), HW, C, ld, out));
+  VPB_CUDA_OK(dispatch_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::T;
+    return launch_k(gap_kernel<decltype(tag)>, dim3((C + 255) / 256, batch), dim3(256), 0, st, static_cast<const T*>(in), static_cast<const T*>(in_lo), HW, C, ld, out);
+  }));
   return VPB_OK;
 }
 
@@ -688,10 +677,10 @@ int vpb::ctx_conv1_x(int dtype, const float* in, int H, int W, const float* w, c
   if (act != VPB_ACT_GELU && act != VPB_ACT_SILU) { vpb_set_error("ctx_conv1: act %d (GELU or SILU)", act); return VPB_ERR_ARG; }
   if (const int rc = check_batch("ctx_conv1", batch, out_lo != nullptr)) return rc;
   const int n = H * W * Cout;
-  if (dtype == VPB_BF16)
-    VPB_CUDA_OK(launch_k(ctx_conv1_kernel<BF16>, dim3((n + 255) / 256, batch), dim3(256), 0, st, in, H, W, w, b, Cout, static_cast<__nv_bfloat16*>(out), static_cast<__nv_bfloat16*>(out_lo), out_pad, act));
-  else
-    VPB_CUDA_OK(launch_k(ctx_conv1_kernel<F16>, dim3((n + 255) / 256, batch), dim3(256), 0, st, in, H, W, w, b, Cout, static_cast<__half*>(out), static_cast<__half*>(out_lo), out_pad, act));
+  VPB_CUDA_OK(dispatch_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::T;
+    return launch_k(ctx_conv1_kernel<decltype(tag)>, dim3((n + 255) / 256, batch), dim3(256), 0, st, in, H, W, w, b, Cout, static_cast<T*>(out), static_cast<T*>(out_lo), out_pad, act);
+  }));
   return VPB_OK;
 }
 
@@ -723,16 +712,12 @@ int vpb::fuse_pool_x(int dtype, const void* f0, const void* f1, const void* f2, 
   if (const int rc = check_batch("fuse_pool_concat", batch, out_lo != nullptr)) return rc;
   const long warps = static_cast<long>(H4) * W4 * 182;
   const int blocks = static_cast<int>((warps * 32 + 255) / 256);
-#define FP_ARGS static_cast<const uint4*>(f0), static_cast<const uint4*>(f1), static_cast<const uint4*>(f2), \
-                static_cast<const uint4*>(f3), static_cast<const uint4*>(f4), H4, W4, static_cast<uint4*>(out), \
-                lo_off[0], lo_off[1], lo_off[2], lo_off[3], lo_off[4], static_cast<uint4*>(out_lo)
-  if (batch > 1) {
-    if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(fuse_pool_kernel<BF16, true>, dim3(blocks, batch), dim3(256), 0, st, FP_ARGS));
-    else VPB_CUDA_OK(launch_k(fuse_pool_kernel<F16, true>, dim3(blocks, batch), dim3(256), 0, st, FP_ARGS));
-  } else {
-    if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(fuse_pool_kernel<BF16, false>, dim3(blocks), dim3(256), 0, st, FP_ARGS));
-    else VPB_CUDA_OK(launch_k(fuse_pool_kernel<F16, false>, dim3(blocks), dim3(256), 0, st, FP_ARGS));
-  }
-#undef FP_ARGS
+  VPB_CUDA_OK(dispatch_dtype(dtype, [&](auto tag) {
+    using E = decltype(tag);
+    return launch_k(batch > 1 ? fuse_pool_kernel<E, true> : fuse_pool_kernel<E, false>, dim3(blocks, batch), dim3(256), 0, st,
+                    static_cast<const uint4*>(f0), static_cast<const uint4*>(f1), static_cast<const uint4*>(f2),
+                    static_cast<const uint4*>(f3), static_cast<const uint4*>(f4), H4, W4, static_cast<uint4*>(out), lo_off[0],
+                    lo_off[1], lo_off[2], lo_off[3], lo_off[4], static_cast<uint4*>(out_lo));
+  }));
   return VPB_OK;
 }

@@ -96,11 +96,10 @@ struct vp_engine : EngineRuntime {
   struct EncOut { Tens f[5]; };
   std::map<uint64_t, EncOut> enc_cache;
   std::map<uint64_t, Tens> trunk_cache;    // hash(enc)+hash(ctx)+hash(neck) -> neck output
-  // Execution lanes: every model's own ops form a lane that starts after the op producing the
+  // Execution lanes (EngineRuntime::cur_lane): every model's own ops form a lane that starts after the op producing the
   // tensor it consumes (pre-process, a shared encoder, or a shared neck).  Lanes are separate
   // streams forked/joined inside the frame graph, so the latency-bound small kernels of one
   // network overlap with the other networks.
-  int cur_lane = 0;
   std::vector<int> lane_dep;               // per lane: producer op index, -1 = the pre-process
   std::map<uint64_t, int> enc_last_op, trunk_last_op;
   std::vector<cudaStream_t> lane_streams;  // [lane], lane 0 = the engine stream
@@ -121,45 +120,9 @@ struct vp_engine : EngineRuntime {
     if (ev_pre) cudaEventDestroy(ev_pre);
   }
 
-  Tens act_alloc(int H, int W, int C, int pad = 0) {
-    Tens a; a.H = H; a.W = W; a.C = C; a.ld = C; a.pad = pad;
-    a.p = dalloc(a.bytes() * batch * (split ? 2 : 1), false);
-    if (split && a.p) a.lo = static_cast<uint8_t*>(a.p) + a.bytes();
-    return a;
-  }
-
-  // ---------------------------------------------------------- op emitters
-  int add_conv(const std::string& name, const Tens& in, int Cout, int taps, int phases, const void* w,
-               const float* bias, int act, int mode, const Tens* out, const Tens* res,
-               int final_kind = 0, float* out_f32 = nullptr, uint8_t* out_cls = nullptr,
-               const Tens* in2 = nullptr, const void* w2 = nullptr, int taps2 = 0) {
-    vpb_conv_args a{};
-    a.batch = batch;
-    a.dtype = dtype; a.H = in.H; a.W = in.W; a.Cin = in.C; a.ldi = in.ld;
-    a.Cout = Cout; a.taps = taps; a.phases = phases; a.act = act; a.mode = mode;
-    a.final_kind = final_kind; a.in = in.p; a.w = w; a.bias = bias;
-    a.in_pad = in.pad;
-    if (out) { a.out = out->p; a.ldo = out->ld; a.out_pad = out->pad; }
-    if (res) { a.res = res->p; a.ldr = res->ld; a.res_pad = res->pad; }
-    // 3x3 on a zero-bordered input -> LINEAR: the layer also writes its output's zero border, so the next 3x3 layer
-    // reads it as it stands; the split-fp16 mode runs everything as TILE (three K segments per chunk)
-    a.algo = (taps == 9 && in.pad && !split) ? VPB_ALGO_LINEAR : VPB_ALGO_TILE;
-    if (split) {
-      a.in_lo = in.lo; a.w_lo = lo(w);
-      if (out) a.out_lo = out->lo;
-      if (res) a.res_lo = res->lo;
-      if (in2) { a.in2_lo = in2->lo; a.w2_lo = lo(w2); }
-    }
-    a.out_f32 = out_f32; a.out_cls = out_cls;
-    if (in2) { a.in2 = in2->p; a.w2 = w2; a.Cin2 = in2->C; a.ld2 = in2->ld; a.in2_pad = in2->pad; a.taps2 = taps2; }
-    return append_conv(name, a, cur_lane);
-  }
-  // flops: per sample (counted for the whole batch); bytes: per launch
-  void add_op(const std::string& name, const char* kname, std::function<int(cudaStream_t)> fn, double flops = 0,
-              double bytes = 0) {
-    OpRec op; op.name = name; op.kname = kname; op.launch = std::move(fn); op.flops = flops * batch; op.bytes = bytes; op.lane = cur_lane;
-    ops.push_back(std::move(op));
-  }
+  int geoms(const vpb_frame* frames, const char* who, PreGeom* g) override;
+  int enqueue(const Frames& f, const PreGeom* g) override;
+  int fetch(bool raw) override;
 };
 
 namespace vpb {
@@ -230,7 +193,7 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
         void* dw_ = e.upload_16(pack_conv(*ew, &s));
         float* db = e.upload_f32(t);
         Tens ex = e.act_alloc(x.H, x.W, ce);
-        int rc = e.add_conv(nm + "expand", x, ce, 1, 1, dw_, db, ACT_SILU, VPB_EPI_STORE, &ex, nullptr);
+        int rc = e.append_conv(nm + "expand", e.conv_args(x, &ex, nullptr, ce, 1, 1, dw_, db, ACT_SILU, VPB_EPI_STORE));
         if (rc) return rc;
         cur = ex; bi = 1;
       }
@@ -274,8 +237,8 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
       // 1x1 project + BN (+ residual; StochasticDepth is identity in eval)
       const bool residual = (s_ == 1 && ci == cout);
       Tens po = e.act_alloc(dwo.H, dwo.W, cout);
-      int rc = e.add_conv(nm + "project", dwo, cout, 1, 1, d_wproj, d_pb, ACT_NONE,
-                          residual ? VPB_EPI_ADD : VPB_EPI_STORE, &po, residual ? &x : nullptr);
+      int rc = e.append_conv(nm + "project", e.conv_args(dwo, &po, residual ? &x : nullptr, cout, 1, 1, d_wproj, d_pb, ACT_NONE,
+                                                         residual ? VPB_EPI_ADD : VPB_EPI_STORE));
       if (rc) return rc;
       x = po;
     }
@@ -287,7 +250,7 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
   void* d_hw = e.upload_16(pack_conv(*hw, &s));
   float* d_hb = e.upload_f32(t);
   Tens f4 = e.act_alloc(x.H, x.W, 1280);
-  int rc = e.add_conv(tag + "enc8", x, 1280, 1, 1, d_hw, d_hb, ACT_SILU, VPB_EPI_STORE, &f4, nullptr);
+  int rc = e.append_conv(tag + "enc8", e.conv_args(x, &f4, nullptr, 1280, 1, 1, d_hw, d_hb, ACT_SILU, VPB_EPI_STORE));
   if (rc) return rc;
   out.f[0] = stage_out[0]; out.f[1] = stage_out[2]; out.f[2] = stage_out[3]; out.f[3] = stage_out[4]; out.f[4] = f4;
   return VPB_OK;
@@ -303,7 +266,7 @@ static int conv_layer(vp_engine& e, const WeightMap& w, const std::string& key, 
   void* dw_ = e.upload_16(pack_conv(*wt, nullptr));
   float* db = e.upload_f32(bt->f);
   if (!out->p) *out = e.act_alloc(in.H, in.W, (Cout + 7) / 8 * 8, /*pad=*/1);
-  return e.add_conv(name, in, Cout, taps, 1, dw_, db, act, mode, out, res);
+  return e.append_conv(name, e.conv_args(in, out, res, Cout, taps, 1, dw_, db, act, mode));
 }
 
 // ConvTranspose2d(k2,s2) [+ Conv1x1(skip)] summed before any activation (scene_neck.py:30-32)
@@ -317,8 +280,8 @@ static int up_skip(vp_engine& e, const WeightMap& w, const std::string& p, int i
   *out = e.act_alloc(in.H * 2, in.W * 2, Cout, /*pad=*/1);
   void* dw_ = e.upload_16(pack_convT(*ut));
   if (!skip)
-    return e.add_conv(tag + "up" + std::to_string(i), in, Cout, 1, 4, dw_, e.upload_f32(ub->f), ACT_NONE,
-                      VPB_EPI_STORE, out, nullptr);
+    return e.append_conv(tag + "up" + std::to_string(i),
+                         e.conv_args(in, out, nullptr, Cout, 1, 4, dw_, e.upload_f32(ub->f), ACT_NONE, VPB_EPI_STORE));
   // the skip link's 1x1 conv is a second K segment of the same GEMM: both layers accumulate in the
   // fp32 accumulator and the sum is rounded and written once (no intermediate tensor)
   const std::string sk = p + "skip_link_layer_" + std::to_string(i);
@@ -332,8 +295,8 @@ static int up_skip(vp_engine& e, const WeightMap& w, const std::string& p, int i
   void* dw2 = e.upload_16(pack_conv(*st, nullptr));
   std::vector<float> bsum(ub->f);
   for (int c = 0; c < Cout; ++c) bsum[c] += sb->f[c];
-  return e.add_conv(tag + "up" + std::to_string(i), in, Cout, 1, 4, dw_, e.upload_f32(bsum), ACT_NONE,
-                    VPB_EPI_STORE, out, nullptr, 0, nullptr, nullptr, skip, dw2);
+  return e.append_conv(tag + "up" + std::to_string(i),
+                       e.conv_args(in, out, nullptr, Cout, 1, 4, dw_, e.upload_f32(bsum), ACT_NONE, VPB_EPI_STORE, skip, dw2));
 }
 
 // ConvTranspose2d(k2,s2) [+ Conv1x1(skip)] and the Conv3x3 + GELU that follows it (scene_neck.py:30-37,
@@ -405,8 +368,9 @@ static int upconv_layer(vp_engine& e, const WeightMap& w, const std::string& p, 
   if (rc != VPB_OK) return done(rc);
   done(VPB_OK);
   *out = e.act_alloc(in.H * 2, in.W * 2, (Cout + 7) / 8 * 8, /*pad=*/1);
-  rc = e.add_conv(tag + "up" + std::to_string(i) + "dec" + std::to_string(dec), in, Cout, 4, 4, d_wf16, d_b9, ACT_GELU,
-                  VPB_EPI_STORE, out, nullptr, 0, nullptr, nullptr, skip, d_w216, C2 ? 9 : 0);
+  vpb_conv_args a = e.conv_args(in, out, nullptr, Cout, 4, 4, d_wf16, d_b9, ACT_GELU, VPB_EPI_STORE, skip, d_w216);
+  a.taps2 = C2 ? 9 : 0;
+  rc = e.append_conv(tag + "up" + std::to_string(i) + "dec" + std::to_string(dec), a);
   if (rc == VPB_OK)   // what the reference's three layers cost: ConvTranspose + skip 1x1 at 4 phases, then the 3x3 at 2H x 2W
     e.ops.back().flops_ref = e.batch * (2.0 * in.H * in.W * 4.0 * Cmid * (Cin + C2) + 2.0 * (4.0 * in.H * in.W) * Cout * 9.0 * Cmid);
   return rc;
@@ -500,8 +464,9 @@ static int final_conv(vp_engine& e, const WeightMap& w, const std::string& key, 
   if (mo.has_cls) mo.h_cls = static_cast<uint8_t*>(e.halloc(plane * nb));
   if (!mo.h_raw || (mo.has_cls && !mo.h_cls)) return VPB_ERR_CUDA;
   float* d_taps = static_cast<float*>(e.dalloc(plane * 9 * Cout * 4 * nb, false));   // P [batch][9*Cout][H][W]
-  int rc = e.add_conv(name + "taps", in, 9 * Cout, 1, 1, dw_, nullptr, ACT_NONE, VPB_EPI_FINAL, nullptr, nullptr,
-                      VPB_FINAL_NONE, d_taps);
+  vpb_conv_args a = e.conv_args(in, nullptr, nullptr, 9 * Cout, 1, 1, dw_, nullptr, ACT_NONE, VPB_EPI_FINAL);
+  a.final_kind = VPB_FINAL_NONE; a.out_f32 = d_taps;
+  int rc = e.append_conv(name + "taps", a);
   if (rc) return rc;
   float* raw = mo.d_raw; uint8_t* cls = mo.d_cls;
   e.add_op(name + "sum", "final_tapsum_kernel",
@@ -650,18 +615,6 @@ static int launch_all(vp_engine& e, const vpb_frame* frames, cudaStream_t st) {
   return VPB_OK;
 }
 
-// Every frame resizes to the 640 x 320 network input: VPB_ERR_ARG (naming `who` and the frame) if one cannot in the
-// engine's resize mode.  Host-only: callers run it before any device work.
-static int engine_geoms(const vp_engine& e, const vpb_frame* frames, const char* who, PreGeom* g) {
-  for (int k = 0; k < e.batch; ++k) {
-    g[k] = PreGeom{};
-    g[k].h = frames[k].h; g[k].w = frames[k].w;
-    const int rc = PreprocessPlan::check(g[k], e.cfg.resize_mode, who, k);
-    if (rc) return rc;
-  }
-  return VPB_OK;
-}
-
 // The source-output jobs of frames f: sample k's buffers grown to its frame (outside any capture; a grown buffer drops
 // the captured graph, whose node holds the old pointer), destinations, sizes and frame pointers of this call.
 static int prepare_source(vp_engine& e, const Frames& f) {
@@ -687,28 +640,6 @@ static int prepare_source(vp_engine& e, const Frames& f) {
   for (const auto& so : e.src_outs) e.src_jobs.push_back(so.job);
   e.ops.back().bytes = source_outputs_bytes(e.src_jobs.data(), static_cast<int>(e.src_jobs.size()));
   return VPB_OK;
-}
-
-// Enqueue one call's kernels for the e.batch frames f[0 .. batch-1] (graph replay when enabled and the geometries are
-// unchanged).
-static int enqueue_frames(vp_engine& e, const Frames& f, const PreGeom* g) {
-  int rc = e.pre.configure(g, e.batch, e.cfg.resize_mode);
-  if (rc) return rc;
-  if (!e.src_outs.empty()) {
-    rc = prepare_source(e, f);
-    if (rc) return rc;
-  }
-  if (!e.cfg.use_graph) rc = launch_all(e, f.data(), e.stream);
-  else
-    rc = e.frame_graph.run(
-        e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return launch_all(e, f.data(), st); },
-        [&](cudaGraphExec_t x, cudaGraphNode_t pre, cudaGraphNode_t post) {
-          const int r = e.pre.update_graph_node(x, pre, f.data(), e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
-          if (r || !post) return r;
-          return source_outputs_update_node(x, post, e.src_jobs.data(), static_cast<int>(e.src_jobs.size()));
-        });
-  if (rc == VPB_OK) e.src_ready = true;
-  return rc;
 }
 
 // VP_SRC_* flags -> the source-output jobs of every model and sample, and their launch after the lanes' join
@@ -741,10 +672,9 @@ static int build_source_outputs(vp_engine& e) {
   const int rc = viz_tables_init();
   if (rc) return rc;
   vp_engine* ep = &e;
-  OpRec op;
-  op.name = "source_outputs"; op.kname = "source_outputs_kernel"; op.lane = -1;
-  op.launch = [ep](cudaStream_t st) { return source_outputs_x(ep->src_jobs.data(), static_cast<int>(ep->src_jobs.size()), st); };
-  e.ops.push_back(std::move(op));
+  e.cur_lane = -1;
+  e.add_op("source_outputs", "source_outputs_kernel",
+           [ep](cudaStream_t st) { return source_outputs_x(ep->src_jobs.data(), static_cast<int>(ep->src_jobs.size()), st); });
   e.frame_graph.has_post = true;
   return VPB_OK;
 }
@@ -772,6 +702,56 @@ static int check_source_flags(const vp_engine_config& c) {
 }
 
 }  // namespace vpb
+
+// Every frame resizes to the 640 x 320 network input: VPB_ERR_ARG (naming `who` and the frame) if one cannot in the
+// engine's resize mode.  Host-only: callers run it before any device work.
+int vp_engine::geoms(const vpb_frame* frames, const char* who, PreGeom* g) {
+  for (int k = 0; k < batch; ++k) {
+    g[k] = PreGeom{};
+    g[k].h = frames[k].h; g[k].w = frames[k].w;
+    const int rc = PreprocessPlan::check(g[k], cfg.resize_mode, who, k);
+    if (rc) return rc;
+  }
+  return VPB_OK;
+}
+
+// Enqueue one call's kernels for the batch frames f[0 .. batch-1] (graph replay when enabled and the geometries are
+// unchanged).  The pinned host copies of the source outputs are stale from here on.
+int vp_engine::enqueue(const Frames& f, const PreGeom* g) {
+  vp_engine& e = *this;
+  e.src_host = false;
+  int rc = e.pre.configure(g, e.batch, e.cfg.resize_mode);
+  if (rc) return rc;
+  if (!e.src_outs.empty()) {
+    rc = prepare_source(e, f);
+    if (rc) return rc;
+  }
+  if (!e.cfg.use_graph) rc = launch_all(e, f.data(), e.stream);
+  else
+    rc = e.frame_graph.run(
+        e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return launch_all(e, f.data(), st); },
+        [&](cudaGraphExec_t x, cudaGraphNode_t pre, cudaGraphNode_t post) {
+          const int r = e.pre.update_graph_node(x, pre, f.data(), e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
+          if (r || !post) return r;
+          return source_outputs_update_node(x, post, e.src_jobs.data(), static_cast<int>(e.src_jobs.size()));
+        });
+  if (rc == VPB_OK) e.src_ready = true;
+  return rc;
+}
+
+// the class maps, the raw tensors the engine returns on the host (all with cfg.fetch_raw or raw), the source outputs
+int vp_engine::fetch(bool raw) {
+  for (auto& mo : outs) {
+    if (mo.has_cls)
+      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, static_cast<size_t>(mo.H) * mo.W * batch, cudaMemcpyDeviceToHost, stream));
+    if (raw || cfg.fetch_raw || !mo.has_cls || mo.kind == VP_EGO_LANES)
+      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4 * batch, cudaMemcpyDeviceToHost, stream));
+  }
+  for (const auto& so : src_outs)
+    VPB_CUDA_OK(cudaMemcpyAsync(so.h, so.d, static_cast<size_t>(so.job.dh) * so.job.dst_pitch, cudaMemcpyDeviceToHost, stream));
+  src_host = true;
+  return VPB_OK;
+}
 
 // ====================================================================== C-ABI
 extern "C" const char* vp_last_error(void) { return vpb_last_error(); }
@@ -850,27 +830,14 @@ extern "C" uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes) {
   return e->h_frame;
 }
 
-static int infer_device_frames(vp_engine* e, const Frames& f, int n, const char* who) {
-  if (!frames_ok(e, f.data(), n, who)) return VPB_ERR_ARG;
-  PreGeom g[kMaxBatch];
-  if (engine_geoms(*e, f.data(), who, g)) return VPB_ERR_ARG;
-  DeviceGuard guard(e->gpu_id);
-  e->src_host = false;
-  return enqueue_frames(*e, f, g);
-}
-
 extern "C" int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev, int n, int h, int w, int stride) {
   Frames f;
   if (!batch_frames(e, frames_dev, n, h, w, stride, "vp_engine_infer_device", f)) return VPB_ERR_ARG;
-  return infer_device_frames(e, f, n, "vp_engine_infer_device");
+  return call_device(e, f.data(), n, "vp_engine_infer_device");
 }
 
 extern "C" int vp_engine_infer_device_frames(vp_engine* e, const vpb_frame* frames_dev, int n) {
-  const char* who = "vp_engine_infer_device_frames";
-  if (!frames_ok(e, frames_dev, n, who)) return VPB_ERR_ARG;
-  Frames f{};
-  std::copy(frames_dev, frames_dev + n, f.begin());
-  return infer_device_frames(e, f, n, who);
+  return call_device(e, frames_dev, n, "vp_engine_infer_device_frames");
 }
 
 extern "C" int vp_engine_infer_device(vp_engine* e, const uint8_t* frame_dev, int h, int w, int stride) {
@@ -884,34 +851,11 @@ extern "C" int vp_engine_sync(vp_engine* e) {
   return VPB_OK;
 }
 
-static int submit_host_frames(vp_engine* e, const vpb_frame* frames, int n, bool sync, const char* who) {
-  if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
-  PreGeom g[kMaxBatch];
-  if (engine_geoms(*e, frames, who, g)) return VPB_ERR_ARG;
-  DeviceGuard guard(e->gpu_id);
-  Frames dev;
-  int rc = e->upload_frames(frames, n, dev);
-  if (rc) return rc;
-  rc = enqueue_frames(*e, dev, g);
-  if (rc) return rc;
-  for (auto& mo : e->outs) {
-    if (mo.has_cls)
-      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, static_cast<size_t>(mo.H) * mo.W * n, cudaMemcpyDeviceToHost, e->stream));
-    if (e->cfg.fetch_raw || !mo.has_cls || mo.kind == VP_EGO_LANES)
-      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4 * n, cudaMemcpyDeviceToHost, e->stream));
-  }
-  for (const auto& so : e->src_outs)
-    VPB_CUDA_OK(cudaMemcpyAsync(so.h, so.d, static_cast<size_t>(so.job.dh) * so.job.dst_pitch, cudaMemcpyDeviceToHost, e->stream));
-  e->src_host = true;
-  if (sync) VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return VPB_OK;
-}
-
 static int submit_host_batch(vp_engine* e, const uint8_t* const* frames, int n, int h, int w, int stride, bool sync) {
   const char* who = sync ? "vp_engine_infer" : "vp_engine_submit";
   Frames f;
   if (!batch_frames(e, frames, n, h, w, stride, who, f)) return VPB_ERR_ARG;
-  return submit_host_frames(e, f.data(), n, sync, who);
+  return call_host(e, f.data(), n, sync, false, who);
 }
 
 extern "C" int vp_engine_infer(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride) {
@@ -931,11 +875,11 @@ extern "C" int vp_engine_submit_batch(vp_engine* e, const uint8_t* const* frames
 }
 
 extern "C" int vp_engine_infer_frames(vp_engine* e, const vpb_frame* frames_host, int n) {
-  return submit_host_frames(e, frames_host, n, true, "vp_engine_infer_frames");
+  return call_host(e, frames_host, n, true, false, "vp_engine_infer_frames");
 }
 
 extern "C" int vp_engine_submit_frames(vp_engine* e, const vpb_frame* frames_host, int n) {
-  return submit_host_frames(e, frames_host, n, false, "vp_engine_submit_frames");
+  return call_host(e, frames_host, n, false, false, "vp_engine_submit_frames");
 }
 
 extern "C" int vp_engine_fetch_raw(vp_engine* e, int idx) {
@@ -1032,28 +976,7 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
 extern "C" int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flops, int* launches) {
   if (!e || !ms || reps <= 0) return VPB_ERR_ARG;
   if (!e->frame_graph.n) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
-  DeviceGuard guard(e->gpu_id);
-  cudaEvent_t a, b;
-  VPB_CUDA_OK(cudaEventCreate(&a));
-  VPB_CUDA_OK(cudaEventCreate(&b));
-  double fl = 0.0;
-  int n = 0;
-  for (int r = -1; r < reps; ++r) {            // r = -1: untimed warm-up pass
-    if (r == 0) VPB_CUDA_OK(cudaEventRecord(a, e->stream));
-    for (auto& op : e->ops) {
-      if (!op.gemm || op.kind != kind) continue;
-      const int rc = op.launch(e->stream);
-      if (rc) return rc;
-      if (r >= 0) { fl += op.flops; ++n; }
-    }
-  }
-  VPB_CUDA_OK(cudaEventRecord(b, e->stream));
-  VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
-  VPB_CUDA_OK(cudaEventElapsedTime(ms, a, b));
-  cudaEventDestroy(a); cudaEventDestroy(b);
-  if (flops) *flops = fl;
-  if (launches) *launches = n;
-  return VPB_OK;
+  return e->time_ops(e->ops, [&](const OpRec& op) { return op.gemm && op.kind == kind; }, reps, ms, flops, nullptr, launches);
 }
 
 extern "C" int vp_engine_read_resized(vp_engine* e, uint8_t* dst) { return vp_engine_read_resized_at(e, 0, dst); }
@@ -1070,9 +993,7 @@ extern "C" int vp_engine_read_resized_at(vp_engine* e, int sample, uint8_t* dst)
 
 extern "C" long vp_engine_read_tap(vp_engine* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {
   if (!e || !name) return VPB_ERR_ARG;
-  Tap a;
-  if (!e->find_tap(name, &a)) return VPB_ERR_ARG;
-  return e->read_tap(a.t, a.channels, dst, cap, c, h, w);
+  return e->read_tap(name, dst, cap, c, h, w);
 }
 
 extern "C" int vp_engine_tap_dev(vp_engine* e, const char* name, vp_tap_view* v) {
@@ -1105,39 +1026,14 @@ extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, 
                                      double* bytes, int* launches) {
   if (!e || !kname || !ms || reps <= 0) return VPB_ERR_ARG;
   if (!e->frame_graph.n) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
-  DeviceGuard guard(e->gpu_id);
-  const bool is_pre = strcmp(kname, "preprocess") == 0;
-  cudaEvent_t a, b;
-  VPB_CUDA_OK(cudaEventCreate(&a));
-  VPB_CUDA_OK(cudaEventCreate(&b));
-  double fl = 0.0, by = 0.0;
-  int n = 0;
-  for (int r = -1; r < reps; ++r) {            // r = -1: untimed warm-up pass
-    if (r == 0) VPB_CUDA_OK(cudaEventRecord(a, e->stream));
-    if (is_pre) {
-      const int rc = e->pre.launch(e->frame_graph.frames.data(), e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
-      if (rc) return rc;
-      // SURVEY.md 8d: frame read + 3 x 320 x 640 16-bit tensor written, per sample
-      if (r >= 0) {
-        for (int k = 0; k < e->batch; ++k)
-          by += 3.0 * e->frame_graph.frames[k].h * e->frame_graph.frames[k].w + 2.0 * 3 * kNetH * kNetW;
-        ++n;
-      }
-      continue;
-    }
-    for (auto& op : e->ops) {
-      if (op.kname != kname) continue;
-      const int rc = op.launch(e->stream);
-      if (rc) return rc;
-      if (r >= 0) { fl += op.flops; by += op.bytes; ++n; }
-    }
-  }
-  VPB_CUDA_OK(cudaEventRecord(b, e->stream));
-  VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
-  VPB_CUDA_OK(cudaEventElapsedTime(ms, a, b));
-  cudaEventDestroy(a); cudaEventDestroy(b);
-  if (flops) *flops = fl;
-  if (bytes) *bytes = by;
-  if (launches) *launches = n;
-  return VPB_OK;
+  if (strcmp(kname, "preprocess") != 0)
+    return e->time_ops(e->ops, [&](const OpRec& op) { return op.kname == kname; }, reps, ms, flops, bytes, launches);
+  std::vector<OpRec> pre(1);
+  pre[0].launch = [e](cudaStream_t st) {
+    return e->pre.launch(e->frame_graph.frames.data(), e->cfg.convention, e->dtype, e->d_pre, e->d_resized, st);
+  };
+  // SURVEY.md 8d: frame read + 3 x 320 x 640 16-bit tensor written, per sample
+  for (int k = 0; k < e->batch; ++k)
+    pre[0].bytes += 3.0 * e->frame_graph.frames[k].h * e->frame_graph.frames[k].w + 2.0 * 3 * kNetH * kNetW;
+  return e->time_ops(pre, [](const OpRec&) { return true; }, reps, ms, flops, bytes, launches);
 }

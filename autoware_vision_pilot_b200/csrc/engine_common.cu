@@ -3,6 +3,7 @@
 #include "conv_gemm.cuh"
 #include "engine_internal.h"
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -250,13 +251,43 @@ void* EngineRuntime::upload_16(const std::vector<float>& v) {
   return p;
 }
 
-int EngineRuntime::append_conv(const std::string& name, const vpb_conv_args& a, int lane) {
+Tens EngineRuntime::act_alloc(int H, int W, int C, int pad) {
+  Tens a; a.H = H; a.W = W; a.C = C; a.ld = C; a.pad = pad;
+  a.p = dalloc(a.bytes() * batch * (split ? 2 : 1), false);
+  if (split && a.p) a.lo = static_cast<uint8_t*>(a.p) + a.bytes();
+  return a;
+}
+
+void EngineRuntime::add_op(const std::string& name, const char* kname, std::function<int(cudaStream_t)> fn, double flops,
+                           double bytes) {
+  OpRec op; op.name = name; op.kname = kname; op.launch = std::move(fn); op.flops = flops * batch; op.bytes = bytes; op.lane = cur_lane;
+  ops.push_back(std::move(op));
+}
+
+vpb_conv_args EngineRuntime::conv_args(const Tens& in, const Tens* out, const Tens* res, int Cout, int taps, int phases,
+                                       const void* w, const float* bias, int act, int mode, const Tens* in2,
+                                       const void* w2) const {
+  vpb_conv_args a{};
+  a.batch = batch;
+  a.dtype = dtype; a.H = in.H; a.W = in.W; a.Cin = in.C; a.ldi = in.ld;
+  a.Cout = Cout; a.taps = taps; a.phases = phases; a.act = act; a.mode = mode;
+  // the low halves are NULL outside the split-fp16 mode
+  a.in = in.p; a.in_lo = in.lo; a.w = w; a.w_lo = lo(w); a.bias = bias;
+  a.in_pad = in.pad;
+  a.algo = (taps == 9 && in.pad && !split) ? VPB_ALGO_LINEAR : VPB_ALGO_TILE;
+  if (out) { a.out = out->p; a.out_lo = out->lo; a.ldo = out->ld; a.out_pad = out->pad; }
+  if (res) { a.res = res->p; a.res_lo = res->lo; a.ldr = res->ld; a.res_pad = res->pad; }
+  if (in2) { a.in2 = in2->p; a.in2_lo = in2->lo; a.w2 = w2; a.w2_lo = lo(w2); a.Cin2 = in2->C; a.ld2 = in2->ld; a.in2_pad = in2->pad; }
+  return a;
+}
+
+int EngineRuntime::append_conv(const std::string& name, const vpb_conv_args& a) {
   auto plan = std::make_unique<ConvPlan>();
   const int rc = conv_plan_build(&a, plan.get());
   if (rc != VPB_OK) { const std::string e = vpb_last_error(); vpb_set_error("%s: %s", name.c_str(), e.c_str()); return rc; }
   ConvPlan* pp = plan.get();
   plans.push_back(std::move(plan));
-  OpRec op; op.name = name; op.flops = pp->flops; op.gemm = true; op.lane = lane;
+  OpRec op; op.name = name; op.flops = pp->flops; op.gemm = true; op.lane = cur_lane;
   op.kind = a.algo == VPB_ALGO_LINEAR ? 2 : 1;
   op.kname = "conv_wgmma_kernel";
   op.launch = [pp](cudaStream_t s) { return conv_plan_launch(pp, s); };
@@ -289,6 +320,32 @@ bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int
   out = {};
   for (int k = 0; k < n && k < kMaxBatch; ++k) out[k] = vpb_frame{ptrs[k], h, w, stride};
   return frames_ok(e, out.data(), n, who);
+}
+
+int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool raw, const char* who) {
+  if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
+  PreGeom g[kMaxBatch];
+  if (e->geoms(frames, who, g)) return VPB_ERR_ARG;
+  DeviceGuard guard(e->gpu_id);
+  Frames dev;
+  int rc = e->upload_frames(frames, n, dev);
+  if (rc) return rc;
+  rc = e->enqueue(dev, g);
+  if (rc) return rc;
+  rc = e->fetch(raw);
+  if (rc) return rc;
+  if (sync) VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
+  return VPB_OK;
+}
+
+int call_device(EngineRuntime* e, const vpb_frame* frames, int n, const char* who) {
+  if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
+  PreGeom g[kMaxBatch];
+  if (e->geoms(frames, who, g)) return VPB_ERR_ARG;
+  Frames f{};
+  std::copy(frames, frames + n, f.begin());
+  DeviceGuard guard(e->gpu_id);
+  return e->enqueue(f, g);
 }
 
 int EngineRuntime::upload_frames(const vpb_frame* frames, int n, Frames& dev) {
@@ -328,7 +385,11 @@ __global__ void tap_to_f32_nchw(const T* in, const T* in_lo, int H, int W, int C
   out[i] = in_lo ? v + static_cast<float>(in_lo[si]) : v;
 }
 
-long EngineRuntime::read_tap(const Tens& t, int channels, float* dst, long cap, int* c, int* h, int* w) {
+long EngineRuntime::read_tap(const char* name, float* dst, long cap, int* c, int* h, int* w) {
+  Tap tap;
+  if (!find_tap(name, &tap)) return VPB_ERR_ARG;
+  const Tens& t = tap.t;
+  const int channels = tap.channels;
   const long n = static_cast<long>(t.H) * t.W * channels;
   if (c) *c = channels; if (h) *h = t.H; if (w) *w = t.W;
   if (!dst) return n;
@@ -340,12 +401,11 @@ long EngineRuntime::read_tap(const Tens& t, int channels, float* dst, long cap, 
     tap_scratch_cap = static_cast<size_t>(n);
   }
   const int blocks = static_cast<int>((n + 255) / 256);
-  if (dtype == VPB_BF16)
-    tap_to_f32_nchw<<<blocks, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(t.p), static_cast<const __nv_bfloat16*>(t.lo),
-                                               t.H, t.W, channels, t.ld, t.pad, d_tap_scratch);
-  else
-    tap_to_f32_nchw<<<blocks, 256, 0, stream>>>(static_cast<const __half*>(t.p), static_cast<const __half*>(t.lo),
-                                               t.H, t.W, channels, t.ld, t.pad, d_tap_scratch);
+  dispatch_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::T;
+    tap_to_f32_nchw<<<blocks, 256, 0, stream>>>(static_cast<const T*>(t.p), static_cast<const T*>(t.lo), t.H, t.W, channels,
+                                               t.ld, t.pad, d_tap_scratch);
+  });
   cudaError_t ce = cudaMemcpyAsync(dst, d_tap_scratch, n * 4, cudaMemcpyDeviceToHost, stream);
   if (ce == cudaSuccess) ce = cudaStreamSynchronize(stream);
   if (ce != cudaSuccess) { vpb_set_error("read_tap: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
@@ -369,6 +429,33 @@ bool EngineRuntime::find_tap(const char* name, Tap* out) const {
   *out = it->second;
   out->t.p = static_cast<uint8_t*>(out->t.p) + out->t.bytes() * k;    // split-fp16 engines (lo != NULL) have batch 1
   return true;
+}
+
+int EngineRuntime::time_ops(const std::vector<OpRec>& list, const std::function<bool(const OpRec&)>& keep, int reps,
+                            float* ms, double* flops, double* bytes, int* launches) {
+  DeviceGuard guard(gpu_id);
+  cudaEvent_t a, b;
+  VPB_CUDA_OK(cudaEventCreate(&a));
+  VPB_CUDA_OK(cudaEventCreate(&b));
+  double fl = 0.0, by = 0.0;
+  int n = 0;
+  for (int r = -1; r < reps; ++r) {            // r = -1: untimed warm-up pass
+    if (r == 0) VPB_CUDA_OK(cudaEventRecord(a, stream));
+    for (const auto& op : list) {
+      if (!keep(op)) continue;
+      const int rc = op.launch(stream);
+      if (rc) return rc;
+      if (r >= 0) { fl += op.flops; by += op.bytes; ++n; }
+    }
+  }
+  VPB_CUDA_OK(cudaEventRecord(b, stream));
+  VPB_CUDA_OK(cudaStreamSynchronize(stream));
+  VPB_CUDA_OK(cudaEventElapsedTime(ms, a, b));
+  cudaEventDestroy(a); cudaEventDestroy(b);
+  if (flops) *flops = fl;
+  if (bytes) *bytes = by;
+  if (launches) *launches = n;
+  return VPB_OK;
 }
 
 }  // namespace vpb

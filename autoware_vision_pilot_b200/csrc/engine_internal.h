@@ -1,7 +1,8 @@
 // engine_internal.h — host-side runtime shared by the engines (engine.cu: the four segmentation / depth / lane
 // networks; autospeed.cu: the AutoSpeed detector), defined in engine_common.cu: the .vpw weight-file reader,
 // shape-checked lookups, K-major repacking, the device guard, and EngineRuntime (device and stream set-up, device /
-// pinned allocations, weight uploads, the op list, the frame graph, host frame upload, tap read-back).
+// pinned allocations, weight uploads, activation tensors, the op list and its convolutions, the frame graph, the frame
+// calls, kernel timing, tap read-back).
 #pragma once
 #include <cuda_runtime.h>
 #include <array>
@@ -100,6 +101,7 @@ struct ConvPlan;
 // What every engine owns: its device and stream, device / pinned allocations, the op list and the frame graph.
 struct EngineRuntime {
   int gpu_id = 0, dtype = VPB_F16;
+  int cur_lane = 0;                       // lane of the ops appended next
   // frames per call: every per-frame buffer holds `batch` samples back to back (sample outermost); weights, the launch
   // list and the graph are those of one call
   int batch = 1;
@@ -119,7 +121,7 @@ struct EngineRuntime {
   EngineRuntime() = default;
   EngineRuntime(const EngineRuntime&) = delete;
   EngineRuntime& operator=(const EngineRuntime&) = delete;
-  ~EngineRuntime();
+  virtual ~EngineRuntime();
 
   // Device gpu exists and is an sm_90 part; then borrow user_stream or create a non-blocking stream.  Errors name `who`.
   int open(const char* who, int gpu, void* user_stream);
@@ -130,18 +132,47 @@ struct EngineRuntime {
   float* upload_f32(const std::vector<float>& v);
   void* upload_16(const std::vector<float>& v);   // split mode: [hi | lo], lo = round16(v - hi)
   void* lo(const void* hi) const { auto it = lo_of.find(hi); return it == lo_of.end() ? nullptr : it->second; }
-  // build the plan of one wgmma convolution, keep it, append its launch (errors are prefixed with name)
-  int append_conv(const std::string& name, const vpb_conv_args& a, int lane = 0);
+  // NHWC activation of `batch` samples, zero border of width pad; split mode: the low half follows the batch
+  Tens act_alloc(int H, int W, int C, int pad = 0);
+  // append an op of kernel kname on lane cur_lane; flops: per sample (counted for the whole batch); bytes: per launch
+  void add_op(const std::string& name, const char* kname, std::function<int(cudaStream_t)> fn, double flops = 0,
+              double bytes = 0);
+  // vpb_conv_args of a convolution in -> out (+ res, + the second input in2 with weights w2) from the views: shapes,
+  // ld, pad, the split low halves and the batch.  3x3 on a zero-bordered input runs LINEAR (the layer also writes its
+  // output's zero border, so the next 3x3 layer reads it as it stands), everything else and the split-fp16 mode
+  // (three K segments per chunk) TILE.  The caller sets the fields only some layers use.
+  vpb_conv_args conv_args(const Tens& in, const Tens* out, const Tens* res, int Cout, int taps, int phases, const void* w,
+                          const float* bias, int act, int mode, const Tens* in2 = nullptr, const void* w2 = nullptr) const;
+  // build the plan of one wgmma convolution, keep it, append its launch on lane cur_lane (errors are prefixed with name)
+  int append_conv(const std::string& name, const vpb_conv_args& a);
   void tap(const std::string& name, const Tens& t, int channels = 0) { taps[name] = Tap{t, channels > 0 ? channels : t.C}; }
   // Copy n host frames to d_frame (grown on demand), back to back, frame k with pitch w_k*3: only the w_k*3 valid bytes
   // of every row are read from the caller's buffer, so a cv::Mat ROI / strided view is never read past its last row.
   // dev[k] describes the device copy of frame k.
   int upload_frames(const vpb_frame* frames, int n, Frames& dev);
-  // the first `channels` channels of t as fp32 [channels][H][W] into dst (NULL: size query); element count or < 0
-  long read_tap(const Tens& t, int channels, float* dst, long cap, int* c, int* h, int* w);
   // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
   bool find_tap(const char* name, Tap* out) const;
+  // tap `name` (find_tap) as fp32 [channels][H][W] into dst (NULL: size query); element count or < 0
+  long read_tap(const char* name, float* dst, long cap, int* c, int* h, int* w);
+  // Device time of the ops of `list` keep() selects, launched back to back on the engine stream: one untimed warm-up
+  // pass, then `reps` passes between one event pair, then a synchronise.  flops / bytes / launches (each may be NULL)
+  // are summed over the timed passes.
+  int time_ops(const std::vector<OpRec>& list, const std::function<bool(const OpRec&)>& keep, int reps, float* ms,
+               double* flops, double* bytes, int* launches);
+
+  // The engine's steps of a frame call (call_host, call_device).  geoms: host-only checks of the geometries of the
+  // `batch` frames (VPB_ERR_ARG naming who and the frame); enqueue: the call on device frames f; fetch: copies of the
+  // outputs to the pinned host buffers (raw: also the raw tensors the engine does not copy by default).
+  virtual int geoms(const vpb_frame* frames, const char* who, PreGeom* g) = 0;
+  virtual int enqueue(const Frames& f, const PreGeom* g) = 0;
+  virtual int fetch(bool raw) = 0;
 };
+
+// A call on n host frames: frames_ok, the engine's geometries, its device, the upload of the frames, enqueue, fetch and
+// with sync a stream synchronise.
+int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool raw, const char* who);
+// A call on n device frames: frames_ok, the engine's geometries, its device and enqueue.
+int call_device(EngineRuntime* e, const vpb_frame* frames, int n, const char* who);
 
 // n == e's batch descriptors, each with non-NULL data, h, w > 0 and stride >= 3*w (who names the call and the message
 // the frame index)

@@ -466,19 +466,22 @@ static int fill_params(const PreprocessPlan& pl, const vpb_frame* frames, int co
   return VPB_OK;
 }
 
-static const void* kernel_func(int mode, int dtype, int xt) {
-  if (is_pil(mode)) {
-    if (xt == 16)
-      return dtype == VPB_BF16 ? reinterpret_cast<const void*>(preprocess_pil_kernel<BF16, 16>)
-                               : reinterpret_cast<const void*>(preprocess_pil_kernel<F16, 16>);
-    return dtype == VPB_BF16 ? reinterpret_cast<const void*>(preprocess_pil_kernel<BF16, 32>)
-                             : reinterpret_cast<const void*>(preprocess_pil_kernel<F16, 32>);
-  }
-  return dtype == VPB_BF16 ? reinterpret_cast<const void*>(preprocess_direct_kernel<BF16>)
-                           : reinterpret_cast<const void*>(preprocess_direct_kernel<F16>);
+// The kernel of a resize mode, element type and tap capacity: the PIL kernel (params, rows_cap, pitch, TY) for the PIL
+// modes, else the direct kernel (params); the other member is NULL.
+struct PreKernel {
+  void (*pil)(PreParams, int, int, int);
+  void (*direct)(PreParams);
+  const void* func() const { return pil ? reinterpret_cast<const void*>(pil) : reinterpret_cast<const void*>(direct); }
+};
+static PreKernel pre_kernel(int mode, int dtype, int xt) {
+  return dispatch_dtype(dtype, [&](auto tag) {
+    using E = decltype(tag);
+    if (!is_pil(mode)) return PreKernel{nullptr, preprocess_direct_kernel<E>};
+    return PreKernel{xt == 16 ? preprocess_pil_kernel<E, 16> : preprocess_pil_kernel<E, 32>, nullptr};
+  });
 }
 
-bool PreprocessPlan::owns_kernel(const void* func, int dtype) const { return func == kernel_func(mode, dtype, xt); }
+bool PreprocessPlan::owns_kernel(const void* func, int dtype) const { return func == pre_kernel(mode, dtype, xt).func(); }
 
 // Re-point the captured pre-process node at other source frames (same geometries): lets the frame graph be replayed
 // on any device buffers without re-capturing.
@@ -490,7 +493,7 @@ int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node
   int rc_ = rows_cap, pitch_ = pitch, ty_ = TY;
   void* args[4] = {&p, &rc_, &pitch_, &ty_};
   cudaKernelNodeParams kp{};
-  kp.func = const_cast<void*>(kernel_func(mode, dtype, xt));
+  kp.func = const_cast<void*>(pre_kernel(mode, dtype, xt).func());
   kp.kernelParams = args;
   kp.extra = nullptr;
   if (is_pil(mode)) {
@@ -511,7 +514,8 @@ int PreprocessPlan::launch(const vpb_frame* frames, int convention, int dtype, v
   PreParams p;
   const int rc = fill_params(*this, frames, convention, out, out_u8, p);
   if (rc) return rc;
-  if (is_pil(mode)) {
+  const PreKernel k = pre_kernel(mode, dtype, xt);
+  if (k.pil) {
     dim3 grid((OWmax + kTX - 1) / kTX, (OHmax + TY - 1) / TY, n);
     {
       std::lock_guard<std::mutex> g(init_mutex());
@@ -524,18 +528,9 @@ int PreprocessPlan::launch(const vpb_frame* frames, int convention, int dtype, v
         *done = true;
       }
     }
-    const dim3 blk(kPreThreads);
-    if (xt == 16) {
-      if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(preprocess_pil_kernel<BF16, 16>, grid, blk, smem_bytes, stream, p, rows_cap, pitch, TY));
-      else VPB_CUDA_OK(launch_k(preprocess_pil_kernel<F16, 16>, grid, blk, smem_bytes, stream, p, rows_cap, pitch, TY));
-    } else {
-      if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(preprocess_pil_kernel<BF16, 32>, grid, blk, smem_bytes, stream, p, rows_cap, pitch, TY));
-      else VPB_CUDA_OK(launch_k(preprocess_pil_kernel<F16, 32>, grid, blk, smem_bytes, stream, p, rows_cap, pitch, TY));
-    }
+    VPB_CUDA_OK(launch_k(k.pil, grid, dim3(kPreThreads), smem_bytes, stream, p, rows_cap, pitch, TY));
   } else {
-    dim3 grid((OWmax + 255) / 256, OHmax, n);
-    if (dtype == VPB_BF16) VPB_CUDA_OK(launch_k(preprocess_direct_kernel<BF16>, grid, dim3(256), 0, stream, p));
-    else VPB_CUDA_OK(launch_k(preprocess_direct_kernel<F16>, grid, dim3(256), 0, stream, p));
+    VPB_CUDA_OK(launch_k(k.direct, dim3((OWmax + 255) / 256, OHmax, n), dim3(256), 0, stream, p));
   }
   return VPB_OK;
 }

@@ -130,8 +130,10 @@ extern "C" int vpb_f32_to_16(int dtype, const float* src, void* dst, long long n
   if (n == 0) return VPB_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int blocks = static_cast<int>(std::min<long long>((n + 255) / 256, 132 * 16));
-  if (dtype == VPB_BF16) f32_to_16_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>(src, static_cast<__nv_bfloat16*>(dst), n);
-  else f32_to_16_kernel<__half><<<blocks, 256, 0, st>>>(src, static_cast<__half*>(dst), n);
+  dispatch_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::T;
+    f32_to_16_kernel<T><<<blocks, 256, 0, st>>>(src, static_cast<T*>(dst), n);
+  });
   VPB_CUDA_OK(cudaGetLastError());
   return VPB_OK;
 }

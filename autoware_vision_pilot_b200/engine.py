@@ -100,6 +100,11 @@ def _bind():
     lib.vp_engine_stream.argtypes = [C.c_void_p]
     lib.vp_engine_stream.restype = C.c_void_p
     lib.vp_engine_source_output.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_SourceOutput)]
+    lib.vp_engine_time_kind.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_double),
+                                        C.POINTER(C.c_int)]
+    lib.vp_engine_kernel_names.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int)]
+    lib.vp_engine_time_kernel.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_double),
+                                          C.POINTER(C.c_double), C.POINTER(C.c_int)]
     _bound = True
     return lib
 
@@ -339,8 +344,6 @@ class Engine:
     def time_kernel(self, kind: int, reps: int = 10) -> dict:
         """Back-to-back device time of every convolution launch of one kind (1 tile layout, 2 3x3 on a padded input)."""
         ms, fl, n = C.c_float(), C.c_double(), C.c_int()
-        self._lib.vp_engine_time_kind.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float),
-                                                  C.POINTER(C.c_double), C.POINTER(C.c_int)]
         L.check(self._lib.vp_engine_time_kind(self._h, kind, reps, C.byref(ms), C.byref(fl), C.byref(n)),
                 "vp_engine_time_kind")
         return {"ms": ms.value, "flops": fl.value, "launches": n.value}
@@ -348,15 +351,12 @@ class Engine:
     def kernel_names(self) -> List[str]:
         n = C.c_int()
         names = (C.c_char_p * 64)()
-        self._lib.vp_engine_kernel_names.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int)]
         L.check(self._lib.vp_engine_kernel_names(self._h, names, 64, C.byref(n)), "vp_engine_kernel_names")
         return [names[i].decode() for i in range(min(n.value, 64))]
 
     def time_kernel_name(self, kname: str, reps: int = 10) -> dict:
         """All launches of kernel `kname` of one frame, back to back `reps` times between one CUDA-event pair."""
         ms, fl, by, n = C.c_float(), C.c_double(), C.c_double(), C.c_int()
-        self._lib.vp_engine_time_kernel.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_float),
-                                                    C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int)]
         L.check(self._lib.vp_engine_time_kernel(self._h, kname.encode(), reps, C.byref(ms), C.byref(fl), C.byref(by),
                                                 C.byref(n)), "vp_engine_time_kernel")
         return {"ms": ms.value, "flops": fl.value, "bytes": by.value, "launches": n.value}

@@ -371,7 +371,6 @@ using namespace vpb;
 // Per-frame buffers hold `batch` samples (sample outermost): canvas [N][512][1024][8], raw [N][8][kNA], cand / order /
 // det [N][...], counts [N][2], every activation [N][H][W][C].
 struct vp_autospeed : EngineRuntime {
-  PreprocessPlan pre;
   void* d_canvas = nullptr;
   float* d_raw = nullptr; float* h_raw = nullptr;
   float* d_cand = nullptr; int* d_order = nullptr; float* d_det = nullptr; int* d_counts = nullptr;
@@ -383,7 +382,7 @@ struct vp_autospeed : EngineRuntime {
   static constexpr int kMaxCand = 4096, kMaxDet = 1024;
 
   int geoms(const vpb_frame* frames, const char* who, PreGeom* g) override;
-  int enqueue(const Frames& f, const PreGeom* g) override;
+  int enqueue(const PreGeom* g) override;
   int fetch(bool raw) override;
 };
 
@@ -619,6 +618,7 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   ASBuilder b{e, w};
   const int W0 = kASW, H0 = kASH;
   e.d_gap_scratch = static_cast<long long*>(e.dalloc(static_cast<size_t>(kGapReplicas) * 256 * 8 * e.batch + 64));
+  e.add_preprocess(VPB_CONV_RGB_UNIT, e.d_canvas, nullptr);
   Tens x0; x0.p = e.d_canvas; x0.H = H0; x0.W = W0; x0.C = 8; x0.ld = 8;
   // ---- backbone (auto_speed_backbone.py:9-48)
   Tens p1 = e.act_alloc(H0 / 2, W0 / 2, 16);
@@ -708,6 +708,24 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
       a0 += h * wd;
     }
   }
+  // ---- NMS and the map back to each source frame, with the thresholds and letterboxes of the call
+  {
+    vp_autospeed* ep = &e;
+    e.add_op("postprocess", "postprocess_kernel", [ep](cudaStream_t st) {
+      PostParams pp{};
+      pp.raw = ep->d_raw; pp.NA = kNA; pp.conf = ep->conf; pp.iou = ep->iou;
+      for (int k = 0; k < ep->batch; ++k) {
+        const PreGeom& g = ep->pre.geom[k];
+        pp.scale[k] = ep->scale[k]; pp.pad_x[k] = g.x0; pp.pad_y[k] = g.y0; pp.orig_w[k] = g.w; pp.orig_h[k] = g.h;
+      }
+      pp.max_cand = vp_autospeed::kMaxCand; pp.max_det = vp_autospeed::kMaxDet;
+      pp.cand = ep->d_cand; pp.order = ep->d_order; pp.det = ep->d_det; pp.counts = ep->d_counts;
+      const size_t smem = vp_autospeed::kMaxCand;
+      if (ep->batch > 1) VPB_CUDA_OK(launch_k(postprocess_kernel<true>, dim3(ep->batch), dim3(1024), smem, st, pp));
+      else VPB_CUDA_OK(launch_k(postprocess_kernel<false>, dim3(1), dim3(1024), smem, st, pp));
+      return VPB_OK;
+    });
+  }
   e.tap("p1", p1); e.tap("p2", p2); e.tap("p3", p3); e.tap("p4", p4); e.tap("p5_ctx", q5); e.tap("p5_sppf", s5);
   e.tap("p5", p5); e.tap("n3", n3); e.tap("n4", n4); e.tap("n5", n5);
   for (int i = 0; i < 3; ++i) e.tap("head" + std::to_string(i), lv[i], 4 * kDfl + kNC);   // box | class logits, no padding
@@ -715,21 +733,11 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   return VPB_OK;
 }
 
-static int as_launch_all(vp_autospeed& e, const vpb_frame* frames, cudaStream_t st) {
-  int rc = e.pre.launch(frames, VPB_CONV_RGB_UNIT, e.dtype, e.d_canvas, nullptr, st);
-  if (rc) return rc;
-  for (auto& op : e.ops) { rc = op.launch(st); if (rc) return rc; }
-  PostParams pp{};
-  pp.raw = e.d_raw; pp.NA = kNA; pp.conf = e.conf; pp.iou = e.iou;
-  for (int k = 0; k < e.batch; ++k) {
-    const PreGeom& g = e.pre.geom[k];
-    pp.scale[k] = e.scale[k]; pp.pad_x[k] = g.x0; pp.pad_y[k] = g.y0; pp.orig_w[k] = g.w; pp.orig_h[k] = g.h;
+static int as_launch_all(vp_autospeed& e, cudaStream_t st) {
+  for (size_t i = 0; i < e.ops.size(); ++i) {
+    const int rc = e.launch_op(i, st);
+    if (rc) return rc;
   }
-  pp.max_cand = vp_autospeed::kMaxCand; pp.max_det = vp_autospeed::kMaxDet;
-  pp.cand = e.d_cand; pp.order = e.d_order; pp.det = e.d_det; pp.counts = e.d_counts;
-  const size_t smem = vp_autospeed::kMaxCand;
-  if (e.batch > 1) VPB_CUDA_OK(launch_k(postprocess_kernel<true>, dim3(e.batch), dim3(1024), smem, st, pp));
-  else VPB_CUDA_OK(launch_k(postprocess_kernel<false>, dim3(1), dim3(1024), smem, st, pp));
   return VPB_OK;
 }
 
@@ -756,7 +764,7 @@ int vp_autospeed::geoms(const vpb_frame* frames, const char* who, PreGeom* g) {
 // Enqueue one call for the batch frames f[0 .. batch-1]: tables for the call's letterboxes; the gray border of a
 // sample's canvas is refilled only when its letterbox changed (the pre-process overwrites the pasted region on every
 // call).
-int vp_autospeed::enqueue(const Frames& f, const PreGeom* g) {
+int vp_autospeed::enqueue(const PreGeom* g) {
   int rc = pre.configure(g, batch, VPB_RESIZE_PIL_BILINEAR);
   if (rc) return rc;
   const int npix = kASW * kASH;
@@ -771,11 +779,7 @@ int vp_autospeed::enqueue(const Frames& f, const PreGeom* g) {
     VPB_CUDA_OK(cudaGetLastError());
     canvas_geom[k] = g[k];
   }
-  return frame_graph.run(
-      stream, pre, dtype, f, batch, [&](cudaStream_t st) { return as_launch_all(*this, f.data(), st); },
-      [&](cudaGraphExec_t x, cudaGraphNode_t n, cudaGraphNode_t) {
-        return pre.update_graph_node(x, n, f.data(), VPB_CONV_RGB_UNIT, dtype, d_canvas, nullptr);
-      });
+  return frame_graph.run(stream, frames, n_frames, [&](cudaStream_t st) { return as_launch_all(*this, st); });
 }
 
 // detections (and with raw the raw tensors) of every sample to the host buffers
@@ -926,7 +930,7 @@ extern "C" int vp_autospeed_raw(vp_autospeed* e, const float** raw_host, const f
 
 extern "C" int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flops) {
   if (!e) return VPB_ERR_ARG;
-  if (n_launches) *n_launches = static_cast<int>(e->ops.size()) + 2;     // per call, whatever the batch
+  if (n_launches) *n_launches = static_cast<int>(e->ops.size());         // per call, whatever the batch
   if (flops) {
     double f = 0;
     for (const auto& op : e->ops) f += op.flops;       // build order: the same sum as accumulated while building

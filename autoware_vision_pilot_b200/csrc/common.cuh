@@ -296,13 +296,8 @@ __device__ __forceinline__ bool elect_one() {
 }  // namespace vpb
 
 // Host-side launch helper: every kernel of the frame graph is launched with the PDL attribute so that
-// its launch latency and prologue overlap the tail of its predecessor (VPB_PDL=0 disables).
+// its launch latency and prologue overlap the tail of its predecessor.
 namespace vpb {
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("VPB_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v != 0;
-}
 template <class... KArgs, class... Args>
 inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
                             Args&&... args) {
@@ -311,21 +306,7 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-// Same, with a runtime cluster size along x (kernels without __cluster_dims__).
-template <class... KArgs, class... Args>
-inline cudaError_t launch_k_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                                    int cluster_x, Args&&... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = cluster_x; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl_enabled() ? 2 : 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 }  // namespace vpb

@@ -74,7 +74,6 @@ using namespace vpb;
 struct vp_engine : EngineRuntime {
   vp_engine_config cfg{};
   void* d_pre_lo = nullptr;
-  PreprocessPlan pre;
   uint8_t* h_frame = nullptr; size_t h_frame_cap = 0;
   void* d_pre = nullptr;                  // [320][640][4]
   uint8_t* d_resized = nullptr;           // optional uint8 resized image (tap "resized")
@@ -97,14 +96,13 @@ struct vp_engine : EngineRuntime {
   std::map<uint64_t, EncOut> enc_cache;
   std::map<uint64_t, Tens> trunk_cache;    // hash(enc)+hash(ctx)+hash(neck) -> neck output
   // Execution lanes (EngineRuntime::cur_lane): every model's own ops form a lane that starts after the op producing the
-  // tensor it consumes (pre-process, a shared encoder, or a shared neck).  Lanes are separate
+  // tensor it consumes (the pre-process, op 0; a shared encoder; or a shared neck).  Lanes are separate
   // streams forked/joined inside the frame graph, so the latency-bound small kernels of one
   // network overlap with the other networks.
-  std::vector<int> lane_dep;               // per lane: producer op index, -1 = the pre-process
+  std::vector<int> lane_dep;               // per lane: producer op index
   std::map<uint64_t, int> enc_last_op, trunk_last_op;
   std::vector<cudaStream_t> lane_streams;  // [lane], lane 0 = the engine stream
   std::vector<cudaEvent_t> op_events;      // [op], only for ops some lane waits on
-  cudaEvent_t ev_pre = nullptr;
   std::vector<cudaEvent_t> lane_done;
   // source-resolution outputs: one entry per (model, sample, flag); src_jobs is the job table of the current call
   std::vector<SrcOut> src_outs;
@@ -117,11 +115,10 @@ struct vp_engine : EngineRuntime {
     for (size_t i = 1; i < lane_streams.size(); ++i) if (lane_streams[i]) cudaStreamDestroy(lane_streams[i]);
     for (auto ev : op_events) if (ev) cudaEventDestroy(ev);
     for (auto ev : lane_done) if (ev) cudaEventDestroy(ev);
-    if (ev_pre) cudaEventDestroy(ev_pre);
   }
 
   int geoms(const vpb_frame* frames, const char* who, PreGeom* g) override;
-  int enqueue(const Frames& f, const PreGeom* g) override;
+  int enqueue(const PreGeom* g) override;
   int fetch(bool raw) override;
 };
 
@@ -302,13 +299,7 @@ static int up_skip(vp_engine& e, const WeightMap& w, const std::string& p, int i
 // ConvTranspose2d(k2,s2) [+ Conv1x1(skip)] and the Conv3x3 + GELU that follows it (scene_neck.py:30-37,
 // scene_seg_head.py:25-33) as ONE GEMM over the low-resolution tensor: no activation separates the layers, so their
 // weights are composed once at load time (vpb_upconv_compose, upconv_compose.cu) and the upsampled tensor is never
-// materialised.  16-bit mode only — the split-fp16 mode keeps the reference's layer-by-layer graph.  VPB_UPCONV=0
-// switches the fusion off (A/B measurements).
-static bool upconv_enabled(const vp_engine& e) {
-  static int v = -1;
-  if (v < 0) { const char* s = getenv("VPB_UPCONV"); v = (s && s[0] == '0') ? 0 : 1; }
-  return v != 0 && !e.split;
-}
+// materialised.  16-bit mode only — the split-fp16 mode keeps the reference's layer-by-layer graph.
 static int upconv_layer(vp_engine& e, const WeightMap& w, const std::string& p, int i, int dec, const std::string& tag,
                         const Tens& in, const Tens* skip, Tens* out) {
   const std::string uk = p + "upsample_layer_" + std::to_string(i), dk = p + "decode_layer_" + std::to_string(dec);
@@ -426,7 +417,7 @@ static int build_neck(vp_engine& e, const WeightMap& w, const std::string& p, co
   for (int b = 0; b < 3; ++b) {
     Tens a, c;
     int rc;
-    if (upconv_enabled(e)) {
+    if (!e.split) {
       rc = upconv_layer(e, w, p, b, 2 * b, tag, d, &enc.f[skip_src[b]], &a);
       if (rc) return rc;
     } else {
@@ -486,7 +477,7 @@ static int build_head(vp_engine& e, const WeightMap& w, const std::string& p, co
     return final_conv(e, w, p + "decode_layer_8", tag + "dec8", b, VPB_FINAL_EGOLANES, mo);
   }
   Tens u3, a, b, u4, c, d;
-  if (upconv_enabled(e)) {
+  if (!e.split) {
     rc = upconv_layer(e, w, p, 3, 6, tag, neck, &enc.f[0], &a); if (rc) return rc;
     rc = conv_layer(e, w, p + "decode_layer_7", tag + "dec7", a, 9, ACT_GELU, VPB_EPI_STORE, &b, nullptr); if (rc) return rc;
     rc = upconv_layer(e, w, p, 4, 8, tag, b, nullptr, &c); if (rc) return rc;
@@ -508,7 +499,7 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
   const std::string tag = std::to_string(idx) + "/";
   const uint64_t h_enc = hash_prefix(w, pf.enc);
   e.cur_lane = idx;
-  int dep = -1;
+  int dep = 0;                              // the pre-process
   vp_engine::EncOut enc;
   auto ie = e.enc_cache.find(h_enc);
   if (ie != e.enc_cache.end()) { enc = ie->second; ++e.shared_encoders; dep = e.enc_last_op[h_enc]; }
@@ -547,7 +538,7 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
     e.trunk_cache[h_trunk] = neck;
     e.trunk_last_op[h_trunk] = static_cast<int>(e.ops.size()) - 1;
   }
-  e.lane_dep.resize(idx + 1, -1);
+  e.lane_dep.resize(idx + 1);
   e.lane_dep[idx] = dep;
   e.tap(tag + "neck", neck);
   ModelOut mo; mo.kind = kind;
@@ -567,38 +558,33 @@ static int prepare_lanes(vp_engine& e) {
     VPB_CUDA_OK(cudaStreamCreateWithFlags(&e.lane_streams[l], cudaStreamNonBlocking));
     VPB_CUDA_OK(cudaEventCreateWithFlags(&e.lane_done[l], cudaEventDisableTiming));
   }
-  VPB_CUDA_OK(cudaEventCreateWithFlags(&e.ev_pre, cudaEventDisableTiming));
   e.op_events.assign(e.ops.size(), nullptr);
   for (size_t l = 1; l < nl; ++l)
-    if (e.lane_dep[l] >= 0 && !e.op_events[e.lane_dep[l]])
+    if (!e.op_events[e.lane_dep[l]])
       VPB_CUDA_OK(cudaEventCreateWithFlags(&e.op_events[e.lane_dep[l]], cudaEventDisableTiming));
   return VPB_OK;
 }
 
-static int launch_all(vp_engine& e, const vpb_frame* frames, cudaStream_t st) {
+static int launch_all(vp_engine& e, cudaStream_t st) {
   int rc = prepare_lanes(e);
   if (rc) return rc;
   const size_t nl = e.lane_dep.size();
   const bool multi = nl > 1 && e.cfg.single_stream == 0;
   if (e.d_gap) VPB_CUDA_OK(cudaMemsetAsync(e.d_gap, 0, e.gap_used * 8, st));
-  rc = e.pre.launch(frames, e.cfg.convention, e.dtype, e.d_pre, e.d_resized, st);
-  if (rc) return rc;
   if (!multi) {
-    for (auto& op : e.ops) { rc = op.launch(st); if (rc) return rc; }
+    for (size_t i = 0; i < e.ops.size(); ++i) { rc = e.launch_op(i, st); if (rc) return rc; }
     return VPB_OK;
   }
-  VPB_CUDA_OK(cudaEventRecord(e.ev_pre, st));
   std::vector<char> started(nl, 0);
   for (size_t i = 0; i < e.ops.size(); ++i) {
     auto& op = e.ops[i];
     if (op.lane < 0) continue;               // after the join
     cudaStream_t s = op.lane == 0 ? st : e.lane_streams[op.lane];
     if (op.lane > 0 && !started[op.lane]) {   // fork: wait for the producer of this lane's input
-      const int dep = e.lane_dep[op.lane];
-      VPB_CUDA_OK(cudaStreamWaitEvent(s, dep < 0 ? e.ev_pre : e.op_events[dep], 0));
+      VPB_CUDA_OK(cudaStreamWaitEvent(s, e.op_events[e.lane_dep[op.lane]], 0));
       started[op.lane] = 1;
     }
-    rc = op.launch(s);
+    rc = e.launch_op(i, s);
     if (rc) return rc;
     if (e.op_events[i]) VPB_CUDA_OK(cudaEventRecord(e.op_events[i], s));
   }
@@ -607,19 +593,19 @@ static int launch_all(vp_engine& e, const vpb_frame* frames, cudaStream_t st) {
     VPB_CUDA_OK(cudaEventRecord(e.lane_done[l], e.lane_streams[l]));
     VPB_CUDA_OK(cudaStreamWaitEvent(st, e.lane_done[l], 0));
   }
-  for (auto& op : e.ops) {
-    if (op.lane >= 0) continue;
-    rc = op.launch(st);
+  for (size_t i = 0; i < e.ops.size(); ++i) {
+    if (e.ops[i].lane >= 0) continue;
+    rc = e.launch_op(i, st);
     if (rc) return rc;
   }
   return VPB_OK;
 }
 
-// The source-output jobs of frames f: sample k's buffers grown to its frame (outside any capture; a grown buffer drops
-// the captured graph, whose node holds the old pointer), destinations, sizes and frame pointers of this call.
-static int prepare_source(vp_engine& e, const Frames& f) {
+// The source-output jobs of the call's frames: sample k's buffers grown to its frame (outside any capture; a grown
+// buffer drops the captured graph, whose node holds the old pointer), destinations, sizes and frame pointers.
+static int prepare_source(vp_engine& e) {
   for (auto& so : e.src_outs) {
-    const vpb_frame& fr = f[so.sample];
+    const vpb_frame& fr = e.frames[so.sample];
     vpb_src_job& j = so.job;
     const int el = j.kind == VPB_SRC_DEPTH ? 4 : j.kind == VPB_SRC_OVERLAY ? 3 : 1;
     const size_t bytes = static_cast<size_t>(fr.h) * fr.w * el;
@@ -675,7 +661,9 @@ static int build_source_outputs(vp_engine& e) {
   e.cur_lane = -1;
   e.add_op("source_outputs", "source_outputs_kernel",
            [ep](cudaStream_t st) { return source_outputs_x(ep->src_jobs.data(), static_cast<int>(ep->src_jobs.size()), st); });
-  e.frame_graph.has_post = true;
+  e.ops.back().repoint = [ep](cudaGraphExec_t x, cudaGraphNode_t node) {
+    return source_outputs_update_node(x, node, ep->src_jobs.data(), static_cast<int>(ep->src_jobs.size()));
+  };
   return VPB_OK;
 }
 
@@ -715,26 +703,19 @@ int vp_engine::geoms(const vpb_frame* frames, const char* who, PreGeom* g) {
   return VPB_OK;
 }
 
-// Enqueue one call's kernels for the batch frames f[0 .. batch-1] (graph replay when enabled and the geometries are
+// Enqueue one call's kernels for the batch frames of the call (graph replay when enabled and the geometries are
 // unchanged).  The pinned host copies of the source outputs are stale from here on.
-int vp_engine::enqueue(const Frames& f, const PreGeom* g) {
+int vp_engine::enqueue(const PreGeom* g) {
   vp_engine& e = *this;
   e.src_host = false;
   int rc = e.pre.configure(g, e.batch, e.cfg.resize_mode);
   if (rc) return rc;
   if (!e.src_outs.empty()) {
-    rc = prepare_source(e, f);
+    rc = prepare_source(e);
     if (rc) return rc;
   }
-  if (!e.cfg.use_graph) rc = launch_all(e, f.data(), e.stream);
-  else
-    rc = e.frame_graph.run(
-        e.stream, e.pre, e.dtype, f, e.batch, [&](cudaStream_t st) { return launch_all(e, f.data(), st); },
-        [&](cudaGraphExec_t x, cudaGraphNode_t pre, cudaGraphNode_t post) {
-          const int r = e.pre.update_graph_node(x, pre, f.data(), e.cfg.convention, e.dtype, e.d_pre, e.d_resized);
-          if (r || !post) return r;
-          return source_outputs_update_node(x, post, e.src_jobs.data(), static_cast<int>(e.src_jobs.size()));
-        });
+  if (!e.cfg.use_graph) rc = launch_all(e, e.stream);
+  else rc = e.frame_graph.run(e.stream, e.frames, e.n_frames, [&](cudaStream_t st) { return launch_all(e, st); });
   if (rc == VPB_OK) e.src_ready = true;
   return rc;
 }
@@ -793,6 +774,7 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
     Tens pre; pre.p = e->d_pre; pre.lo = e->d_pre_lo; pre.H = kNetH; pre.W = kNetW; pre.C = 4; pre.ld = 4;
     e->tap("pre", pre, 3);                 // RGB of the [320][640][4] network input
   }
+  e->add_preprocess(cfg->convention, e->d_pre, e->d_resized);
   for (int i = 0; i < cfg->n_models; ++i) {
     if (!cfg->weights[i] || !cfg->weights[i][0]) {
       // same condition the reference rejects: scene_seg_infer.py:32-33
@@ -931,7 +913,7 @@ extern "C" int vp_engine_source_output(vp_engine* e, int idx, int sample, int ki
 extern "C" int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s) {
   if (!e || !s) return VPB_ERR_ARG;
   memset(s, 0, sizeof(*s));
-  s->n_launches = static_cast<int>(e->ops.size()) + 1;
+  s->n_launches = static_cast<int>(e->ops.size());
   for (const auto& op : e->ops) {
     s->total_flops += op.flops;
     s->reference_flops += op.flops_ref >= 0 ? op.flops_ref : op.flops;
@@ -944,30 +926,26 @@ extern "C" int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s) {
 
 extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* flops, const char** names, int* is_gemm, int* n_ops) {
   if (!e || !ms || !n_ops) return VPB_ERR_ARG;
-  if (!e->frame_graph.n) { vpb_set_error("vp_engine_profile: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->n_frames) { vpb_set_error("vp_engine_profile: run one inference first"); return VPB_ERR_STATE; }
   DeviceGuard guard(e->gpu_id);
-  const int n = static_cast<int>(e->ops.size()) + 1;
+  const int n = static_cast<int>(e->ops.size());
   *n_ops = n;
   if (n > max_ops) { vpb_set_error("vp_engine_profile: need room for %d ops", n); return VPB_ERR_ARG; }
   std::vector<cudaEvent_t> ev(n + 1);
   for (auto& x : ev) VPB_CUDA_OK(cudaEventCreate(&x));
   if (e->d_gap) VPB_CUDA_OK(cudaMemsetAsync(e->d_gap, 0, e->gap_used * 8, e->stream));
   VPB_CUDA_OK(cudaEventRecord(ev[0], e->stream));
-  int rc = e->pre.launch(e->frame_graph.frames.data(), e->cfg.convention, e->dtype, e->d_pre, e->d_resized, e->stream);
-  if (rc) return rc;
-  VPB_CUDA_OK(cudaEventRecord(ev[1], e->stream));
-  for (int i = 0; i < n - 1; ++i) {
-    rc = e->ops[i].launch(e->stream);
+  for (int i = 0; i < n; ++i) {
+    const int rc = e->ops[i].launch(e->stream);
     if (rc) return rc;
-    VPB_CUDA_OK(cudaEventRecord(ev[i + 2], e->stream));
+    VPB_CUDA_OK(cudaEventRecord(ev[i + 1], e->stream));
   }
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
-  static const char* kPre = "preprocess";
   for (int i = 0; i < n; ++i) {
     VPB_CUDA_OK(cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]));
-    if (flops) flops[i] = i == 0 ? 0.0 : e->ops[i - 1].flops;
-    if (names) names[i] = i == 0 ? kPre : e->ops[i - 1].name.c_str();
-    if (is_gemm) is_gemm[i] = i == 0 ? 0 : (e->ops[i - 1].gemm ? e->ops[i - 1].kind : 0);
+    if (flops) flops[i] = e->ops[i].flops;
+    if (names) names[i] = e->ops[i].name.c_str();
+    if (is_gemm) is_gemm[i] = e->ops[i].gemm ? e->ops[i].kind : 0;
   }
   for (auto& x : ev) cudaEventDestroy(x);
   return VPB_OK;
@@ -975,7 +953,7 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
 
 extern "C" int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flops, int* launches) {
   if (!e || !ms || reps <= 0) return VPB_ERR_ARG;
-  if (!e->frame_graph.n) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
+  if (!e->n_frames) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
   return e->time_ops(e->ops, [&](const OpRec& op) { return op.gemm && op.kind == kind; }, reps, ms, flops, nullptr, launches);
 }
 
@@ -1010,8 +988,7 @@ extern "C" void* vp_engine_stream(vp_engine* e) { return e ? static_cast<void*>(
 // ---------------------------------------------------------------- per-kernel timing for the roofline report
 extern "C" int vp_engine_kernel_names(vp_engine* e, const char** names, int cap, int* n) {
   if (!e || !n) return VPB_ERR_ARG;
-  static const char* kPreName = "preprocess";
-  std::vector<const char*> v{kPreName};
+  std::vector<const char*> v;
   for (const auto& op : e->ops) {
     bool seen = false;
     for (const char* x : v) if (op.kname == x) { seen = true; break; }
@@ -1025,15 +1002,6 @@ extern "C" int vp_engine_kernel_names(vp_engine* e, const char** names, int cap,
 extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, float* ms, double* flops,
                                      double* bytes, int* launches) {
   if (!e || !kname || !ms || reps <= 0) return VPB_ERR_ARG;
-  if (!e->frame_graph.n) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
-  if (strcmp(kname, "preprocess") != 0)
-    return e->time_ops(e->ops, [&](const OpRec& op) { return op.kname == kname; }, reps, ms, flops, bytes, launches);
-  std::vector<OpRec> pre(1);
-  pre[0].launch = [e](cudaStream_t st) {
-    return e->pre.launch(e->frame_graph.frames.data(), e->cfg.convention, e->dtype, e->d_pre, e->d_resized, st);
-  };
-  // SURVEY.md 8d: frame read + 3 x 320 x 640 16-bit tensor written, per sample
-  for (int k = 0; k < e->batch; ++k)
-    pre[0].bytes += 3.0 * e->frame_graph.frames[k].h * e->frame_graph.frames[k].w + 2.0 * 3 * kNetH * kNetW;
-  return e->time_ops(pre, [](const OpRec&) { return true; }, reps, ms, flops, bytes, launches);
+  if (!e->n_frames) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
+  return e->time_ops(e->ops, [&](const OpRec& op) { return op.kname == kname; }, reps, ms, flops, bytes, launches);
 }

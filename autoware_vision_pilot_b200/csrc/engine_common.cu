@@ -108,43 +108,33 @@ namespace vpb {
 // =============================================================== frame graph
 static bool same_geometry(const vpb_frame& a, const vpb_frame& b) { return a.h == b.h && a.w == b.w && a.stride == b.stride; }
 
-int FrameGraph::run(cudaStream_t st, const PreprocessPlan& pre, int dtype, const Frames& f, int n_,
-                    const std::function<int(cudaStream_t)>& launch,
-                    const std::function<int(cudaGraphExec_t, cudaGraphNode_t, cudaGraphNode_t)>& repoint) {
+int FrameGraph::run(cudaStream_t st, const Frames& f, int n_, const std::function<int(cudaStream_t)>& launch) {
   bool same_geom = exec && n == n_, same_src = n == n_;
   for (int k = 0; k < n_ && same_geom; ++k) same_geom = same_geometry(frames[k], f[k]);
   for (int k = 0; k < n_ && same_src; ++k) same_src = frames[k].data == f[k].data;
-  if (same_geom && !same_src && pre_node && (!has_post || post_node)) {
-    const int rc = repoint(exec, pre_node, post_node);
-    if (rc) return rc;
+  if (same_geom && !same_src) {
+    for (const auto& [i, node] : nodes) {
+      const int rc = ops[i].repoint(exec, node);
+      if (rc) return rc;
+    }
     frames = f;
     same_src = true;
   }
   if (!same_geom || !same_src) {
     invalidate();
-    pre_node = post_node = nullptr;
+    nodes.clear();
     n = 0;
     int rc = launch(st);
     if (rc) return rc;
     VPB_CUDA_OK(cudaStreamSynchronize(st));
     cudaGraph_t g = nullptr;
     VPB_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    capturing = true;
     rc = launch(st);
+    capturing = false;
     cudaError_t ce = cudaStreamEndCapture(st, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
     if (ce != cudaSuccess) { vpb_set_error("graph capture failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    size_t nn = 0;
-    cudaGraphGetNodes(g, nullptr, &nn);
-    std::vector<cudaGraphNode_t> nodes(nn);
-    cudaGraphGetNodes(g, nodes.data(), &nn);
-    for (size_t i = 0; i < nn; ++i) {
-      cudaGraphNodeType ty;
-      if (cudaGraphNodeGetType(nodes[i], &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
-      cudaKernelNodeParams kp{};
-      if (cudaGraphKernelNodeGetParams(nodes[i], &kp) != cudaSuccess) continue;
-      if (!pre_node && pre.owns_kernel(kp.func, dtype)) pre_node = nodes[i];
-      else if (has_post && !post_node && source_outputs_owns(kp.func)) post_node = nodes[i];
-    }
     ce = cudaGraphInstantiate(&exec, g, 0);
     if (graph) cudaGraphDestroy(graph);
     graph = g;
@@ -264,6 +254,37 @@ void EngineRuntime::add_op(const std::string& name, const char* kname, std::func
   ops.push_back(std::move(op));
 }
 
+void EngineRuntime::add_preprocess(int convention, void* out, uint8_t* out_u8) {
+  cur_lane = 0;
+  add_op("preprocess", "preprocess", [this, convention, out, out_u8](cudaStream_t st) {
+    return pre.launch(frames.data(), convention, dtype, out, out_u8, st);
+  });
+  ops.back().repoint = [this, convention, out, out_u8](cudaGraphExec_t x, cudaGraphNode_t node) {
+    return pre.update_graph_node(x, node, frames.data(), convention, dtype, out, out_u8);
+  };
+}
+
+int EngineRuntime::launch_op(size_t i, cudaStream_t st) {
+  const OpRec& op = ops[i];
+  const int rc = op.launch(st);
+  if (rc || !frame_graph.capturing || !op.repoint) return rc;
+  // the op's launch is now the stream's only dependency; the edge data of the programmatic (PDL) edges is asked for
+  // too, or the query would fail as lossy
+  cudaStreamCaptureStatus cs;
+  const cudaGraphNode_t* deps = nullptr;
+  const cudaGraphEdgeData* edges = nullptr;
+  size_t nd = 0;
+  VPB_CUDA_OK(cudaStreamGetCaptureInfo_v3(st, &cs, nullptr, nullptr, &deps, &edges, &nd));
+  cudaGraphNodeType ty;
+  if (cs != cudaStreamCaptureStatusActive || nd != 1 || cudaGraphNodeGetType(deps[0], &ty) != cudaSuccess ||
+      ty != cudaGraphNodeTypeKernel) {
+    vpb_set_error("graph capture: op '%s' did not capture as one kernel node (%zu dependencies)", op.name.c_str(), nd);
+    return VPB_ERR_CUDA;
+  }
+  frame_graph.nodes.emplace_back(i, deps[0]);
+  return VPB_OK;
+}
+
 vpb_conv_args EngineRuntime::conv_args(const Tens& in, const Tens* out, const Tens* res, int Cout, int taps, int phases,
                                        const void* w, const float* bias, int act, int mode, const Tens* in2,
                                        const void* w2) const {
@@ -322,6 +343,20 @@ bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int
   return frames_ok(e, out.data(), n, who);
 }
 
+// The device frames f of geometries g become the runtime's frames, and op 0, the pre-process, gets the algorithmic
+// bytes of the call (SURVEY.md 8d: frame read + 3 x OH x OW 16-bit written, per sample).  A failed call leaves no
+// frames, so nothing launches the pre-process on frames its tables were not built for.
+static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeom* g) {
+  e->frames = f;
+  e->n_frames = n;
+  double bytes = 0;
+  for (int k = 0; k < n; ++k) bytes += 3.0 * g[k].h * g[k].w + 2.0 * 3 * g[k].OH * g[k].OW;
+  e->ops[0].bytes = bytes;
+  const int rc = e->enqueue(g);
+  if (rc) e->n_frames = 0;
+  return rc;
+}
+
 int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool raw, const char* who) {
   if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
   PreGeom g[kMaxBatch];
@@ -330,7 +365,7 @@ int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool 
   Frames dev;
   int rc = e->upload_frames(frames, n, dev);
   if (rc) return rc;
-  rc = e->enqueue(dev, g);
+  rc = enqueue_frames(e, dev, n, g);
   if (rc) return rc;
   rc = e->fetch(raw);
   if (rc) return rc;
@@ -345,7 +380,7 @@ int call_device(EngineRuntime* e, const vpb_frame* frames, int n, const char* wh
   Frames f{};
   std::copy(frames, frames + n, f.begin());
   DeviceGuard guard(e->gpu_id);
-  return e->enqueue(f, g);
+  return enqueue_frames(e, f, n, g);
 }
 
 int EngineRuntime::upload_frames(const vpb_frame* frames, int n, Frames& dev) {

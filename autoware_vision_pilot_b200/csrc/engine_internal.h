@@ -12,6 +12,7 @@
 #include <memory>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 #include "ops_internal.h"
 
@@ -68,30 +69,29 @@ struct OpRec {
   int kind = 0;   // 0 = not a convolution GEMM; conv_wgmma_kernel with 1 = VPB_ALGO_TILE, 2 = VPB_ALGO_LINEAR
   int lane = 0;   // execution lane (= index of the model that owns the op); lanes run concurrently; -1: after every
                   // lane has joined the engine stream
+  // Set on the ops that read the frames of the call: re-point the op's captured kernel node at the current frames.
+  std::function<int(cudaGraphExec_t, cudaGraphNode_t)> repoint;
 };
 
 // The frames of one call: descriptor k is sample k (entries past the batch are unused).
 using Frames = std::array<vpb_frame, kMaxBatch>;
 
-// The CUDA graph of one call, keyed on the n (h, w, stride) triples and the frame pointers.  Frames of the captured
-// geometries in other buffers only re-point the captured kernel nodes that read the frames: the pre-process, and the
-// source-output launch when the engine has one.
+// The CUDA graph of one call of the launch list `ops`, keyed on the n (h, w, stride) triples and the frame pointers.
+// Frames of the captured geometries in other buffers only re-point the captured nodes of the ops that have repoint.
 struct FrameGraph {
-  cudaGraph_t graph = nullptr;           // kept alive: pre_node / post_node are handles into it
+  explicit FrameGraph(const std::vector<OpRec>& ops_) : ops(ops_) {}
+  const std::vector<OpRec>& ops;
+  cudaGraph_t graph = nullptr;           // kept alive: the recorded nodes are handles into it
   cudaGraphExec_t exec = nullptr;
-  cudaGraphNode_t pre_node = nullptr;    // the captured pre-process kernel node (re-pointed per call)
-  cudaGraphNode_t post_node = nullptr;   // the captured source_outputs_kernel node (re-pointed per call), if any
-  bool has_post = false;                 // the launch list ends with a source-output launch (set by the engine)
-  int n = 0;                             // frames of the captured / last call (0: none yet)
+  bool capturing = false;                // inside run()'s capture: EngineRuntime::launch_op records nodes
+  std::vector<std::pair<size_t, cudaGraphNode_t>> nodes;   // (op index, its captured kernel node) of the ops with repoint
+  int n = 0;                             // the key: frames f[0 .. n-1] of the graph's last launch (0: none)
   Frames frames{};
 
   // Launch the graph for frames f[0 .. n_-1] on st.  When the key differs in more than the frame pointers: launch(st)
-  // once outside capture (sets function attributes; its results are correct), capture launch(st), find the nodes of
-  // `pre` (and of the source outputs when has_post) and instantiate.  When only the pointers differ:
-  // repoint(exec, pre_node, post_node); post_node is NULL without source outputs.
-  int run(cudaStream_t st, const PreprocessPlan& pre, int dtype, const Frames& f, int n_,
-          const std::function<int(cudaStream_t)>& launch,
-          const std::function<int(cudaGraphExec_t, cudaGraphNode_t, cudaGraphNode_t)>& repoint);
+  // once outside capture (sets function attributes; its results are correct), capture launch(st) and instantiate.
+  // When only the pointers differ: ops[i].repoint(exec, node) for every recorded node.
+  int run(cudaStream_t st, const Frames& f, int n_, const std::function<int(cudaStream_t)>& launch);
   void invalidate();                     // the next run() captures again
   void release();
 };
@@ -112,9 +112,12 @@ struct EngineRuntime {
   std::vector<void*> dev_allocs, host_allocs;
   size_t weight_bytes = 0, act_bytes = 0;
   std::vector<std::unique_ptr<ConvPlan>> plans;
-  std::vector<OpRec> ops;                 // network ops (after the pre-process)
+  std::vector<OpRec> ops;                 // every launch of a call, in order; op 0 is the pre-process
   std::map<std::string, Tap> taps;
-  FrameGraph frame_graph;
+  PreprocessPlan pre;
+  Frames frames{};                        // device frames of the current / last call
+  int n_frames = 0;                       // frames of that call (0: no call has run, or the last one failed)
+  FrameGraph frame_graph{ops};
   uint8_t* d_frame = nullptr; size_t d_frame_cap = 0;           // device copy of the host frames
   float* d_tap_scratch = nullptr; size_t tap_scratch_cap = 0;   // read_tap staging (grown on demand)
 
@@ -137,6 +140,11 @@ struct EngineRuntime {
   // append an op of kernel kname on lane cur_lane; flops: per sample (counted for the whole batch); bytes: per launch
   void add_op(const std::string& name, const char* kname, std::function<int(cudaStream_t)> fn, double flops = 0,
               double bytes = 0);
+  // append the pre-process of the call's frames into out (+ the uint8 resized image out_u8, may be NULL) as op
+  // "preprocess" on lane 0; the engines call it before their first op
+  void add_preprocess(int convention, void* out, uint8_t* out_u8);
+  // launch ops[i] on st; while frame_graph captures, an op with repoint records its kernel node
+  int launch_op(size_t i, cudaStream_t st);
   // vpb_conv_args of a convolution in -> out (+ res, + the second input in2 with weights w2) from the views: shapes,
   // ld, pad, the split low halves and the batch.  3x3 on a zero-bordered input runs LINEAR (the layer also writes its
   // output's zero border, so the next 3x3 layer reads it as it stands), everything else and the split-fp16 mode
@@ -161,10 +169,11 @@ struct EngineRuntime {
                double* flops, double* bytes, int* launches);
 
   // The engine's steps of a frame call (call_host, call_device).  geoms: host-only checks of the geometries of the
-  // `batch` frames (VPB_ERR_ARG naming who and the frame); enqueue: the call on device frames f; fetch: copies of the
-  // outputs to the pinned host buffers (raw: also the raw tensors the engine does not copy by default).
+  // `batch` frames (VPB_ERR_ARG naming who and the frame); enqueue: the call on the device frames `frames` of
+  // geometries g; fetch: copies of the outputs to the pinned host buffers (raw: also the raw tensors the engine does
+  // not copy by default).
   virtual int geoms(const vpb_frame* frames, const char* who, PreGeom* g) = 0;
-  virtual int enqueue(const Frames& f, const PreGeom* g) = 0;
+  virtual int enqueue(const PreGeom* g) = 0;
   virtual int fetch(bool raw) = 0;
 };
 

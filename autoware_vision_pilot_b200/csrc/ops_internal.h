@@ -48,7 +48,6 @@ struct PreprocessPlan {
   // frames[0 .. n-1]: image k reads frames[k].data with frames[k].stride (its h, w are geom[k]'s); out / out_u8 hold
   // n images back to back (16-bit mode only for n > 1)
   int launch(const vpb_frame* frames, int convention, int dtype, void* out, uint8_t* out_u8, cudaStream_t stream) const;
-  bool owns_kernel(const void* func, int dtype) const;
   int update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame* frames, int convention, int dtype,
                         void* out, uint8_t* out_u8) const;
   ~PreprocessPlan();
@@ -82,12 +81,10 @@ int fuse_pool_x(int dtype, const void* f0, const void* f1, const void* f2, const
 // vpb_final_tapsum (conv_gemm.cu)
 int final_tapsum_x(const float* P, const float* bias, int Cout, int H, int W, int final_kind, float* out, uint8_t* cls,
                    cudaStream_t st, int batch = 1);
-// vpb_source_outputs (post_ops.cu).  source_outputs_owns: func is source_outputs_kernel (finds the captured node);
-// source_outputs_update_node re-points that node at another job table; source_outputs_bytes: algorithmic HBM bytes of
-// one launch (each distinct source map read once, frames read, outputs written); viz_tables_init uploads the palettes
-// once per device (not during a stream capture).
+// vpb_source_outputs (post_ops.cu).  source_outputs_update_node re-points a captured source_outputs_kernel node at
+// another job table; source_outputs_bytes: algorithmic HBM bytes of one launch (each distinct source map read once,
+// frames read, outputs written); viz_tables_init uploads the palettes once per device (not during a stream capture).
 int source_outputs_x(const vpb_src_job* jobs, int n, cudaStream_t st);
-bool source_outputs_owns(const void* func);
 int source_outputs_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_src_job* jobs, int n);
 double source_outputs_bytes(const vpb_src_job* jobs, int n);
 int viz_tables_init();

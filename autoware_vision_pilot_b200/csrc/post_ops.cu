@@ -423,8 +423,6 @@ int source_outputs_x(const vpb_src_job* jobs, int n, cudaStream_t st) {
   return VPB_OK;
 }
 
-bool source_outputs_owns(const void* func) { return func == reinterpret_cast<const void*>(source_outputs_kernel); }
-
 int source_outputs_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_src_job* jobs, int n) {
   SrcParams p;
   dim3 grid;

@@ -481,8 +481,6 @@ static PreKernel pre_kernel(int mode, int dtype, int xt) {
   });
 }
 
-bool PreprocessPlan::owns_kernel(const void* func, int dtype) const { return func == pre_kernel(mode, dtype, xt).func(); }
-
 // Re-point the captured pre-process node at other source frames (same geometries): lets the frame graph be replayed
 // on any device buffers without re-capturing.
 int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame* frames,

@@ -733,14 +733,6 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   return VPB_OK;
 }
 
-static int as_launch_all(vp_autospeed& e, cudaStream_t st) {
-  for (size_t i = 0; i < e.ops.size(); ++i) {
-    const int rc = e.launch_op(i, st);
-    if (rc) return rc;
-  }
-  return VPB_OK;
-}
-
 // letterbox scale of an h x w frame (auto_speed_infer.py:31-43)
 static double as_scale(int h, int w) { return std::min(static_cast<double>(kASW) / w, static_cast<double>(kASH) / h); }
 
@@ -779,7 +771,7 @@ int vp_autospeed::enqueue(const PreGeom* g) {
     VPB_CUDA_OK(cudaGetLastError());
     canvas_geom[k] = g[k];
   }
-  return frame_graph.run(stream, frames, n_frames, [&](cudaStream_t st) { return as_launch_all(*this, st); });
+  return run_call();
 }
 
 // detections (and with raw the raw tensors) of every sample to the host buffers

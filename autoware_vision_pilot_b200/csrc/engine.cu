@@ -79,43 +79,26 @@ struct vp_engine : EngineRuntime {
   uint8_t* d_resized = nullptr;           // optional uint8 resized image (tap "resized")
   std::vector<ModelOut> outs;
   int shared_encoders = 0, shared_trunks = 0;
-  // SE pooling accumulators of every MBConv block: one arena, zeroed by one memset per frame; one accumulator set per
-  // sample of the batch
-  long long* d_gap = nullptr; size_t gap_used = 0;
+  // SE pooling accumulators of every MBConv block: one arena, one accumulator set per sample of the batch.  Its used
+  // extent is what a call zeroes (EngineRuntime::call_zero, call_zero_bytes).
   static constexpr size_t kGapCap = 512 * 1024;  // int64 slots per sample (16 blocks x <=1152 ch x 8 replicas per encoder)
   long long* gap_alloc(int C) {
-    if (!d_gap) d_gap = static_cast<long long*>(dalloc(kGapCap * batch * 8, false));
-    const size_t need = static_cast<size_t>(C) * kGapReplicas * batch;
-    if (gap_used + need > kGapCap * batch) return nullptr;
-    long long* p = d_gap + gap_used;
-    gap_used += (need + 31) / 32 * 32;
-    return p;
+    if (!call_zero) call_zero = dalloc(kGapCap * batch * 8, false);
+    const size_t need = static_cast<size_t>(C) * kGapReplicas * batch, used = call_zero_bytes / 8;
+    if (used + need > kGapCap * batch) return nullptr;
+    call_zero_bytes += (need + 31) / 32 * 32 * 8;
+    return static_cast<long long*>(call_zero) + used;
   }
   // module caches for sharing
   struct EncOut { Tens f[5]; };
   std::map<uint64_t, EncOut> enc_cache;
   std::map<uint64_t, Tens> trunk_cache;    // hash(enc)+hash(ctx)+hash(neck) -> neck output
-  // Execution lanes (EngineRuntime::cur_lane): every model's own ops form a lane that starts after the op producing the
-  // tensor it consumes (the pre-process, op 0; a shared encoder; or a shared neck).  Lanes are separate
-  // streams forked/joined inside the frame graph, so the latency-bound small kernels of one
-  // network overlap with the other networks.
-  std::vector<int> lane_dep;               // per lane: producer op index
-  std::map<uint64_t, int> enc_last_op, trunk_last_op;
-  std::vector<cudaStream_t> lane_streams;  // [lane], lane 0 = the engine stream
-  std::vector<cudaEvent_t> op_events;      // [op], only for ops some lane waits on
-  std::vector<cudaEvent_t> lane_done;
+  std::map<uint64_t, int> enc_last_op, trunk_last_op;   // last op of a cached module: where a lane sharing it starts
   // source-resolution outputs: one entry per (model, sample, flag); src_jobs is the job table of the current call
   std::vector<SrcOut> src_outs;
   std::vector<vpb_src_job> src_jobs;
   bool src_ready = false;                  // a call has run (vp_engine_source_output answers)
   bool src_host = false;                   // the last call was a host call: the pinned copies are current
-
-  ~vp_engine() {
-    DeviceGuard guard(gpu_id);
-    for (size_t i = 1; i < lane_streams.size(); ++i) if (lane_streams[i]) cudaStreamDestroy(lane_streams[i]);
-    for (auto ev : op_events) if (ev) cudaEventDestroy(ev);
-    for (auto ev : lane_done) if (ev) cudaEventDestroy(ev);
-  }
 
   int geoms(const vpb_frame* frames, const char* who, PreGeom* g) override;
   int enqueue(const PreGeom* g) override;
@@ -498,11 +481,14 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
   const Prefixes pf = prefixes_for(kind);
   const std::string tag = std::to_string(idx) + "/";
   const uint64_t h_enc = hash_prefix(w, pf.enc);
-  e.cur_lane = idx;
-  int dep = 0;                              // the pre-process
+  uint64_t h_trunk = h_enc;
+  { const uint64_t a = hash_prefix(w, pf.ctx), b = hash_prefix(w, pf.neck); h_trunk = fnv1a(fnv1a(h_trunk, &a, 8), &b, 8); }
+  const auto ie = e.enc_cache.find(h_enc);
+  const auto it = e.trunk_cache.find(h_trunk);
+  // the model's lane starts after the op producing its input: a shared neck, a shared encoder, or the pre-process (op 0)
+  e.begin_lane(idx, it != e.trunk_cache.end() ? e.trunk_last_op[h_trunk] : ie != e.enc_cache.end() ? e.enc_last_op[h_enc] : 0);
   vp_engine::EncOut enc;
-  auto ie = e.enc_cache.find(h_enc);
-  if (ie != e.enc_cache.end()) { enc = ie->second; ++e.shared_encoders; dep = e.enc_last_op[h_enc]; }
+  if (ie != e.enc_cache.end()) { enc = ie->second; ++e.shared_encoders; }
   else {
     int rc = build_encoder(e, w, pf.enc, tag, enc);
     if (rc) return rc;
@@ -510,11 +496,8 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
     e.enc_last_op[h_enc] = static_cast<int>(e.ops.size()) - 1;
   }
   for (int i = 0; i < 5; ++i) e.tap(tag + "f" + std::to_string(i), enc.f[i]);
-  uint64_t h_trunk = h_enc;
-  { const uint64_t a = hash_prefix(w, pf.ctx), b = hash_prefix(w, pf.neck); h_trunk = fnv1a(fnv1a(h_trunk, &a, 8), &b, 8); }
   Tens neck;
-  auto it = e.trunk_cache.find(h_trunk);
-  if (it != e.trunk_cache.end()) { neck = it->second; ++e.shared_trunks; dep = e.trunk_last_op[h_trunk]; }
+  if (it != e.trunk_cache.end()) { neck = it->second; ++e.shared_trunks; }
   else {
     Tens feat = enc.f[4];
     if (kind == VP_EGO_LANES) {  // BackboneFeatureFusion (backbone_feature_fusion.py:13-38)
@@ -538,66 +521,11 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
     e.trunk_cache[h_trunk] = neck;
     e.trunk_last_op[h_trunk] = static_cast<int>(e.ops.size()) - 1;
   }
-  e.lane_dep.resize(idx + 1);
-  e.lane_dep[idx] = dep;
   e.tap(tag + "neck", neck);
   ModelOut mo; mo.kind = kind;
   int rc = build_head(e, w, pf.head, tag, kind, neck, enc, mo);
   if (rc) return rc;
   e.outs.push_back(mo);
-  return VPB_OK;
-}
-
-static int prepare_lanes(vp_engine& e) {
-  const size_t nl = e.lane_dep.size();
-  if (e.lane_streams.size() == nl) return VPB_OK;
-  e.lane_streams.assign(nl, nullptr);
-  e.lane_done.assign(nl, nullptr);
-  e.lane_streams[0] = e.stream;
-  for (size_t l = 1; l < nl; ++l) {
-    VPB_CUDA_OK(cudaStreamCreateWithFlags(&e.lane_streams[l], cudaStreamNonBlocking));
-    VPB_CUDA_OK(cudaEventCreateWithFlags(&e.lane_done[l], cudaEventDisableTiming));
-  }
-  e.op_events.assign(e.ops.size(), nullptr);
-  for (size_t l = 1; l < nl; ++l)
-    if (!e.op_events[e.lane_dep[l]])
-      VPB_CUDA_OK(cudaEventCreateWithFlags(&e.op_events[e.lane_dep[l]], cudaEventDisableTiming));
-  return VPB_OK;
-}
-
-static int launch_all(vp_engine& e, cudaStream_t st) {
-  int rc = prepare_lanes(e);
-  if (rc) return rc;
-  const size_t nl = e.lane_dep.size();
-  const bool multi = nl > 1 && e.cfg.single_stream == 0;
-  if (e.d_gap) VPB_CUDA_OK(cudaMemsetAsync(e.d_gap, 0, e.gap_used * 8, st));
-  if (!multi) {
-    for (size_t i = 0; i < e.ops.size(); ++i) { rc = e.launch_op(i, st); if (rc) return rc; }
-    return VPB_OK;
-  }
-  std::vector<char> started(nl, 0);
-  for (size_t i = 0; i < e.ops.size(); ++i) {
-    auto& op = e.ops[i];
-    if (op.lane < 0) continue;               // after the join
-    cudaStream_t s = op.lane == 0 ? st : e.lane_streams[op.lane];
-    if (op.lane > 0 && !started[op.lane]) {   // fork: wait for the producer of this lane's input
-      VPB_CUDA_OK(cudaStreamWaitEvent(s, e.op_events[e.lane_dep[op.lane]], 0));
-      started[op.lane] = 1;
-    }
-    rc = e.launch_op(i, s);
-    if (rc) return rc;
-    if (e.op_events[i]) VPB_CUDA_OK(cudaEventRecord(e.op_events[i], s));
-  }
-  for (size_t l = 1; l < nl; ++l) {           // join
-    if (!started[l]) continue;
-    VPB_CUDA_OK(cudaEventRecord(e.lane_done[l], e.lane_streams[l]));
-    VPB_CUDA_OK(cudaStreamWaitEvent(st, e.lane_done[l], 0));
-  }
-  for (size_t i = 0; i < e.ops.size(); ++i) {
-    if (e.ops[i].lane >= 0) continue;
-    rc = e.launch_op(i, st);
-    if (rc) return rc;
-  }
   return VPB_OK;
 }
 
@@ -706,27 +634,27 @@ int vp_engine::geoms(const vpb_frame* frames, const char* who, PreGeom* g) {
 // Enqueue one call's kernels for the batch frames of the call (graph replay when enabled and the geometries are
 // unchanged).  The pinned host copies of the source outputs are stale from here on.
 int vp_engine::enqueue(const PreGeom* g) {
-  vp_engine& e = *this;
-  e.src_host = false;
-  int rc = e.pre.configure(g, e.batch, e.cfg.resize_mode);
-  if (rc) return rc;
-  if (!e.src_outs.empty()) {
-    rc = prepare_source(e);
-    if (rc) return rc;
-  }
-  if (!e.cfg.use_graph) rc = launch_all(e, e.stream);
-  else rc = e.frame_graph.run(e.stream, e.frames, e.n_frames, [&](cudaStream_t st) { return launch_all(e, st); });
-  if (rc == VPB_OK) e.src_ready = true;
+  src_host = false;
+  int rc = pre.configure(g, batch, cfg.resize_mode);
+  if (rc == VPB_OK && !src_outs.empty()) rc = prepare_source(*this);
+  if (rc == VPB_OK) rc = run_call();
+  if (rc == VPB_OK) src_ready = true;
   return rc;
+}
+
+// mo's class map, if it has one, and with_raw its raw tensor to the pinned host buffers
+static int fetch_out(const vp_engine& e, const ModelOut& mo, bool with_raw) {
+  const size_t plane = static_cast<size_t>(mo.H) * mo.W * e.batch;
+  if (mo.has_cls) VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, plane, cudaMemcpyDeviceToHost, e.stream));
+  if (with_raw) VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, plane * mo.C * 4, cudaMemcpyDeviceToHost, e.stream));
+  return VPB_OK;
 }
 
 // the class maps, the raw tensors the engine returns on the host (all with cfg.fetch_raw or raw), the source outputs
 int vp_engine::fetch(bool raw) {
-  for (auto& mo : outs) {
-    if (mo.has_cls)
-      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, static_cast<size_t>(mo.H) * mo.W * batch, cudaMemcpyDeviceToHost, stream));
-    if (raw || cfg.fetch_raw || !mo.has_cls || mo.kind == VP_EGO_LANES)
-      VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4 * batch, cudaMemcpyDeviceToHost, stream));
+  for (const auto& mo : outs) {
+    const int rc = fetch_out(*this, mo, raw || cfg.fetch_raw || !mo.has_cls || mo.kind == VP_EGO_LANES);
+    if (rc) return rc;
   }
   for (const auto& so : src_outs)
     VPB_CUDA_OK(cudaMemcpyAsync(so.h, so.d, static_cast<size_t>(so.job.dh) * so.job.dst_pitch, cudaMemcpyDeviceToHost, stream));
@@ -750,6 +678,7 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
   if (rc) return rc;
   DeviceGuard guard(cfg->gpu_id);
   e->cfg = *cfg;
+  e->use_graph = cfg->use_graph != 0; e->single_stream = cfg->single_stream != 0;
   e->dtype = cfg->dtype == VPB_BF16 ? VPB_BF16 : VPB_F16;
   if (cfg->precision != VP_PREC_16 && cfg->precision != VP_PREC_SPLIT) {
     vpb_set_error("vp_engine_create: unknown precision %d", cfg->precision);
@@ -796,7 +725,7 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
   return VPB_OK;
 }
 
-extern "C" void vp_engine_destroy(vp_engine* e) { delete e; }   // ~vp_engine switches to the engine's device
+extern "C" void vp_engine_destroy(vp_engine* e) { delete e; }   // ~EngineRuntime switches to the engine's device
 
 extern "C" int vp_engine_num_models(const vp_engine* e) { return e ? static_cast<int>(e->outs.size()) : 0; }
 int vpb_engine_batch(const vp_engine* e) { return e ? e->batch : 0; }
@@ -867,11 +796,8 @@ extern "C" int vp_engine_submit_frames(vp_engine* e, const vpb_frame* frames_hos
 extern "C" int vp_engine_fetch_raw(vp_engine* e, int idx) {
   if (!e || idx < 0 || idx >= static_cast<int>(e->outs.size())) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  auto& mo = e->outs[idx];
-  const size_t nb = e->batch;
-  VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, static_cast<size_t>(mo.C) * mo.H * mo.W * 4 * nb, cudaMemcpyDeviceToHost, e->stream));
-  if (mo.has_cls)
-    VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, static_cast<size_t>(mo.H) * mo.W * nb, cudaMemcpyDeviceToHost, e->stream));
+  const int rc = fetch_out(*e, e->outs[idx], true);
+  if (rc) return rc;
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   return VPB_OK;
 }
@@ -931,23 +857,23 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
   const int n = static_cast<int>(e->ops.size());
   *n_ops = n;
   if (n > max_ops) { vpb_set_error("vp_engine_profile: need room for %d ops", n); return VPB_ERR_ARG; }
-  std::vector<cudaEvent_t> ev(n + 1);
-  for (auto& x : ev) VPB_CUDA_OK(cudaEventCreate(&x));
-  if (e->d_gap) VPB_CUDA_OK(cudaMemsetAsync(e->d_gap, 0, e->gap_used * 8, e->stream));
-  VPB_CUDA_OK(cudaEventRecord(ev[0], e->stream));
+  std::vector<Event> ev(n + 1);
+  for (auto& x : ev) VPB_CUDA_OK(make_event(x));
+  int rc = e->reset_call(e->stream);
+  if (rc) return rc;
+  VPB_CUDA_OK(cudaEventRecord(ev[0].get(), e->stream));
   for (int i = 0; i < n; ++i) {
-    const int rc = e->ops[i].launch(e->stream);
+    rc = e->launch_op(i, e->stream);
     if (rc) return rc;
-    VPB_CUDA_OK(cudaEventRecord(ev[i + 1], e->stream));
+    VPB_CUDA_OK(cudaEventRecord(ev[i + 1].get(), e->stream));
   }
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   for (int i = 0; i < n; ++i) {
-    VPB_CUDA_OK(cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]));
+    VPB_CUDA_OK(cudaEventElapsedTime(&ms[i], ev[i].get(), ev[i + 1].get()));
     if (flops) flops[i] = e->ops[i].flops;
     if (names) names[i] = e->ops[i].name.c_str();
     if (is_gemm) is_gemm[i] = e->ops[i].gemm ? e->ops[i].kind : 0;
   }
-  for (auto& x : ev) cudaEventDestroy(x);
   return VPB_OK;
 }
 

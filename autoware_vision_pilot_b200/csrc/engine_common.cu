@@ -108,29 +108,30 @@ namespace vpb {
 // =============================================================== frame graph
 static bool same_geometry(const vpb_frame& a, const vpb_frame& b) { return a.h == b.h && a.w == b.w && a.stride == b.stride; }
 
-int FrameGraph::run(cudaStream_t st, const Frames& f, int n_, const std::function<int(cudaStream_t)>& launch) {
-  bool same_geom = exec && n == n_, same_src = n == n_;
-  for (int k = 0; k < n_ && same_geom; ++k) same_geom = same_geometry(frames[k], f[k]);
-  for (int k = 0; k < n_ && same_src; ++k) same_src = frames[k].data == f[k].data;
+int FrameGraph::run(EngineRuntime& e) {
+  const cudaStream_t st = e.stream;
+  bool same_geom = exec && n == e.n_frames, same_src = n == e.n_frames;
+  for (int k = 0; k < e.n_frames && same_geom; ++k) same_geom = same_geometry(frames[k], e.frames[k]);
+  for (int k = 0; k < e.n_frames && same_src; ++k) same_src = frames[k].data == e.frames[k].data;
   if (same_geom && !same_src) {
     for (const auto& [i, node] : nodes) {
-      const int rc = ops[i].repoint(exec, node);
+      const int rc = e.ops[i].repoint(exec, node);
       if (rc) return rc;
     }
-    frames = f;
+    frames = e.frames;
     same_src = true;
   }
   if (!same_geom || !same_src) {
     invalidate();
     nodes.clear();
     n = 0;
-    int rc = launch(st);
+    int rc = e.launch_all(st);
     if (rc) return rc;
     VPB_CUDA_OK(cudaStreamSynchronize(st));
     cudaGraph_t g = nullptr;
     VPB_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     capturing = true;
-    rc = launch(st);
+    rc = e.launch_all(st);
     capturing = false;
     cudaError_t ce = cudaStreamEndCapture(st, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
@@ -139,7 +140,7 @@ int FrameGraph::run(cudaStream_t st, const Frames& f, int n_, const std::functio
     if (graph) cudaGraphDestroy(graph);
     graph = g;
     if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    frames = f; n = n_;
+    frames = e.frames; n = e.n_frames;
   }
   VPB_CUDA_OK(cudaGraphLaunch(exec, st));
   return VPB_OK;
@@ -157,6 +158,8 @@ void FrameGraph::release() {
 // =============================================================== engine runtime
 EngineRuntime::~EngineRuntime() {
   DeviceGuard guard(gpu_id);
+  for (cudaStream_t s : lane_streams) if (s) cudaStreamDestroy(s);
+  op_events.clear(); lane_done.clear();
   frame_graph.release();
   if (d_tap_scratch) cudaFree(d_tap_scratch);
   for (void* p : dev_allocs) cudaFree(p);
@@ -283,6 +286,58 @@ int EngineRuntime::launch_op(size_t i, cudaStream_t st) {
   }
   frame_graph.nodes.emplace_back(i, deps[0]);
   return VPB_OK;
+}
+
+int EngineRuntime::reset_call(cudaStream_t st) {
+  if (call_zero) VPB_CUDA_OK(cudaMemsetAsync(call_zero, 0, call_zero_bytes, st));
+  return VPB_OK;
+}
+
+static int prepare_lanes(EngineRuntime& e) {
+  const size_t nl = e.lane_dep.size();
+  if (e.lane_streams.size() == nl) return VPB_OK;
+  e.lane_streams.assign(nl, nullptr);
+  e.lane_done.resize(nl);
+  e.op_events.resize(e.ops.size());
+  for (size_t l = 1; l < nl; ++l) {
+    VPB_CUDA_OK(cudaStreamCreateWithFlags(&e.lane_streams[l], cudaStreamNonBlocking));
+    VPB_CUDA_OK(make_event(e.lane_done[l], cudaEventDisableTiming));
+    Event& dep = e.op_events[e.lane_dep[l]];
+    if (!dep) VPB_CUDA_OK(make_event(dep, cudaEventDisableTiming));
+  }
+  return VPB_OK;
+}
+
+int EngineRuntime::launch_all(cudaStream_t st) {
+  int rc = prepare_lanes(*this);
+  if (rc == VPB_OK) rc = reset_call(st);
+  if (rc) return rc;
+  const size_t nl = lane_dep.size();
+  if (nl <= 1 || single_stream) {
+    for (size_t i = 0; i < ops.size() && rc == VPB_OK; ++i) rc = launch_op(i, st);
+    return rc;
+  }
+  std::vector<char> started(nl, 0);
+  for (size_t i = 0; i < ops.size(); ++i) {
+    const int lane = ops[i].lane;
+    if (lane < 0) continue;                   // after the join
+    cudaStream_t s = lane == 0 ? st : lane_streams[lane];
+    if (lane > 0 && !started[lane]) {         // fork: wait for the producer of this lane's input
+      VPB_CUDA_OK(cudaStreamWaitEvent(s, op_events[lane_dep[lane]].get(), 0));
+      started[lane] = 1;
+    }
+    rc = launch_op(i, s);
+    if (rc) return rc;
+    if (op_events[i]) VPB_CUDA_OK(cudaEventRecord(op_events[i].get(), s));
+  }
+  for (size_t l = 1; l < nl; ++l) {           // join
+    if (!started[l]) continue;
+    VPB_CUDA_OK(cudaEventRecord(lane_done[l].get(), lane_streams[l]));
+    VPB_CUDA_OK(cudaStreamWaitEvent(st, lane_done[l].get(), 0));
+  }
+  for (size_t i = 0; i < ops.size() && rc == VPB_OK; ++i)
+    if (ops[i].lane < 0) rc = launch_op(i, st);
+  return rc;
 }
 
 vpb_conv_args EngineRuntime::conv_args(const Tens& in, const Tens* out, const Tens* res, int Cout, int taps, int phases,
@@ -469,13 +524,13 @@ bool EngineRuntime::find_tap(const char* name, Tap* out) const {
 int EngineRuntime::time_ops(const std::vector<OpRec>& list, const std::function<bool(const OpRec&)>& keep, int reps,
                             float* ms, double* flops, double* bytes, int* launches) {
   DeviceGuard guard(gpu_id);
-  cudaEvent_t a, b;
-  VPB_CUDA_OK(cudaEventCreate(&a));
-  VPB_CUDA_OK(cudaEventCreate(&b));
+  Event a, b;
+  VPB_CUDA_OK(make_event(a));
+  VPB_CUDA_OK(make_event(b));
   double fl = 0.0, by = 0.0;
   int n = 0;
   for (int r = -1; r < reps; ++r) {            // r = -1: untimed warm-up pass
-    if (r == 0) VPB_CUDA_OK(cudaEventRecord(a, stream));
+    if (r == 0) VPB_CUDA_OK(cudaEventRecord(a.get(), stream));
     for (const auto& op : list) {
       if (!keep(op)) continue;
       const int rc = op.launch(stream);
@@ -483,10 +538,9 @@ int EngineRuntime::time_ops(const std::vector<OpRec>& list, const std::function<
       if (r >= 0) { fl += op.flops; by += op.bytes; ++n; }
     }
   }
-  VPB_CUDA_OK(cudaEventRecord(b, stream));
+  VPB_CUDA_OK(cudaEventRecord(b.get(), stream));
   VPB_CUDA_OK(cudaStreamSynchronize(stream));
-  VPB_CUDA_OK(cudaEventElapsedTime(ms, a, b));
-  cudaEventDestroy(a); cudaEventDestroy(b);
+  VPB_CUDA_OK(cudaEventElapsedTime(ms, a.get(), b.get()));
   if (flops) *flops = fl;
   if (bytes) *bytes = by;
   if (launches) *launches = n;

@@ -1,8 +1,8 @@
 // engine_internal.h — host-side runtime shared by the engines (engine.cu: the four segmentation / depth / lane
 // networks; autospeed.cu: the AutoSpeed detector), defined in engine_common.cu: the .vpw weight-file reader,
-// shape-checked lookups, K-major repacking, the device guard, and EngineRuntime (device and stream set-up, device /
-// pinned allocations, weight uploads, activation tensors, the op list and its convolutions, the frame graph, the frame
-// calls, kernel timing, tap read-back).
+// shape-checked lookups, K-major repacking, the device guard, the event owner, and EngineRuntime (device and stream
+// set-up, device / pinned allocations, weight uploads, activation tensors, the op list and its convolutions, the
+// launcher of a call with its lanes and per-call reset, the frame graph, the frame calls, kernel timing, tap read-back).
 #pragma once
 #include <cuda_runtime.h>
 #include <array>
@@ -40,6 +40,16 @@ struct DeviceGuard {
   ~DeviceGuard() { if (changed) cudaSetDevice(prev); }
 };
 
+// RAII: a CUDA event destroyed with its owner, on every return path.  Empty until make_event succeeds.
+struct EventDeleter { void operator()(cudaEvent_t ev) const { cudaEventDestroy(ev); } };
+using Event = std::unique_ptr<CUevent_st, EventDeleter>;
+inline cudaError_t make_event(Event& e, unsigned flags = cudaEventDefault) {
+  cudaEvent_t ev = nullptr;
+  const cudaError_t ce = cudaEventCreateWithFlags(&ev, flags);
+  e.reset(ev);
+  return ce;
+}
+
 // NHWC 16-bit activation view.  p points at the first channel of the view; ld = channel stride of a pixel;
 // pad = 1: zero-bordered [(H+2)*(W+2)][ld]; lo: split-fp16 low half (same layout), NULL otherwise.
 struct Tens {
@@ -76,11 +86,10 @@ struct OpRec {
 // The frames of one call: descriptor k is sample k (entries past the batch are unused).
 using Frames = std::array<vpb_frame, kMaxBatch>;
 
-// The CUDA graph of one call of the launch list `ops`, keyed on the n (h, w, stride) triples and the frame pointers.
+struct EngineRuntime;
+// The CUDA graph of one call of a runtime's launch list, keyed on the n (h, w, stride) triples and the frame pointers.
 // Frames of the captured geometries in other buffers only re-point the captured nodes of the ops that have repoint.
 struct FrameGraph {
-  explicit FrameGraph(const std::vector<OpRec>& ops_) : ops(ops_) {}
-  const std::vector<OpRec>& ops;
   cudaGraph_t graph = nullptr;           // kept alive: the recorded nodes are handles into it
   cudaGraphExec_t exec = nullptr;
   bool capturing = false;                // inside run()'s capture: EngineRuntime::launch_op records nodes
@@ -88,10 +97,10 @@ struct FrameGraph {
   int n = 0;                             // the key: frames f[0 .. n-1] of the graph's last launch (0: none)
   Frames frames{};
 
-  // Launch the graph for frames f[0 .. n_-1] on st.  When the key differs in more than the frame pointers: launch(st)
-  // once outside capture (sets function attributes; its results are correct), capture launch(st) and instantiate.
-  // When only the pointers differ: ops[i].repoint(exec, node) for every recorded node.
-  int run(cudaStream_t st, const Frames& f, int n_, const std::function<int(cudaStream_t)>& launch);
+  // Launch the graph for e's frames on e's stream.  When the key differs in more than the frame pointers: e.launch_all
+  // once outside capture (sets function attributes; its results are correct), capture e.launch_all and instantiate.
+  // When only the pointers differ: e.ops[i].repoint(exec, node) for every recorded node.
+  int run(EngineRuntime& e);
   void invalidate();                     // the next run() captures again
   void release();
 };
@@ -101,7 +110,16 @@ struct ConvPlan;
 // What every engine owns: its device and stream, device / pinned allocations, the op list and the frame graph.
 struct EngineRuntime {
   int gpu_id = 0, dtype = VPB_F16;
+  // Execution lanes: a lane's ops run on their own stream, forked inside the frame graph after the op producing the
+  // tensor the lane consumes and joined on the engine stream, so the latency-bound small kernels of one network
+  // overlap with the other networks.
   int cur_lane = 0;                       // lane of the ops appended next
+  std::vector<int> lane_dep;              // [lane] producer op index; empty: no lanes were opened
+  std::vector<cudaStream_t> lane_streams; // [lane] for the lanes > 0; lane 0 is the engine stream
+  std::vector<Event> op_events, lane_done;   // [op], only for ops some lane waits on; [lane] its join
+  bool single_stream = false;             // the lanes run one after another on the engine stream
+  bool use_graph = true;                  // run_call replays the frame graph
+  void* call_zero = nullptr; size_t call_zero_bytes = 0;   // what a call zeroes before its first op
   // frames per call: every per-frame buffer holds `batch` samples back to back (sample outermost); weights, the launch
   // list and the graph are those of one call
   int batch = 1;
@@ -117,7 +135,7 @@ struct EngineRuntime {
   PreprocessPlan pre;
   Frames frames{};                        // device frames of the current / last call
   int n_frames = 0;                       // frames of that call (0: no call has run, or the last one failed)
-  FrameGraph frame_graph{ops};
+  FrameGraph frame_graph;
   uint8_t* d_frame = nullptr; size_t d_frame_cap = 0;           // device copy of the host frames
   float* d_tap_scratch = nullptr; size_t tap_scratch_cap = 0;   // read_tap staging (grown on demand)
 
@@ -143,8 +161,16 @@ struct EngineRuntime {
   // append the pre-process of the call's frames into out (+ the uint8 resized image out_u8, may be NULL) as op
   // "preprocess" on lane 0; the engines call it before their first op
   void add_preprocess(int convention, void* out, uint8_t* out_u8);
+  // the ops appended next form `lane`, which starts after ops[dep_op]
+  void begin_lane(int lane, int dep_op) { cur_lane = lane; lane_dep.resize(lane + 1); lane_dep[lane] = dep_op; }
   // launch ops[i] on st; while frame_graph captures, an op with repoint records its kernel node
   int launch_op(size_t i, cudaStream_t st);
+  int reset_call(cudaStream_t st);        // zero call_zero on st: a memset, not an op
+  // One call on st: reset_call; the ops of lanes >= 0 in list order, lane l > 0 on its own stream after waiting for
+  // ops[lane_dep[l]]; the joins in lane order; the ops of lane -1.  One lane or single_stream: every op on st in order.
+  int launch_all(cudaStream_t st);
+  // launch_all through the frame graph (use_graph) or on the engine stream
+  int run_call() { return use_graph ? frame_graph.run(*this) : launch_all(stream); }
   // vpb_conv_args of a convolution in -> out (+ res, + the second input in2 with weights w2) from the views: shapes,
   // ld, pad, the split low halves and the batch.  3x3 on a zero-bordered input runs LINEAR (the layer also writes its
   // output's zero border, so the next 3x3 layer reads it as it stands), everything else and the split-fp16 mode
@@ -164,7 +190,8 @@ struct EngineRuntime {
   long read_tap(const char* name, float* dst, long cap, int* c, int* h, int* w);
   // Device time of the ops of `list` keep() selects, launched back to back on the engine stream: one untimed warm-up
   // pass, then `reps` passes between one event pair, then a synchronise.  flops / bytes / launches (each may be NULL)
-  // are summed over the timed passes.
+  // are summed over the timed passes.  No reset_call: the SE ops read whatever the accumulators hold, and their cost
+  // does not depend on it.
   int time_ops(const std::vector<OpRec>& list, const std::function<bool(const OpRec&)>& keep, int reps, float* ms,
                double* flops, double* bytes, int* launches);
 

@@ -349,16 +349,15 @@ extern "C" int vp_multicam_time_allgather(vp_multicam* mc, int reps, float* ms_t
     return VPB_ERR_STATE;
   }
   DeviceGuard g(mc->gpu_id);
-  cudaEvent_t a, b;
-  VPB_CUDA_OK(cudaEventCreate(&a));
-  VPB_CUDA_OK(cudaEventCreate(&b));
+  Event a, b;
+  VPB_CUDA_OK(make_event(a));
+  VPB_CUDA_OK(make_event(b));
   int rc = multicam_allgather(mc);                 // untimed warm-up (connection setup on first use)
   if (rc) return rc;
-  VPB_CUDA_OK(cudaEventRecord(a, mc->stream));
+  VPB_CUDA_OK(cudaEventRecord(a.get(), mc->stream));
   for (int i = 0; i < reps; ++i) { rc = multicam_allgather(mc); if (rc) return rc; }
-  VPB_CUDA_OK(cudaEventRecord(b, mc->stream));
+  VPB_CUDA_OK(cudaEventRecord(b.get(), mc->stream));
   VPB_CUDA_OK(cudaStreamSynchronize(mc->stream));
-  VPB_CUDA_OK(cudaEventElapsedTime(ms_total, a, b));
-  cudaEventDestroy(a); cudaEventDestroy(b);
+  VPB_CUDA_OK(cudaEventElapsedTime(ms_total, a.get(), b.get()));
   return VPB_OK;
 }

@@ -31,6 +31,7 @@
 #include <algorithm>
 #include <cmath>
 #include <functional>
+#include <initializer_list>
 #include <memory>
 #include <string>
 #include <vector>
@@ -363,6 +364,136 @@ __global__ void fill_canvas_kernel(typename E::T* __restrict__ x, int npix) {
   for (int c = 0; c < 8; ++c) x[static_cast<size_t>(i) * 8 + c] = c < 3 ? g : z;
 }
 
+// ------------------------------------------------------------------ launchers
+// One launcher per SIMT kernel, shared by the engine's ops and the op-level entry points of vp_b200_autospeed.h, so the
+// entry points run exactly the engine's launches (grid, block, scratch size, single-image or batched code).  Each checks
+// the preconditions its kernel assumes and returns VPB_ERR_ARG with a message before any device work.
+static bool batch_ok(const char* op, int batch) {
+  if (batch >= 1 && batch <= kMaxBatch) return true;
+  vpb_set_error("%s: batch %d (1..%d)", op, batch, kMaxBatch);
+  return false;
+}
+static bool ptrs_ok(const char* op, std::initializer_list<const void*> ps) {
+  for (const void* p : ps)
+    if (!p) { vpb_set_error("%s: NULL pointer", op); return false; }
+  return true;
+}
+// upsample / max-pool move 8 channels per 16-byte access
+static bool vec8_ok(const char* op, int C, std::initializer_list<int> lds, std::initializer_list<const void*> ps) {
+  bool ok = C >= 8 && C % 8 == 0;
+  for (int ld : lds) ok = ok && ld % 8 == 0 && ld >= C;
+  for (const void* p : ps) ok = ok && reinterpret_cast<uintptr_t>(p) % 16 == 0;
+  if (!ok) vpb_set_error("%s: C=%d and ld must be multiples of 8 (ld >= C), pointers 16-byte aligned", op, C);
+  return ok;
+}
+
+// blocks of the mean's first stage: one per 64 pixels, at most 148 (a constant kept from the first version of the CTX
+// block, not tuned for the H100)
+static int as_mean_blocks(int HW) { return std::min(148, std::max(1, HW / 64)); }
+
+static int as_mean_x(int dt, const void* in, int HW, int C, int ld, float* part, float* out, int nb, cudaStream_t st) {
+  const char* op = "as_mean";
+  if (!batch_ok(op, nb) || !ptrs_ok(op, {in, part, out})) return VPB_ERR_ARG;
+  // ppb = 256 / C pixels per pass: C > 256 would make it 0 and the mean silently zero
+  if (C < 1 || C > 256 || HW < 1 || ld < C) { vpb_set_error("%s: HW=%d C=%d ld=%d (C 1..256, ld >= C)", op, HW, C, ld); return VPB_ERR_ARG; }
+  const int nblk = as_mean_blocks(HW);
+  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+    using E = decltype(tag);
+    return launch_k(nb > 1 ? mean_part_kernel<E, true> : mean_part_kernel<E, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const typename E::T*>(in), HW, C, ld, part);
+  }));
+  VPB_CUDA_OK(launch_k(nb > 1 ? mean_final_kernel<true> : mean_final_kernel<false>, dim3((C + 127) / 128, nb), dim3(128), 0, st, static_cast<const float*>(part), nblk, C, 1.0f / HW, out));
+  return VPB_OK;
+}
+
+static int as_upsample2_x(int dt, const void* in, int H, int W, int C, int ld_in, void* out, int ld_out, int nb, cudaStream_t st) {
+  const char* op = "as_upsample2";
+  if (!batch_ok(op, nb) || !ptrs_ok(op, {in, out}) || !vec8_ok(op, C, {ld_in, ld_out}, {in, out})) return VPB_ERR_ARG;
+  if (H < 1 || W < 1) { vpb_set_error("%s: H=%d W=%d", op, H, W); return VPB_ERR_ARG; }
+  const long n = 4L * H * W * (C / 8);
+  const dim3 g(static_cast<unsigned>((n + 255) / 256), nb), b(256);
+  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+    using E = decltype(tag);
+    return launch_k(nb > 1 ? upsample2_kernel<E, true> : upsample2_kernel<E, false>, g, b, 0, st, static_cast<const uint4*>(in), H, W, C / 8, ld_in / 8, static_cast<uint4*>(out), ld_out / 8);
+  }));
+  return VPB_OK;
+}
+
+static int as_maxpool5_x(int dt, const void* in, int H, int W, int C, int ld, void* out, int nb, cudaStream_t st) {
+  const char* op = "as_maxpool5";
+  if (!batch_ok(op, nb) || !ptrs_ok(op, {in, out}) || !vec8_ok(op, C, {ld}, {in, out})) return VPB_ERR_ARG;
+  if (H < 1 || W < 1) { vpb_set_error("%s: H=%d W=%d", op, H, W); return VPB_ERR_ARG; }
+  const dim3 g((H * W * (C / 8) + 255) / 256, nb), b(256);
+  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+    using E = decltype(tag);
+    return launch_k(nb > 1 ? maxpool5_kernel<E, true> : maxpool5_kernel<E, false>, g, b, 0, st, static_cast<const uint4*>(in), H, W, C / 8, ld / 8, static_cast<uint4*>(out));
+  }));
+  return VPB_OK;
+}
+
+static int as_split_v_x(int dt, const void* qkv, int T, int nh, int dk, int dh, void* vc, void* vt, int nb, cudaStream_t st) {
+  const char* op = "as_split_v";
+  if (!batch_ok(op, nb) || !ptrs_ok(op, {qkv, vc, vt})) return VPB_ERR_ARG;
+  if (T < 1 || nh < 1 || dk < 0 || dh < 1) { vpb_set_error("%s: T=%d nh=%d dk=%d dh=%d", op, T, nh, dk, dh); return VPB_ERR_ARG; }
+  const dim3 g((T * nh * dh + 255) / 256, nb), b(256);
+  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+    using E = decltype(tag);
+    using T16 = typename E::T;
+    return launch_k(nb > 1 ? split_v_kernel<E, true> : split_v_kernel<E, false>, g, b, 0, st, static_cast<const T16*>(qkv), T, nh, dk, dh, static_cast<T16*>(vc), static_cast<T16*>(vt));
+  }));
+  return VPB_OK;
+}
+
+static int as_softmax_rows_x(int dt, const void* s, int rows, int cols, float scale, void* p, cudaStream_t st) {
+  const char* op = "as_softmax_rows";
+  if (!ptrs_ok(op, {s, p})) return VPB_ERR_ARG;
+  // one warp holds a row in 16 registers per lane
+  if (rows < 1 || cols < 1 || cols > 512) { vpb_set_error("%s: rows=%d cols=%d (cols 1..512)", op, rows, cols); return VPB_ERR_ARG; }
+  const dim3 g((rows + 7) / 8), b(256);
+  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+    using E = decltype(tag);
+    return launch_k(softmax_rows_kernel<E>, g, b, 0, st, static_cast<const typename E::T*>(s), rows, cols, scale, static_cast<typename E::T*>(p));
+  }));
+  return VPB_OK;
+}
+
+static int as_decode_x(int dt, const void* lvl, int h, int w, int ld, float stride, int a0, int NA, float* out, int nb,
+                       cudaStream_t st) {
+  const char* op = "as_decode";
+  if (!batch_ok(op, nb) || !ptrs_ok(op, {lvl, out})) return VPB_ERR_ARG;
+  if (h < 1 || w < 1 || ld < 4 * kDfl + kNC || a0 < 0 || a0 + h * w > NA) {
+    vpb_set_error("%s: h=%d w=%d ld=%d a0=%d NA=%d (ld >= %d, a0 + h*w <= NA)", op, h, w, ld, a0, NA, 4 * kDfl + kNC);
+    return VPB_ERR_ARG;
+  }
+  const dim3 g((h * w + 127) / 128, nb), bb(128);
+  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+    using E = decltype(tag);
+    return launch_k(nb > 1 ? decode_kernel<E, true> : decode_kernel<E, false>, g, bb, 0, st, static_cast<const typename E::T*>(lvl), h, w, ld, stride, a0, NA, out);
+  }));
+  return VPB_OK;
+}
+
+// Every buffer holds NA entries per image, so no candidate and no detection is ever cut; the dead flags (one byte per
+// candidate) live in shared memory, NA <= kNA keeps them under the 48 KB default.
+static int as_postprocess_x(const float* raw, int NA, int nb, float conf, float iou, const float* scale, const int* pad_x,
+                            const int* pad_y, const int* orig_w, const int* orig_h, float* cand, int* order, float* det,
+                            int* counts, cudaStream_t st) {
+  const char* op = "as_postprocess";
+  if (!batch_ok(op, nb) || !ptrs_ok(op, {raw, scale, pad_x, pad_y, orig_w, orig_h, cand, order, det, counts})) return VPB_ERR_ARG;
+  if (NA < 1 || NA > kNA) { vpb_set_error("%s: NA=%d (1..%d)", op, NA, kNA); return VPB_ERR_ARG; }
+  PostParams pp{};
+  pp.raw = raw; pp.NA = NA; pp.conf = conf; pp.iou = iou;
+  for (int k = 0; k < nb; ++k) {
+    if (!(scale[k] > 0.f)) { vpb_set_error("%s: image %d: scale %g", op, k, scale[k]); return VPB_ERR_ARG; }
+    pp.scale[k] = scale[k]; pp.pad_x[k] = pad_x[k]; pp.pad_y[k] = pad_y[k]; pp.orig_w[k] = orig_w[k]; pp.orig_h[k] = orig_h[k];
+  }
+  pp.max_cand = NA; pp.max_det = NA;
+  pp.cand = cand; pp.order = order; pp.det = det; pp.counts = counts;
+  const size_t smem = NA;                      // s_dead
+  if (nb > 1) VPB_CUDA_OK(launch_k(postprocess_kernel<true>, dim3(nb), dim3(1024), smem, st, pp));
+  else VPB_CUDA_OK(launch_k(postprocess_kernel<false>, dim3(1), dim3(1024), smem, st, pp));
+  return VPB_OK;
+}
+
 }  // namespace vpb
 
 using namespace vpb;
@@ -379,11 +510,15 @@ struct vp_autospeed : EngineRuntime {
   float scale[kMaxBatch] = {};             // letterbox of each sample of the last call (geometry in pre.geom)
   PreGeom canvas_geom[kMaxBatch];          // the letterbox each sample's canvas border was last filled for
   float conf = 0.6f, iou = 0.45f;
-  static constexpr int kMaxCand = 4096, kMaxDet = 1024;
+  // Candidates and detections have room for every anchor (no threshold cuts the NMS short).  fetch copies the first
+  // kDetFetch detections of each sample, which hold every detection at the default thresholds; fetch_rest copies the
+  // others of a sample that has more, after the call has completed.
+  static constexpr int kDetFetch = 1024;
 
   int geoms(const vpb_frame* frames, const char* who, PreGeom* g) override;
   int enqueue(const PreGeom* g) override;
   int fetch(bool raw) override;
+  int fetch_rest();
 };
 
 namespace vpb {
@@ -467,20 +602,13 @@ struct ASBuilder {
     const HostTensor *c0w = find_w_shaped(w, p + ".ctx0.weight", {C / 2, 1, 3, 3}), *c0b = find_w_shaped(w, p + ".ctx0.bias", {C / 2});
     if (!ew || !eb || !c0w || !c0b) { rc = VPB_ERR_IO; return; }
     // mean over H x W
-    const int nblk = std::min(148, std::max(1, HW / 64));
-    float* d_part = static_cast<float*>(e.dalloc(static_cast<size_t>(nblk) * C * 4 * nb));
+    float* d_part = static_cast<float*>(e.dalloc(static_cast<size_t>(as_mean_blocks(HW)) * C * 4 * nb));
     float* d_mean = static_cast<float*>(e.dalloc(static_cast<size_t>(C) * 4 * nb));
     {
       const void* ip = x.p; const int ld = x.ld;
       // two launches; the partial sums and the means are small next to the activation read
-      e.add_op(p + ".mean", "mean_part_kernel", [=](cudaStream_t st) {
-        VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
-          using E = decltype(tag);
-          return launch_k(nb > 1 ? mean_part_kernel<E, true> : mean_part_kernel<E, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const typename E::T*>(ip), HW, C, ld, d_part);
-        }));
-        VPB_CUDA_OK(launch_k(nb > 1 ? mean_final_kernel<true> : mean_final_kernel<false>, dim3((C + 127) / 128, nb), dim3(128), 0, st, static_cast<const float*>(d_part), nblk, C, 1.0f / HW, d_mean));
-        return VPB_OK;
-      }, 0.0, nb * 2.0 * HW * C);
+      e.add_op(p + ".mean", "mean_part_kernel", [=](cudaStream_t st) { return as_mean_x(dt, ip, HW, C, ld, d_part, d_mean, nb, st); },
+               0.0, nb * 2.0 * HW * C);
     }
     // exp0: Conv1d(k=3, pad 1) on a length-1 sequence == the centre tap as a Linear(C -> h*w); SiLU twice (:218-221)
     std::vector<float> lw(static_cast<size_t>(HW) * C);
@@ -530,29 +658,16 @@ struct ASBuilder {
     cbs(p + ".conv2", cat, out, cout, 1, 1, true);
   }
   void upsample(const std::string& name, const Tens& in, const Tens& out) {
-    const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, li = in.ld / 8, lo = out.ld / 8, nb = e.batch;
+    const int dt = e.dtype, H = in.H, W = in.W, C = in.C, li = in.ld, lo = out.ld, nb = e.batch;
     const void* ip = in.p; void* op_ = out.p;
-    const long n = 4L * H * W * C8;
-    e.add_op(name, "upsample2_kernel", [=](cudaStream_t st) {
-      const dim3 g(static_cast<unsigned>((n + 255) / 256), nb), b(256);
-      VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
-        using E = decltype(tag);
-        return launch_k(nb > 1 ? upsample2_kernel<E, true> : upsample2_kernel<E, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, li, static_cast<uint4*>(op_), lo);
-      }));
-      return VPB_OK;
-    }, 0.0, nb * 80.0 * H * W * C8);
+    e.add_op(name, "upsample2_kernel", [=](cudaStream_t st) { return as_upsample2_x(dt, ip, H, W, C, li, op_, lo, nb, st); },
+             0.0, nb * 10.0 * H * W * C);
   }
   void maxpool(const std::string& name, const Tens& in, const Tens& out) {
-    const int dt = e.dtype, H = in.H, W = in.W, C8 = in.C / 8, ld8 = in.ld / 8, nb = e.batch;
+    const int dt = e.dtype, H = in.H, W = in.W, C = in.C, ld = in.ld, nb = e.batch;
     const void* ip = in.p; void* op_ = out.p;
-    e.add_op(name, "maxpool5_kernel", [=](cudaStream_t st) {
-      const dim3 g((H * W * C8 + 255) / 256, nb), b(256);
-      VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
-        using E = decltype(tag);
-        return launch_k(nb > 1 ? maxpool5_kernel<E, true> : maxpool5_kernel<E, false>, g, b, 0, st, static_cast<const uint4*>(ip), H, W, C8, ld8, static_cast<uint4*>(op_));
-      }));
-      return VPB_OK;
-    }, 0.0, nb * 32.0 * H * W * C8);
+    e.add_op(name, "maxpool5_kernel", [=](cudaStream_t st) { return as_maxpool5_x(dt, ip, H, W, C, ld, op_, nb, st); },
+             0.0, nb * 4.0 * H * W * C);
   }
   // PSABlock on y (in place): y += attention(y); y += ffn(y)   (common_layers.py:77-118)
   void psablock(const std::string& p, const Tens& y, int nh) {
@@ -564,15 +679,8 @@ struct ASBuilder {
     void* vt = e.dalloc(static_cast<size_t>(nh) * dh * T * 2 * nb);          // [N][nh][dh][T]
     {
       const void* q = qkv.p; void* vcp = vc.p;
-      e.add_op(p + ".split_v", "split_v_kernel", [=](cudaStream_t st) {
-        const dim3 g((T * nh * dh + 255) / 256, nb), b(256);
-        VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
-          using E = decltype(tag);
-          using T16 = typename E::T;
-          return launch_k(nb > 1 ? split_v_kernel<E, true> : split_v_kernel<E, false>, g, b, 0, st, static_cast<const T16*>(q), T, nh, dk, dh, static_cast<T16*>(vcp), static_cast<T16*>(vt));
-        }));
-        return VPB_OK;
-      }, 0.0, nb * 6.0 * T * nh * dh);
+      e.add_op(p + ".split_v", "split_v_kernel", [=](cudaStream_t st) { return as_split_v_x(dt, q, T, nh, dk, dh, vcp, vt, nb, st); },
+               0.0, nb * 6.0 * T * nh * dh);
     }
     Tens dwv = e.act_alloc(y.H, y.W, C);
     dw(p + ".conv1.conv1", vc, dwv, false);                     // positional term: depthwise 3x3 on v, no activation
@@ -591,14 +699,8 @@ struct ASBuilder {
       if (!ok()) return;
       {
         const void* sp = s.p; void* pp = pm.p;
-        e.add_op(p + ".attn.softmax" + std::to_string(h), "softmax_rows_kernel", [=](cudaStream_t st) {
-          const dim3 g((nb * T + 7) / 8), b(256);
-          VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
-            using E = decltype(tag);
-            return launch_k(softmax_rows_kernel<E>, g, b, 0, st, static_cast<const typename E::T*>(sp), nb * T, T, scale, static_cast<typename E::T*>(pp));
-          }));
-          return VPB_OK;
-        }, 0.0, nb * 4.0 * T * T);
+        e.add_op(p + ".attn.softmax" + std::to_string(h), "softmax_rows_kernel",
+                 [=](cudaStream_t st) { return as_softmax_rows_x(dt, sp, nb * T, T, scale, pp, st); }, 0.0, nb * 4.0 * T * T);
       }
       // O = P V^T (+ depthwise term): Cin = key tokens, "weights" = Vt[h] [dh][T] of the same sample
       Tens o = att.slice(h * dh, dh); o.H = 1; o.W = T;
@@ -697,14 +799,9 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
     for (int i = 0; i < 3; ++i) {
       const void* lp = lv[i].p; const int h = lv[i].H, wd = lv[i].W, ld = lv[i].ld, off = a0; const float st_ = strides[i];
       // 4 * kDfl box and kNC class logits read, 8 fp32 written per anchor
-      e.add_op("head.decode" + std::to_string(i), "decode_kernel", [=](cudaStream_t st) {
-        const dim3 g((h * wd + 127) / 128, nb), bb(128);
-        VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
-          using E = decltype(tag);
-          return launch_k(nb > 1 ? decode_kernel<E, true> : decode_kernel<E, false>, g, bb, 0, st, static_cast<const typename E::T*>(lp), h, wd, ld, st_, off, kNA, raw);
-        }));
-        return VPB_OK;
-      }, 0.0, nb * (2.0 * (4 * kDfl + kNC) + 32.0) * h * wd);
+      e.add_op("head.decode" + std::to_string(i), "decode_kernel",
+               [=](cudaStream_t st) { return as_decode_x(dt, lp, h, wd, ld, st_, off, kNA, raw, nb, st); }, 0.0,
+               nb * (2.0 * (4 * kDfl + kNC) + 32.0) * h * wd);
       a0 += h * wd;
     }
   }
@@ -712,18 +809,13 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   {
     vp_autospeed* ep = &e;
     e.add_op("postprocess", "postprocess_kernel", [ep](cudaStream_t st) {
-      PostParams pp{};
-      pp.raw = ep->d_raw; pp.NA = kNA; pp.conf = ep->conf; pp.iou = ep->iou;
+      int pad_x[kMaxBatch], pad_y[kMaxBatch], orig_w[kMaxBatch], orig_h[kMaxBatch];
       for (int k = 0; k < ep->batch; ++k) {
         const PreGeom& g = ep->pre.geom[k];
-        pp.scale[k] = ep->scale[k]; pp.pad_x[k] = g.x0; pp.pad_y[k] = g.y0; pp.orig_w[k] = g.w; pp.orig_h[k] = g.h;
+        pad_x[k] = g.x0; pad_y[k] = g.y0; orig_w[k] = g.w; orig_h[k] = g.h;
       }
-      pp.max_cand = vp_autospeed::kMaxCand; pp.max_det = vp_autospeed::kMaxDet;
-      pp.cand = ep->d_cand; pp.order = ep->d_order; pp.det = ep->d_det; pp.counts = ep->d_counts;
-      const size_t smem = vp_autospeed::kMaxCand;
-      if (ep->batch > 1) VPB_CUDA_OK(launch_k(postprocess_kernel<true>, dim3(ep->batch), dim3(1024), smem, st, pp));
-      else VPB_CUDA_OK(launch_k(postprocess_kernel<false>, dim3(1), dim3(1024), smem, st, pp));
-      return VPB_OK;
+      return as_postprocess_x(ep->d_raw, kNA, ep->batch, ep->conf, ep->iou, ep->scale, pad_x, pad_y, orig_w, orig_h,
+                              ep->d_cand, ep->d_order, ep->d_det, ep->d_counts, st);
     });
   }
   e.tap("p1", p1); e.tap("p2", p2); e.tap("p3", p3); e.tap("p4", p4); e.tap("p5_ctx", q5); e.tap("p5_sppf", s5);
@@ -778,8 +870,24 @@ int vp_autospeed::enqueue(const PreGeom* g) {
 int vp_autospeed::fetch(bool raw) {
   const size_t nb = batch;
   VPB_CUDA_OK(cudaMemcpyAsync(h_counts, d_counts, 8 * nb, cudaMemcpyDeviceToHost, stream));
-  VPB_CUDA_OK(cudaMemcpyAsync(h_det, d_det, static_cast<size_t>(kMaxDet) * 6 * 4 * nb, cudaMemcpyDeviceToHost, stream));
+  const size_t pitch = static_cast<size_t>(kNA) * 6 * 4;
+  VPB_CUDA_OK(cudaMemcpy2DAsync(h_det, pitch, d_det, pitch, static_cast<size_t>(kDetFetch) * 6 * 4, nb, cudaMemcpyDeviceToHost, stream));
   if (raw) VPB_CUDA_OK(cudaMemcpyAsync(h_raw, d_raw, static_cast<size_t>(8) * kNA * 4 * nb, cudaMemcpyDeviceToHost, stream));
+  return VPB_OK;
+}
+
+// after fetch and a synchronise: the detections past the first kDetFetch of every sample that has more
+int vp_autospeed::fetch_rest() {
+  DeviceGuard guard(gpu_id);
+  bool copied = false;
+  for (int k = 0; k < batch; ++k) {
+    const int n = h_counts[2 * k];
+    if (n <= kDetFetch) continue;
+    const size_t off = (static_cast<size_t>(k) * kNA + kDetFetch) * 6;
+    VPB_CUDA_OK(cudaMemcpyAsync(h_det + off, d_det + off, static_cast<size_t>(n - kDetFetch) * 6 * 4, cudaMemcpyDeviceToHost, stream));
+    copied = true;
+  }
+  if (copied) VPB_CUDA_OK(cudaStreamSynchronize(stream));
   return VPB_OK;
 }
 
@@ -803,11 +911,11 @@ static int as_create(const char* who, const char* weights_vpw, int gpu_id, int d
   for (int k = 0; k < batch; ++k) e->canvas_geom[k].h = -1;   // no border filled yet
   e->d_raw = static_cast<float*>(e->dalloc(static_cast<size_t>(8) * kNA * 4 * nb));
   e->h_raw = static_cast<float*>(e->halloc(static_cast<size_t>(8) * kNA * 4 * nb));
-  e->d_cand = static_cast<float*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxCand) * 6 * 4 * nb));
-  e->d_order = static_cast<int*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxCand) * 4 * nb));
-  e->d_det = static_cast<float*>(e->dalloc(static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4 * nb));
+  e->d_cand = static_cast<float*>(e->dalloc(static_cast<size_t>(kNA) * 6 * 4 * nb));
+  e->d_order = static_cast<int*>(e->dalloc(static_cast<size_t>(kNA) * 4 * nb));
+  e->d_det = static_cast<float*>(e->dalloc(static_cast<size_t>(kNA) * 6 * 4 * nb));
   e->d_counts = static_cast<int*>(e->dalloc(64 * nb));
-  e->h_det = static_cast<float*>(e->halloc(static_cast<size_t>(vp_autospeed::kMaxDet) * 6 * 4 * nb));
+  e->h_det = static_cast<float*>(e->halloc(static_cast<size_t>(kNA) * 6 * 4 * nb));
   e->h_counts = static_cast<int*>(e->halloc(64 * nb));
   if (e->oom || !e->h_raw || !e->h_det || !e->h_counts) return VPB_ERR_CUDA;
   WeightMap w;
@@ -825,7 +933,8 @@ static int as_infer_host_batch(vp_autospeed* e, const uint8_t* const* frames, in
                                int fetch_raw, const char* who) {
   Frames f;
   if (!batch_frames(e, frames, n, h, w, stride, who, f)) return VPB_ERR_ARG;
-  return call_host(e, f.data(), n, true, fetch_raw != 0, who);
+  const int rc = call_host(e, f.data(), n, true, fetch_raw != 0, who);
+  return rc ? rc : e->fetch_rest();
 }
 
 static bool sample_ok(const vp_autospeed* e, int sample, const char* who) {
@@ -866,7 +975,8 @@ extern "C" int vp_autospeed_infer_batch(vp_autospeed* e, const uint8_t* const* f
 }
 
 extern "C" int vp_autospeed_infer_frames(vp_autospeed* e, const vpb_frame* frames_host, int n, int fetch_raw) {
-  return call_host(e, frames_host, n, true, fetch_raw != 0, "vp_autospeed_infer_frames");
+  const int rc = call_host(e, frames_host, n, true, fetch_raw != 0, "vp_autospeed_infer_frames");
+  return rc ? rc : e->fetch_rest();
 }
 
 extern "C" int vp_autospeed_infer_device_batch(vp_autospeed* e, const uint8_t* const* frames_dev, int n, int h, int w,
@@ -889,13 +999,13 @@ extern "C" int vp_autospeed_sync(vp_autospeed* e, int fetch) {
   DeviceGuard guard(e->gpu_id);
   if (fetch) { int rc = e->fetch(fetch > 1); if (rc) return rc; }
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return VPB_OK;
+  return fetch ? e->fetch_rest() : VPB_OK;
 }
 
 extern "C" int vp_autospeed_detections_at(vp_autospeed* e, int sample, const float** det, int* n, int* n_candidates) {
   if (!e || !det || !n) return VPB_ERR_ARG;
   if (!sample_ok(e, sample, "vp_autospeed_detections")) return VPB_ERR_ARG;
-  *det = e->h_det + static_cast<size_t>(sample) * vp_autospeed::kMaxDet * 6; *n = e->h_counts[2 * sample];
+  *det = e->h_det + static_cast<size_t>(sample) * kNA * 6; *n = e->h_counts[2 * sample];
   if (n_candidates) *n_candidates = e->h_counts[2 * sample + 1];
   return VPB_OK;
 }
@@ -934,4 +1044,41 @@ extern "C" int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flop
 extern "C" long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {
   if (!e || !name) return VPB_ERR_ARG;
   return e->read_tap(name, dst, cap, c, h, w);
+}
+
+// ---- op level: the engine's launchers (vpb::as_*_x) on caller buffers
+extern "C" int vpb_as_mean_blocks(int HW) { return as_mean_blocks(HW); }
+
+extern "C" int vpb_as_mean(int dtype, const void* in, int HW, int C, int ld, float* part, float* out, int batch, void* stream) {
+  return as_mean_x(dtype, in, HW, C, ld, part, out, batch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_upsample2(int dtype, const void* in, int H, int W, int C, int ld_in, void* out, int ld_out, int batch,
+                                void* stream) {
+  return as_upsample2_x(dtype, in, H, W, C, ld_in, out, ld_out, batch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_maxpool5(int dtype, const void* in, int H, int W, int C, int ld, void* out, int batch, void* stream) {
+  return as_maxpool5_x(dtype, in, H, W, C, ld, out, batch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_split_v(int dtype, const void* qkv, int T, int nh, int dk, int dh, void* vc, void* vt, int batch,
+                              void* stream) {
+  return as_split_v_x(dtype, qkv, T, nh, dk, dh, vc, vt, batch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_softmax_rows(int dtype, const void* s, int rows, int cols, float scale, void* p, void* stream) {
+  return as_softmax_rows_x(dtype, s, rows, cols, scale, p, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_decode(int dtype, const void* lvl, int h, int w, int ld, float stride, int a0, int NA, float* out,
+                             int batch, void* stream) {
+  return as_decode_x(dtype, lvl, h, w, ld, stride, a0, NA, out, batch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_postprocess(const float* raw, int NA, int batch, float conf, float iou, const float* scale,
+                                  const int* pad_x, const int* pad_y, const int* orig_w, const int* orig_h, float* cand,
+                                  int* order, float* det, int* counts, void* stream) {
+  return as_postprocess_x(raw, NA, batch, conf, iou, scale, pad_x, pad_y, orig_w, orig_h, cand, order, det, counts,
+                          static_cast<cudaStream_t>(stream));
 }

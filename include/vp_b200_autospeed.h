@@ -65,7 +65,8 @@ int vp_autospeed_infer_device_frames(vp_autospeed* e, const vpb_frame* frames_de
 int vp_autospeed_sync(vp_autospeed* e, int fetch);
 
 /* det: engine-owned host buffer [n][6] = x1, y1, x2, y2, score, class (descending score, as torchvision.ops.nms
- * orders them); n_candidates (optional) = anchors that passed the confidence filter. Valid until the next inference. */
+ * orders them); n_candidates (optional) = anchors that passed the confidence filter. Valid until the next inference.
+ * Nothing is cut: every candidate enters the NMS and n can reach n_candidates (at most the 10752 anchors). */
 int vp_autospeed_detections(vp_autospeed* e, const float** det, int* n, int* n_candidates);
 /* raw prediction tensor, fp32 planar [channels = 8][anchors = 10752]: cx, cy, w, h (canvas pixels), 4 class scores */
 int vp_autospeed_raw(vp_autospeed* e, const float** raw_host, const float** raw_dev, int* channels, int* anchors);
@@ -78,6 +79,47 @@ int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flops);
 /* intermediate tensors for the parity tests ("canvas", "p1".."p5", "p5_ctx", "p5_sppf", "n3".."n5", "head0".."head2";
  * "<name>@k" = sample k, default 0) as fp32 NCHW; returns the element count (dst == NULL: size query) */
 long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* dst, long cap, int* c, int* h, int* w);
+
+/* ---- op level: the detector's SIMT kernels, launched exactly as the engine launches them ----
+ * Conventions of vp_b200_ops.h: DEVICE pointers (the postprocess letterbox arrays are HOST arrays), dtype VPB_F16 |
+ * VPB_BF16 for the 16-bit tensors, NHWC activations, `batch` 1..VP_MAX_BATCH images stored back to back in every tensor
+ * (each image's result is bit-identical to a batch-1 call on it).  Arguments outside a contract (including NULL
+ * pointers) return VPB_ERR_ARG with a message before any device work.  Citations are to the reference repo. */
+/* mean over H*W per channel (CTX block, common_layers.py:214), fp32, in two fixed-order stages:
+ * in [batch][HW][ld] (C 1..256, ld >= C) -> part [batch][vpb_as_mean_blocks(HW)][C] fp32 scratch -> out [batch][C] fp32.
+ * vpb_as_mean_blocks(HW) = min(148, max(1, HW / 64)) blocks, block b summing pixels [b*chunk, (b+1)*chunk),
+ * chunk = ceil(HW / blocks). */
+int vpb_as_mean_blocks(int HW);
+int vpb_as_mean(int dtype, const void* in, int HW, int C, int ld, float* part, float* out, int batch, void* stream);
+/* nn.Upsample(scale_factor=2, nearest) (auto_speed_neck.py:10): in [batch][H][W][ld_in] -> out [batch][2H][2W][ld_out],
+ * channels 0..C-1 of each row (a channel slice of a wider concat tensor); the rest of out is not written.
+ * C, ld_in, ld_out multiples of 8 (>= C), in / out 16-byte aligned. */
+int vpb_as_upsample2(int dtype, const void* in, int H, int W, int C, int ld_in, void* out, int ld_out, int batch,
+                     void* stream);
+/* MaxPool2d(5, stride 1, padding 2) (SPPF, common_layers.py:249), channel slice -> channel slice of one ld:
+ * in / out [batch][H][W][ld], channels 0..C-1; C and ld multiples of 8, pointers 16-byte aligned.
+ * Unlike torch, a NaN input is dropped (fmaxf), not propagated. */
+int vpb_as_maxpool5(int dtype, const void* in, int H, int W, int C, int ld, void* out, int batch, void* stream);
+/* attention V split (common_layers.py:95-102): qkv [batch][T][nh*(2dk+dh)] (per head q | k | v) ->
+ * vc [batch][T][nh*dh] (token-major) and vt [batch][nh][dh][T] (key-token-major) */
+int vpb_as_split_v(int dtype, const void* qkv, int T, int nh, int dk, int dh, void* vc, void* vt, int batch,
+                   void* stream);
+/* softmax(s * scale) over each row (common_layers.py:99-100), fp32 math: s, p [rows][cols], cols 1..512 */
+int vpb_as_softmax_rows(int dtype, const void* s, int rows, int cols, float scale, void* p, void* stream);
+/* AutoSpeedHead decode of one level (auto_speed_head.py:53-63): lvl [batch][h*w][ld] (channels 0..63 box logits
+ * side-major, 64..67 class logits; ld >= 68, channels 68.. are not read) -> anchors a0 .. a0+h*w-1 of
+ * out fp32 [batch][8][NA] (cx, cy, w, h in canvas pixels, 4 class sigmoids); a0 + h*w <= NA. */
+int vpb_as_decode(int dtype, const void* lvl, int h, int w, int ld, float stride, int a0, int NA, float* out, int batch,
+                  void* stream);
+/* confidence filter + class-agnostic NMS + un-letterbox of the helper (auto_speed_infer.py:71-106) on raw fp32
+ * [batch][8][NA] (NA 1..10752): scores = max_c sigmoid(raw class score), candidates score > conf in anchor order,
+ * greedy NMS by (score desc, anchor asc) suppressing IoU > iou, boxes mapped back by ((x - pad) / scale) clamped to
+ * [0, orig].  scale / pad_x / pad_y / orig_w / orig_h: HOST arrays of batch entries (scale > 0).  Scratch: cand fp32
+ * [batch][NA][6], order int [batch][NA]; outputs det fp32 [batch][NA][6] (x1, y1, x2, y2, score, class, first n rows
+ * valid), counts int [batch][2] = (n, candidates).  Nothing is cut: n can reach the candidate count. */
+int vpb_as_postprocess(const float* raw, int NA, int batch, float conf, float iou, const float* scale, const int* pad_x,
+                       const int* pad_y, const int* orig_w, const int* orig_h, float* cand, int* order, float* det,
+                       int* counts, void* stream);
 
 #ifdef __cplusplus
 }

@@ -154,6 +154,81 @@ def test_encoder_ops_reject_bad_arguments_without_a_gpu():
         assert msg in L.last_error(), (name, L.last_error())
 
 
+def test_autospeed_ops_reject_bad_arguments_without_a_gpu():
+    """Every contract violation of the AutoSpeed op entry points (the preconditions the SIMT kernels assume) returns
+    VPB_ERR_ARG with a message before any device work."""
+    lib = L.lib()
+    vp, i, f = C.c_void_p, C.c_int, C.c_float
+    lib.vpb_as_mean.argtypes = [i, vp, i, i, i, vp, vp, i, vp]
+    lib.vpb_as_upsample2.argtypes = [i, vp, i, i, i, i, vp, i, i, vp]
+    lib.vpb_as_maxpool5.argtypes = [i, vp, i, i, i, i, vp, i, vp]
+    lib.vpb_as_split_v.argtypes = [i, vp, i, i, i, i, vp, vp, i, vp]
+    lib.vpb_as_softmax_rows.argtypes = [i, vp, i, i, f, vp, vp]
+    lib.vpb_as_decode.argtypes = [i, vp, i, i, i, f, i, i, vp, i, vp]
+    lib.vpb_as_postprocess.argtypes = [vp, i, i, f, f] + [vp] * 10
+    buf = (C.c_float * 64)()
+    p = (C.addressof(buf) + 15) & ~15   # never dereferenced: every call below must fail validation first
+    odd = p + 2                          # 2-byte aligned, not 16
+    sc = (C.c_float * 8)(*[1.0] * 8)
+    sc0 = (C.c_float * 8)(*[0.0] * 8)
+    ints = (C.c_int * 8)()
+
+    def mean(HW=64, C_=32, ld=32, part=p, batch=1):
+        return lib.vpb_as_mean(0, p, HW, C_, ld, part, p, batch, None)
+
+    def up(C_=32, li=32, lo=64, inp=p, out=p, H=3, batch=1):
+        return lib.vpb_as_upsample2(0, inp, H, 5, C_, li, out, lo, batch, None)
+
+    def pool(C_=32, ld=64, inp=p, out=p, W=5, batch=1):
+        return lib.vpb_as_maxpool5(0, inp, 3, W, C_, ld, out, batch, None)
+
+    def split(T=16, vt=p, batch=1):
+        return lib.vpb_as_split_v(0, p, T, 2, 32, 64, p, vt, batch, None)
+
+    def soft(rows=8, cols=512, s=p):
+        return lib.vpb_as_softmax_rows(0, s, rows, cols, 0.125, p, None)
+
+    def dec(ld=72, a0=0, h=64, w=128, NA=10752, out=p, batch=1):
+        return lib.vpb_as_decode(0, p, h, w, ld, 8.0, a0, NA, out, batch, None)
+
+    def post(NA=10752, batch=1, scale=sc, det=p):
+        return lib.vpb_as_postprocess(p, NA, batch, 0.6, 0.45, C.addressof(scale), *[C.addressof(ints)] * 4,
+                                      p, p, det, p, None)
+
+    cases = [
+        ("mean C 257", lambda: mean(C_=257, ld=264), "C 1..256"), ("mean C 512", lambda: mean(C_=512, ld=512), "C 1..256"),
+        ("mean C 0", lambda: mean(C_=0), "C 1..256"), ("mean ld < C", lambda: mean(ld=24), "ld >= C"),
+        ("mean HW 0", lambda: mean(HW=0), "as_mean"), ("mean NULL part", lambda: mean(part=None), "NULL"),
+        ("mean batch 0", lambda: mean(batch=0), "batch"), ("mean batch 9", lambda: mean(batch=9), "batch"),
+        ("upsample C 12", lambda: up(C_=12, li=16, lo=16), "multiples of 8"),
+        ("upsample ld_in 36", lambda: up(li=36), "multiples of 8"), ("upsample ld_out 68", lambda: up(lo=68), "multiples of 8"),
+        ("upsample ld_out < C", lambda: up(lo=24), "multiples of 8"),
+        ("upsample unaligned in", lambda: up(inp=odd), "aligned"), ("upsample unaligned out", lambda: up(out=odd), "aligned"),
+        ("upsample NULL out", lambda: up(out=None), "NULL"), ("upsample H 0", lambda: up(H=0), "as_upsample2"),
+        ("upsample batch 9", lambda: up(batch=9), "batch"),
+        ("maxpool C 4", lambda: pool(C_=4), "multiples of 8"), ("maxpool ld 68", lambda: pool(ld=68), "multiples of 8"),
+        ("maxpool unaligned in", lambda: pool(inp=odd), "aligned"), ("maxpool unaligned out", lambda: pool(out=odd), "aligned"),
+        ("maxpool NULL in", lambda: pool(inp=None), "NULL"), ("maxpool W 0", lambda: pool(W=0), "as_maxpool5"),
+        ("maxpool batch 0", lambda: pool(batch=0), "batch"),
+        ("split_v T 0", lambda: split(T=0), "as_split_v"), ("split_v NULL vt", lambda: split(vt=None), "NULL"),
+        ("split_v batch 9", lambda: split(batch=9), "batch"),
+        ("softmax cols 513", lambda: soft(cols=513), "cols 1..512"), ("softmax cols 0", lambda: soft(cols=0), "cols 1..512"),
+        ("softmax rows 0", lambda: soft(rows=0), "as_softmax_rows"), ("softmax NULL s", lambda: soft(s=None), "NULL"),
+        ("decode ld 64", lambda: dec(ld=64), "ld >= 68"), ("decode ld 67", lambda: dec(ld=67), "ld >= 68"),
+        ("decode past NA", lambda: dec(a0=8192), "a0 + h*w <= NA"), ("decode a0 < 0", lambda: dec(a0=-1), "as_decode"),
+        ("decode NA short", lambda: dec(NA=8191), "a0 + h*w <= NA"), ("decode NULL out", lambda: dec(out=None), "NULL"),
+        ("decode batch 9", lambda: dec(batch=9), "batch"),
+        ("postprocess NA 10753", lambda: post(NA=10753), "NA="), ("postprocess NA 0", lambda: post(NA=0), "NA="),
+        ("postprocess scale 0", lambda: post(scale=sc0), "scale"), ("postprocess NULL det", lambda: post(det=None), "NULL"),
+        ("postprocess batch 0", lambda: post(batch=0), "batch"), ("postprocess batch 9", lambda: post(batch=9), "batch"),
+    ]
+    for name, call, msg in cases:
+        assert call() == -1, name
+        assert msg in L.last_error(), (name, L.last_error())
+    lib.vpb_as_mean_blocks.argtypes = [i]
+    assert [lib.vpb_as_mean_blocks(hw) for hw in (1, 63, 64, 128 * 256, 16 * 32)] == [1, 1, 1, 148, 8]
+
+
 def test_vpw_writer_layout(tmp_path):
     sd = {"a.weight": np.arange(24, dtype=np.float32).reshape(2, 3, 2, 2),
           "a.num_batches_tracked": np.array(7, dtype=np.int64)}

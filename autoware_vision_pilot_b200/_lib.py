@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvp_b200.so")
 
@@ -62,6 +64,107 @@ def frame_descs(descs) -> "C.Array":
             raise ValueError(f"frame {k}: bad descriptor (ptr {ptr:#x}, h {h}, w {w}, stride {stride}): need a non-NULL "
                              "pointer, h, w > 0 and stride >= 3*w")
         arr[k] = Frame(ptr, h, w, stride)
+    return arr
+
+
+PIX_PACKED, PIX_NV12, PIX_UYVY, PIX_YUYV = 0, 1, 2, 3    # VPB_PIX_*
+
+
+class FrameFmt(C.Structure):
+    """Mirror of vpb_frame_fmt (include/vp_b200_ops.h): a frame in a VPB_PIX_* layout."""
+
+    _fields_ = [("format", C.c_int), ("data", C.c_void_p), ("h", C.c_int), ("w", C.c_int), ("stride", C.c_int),
+                ("uv", C.c_void_p), ("uv_stride", C.c_int)]
+
+
+def _rows(a: np.ndarray, row_bytes: int, what: str, allow_copy: bool) -> np.ndarray:
+    """a as uint8 rows of `row_bytes` contiguous bytes (the row stride may be larger: an ROI / padded view)"""
+    if not isinstance(a, np.ndarray) or a.dtype != np.uint8:
+        raise ValueError(f"{what} must be a uint8 array")
+    flat = a.reshape(a.shape[0], -1) if a.ndim > 1 and a[0].flags.c_contiguous else None
+    if flat is None or flat.shape[1] != row_bytes or flat.strides[1] != 1 or a.strides[0] < row_bytes:
+        if not allow_copy:
+            raise ValueError(f"{what} needs contiguous rows (it is read asynchronously)")
+        a = np.ascontiguousarray(a)
+    return a
+
+
+class NV12:
+    """A host NV12 frame in cv2's layout: y uint8 [h, w] (the Y plane), uv uint8 [h/2, w] (interleaved U, V; or
+    [h/2, w/2, 2]).  The planes may live in separate buffers and have padded rows.  NV12.from_cv(a) takes the single
+    [h*3/2, w] array cv2.cvtColor(..., COLOR_YUV2RGB_NV12) reads."""
+
+    format = PIX_NV12
+
+    def __init__(self, y: np.ndarray, uv: np.ndarray):
+        self.y, self.uv = y, uv
+        if y.ndim != 2 or uv.shape[0] * 2 != y.shape[0] or uv.reshape(uv.shape[0], -1).shape[1] != y.shape[1]:
+            raise ValueError(f"NV12: y [h, w] and uv [h/2, w] expected, got {y.shape} and {uv.shape}")
+        self.h, self.w = y.shape
+
+    @classmethod
+    def from_cv(cls, a: np.ndarray) -> "NV12":
+        if a.ndim != 2 or a.shape[0] % 3:
+            raise ValueError(f"NV12.from_cv: [h*3/2, w] expected, got {a.shape}")
+        h = a.shape[0] * 2 // 3
+        return cls(a[:h], a[h:])
+
+    def planes(self, allow_copy: bool):
+        y = _rows(self.y, self.w, "NV12 y", allow_copy)
+        uv = _rows(self.uv, self.w, "NV12 uv", allow_copy)
+        return y, uv
+
+    def desc(self, allow_copy: bool = True):
+        """(FrameFmt, arrays that must stay alive while the descriptor is used)"""
+        y, uv = self.planes(allow_copy)
+        return FrameFmt(PIX_NV12, y.ctypes.data, self.h, self.w, y.strides[0], uv.ctypes.data, uv.strides[0]), (y, uv)
+
+
+class _Packed422:
+    format = PIX_PACKED
+
+    def __init__(self, a: np.ndarray):
+        if not isinstance(a, np.ndarray) or a.ndim != 3 or a.shape[2] != 2:
+            raise ValueError(f"{type(self).__name__}: [h, w, 2] expected, got {getattr(a, 'shape', a)}")
+        self.a = a
+        self.h, self.w = a.shape[:2]
+
+    def desc(self, allow_copy: bool = True):
+        a = _rows(self.a, 2 * self.w, type(self).__name__, allow_copy)
+        return FrameFmt(self.format, a.ctypes.data, self.h, self.w, a.strides[0], None, 0), (a,)
+
+
+class UYVY(_Packed422):
+    """A host UYVY frame in cv2's layout, uint8 [h, w, 2] (U Y0 V Y1 per pixel pair; ROS "yuv422", GMSL cameras)."""
+
+    format = PIX_UYVY
+
+
+class YUYV(_Packed422):
+    """A host YUYV frame in cv2's layout, uint8 [h, w, 2] (Y0 U Y1 V per pixel pair; ROS "yuv422_yuy2", UVC cameras)."""
+
+    format = PIX_YUYV
+
+
+YUV_TYPES = (NV12, UYVY, YUYV)
+
+
+def packed_desc(frame: np.ndarray):
+    """A uint8 [h, w, 3] array with unit pixel strides as a VPB_PIX_PACKED FrameFmt"""
+    h, w, _ = frame.shape
+    return FrameFmt(PIX_PACKED, frame.ctypes.data, h, w, frame.strides[0], None, 0), (frame,)
+
+
+def frame_fmt_descs(descs) -> "C.Array":
+    """(format, data_ptr, h, w, stride, uv_ptr, uv_stride) tuples as a vpb_frame_fmt array (device frames); ValueError
+    for a tuple of the wrong length (the library checks the rest)."""
+    descs = list(descs)
+    arr = (FrameFmt * max(len(descs), 1))()
+    for k, d in enumerate(descs):
+        if len(d) != 7:
+            raise ValueError(f"frame {k}: need (format, data_ptr, h, w, stride, uv_ptr, uv_stride), got {d!r}")
+        fmt, ptr, h, w, stride, uv, uv_stride = d
+        arr[k] = FrameFmt(int(fmt), int(ptr) or None, int(h), int(w), int(stride), int(uv or 0) or None, int(uv_stride))
     return arr
 
 

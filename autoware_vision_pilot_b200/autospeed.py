@@ -29,6 +29,8 @@ def _bind():
     lib.vp_autospeed_infer_device_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
     lib.vp_autospeed_infer_frames.argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int, C.c_int]
     lib.vp_autospeed_infer_device_frames.argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int]
+    lib.vp_autospeed_infer_frames_fmt.argtypes = [C.c_void_p, C.POINTER(L.FrameFmt), C.c_int, C.c_int]
+    lib.vp_autospeed_infer_device_frames_fmt.argtypes = [C.c_void_p, C.POINTER(L.FrameFmt), C.c_int]
     lib.vp_autospeed_sync.argtypes = [C.c_void_p, C.c_int]
     lib.vp_autospeed_detections.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.vp_autospeed_raw.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
@@ -119,11 +121,21 @@ class AutoSpeedEngine:
         L.check(self._lib.vp_autospeed_infer_device_batch(self._h, ptrs, len(dev_ptrs), h, w, stride),
                 "vp_autospeed_infer_device_batch")
 
-    def infer_frames(self, frames: Sequence[np.ndarray], fetch_raw: bool = False) -> List[np.ndarray]:
+    def infer_frames(self, frames, fetch_raw: bool = False) -> List[np.ndarray]:
         """`batch` uint8 [h_k, w_k, 3] RGB frames, each of its own size, in one call (each gets its own letterbox)
-        -> detections of frame k, in frame k's pixels, at index k."""
+        -> detections of frame k, in frame k's pixels, at index k.  A frame may also be a camera-native NV12 / UYVY /
+        YUYV object (autoware_vision_pilot_b200._lib), converted to RGB inside the letterbox as cv2.cvtColor would."""
         frames = list(frames)
         self._check_count(len(frames))
+        if any(isinstance(f, L.YUV_TYPES) for f in frames):
+            arr, keep = (L.FrameFmt * len(frames))(), []
+            for k, f in enumerate(frames):
+                d, alive = f.desc() if isinstance(f, L.YUV_TYPES) else L.packed_desc(self._check_frame(f))
+                arr[k] = d
+                keep.append(alive)
+            L.check(self._lib.vp_autospeed_infer_frames_fmt(self._h, arr, len(frames), int(fetch_raw)),
+                    "vp_autospeed_infer_frames_fmt")
+            return [self.detections(k) for k in range(self.batch)]
         frames = [self._check_frame(f) for f in frames]
         descs = L.frame_descs([(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames])
         L.check(self._lib.vp_autospeed_infer_frames(self._h, descs, len(frames), int(fetch_raw)),
@@ -137,6 +149,14 @@ class AutoSpeedEngine:
         self._check_count(len(descs))
         L.check(self._lib.vp_autospeed_infer_device_frames(self._h, L.frame_descs(descs), len(descs)),
                 "vp_autospeed_infer_device_frames")
+
+    def infer_device_frames_fmt(self, descs: Sequence[Sequence[int]]) -> None:
+        """`batch` device frames as (format, data_ptr, h, w, stride, uv_ptr, uv_stride) tuples (format one of _lib.PIX_*),
+        enqueued as one call; sync() completes it."""
+        descs = list(descs)
+        self._check_count(len(descs))
+        L.check(self._lib.vp_autospeed_infer_device_frames_fmt(self._h, L.frame_fmt_descs(descs), len(descs)),
+                "vp_autospeed_infer_device_frames_fmt")
 
     def sync(self, fetch: int = 1) -> None:
         L.check(self._lib.vp_autospeed_sync(self._h, fetch), "vp_autospeed_sync")

@@ -515,7 +515,7 @@ struct vp_autospeed : EngineRuntime {
   // others of a sample that has more, after the call has completed.
   static constexpr int kDetFetch = 1024;
 
-  int geoms(const vpb_frame* frames, const char* who, PreGeom* g) override;
+  int geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) override;
   int enqueue(const PreGeom* g) override;
   int fetch(bool raw) override;
   int fetch_rest();
@@ -831,7 +831,7 @@ static double as_scale(int h, int w) { return std::min(static_cast<double>(kASW)
 }  // namespace vpb
 
 // letterbox geometry of every frame; VPB_ERR_ARG (naming `who` and the frame) if one cannot be resized.  Host-only.
-int vp_autospeed::geoms(const vpb_frame* frames, const char* who, PreGeom* g) {
+int vp_autospeed::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
   for (int k = 0; k < batch; ++k) {
     const int h = frames[k].h, w = frames[k].w;
     const double sc = as_scale(h, w);
@@ -977,6 +977,15 @@ extern "C" int vp_autospeed_infer_batch(vp_autospeed* e, const uint8_t* const* f
 extern "C" int vp_autospeed_infer_frames(vp_autospeed* e, const vpb_frame* frames_host, int n, int fetch_raw) {
   const int rc = call_host(e, frames_host, n, true, fetch_raw != 0, "vp_autospeed_infer_frames");
   return rc ? rc : e->fetch_rest();
+}
+
+extern "C" int vp_autospeed_infer_frames_fmt(vp_autospeed* e, const vpb_frame_fmt* frames_host, int n, int fetch_raw) {
+  const int rc = call_host(e, frames_host, n, true, fetch_raw != 0, "vp_autospeed_infer_frames_fmt");
+  return rc ? rc : e->fetch_rest();
+}
+
+extern "C" int vp_autospeed_infer_device_frames_fmt(vp_autospeed* e, const vpb_frame_fmt* frames_dev, int n) {
+  return call_device(e, frames_dev, n, "vp_autospeed_infer_device_frames_fmt");
 }
 
 extern "C" int vp_autospeed_infer_device_batch(vp_autospeed* e, const uint8_t* const* frames_dev, int n, int h, int w,

@@ -100,7 +100,7 @@ struct vp_engine : EngineRuntime {
   bool src_ready = false;                  // a call has run (vp_engine_source_output answers)
   bool src_host = false;                   // the last call was a host call: the pinned copies are current
 
-  int geoms(const vpb_frame* frames, const char* who, PreGeom* g) override;
+  int geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) override;
   int enqueue(const PreGeom* g) override;
   int fetch(bool raw) override;
 };
@@ -533,7 +533,7 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
 // buffer drops the captured graph, whose node holds the old pointer), destinations, sizes and frame pointers.
 static int prepare_source(vp_engine& e) {
   for (auto& so : e.src_outs) {
-    const vpb_frame& fr = e.frames[so.sample];
+    const vpb_frame_fmt& fr = e.frames[so.sample];   // packed when a job is an overlay (vp_engine::geoms)
     vpb_src_job& j = so.job;
     const int el = j.kind == VPB_SRC_DEPTH ? 4 : j.kind == VPB_SRC_OVERLAY ? 3 : 1;
     const size_t bytes = static_cast<size_t>(fr.h) * fr.w * el;
@@ -620,9 +620,15 @@ static int check_source_flags(const vp_engine_config& c) {
 }  // namespace vpb
 
 // Every frame resizes to the 640 x 320 network input: VPB_ERR_ARG (naming `who` and the frame) if one cannot in the
-// engine's resize mode.  Host-only: callers run it before any device work.
-int vp_engine::geoms(const vpb_frame* frames, const char* who, PreGeom* g) {
+// engine's resize mode, or if the engine makes overlays and the frame is not packed (the overlay blends the camera
+// frame's pixels as vpb_src_job reads them).  Host-only: callers run it before any device work.
+int vp_engine::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
   for (int k = 0; k < batch; ++k) {
+    if ((cfg.source_outputs & VP_SRC_OVERLAY) && frames[k].format != VPB_PIX_PACKED) {
+      vpb_set_error("%s: frame %d: VP_SRC_OVERLAY blends the packed camera frame; this engine cannot take a YUV frame "
+                    "(format %d)", who, k, frames[k].format);
+      return VPB_ERR_ARG;
+    }
     g[k] = PreGeom{};
     g[k].h = frames[k].h; g[k].w = frames[k].w;
     const int rc = PreprocessPlan::check(g[k], cfg.resize_mode, who, k);
@@ -791,6 +797,18 @@ extern "C" int vp_engine_infer_frames(vp_engine* e, const vpb_frame* frames_host
 
 extern "C" int vp_engine_submit_frames(vp_engine* e, const vpb_frame* frames_host, int n) {
   return call_host(e, frames_host, n, false, false, "vp_engine_submit_frames");
+}
+
+extern "C" int vp_engine_infer_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n) {
+  return call_host(e, frames_host, n, true, false, "vp_engine_infer_frames_fmt");
+}
+
+extern "C" int vp_engine_submit_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n) {
+  return call_host(e, frames_host, n, false, false, "vp_engine_submit_frames_fmt");
+}
+
+extern "C" int vp_engine_infer_device_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_dev, int n) {
+  return call_device(e, frames_dev, n, "vp_engine_infer_device_frames_fmt");
 }
 
 extern "C" int vp_engine_fetch_raw(vp_engine* e, int idx) {

@@ -106,13 +106,15 @@ extern "C" int vpb_final_conv_weights_host(const float* w, int Cout, int Cin, fl
 namespace vpb {
 
 // =============================================================== frame graph
-static bool same_geometry(const vpb_frame& a, const vpb_frame& b) { return a.h == b.h && a.w == b.w && a.stride == b.stride; }
+static bool same_geometry(const vpb_frame_fmt& a, const vpb_frame_fmt& b) {
+  return a.format == b.format && a.h == b.h && a.w == b.w && a.stride == b.stride && a.uv_stride == b.uv_stride;
+}
 
 int FrameGraph::run(EngineRuntime& e) {
   const cudaStream_t st = e.stream;
   bool same_geom = exec && n == e.n_frames, same_src = n == e.n_frames;
   for (int k = 0; k < e.n_frames && same_geom; ++k) same_geom = same_geometry(frames[k], e.frames[k]);
-  for (int k = 0; k < e.n_frames && same_src; ++k) same_src = frames[k].data == e.frames[k].data;
+  for (int k = 0; k < e.n_frames && same_src; ++k) same_src = frames[k].data == e.frames[k].data && frames[k].uv == e.frames[k].uv;
   if (same_geom && !same_src) {
     for (const auto& [i, node] : nodes) {
       const int rc = e.ops[i].repoint(exec, node);
@@ -371,22 +373,23 @@ int EngineRuntime::append_conv(const std::string& name, const vpb_conv_args& a) 
   return VPB_OK;
 }
 
-bool frames_ok(const EngineRuntime* e, const vpb_frame* frames, int n, const char* who) {
+bool frames_ok(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who) {
   if (!e || !frames) { vpb_set_error("%s: bad arguments", who); return false; }
   if (n != e->batch) {
     vpb_set_error("%s: %d frame(s) for an engine of batch %d%s", who, n, e->batch,
                   n == 1 ? " (use the *_batch calls)" : "");
     return false;
   }
-  for (int k = 0; k < n; ++k) {
-    const vpb_frame& f = frames[k];
-    if (!f.data) { vpb_set_error("%s: frame %d is NULL", who, k); return false; }
-    if (f.h <= 0 || f.w <= 0 || f.stride < 3 * f.w) {
-      vpb_set_error("%s: frame %d: bad geometry h %d, w %d, stride %d (need h, w > 0 and stride >= 3*w)", who, k, f.h,
-                    f.w, f.stride);
-      return false;
-    }
-  }
+  for (int k = 0; k < n; ++k)
+    if (frame_fmt_check(frames[k], who, k)) return false;
+  return true;
+}
+
+// vpb_frame descriptors as VPB_PIX_PACKED ones (the first kMaxBatch; frames_ok rejects a count other than the batch)
+static bool packed_frames(const EngineRuntime* e, const vpb_frame* frames, int n, const char* who, Frames& out) {
+  if (!e || !frames) { vpb_set_error("%s: bad arguments", who); return false; }
+  out = {};
+  for (int k = 0; k < n && k < kMaxBatch; ++k) out[k] = packed_frame(frames[k]);
   return true;
 }
 
@@ -394,25 +397,27 @@ bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int
                   Frames& out) {
   if (!e || !ptrs || h <= 0 || w <= 0 || stride < w * 3) { vpb_set_error("%s: bad arguments", who); return false; }
   out = {};
-  for (int k = 0; k < n && k < kMaxBatch; ++k) out[k] = vpb_frame{ptrs[k], h, w, stride};
+  for (int k = 0; k < n && k < kMaxBatch; ++k) out[k] = packed_frame(vpb_frame{ptrs[k], h, w, stride});
   return frames_ok(e, out.data(), n, who);
 }
 
 // The device frames f of geometries g become the runtime's frames, and op 0, the pre-process, gets the algorithmic
-// bytes of the call (SURVEY.md 8d: frame read + 3 x OH x OW 16-bit written, per sample).  A failed call leaves no
+// bytes of the call (SURVEY.md 8d: frame read + 3 x OH x OW 16-bit written, per sample; a frame reads h x w x 3 bytes
+// packed, x 2 in 4:2:2, x 1.5 in NV12).  A failed call leaves no
 // frames, so nothing launches the pre-process on frames its tables were not built for.
 static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeom* g) {
   e->frames = f;
   e->n_frames = n;
   double bytes = 0;
-  for (int k = 0; k < n; ++k) bytes += 3.0 * g[k].h * g[k].w + 2.0 * 3 * g[k].OH * g[k].OW;
+  static const double kBytesPerPixel[4] = {3.0, 1.5, 2.0, 2.0};
+  for (int k = 0; k < n; ++k) bytes += kBytesPerPixel[f[k].format] * g[k].h * g[k].w + 2.0 * 3 * g[k].OH * g[k].OW;
   e->ops[0].bytes = bytes;
   const int rc = e->enqueue(g);
   if (rc) e->n_frames = 0;
   return rc;
 }
 
-int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool raw, const char* who) {
+int call_host(EngineRuntime* e, const vpb_frame_fmt* frames, int n, bool sync, bool raw, const char* who) {
   if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
   PreGeom g[kMaxBatch];
   if (e->geoms(frames, who, g)) return VPB_ERR_ARG;
@@ -428,7 +433,7 @@ int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool 
   return VPB_OK;
 }
 
-int call_device(EngineRuntime* e, const vpb_frame* frames, int n, const char* who) {
+int call_device(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who) {
   if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
   PreGeom g[kMaxBatch];
   if (e->geoms(frames, who, g)) return VPB_ERR_ARG;
@@ -438,9 +443,31 @@ int call_device(EngineRuntime* e, const vpb_frame* frames, int n, const char* wh
   return enqueue_frames(e, f, n, g);
 }
 
-int EngineRuntime::upload_frames(const vpb_frame* frames, int n, Frames& dev) {
+int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool raw, const char* who) {
+  Frames f;
+  if (!packed_frames(e, frames, n, who, f)) return VPB_ERR_ARG;
+  return call_host(e, f.data(), n, sync, raw, who);
+}
+
+int call_device(EngineRuntime* e, const vpb_frame* frames, int n, const char* who) {
+  Frames f;
+  if (!packed_frames(e, frames, n, who, f)) return VPB_ERR_ARG;
+  return call_device(e, f.data(), n, who);
+}
+
+// One plane of rows rows, `row` valid bytes each, from the host (pitch spitch) to d (pitch row) on st
+static int upload_plane(uint8_t* d, const uint8_t* s, int spitch, int row, int rows, cudaStream_t st) {
+  if (spitch == row) VPB_CUDA_OK(cudaMemcpyAsync(d, s, static_cast<size_t>(rows) * row, cudaMemcpyHostToDevice, st));
+  else VPB_CUDA_OK(cudaMemcpy2DAsync(d, row, s, spitch, row, rows, cudaMemcpyHostToDevice, st));
+  return VPB_OK;
+}
+
+int EngineRuntime::upload_frames(const vpb_frame_fmt* frames, int n, Frames& dev) {
   size_t total = 0;
-  for (int k = 0; k < n; ++k) total += static_cast<size_t>(frames[k].h) * frames[k].w * 3;
+  for (int k = 0; k < n; ++k) {
+    const vpb_frame_fmt& f = frames[k];
+    total += static_cast<size_t>(f.h) * frame_row_bytes(f) + (f.format == VPB_PIX_NV12 ? static_cast<size_t>(f.h / 2) * f.w : 0);
+  }
   if (total > d_frame_cap) {
     frame_graph.invalidate();
     void* p = nullptr;
@@ -451,13 +478,20 @@ int EngineRuntime::upload_frames(const vpb_frame* frames, int n, Frames& dev) {
   dev = {};
   size_t off = 0;
   for (int k = 0; k < n; ++k) {
-    const vpb_frame& f = frames[k];
-    const int dpitch = f.w * 3;
+    const vpb_frame_fmt& f = frames[k];
+    const int dpitch = frame_row_bytes(f);
     uint8_t* d = d_frame + off;
-    dev[k] = vpb_frame{d, f.h, f.w, dpitch};
-    if (f.stride == dpitch) VPB_CUDA_OK(cudaMemcpyAsync(d, f.data, static_cast<size_t>(f.h) * dpitch, cudaMemcpyHostToDevice, stream));
-    else VPB_CUDA_OK(cudaMemcpy2DAsync(d, dpitch, f.data, f.stride, dpitch, f.h, cudaMemcpyHostToDevice, stream));
+    dev[k] = f;
+    dev[k].data = d; dev[k].stride = dpitch;
+    int rc = upload_plane(d, f.data, f.stride, dpitch, f.h, stream);
+    if (rc) return rc;
     off += static_cast<size_t>(f.h) * dpitch;
+    if (f.format == VPB_PIX_NV12) {
+      dev[k].uv = d_frame + off; dev[k].uv_stride = f.w;
+      rc = upload_plane(d_frame + off, f.uv, f.uv_stride, f.w, f.h / 2, stream);
+      if (rc) return rc;
+      off += static_cast<size_t>(f.h / 2) * f.w;
+    }
   }
   return VPB_OK;
 }

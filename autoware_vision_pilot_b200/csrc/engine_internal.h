@@ -83,12 +83,13 @@ struct OpRec {
   std::function<int(cudaGraphExec_t, cudaGraphNode_t)> repoint;
 };
 
-// The frames of one call: descriptor k is sample k (entries past the batch are unused).
-using Frames = std::array<vpb_frame, kMaxBatch>;
+// The frames of one call: descriptor k is sample k, in its own VPB_PIX_* format (entries past the batch are unused).
+using Frames = std::array<vpb_frame_fmt, kMaxBatch>;
 
 struct EngineRuntime;
-// The CUDA graph of one call of a runtime's launch list, keyed on the n (h, w, stride) triples and the frame pointers.
-// Frames of the captured geometries in other buffers only re-point the captured nodes of the ops that have repoint.
+// The CUDA graph of one call of a runtime's launch list, keyed on the n (format, h, w, stride, uv_stride) tuples and the
+// frame pointers (data, uv).  Frames of the captured geometries and formats in other buffers only re-point the captured
+// nodes of the ops that have repoint; a new format captures again (it selects another pre-process kernel).
 struct FrameGraph {
   cudaGraph_t graph = nullptr;           // kept alive: the recorded nodes are handles into it
   cudaGraphExec_t exec = nullptr;
@@ -180,10 +181,11 @@ struct EngineRuntime {
   // build the plan of one wgmma convolution, keep it, append its launch on lane cur_lane (errors are prefixed with name)
   int append_conv(const std::string& name, const vpb_conv_args& a);
   void tap(const std::string& name, const Tens& t, int channels = 0) { taps[name] = Tap{t, channels > 0 ? channels : t.C}; }
-  // Copy n host frames to d_frame (grown on demand), back to back, frame k with pitch w_k*3: only the w_k*3 valid bytes
-  // of every row are read from the caller's buffer, so a cv::Mat ROI / strided view is never read past its last row.
-  // dev[k] describes the device copy of frame k.
-  int upload_frames(const vpb_frame* frames, int n, Frames& dev);
+  // Copy n host frames to d_frame (grown on demand), plane after plane, frame after frame, each row with the pitch of its
+  // valid bytes (3w packed, 2w UYVY / YUYV, w for the Y and the UV rows of NV12): only those bytes of every row are read
+  // from the caller's buffer, so a cv::Mat ROI / strided view is never read past its last row.  dev[k] describes the
+  // device copy of frame k (its uv inside d_frame for NV12).
+  int upload_frames(const vpb_frame_fmt* frames, int n, Frames& dev);
   // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
   bool find_tap(const char* name, Tap* out) const;
   // tap `name` (find_tap) as fp32 [channels][H][W] into dst (NULL: size query); element count or < 0
@@ -199,20 +201,22 @@ struct EngineRuntime {
   // `batch` frames (VPB_ERR_ARG naming who and the frame); enqueue: the call on the device frames `frames` of
   // geometries g; fetch: copies of the outputs to the pinned host buffers (raw: also the raw tensors the engine does
   // not copy by default).
-  virtual int geoms(const vpb_frame* frames, const char* who, PreGeom* g) = 0;
+  virtual int geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) = 0;
   virtual int enqueue(const PreGeom* g) = 0;
   virtual int fetch(bool raw) = 0;
 };
 
 // A call on n host frames: frames_ok, the engine's geometries, its device, the upload of the frames, enqueue, fetch and
 // with sync a stream synchronise.
-int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool raw, const char* who);
+int call_host(EngineRuntime* e, const vpb_frame_fmt* frames, int n, bool sync, bool raw, const char* who);
 // A call on n device frames: frames_ok, the engine's geometries, its device and enqueue.
+int call_device(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who);
+// The packed-frame calls (vpb_frame): the same calls on VPB_PIX_PACKED descriptors
+int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool raw, const char* who);
 int call_device(EngineRuntime* e, const vpb_frame* frames, int n, const char* who);
 
-// n == e's batch descriptors, each with non-NULL data, h, w > 0 and stride >= 3*w (who names the call and the message
-// the frame index)
-bool frames_ok(const EngineRuntime* e, const vpb_frame* frames, int n, const char* who);
+// n == e's batch descriptors, each passing frame_fmt_check (who names the call and the message the frame index)
+bool frames_ok(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who);
 // n frames of one geometry (the *_batch calls) as descriptors; false (error set as frames_ok does) on bad arguments
 bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int h, int w, int stride, const char* who,
                   Frames& out);

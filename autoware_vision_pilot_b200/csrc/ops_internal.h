@@ -24,6 +24,20 @@ struct PreGeom {
   bool operator!=(const PreGeom& o) const { return !(*this == o); }
 };
 
+// Host-only check of one frame descriptor: VPB_OK, or VPB_ERR_ARG with "<who>: frame <k> ..." set for an unknown
+// format, a NULL plane, a non-positive or (for the format) odd size, or a stride below the format's minimum.  The
+// messages for packed frames are those vpb_frame has always had.
+int frame_fmt_check(const vpb_frame_fmt& f, const char* who, int k);
+// Bytes of each row of the frame's main plane that belong to the image (3w packed, 2w 4:2:2, w NV12)
+inline int frame_row_bytes(const vpb_frame_fmt& f) {
+  return f.format == VPB_PIX_PACKED ? 3 * f.w : f.format == VPB_PIX_NV12 ? f.w : 2 * f.w;
+}
+inline vpb_frame_fmt packed_frame(const vpb_frame& f) {
+  vpb_frame_fmt o{};
+  o.format = VPB_PIX_PACKED; o.data = f.data; o.h = f.h; o.w = f.w; o.stride = f.stride;
+  return o;
+}
+
 // Pre-process plan: coefficient tables resident on the device for the images of one call (one table set per distinct
 // geometry, one allocation) and one mode; the launch shape (XT, TY, shared memory) covers every image.
 struct PreprocessPlan {
@@ -45,11 +59,13 @@ struct PreprocessPlan {
   static int check(const PreGeom& g, int mode, const char* who, int k);
   // n images (1..kMaxBatch); rebuilds the tables only when a geometry or the mode changed
   int configure(const PreGeom* g, int n, int mode);
-  // frames[0 .. n-1]: image k reads frames[k].data with frames[k].stride (its h, w are geom[k]'s); out / out_u8 hold
-  // n images back to back (16-bit mode only for n > 1)
-  int launch(const vpb_frame* frames, int convention, int dtype, void* out, uint8_t* out_u8, cudaStream_t stream) const;
-  int update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame* frames, int convention, int dtype,
-                        void* out, uint8_t* out_u8) const;
+  // frames[0 .. n-1]: image k reads frames[k] in its format (data, stride, and uv, uv_stride for NV12; its h, w are
+  // geom[k]'s); out / out_u8 hold n images back to back (16-bit mode only for n > 1).  A call whose frames are all
+  // packed launches the packed-only kernel instantiations; one YUV frame selects the converting ones.
+  int launch(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8,
+             cudaStream_t stream) const;
+  int update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames, int convention,
+                        int dtype, void* out, uint8_t* out_u8) const;
   ~PreprocessPlan();
 };
 

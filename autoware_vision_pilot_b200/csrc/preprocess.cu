@@ -20,6 +20,7 @@
 #include "ops_internal.h"
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 #include <vector>
 
 namespace vpb {
@@ -120,6 +121,47 @@ struct PreParams {      // by value (__grid_constant__): under 0.8 KB at kMaxBat
   uint8_t* out_u8;      // optional resized image in tensor channel order, [out_rows][out_pitch][3] per image
   size_t out_img;       // elements between the canvases of out (out_lo); out_u8 images are out_img / out_c * 3 bytes apart
 };
+// The per-image format fields of a call with a YUV frame follow the PreParams block instead of widening PreImg: the
+// packed-only instantiations take PreParams itself, so their parameter layout, and their code, are those of a build
+// without YUV input.  PreParamsYuv stays under 1 KB at kMaxBatch images.
+struct PreYuv {
+  const uint8_t* uv;    // NV12: the interleaved U,V plane [h/2][uv_stride]
+  int fmt, uv_stride;   // VPB_PIX_*
+  int bgr;              // 1: a YUV image converts to B, G, R (the BGR conventions), 0: to R, G, B
+};
+struct PreParamsYuv : PreParams {
+  PreYuv yuv[kMaxBatch];
+};
+template <bool YUV> using PreParamsOf = typename std::conditional<YUV, PreParamsYuv, PreParams>::type;
+static_assert(sizeof(PreParamsYuv) < 1024, "the by-value parameter block of a YUV call stays under 1 KB");
+
+__device__ __forceinline__ PreYuv yuv_of(const PreParams&, int) { return PreYuv{nullptr, VPB_PIX_PACKED, 0, 0}; }
+__device__ __forceinline__ PreYuv yuv_of(const PreParamsYuv& p, int img) { return p.yuv[img]; }
+
+// OpenCV's YUV -> RGB of COLOR_YUV2RGB_NV12 / _UYVY / _YUYV (BT.601 limited range, 20-bit fixed point): y' = max(Y -
+// 16, 0) * 1220542 + 2^19, R = (y' + 1673527 v) >> 20, G = (y' - 852492 v - 409993 u) >> 20, B = (y' + 2116026 u) >> 20,
+// u = U - 128, v = V - 128, each clipped to [0, 255].  No term overflows 32 bits.
+__device__ __forceinline__ void yuv_px(int Y, int U, int V, int bgr, int (&o)[3]) {
+  const int y = max(Y - 16, 0) * 1220542 + (1 << 19);
+  const int u = U - 128, v = V - 128;
+  const int r = min(max((y + 1673527 * v) >> 20, 0), 255);
+  const int g = min(max((y - 852492 * v - 409993 * u) >> 20, 0), 255);
+  const int b = min(max((y + 2116026 * u) >> 20, 0), 255);
+  o[0] = bgr ? b : r; o[1] = g; o[2] = bgr ? r : b;
+}
+
+// Source pixel (x, y) of a YUV image, converted: chroma of the 2x2 block (NV12) or the horizontal pair (UYVY, YUYV)
+__device__ __forceinline__ void yuv_load(const PreImg& im, const PreYuv& yv, int y, int x, int (&o)[3]) {
+  const uint8_t* row = im.src + static_cast<size_t>(y) * im.stride;
+  if (yv.fmt == VPB_PIX_NV12) {
+    const uint8_t* c = yv.uv + static_cast<size_t>(y >> 1) * yv.uv_stride + (x & ~1);
+    yuv_px(__ldg(row + x), __ldg(c), __ldg(c + 1), yv.bgr, o);
+  } else {
+    const uint8_t* m = row + (x & ~1) * 2;        // macropixel: U Y0 V Y1 (UYVY) or Y0 U Y1 V (YUYV)
+    if (yv.fmt == VPB_PIX_UYVY) yuv_px(__ldg(m + 1 + ((x & 1) << 1)), __ldg(m), __ldg(m + 2), yv.bgr, o);
+    else yuv_px(__ldg(m + ((x & 1) << 1)), __ldg(m + 1), __ldg(m + 3), yv.bgr, o);
+  }
+}
 
 template <class E>
 __device__ __forceinline__ void emit_pixel(const PreParams& p, const PreImg& im, int img, int oy, int ox, const int (&u)[3]) {
@@ -158,9 +200,12 @@ static constexpr int kRowBytes = kTX * 3;     // 96
 // re-staged every input row 1.75x) took 50 us per 1080p frame = 2 % of the HBM roofline.
 // A call may mix geometries: the grid covers the largest output, and a block outside its own image's output returns
 // (as a whole block, before the first barrier).
-template <class E, int XT>
-__global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __grid_constant__ PreParams p, int rows_cap,
-                                                                     int pitch, int TY) {
+// YUV (a call with at least one YUV image): phase 1 of a YUV image stages the CONVERTED bytes, 3 per pixel from offset 0
+// of each patch row (mis = 0), so phases 2 and 3 run unchanged.  The converted patch row is (x_hi - x_lo) * 3 bytes,
+// never wider than the packed one the plan sizes (which adds the misalignment), so the plan needs no change.
+template <class E, int XT, bool YUV>
+__global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __grid_constant__ PreParamsOf<YUV> p,
+                                                                     int rows_cap, int pitch, int TY) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ __align__(16) uint8_t sm[];
@@ -189,12 +234,26 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __gri
   // ---- phase 1: stage (coalesced aligned words)
   const uintptr_t base = reinterpret_cast<uintptr_t>(im.src) + static_cast<size_t>(x_lo) * 3;
   const int stride = im.stride;
-  for (int r = warp; r < rows; r += kPreThreads / 32) {
-    const uintptr_t a = base + static_cast<size_t>(y_lo + r) * stride;
-    const uint32_t* w0 = reinterpret_cast<const uint32_t*>(a & ~static_cast<uintptr_t>(3));
-    const int words = (static_cast<int>(a & 3) + pwb + 3) >> 2;
-    uint32_t* dst = reinterpret_cast<uint32_t*>(patch + r * pitch);
-    for (int wi = lane; wi < words; wi += 32) dst[wi] = __ldg(w0 + wi);
+  const PreYuv yv = yuv_of(p, img);
+  const bool conv = YUV && yv.fmt != VPB_PIX_PACKED;
+  if (conv) {
+    for (int r = warp; r < rows; r += kPreThreads / 32) {
+      uint8_t* dst = patch + r * pitch;
+      for (int x = lane; x < x_hi - x_lo; x += 32) {
+        int o[3];
+        yuv_load(im, yv, y_lo + r, x_lo + x, o);
+        dst[3 * x] = static_cast<uint8_t>(o[0]); dst[3 * x + 1] = static_cast<uint8_t>(o[1]);
+        dst[3 * x + 2] = static_cast<uint8_t>(o[2]);
+      }
+    }
+  } else {
+    for (int r = warp; r < rows; r += kPreThreads / 32) {
+      const uintptr_t a = base + static_cast<size_t>(y_lo + r) * stride;
+      const uint32_t* w0 = reinterpret_cast<const uint32_t*>(a & ~static_cast<uintptr_t>(3));
+      const int words = (static_cast<int>(a & 3) + pwb + 3) >> 2;
+      uint32_t* dst = reinterpret_cast<uint32_t*>(patch + r * pitch);
+      for (int wi = lane; wi < words; wi += 32) dst[wi] = __ldg(w0 + wi);
+    }
   }
   // horizontal coefficients of this thread's output byte column -> registers
   const int ob = tid % kRowBytes, par = tid / kRowBytes;          // par: which row of a group of kPreThreads / 96
@@ -209,7 +268,7 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __gri
 
   // ---- phase 2: horizontal pass (taps beyond the filter multiply staged bytes by 0: the row pitch covers XT taps)
   for (int r = par; r < rows; r += kPreThreads / kRowBytes) {
-    const int mis = (mis0 + (y_lo + r) * smis) & 3;
+    const int mis = conv ? 0 : (mis0 + (y_lo + r) * smis) & 3;
     const uint8_t* row = patch + r * pitch + mis + boff;
     int acc = 1 << 21, acc1 = 0, acc2 = 0, acc3 = 0;            // four independent IMAD chains (integer: exact)
 #pragma unroll
@@ -275,32 +334,51 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __gri
   }
 }
 
-// OpenCV path (and the no-resize path): one thread per output pixel, gather from global.
-template <class E>
-__global__ void __launch_bounds__(256) preprocess_direct_kernel(const __grid_constant__ PreParams p) {
+// OpenCV path (and the no-resize path): one thread per output pixel, gather from global.  YUV: a YUV image's source
+// pixels are loaded through the conversion.
+template <class E, bool YUV>
+__global__ void __launch_bounds__(256) preprocess_direct_kernel(const __grid_constant__ PreParamsOf<YUV> p) {
   pdl_launch_dependents();
   pdl_wait();
   const int ox = blockIdx.x * blockDim.x + threadIdx.x;
   const int oy = blockIdx.y, img = blockIdx.z;
   const PreImg im = p.im[img];                                      // this image's fields, loaded once
   if (ox >= im.OW || oy >= im.OH) return;
+  const PreYuv yv = yuv_of(p, img);
+  const bool conv = YUV && yv.fmt != VPB_PIX_PACKED;
   const uint8_t* src = im.src;
   int u[3];
   if (p.mode == VPB_RESIZE_NONE) {
-    const uint8_t* s = src + static_cast<size_t>(oy) * im.stride + ox * 3;
-    u[0] = s[0]; u[1] = s[1]; u[2] = s[2];
+    if (conv) {
+      yuv_load(im, yv, oy, ox, u);
+    } else {
+      const uint8_t* s = src + static_cast<size_t>(oy) * im.stride + ox * 3;
+      u[0] = s[0]; u[1] = s[1]; u[2] = s[2];
+    }
   } else {
     const int sx = im.xb[ox], sy = im.yb[oy];
     const int sx1 = min(sx + 1, im.w - 1), sy1 = min(sy + 1, im.h - 1);
     const int a0 = im.xk[2 * ox], a1 = im.xk[2 * ox + 1];
     const int b0 = im.yk[2 * oy], b1 = im.yk[2 * oy + 1];
-    const uint8_t* r0 = src + static_cast<size_t>(sy) * im.stride;
-    const uint8_t* r1 = src + static_cast<size_t>(sy1) * im.stride;
+    if (conv) {
+      int q00[3], q01[3], q10[3], q11[3];
+      yuv_load(im, yv, sy, sx, q00); yuv_load(im, yv, sy, sx1, q01);
+      yuv_load(im, yv, sy1, sx, q10); yuv_load(im, yv, sy1, sx1, q11);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const int h0 = r0[sx * 3 + c] * a0 + r0[sx1 * 3 + c] * a1;
-      const int h1 = r1[sx * 3 + c] * a0 + r1[sx1 * 3 + c] * a1;
-      u[c] = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
+      for (int c = 0; c < 3; ++c) {
+        const int h0 = q00[c] * a0 + q01[c] * a1;
+        const int h1 = q10[c] * a0 + q11[c] * a1;
+        u[c] = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
+      }
+    } else {
+      const uint8_t* r0 = src + static_cast<size_t>(sy) * im.stride;
+      const uint8_t* r1 = src + static_cast<size_t>(sy1) * im.stride;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const int h0 = r0[sx * 3 + c] * a0 + r0[sx1 * 3 + c] * a1;
+        const int h1 = r1[sx * 3 + c] * a0 + r1[sx1 * 3 + c] * a1;
+        u[c] = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
+      }
     }
   }
   emit_pixel<E>(p, im, img, oy, ox, u);
@@ -433,14 +511,18 @@ PreprocessPlan::~PreprocessPlan() {
   if (d_tables) cudaFree(d_tables);
 }
 
-static int fill_params(const PreprocessPlan& pl, const vpb_frame* frames, int convention, void* out, uint8_t* out_u8,
-                       PreParams& p) {
+// The parameter block of a call (base PreParams + the per-image format fields); returns whether any image is YUV.
+static int fill_params(const PreprocessPlan& pl, const vpb_frame_fmt* frames, int convention, void* out, uint8_t* out_u8,
+                       PreParamsYuv& p, bool& yuv) {
   if (pl.n < 1 || (pl.n > 1 && pl.out_lo)) {
     vpb_set_error("preprocess: batch %d (1..%d, 16-bit output only)", pl.n, kMaxBatch);
     return VPB_ERR_ARG;
   }
   p.out_lo = pl.out_lo;
   p.out_pitch = pl.out_pitch; p.out_c = pl.out_c;
+  // a YUV image converts to the channel order the convention takes as input
+  const int bgr = (convention == VPB_CONV_BGR_NOSWAP || convention == VPB_CONV_BGR_SWAP) ? 1 : 0;
+  yuv = false;
   for (int i = 0; i < kMaxBatch; ++i) {
     const int k = i < pl.n ? i : 0;
     PreImg& im = p.im[i];
@@ -450,6 +532,11 @@ static int fill_params(const PreprocessPlan& pl, const vpb_frame* frames, int co
     im.h = g.h; im.w = g.w; im.OH = g.OH; im.OW = g.OW; im.out_x0 = g.x0; im.out_y0 = g.y0;
     im.xb = pl.d_tables + t.xb; im.xk = pl.d_tables + t.xk; im.xks = t.xks;
     im.yb = pl.d_tables + t.yb; im.yk = pl.d_tables + t.yk; im.yks = t.yks;
+    PreYuv& y = p.yuv[i];
+    y.fmt = frames[k].format; y.bgr = bgr;
+    y.uv = y.fmt == VPB_PIX_NV12 ? frames[k].uv : nullptr;
+    y.uv_stride = y.fmt == VPB_PIX_NV12 ? frames[k].uv_stride : 0;
+    yuv |= y.fmt != VPB_PIX_PACKED;
   }
   p.mode = pl.mode;
   p.out_img = static_cast<size_t>(pl.out_rows) * p.out_pitch * pl.out_c;   // whole canvases
@@ -466,32 +553,39 @@ static int fill_params(const PreprocessPlan& pl, const vpb_frame* frames, int co
   return VPB_OK;
 }
 
-// The kernel of a resize mode, element type and tap capacity: the PIL kernel (params, rows_cap, pitch, TY) for the PIL
-// modes, else the direct kernel (params); the other member is NULL.
+// The kernel of a resize mode, element type, tap capacity and input kind (YUV: the call has a YUV image): the PIL
+// kernel (params, rows_cap, pitch, TY) for the PIL modes, else the direct kernel (params); the other member is NULL.
+template <bool YUV>
 struct PreKernel {
-  void (*pil)(PreParams, int, int, int);
-  void (*direct)(PreParams);
+  void (*pil)(PreParamsOf<YUV>, int, int, int);
+  void (*direct)(PreParamsOf<YUV>);
   const void* func() const { return pil ? reinterpret_cast<const void*>(pil) : reinterpret_cast<const void*>(direct); }
 };
-static PreKernel pre_kernel(int mode, int dtype, int xt) {
+template <bool YUV>
+static PreKernel<YUV> pre_kernel(int mode, int dtype, int xt) {
   return dispatch_dtype(dtype, [&](auto tag) {
     using E = decltype(tag);
-    if (!is_pil(mode)) return PreKernel{nullptr, preprocess_direct_kernel<E>};
-    return PreKernel{xt == 16 ? preprocess_pil_kernel<E, 16> : preprocess_pil_kernel<E, 32>, nullptr};
+    if (!is_pil(mode)) return PreKernel<YUV>{nullptr, preprocess_direct_kernel<E, YUV>};
+    return PreKernel<YUV>{xt == 16 ? preprocess_pil_kernel<E, 16, YUV> : preprocess_pil_kernel<E, 32, YUV>, nullptr};
   });
 }
+static const void* pre_func(int mode, int dtype, int xt, bool yuv) {
+  return yuv ? pre_kernel<true>(mode, dtype, xt).func() : pre_kernel<false>(mode, dtype, xt).func();
+}
 
-// Re-point the captured pre-process node at other source frames (same geometries): lets the frame graph be replayed
-// on any device buffers without re-capturing.
-int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame* frames,
+// Re-point the captured pre-process node at other source frames (same geometries and formats): lets the frame graph be
+// replayed on any device buffers without re-capturing.  The node's kernel takes PreParams (packed-only call) or the
+// whole PreParamsYuv; PreParams is its first sub-object, so one pointer serves both.
+int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames,
                                       int convention, int dtype, void* out, uint8_t* out_u8) const {
-  PreParams p;
-  const int rc = fill_params(*this, frames, convention, out, out_u8, p);
+  PreParamsYuv p;
+  bool yuv = false;
+  const int rc = fill_params(*this, frames, convention, out, out_u8, p, yuv);
   if (rc) return rc;
   int rc_ = rows_cap, pitch_ = pitch, ty_ = TY;
-  void* args[4] = {&p, &rc_, &pitch_, &ty_};
+  void* args[4] = {static_cast<PreParams*>(&p), &rc_, &pitch_, &ty_};
   cudaKernelNodeParams kp{};
-  kp.func = const_cast<void*>(pre_kernel(mode, dtype, xt).func());
+  kp.func = const_cast<void*>(pre_func(mode, dtype, xt, yuv));
   kp.kernelParams = args;
   kp.extra = nullptr;
   if (is_pil(mode)) {
@@ -507,28 +601,74 @@ int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node
   return VPB_OK;
 }
 
-int PreprocessPlan::launch(const vpb_frame* frames, int convention, int dtype, void* out, uint8_t* out_u8,
-                           cudaStream_t stream) const {
-  PreParams p;
-  const int rc = fill_params(*this, frames, convention, out, out_u8, p);
-  if (rc) return rc;
-  const PreKernel k = pre_kernel(mode, dtype, xt);
+template <bool YUV>
+static int launch_pre(const PreprocessPlan& pl, const PreParamsYuv& p, int dtype, cudaStream_t stream) {
+  const PreKernel<YUV> k = pre_kernel<YUV>(pl.mode, dtype, pl.xt);
   if (k.pil) {
-    dim3 grid((OWmax + kTX - 1) / kTX, (OHmax + TY - 1) / TY, n);
+    dim3 grid((pl.OWmax + kTX - 1) / kTX, (pl.OHmax + pl.TY - 1) / pl.TY, pl.n);
     {
       std::lock_guard<std::mutex> g(init_mutex());
       bool* done = device_flag(kInitPreprocess);
       if (!*done) {
-        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<BF16, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<F16, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<BF16, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<F16, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<BF16, 16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<F16, 16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<BF16, 32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<F16, 32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<BF16, 16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<F16, 16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<BF16, 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPB_CUDA_OK(cudaFuncSetAttribute(preprocess_pil_kernel<F16, 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         *done = true;
       }
     }
-    VPB_CUDA_OK(launch_k(k.pil, grid, dim3(kPreThreads), smem_bytes, stream, p, rows_cap, pitch, TY));
+    VPB_CUDA_OK(launch_k(k.pil, grid, dim3(kPreThreads), pl.smem_bytes, stream, p, pl.rows_cap, pl.pitch, pl.TY));
   } else {
-    VPB_CUDA_OK(launch_k(k.direct, dim3((OWmax + 255) / 256, OHmax, n), dim3(256), 0, stream, p));
+    VPB_CUDA_OK(launch_k(k.direct, dim3((pl.OWmax + 255) / 256, pl.OHmax, pl.n), dim3(256), 0, stream, p));
+  }
+  return VPB_OK;
+}
+
+int PreprocessPlan::launch(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8,
+                           cudaStream_t stream) const {
+  PreParamsYuv p;
+  bool yuv = false;
+  const int rc = fill_params(*this, frames, convention, out, out_u8, p, yuv);
+  if (rc) return rc;
+  return yuv ? launch_pre<true>(*this, p, dtype, stream) : launch_pre<false>(*this, p, dtype, stream);
+}
+
+int frame_fmt_check(const vpb_frame_fmt& f, const char* who, int k) {
+  if (f.format < VPB_PIX_PACKED || f.format > VPB_PIX_YUYV) {
+    vpb_set_error("%s: frame %d: unknown format %d (VPB_PIX_PACKED, _NV12, _UYVY or _YUYV)", who, k, f.format);
+    return VPB_ERR_ARG;
+  }
+  static const char* kName[4] = {"packed", "NV12", "UYVY", "YUYV"};
+  if (f.format == VPB_PIX_PACKED) {             // the messages of vpb_frame
+    if (!f.data) { vpb_set_error("%s: frame %d is NULL", who, k); return VPB_ERR_ARG; }
+    if (f.h <= 0 || f.w <= 0 || f.stride < 3 * f.w) {
+      vpb_set_error("%s: frame %d: bad geometry h %d, w %d, stride %d (need h, w > 0 and stride >= 3*w)", who, k, f.h,
+                    f.w, f.stride);
+      return VPB_ERR_ARG;
+    }
+    return VPB_OK;
+  }
+  const char* nm = kName[f.format];
+  if (!f.data) { vpb_set_error("%s: frame %d is NULL (%s data)", who, k, nm); return VPB_ERR_ARG; }
+  if (f.format == VPB_PIX_NV12 && !f.uv) { vpb_set_error("%s: frame %d: NV12 uv plane is NULL", who, k); return VPB_ERR_ARG; }
+  if (f.h <= 0 || f.w <= 0 || (f.w & 1) || (f.format == VPB_PIX_NV12 && (f.h & 1))) {
+    vpb_set_error("%s: frame %d: bad %s size h %d, w %d (need h, w > 0, w even%s)", who, k, nm, f.h, f.w,
+                  f.format == VPB_PIX_NV12 ? ", h even" : "");
+    return VPB_ERR_ARG;
+  }
+  const int min_stride = f.format == VPB_PIX_NV12 ? f.w : 2 * f.w;
+  if (f.stride < min_stride) {
+    vpb_set_error("%s: frame %d: %s stride %d < %d (%s)", who, k, nm, f.stride, min_stride,
+                  f.format == VPB_PIX_NV12 ? "w" : "2*w");
+    return VPB_ERR_ARG;
+  }
+  if (f.format == VPB_PIX_NV12 && f.uv_stride < f.w) {
+    vpb_set_error("%s: frame %d: NV12 uv_stride %d < w %d", who, k, f.uv_stride, f.w);
+    return VPB_ERR_ARG;
   }
   return VPB_OK;
 }
@@ -564,6 +704,30 @@ extern "C" int vpb_preprocess(const uint8_t* src_dev, int h, int w, int stride, 
   g.h = h; g.w = w;
   int rc = plan.configure(&g, 1, resize_mode);
   if (rc != VPB_OK) return rc;
-  const vpb_frame f{src_dev, h, w, stride};
+  const vpb_frame_fmt f = vpb::packed_frame(vpb_frame{src_dev, h, w, stride});
   return plan.launch(&f, convention, dtype, out_dev, out_u8_dev, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_preprocess_fmt(const vpb_frame_fmt* frame_dev, int resize_mode, int convention, int dtype,
+                                  void* out_dev, uint8_t* out_u8_dev, void* stream) {
+  static const char* who = "vpb_preprocess_fmt";
+  if (!frame_dev || !out_dev) { vpb_set_error("%s: bad arguments (NULL descriptor or output)", who); return VPB_ERR_ARG; }
+  if (convention < VPB_CONV_RGB || convention > VPB_CONV_RGB_UNIT) {
+    vpb_set_error("%s: unknown convention %d", who, convention);
+    return VPB_ERR_ARG;
+  }
+  if (resize_mode < VPB_RESIZE_NONE || resize_mode > VPB_RESIZE_PIL_BILINEAR) {
+    vpb_set_error("%s: unknown resize mode %d", who, resize_mode);
+    return VPB_ERR_ARG;
+  }
+  int rc = vpb::frame_fmt_check(*frame_dev, who, 0);
+  if (rc) return rc;
+  vpb::PreGeom g;
+  g.h = frame_dev->h; g.w = frame_dev->w;
+  rc = vpb::PreprocessPlan::check(g, resize_mode, who, 0);
+  if (rc) return rc;
+  static thread_local vpb::PreprocessPlan plan;
+  rc = plan.configure(&g, 1, resize_mode);
+  if (rc != VPB_OK) return rc;
+  return plan.launch(frame_dev, convention, dtype, out_dev, out_u8_dev, static_cast<cudaStream_t>(stream));
 }

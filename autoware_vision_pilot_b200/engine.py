@@ -96,6 +96,8 @@ def _bind():
     lib.vp_engine_read_resized_at.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     for fn in ("vp_engine_infer_frames", "vp_engine_submit_frames", "vp_engine_infer_device_frames"):
         getattr(lib, fn).argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int]
+    for fn in ("vp_engine_infer_frames_fmt", "vp_engine_submit_frames_fmt", "vp_engine_infer_device_frames_fmt"):
+        getattr(lib, fn).argtypes = [C.c_void_p, C.POINTER(L.FrameFmt), C.c_int]
     lib.vp_engine_tap_dev.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(_TapView)]
     lib.vp_engine_stream.argtypes = [C.c_void_p]
     lib.vp_engine_stream.restype = C.c_void_p
@@ -226,16 +228,49 @@ class Engine:
     def _descs(frames: Sequence[np.ndarray]):
         return L.frame_descs([(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames])
 
-    def infer_frames(self, frames: Sequence[np.ndarray]) -> None:
-        """`batch` uint8 [h_k, w_k, 3] host frames, each of its own size (a mixed camera rig), in one call; outputs of
-        frame k are sample k."""
-        frames = self._check_frames(frames, allow_copy=True)
-        L.check(self._lib.vp_engine_infer_frames(self._h, self._descs(frames), len(frames)), "vp_engine_infer_frames")
+    def _fmt_descs(self, frames, allow_copy: bool):
+        """`batch` frames, packed arrays and NV12 / UYVY / YUYV objects mixed, as a vpb_frame_fmt array (and the arrays
+        it points into, to keep alive for the call)"""
+        frames = list(frames)
+        if len(frames) != self.batch:
+            raise ValueError(f"{len(frames)} frame(s) for an engine of batch {self.batch}")
+        arr, keep = (L.FrameFmt * len(frames))(), []
+        for k, f in enumerate(frames):
+            d, alive = f.desc(allow_copy) if isinstance(f, L.YUV_TYPES) else L.packed_desc(self._check_frame(f, allow_copy))
+            arr[k] = d
+            keep.append(alive)
+        return arr, keep
 
-    def submit_frames(self, frames: Sequence[np.ndarray]) -> None:
+    def infer_frames(self, frames) -> None:
+        """`batch` host frames, each of its own size (a mixed camera rig), in one call; outputs of frame k are sample k.
+        A frame is a uint8 [h_k, w_k, 3] array in the convention's channel order, or a camera-native NV12 / UYVY / YUYV
+        object (autoware_vision_pilot_b200._lib), converted inside the pre-process exactly as cv2.cvtColor would."""
+        frames = list(frames)
+        if not any(isinstance(f, L.YUV_TYPES) for f in frames):
+            frames = self._check_frames(frames, allow_copy=True)
+            L.check(self._lib.vp_engine_infer_frames(self._h, self._descs(frames), len(frames)), "vp_engine_infer_frames")
+            return
+        arr, _keep = self._fmt_descs(frames, allow_copy=True)
+        L.check(self._lib.vp_engine_infer_frames_fmt(self._h, arr, len(frames)), "vp_engine_infer_frames_fmt")
+
+    def submit_frames(self, frames) -> None:
         """Asynchronous infer_frames() (pinned frames: pinned_frames(shapes)); sync() completes it."""
-        frames = self._check_frames(frames, allow_copy=False)
-        L.check(self._lib.vp_engine_submit_frames(self._h, self._descs(frames), len(frames)), "vp_engine_submit_frames")
+        frames = list(frames)
+        if not any(isinstance(f, L.YUV_TYPES) for f in frames):
+            frames = self._check_frames(frames, allow_copy=False)
+            L.check(self._lib.vp_engine_submit_frames(self._h, self._descs(frames), len(frames)), "vp_engine_submit_frames")
+            return
+        arr, _keep = self._fmt_descs(frames, allow_copy=False)
+        L.check(self._lib.vp_engine_submit_frames_fmt(self._h, arr, len(frames)), "vp_engine_submit_frames_fmt")
+
+    def infer_device_frames_fmt(self, descs: Sequence[Sequence[int]]) -> None:
+        """`batch` device frames as (format, data_ptr, h, w, stride, uv_ptr, uv_stride) tuples (format one of _lib.PIX_*,
+        uv for NV12 only), each of its own format and geometry, in one asynchronous call."""
+        descs = list(descs)
+        if len(descs) != self.batch:
+            raise ValueError(f"{len(descs)} frame(s) for an engine of batch {self.batch}")
+        L.check(self._lib.vp_engine_infer_device_frames_fmt(self._h, L.frame_fmt_descs(descs), len(descs)),
+                "vp_engine_infer_device_frames_fmt")
 
     def infer_device_frames(self, descs: Sequence[Sequence[int]]) -> None:
         """`batch` device frames as (data_ptr, h, w, stride) tuples, each of its own geometry, in one asynchronous
@@ -261,20 +296,33 @@ class Engine:
         a = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(size,))
         return a.reshape(h, w, 3) if n is None else a.reshape(n, h, w, 3)
 
-    def pinned_frames(self, shapes: Sequence[Sequence[int]]) -> List[np.ndarray]:
-        """Views [h_k, w_k, 3] into one engine-owned pinned host buffer, one per (h, w) in shapes
-        (submit_frames(views))."""
-        shapes = [(int(h), int(w)) for h, w in shapes]
-        if any(h <= 0 or w <= 0 for h, w in shapes):
-            raise ValueError(f"frame shapes must be positive, got {shapes}")
-        sizes = [h * w * 3 for h, w in shapes]
-        p = self._lib.vp_engine_pinned_frame(self._h, max(sum(sizes), 1))
+    def pinned_frames(self, shapes: Sequence[Sequence]) -> List:
+        """Views into one engine-owned pinned host buffer, one per entry of shapes (submit_frames(views)): (h, w) or
+        (h, w, "packed") gives a [h, w, 3] array, (h, w, "nv12") an NV12 object (y [h, w], uv [h/2, w]), (h, w, "uyvy")
+        / (h, w, "yuyv") a UYVY / YUYV object ([h, w, 2]).  Fill the arrays in place."""
+        kinds = {"packed": 3, "nv12": 1.5, "uyvy": 2, "yuyv": 2}
+        spec = []
+        for s in shapes:
+            h, w, kind = int(s[0]), int(s[1]), (s[2] if len(s) > 2 else "packed")
+            if kind not in kinds:
+                raise ValueError(f"unknown frame format {kind!r} (one of {sorted(kinds)})")
+            if h <= 0 or w <= 0 or (kind != "packed" and (w % 2 or (kind == "nv12" and h % 2))):
+                raise ValueError(f"bad {kind} frame shape {h}x{w}")
+            spec.append((h, w, kind, int(h * w * kinds[kind])))
+        total = max(sum(n for *_, n in spec), 1)
+        p = self._lib.vp_engine_pinned_frame(self._h, total)
         if not p:
             raise RuntimeError(L.last_error())
-        a = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(max(sum(sizes), 1),))
+        a = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(total,))
         views, off = [], 0
-        for (h, w), n in zip(shapes, sizes):
-            views.append(a[off:off + n].reshape(h, w, 3))
+        for h, w, kind, n in spec:
+            v = a[off:off + n]
+            if kind == "packed":
+                views.append(v.reshape(h, w, 3))
+            elif kind == "nv12":
+                views.append(L.NV12(v[:h * w].reshape(h, w), v[h * w:].reshape(h // 2, w)))
+            else:
+                views.append((L.UYVY if kind == "uyvy" else L.YUYV)(v.reshape(h, w, 2)))
             off += n
         return views
 

@@ -137,6 +137,19 @@ int vp_engine_infer_device_batch(vp_engine* e, const uint8_t* const* frames_dev,
 int vp_engine_infer_frames(vp_engine* e, const vpb_frame* frames_host, int n);
 int vp_engine_submit_frames(vp_engine* e, const vpb_frame* frames_host, int n);
 int vp_engine_infer_device_frames(vp_engine* e, const vpb_frame* frames_dev, int n);
+/* The three *_frames calls on camera-native frames (vpb_frame_fmt, vp_b200_ops.h): NV12 from NVDEC or an ISP, UYVY
+ * (ROS "yuv422", GMSL) or YUYV (ROS "yuv422_yuy2", UVC), mixed with packed frames in one call, each descriptor with
+ * its own format and geometry.  They replace the caller's cv::cvtColor (cv_bridge::toCvCopy(msg, BGR8),
+ * run_model_node.cpp:70) before the call: the YUV frame converts inside the pre-process to the channel order of the
+ * engine's convention, and every output is byte-equal to the packed call on the cvtColor-converted frame.  Host frames
+ * upload only their valid bytes per row (2w per 4:2:2 row, w per Y and UV row of NV12: 1.5 or 2 bytes per pixel
+ * instead of 3).  Checks as for the *_frames calls plus those of vpb_preprocess_fmt; VP_SRC_OVERLAY needs the camera
+ * frame as packed pixels, so an overlay engine given a YUV frame returns VPB_ERR_ARG before any device work.  The
+ * frame graph's key adds each frame's format and uv_stride: new data / uv pointers re-point the captured nodes, a new
+ * format captures again.  The split-fp16 mode takes them with n = 1. */
+int vp_engine_infer_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n);
+int vp_engine_submit_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n);
+int vp_engine_infer_device_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_dev, int n);
 /* Copy the raw fp32 tensor of one model to its host buffer (after a device/async inference). */
 int vp_engine_fetch_raw(vp_engine* e, int model_idx);
 

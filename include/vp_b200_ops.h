@@ -46,6 +46,27 @@ enum { VPB_ALGO_TILE = 0, VPB_ALGO_LINEAR = 1 };
  * channels, `stride` bytes per row (>= 3*w).  Each frame of a call may have its own h, w and stride. */
 typedef struct { const uint8_t* data; int h, w, stride; } vpb_frame;
 
+/* A camera frame in the layout the camera or decoder delivers it (vp_engine_*_frames_fmt, vp_autospeed_*_frames_fmt,
+ * vpb_preprocess_fmt).  The YUV layouts are converted inside the pre-process with OpenCV's BT.601 limited-range
+ * fixed-point arithmetic (COLOR_YUV2RGB_NV12 / _UYVY / _YUYV, or the COLOR_YUV2BGR_* codes for the BGR conventions),
+ * chroma shared by each 2x2 block (NV12) or horizontal pair (UYVY, YUYV) without interpolation: the result is
+ * byte-equal to the caller's cv::cvtColor followed by the packed call.
+ *   NV12  data = the Y plane [h][stride], uv = the interleaved U,V plane [h/2][uv_stride] (anywhere: it need not
+ *         follow the Y plane); h and w even
+ *   UYVY  data [h][stride], each pair of pixels U Y0 V Y1 (GMSL cameras, ROS "yuv422"); w even
+ *   YUYV  data [h][stride], each pair of pixels Y0 U Y1 V (UVC cameras, ROS "yuv422_yuy2"); w even
+ * A crop of a YUV frame must start on an even row and column: the descriptor has no way to state another chroma
+ * phase, and it is not detected. */
+enum { VPB_PIX_PACKED = 0, /* a vpb_frame: 3 interleaved channels, RGB or BGR as the convention says */
+       VPB_PIX_NV12 = 1, VPB_PIX_UYVY = 2, VPB_PIX_YUYV = 3 };
+typedef struct {
+  int format;                 /* VPB_PIX_* */
+  const uint8_t* data;        /* PACKED / UYVY / YUYV: the frame; NV12: the Y plane [h][stride] */
+  int h, w, stride;           /* bytes per row of data: >= 3w (PACKED), >= 2w (UYVY, YUYV), >= w (NV12) */
+  const uint8_t* uv;          /* NV12: the interleaved U,V plane [h/2][uv_stride]; ignored otherwise */
+  int uv_stride;              /* NV12: >= w */
+} vpb_frame_fmt;
+
 const char* vpb_last_error(void);
 void vpb_set_error(const char* fmt, ...);
 
@@ -181,6 +202,14 @@ enum { VPB_CONV_RGB = 0, VPB_CONV_BGR_NOSWAP = 1, VPB_CONV_BGR_SWAP = 2,
        VPB_CONV_RGB_UNIT = 3 /* RGB in, x/255 only (transforms.ToTensor, auto_speed_infer.py:50) */ };
 int vpb_preprocess(const uint8_t* src_dev, int h, int w, int stride, int resize_mode, int convention,
                    int dtype, void* out_dev, uint8_t* out_u8_dev, void* stream);
+/* vpb_preprocess of one frame in any VPB_PIX_* layout (device pointers in *frame_dev, the descriptor itself on the
+ * host).  A YUV frame converts to RGB for VPB_CONV_RGB / _RGB_UNIT and to BGR for VPB_CONV_BGR_NOSWAP / _SWAP, so the
+ * result equals vpb_preprocess on cv::cvtColor(frame, COLOR_YUV2{RGB,BGR}_*).  VPB_ERR_ARG before any device work,
+ * the message naming the call and frame 0, for an unknown format or convention, NULL data (or NULL uv for NV12), odd w
+ * (odd h for NV12), a stride below the format's minimum, uv_stride < w (NV12), a frame other than 640x320 under
+ * VPB_RESIZE_NONE, or a Pillow filter of more than 32 taps. */
+int vpb_preprocess_fmt(const vpb_frame_fmt* frame_dev, int resize_mode, int convention, int dtype, void* out_dev,
+                       uint8_t* out_u8_dev, void* stream);
 /* Host-only: the integer coefficient tables the kernel uses (bounds[out_size],
  * coeffs[out_size*ksize]); lets a CPU test pin them against Pillow / OpenCV without a GPU. */
 int vpb_resize_tables_host(int mode, int in_size, int out_size, int* bounds, int* coeffs,

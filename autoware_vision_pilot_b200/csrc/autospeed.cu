@@ -1050,6 +1050,11 @@ extern "C" int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flop
   return VPB_OK;
 }
 
+extern "C" int vp_autospeed_conv_args(vp_autospeed* e, int op, vpb_conv_args* out, const char** name) {
+  if (!e) { vpb_set_error("vp_autospeed_conv_args: NULL engine"); return VPB_ERR_ARG; }
+  return e->conv_args_of(op, out, name, "vp_autospeed_conv_args");
+}
+
 extern "C" long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {
   if (!e || !name) return VPB_ERR_ARG;
   return e->read_tap(name, dst, cap, c, h, w);

@@ -895,6 +895,11 @@ extern "C" int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* f
   return VPB_OK;
 }
 
+extern "C" int vp_engine_conv_args(vp_engine* e, int op, vpb_conv_args* out, const char** name) {
+  if (!e) { vpb_set_error("vp_engine_conv_args: NULL engine"); return VPB_ERR_ARG; }
+  return e->conv_args_of(op, out, name, "vp_engine_conv_args");
+}
+
 extern "C" int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flops, int* launches) {
   if (!e || !ms || reps <= 0) return VPB_ERR_ARG;
   if (!e->n_frames) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }

@@ -365,11 +365,25 @@ int EngineRuntime::append_conv(const std::string& name, const vpb_conv_args& a) 
   if (rc != VPB_OK) { const std::string e = vpb_last_error(); vpb_set_error("%s: %s", name.c_str(), e.c_str()); return rc; }
   ConvPlan* pp = plan.get();
   plans.push_back(std::move(plan));
+  conv_list.push_back(a);
   OpRec op; op.name = name; op.flops = pp->flops; op.gemm = true; op.lane = cur_lane;
+  op.conv = static_cast<int>(plans.size()) - 1;
   op.kind = a.algo == VPB_ALGO_LINEAR ? 2 : 1;
   op.kname = "conv_wgmma_kernel";
   op.launch = [pp](cudaStream_t s) { return conv_plan_launch(pp, s); };
   ops.push_back(std::move(op));
+  return VPB_OK;
+}
+
+int EngineRuntime::conv_args_of(int op, vpb_conv_args* out, const char** name, const char* who) const {
+  if (!out) { vpb_set_error("%s: NULL output", who); return VPB_ERR_ARG; }
+  if (op < 0 || op >= static_cast<int>(ops.size())) {
+    vpb_set_error("%s: op %d out of range (the engine has %d ops)", who, op, static_cast<int>(ops.size()));
+    return VPB_ERR_ARG;
+  }
+  if (ops[op].conv < 0) { vpb_set_error("%s: op %d (%s) is not a convolution", who, op, ops[op].name.c_str()); return VPB_ERR_ARG; }
+  *out = conv_list[ops[op].conv];
+  if (name) *name = ops[op].name.c_str();
   return VPB_OK;
 }
 

@@ -79,6 +79,7 @@ struct OpRec {
   int kind = 0;   // 0 = not a convolution GEMM; conv_wgmma_kernel with 1 = VPB_ALGO_TILE, 2 = VPB_ALGO_LINEAR
   int lane = 0;   // execution lane (= index of the model that owns the op); lanes run concurrently; -1: after every
                   // lane has joined the engine stream
+  int conv = -1;  // index into EngineRuntime::plans / conv_list of a convolution op (append_conv), -1 otherwise
   // Set on the ops that read the frames of the call: re-point the op's captured kernel node at the current frames.
   std::function<int(cudaGraphExec_t, cudaGraphNode_t)> repoint;
 };
@@ -131,7 +132,8 @@ struct EngineRuntime {
   std::vector<void*> dev_allocs, host_allocs;
   size_t weight_bytes = 0, act_bytes = 0;
   std::vector<std::unique_ptr<ConvPlan>> plans;
-  std::vector<OpRec> ops;                 // every launch of a call, in order; op 0 is the pre-process
+  std::vector<vpb_conv_args> conv_list;   // [plan] the arguments each plan was built from
+  std::vector<OpRec> ops;                // every launch of a call, in order; op 0 is the pre-process
   std::map<std::string, Tap> taps;
   PreprocessPlan pre;
   Frames frames{};                        // device frames of the current / last call
@@ -180,6 +182,9 @@ struct EngineRuntime {
                           const float* bias, int act, int mode, const Tens* in2 = nullptr, const void* w2 = nullptr) const;
   // build the plan of one wgmma convolution, keep it, append its launch on lane cur_lane (errors are prefixed with name)
   int append_conv(const std::string& name, const vpb_conv_args& a);
+  // a copy of the vpb_conv_args append_conv built op `op` from (device pointers included) and the op's name;
+  // VPB_ERR_ARG, the message prefixed with who, for an op out of range or one that is not a convolution
+  int conv_args_of(int op, vpb_conv_args* out, const char** name, const char* who) const;
   void tap(const std::string& name, const Tens& t, int channels = 0) { taps[name] = Tap{t, channels > 0 ? channels : t.C}; }
   // Copy n host frames to d_frame (grown on demand), plane after plane, frame after frame, each row with the pitch of its
   // valid bytes (3w packed, 2w UYVY / YUYV, w for the Y and the UV rows of NV12): only those bytes of every row are read

@@ -200,6 +200,11 @@ int vp_engine_get_stats(const vp_engine* e, vp_engine_stats* s);
  * names[i] point into engine-owned storage. */
 int vp_engine_profile(vp_engine* e, int max_ops, float* ms, double* flops, const char** names,
                       int* is_gemm, int* n_ops);
+/* For op-level testing: the vpb_conv_args convolution op `op` (0 .. n_launches-1, the launch order of
+ * vp_engine_profile) was built from, device pointers included, so that a test can re-run the op with vpb_conv_gemm on
+ * the engine's own tensors after a call; name (may be NULL) = the op's name as vp_engine_profile reports it, in
+ * engine-owned storage.  VPB_ERR_ARG for an op out of range or one that is not a convolution. */
+int vp_engine_conv_args(vp_engine* e, int op, vpb_conv_args* out, const char** name);
 /* Device time of all launches of ONE convolution kernel (kind as in is_gemm above) of the frame, issued
  * back to back `reps` times between a single CUDA-event pair on the engine's stream (after one untimed
  * pass): ms = total, flops = algorithmic 2*MAC of the timed launches.  This is the "average launch

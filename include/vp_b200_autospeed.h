@@ -82,6 +82,10 @@ int vp_autospeed_raw_at(vp_autospeed* e, int sample, const float** raw_host, con
                         int* anchors);
 /* launches per call (any batch) and the FLOPs of all samples of a call */
 int vp_autospeed_stats(vp_autospeed* e, int* n_launches, double* flops);
+/* For op-level testing, as vp_engine_conv_args (vp_b200.h): the vpb_conv_args of convolution op `op` (0 .. n_launches-1,
+ * launch order) with its device pointers, and the op's name (may be NULL).  VPB_ERR_ARG for an op out of range or one
+ * that is not a convolution. */
+int vp_autospeed_conv_args(vp_autospeed* e, int op, vpb_conv_args* out, const char** name);
 /* intermediate tensors for the parity tests ("canvas", "p1".."p5", "p5_ctx", "p5_sppf", "n3".."n5", "head0".."head2";
  * "<name>@k" = sample k, default 0) as fp32 NCHW; returns the element count (dst == NULL: size query) */
 long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* dst, long cap, int* c, int* h, int* w);

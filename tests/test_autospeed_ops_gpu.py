@@ -36,7 +36,7 @@ import torch
 import torch.nn.functional as F
 
 from autoware_vision_pilot_b200 import _lib as L
-from tests.test_encoder_ops_gpu import assert_within, rand, same_bits, tdt, ulp
+from tests.test_encoder_ops_gpu import ACT_ERR, act64, assert_within, rand, same_bits, tdt, ulp
 
 pytestmark = pytest.mark.gpu
 
@@ -633,23 +633,57 @@ def silu64(x):
     return x * torch.sigmoid(x)
 
 
-def conv64(x, w, b, stride):
-    """float64 conv of NHWC x with w [taps][Cout][Cin] (pad 1 for 3x3) and its S = sum |w x| + |b|: NHWC both."""
-    k = 3 if w.shape[0] == 9 else 1
-    wt = w.double().view(k, k, w.shape[1], w.shape[2]).permute(2, 3, 0, 1)
-    xd = x.double().permute(0, 3, 1, 2)
-    bd = None if b is None else b.double()
-    pre = F.conv2d(xd, wt, bd, stride=stride, padding=k // 2).permute(0, 2, 3, 1)
-    S = F.conv2d(xd.abs(), wt.abs(), None if b is None else bd.abs(), stride=stride, padding=k // 2).permute(0, 2, 3, 1)
+def conv64(x, w, b, stride=1, phases=1, x2=None, w2=None):
+    """float64 conv of NHWC x with w [taps][Cout][Cin] and its S = sum |w x| + |b|: NHWC both, on x's device.
+      phases 1:             taps 9 (pad 1) or 1, at `stride`;
+      phases 4, taps 1:     ConvTranspose2d k2 s2, out[2h + a][2w + c] = w[a * 2 + c] x[h][w];
+      phases 4, taps 4:     upconv, out[2h + a][2w + c] = sum_t w[(a * 2 + c) * 4 + t] x[h + t // 2 - 1 + a][w + t % 2 - 1 + c];
+      x2, w2 [1 | 9][Cout][Cin2]: a second input at the output resolution through a 1x1 or a 3x3 (pad 1) convolution;
+      b [Cout], or [9][Cout] (upconv: the row of the output pixel's border class cy * 3 + cx), or None."""
+    def lin(xd, wd, x2d, w2d):
+        Cout, Cin = wd.shape[1:]
+        xc = xd.permute(0, 3, 1, 2)
+        if phases == 1:
+            k = 3 if wd.shape[0] == 9 else 1
+            y = F.conv2d(xc, wd.view(k, k, Cout, Cin).permute(2, 3, 0, 1), stride=stride, padding=k // 2)
+        elif wd.shape[0] == 4:
+            y = F.conv_transpose2d(xc, wd.view(2, 2, Cout, Cin).permute(3, 2, 0, 1), stride=2)
+        else:
+            B, _, H, W = xc.shape
+            xp = F.pad(xc, (1, 1, 1, 1))
+            y = xc.new_zeros(B, Cout, 2 * H, 2 * W)
+            for a in range(2):
+                for c in range(2):
+                    k = wd[(a * 2 + c) * 4:(a * 2 + c + 1) * 4].view(2, 2, Cout, Cin).permute(2, 3, 0, 1)
+                    y[:, :, a::2, c::2] = F.conv2d(xp, k)[:, :, a:a + H, c:c + W]
+        if x2d is not None:
+            k2 = 3 if w2d.shape[0] == 9 else 1
+            y = y + F.conv2d(x2d.permute(0, 3, 1, 2), w2d.view(k2, k2, Cout, -1).permute(2, 3, 0, 1), padding=k2 // 2)
+        return y.permute(0, 2, 3, 1)
+
+    xd, wd = x.double(), w.double().to(x.device)
+    x2d = None if x2 is None else x2.double()
+    w2d = None if w2 is None else w2.double().to(x.device)
+    pre = lin(xd, wd, x2d, w2d)
+    S = lin(xd.abs(), wd.abs(), None if x2d is None else x2d.abs(), None if w2d is None else w2d.abs())
+    if b is not None:
+        bd = b.double().to(x.device)
+        if bd.dim() == 2:
+            Ho, Wo = pre.shape[1:3]
+            cy = torch.ones(Ho, dtype=torch.long, device=x.device)
+            cx = torch.ones(Wo, dtype=torch.long, device=x.device)
+            cy[0], cy[-1], cx[0], cx[-1] = 0, 2, 0, 2
+            bd = bd[cy[:, None] * 3 + cx[None, :]]
+        pre, S = pre + bd, S + bd.abs()
     return pre, S
 
 
 def conv_gate(pre, S, K, act):
-    """error of act(acc + b) before the 16-bit store, and the value"""
-    if act == L.ACT_SILU:
-        ref = silu64(pre)
-        return ref, 1.1 * (2 * K + 1) * U * S + 6 * U * torch.maximum(pre.abs(), ref.abs())
-    return pre, (2 * K + 1) * U * S
+    """error of act(acc + b) before the 16-bit store, and the value: the chain's (2K + 1) u S through the activation's
+    Lipschitz bound, plus its own error (ACT_ERR)"""
+    Lc, a = ACT_ERR[act]
+    ref = act64(pre, act)
+    return ref, Lc * (2 * K + 1) * U * S + a * U * torch.maximum(pre.abs(), ref.abs())
 
 
 def conv_case(dt, B, Hi, Wi, ldi, cin, cout, taps, seed, zero_from=None):

@@ -83,6 +83,20 @@ def test_conv_rejects_bad_arguments_without_a_gpu():
     assert lib.vpb_upconv_compose(None, None, None, None, None, None, 8, 8, 8, 0, None, None, None, None) == -1
 
 
+def test_engine_conv_args_reject_bad_arguments_without_a_gpu():
+    """The op-level introspection entries refuse a NULL engine with a message naming the call (the out-of-range and
+    not-a-convolution cases need an engine, so a GPU: tests/test_conv_ops_gpu.py)."""
+    lib = L.lib()
+    for fn in ("vp_engine_conv_args", "vp_autospeed_conv_args"):
+        f = getattr(lib, fn)
+        f.argtypes = [C.c_void_p, C.c_int, C.POINTER(L.ConvArgs), C.POINTER(C.c_char_p)]
+        a = L.ConvArgs()
+        name = C.c_char_p()
+        for op in (0, -1):
+            assert f(None, op, C.byref(a), C.byref(name)) == -1
+            assert fn in L.last_error()
+
+
 def test_encoder_ops_reject_bad_arguments_without_a_gpu():
     """Every contract violation of the encoder / context op entry points returns VPB_ERR_ARG with a message before
     any device work (so no GPU is needed to see it)."""

@@ -25,8 +25,14 @@
 namespace vpb {
 
 static constexpr int kMaxH = 128, kMaxWords = 8;      // masks up to 128 x 256
-static constexpr int kMaxPts = 2048;                  // <= 40 windows x 48 pixels per lane line
-static constexpr int kMaxGen = 256;                   // points generated from one polynomial (step 5)
+// Points of one lane line: two passes of at most H/4 windows, each at most 4 rows x 12 columns.
+static constexpr int kMaxPts = 2 * (kMaxH / 4) * 48;
+// Points generated from one polynomial: y from min_y to max_y in steps of 5 source rows.  The fitted y-limits are
+// mask rows (at most H - 1, smoothing keeps them there), so the count is at most (H-1)/H * img_h / 5 + 1, one more
+// for the rounding of the accumulated y: this bounds the source height the launcher accepts.
+static constexpr int kMaxImgH = 4320;
+static constexpr int kMaxGen = 896;
+static_assert(kMaxGen >= kMaxImgH / 5 + 2, "generated-point buffers too small for the tallest accepted source");
 
 struct LatShared {
   uint32_t bits[3][kMaxH][kMaxWords];
@@ -101,15 +107,20 @@ __device__ void warp_fit(const T* xs, const T* ys, int n, int order, bool intege
       const double k = mean / (v0[0] * v0[0] + v0[1] * v0[1] + v0[2] * v0[2]);
       c[0] = k * v0[0]; c[1] = k * v0[1]; c[2] = k * v0[2];
     } else {   // order 2, two distinct rows
-      const double y1 = static_cast<double>(node[1]);
-      const double v1[3] = {1.0, y1, y1 * y1};
-      const double g00 = v0[0] * v0[0] + v0[1] * v0[1] + v0[2] * v0[2];
-      const double g01 = v0[0] * v1[0] + v0[1] * v1[1] + v0[2] * v1[2];
-      const double g11 = v1[0] * v1[0] + v1[1] * v1[1] + v1[2] * v1[2];
-      const double b0 = sx[0] / cn[0], b1 = sx[1] / cn[1];
-      const double det = g00 * g11 - g01 * g01;
-      const double l0 = (b0 * g11 - b1 * g01) / det, l1 = (b1 * g00 - b0 * g01) / det;
-      for (int k = 0; k < 3; ++k) c[k] = l0 * v0[k] + l1 * v1[k];
+      // c = l0 v0 + l1 v1 with the 2 x 2 Gram system of the rows' basis vectors.  For neighbouring rows those are
+      // nearly parallel (sin ~ 2e-4 at rows 74 / 75), and in fp64 the cancellations lose ~1e-9 of lane_offset that
+      // cv::solve keeps.  Rows, x sums and counts are integers, so the whole solution is taken exactly in integers
+      // (|p| < 2^62, products < 2^80) and rounded only in the final quotients.
+      const long long r0 = node[0], r1 = node[1];
+      const long long u0[3] = {1, r0, r0 * r0}, u1[3] = {1, r1, r1 * r1};
+      const long long g00 = u0[0] * u0[0] + u0[1] * u0[1] + u0[2] * u0[2];
+      const long long g01 = u0[0] * u1[0] + u0[1] * u1[1] + u0[2] * u1[2];
+      const long long g11 = u1[0] * u1[0] + u1[1] * u1[1] + u1[2] * u1[2];
+      const long long s0 = llrint(sx[0]), s1 = llrint(sx[1]), n0 = llrint(cn[0]), n1 = llrint(cn[1]);
+      const long long p0 = s0 * n1 * g11 - s1 * n0 * g01, p1 = s1 * n0 * g00 - s0 * n1 * g01;   // (l0, l1) * den
+      const double den = static_cast<double>(static_cast<__int128>(n0 * n1) * (g00 * g11 - g01 * g01));
+      for (int k = 0; k < 3; ++k)
+        c[k] = static_cast<double>(static_cast<__int128>(p0) * u0[k] + static_cast<__int128>(p1) * u1[k]) / den;
     }
     return;
   }
@@ -164,7 +175,7 @@ __device__ __forceinline__ int pos_sum(uint32_t b) {
 
 // slidingWindowSearch (lane_filter.cpp:376-590) by one warp: lanes 0..3 each own one row of the (<= 4 x 12)
 // window as a bit field, counts / centroid sums are a handful of popcounts, points are appended in the
-// reference's push order (row-major inside a window).  Returns the number of points (capped at kMaxPts).
+// reference's push order (row-major inside a window).  Returns the number of points (at most kMaxPts).
 __device__ int sliding_search(const LatShared& s, uint8_t* px, uint8_t* py, int H, int W, int sx0, int sy0,
                               bool is_left) {
   const int lane = threadIdx.x & 31;
@@ -210,11 +221,11 @@ __device__ int sliding_search(const LatShared& s, uint8_t* px, uint8_t* py, int 
         syr += __shfl_xor_sync(0xffffffffu, syr, 1); syr += __shfl_xor_sync(0xffffffffu, syr, 2);
         const long sum_x = __shfl_sync(0xffffffffu, sxr, 0), sum_y = __shfl_sync(0xffffffffu, syr, 0);
         int pos = n_pts + (lane > 0 ? c0 : 0) + (lane > 1 ? c1 : 0) + (lane > 2 ? c2 : 0);
-        for (uint32_t b = bits; b; b &= b - 1) {
-          if (pos < kMaxPts) { px[pos] = static_cast<uint8_t>(x_lo + __ffs(b) - 1); py[pos] = static_cast<uint8_t>(y); }
-          ++pos;
+        for (uint32_t b = bits; b; b &= b - 1, ++pos) {
+          px[pos] = static_cast<uint8_t>(x_lo + __ffs(b) - 1);
+          py[pos] = static_cast<uint8_t>(y);
         }
-        n_pts = min(kMaxPts, n_pts + cnt);
+        n_pts += cnt;
         const float cxf = static_cast<float>(sum_x) / static_cast<float>(cnt);
         const float cyf = static_cast<float>(sum_y) / static_cast<float>(cnt);
         empty = 0;
@@ -271,16 +282,25 @@ __device__ int gen_and_warp(const double c6[6], const LatCam& cam, float* ox, fl
   up[3] = c6[3] * cam.sx;
   up[4] = c6[4] * cam.sy;
   up[5] = c6[5] * cam.sy;
-  // y = min_y + 5k (the reference accumulates y += 5 in double: exact for these magnitudes)
+  // The reference's loop: for (y = min_y; y <= max_y; y += 5) in double.  The rounded sums are not min_y + 5k, so
+  // neither the points nor their count have a closed form.  32 points per step: lane l adds 5 l times to the y of
+  // the step's first point, lane 31's y + 5 starts the next step.  y only grows, so the points kept are a prefix.
+  // kMaxGen is never reached within the launcher's limits; it only keeps the stores in bounds.
   int n = 0;
-  if (up[5] >= up[4]) n = static_cast<int>(floor((up[5] - up[4]) / 5.0)) + 1;
-  n = min(n, kMaxGen);
-  for (int k = lane; k < n; k += 32) {
-    double y = up[4];
-    for (int j = 0; j < k; ++j) y += 5.0;                 // same accumulation as the reference loop
-    const double x = (up[1] != 0.0) ? __dadd_rn(__dadd_rn(__dmul_rn(__dmul_rn(up[1], y), y), __dmul_rn(up[2], y)), up[3])
-                                    : __dadd_rn(__dmul_rn(up[2], y), up[3]);
-    warp_pt(cam.Hm, static_cast<float>(x), static_cast<float>(y), &ox[k], &oy[k]);
+  double y0 = up[4];
+  for (;;) {
+    double y = y0;
+    for (int j = 0; j < lane; ++j) y += 5.0;
+    const bool in = y <= up[5] && n + lane < kMaxGen;
+    if (in) {
+      const double x = (up[1] != 0.0) ? __dadd_rn(__dadd_rn(__dmul_rn(__dmul_rn(up[1], y), y), __dmul_rn(up[2], y)), up[3])
+                                      : __dadd_rn(__dmul_rn(up[2], y), up[3]);
+      warp_pt(cam.Hm, static_cast<float>(x), static_cast<float>(y), &ox[n + lane], &oy[n + lane]);
+    }
+    const uint32_t kept = __ballot_sync(0xffffffffu, in);
+    n += __popc(kept);
+    if (kept != 0xffffffffu) break;
+    y0 = __shfl_sync(0xffffffffu, y, 31) + 5.0;
   }
   __syncwarp();
   return n;
@@ -585,11 +605,21 @@ static int lateral_launch(const char* who, const float* masks, int n, int H, int
     vpb_set_error("%s: %s, and img_w / img_h arrays (NULL)", who, kNeed);
     return VPB_ERR_ARG;
   }
-  for (int c = 0; c < n; ++c)
+  for (int c = 0; c < n; ++c) {
     if (img_w[c] <= 0 || img_h[c] <= 0) {
       vpb_set_error("%s: %s; camera %d: image size %dx%d is not positive", who, kNeed, c, img_w[c], img_h[c]);
       return VPB_ERR_ARG;
     }
+    if (img_h[c] > vpb::kMaxImgH) {
+      vpb_set_error("%s: camera %d: image height %d is above %d", who, c, img_h[c], vpb::kMaxImgH);
+      return VPB_ERR_ARG;
+    }
+  }
+  // outside [0, 1] the smoothed y-limits leave the mask rows and the generated points have no bound
+  if (!(smoothing >= 0.0f && smoothing <= 1.0f)) {
+    vpb_set_error("%s: smoothing %g is outside [0, 1]", who, static_cast<double>(smoothing));
+    return VPB_ERR_ARG;
+  }
   // lane_tracking.hpp:75-79 (hard-coded in the reference; overridable here)
   static const double kH[9] = {-1.79887412e-01, -6.05811422e-01, 6.02998251e+02,
                                1.85824549e-14,  -1.28170839e+00, 8.63871455e+02,

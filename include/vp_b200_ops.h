@@ -382,7 +382,10 @@ typedef struct {
 /* LaneFilter::reset + LaneTracker defaults */
 int vpb_lateral_init(vpb_lateral_state* state_dev, void* stream);
 /* masks: device float [3][H][W] (ego_left, ego_right, other_lanes; the output of vpb_lane_masks),
- * H <= 128 (>= 41), W <= 256; img_w x img_h = size of the source frame the homography refers to;
+ * H <= 128 (>= 41), W <= 256; img_w x img_h = size of the source frame the homography refers to, img_h <= 4320;
+ * smoothing: LaneFilter's factor, in [0, 1].  Every window point (up to 3072 per line at H = 128) and every point
+ * generated from a fit (one per 5 source rows) is kept, as in the reference; the two limits
+ * bound those buffers.  A state's fits are in mask rows, so one state takes masks of one size;
  * homography: host pointer to 9 doubles (orig -> BEV) or NULL for the reference's matrix
  * (lane_tracking.hpp:75-79); autosteer_steering_rad: the steering value PathFinder takes as its
  * curvature measurement (main.cpp:577). */
@@ -397,14 +400,14 @@ int vpb_lateral_update(const float* masks, int H, int W, int img_w, int img_h, f
  * Camera k's state and record are byte-identical to vpb_lateral_update on the same inputs.  The per-camera
  * parameters travel by value in the launch (no copy), so the call can be captured in a CUDA graph.
  * VPB_ERR_ARG before any device work: n outside 1..VP_MAX_BATCH, H outside 41..128, W outside 2..256, a NULL
- * device pointer, or a non-positive image size. */
+ * device pointer, a non-positive image size, an image height above 4320 or smoothing outside [0, 1]. */
 int vpb_lateral_update_batch(const float* masks, int n, int H, int W, int img_w, int img_h, float smoothing,
                              const double* homographies, const double* steering_rad,
                              vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream);
 /* vpb_lateral_update_batch with one source size per camera: camera k's frame is img_w[k] x img_h[k] (host arrays of
  * n ints), so cameras of different resolutions, or a cropped view next to a full frame, share one launch.  Camera k's
  * state and record are byte-identical to vpb_lateral_update with img_w[k] x img_h[k].  VPB_ERR_ARG before any device
- * work as above, and for NULL img_w / img_h or a non-positive size (the message names the camera).
+ * work as above, and for NULL img_w / img_h, a non-positive size or a height above 4320 (the message names the camera).
  * vpb_lateral_update_batch and vpb_lateral_update are the case of n equal sizes. */
 int vpb_lateral_update_cameras(const float* masks, int n, int H, int W, const int* img_w, const int* img_h,
                                float smoothing, const double* homographies, const double* steering_rad,

@@ -11,14 +11,14 @@ VPB_ERR_ARG = -1
 
 
 def _cameras_call(n=2, sizes=((1920, 1080), (1280, 720)), masks=True, states=True, outs=True, null_w=False,
-                  null_h=False):
+                  null_h=False, smoothing=0.5):
     lib = LT._bind()
     buf = (C.c_double * 64)()
     p = C.addressof(buf)            # never dereferenced: every call below must fail validation first
     ws = (C.c_int * max(len(sizes), 1))(*[s[0] for s in sizes])
     hs = (C.c_int * max(len(sizes), 1))(*[s[1] for s in sizes])
     return lib.vpb_lateral_update_cameras(p if masks else None, n, 80, 160, None if null_w else ws,
-                                          None if null_h else hs, 0.5, None, None, p if states else None,
+                                          None if null_h else hs, smoothing, None, None, p if states else None,
                                           p if outs else None, None)
 
 
@@ -44,6 +44,38 @@ def test_cameras_rejects_a_non_positive_image_size_naming_the_camera(sizes, cam)
 def test_cameras_rejects_null_arrays(kw):
     assert _cameras_call(**kw) == VPB_ERR_ARG
     assert "vpb_lateral_update_cameras: need masks" in L.last_error()
+
+
+@pytest.mark.parametrize("sizes,cam", [
+    (((1920, 1080), (7680, 4321)), 1),
+    (((1920, 4321), (1280, 720)), 0),
+])
+def test_cameras_rejects_an_image_taller_than_4320_naming_the_camera(sizes, cam):
+    assert _cameras_call(sizes=sizes) == VPB_ERR_ARG
+    assert f"vpb_lateral_update_cameras: camera {cam}: image height 4321 is above 4320" in L.last_error()
+
+
+@pytest.mark.parametrize("smoothing", [-0.01, 1.01, float("nan"), float("inf"), float("-inf")])
+def test_every_lateral_call_rejects_smoothing_outside_0_to_1(smoothing):
+    lib = LT._bind()
+    buf = (C.c_double * 64)()
+    p = C.addressof(buf)
+    assert _cameras_call(smoothing=smoothing) == VPB_ERR_ARG
+    assert "vpb_lateral_update_cameras: smoothing" in L.last_error() and "outside [0, 1]" in L.last_error()
+    assert lib.vpb_lateral_update_batch(p, 2, 80, 160, 1920, 1080, smoothing, None, None, p, p, None) == VPB_ERR_ARG
+    assert "vpb_lateral_update_batch: smoothing" in L.last_error()
+    assert lib.vpb_lateral_update(p, 80, 160, 1920, 1080, smoothing, None, 0.0, p, p, None) == VPB_ERR_ARG
+    assert "lateral: smoothing" in L.last_error()
+
+
+def test_single_and_batch_calls_reject_an_image_taller_than_4320():
+    lib = LT._bind()
+    buf = (C.c_double * 64)()
+    p = C.addressof(buf)
+    assert lib.vpb_lateral_update(p, 128, 256, 7680, 4321, 0.5, None, 0.0, p, p, None) == VPB_ERR_ARG
+    assert "lateral: camera 0: image height 4321 is above 4320" in L.last_error()
+    assert lib.vpb_lateral_update_batch(p, 3, 80, 160, 7680, 4800, 1.0, None, None, p, p, None) == VPB_ERR_ARG
+    assert "vpb_lateral_update_batch: camera 0: image height 4800 is above 4320" in L.last_error()
 
 
 def test_batch_call_names_the_camera_of_a_bad_size_and_keeps_its_message():

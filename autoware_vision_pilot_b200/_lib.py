@@ -67,7 +67,10 @@ def frame_descs(descs) -> "C.Array":
     return arr
 
 
-PIX_PACKED, PIX_NV12, PIX_UYVY, PIX_YUYV = 0, 1, 2, 3    # VPB_PIX_*
+PIX_PACKED, PIX_NV12, PIX_UYVY, PIX_YUYV = 0, 1, 2, 3    # VPB_PIX_* (4 is unassigned)
+PIX_BGRA, PIX_RGBA = 5, 6
+PIX_BAYER_RGGB, PIX_BAYER_BGGR, PIX_BAYER_GBRG, PIX_BAYER_GRBG = 7, 8, 9, 10
+BAYER_PATTERNS = {"rggb": PIX_BAYER_RGGB, "bggr": PIX_BAYER_BGGR, "gbrg": PIX_BAYER_GBRG, "grbg": PIX_BAYER_GRBG}
 
 
 class FrameFmt(C.Structure):
@@ -120,33 +123,70 @@ class NV12:
         return FrameFmt(PIX_NV12, y.ctypes.data, self.h, self.w, y.strides[0], uv.ctypes.data, uv.strides[0]), (y, uv)
 
 
-class _Packed422:
+class _Interleaved:
+    """One plane of `channels` bytes per pixel, uint8 [h, w, channels]"""
+
     format = PIX_PACKED
+    channels = 2
 
     def __init__(self, a: np.ndarray):
-        if not isinstance(a, np.ndarray) or a.ndim != 3 or a.shape[2] != 2:
-            raise ValueError(f"{type(self).__name__}: [h, w, 2] expected, got {getattr(a, 'shape', a)}")
+        if not isinstance(a, np.ndarray) or a.ndim != 3 or a.shape[2] != self.channels:
+            raise ValueError(f"{type(self).__name__}: [h, w, {self.channels}] expected, got {getattr(a, 'shape', a)}")
         self.a = a
         self.h, self.w = a.shape[:2]
 
     def desc(self, allow_copy: bool = True):
-        a = _rows(self.a, 2 * self.w, type(self).__name__, allow_copy)
+        a = _rows(self.a, self.channels * self.w, type(self).__name__, allow_copy)
         return FrameFmt(self.format, a.ctypes.data, self.h, self.w, a.strides[0], None, 0), (a,)
 
 
-class UYVY(_Packed422):
+class UYVY(_Interleaved):
     """A host UYVY frame in cv2's layout, uint8 [h, w, 2] (U Y0 V Y1 per pixel pair; ROS "yuv422", GMSL cameras)."""
 
     format = PIX_UYVY
 
 
-class YUYV(_Packed422):
+class YUYV(_Interleaved):
     """A host YUYV frame in cv2's layout, uint8 [h, w, 2] (Y0 U Y1 V per pixel pair; ROS "yuv422_yuy2", UVC cameras)."""
 
     format = PIX_YUYV
 
 
-YUV_TYPES = (NV12, UYVY, YUYV)
+class BGRA(_Interleaved):
+    """A host 4-channel frame, uint8 [h, w, 4] in B, G, R, A order (ROS "bgra8", CARLA, GStreamer "BGRx"); the alpha
+    byte is ignored."""
+
+    format = PIX_BGRA
+    channels = 4
+
+
+class RGBA(_Interleaved):
+    """A host 4-channel frame, uint8 [h, w, 4] in R, G, B, A order (ROS "rgba8"); the alpha byte is ignored."""
+
+    format = PIX_RGBA
+    channels = 4
+
+
+class Bayer:
+    """A host raw Bayer mosaic, uint8 [h, w] (h, w >= 3; padded rows allowed), demosaiced inside the pre-process as
+    cv2.cvtColor(COLOR_Bayer**2RGB) does it.  `pattern` is the ROS encoding's pattern ("rggb" for "bayer_rggb8",
+    "bggr", "gbrg", "grbg"): the colours of the 2x2 block at (0, 0), so a crop starting at an odd row or column names
+    the pattern it starts with."""
+
+    def __init__(self, a: np.ndarray, pattern: str):
+        if pattern not in BAYER_PATTERNS:
+            raise ValueError(f"Bayer: unknown pattern {pattern!r} (one of {sorted(BAYER_PATTERNS)})")
+        if not isinstance(a, np.ndarray) or a.ndim != 2:
+            raise ValueError(f"Bayer: [h, w] expected, got {getattr(a, 'shape', a)}")
+        self.a, self.pattern, self.format = a, pattern, BAYER_PATTERNS[pattern]
+        self.h, self.w = a.shape
+
+    def desc(self, allow_copy: bool = True):
+        a = _rows(self.a, self.w, "Bayer", allow_copy)
+        return FrameFmt(self.format, a.ctypes.data, self.h, self.w, a.strides[0], None, 0), (a,)
+
+
+FRAME_TYPES = (NV12, UYVY, YUYV, BGRA, RGBA, Bayer)    # the camera-native frame objects the engines take
 
 
 def packed_desc(frame: np.ndarray):

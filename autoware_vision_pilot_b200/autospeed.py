@@ -124,13 +124,14 @@ class AutoSpeedEngine:
     def infer_frames(self, frames, fetch_raw: bool = False) -> List[np.ndarray]:
         """`batch` uint8 [h_k, w_k, 3] RGB frames, each of its own size, in one call (each gets its own letterbox)
         -> detections of frame k, in frame k's pixels, at index k.  A frame may also be a camera-native NV12 / UYVY /
-        YUYV object (autoware_vision_pilot_b200._lib), converted to RGB inside the letterbox as cv2.cvtColor would."""
+        YUYV / BGRA / RGBA / Bayer object (autoware_vision_pilot_b200._lib), converted to RGB inside the letterbox as
+        cv2.cvtColor would."""
         frames = list(frames)
         self._check_count(len(frames))
-        if any(isinstance(f, L.YUV_TYPES) for f in frames):
+        if any(isinstance(f, L.FRAME_TYPES) for f in frames):
             arr, keep = (L.FrameFmt * len(frames))(), []
             for k, f in enumerate(frames):
-                d, alive = f.desc() if isinstance(f, L.YUV_TYPES) else L.packed_desc(self._check_frame(f))
+                d, alive = f.desc() if isinstance(f, L.FRAME_TYPES) else L.packed_desc(self._check_frame(f))
                 arr[k] = d
                 keep.append(alive)
             L.check(self._lib.vp_autospeed_infer_frames_fmt(self._h, arr, len(frames), int(fetch_raw)),

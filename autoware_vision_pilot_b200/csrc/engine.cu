@@ -625,7 +625,7 @@ static int check_source_flags(const vp_engine_config& c) {
 int vp_engine::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
   for (int k = 0; k < batch; ++k) {
     if ((cfg.source_outputs & VP_SRC_OVERLAY) && frames[k].format != VPB_PIX_PACKED) {
-      vpb_set_error("%s: frame %d: VP_SRC_OVERLAY blends the packed camera frame; this engine cannot take a YUV frame "
+      vpb_set_error("%s: frame %d: VP_SRC_OVERLAY blends the packed camera frame; this engine cannot take a non-packed frame "
                     "(format %d)", who, k, frames[k].format);
       return VPB_ERR_ARG;
     }

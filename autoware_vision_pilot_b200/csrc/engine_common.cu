@@ -417,13 +417,13 @@ bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int
 
 // The device frames f of geometries g become the runtime's frames, and op 0, the pre-process, gets the algorithmic
 // bytes of the call (SURVEY.md 8d: frame read + 3 x OH x OW 16-bit written, per sample; a frame reads h x w x 3 bytes
-// packed, x 2 in 4:2:2, x 1.5 in NV12).  A failed call leaves no
+// packed, x 2 in 4:2:2, x 1.5 in NV12, x 4 in BGRA / RGBA, x 1 in Bayer).  A failed call leaves no
 // frames, so nothing launches the pre-process on frames its tables were not built for.
 static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeom* g) {
   e->frames = f;
   e->n_frames = n;
   double bytes = 0;
-  static const double kBytesPerPixel[4] = {3.0, 1.5, 2.0, 2.0};
+  static const double kBytesPerPixel[VPB_PIX_BAYER_GRBG + 1] = {3.0, 1.5, 2.0, 2.0, 0.0, 4.0, 4.0, 1.0, 1.0, 1.0, 1.0};
   for (int k = 0; k < n; ++k) bytes += kBytesPerPixel[f[k].format] * g[k].h * g[k].w + 2.0 * 3 * g[k].OH * g[k].OW;
   e->ops[0].bytes = bytes;
   const int rc = e->enqueue(g);

@@ -28,9 +28,15 @@ struct PreGeom {
 // format, a NULL plane, a non-positive or (for the format) odd size, or a stride below the format's minimum.  The
 // messages for packed frames are those vpb_frame has always had.
 int frame_fmt_check(const vpb_frame_fmt& f, const char* who, int k);
-// Bytes of each row of the frame's main plane that belong to the image (3w packed, 2w 4:2:2, w NV12)
+// Bytes of each row of the frame's main plane that belong to the image (3w packed, 2w 4:2:2, 4w BGRA / RGBA, w NV12 and
+// Bayer)
 inline int frame_row_bytes(const vpb_frame_fmt& f) {
-  return f.format == VPB_PIX_PACKED ? 3 * f.w : f.format == VPB_PIX_NV12 ? f.w : 2 * f.w;
+  switch (f.format) {
+    case VPB_PIX_PACKED: return 3 * f.w;
+    case VPB_PIX_UYVY: case VPB_PIX_YUYV: return 2 * f.w;
+    case VPB_PIX_BGRA: case VPB_PIX_RGBA: return 4 * f.w;
+    default: return f.w;
+  }
 }
 inline vpb_frame_fmt packed_frame(const vpb_frame& f) {
   vpb_frame_fmt o{};
@@ -61,7 +67,7 @@ struct PreprocessPlan {
   int configure(const PreGeom* g, int n, int mode);
   // frames[0 .. n-1]: image k reads frames[k] in its format (data, stride, and uv, uv_stride for NV12; its h, w are
   // geom[k]'s); out / out_u8 hold n images back to back (16-bit mode only for n > 1).  A call whose frames are all
-  // packed launches the packed-only kernel instantiations; one YUV frame selects the converting ones.
+  // packed launches the packed-only kernel instantiations; one non-packed frame selects the converting ones.
   int launch(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8,
              cudaStream_t stream) const;
   int update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames, int convention,

@@ -121,22 +121,22 @@ struct PreParams {      // by value (__grid_constant__): under 0.8 KB at kMaxBat
   uint8_t* out_u8;      // optional resized image in tensor channel order, [out_rows][out_pitch][3] per image
   size_t out_img;       // elements between the canvases of out (out_lo); out_u8 images are out_img / out_c * 3 bytes apart
 };
-// The per-image format fields of a call with a YUV frame follow the PreParams block instead of widening PreImg: the
-// packed-only instantiations take PreParams itself, so their parameter layout, and their code, are those of a build
-// without YUV input.  PreParamsYuv stays under 1 KB at kMaxBatch images.
-struct PreYuv {
+// The per-image format fields of a call with a non-packed frame follow the PreParams block instead of widening PreImg:
+// the packed-only instantiations take PreParams itself, so their parameter layout, and their code, are those of a build
+// without camera-native input.  PreParamsCvt stays under 1 KB at kMaxBatch images.
+struct PreCvt {
   const uint8_t* uv;    // NV12: the interleaved U,V plane [h/2][uv_stride]
   int fmt, uv_stride;   // VPB_PIX_*
-  int bgr;              // 1: a YUV image converts to B, G, R (the BGR conventions), 0: to R, G, B
+  int bgr;              // 1: a non-packed image converts to B, G, R (the BGR conventions), 0: to R, G, B
 };
-struct PreParamsYuv : PreParams {
-  PreYuv yuv[kMaxBatch];
+struct PreParamsCvt : PreParams {
+  PreCvt cvt[kMaxBatch];
 };
-template <bool YUV> using PreParamsOf = typename std::conditional<YUV, PreParamsYuv, PreParams>::type;
-static_assert(sizeof(PreParamsYuv) < 1024, "the by-value parameter block of a YUV call stays under 1 KB");
+template <bool CVT> using PreParamsOf = typename std::conditional<CVT, PreParamsCvt, PreParams>::type;
+static_assert(sizeof(PreParamsCvt) < 1024, "the by-value parameter block of a converting call stays under 1 KB");
 
-__device__ __forceinline__ PreYuv yuv_of(const PreParams&, int) { return PreYuv{nullptr, VPB_PIX_PACKED, 0, 0}; }
-__device__ __forceinline__ PreYuv yuv_of(const PreParamsYuv& p, int img) { return p.yuv[img]; }
+__device__ __forceinline__ PreCvt cvt_of(const PreParams&, int) { return PreCvt{nullptr, VPB_PIX_PACKED, 0, 0}; }
+__device__ __forceinline__ PreCvt cvt_of(const PreParamsCvt& p, int img) { return p.cvt[img]; }
 
 // OpenCV's YUV -> RGB of COLOR_YUV2RGB_NV12 / _UYVY / _YUYV (BT.601 limited range, 20-bit fixed point): y' = max(Y -
 // 16, 0) * 1220542 + 2^19, R = (y' + 1673527 v) >> 20, G = (y' - 852492 v - 409993 u) >> 20, B = (y' + 2116026 u) >> 20,
@@ -151,7 +151,7 @@ __device__ __forceinline__ void yuv_px(int Y, int U, int V, int bgr, int (&o)[3]
 }
 
 // Source pixel (x, y) of a YUV image, converted: chroma of the 2x2 block (NV12) or the horizontal pair (UYVY, YUYV)
-__device__ __forceinline__ void yuv_load(const PreImg& im, const PreYuv& yv, int y, int x, int (&o)[3]) {
+__device__ __forceinline__ void yuv_load(const PreImg& im, const PreCvt& yv, int y, int x, int (&o)[3]) {
   const uint8_t* row = im.src + static_cast<size_t>(y) * im.stride;
   if (yv.fmt == VPB_PIX_NV12) {
     const uint8_t* c = yv.uv + static_cast<size_t>(y >> 1) * yv.uv_stride + (x & ~1);
@@ -160,6 +160,52 @@ __device__ __forceinline__ void yuv_load(const PreImg& im, const PreYuv& yv, int
     const uint8_t* m = row + (x & ~1) * 2;        // macropixel: U Y0 V Y1 (UYVY) or Y0 U Y1 V (YUYV)
     if (yv.fmt == VPB_PIX_UYVY) yuv_px(__ldg(m + 1 + ((x & 1) << 1)), __ldg(m), __ldg(m + 2), yv.bgr, o);
     else yuv_px(__ldg(m + ((x & 1) << 1)), __ldg(m + 1), __ldg(m + 3), yv.bgr, o);
+  }
+}
+
+// OpenCV's bilinear demosaic (COLOR_Bayer**2RGB): pixel (x, y) of a Bayer image, with the border rule folded in: x, y
+// are clamped to the interior [1, w-2] x [1, h-2] (OpenCV copies column 1 to 0 and w-2 to w-1, then row 1 to 0 and h-2
+// to h-1), so only the 3x3 neighbourhood of an interior pixel is read, never a byte outside the descriptor.  At an R
+// or B site: G = (4 neighbours + 2) >> 2, the other colour = (4 diagonals + 2) >> 2; at a G site, the colour of its
+// row's R/B neighbours = (left + right + 1) >> 1 and the other = (up + down + 1) >> 1.
+__device__ __forceinline__ void bayer_load(const PreImg& im, const PreCvt& cv, int y, int x, int (&o)[3]) {
+  x = min(max(x, 1), im.w - 2);
+  y = min(max(y, 1), im.h - 2);
+  // red's site in the 2x2 block at (0, 0): RGGB (0, 0), BGGR (1, 1), GBRG (0, 1), GRBG (1, 0)
+  const int rx = cv.fmt == VPB_PIX_BAYER_BGGR || cv.fmt == VPB_PIX_BAYER_GRBG;
+  const int ry = cv.fmt == VPB_PIX_BAYER_BGGR || cv.fmt == VPB_PIX_BAYER_GBRG;
+  const uint8_t* m = im.src + static_cast<size_t>(y) * im.stride + x;
+  const uint8_t* u = m - im.stride;
+  const uint8_t* d = m + im.stride;
+  const int c = __ldg(m), l = __ldg(m - 1), r = __ldg(m + 1), up = __ldg(u), dn = __ldg(d);
+  const int px = (x ^ rx) & 1, py = (y ^ ry) & 1;        // (0, 0): an R site, (1, 1): a B site, else G
+  int R, G, B;
+  if (px == py) {
+    const int diag = (__ldg(u - 1) + __ldg(u + 1) + __ldg(d - 1) + __ldg(d + 1) + 2) >> 2;
+    G = (l + r + up + dn + 2) >> 2;
+    R = px ? diag : c;
+    B = px ? c : diag;
+  } else {
+    const int hz = (l + r + 1) >> 1, vt = (up + dn + 1) >> 1;
+    G = c;
+    R = py ? vt : hz;                                     // py == 0: a G site on a row of R sites
+    B = py ? hz : vt;
+  }
+  o[0] = cv.bgr ? B : R; o[1] = G; o[2] = cv.bgr ? R : B;
+}
+
+// Source pixel (x, y) of a non-packed image as 3 bytes in the convention's order: YUV converted, BGRA / RGBA without
+// alpha, Bayer demosaiced
+__device__ __forceinline__ void cvt_load(const PreImg& im, const PreCvt& cv, int y, int x, int (&o)[3]) {
+  if (cv.fmt >= VPB_PIX_BAYER_RGGB) {
+    bayer_load(im, cv, y, x, o);
+  } else if (cv.fmt >= VPB_PIX_BGRA) {
+    const uint8_t* q = im.src + static_cast<size_t>(y) * im.stride + 4 * x;
+    const bool rev = (cv.fmt == VPB_PIX_BGRA) != (cv.bgr != 0);   // stored order differs from the wanted one
+    const int a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 2);
+    o[0] = rev ? c : a; o[1] = b; o[2] = rev ? a : c;
+  } else {
+    yuv_load(im, cv, y, x, o);
   }
 }
 
@@ -200,11 +246,11 @@ static constexpr int kRowBytes = kTX * 3;     // 96
 // re-staged every input row 1.75x) took 50 us per 1080p frame = 2 % of the HBM roofline.
 // A call may mix geometries: the grid covers the largest output, and a block outside its own image's output returns
 // (as a whole block, before the first barrier).
-// YUV (a call with at least one YUV image): phase 1 of a YUV image stages the CONVERTED bytes, 3 per pixel from offset 0
-// of each patch row (mis = 0), so phases 2 and 3 run unchanged.  The converted patch row is (x_hi - x_lo) * 3 bytes,
-// never wider than the packed one the plan sizes (which adds the misalignment), so the plan needs no change.
-template <class E, int XT, bool YUV>
-__global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __grid_constant__ PreParamsOf<YUV> p,
+// CVT (a call with at least one non-packed image): phase 1 of such an image stages the CONVERTED bytes, 3 per pixel from
+// offset 0 of each patch row (mis = 0), so phases 2 and 3 run unchanged.  The converted patch row is (x_hi - x_lo) * 3
+// bytes, never wider than the packed one the plan sizes (which adds the misalignment), so the plan needs no change.
+template <class E, int XT, bool CVT>
+__global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __grid_constant__ PreParamsOf<CVT> p,
                                                                      int rows_cap, int pitch, int TY) {
   pdl_launch_dependents();
   pdl_wait();
@@ -234,14 +280,14 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __gri
   // ---- phase 1: stage (coalesced aligned words)
   const uintptr_t base = reinterpret_cast<uintptr_t>(im.src) + static_cast<size_t>(x_lo) * 3;
   const int stride = im.stride;
-  const PreYuv yv = yuv_of(p, img);
-  const bool conv = YUV && yv.fmt != VPB_PIX_PACKED;
+  const PreCvt fv = cvt_of(p, img);
+  const bool conv = CVT && fv.fmt != VPB_PIX_PACKED;
   if (conv) {
     for (int r = warp; r < rows; r += kPreThreads / 32) {
       uint8_t* dst = patch + r * pitch;
       for (int x = lane; x < x_hi - x_lo; x += 32) {
         int o[3];
-        yuv_load(im, yv, y_lo + r, x_lo + x, o);
+        cvt_load(im, fv, y_lo + r, x_lo + x, o);
         dst[3 * x] = static_cast<uint8_t>(o[0]); dst[3 * x + 1] = static_cast<uint8_t>(o[1]);
         dst[3 * x + 2] = static_cast<uint8_t>(o[2]);
       }
@@ -334,23 +380,23 @@ __global__ void __launch_bounds__(kPreThreads) preprocess_pil_kernel(const __gri
   }
 }
 
-// OpenCV path (and the no-resize path): one thread per output pixel, gather from global.  YUV: a YUV image's source
-// pixels are loaded through the conversion.
-template <class E, bool YUV>
-__global__ void __launch_bounds__(256) preprocess_direct_kernel(const __grid_constant__ PreParamsOf<YUV> p) {
+// OpenCV path (and the no-resize path): one thread per output pixel, gather from global.  CVT: a non-packed image's
+// source pixels are loaded through the conversion.
+template <class E, bool CVT>
+__global__ void __launch_bounds__(256) preprocess_direct_kernel(const __grid_constant__ PreParamsOf<CVT> p) {
   pdl_launch_dependents();
   pdl_wait();
   const int ox = blockIdx.x * blockDim.x + threadIdx.x;
   const int oy = blockIdx.y, img = blockIdx.z;
   const PreImg im = p.im[img];                                      // this image's fields, loaded once
   if (ox >= im.OW || oy >= im.OH) return;
-  const PreYuv yv = yuv_of(p, img);
-  const bool conv = YUV && yv.fmt != VPB_PIX_PACKED;
+  const PreCvt fv = cvt_of(p, img);
+  const bool conv = CVT && fv.fmt != VPB_PIX_PACKED;
   const uint8_t* src = im.src;
   int u[3];
   if (p.mode == VPB_RESIZE_NONE) {
     if (conv) {
-      yuv_load(im, yv, oy, ox, u);
+      cvt_load(im, fv, oy, ox, u);
     } else {
       const uint8_t* s = src + static_cast<size_t>(oy) * im.stride + ox * 3;
       u[0] = s[0]; u[1] = s[1]; u[2] = s[2];
@@ -362,8 +408,8 @@ __global__ void __launch_bounds__(256) preprocess_direct_kernel(const __grid_con
     const int b0 = im.yk[2 * oy], b1 = im.yk[2 * oy + 1];
     if (conv) {
       int q00[3], q01[3], q10[3], q11[3];
-      yuv_load(im, yv, sy, sx, q00); yuv_load(im, yv, sy, sx1, q01);
-      yuv_load(im, yv, sy1, sx, q10); yuv_load(im, yv, sy1, sx1, q11);
+      cvt_load(im, fv, sy, sx, q00); cvt_load(im, fv, sy, sx1, q01);
+      cvt_load(im, fv, sy1, sx, q10); cvt_load(im, fv, sy1, sx1, q11);
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
         const int h0 = q00[c] * a0 + q01[c] * a1;
@@ -511,18 +557,18 @@ PreprocessPlan::~PreprocessPlan() {
   if (d_tables) cudaFree(d_tables);
 }
 
-// The parameter block of a call (base PreParams + the per-image format fields); returns whether any image is YUV.
+// The parameter block of a call (base PreParams + the per-image format fields); returns whether any image is not packed.
 static int fill_params(const PreprocessPlan& pl, const vpb_frame_fmt* frames, int convention, void* out, uint8_t* out_u8,
-                       PreParamsYuv& p, bool& yuv) {
+                       PreParamsCvt& p, bool& cvt) {
   if (pl.n < 1 || (pl.n > 1 && pl.out_lo)) {
     vpb_set_error("preprocess: batch %d (1..%d, 16-bit output only)", pl.n, kMaxBatch);
     return VPB_ERR_ARG;
   }
   p.out_lo = pl.out_lo;
   p.out_pitch = pl.out_pitch; p.out_c = pl.out_c;
-  // a YUV image converts to the channel order the convention takes as input
+  // a non-packed image converts to the channel order the convention takes as input
   const int bgr = (convention == VPB_CONV_BGR_NOSWAP || convention == VPB_CONV_BGR_SWAP) ? 1 : 0;
-  yuv = false;
+  cvt = false;
   for (int i = 0; i < kMaxBatch; ++i) {
     const int k = i < pl.n ? i : 0;
     PreImg& im = p.im[i];
@@ -532,11 +578,11 @@ static int fill_params(const PreprocessPlan& pl, const vpb_frame_fmt* frames, in
     im.h = g.h; im.w = g.w; im.OH = g.OH; im.OW = g.OW; im.out_x0 = g.x0; im.out_y0 = g.y0;
     im.xb = pl.d_tables + t.xb; im.xk = pl.d_tables + t.xk; im.xks = t.xks;
     im.yb = pl.d_tables + t.yb; im.yk = pl.d_tables + t.yk; im.yks = t.yks;
-    PreYuv& y = p.yuv[i];
+    PreCvt& y = p.cvt[i];
     y.fmt = frames[k].format; y.bgr = bgr;
     y.uv = y.fmt == VPB_PIX_NV12 ? frames[k].uv : nullptr;
     y.uv_stride = y.fmt == VPB_PIX_NV12 ? frames[k].uv_stride : 0;
-    yuv |= y.fmt != VPB_PIX_PACKED;
+    cvt |= y.fmt != VPB_PIX_PACKED;
   }
   p.mode = pl.mode;
   p.out_img = static_cast<size_t>(pl.out_rows) * p.out_pitch * pl.out_c;   // whole canvases
@@ -553,39 +599,39 @@ static int fill_params(const PreprocessPlan& pl, const vpb_frame_fmt* frames, in
   return VPB_OK;
 }
 
-// The kernel of a resize mode, element type, tap capacity and input kind (YUV: the call has a YUV image): the PIL
+// The kernel of a resize mode, element type, tap capacity and input kind (CVT: the call has a non-packed image): the PIL
 // kernel (params, rows_cap, pitch, TY) for the PIL modes, else the direct kernel (params); the other member is NULL.
-template <bool YUV>
+template <bool CVT>
 struct PreKernel {
-  void (*pil)(PreParamsOf<YUV>, int, int, int);
-  void (*direct)(PreParamsOf<YUV>);
+  void (*pil)(PreParamsOf<CVT>, int, int, int);
+  void (*direct)(PreParamsOf<CVT>);
   const void* func() const { return pil ? reinterpret_cast<const void*>(pil) : reinterpret_cast<const void*>(direct); }
 };
-template <bool YUV>
-static PreKernel<YUV> pre_kernel(int mode, int dtype, int xt) {
+template <bool CVT>
+static PreKernel<CVT> pre_kernel(int mode, int dtype, int xt) {
   return dispatch_dtype(dtype, [&](auto tag) {
     using E = decltype(tag);
-    if (!is_pil(mode)) return PreKernel<YUV>{nullptr, preprocess_direct_kernel<E, YUV>};
-    return PreKernel<YUV>{xt == 16 ? preprocess_pil_kernel<E, 16, YUV> : preprocess_pil_kernel<E, 32, YUV>, nullptr};
+    if (!is_pil(mode)) return PreKernel<CVT>{nullptr, preprocess_direct_kernel<E, CVT>};
+    return PreKernel<CVT>{xt == 16 ? preprocess_pil_kernel<E, 16, CVT> : preprocess_pil_kernel<E, 32, CVT>, nullptr};
   });
 }
-static const void* pre_func(int mode, int dtype, int xt, bool yuv) {
-  return yuv ? pre_kernel<true>(mode, dtype, xt).func() : pre_kernel<false>(mode, dtype, xt).func();
+static const void* pre_func(int mode, int dtype, int xt, bool cvt) {
+  return cvt ? pre_kernel<true>(mode, dtype, xt).func() : pre_kernel<false>(mode, dtype, xt).func();
 }
 
 // Re-point the captured pre-process node at other source frames (same geometries and formats): lets the frame graph be
 // replayed on any device buffers without re-capturing.  The node's kernel takes PreParams (packed-only call) or the
-// whole PreParamsYuv; PreParams is its first sub-object, so one pointer serves both.
+// whole PreParamsCvt; PreParams is its first sub-object, so one pointer serves both.
 int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames,
                                       int convention, int dtype, void* out, uint8_t* out_u8) const {
-  PreParamsYuv p;
-  bool yuv = false;
-  const int rc = fill_params(*this, frames, convention, out, out_u8, p, yuv);
+  PreParamsCvt p;
+  bool cvt = false;
+  const int rc = fill_params(*this, frames, convention, out, out_u8, p, cvt);
   if (rc) return rc;
   int rc_ = rows_cap, pitch_ = pitch, ty_ = TY;
   void* args[4] = {static_cast<PreParams*>(&p), &rc_, &pitch_, &ty_};
   cudaKernelNodeParams kp{};
-  kp.func = const_cast<void*>(pre_func(mode, dtype, xt, yuv));
+  kp.func = const_cast<void*>(pre_func(mode, dtype, xt, cvt));
   kp.kernelParams = args;
   kp.extra = nullptr;
   if (is_pil(mode)) {
@@ -601,9 +647,9 @@ int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node
   return VPB_OK;
 }
 
-template <bool YUV>
-static int launch_pre(const PreprocessPlan& pl, const PreParamsYuv& p, int dtype, cudaStream_t stream) {
-  const PreKernel<YUV> k = pre_kernel<YUV>(pl.mode, dtype, pl.xt);
+template <bool CVT>
+static int launch_pre(const PreprocessPlan& pl, const PreParamsCvt& p, int dtype, cudaStream_t stream) {
+  const PreKernel<CVT> k = pre_kernel<CVT>(pl.mode, dtype, pl.xt);
   if (k.pil) {
     dim3 grid((pl.OWmax + kTX - 1) / kTX, (pl.OHmax + pl.TY - 1) / pl.TY, pl.n);
     {
@@ -630,19 +676,21 @@ static int launch_pre(const PreprocessPlan& pl, const PreParamsYuv& p, int dtype
 
 int PreprocessPlan::launch(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8,
                            cudaStream_t stream) const {
-  PreParamsYuv p;
-  bool yuv = false;
-  const int rc = fill_params(*this, frames, convention, out, out_u8, p, yuv);
+  PreParamsCvt p;
+  bool cvt = false;
+  const int rc = fill_params(*this, frames, convention, out, out_u8, p, cvt);
   if (rc) return rc;
-  return yuv ? launch_pre<true>(*this, p, dtype, stream) : launch_pre<false>(*this, p, dtype, stream);
+  return cvt ? launch_pre<true>(*this, p, dtype, stream) : launch_pre<false>(*this, p, dtype, stream);
 }
 
 int frame_fmt_check(const vpb_frame_fmt& f, const char* who, int k) {
-  if (f.format < VPB_PIX_PACKED || f.format > VPB_PIX_YUYV) {
-    vpb_set_error("%s: frame %d: unknown format %d (VPB_PIX_PACKED, _NV12, _UYVY or _YUYV)", who, k, f.format);
+  if (f.format < VPB_PIX_PACKED || f.format > VPB_PIX_BAYER_GRBG || f.format == 4) {
+    vpb_set_error("%s: frame %d: unknown format %d (VPB_PIX_PACKED, _NV12, _UYVY, _YUYV, _BGRA, _RGBA or _BAYER_*)", who,
+                  k, f.format);
     return VPB_ERR_ARG;
   }
-  static const char* kName[4] = {"packed", "NV12", "UYVY", "YUYV"};
+  static const char* kName[11] = {"packed", "NV12", "UYVY", "YUYV", nullptr, "BGRA", "RGBA",
+                                  "Bayer RGGB", "Bayer BGGR", "Bayer GBRG", "Bayer GRBG"};
   if (f.format == VPB_PIX_PACKED) {             // the messages of vpb_frame
     if (!f.data) { vpb_set_error("%s: frame %d is NULL", who, k); return VPB_ERR_ARG; }
     if (f.h <= 0 || f.w <= 0 || f.stride < 3 * f.w) {
@@ -654,6 +702,20 @@ int frame_fmt_check(const vpb_frame_fmt& f, const char* who, int k) {
   }
   const char* nm = kName[f.format];
   if (!f.data) { vpb_set_error("%s: frame %d is NULL (%s data)", who, k, nm); return VPB_ERR_ARG; }
+  if (f.format >= VPB_PIX_BGRA) {               // 4-channel and Bayer: one plane of 4 or 1 bytes per pixel
+    const bool bayer = f.format >= VPB_PIX_BAYER_RGGB;
+    const int min_hw = bayer ? 3 : 1;             // the demosaic needs an interior pixel (cv::cvtColor gives zeros)
+    if (f.h < min_hw || f.w < min_hw) {
+      vpb_set_error("%s: frame %d: bad %s size h %d, w %d (need h, w >= %d)", who, k, nm, f.h, f.w, min_hw);
+      return VPB_ERR_ARG;
+    }
+    const int min_stride = bayer ? f.w : 4 * f.w;
+    if (f.stride < min_stride) {
+      vpb_set_error("%s: frame %d: %s stride %d < %d (%s)", who, k, nm, f.stride, min_stride, bayer ? "w" : "4*w");
+      return VPB_ERR_ARG;
+    }
+    return VPB_OK;
+  }
   if (f.format == VPB_PIX_NV12 && !f.uv) { vpb_set_error("%s: frame %d: NV12 uv plane is NULL", who, k); return VPB_ERR_ARG; }
   if (f.h <= 0 || f.w <= 0 || (f.w & 1) || (f.format == VPB_PIX_NV12 && (f.h & 1))) {
     vpb_set_error("%s: frame %d: bad %s size h %d, w %d (need h, w > 0, w even%s)", who, k, nm, f.h, f.w,

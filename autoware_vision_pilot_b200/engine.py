@@ -229,24 +229,25 @@ class Engine:
         return L.frame_descs([(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames])
 
     def _fmt_descs(self, frames, allow_copy: bool):
-        """`batch` frames, packed arrays and NV12 / UYVY / YUYV objects mixed, as a vpb_frame_fmt array (and the arrays
+        """`batch` frames, packed arrays and camera-native frame objects mixed, as a vpb_frame_fmt array (and the arrays
         it points into, to keep alive for the call)"""
         frames = list(frames)
         if len(frames) != self.batch:
             raise ValueError(f"{len(frames)} frame(s) for an engine of batch {self.batch}")
         arr, keep = (L.FrameFmt * len(frames))(), []
         for k, f in enumerate(frames):
-            d, alive = f.desc(allow_copy) if isinstance(f, L.YUV_TYPES) else L.packed_desc(self._check_frame(f, allow_copy))
+            d, alive = f.desc(allow_copy) if isinstance(f, L.FRAME_TYPES) else L.packed_desc(self._check_frame(f, allow_copy))
             arr[k] = d
             keep.append(alive)
         return arr, keep
 
     def infer_frames(self, frames) -> None:
         """`batch` host frames, each of its own size (a mixed camera rig), in one call; outputs of frame k are sample k.
-        A frame is a uint8 [h_k, w_k, 3] array in the convention's channel order, or a camera-native NV12 / UYVY / YUYV
-        object (autoware_vision_pilot_b200._lib), converted inside the pre-process exactly as cv2.cvtColor would."""
+        A frame is a uint8 [h_k, w_k, 3] array in the convention's channel order, or a camera-native NV12 / UYVY / YUYV /
+        BGRA / RGBA / Bayer object (autoware_vision_pilot_b200._lib), converted inside the pre-process exactly as
+        cv2.cvtColor would."""
         frames = list(frames)
-        if not any(isinstance(f, L.YUV_TYPES) for f in frames):
+        if not any(isinstance(f, L.FRAME_TYPES) for f in frames):
             frames = self._check_frames(frames, allow_copy=True)
             L.check(self._lib.vp_engine_infer_frames(self._h, self._descs(frames), len(frames)), "vp_engine_infer_frames")
             return
@@ -256,7 +257,7 @@ class Engine:
     def submit_frames(self, frames) -> None:
         """Asynchronous infer_frames() (pinned frames: pinned_frames(shapes)); sync() completes it."""
         frames = list(frames)
-        if not any(isinstance(f, L.YUV_TYPES) for f in frames):
+        if not any(isinstance(f, L.FRAME_TYPES) for f in frames):
             frames = self._check_frames(frames, allow_copy=False)
             L.check(self._lib.vp_engine_submit_frames(self._h, self._descs(frames), len(frames)), "vp_engine_submit_frames")
             return
@@ -299,14 +300,18 @@ class Engine:
     def pinned_frames(self, shapes: Sequence[Sequence]) -> List:
         """Views into one engine-owned pinned host buffer, one per entry of shapes (submit_frames(views)): (h, w) or
         (h, w, "packed") gives a [h, w, 3] array, (h, w, "nv12") an NV12 object (y [h, w], uv [h/2, w]), (h, w, "uyvy")
-        / (h, w, "yuyv") a UYVY / YUYV object ([h, w, 2]).  Fill the arrays in place."""
-        kinds = {"packed": 3, "nv12": 1.5, "uyvy": 2, "yuyv": 2}
+        / (h, w, "yuyv") a UYVY / YUYV object ([h, w, 2]), (h, w, "bgra8") / (h, w, "rgba8") a BGRA / RGBA object
+        ([h, w, 4]) and (h, w, "bayer_rggb8") (or bggr, gbrg, grbg: the ROS encodings) a Bayer object ([h, w]).  Fill
+        the arrays in place."""
+        kinds = {"packed": 3, "nv12": 1.5, "uyvy": 2, "yuyv": 2, "bgra8": 4, "rgba8": 4}
+        kinds.update({f"bayer_{p}8": 1 for p in L.BAYER_PATTERNS})
         spec = []
         for s in shapes:
             h, w, kind = int(s[0]), int(s[1]), (s[2] if len(s) > 2 else "packed")
             if kind not in kinds:
                 raise ValueError(f"unknown frame format {kind!r} (one of {sorted(kinds)})")
-            if h <= 0 or w <= 0 or (kind != "packed" and (w % 2 or (kind == "nv12" and h % 2))):
+            if h <= 0 or w <= 0 or (kind in ("nv12", "uyvy", "yuyv") and (w % 2 or (kind == "nv12" and h % 2))) or \
+                    (kind.startswith("bayer") and min(h, w) < 3):
                 raise ValueError(f"bad {kind} frame shape {h}x{w}")
             spec.append((h, w, kind, int(h * w * kinds[kind])))
         total = max(sum(n for *_, n in spec), 1)
@@ -321,8 +326,12 @@ class Engine:
                 views.append(v.reshape(h, w, 3))
             elif kind == "nv12":
                 views.append(L.NV12(v[:h * w].reshape(h, w), v[h * w:].reshape(h // 2, w)))
-            else:
+            elif kind in ("uyvy", "yuyv"):
                 views.append((L.UYVY if kind == "uyvy" else L.YUYV)(v.reshape(h, w, 2)))
+            elif kind in ("bgra8", "rgba8"):
+                views.append((L.BGRA if kind == "bgra8" else L.RGBA)(v.reshape(h, w, 4)))
+            else:
+                views.append(L.Bayer(v.reshape(h, w), kind[6:10]))
             off += n
         return views
 

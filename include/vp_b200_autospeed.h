@@ -61,10 +61,11 @@ int vp_autospeed_infer_device_batch(vp_autospeed* e, const uint8_t* const* frame
  * stride < 3*w, a letterbox filter of more than 32 taps).  The *_batch calls are the case of n equal descriptors. */
 int vp_autospeed_infer_frames(vp_autospeed* e, const vpb_frame* frames_host_rgb, int n, int fetch_raw);
 int vp_autospeed_infer_device_frames(vp_autospeed* e, const vpb_frame* frames_dev_rgb, int n);
-/* The two *_frames calls on camera-native frames (vpb_frame_fmt, vp_b200_ops.h: packed RGB, NV12, UYVY or YUYV, mixed
- * in one call).  They replace the caller's cv::cvtColor(frame, COLOR_YUV2RGB_*) before the call: the letterbox
- * converts each YUV pixel as it reads it, and the raw tensor, candidates and detections are byte-equal to the packed
- * call on the converted frame.  Checks as for the *_frames calls plus those of vpb_preprocess_fmt. */
+/* The two *_frames calls on camera-native frames (vpb_frame_fmt, vp_b200_ops.h: packed RGB, NV12, UYVY, YUYV, BGRA,
+ * RGBA or a raw Bayer mosaic, mixed in one call).  They replace the caller's cv::cvtColor(frame, COLOR_YUV2RGB_* /
+ * COLOR_BGRA2RGB / COLOR_Bayer**2RGB) before the call: the letterbox converts each pixel as it reads it, and the raw
+ * tensor, candidates and detections are byte-equal to the packed call on the converted frame.  Checks as for the
+ * *_frames calls plus those of vpb_preprocess_fmt. */
 int vp_autospeed_infer_frames_fmt(vp_autospeed* e, const vpb_frame_fmt* frames_host, int n, int fetch_raw);
 int vp_autospeed_infer_device_frames_fmt(vp_autospeed* e, const vpb_frame_fmt* frames_dev, int n);
 /* Drain the stream; fetch: 0 nothing, 1 detections, 2 detections + raw tensor to the host buffers (all samples). */

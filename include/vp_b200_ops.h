@@ -56,13 +56,27 @@ typedef struct { const uint8_t* data; int h, w, stride; } vpb_frame;
  *   UYVY  data [h][stride], each pair of pixels U Y0 V Y1 (GMSL cameras, ROS "yuv422"); w even
  *   YUYV  data [h][stride], each pair of pixels Y0 U Y1 V (UVC cameras, ROS "yuv422_yuy2"); w even
  * A crop of a YUV frame must start on an even row and column: the descriptor has no way to state another chroma
- * phase, and it is not detected. */
+ * phase, and it is not detected.
+ *   BGRA, RGBA  data [h][stride], 4 bytes per pixel (CARLA, GStreamer "BGRx"; ROS "bgra8", "rgba8"); alpha is dropped
+ *         as COLOR_{BGRA,RGBA}2{RGB,BGR} drops it
+ *   BAYER_RGGB / _BGGR / _GBRG / _GRBG  data [h][stride], one byte per pixel of a colour filter mosaic (ROS
+ *         "bayer_rggb8", ...); the name gives the colours of the 2x2 block at the descriptor's (0, 0), so a crop at an
+ *         odd row or column names the pattern it starts with.  Demosaiced bilinearly as cv::cvtColor does it (ROS
+ *         rggb = COLOR_BayerBG2RGB, bggr = BayerRG, gbrg = BayerGR, grbg = BayerGB): at an R or B site
+ *         G = (4 neighbours + 2) >> 2 and the other colour = (4 diagonals + 2) >> 2, at a G site each other colour is
+ *         the rounded mean of its two neighbours; the border pixels repeat the nearest interior pixel (clamp x to
+ *         [1, w-2], y to [1, h-2]), reading only the crop itself.  h, w >= 3 (cv::cvtColor returns zeros below).
+ * Value 4 is unassigned: it was rejected as an unknown format before the 4-channel and Bayer layouts existed, and it
+ * still is (the new values start at 5). */
 enum { VPB_PIX_PACKED = 0, /* a vpb_frame: 3 interleaved channels, RGB or BGR as the convention says */
-       VPB_PIX_NV12 = 1, VPB_PIX_UYVY = 2, VPB_PIX_YUYV = 3 };
+       VPB_PIX_NV12 = 1, VPB_PIX_UYVY = 2, VPB_PIX_YUYV = 3,
+       VPB_PIX_BGRA = 5, VPB_PIX_RGBA = 6,
+       VPB_PIX_BAYER_RGGB = 7, VPB_PIX_BAYER_BGGR = 8, VPB_PIX_BAYER_GBRG = 9, VPB_PIX_BAYER_GRBG = 10 };
 typedef struct {
   int format;                 /* VPB_PIX_* */
-  const uint8_t* data;        /* PACKED / UYVY / YUYV: the frame; NV12: the Y plane [h][stride] */
-  int h, w, stride;           /* bytes per row of data: >= 3w (PACKED), >= 2w (UYVY, YUYV), >= w (NV12) */
+  const uint8_t* data;        /* PACKED / UYVY / YUYV / BGRA / RGBA / BAYER_*: the frame; NV12: the Y plane [h][stride] */
+  int h, w, stride;           /* bytes per row of data: >= 3w (PACKED), >= 2w (UYVY, YUYV), >= 4w (BGRA, RGBA),
+                                 >= w (NV12, BAYER_*) */
   const uint8_t* uv;          /* NV12: the interleaved U,V plane [h/2][uv_stride]; ignored otherwise */
   int uv_stride;              /* NV12: >= w */
 } vpb_frame_fmt;
@@ -203,10 +217,11 @@ enum { VPB_CONV_RGB = 0, VPB_CONV_BGR_NOSWAP = 1, VPB_CONV_BGR_SWAP = 2,
 int vpb_preprocess(const uint8_t* src_dev, int h, int w, int stride, int resize_mode, int convention,
                    int dtype, void* out_dev, uint8_t* out_u8_dev, void* stream);
 /* vpb_preprocess of one frame in any VPB_PIX_* layout (device pointers in *frame_dev, the descriptor itself on the
- * host).  A YUV frame converts to RGB for VPB_CONV_RGB / _RGB_UNIT and to BGR for VPB_CONV_BGR_NOSWAP / _SWAP, so the
- * result equals vpb_preprocess on cv::cvtColor(frame, COLOR_YUV2{RGB,BGR}_*).  VPB_ERR_ARG before any device work,
- * the message naming the call and frame 0, for an unknown format or convention, NULL data (or NULL uv for NV12), odd w
- * (odd h for NV12), a stride below the format's minimum, uv_stride < w (NV12), a frame other than 640x320 under
+ * host).  A non-packed frame converts to RGB for VPB_CONV_RGB / _RGB_UNIT and to BGR for VPB_CONV_BGR_NOSWAP / _SWAP,
+ * so the result equals vpb_preprocess on cv::cvtColor(frame, COLOR_{YUV,BGRA,RGBA,Bayer**}2{RGB,BGR}*).  VPB_ERR_ARG
+ * before any device work, the message naming the call and frame 0, for an unknown format or convention, NULL data (or
+ * NULL uv for NV12), odd w (odd h for NV12), h or w below 3 (Bayer), a stride below the format's minimum,
+ * uv_stride < w (NV12), a frame other than 640x320 under
  * VPB_RESIZE_NONE, or a Pillow filter of more than 32 taps. */
 int vpb_preprocess_fmt(const vpb_frame_fmt* frame_dev, int resize_mode, int convention, int dtype, void* out_dev,
                        uint8_t* out_u8_dev, void* stream);

@@ -189,6 +189,45 @@ class Bayer:
 FRAME_TYPES = (NV12, UYVY, YUYV, BGRA, RGBA, Bayer)    # the camera-native frame objects the engines take
 
 
+class Rectify:
+    """Lens rectification maps on one GPU (vpb_rectify_create): map1 int16 [h, w, 2] and map2 uint16 [h, w], the
+    fixed-point pair cv2.initUndistortRectifyMap(K, D, R, P, size, cv2.CV_16SC2) (or cv2.fisheye's) returns, for frames
+    of src_size = (src_h, src_w).  Float maps convert with cv2.convertMaps(mx, my, cv2.CV_16SC2).  Set on an engine
+    sample (Engine.set_rectify, AutoSpeedEngine.set_rectify), every call remaps that sample's frame as
+    cv2.remap(frame, map1, map2, cv2.INTER_LINEAR) does before the pre-process; the outputs are then those of the
+    rectified frame, of size (h, w): pass that size to the lateral post-process as its image size."""
+
+    def __init__(self, map1: np.ndarray, map2: np.ndarray, src_size, gpu_id: int = 0):
+        map1 = np.ascontiguousarray(map1)
+        map2 = np.ascontiguousarray(map2)
+        if map1.dtype != np.int16 or map1.ndim != 3 or map1.shape[2] != 2:
+            raise ValueError(f"Rectify: map1 must be int16 [h, w, 2], got {map1.dtype} {map1.shape}")
+        if map2.dtype != np.uint16 or map2.shape != map1.shape[:2]:
+            raise ValueError(f"Rectify: map2 must be uint16 {map1.shape[:2]}, got {map2.dtype} {map2.shape}")
+        lib_ = lib()
+        lib_.vpb_rectify_create.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                            C.POINTER(C.c_void_p)]
+        lib_.vpb_rectify_destroy.argtypes = [C.c_void_p]
+        lib_.vpb_rectify_destroy.restype = None
+        self._lib, self._h = lib_, C.c_void_p()
+        self.h, self.w = map1.shape[:2]
+        self.src_h, self.src_w = (int(v) for v in src_size)
+        self.gpu_id = gpu_id
+        check(lib_.vpb_rectify_create(map1.ctypes.data, map2.ctypes.data, self.h, self.w, self.src_h, self.src_w,
+                                      gpu_id, C.byref(self._h)), "vpb_rectify_create")
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self._lib.vpb_rectify_destroy(self._h)
+            self._h = C.c_void_p()
+
+    __del__ = close
+
+    @property
+    def handle(self) -> C.c_void_p:
+        return self._h
+
+
 def packed_desc(frame: np.ndarray):
     """A uint8 [h, w, 3] array with unit pixel strides as a VPB_PIX_PACKED FrameFmt"""
     h, w, _ = frame.shape

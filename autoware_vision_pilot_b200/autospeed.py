@@ -31,6 +31,7 @@ def _bind():
     lib.vp_autospeed_infer_device_frames.argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int]
     lib.vp_autospeed_infer_frames_fmt.argtypes = [C.c_void_p, C.POINTER(L.FrameFmt), C.c_int, C.c_int]
     lib.vp_autospeed_infer_device_frames_fmt.argtypes = [C.c_void_p, C.POINTER(L.FrameFmt), C.c_int]
+    lib.vp_autospeed_set_rectify.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     lib.vp_autospeed_sync.argtypes = [C.c_void_p, C.c_int]
     lib.vp_autospeed_detections.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.vp_autospeed_raw.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
@@ -58,6 +59,7 @@ class AutoSpeedEngine:
                                                     L.VPB_BF16 if dtype == "bf16" else L.VPB_F16, stream, batch,
                                                     C.byref(self._h)), "vp_autospeed_create_batch")
         self.batch = batch
+        self._rectify = {}
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -68,6 +70,14 @@ class AutoSpeedEngine:
 
     def set_thresholds(self, conf: float = 0.6, iou: float = 0.45) -> None:
         L.check(self._lib.vp_autospeed_set_thresholds(self._h, conf, iou), "vp_autospeed_set_thresholds")
+
+    def set_rectify(self, sample: int, r: Optional[L.Rectify]) -> None:
+        """Remap sample `sample`'s frame through the maps of r (an _lib.Rectify) before the letterbox in every later
+        call, or stop doing so (r None); detections are then in the rectified frame's pixels.  The engine keeps r alive
+        while it is set."""
+        L.check(self._lib.vp_autospeed_set_rectify(self._h, sample, r.handle if r is not None else None),
+                "vp_autospeed_set_rectify")
+        self._rectify[sample] = r
 
     @staticmethod
     def _check_frame(frame: np.ndarray) -> np.ndarray:

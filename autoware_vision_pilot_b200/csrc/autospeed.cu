@@ -965,6 +965,12 @@ extern "C" int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float io
   return VPB_OK;
 }
 
+extern "C" int vp_autospeed_set_rectify(vp_autospeed* e, int sample, const vpb_rectify* r) {
+  if (!e) { vpb_set_error("vp_autospeed_set_rectify: NULL engine"); return VPB_ERR_ARG; }
+  DeviceGuard guard(e->gpu_id);
+  return e->set_rectify(sample, r, "vp_autospeed_set_rectify");
+}
+
 extern "C" int vp_autospeed_infer(vp_autospeed* e, const uint8_t* frame_host, int h, int w, int stride, int fetch_raw) {
   return as_infer_host_batch(e, &frame_host, 1, h, w, stride, fetch_raw, "vp_autospeed_infer");
 }

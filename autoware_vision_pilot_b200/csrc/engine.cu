@@ -621,7 +621,8 @@ static int check_source_flags(const vp_engine_config& c) {
 
 // Every frame resizes to the 640 x 320 network input: VPB_ERR_ARG (naming `who` and the frame) if one cannot in the
 // engine's resize mode, or if the engine makes overlays and the frame is not packed (the overlay blends the camera
-// frame's pixels as vpb_src_job reads them).  Host-only: callers run it before any device work.
+// frame's pixels as vpb_src_job reads them; a rectified sample's frame here is the packed rectified frame).  Host-only:
+// callers run it before any device work.
 int vp_engine::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
   for (int k = 0; k < batch; ++k) {
     if ((cfg.source_outputs & VP_SRC_OVERLAY) && frames[k].format != VPB_PIX_PACKED) {
@@ -809,6 +810,12 @@ extern "C" int vp_engine_submit_frames_fmt(vp_engine* e, const vpb_frame_fmt* fr
 
 extern "C" int vp_engine_infer_device_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_dev, int n) {
   return call_device(e, frames_dev, n, "vp_engine_infer_device_frames_fmt");
+}
+
+extern "C" int vp_engine_set_rectify(vp_engine* e, int sample, const vpb_rectify* r) {
+  if (!e) { vpb_set_error("vp_engine_set_rectify: NULL engine"); return VPB_ERR_ARG; }
+  DeviceGuard guard(e->gpu_id);
+  return e->set_rectify(sample, r, "vp_engine_set_rectify");
 }
 
 extern "C" int vp_engine_fetch_raw(vp_engine* e, int idx) {

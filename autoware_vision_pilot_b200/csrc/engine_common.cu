@@ -115,12 +115,16 @@ int FrameGraph::run(EngineRuntime& e) {
   bool same_geom = exec && n == e.n_frames, same_src = n == e.n_frames;
   for (int k = 0; k < e.n_frames && same_geom; ++k) same_geom = same_geometry(frames[k], e.frames[k]);
   for (int k = 0; k < e.n_frames && same_src; ++k) same_src = frames[k].data == e.frames[k].data && frames[k].uv == e.frames[k].uv;
+  for (int k = 0; k < e.n_frames && same_src; ++k)
+    same_src = rect[k] == e.rect[k] && (!rect[k] || (same_geometry(in_frames[k], e.in_frames[k]) &&
+                                                     in_frames[k].data == e.in_frames[k].data &&
+                                                     in_frames[k].uv == e.in_frames[k].uv));
   if (same_geom && !same_src) {
     for (const auto& [i, node] : nodes) {
       const int rc = e.ops[i].repoint(exec, node);
       if (rc) return rc;
     }
-    frames = e.frames;
+    frames = e.frames; in_frames = e.in_frames; rect = e.rect;
     same_src = true;
   }
   if (!same_geom || !same_src) {
@@ -142,7 +146,7 @@ int FrameGraph::run(EngineRuntime& e) {
     if (graph) cudaGraphDestroy(graph);
     graph = g;
     if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    frames = e.frames; n = e.n_frames;
+    frames = e.frames; in_frames = e.in_frames; rect = e.rect; n = e.n_frames;
   }
   VPB_CUDA_OK(cudaGraphLaunch(exec, st));
   return VPB_OK;
@@ -261,12 +265,56 @@ void EngineRuntime::add_op(const std::string& name, const char* kname, std::func
 
 void EngineRuntime::add_preprocess(int convention, void* out, uint8_t* out_u8) {
   cur_lane = 0;
+  rect_bgr = (convention == VPB_CONV_BGR_NOSWAP || convention == VPB_CONV_BGR_SWAP) ? 1 : 0;
   add_op("preprocess", "preprocess", [this, convention, out, out_u8](cudaStream_t st) {
     return pre.launch(frames.data(), convention, dtype, out, out_u8, st);
   });
   ops.back().repoint = [this, convention, out, out_u8](cudaGraphExec_t x, cudaGraphNode_t node) {
     return pre.update_graph_node(x, node, frames.data(), convention, dtype, out, out_u8);
   };
+}
+
+int EngineRuntime::rect_list(vpb_frame_fmt* f, const vpb_rectify** r, uint8_t** out) const {
+  int m = 0;
+  for (int k = 0; k < batch; ++k)
+    if (rect[k]) { f[m] = in_frames[k]; r[m] = rect[k]; out[m] = d_rect[k]; ++m; }
+  return m;
+}
+
+int EngineRuntime::set_rectify(int sample, const vpb_rectify* r, const char* who) {
+  if (sample < 0 || sample >= batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, batch); return VPB_ERR_ARG; }
+  if (r && r->gpu_id != gpu_id) {
+    vpb_set_error("%s: sample %d: the map lives on GPU %d, the engine on GPU %d", who, sample, r->gpu_id, gpu_id);
+    return VPB_ERR_ARG;
+  }
+  if ((rect[sample] != nullptr) != (r != nullptr)) frame_graph.invalidate();   // the rectify launch gains or loses a frame
+  rect[sample] = r;
+  n_frames = 0;                           // the last call's frames are not those the op list now reads
+  bool any = false;
+  for (int k = 0; k < batch; ++k) any |= rect[k] != nullptr;
+  if (any == rect_op()) return VPB_OK;
+  const int shift = any ? 1 : -1;
+  if (any) {
+    OpRec op;
+    op.name = "rectify"; op.kname = "rectify_kernel"; op.lane = 0;
+    op.launch = [this](cudaStream_t st) {
+      vpb_frame_fmt f[kMaxBatch]; const vpb_rectify* m[kMaxBatch]; uint8_t* o[kMaxBatch];
+      const int n = rect_list(f, m, o);
+      return rectify_x(f, m, n, rect_bgr, o, st);
+    };
+    op.repoint = [this](cudaGraphExec_t x, cudaGraphNode_t node) {
+      vpb_frame_fmt f[kMaxBatch]; const vpb_rectify* m[kMaxBatch]; uint8_t* o[kMaxBatch];
+      const int n = rect_list(f, m, o);
+      return rectify_update_node(x, node, f, m, n, rect_bgr, o);
+    };
+    ops.insert(ops.begin(), std::move(op));
+    if (!op_events.empty()) op_events.insert(op_events.begin(), Event());
+  } else {
+    ops.erase(ops.begin());
+    if (!op_events.empty()) op_events.erase(op_events.begin());
+  }
+  for (int& d : lane_dep) d += shift;
+  return VPB_OK;
 }
 
 int EngineRuntime::launch_op(size_t i, cudaStream_t st) {
@@ -399,6 +447,25 @@ bool frames_ok(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const
   return true;
 }
 
+// The frames the pre-process sees: a rectified sample's frame must have its map's source size (VPB_ERR_ARG naming who
+// and the frame otherwise) and becomes a packed descriptor of the map's size at d_rect[k] (NULL until the first call
+// grows it: host-only checks read the geometry alone).
+static bool rect_frames(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who, Frames& out) {
+  out = {};
+  std::copy(frames, frames + n, out.begin());
+  for (int k = 0; k < n; ++k) {
+    const vpb_rectify* r = e->rect[k];
+    if (!r) continue;
+    if (frames[k].h != r->src_h || frames[k].w != r->src_w) {
+      vpb_set_error("%s: frame %d is %dx%d; the map set for sample %d rectifies %dx%d frames", who, k, frames[k].w,
+                    frames[k].h, k, r->src_w, r->src_h);
+      return false;
+    }
+    out[k] = packed_frame(vpb_frame{e->d_rect[k], r->map_h, r->map_w, 3 * r->map_w});
+  }
+  return true;
+}
+
 // vpb_frame descriptors as VPB_PIX_PACKED ones (the first kMaxBatch; frames_ok rejects a count other than the batch)
 static bool packed_frames(const EngineRuntime* e, const vpb_frame* frames, int n, const char* who, Frames& out) {
   if (!e || !frames) { vpb_set_error("%s: bad arguments", who); return false; }
@@ -415,17 +482,38 @@ bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int
   return frames_ok(e, out.data(), n, who);
 }
 
-// The device frames f of geometries g become the runtime's frames, and op 0, the pre-process, gets the algorithmic
-// bytes of the call (SURVEY.md 8d: frame read + 3 x OH x OW 16-bit written, per sample; a frame reads h x w x 3 bytes
-// packed, x 2 in 4:2:2, x 1.5 in NV12, x 4 in BGRA / RGBA, x 1 in Bayer).  A failed call leaves no
-// frames, so nothing launches the pre-process on frames its tables were not built for.
+// The device frames f of geometries g (a rectified sample's: its map's size) become the runtime's frames, and the
+// pre-process op gets the algorithmic bytes of the call (SURVEY.md 8d: frame read + 3 x OH x OW 16-bit written, per
+// sample; frame_bytes).  A rectified sample's scratch buffer is grown here, outside any capture (a grown buffer drops
+// the captured graph), and the rectify op gets its bytes.  A failed call leaves no frames, so nothing launches the
+// pre-process on frames its tables were not built for.
 static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeom* g) {
-  e->frames = f;
+  e->in_frames = f;
+  Frames s = f;
+  for (int k = 0; k < n; ++k) {
+    const vpb_rectify* r = e->rect[k];
+    if (!r) continue;
+    const size_t bytes = static_cast<size_t>(r->map_h) * r->map_w * 3;
+    if (bytes > e->d_rect_cap[k]) {
+      e->frame_graph.invalidate();
+      void* p = nullptr;
+      VPB_CUDA_OK(cudaMalloc(&p, bytes));
+      e->dev_allocs.push_back(p);
+      e->d_rect[k] = static_cast<uint8_t*>(p); e->d_rect_cap[k] = bytes;
+    }
+    s[k] = packed_frame(vpb_frame{e->d_rect[k], r->map_h, r->map_w, 3 * r->map_w});
+  }
+  e->frames = s;
   e->n_frames = n;
   double bytes = 0;
-  static const double kBytesPerPixel[VPB_PIX_BAYER_GRBG + 1] = {3.0, 1.5, 2.0, 2.0, 0.0, 4.0, 4.0, 1.0, 1.0, 1.0, 1.0};
-  for (int k = 0; k < n; ++k) bytes += kBytesPerPixel[f[k].format] * g[k].h * g[k].w + 2.0 * 3 * g[k].OH * g[k].OW;
-  e->ops[0].bytes = bytes;
+  for (int k = 0; k < n; ++k) bytes += frame_bytes(s[k]) + 2.0 * 3 * g[k].OH * g[k].OW;
+  const int pre = e->rect_op() ? 1 : 0;
+  e->ops[pre].bytes = bytes;
+  if (pre) {
+    vpb_frame_fmt rf[kMaxBatch]; const vpb_rectify* rm[kMaxBatch]; uint8_t* ro[kMaxBatch];
+    const int m = e->rect_list(rf, rm, ro);
+    e->ops[0].bytes = rectify_bytes(rf, rm, m);
+  }
   const int rc = e->enqueue(g);
   if (rc) e->n_frames = 0;
   return rc;
@@ -433,8 +521,10 @@ static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeo
 
 int call_host(EngineRuntime* e, const vpb_frame_fmt* frames, int n, bool sync, bool raw, const char* who) {
   if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
+  Frames sub;
+  if (!rect_frames(e, frames, n, who, sub)) return VPB_ERR_ARG;
   PreGeom g[kMaxBatch];
-  if (e->geoms(frames, who, g)) return VPB_ERR_ARG;
+  if (e->geoms(sub.data(), who, g)) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
   Frames dev;
   int rc = e->upload_frames(frames, n, dev);
@@ -449,8 +539,10 @@ int call_host(EngineRuntime* e, const vpb_frame_fmt* frames, int n, bool sync, b
 
 int call_device(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who) {
   if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
+  Frames sub;
+  if (!rect_frames(e, frames, n, who, sub)) return VPB_ERR_ARG;
   PreGeom g[kMaxBatch];
-  if (e->geoms(frames, who, g)) return VPB_ERR_ARG;
+  if (e->geoms(sub.data(), who, g)) return VPB_ERR_ARG;
   Frames f{};
   std::copy(frames, frames + n, f.begin());
   DeviceGuard guard(e->gpu_id);

@@ -89,8 +89,10 @@ using Frames = std::array<vpb_frame_fmt, kMaxBatch>;
 
 struct EngineRuntime;
 // The CUDA graph of one call of a runtime's launch list, keyed on the n (format, h, w, stride, uv_stride) tuples and the
-// frame pointers (data, uv).  Frames of the captured geometries and formats in other buffers only re-point the captured
-// nodes of the ops that have repoint; a new format captures again (it selects another pre-process kernel).
+// frame pointers (data, uv) the pre-process reads (a rectified sample's packed descriptor of its map's size).  Frames of
+// the captured geometries and formats in other buffers only re-point the captured nodes of the ops that have repoint; a
+// new format captures again (it selects another pre-process kernel).  A rectified sample's own frame and map only
+// re-point: one rectify kernel takes every format.
 struct FrameGraph {
   cudaGraph_t graph = nullptr;           // kept alive: the recorded nodes are handles into it
   cudaGraphExec_t exec = nullptr;
@@ -98,6 +100,8 @@ struct FrameGraph {
   std::vector<std::pair<size_t, cudaGraphNode_t>> nodes;   // (op index, its captured kernel node) of the ops with repoint
   int n = 0;                             // the key: frames f[0 .. n-1] of the graph's last launch (0: none)
   Frames frames{};
+  Frames in_frames{};                    // and of a rectified sample the frame the rectify op read, and its map
+  std::array<const vpb_rectify*, kMaxBatch> rect{};
 
   // Launch the graph for e's frames on e's stream.  When the key differs in more than the frame pointers: e.launch_all
   // once outside capture (sets function attributes; its results are correct), capture e.launch_all and instantiate.
@@ -140,6 +144,15 @@ struct EngineRuntime {
   int n_frames = 0;                       // frames of that call (0: no call has run, or the last one failed)
   FrameGraph frame_graph;
   uint8_t* d_frame = nullptr; size_t d_frame_cap = 0;           // device copy of the host frames
+  // Lens rectification: rect[k] the map of sample k (NULL: none).  While a map is set, op 0 is "rectify": it writes
+  // sample k's rectified frame, packed, to d_rect[k] (grown on demand outside capture), and frames[k] describes that
+  // buffer, so the pre-process, the letterbox, the source outputs and the resized image see the rectified frame.
+  // in_frames are the call's device frames as given, which the rectify op reads.
+  std::array<const vpb_rectify*, kMaxBatch> rect{};
+  Frames in_frames{};
+  std::array<uint8_t*, kMaxBatch> d_rect{};
+  std::array<size_t, kMaxBatch> d_rect_cap{};
+  int rect_bgr = 0;                       // camera-native frames convert to BGR (the BGR conventions of add_preprocess)
   float* d_tap_scratch = nullptr; size_t tap_scratch_cap = 0;   // read_tap staging (grown on demand)
 
   EngineRuntime() = default;
@@ -164,6 +177,13 @@ struct EngineRuntime {
   // append the pre-process of the call's frames into out (+ the uint8 resized image out_u8, may be NULL) as op
   // "preprocess" on lane 0; the engines call it before their first op
   void add_preprocess(int convention, void* out, uint8_t* out_u8);
+  // Map r (NULL: none) for sample `sample` of every later call: VPB_ERR_ARG (naming who) for a sample out of range or a
+  // map of another GPU.  The first map inserts the op "rectify" at index 0 and clearing the last one removes it (the
+  // lanes' producer indices follow); a sample gaining or losing its map drops the captured graph.
+  int set_rectify(int sample, const vpb_rectify* r, const char* who);
+  bool rect_op() const { return !ops.empty() && ops[0].kname == "rectify_kernel"; }
+  // the rectified samples of the current call, in sample order: their frames, maps and scratch buffers; the count
+  int rect_list(vpb_frame_fmt* f, const vpb_rectify** r, uint8_t** out) const;
   // the ops appended next form `lane`, which starts after ops[dep_op]
   void begin_lane(int lane, int dep_op) { cur_lane = lane; lane_dep.resize(lane + 1); lane_dep[lane] = dep_op; }
   // launch ops[i] on st; while frame_graph captures, an op with repoint records its kernel node

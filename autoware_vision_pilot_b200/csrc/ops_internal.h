@@ -38,6 +38,12 @@ inline int frame_row_bytes(const vpb_frame_fmt& f) {
     default: return f.w;
   }
 }
+// Bytes of the frame's image data (h x w x 3 packed, x 2 in 4:2:2, x 1.5 in NV12, x 4 in BGRA / RGBA, x 1 in Bayer): what a
+// kernel reading the whole frame once reads
+inline double frame_bytes(const vpb_frame_fmt& f) {
+  static const double kBytesPerPixel[VPB_PIX_BAYER_GRBG + 1] = {3.0, 1.5, 2.0, 2.0, 0.0, 4.0, 4.0, 1.0, 1.0, 1.0, 1.0};
+  return kBytesPerPixel[f.format] * f.h * f.w;
+}
 inline vpb_frame_fmt packed_frame(const vpb_frame& f) {
   vpb_frame_fmt o{};
   o.format = VPB_PIX_PACKED; o.data = f.data; o.h = f.h; o.w = f.w; o.stride = f.stride;
@@ -110,6 +116,14 @@ int source_outputs_x(const vpb_src_job* jobs, int n, cudaStream_t st);
 int source_outputs_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_src_job* jobs, int n);
 double source_outputs_bytes(const vpb_src_job* jobs, int n);
 int viz_tables_init();
+// vpb_rectify_frames (rectify.cu) without its argument checks: n frames, rect[k] their maps, out[k] the packed rectified
+// frames, one launch; rectify_update_node re-points a captured rectify_kernel node at other frames, maps of the same
+// sizes and outputs; rectify_bytes: algorithmic HBM bytes of one launch (maps and frames read, outputs written).
+int rectify_x(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out,
+              cudaStream_t st);
+int rectify_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames,
+                        const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out);
+double rectify_bytes(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n);
 
 // One-time per-DEVICE initialisation (function attributes, constant tables): engines for several GPUs may
 // live in one process, and entry points may be called from several threads.
@@ -119,3 +133,10 @@ std::mutex& init_mutex();
 bool* device_flag(InitSlot slot);    // flag of `slot` for the calling thread's current CUDA device
 
 }  // namespace vpb
+
+// A map object of vpb_rectify_create: both maps in one device allocation of the device gpu_id, map2 after map1
+struct vpb_rectify {
+  const int16_t* map1;    // [map_h][map_w][2] (sx, sy)
+  const uint16_t* map2;   // [map_h][map_w] fraction
+  int map_h, map_w, src_h, src_w, gpu_id;
+};

@@ -102,6 +102,7 @@ def _bind():
     lib.vp_engine_stream.argtypes = [C.c_void_p]
     lib.vp_engine_stream.restype = C.c_void_p
     lib.vp_engine_source_output.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_SourceOutput)]
+    lib.vp_engine_set_rectify.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     lib.vp_engine_time_kind.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_double),
                                         C.POINTER(C.c_int)]
     lib.vp_engine_kernel_names.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int)]
@@ -142,6 +143,7 @@ class Engine:
         L.check(self._lib.vp_engine_create(C.byref(cfg), C.byref(self._h)), "vp_engine_create")
         self.kinds = list(kinds)
         self.batch = max(1, batch)
+        self._rectify = {}
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -149,6 +151,14 @@ class Engine:
             self._h = C.c_void_p()
 
     __del__ = close
+
+    def set_rectify(self, sample: int, r: Optional[L.Rectify]) -> None:
+        """Remap sample `sample`'s frame through the maps of r (an _lib.Rectify) in every later call, before the
+        pre-process, or stop doing so (r None).  The outputs, the resized image and the source outputs are then those
+        of the rectified frame (r.h x r.w).  The engine keeps r alive while it is set."""
+        L.check(self._lib.vp_engine_set_rectify(self._h, sample, r.handle if r is not None else None),
+                "vp_engine_set_rectify")
+        self._rectify[sample] = r
 
     # ---- inference
     @staticmethod

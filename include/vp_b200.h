@@ -146,12 +146,24 @@ int vp_engine_infer_device_frames(vp_engine* e, const vpb_frame* frames_dev, int
  * to the packed call on the cvtColor-converted frame.  Host frames upload only their valid bytes per row (2w per 4:2:2
  * row, w per Y and UV row of NV12, 4w per BGRA / RGBA row, w per Bayer row).  Checks as for the *_frames calls plus
  * those of vpb_preprocess_fmt; VP_SRC_OVERLAY needs the camera frame as packed pixels, so an overlay engine given any
- * other format returns VPB_ERR_ARG before any device work.  The
+ * other format returns VPB_ERR_ARG before any device work, unless the sample is rectified (vp_engine_set_rectify: the
+ * overlay blends the packed rectified frame).  The
  * frame graph's key adds each frame's format and uv_stride: new data / uv pointers re-point the captured nodes, a new
  * format captures again.  The split-fp16 mode takes them with n = 1. */
 int vp_engine_infer_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n);
 int vp_engine_submit_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n);
 int vp_engine_infer_device_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_dev, int n);
+/* Lens rectification inside the call (image_proc's rectify): with map r (vpb_rectify_create, vp_b200_ops.h) set for
+ * sample `sample`, every later call of every form (single, *_batch, *_frames, *_frames_fmt; host, submit and device)
+ * first remaps that sample's frame through r, byte-equal to cv::remap(cv::cvtColor(frame), map1, map2, INTER_LINEAR)
+ * (a packed frame is remapped as it is), and runs everything after it on the rectified frame: the outputs, the resized
+ * image and the source outputs (at the map's size; VP_SRC_OVERLAY blends the rectified frame, whatever its camera
+ * format) equal the packed call on the rectified frame.  A call adds the op "rectify" before the pre-process; a frame
+ * whose h x w is not the map's source size returns VPB_ERR_ARG naming the call and the frame, before any device work.
+ * r NULL clears the sample's map.  VPB_ERR_ARG for a sample outside 0 .. batch-1 or a map created on another GPU.  The
+ * engine keeps the pointer: r must outlive every call that uses it.  The lateral post-process of a rectified camera
+ * takes the map's size as its image size. */
+int vp_engine_set_rectify(vp_engine* e, int sample, const vpb_rectify* r);
 /* Copy the raw fp32 tensor of one model to its host buffer (after a device/async inference). */
 int vp_engine_fetch_raw(vp_engine* e, int model_idx);
 

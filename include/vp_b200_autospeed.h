@@ -68,6 +68,9 @@ int vp_autospeed_infer_device_frames(vp_autospeed* e, const vpb_frame* frames_de
  * *_frames calls plus those of vpb_preprocess_fmt. */
 int vp_autospeed_infer_frames_fmt(vp_autospeed* e, const vpb_frame_fmt* frames_host, int n, int fetch_raw);
 int vp_autospeed_infer_device_frames_fmt(vp_autospeed* e, const vpb_frame_fmt* frames_dev, int n);
+/* Lens rectification of sample `sample` in every later call, as vp_engine_set_rectify (vp_b200.h): the letterbox reads
+ * the rectified frame, so detections are in the rectified frame's pixels.  r NULL clears it. */
+int vp_autospeed_set_rectify(vp_autospeed* e, int sample, const vpb_rectify* r);
 /* Drain the stream; fetch: 0 nothing, 1 detections, 2 detections + raw tensor to the host buffers (all samples). */
 int vp_autospeed_sync(vp_autospeed* e, int fetch);
 

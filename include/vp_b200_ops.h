@@ -225,6 +225,33 @@ int vpb_preprocess(const uint8_t* src_dev, int h, int w, int stride, int resize_
  * VPB_RESIZE_NONE, or a Pillow filter of more than 32 taps. */
 int vpb_preprocess_fmt(const vpb_frame_fmt* frame_dev, int resize_mode, int convention, int dtype, void* out_dev,
                        uint8_t* out_u8_dev, void* stream);
+
+/* Lens rectification (image_proc's rectify): a frame remapped through OpenCV's fixed-point undistortion maps, as
+ * cv::remap(src, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) does it, byte for byte.  map1 int16 [map_h][map_w][2] is
+ * the integer source position (sx, sy) of each rectified pixel and map2 uint16 [map_h][map_w] its fraction (f = map2 &
+ * 1023, fx = f & 31, fy = f >> 5): the CV_16SC2 pair of cv::initUndistortRectifyMap / cv::fisheye::
+ * initUndistortRectifyMap, or cv::convertMaps(..., CV_16SC2) of float maps.  Each rectified pixel is
+ * clip((sum_i tab[f][i] * p_i + 2^14) >> 15, 0, 255) per channel over the neighbours (sx, sy), (sx+1, sy), (sx, sy+1),
+ * (sx+1, sy+1), with OpenCV's initInterTab2D(INTER_LINEAR) weights tab[f] and a neighbour outside the frame counting 0.
+ * A camera-native frame is converted first, pixel by pixel as the pre-process converts it (cv::cvtColor, then
+ * cv::remap: image_proc's order).
+ * The map object holds the maps on one device (6 bytes per rectified pixel) for frames of src_h x src_w. */
+typedef struct vpb_rectify vpb_rectify;
+/* map1 int16 [map_h][map_w][2], map2 uint16 [map_h][map_w] (host); frames it rectifies are src_h x src_w.  VPB_ERR_ARG
+ * before the device is opened for NULL maps or output, a size <= 0, or a map larger than every resize mode of the
+ * pre-process takes (map_w > 4800 or map_h > 2400: a Pillow filter of more than 32 taps to 640 x 320). */
+int  vpb_rectify_create(const int16_t* map1, const uint16_t* map2, int map_h, int map_w, int src_h, int src_w,
+                        int gpu_id, vpb_rectify** out);
+/* The caller keeps a map alive while an engine it is set on (vp_engine_set_rectify, vp_autospeed_set_rectify) may run
+ * a call. */
+void vpb_rectify_destroy(vpb_rectify* r);
+/* Op level: n device frames (host array of vpb_frame_fmt, any format), rect[k] their maps, in one launch; out[k] the
+ * packed rectified frame [map_h_k][3*map_w_k] (device).  bgr selects the channel order camera-native formats convert to
+ * (packed frames keep theirs).  VPB_ERR_ARG before any device work for n outside 1..VP_MAX_BATCH, a NULL array, map or
+ * output, a bad descriptor, a frame whose h x w is not its map's source size, or a map of another device than the
+ * current one. */
+int  vpb_rectify_frames(const vpb_frame_fmt* frames_dev, const vpb_rectify* const* rect, int n, int bgr,
+                        uint8_t* const* out, void* stream);
 /* Host-only: the integer coefficient tables the kernel uses (bounds[out_size],
  * coeffs[out_size*ksize]); lets a CPU test pin them against Pillow / OpenCV without a GPU. */
 int vpb_resize_tables_host(int mode, int in_size, int out_size, int* bounds, int* coeffs,

@@ -70,6 +70,8 @@ def frame_descs(descs) -> "C.Array":
 PIX_PACKED, PIX_NV12, PIX_UYVY, PIX_YUYV = 0, 1, 2, 3    # VPB_PIX_* (4 is unassigned)
 PIX_BGRA, PIX_RGBA = 5, 6
 PIX_BAYER_RGGB, PIX_BAYER_BGGR, PIX_BAYER_GBRG, PIX_BAYER_GRBG = 7, 8, 9, 10
+PIX_JPEG = 11
+JPEG_SAMPLING = {0: "444", 1: "422", 2: "420"}     # VPB_JPEG_*
 BAYER_PATTERNS = {"rggb": PIX_BAYER_RGGB, "bggr": PIX_BAYER_BGGR, "gbrg": PIX_BAYER_GBRG, "grbg": PIX_BAYER_GRBG}
 
 
@@ -186,7 +188,63 @@ class Bayer:
         return FrameFmt(self.format, a.ctypes.data, self.h, self.w, a.strides[0], None, 0), (a,)
 
 
+class JPEG:
+    """A host JPEG stream (ROS sensor_msgs/CompressedImage "jpeg", a UVC camera's MJPEG frame): bytes or a 1-D uint8
+    array.  h, w and sampling ("444", "422", "420") come from its headers (vpb_jpeg_info); a stream the decoder does not
+    take (progressive, grayscale, other sampling, ...) raises with the library's reason, and cv2.imdecode plus the
+    packed frame is the fall-back.  Engines decode it on the device byte-equal to
+    cv2.imdecode(buf, cv2.IMREAD_COLOR | cv2.IMREAD_IGNORE_ORIENTATION), in the convention's channel order."""
+
+    format = PIX_JPEG
+
+    def __init__(self, data):
+        if isinstance(data, (bytes, bytearray, memoryview)):
+            data = np.frombuffer(bytes(data), np.uint8)
+        if not isinstance(data, np.ndarray) or data.dtype != np.uint8 or data.ndim != 1:
+            raise ValueError("JPEG: bytes or a 1-D uint8 array expected")
+        self.data = np.ascontiguousarray(data)
+        h, w, s = C.c_int(), C.c_int(), C.c_int()
+        lib_ = lib()
+        lib_.vpb_jpeg_info.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                       C.POINTER(C.c_int)]
+        check(lib_.vpb_jpeg_info(self.data.ctypes.data, self.data.size, C.byref(h), C.byref(w), C.byref(s)),
+              "vpb_jpeg_info")
+        self.h, self.w, self.sampling = h.value, w.value, JPEG_SAMPLING[s.value]
+
+    def desc(self, allow_copy: bool = True):
+        return FrameFmt(PIX_JPEG, self.data.ctypes.data, self.h, self.w, self.data.size, None, 0), (self.data,)
+
+
 FRAME_TYPES = (NV12, UYVY, YUYV, BGRA, RGBA, Bayer)    # the camera-native frame objects the engines take
+HOST_FRAME_TYPES = FRAME_TYPES + (JPEG,)               # and what their host calls also take
+
+
+class JpegDecoder:
+    """The op-level decoder (vpb_jpeg_decoder_create): up to n frames of up to h x w per decode() call on one GPU."""
+
+    def __init__(self, max_h: int, max_w: int, max_n: int = 1, gpu_id: int = 0):
+        lib_ = lib()
+        lib_.vpb_jpeg_decoder_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
+        lib_.vpb_jpeg_decoder_destroy.argtypes = [C.c_void_p]
+        lib_.vpb_jpeg_decoder_destroy.restype = None
+        lib_.vpb_jpeg_decode.argtypes = [C.c_void_p, C.POINTER(FrameFmt), C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                         C.c_void_p]
+        self._lib, self._h = lib_, C.c_void_p()
+        check(lib_.vpb_jpeg_decoder_create(max_h, max_w, max_n, gpu_id, C.byref(self._h)), "vpb_jpeg_decoder_create")
+
+    def decode(self, frames, out_ptrs, bgr: bool = True, stream: int = 0) -> None:
+        """JPEG objects -> device packed frames at out_ptrs (asynchronous on `stream`)"""
+        frames = list(frames)
+        arr = (FrameFmt * len(frames))(*[f.desc()[0] for f in frames])
+        outs = (C.c_void_p * len(frames))(*out_ptrs)
+        check(self._lib.vpb_jpeg_decode(self._h, arr, len(frames), int(bgr), outs, stream or None), "vpb_jpeg_decode")
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self._lib.vpb_jpeg_decoder_destroy(self._h)
+            self._h = C.c_void_p()
+
+    __del__ = close
 
 
 class Rectify:

@@ -138,10 +138,10 @@ class AutoSpeedEngine:
         cv2.cvtColor would."""
         frames = list(frames)
         self._check_count(len(frames))
-        if any(isinstance(f, L.FRAME_TYPES) for f in frames):
+        if any(isinstance(f, L.HOST_FRAME_TYPES) for f in frames):
             arr, keep = (L.FrameFmt * len(frames))(), []
             for k, f in enumerate(frames):
-                d, alive = f.desc() if isinstance(f, L.FRAME_TYPES) else L.packed_desc(self._check_frame(f))
+                d, alive = f.desc() if isinstance(f, L.HOST_FRAME_TYPES) else L.packed_desc(self._check_frame(f))
                 arr[k] = d
                 keep.append(alive)
             L.check(self._lib.vp_autospeed_infer_frames_fmt(self._h, arr, len(frames), int(fetch_raw)),

@@ -119,6 +119,7 @@ int FrameGraph::run(EngineRuntime& e) {
     same_src = rect[k] == e.rect[k] && (!rect[k] || (same_geometry(in_frames[k], e.in_frames[k]) &&
                                                      in_frames[k].data == e.in_frames[k].data &&
                                                      in_frames[k].uv == e.in_frames[k].uv));
+  if (e.n_jpeg) same_src = false;
   if (same_geom && !same_src) {
     for (const auto& [i, node] : nodes) {
       const int rc = e.ops[i].repoint(exec, node);
@@ -281,6 +282,44 @@ int EngineRuntime::rect_list(vpb_frame_fmt* f, const vpb_rectify** r, uint8_t** 
   return m;
 }
 
+int EngineRuntime::op_index(const char* name) const {
+  for (size_t i = 0; i < ops.size(); ++i)
+    if (ops[i].name == name) return static_cast<int>(i);
+  return -1;
+}
+
+void EngineRuntime::insert_ops(size_t at, std::vector<OpRec> add) {
+  frame_graph.invalidate();
+  const int m = static_cast<int>(add.size());
+  ops.insert(ops.begin() + at, std::make_move_iterator(add.begin()), std::make_move_iterator(add.end()));
+  if (!op_events.empty())
+    for (int i = 0; i < m; ++i) op_events.insert(op_events.begin() + at, Event());
+  for (int& d : lane_dep) d += m;
+}
+
+void EngineRuntime::erase_ops(size_t at, size_t m) {
+  frame_graph.invalidate();
+  ops.erase(ops.begin() + at, ops.begin() + at + m);
+  if (!op_events.empty()) op_events.erase(op_events.begin() + at, op_events.begin() + at + m);
+  for (int& d : lane_dep) d -= static_cast<int>(m);
+}
+
+void EngineRuntime::sync_jpeg_ops() {
+  static const char* kOps[3][2] = {{"jpeg_huffman", "jpeg_huffman_kernel"}, {"jpeg_idct", "jpeg_idct_kernel"},
+                                   {"jpeg_color", "jpeg_color_kernel"}};
+  const bool have = op_index(kOps[0][0]) >= 0;
+  if (have == (n_jpeg > 0)) return;
+  if (have) { erase_ops(0, 3); return; }
+  std::vector<OpRec> add(3);
+  for (int k = 0; k < 3; ++k) {
+    OpRec& op = add[k];
+    op.name = kOps[k][0]; op.kname = kOps[k][1]; op.lane = 0;
+    op.launch = [this, k](cudaStream_t st) { return jpeg->launch(k, st); };
+    op.repoint = [this, k](cudaGraphExec_t x, cudaGraphNode_t node) { return jpeg->update_node(k, x, node); };
+  }
+  insert_ops(0, std::move(add));
+}
+
 int EngineRuntime::set_rectify(int sample, const vpb_rectify* r, const char* who) {
   if (sample < 0 || sample >= batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, batch); return VPB_ERR_ARG; }
   if (r && r->gpu_id != gpu_id) {
@@ -293,7 +332,6 @@ int EngineRuntime::set_rectify(int sample, const vpb_rectify* r, const char* who
   bool any = false;
   for (int k = 0; k < batch; ++k) any |= rect[k] != nullptr;
   if (any == rect_op()) return VPB_OK;
-  const int shift = any ? 1 : -1;
   if (any) {
     OpRec op;
     op.name = "rectify"; op.kname = "rectify_kernel"; op.lane = 0;
@@ -307,13 +345,12 @@ int EngineRuntime::set_rectify(int sample, const vpb_rectify* r, const char* who
       const int n = rect_list(f, m, o);
       return rectify_update_node(x, node, f, m, n, rect_bgr, o);
     };
-    ops.insert(ops.begin(), std::move(op));
-    if (!op_events.empty()) op_events.insert(op_events.begin(), Event());
+    std::vector<OpRec> add;
+    add.push_back(std::move(op));
+    insert_ops(op_index("preprocess"), std::move(add));      // after the JPEG decode: rectify reads the decoded frame
   } else {
-    ops.erase(ops.begin());
-    if (!op_events.empty()) op_events.erase(op_events.begin());
+    erase_ops(op_index("rectify"), 1);
   }
-  for (int& d : lane_dep) d += shift;
   return VPB_OK;
 }
 
@@ -448,14 +485,19 @@ bool frames_ok(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const
 }
 
 // The frames the pre-process sees: a rectified sample's frame must have its map's source size (VPB_ERR_ARG naming who
-// and the frame otherwise) and becomes a packed descriptor of the map's size at d_rect[k] (NULL until the first call
-// grows it: host-only checks read the geometry alone).
+// and the frame otherwise) and becomes a packed descriptor of the map's size at d_rect[k], and any other JPEG sample a
+// packed descriptor of its size at d_jpg[k] (NULL until the first call grows them: host-only checks read the geometry
+// alone).
 static bool rect_frames(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who, Frames& out) {
   out = {};
   std::copy(frames, frames + n, out.begin());
   for (int k = 0; k < n; ++k) {
     const vpb_rectify* r = e->rect[k];
-    if (!r) continue;
+    if (!r) {
+      if (frames[k].format == VPB_PIX_JPEG)
+        out[k] = packed_frame(vpb_frame{e->d_jpg[k], frames[k].h, frames[k].w, 3 * frames[k].w});
+      continue;
+    }
     if (frames[k].h != r->src_h || frames[k].w != r->src_w) {
       vpb_set_error("%s: frame %d is %dx%d; the map set for sample %d rectifies %dx%d frames", who, k, frames[k].w,
                     frames[k].h, k, r->src_w, r->src_h);
@@ -485,7 +527,8 @@ bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int
 // The device frames f of geometries g (a rectified sample's: its map's size) become the runtime's frames, and the
 // pre-process op gets the algorithmic bytes of the call (SURVEY.md 8d: frame read + 3 x OH x OW 16-bit written, per
 // sample; frame_bytes).  A rectified sample's scratch buffer is grown here, outside any capture (a grown buffer drops
-// the captured graph), and the rectify op gets its bytes.  A failed call leaves no frames, so nothing launches the
+// the captured graph), and the rectify op gets its bytes.  The JPEG decode ops are there exactly when the call has a
+// JPEG frame, with the bytes of the call's streams.  A failed call leaves no frames, so nothing launches the
 // pre-process on frames its tables were not built for.
 static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeom* g) {
   e->in_frames = f;
@@ -505,14 +548,17 @@ static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeo
   }
   e->frames = s;
   e->n_frames = n;
+  e->sync_jpeg_ops();
+  if (e->n_jpeg)
+    for (int k = 0; k < 3; ++k) e->ops[k].bytes = e->jpeg->bytes(k);
   double bytes = 0;
   for (int k = 0; k < n; ++k) bytes += frame_bytes(s[k]) + 2.0 * 3 * g[k].OH * g[k].OW;
-  const int pre = e->rect_op() ? 1 : 0;
-  e->ops[pre].bytes = bytes;
-  if (pre) {
+  e->ops[e->op_index("preprocess")].bytes = bytes;
+  const int ri = e->op_index("rectify");
+  if (ri >= 0) {
     vpb_frame_fmt rf[kMaxBatch]; const vpb_rectify* rm[kMaxBatch]; uint8_t* ro[kMaxBatch];
     const int m = e->rect_list(rf, rm, ro);
-    e->ops[0].bytes = rectify_bytes(rf, rm, m);
+    e->ops[ri].bytes = rectify_bytes(rf, rm, m);
   }
   const int rc = e->enqueue(g);
   if (rc) e->n_frames = 0;
@@ -538,6 +584,7 @@ int call_host(EngineRuntime* e, const vpb_frame_fmt* frames, int n, bool sync, b
 }
 
 int call_device(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who) {
+  if (no_jpeg(frames, n, who)) return VPB_ERR_ARG;
   if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
   Frames sub;
   if (!rect_frames(e, frames, n, who, sub)) return VPB_ERR_ARG;
@@ -546,6 +593,7 @@ int call_device(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char
   Frames f{};
   std::copy(frames, frames + n, f.begin());
   DeviceGuard guard(e->gpu_id);
+  e->n_jpeg = 0;
   return enqueue_frames(e, f, n, g);
 }
 
@@ -572,6 +620,7 @@ int EngineRuntime::upload_frames(const vpb_frame_fmt* frames, int n, Frames& dev
   size_t total = 0;
   for (int k = 0; k < n; ++k) {
     const vpb_frame_fmt& f = frames[k];
+    if (f.format == VPB_PIX_JPEG) continue;
     total += static_cast<size_t>(f.h) * frame_row_bytes(f) + (f.format == VPB_PIX_NV12 ? static_cast<size_t>(f.h / 2) * f.w : 0);
   }
   if (total > d_frame_cap) {
@@ -582,9 +631,31 @@ int EngineRuntime::upload_frames(const vpb_frame_fmt* frames, int n, Frames& dev
     d_frame = static_cast<uint8_t*>(p); d_frame_cap = total;
   }
   dev = {};
+  n_jpeg = 0;
+  const vpb_frame_fmt* jf[kMaxBatch];
+  uint8_t* jo[kMaxBatch];
+  for (int k = 0; k < n; ++k) {
+    const vpb_frame_fmt& f = frames[k];
+    if (f.format != VPB_PIX_JPEG) continue;
+    const size_t bytes = static_cast<size_t>(f.h) * f.w * 3;
+    if (bytes > d_jpg_cap[k]) {
+      void* p = nullptr;
+      VPB_CUDA_OK(cudaMalloc(&p, bytes));
+      dev_allocs.push_back(p);
+      d_jpg[k] = static_cast<uint8_t*>(p); d_jpg_cap[k] = bytes;
+    }
+    dev[k] = packed_frame(vpb_frame{d_jpg[k], f.h, f.w, 3 * f.w});
+    jf[n_jpeg] = &f; jo[n_jpeg] = d_jpg[k]; ++n_jpeg;
+  }
+  if (n_jpeg) {
+    if (!jpeg) jpeg = std::make_unique<JpegDecoder>();
+    const int rc = jpeg->stage(jf, n_jpeg, jo, rect_bgr, stream);
+    if (rc) { n_jpeg = 0; return rc; }
+  }
   size_t off = 0;
   for (int k = 0; k < n; ++k) {
     const vpb_frame_fmt& f = frames[k];
+    if (f.format == VPB_PIX_JPEG) continue;
     const int dpitch = frame_row_bytes(f);
     uint8_t* d = d_frame + off;
     dev[k] = f;

@@ -89,10 +89,11 @@ using Frames = std::array<vpb_frame_fmt, kMaxBatch>;
 
 struct EngineRuntime;
 // The CUDA graph of one call of a runtime's launch list, keyed on the n (format, h, w, stride, uv_stride) tuples and the
-// frame pointers (data, uv) the pre-process reads (a rectified sample's packed descriptor of its map's size).  Frames of
+// frame pointers (data, uv) the pre-process reads (a rectified or JPEG sample's packed descriptor of its scratch buffer).  Frames of
 // the captured geometries and formats in other buffers only re-point the captured nodes of the ops that have repoint; a
 // new format captures again (it selects another pre-process kernel).  A rectified sample's own frame and map only
-// re-point: one rectify kernel takes every format.
+// re-point: one rectify kernel takes every format.  A call with a JPEG frame always re-points: its streams' lengths,
+// tables and launch grids are those of the call.
 struct FrameGraph {
   cudaGraph_t graph = nullptr;           // kept alive: the recorded nodes are handles into it
   cudaGraphExec_t exec = nullptr;
@@ -137,7 +138,8 @@ struct EngineRuntime {
   size_t weight_bytes = 0, act_bytes = 0;
   std::vector<std::unique_ptr<ConvPlan>> plans;
   std::vector<vpb_conv_args> conv_list;   // [plan] the arguments each plan was built from
-  std::vector<OpRec> ops;                // every launch of a call, in order; op 0 is the pre-process
+  std::vector<OpRec> ops;                // every launch of a call, in order: the JPEG decode and rectify ops while they
+                                         // are needed, then the pre-process
   std::map<std::string, Tap> taps;
   PreprocessPlan pre;
   Frames frames{};                        // device frames of the current / last call
@@ -152,7 +154,15 @@ struct EngineRuntime {
   Frames in_frames{};
   std::array<uint8_t*, kMaxBatch> d_rect{};
   std::array<size_t, kMaxBatch> d_rect_cap{};
-  int rect_bgr = 0;                       // camera-native frames convert to BGR (the BGR conventions of add_preprocess)
+  int rect_bgr = 0;                       // camera-native and JPEG frames convert to BGR (the BGR conventions of
+                                          // add_preprocess)
+  // JPEG frames of host calls: upload_frames stages the call's streams in `jpeg` and gives sample k the packed
+  // descriptor of d_jpg[k] (grown on demand outside capture), which the ops "jpeg_huffman", "jpeg_idct" and
+  // "jpeg_color" (ops 0..2 while the current call has a JPEG frame, n_jpeg > 0) decode into.
+  std::unique_ptr<JpegDecoder> jpeg;
+  std::array<uint8_t*, kMaxBatch> d_jpg{};
+  std::array<size_t, kMaxBatch> d_jpg_cap{};
+  int n_jpeg = 0;
   float* d_tap_scratch = nullptr; size_t tap_scratch_cap = 0;   // read_tap staging (grown on demand)
 
   EngineRuntime() = default;
@@ -181,7 +191,14 @@ struct EngineRuntime {
   // map of another GPU.  The first map inserts the op "rectify" at index 0 and clearing the last one removes it (the
   // lanes' producer indices follow); a sample gaining or losing its map drops the captured graph.
   int set_rectify(int sample, const vpb_rectify* r, const char* who);
-  bool rect_op() const { return !ops.empty() && ops[0].kname == "rectify_kernel"; }
+  bool rect_op() const { return op_index("rectify") >= 0; }
+  int op_index(const char* name) const;   // index of the op of that name, -1 if there is none
+  // insert ops at index `at` / erase m ops from `at`: the op events and the lanes' producer indices follow, and the
+  // captured graph is dropped
+  void insert_ops(size_t at, std::vector<OpRec> add);
+  void erase_ops(size_t at, size_t m);
+  // the three JPEG decode ops at the front of the list exactly while the current call has a JPEG frame
+  void sync_jpeg_ops();
   // the rectified samples of the current call, in sample order: their frames, maps and scratch buffers; the count
   int rect_list(vpb_frame_fmt* f, const vpb_rectify** r, uint8_t** out) const;
   // the ops appended next form `lane`, which starts after ops[dep_op]
@@ -209,7 +226,8 @@ struct EngineRuntime {
   // Copy n host frames to d_frame (grown on demand), plane after plane, frame after frame, each row with the pitch of its
   // valid bytes (3w packed, 2w UYVY / YUYV, w for the Y and the UV rows of NV12): only those bytes of every row are read
   // from the caller's buffer, so a cv::Mat ROI / strided view is never read past its last row.  dev[k] describes the
-  // device copy of frame k (its uv inside d_frame for NV12).
+  // device copy of frame k (its uv inside d_frame for NV12).  JPEG frames are staged in `jpeg` instead (n_jpeg counts
+  // them) and dev[k] is the packed descriptor of d_jpg[k], which the JPEG ops write.
   int upload_frames(const vpb_frame_fmt* frames, int n, Frames& dev);
   // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
   bool find_tap(const char* name, Tap* out) const;

@@ -41,6 +41,7 @@ inline int frame_row_bytes(const vpb_frame_fmt& f) {
 // Bytes of the frame's image data (h x w x 3 packed, x 2 in 4:2:2, x 1.5 in NV12, x 4 in BGRA / RGBA, x 1 in Bayer): what a
 // kernel reading the whole frame once reads
 inline double frame_bytes(const vpb_frame_fmt& f) {
+  if (f.format == VPB_PIX_JPEG) return f.stride;       // the stream's length
   static const double kBytesPerPixel[VPB_PIX_BAYER_GRBG + 1] = {3.0, 1.5, 2.0, 2.0, 0.0, 4.0, 4.0, 1.0, 1.0, 1.0, 1.0};
   return kBytesPerPixel[f.format] * f.h * f.w;
 }
@@ -124,6 +125,50 @@ int rectify_x(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n
 int rectify_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames,
                         const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out);
 double rectify_bytes(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n);
+
+// JPEG frames (jpeg.cu).  jpeg_frame_check: the host header parse of a VPB_PIX_JPEG descriptor (frame_fmt_check's JPEG
+// case): VPB_ERR_ARG "<who>: frame <k>: ..." for a stream the decoder does not take or an h x w other than the SOF's.
+// no_jpeg: VPB_ERR_ARG for a JPEG descriptor among device frames (their headers cannot be parsed on the host).
+int jpeg_frame_check(const vpb_frame_fmt& f, const char* who, int k);
+int no_jpeg(const vpb_frame_fmt* frames, int n, const char* who);
+struct JpegHdrDev;
+struct JpegImg {                 // one stream of a decode call (the kernels' parameter block)
+  const JpegHdrDev* hdr;         // Huffman lookup tables, natural-order quantisation tables
+  const uint32_t* segs;          // [nseg + 1] byte offsets of the restart segments in data, the last = its length
+  const uint8_t* data;           // the entropy-coded data, stuffing removed, RSTn markers dropped, zero-padded
+  int nbits, nwords, nseg, nsub, nctas;
+  int ri_blocks, nblocks, bpm, hs, vs, mx, h, w, ypitch, cpitch;
+  size_t yplane, cplane;         // bytes of the Y plane and of each chroma plane
+  int16_t* coef;                 // [nblocks][64] natural order, zeroed by the staging
+  int* dcv;                      // [nblocks] DC values, zeroed by the staging
+  uint8_t* plane;                // Y, Cb, Cr planes of the padded MCU grid
+  uint8_t* chain;                // the Huffman kernel's CTA chain (zero between calls)
+  uint8_t* out;                  // packed [h][3w]
+};
+struct JpegParams { JpegImg im[kMaxBatch]; int bgr; };
+// Device decoding of the JPEG frames of one call: stage() parses the n host streams, builds the tables, destuffs the
+// data into pinned memory, uploads it and zeroes the coefficients on st (buffers grown on demand, the stream drained
+// first); launch(k) /
+// update_node(k) run or re-point kernel k (0 Huffman, 1 IDCT, 2 colour) of the staged call, writing frame j of the call
+// packed to out[j], B, G, R for bgr, else R, G, B.
+struct JpegDecoder {
+  JpegParams p{};
+  dim3 grid[3];
+  uint8_t* h_stage = nullptr; size_t h_cap = 0;        // pinned
+  uint8_t* d_stage = nullptr; size_t stage_cap = 0;    // headers, data and segment tables
+  uint8_t* d_work = nullptr; size_t work_cap = 0;      // coefficients, DC values, planes
+  uint8_t* d_chain = nullptr; size_t chain_cap = 0;
+  cudaEvent_t staged = nullptr;                        // the last upload has read h_stage
+  double stream_bytes = 0, coef_bytes = 0, plane_bytes = 0, out_bytes = 0;
+  JpegDecoder() = default;
+  JpegDecoder(const JpegDecoder&) = delete;
+  JpegDecoder& operator=(const JpegDecoder&) = delete;
+  ~JpegDecoder();
+  int stage(const vpb_frame_fmt* const* frames, int n, uint8_t* const* out, int bgr, cudaStream_t st);
+  int launch(int k, cudaStream_t st) const;
+  int update_node(int k, cudaGraphExec_t exec, cudaGraphNode_t node) const;
+  double bytes(int k) const;     // algorithmic HBM bytes of kernel k's launch
+};
 
 // One-time per-DEVICE initialisation (function attributes, constant tables): engines for several GPUs may
 // live in one process, and entry points may be called from several threads.

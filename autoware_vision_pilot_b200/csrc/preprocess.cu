@@ -602,11 +602,12 @@ int PreprocessPlan::launch(const vpb_frame_fmt* frames, int convention, int dtyp
 }
 
 int frame_fmt_check(const vpb_frame_fmt& f, const char* who, int k) {
-  if (f.format < VPB_PIX_PACKED || f.format > VPB_PIX_BAYER_GRBG || f.format == 4) {
-    vpb_set_error("%s: frame %d: unknown format %d (VPB_PIX_PACKED, _NV12, _UYVY, _YUYV, _BGRA, _RGBA or _BAYER_*)", who,
-                  k, f.format);
+  if (f.format < VPB_PIX_PACKED || f.format > VPB_PIX_JPEG || f.format == 4) {
+    vpb_set_error("%s: frame %d: unknown format %d (VPB_PIX_PACKED, _NV12, _UYVY, _YUYV, _BGRA, _RGBA, _BAYER_* or _JPEG)",
+                  who, k, f.format);
     return VPB_ERR_ARG;
   }
+  if (f.format == VPB_PIX_JPEG) return jpeg_frame_check(f, who, k);
   static const char* kName[11] = {"packed", "NV12", "UYVY", "YUYV", nullptr, "BGRA", "RGBA",
                                   "Bayer RGGB", "Bayer BGGR", "Bayer GBRG", "Bayer GRBG"};
   if (f.format == VPB_PIX_PACKED) {             // the messages of vpb_frame
@@ -700,7 +701,8 @@ extern "C" int vpb_preprocess_fmt(const vpb_frame_fmt* frame_dev, int resize_mod
     vpb_set_error("%s: unknown resize mode %d", who, resize_mode);
     return VPB_ERR_ARG;
   }
-  int rc = vpb::frame_fmt_check(*frame_dev, who, 0);
+  int rc = vpb::no_jpeg(frame_dev, 1, who);
+  if (rc == VPB_OK) rc = vpb::frame_fmt_check(*frame_dev, who, 0);
   if (rc) return rc;
   vpb::PreGeom g;
   g.h = frame_dev->h; g.w = frame_dev->w;

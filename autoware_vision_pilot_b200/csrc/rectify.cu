@@ -187,6 +187,7 @@ extern "C" int vpb_rectify_frames(const vpb_frame_fmt* frames_dev, const vpb_rec
   }
   int dev = -1;
   cudaGetDevice(&dev);
+  if (vpb::no_jpeg(frames_dev, n, who)) return VPB_ERR_ARG;
   for (int k = 0; k < n; ++k) {
     const int rc = vpb::frame_fmt_check(frames_dev[k], who, k);
     if (rc) return rc;

@@ -246,7 +246,7 @@ class Engine:
             raise ValueError(f"{len(frames)} frame(s) for an engine of batch {self.batch}")
         arr, keep = (L.FrameFmt * len(frames))(), []
         for k, f in enumerate(frames):
-            d, alive = f.desc(allow_copy) if isinstance(f, L.FRAME_TYPES) else L.packed_desc(self._check_frame(f, allow_copy))
+            d, alive = f.desc(allow_copy) if isinstance(f, L.HOST_FRAME_TYPES) else L.packed_desc(self._check_frame(f, allow_copy))
             arr[k] = d
             keep.append(alive)
         return arr, keep
@@ -257,7 +257,7 @@ class Engine:
         BGRA / RGBA / Bayer object (autoware_vision_pilot_b200._lib), converted inside the pre-process exactly as
         cv2.cvtColor would."""
         frames = list(frames)
-        if not any(isinstance(f, L.FRAME_TYPES) for f in frames):
+        if not any(isinstance(f, L.HOST_FRAME_TYPES) for f in frames):
             frames = self._check_frames(frames, allow_copy=True)
             L.check(self._lib.vp_engine_infer_frames(self._h, self._descs(frames), len(frames)), "vp_engine_infer_frames")
             return
@@ -267,7 +267,7 @@ class Engine:
     def submit_frames(self, frames) -> None:
         """Asynchronous infer_frames() (pinned frames: pinned_frames(shapes)); sync() completes it."""
         frames = list(frames)
-        if not any(isinstance(f, L.FRAME_TYPES) for f in frames):
+        if not any(isinstance(f, L.HOST_FRAME_TYPES) for f in frames):
             frames = self._check_frames(frames, allow_copy=False)
             L.check(self._lib.vp_engine_submit_frames(self._h, self._descs(frames), len(frames)), "vp_engine_submit_frames")
             return

@@ -149,7 +149,12 @@ int vp_engine_infer_device_frames(vp_engine* e, const vpb_frame* frames_dev, int
  * other format returns VPB_ERR_ARG before any device work, unless the sample is rectified (vp_engine_set_rectify: the
  * overlay blends the packed rectified frame).  The
  * frame graph's key adds each frame's format and uv_stride: new data / uv pointers re-point the captured nodes, a new
- * format captures again.  The split-fp16 mode takes them with n = 1. */
+ * format captures again.  The split-fp16 mode takes them with n = 1.
+ * The host calls (infer, submit) also take JPEG streams (VPB_PIX_JPEG, vp_b200_ops.h), mixed with the rest: the call
+ * parses each stream's headers on the host (VPB_ERR_ARG, naming the frame and the reason, for a stream it does not
+ * take), uploads the entropy-coded data and decodes it on the device, byte-equal to cv::imdecode, ahead of rectify and
+ * the pre-process; an overlay engine takes a JPEG frame (it blends the decoded frame).  A call with a JPEG frame
+ * re-points the captured graph instead of capturing again.  The device call rejects VPB_PIX_JPEG. */
 int vp_engine_infer_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n);
 int vp_engine_submit_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n);
 int vp_engine_infer_device_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_dev, int n);

@@ -65,7 +65,9 @@ int vp_autospeed_infer_device_frames(vp_autospeed* e, const vpb_frame* frames_de
  * RGBA or a raw Bayer mosaic, mixed in one call).  They replace the caller's cv::cvtColor(frame, COLOR_YUV2RGB_* /
  * COLOR_BGRA2RGB / COLOR_Bayer**2RGB) before the call: the letterbox converts each pixel as it reads it, and the raw
  * tensor, candidates and detections are byte-equal to the packed call on the converted frame.  Checks as for the
- * *_frames calls plus those of vpb_preprocess_fmt. */
+ * *_frames calls plus those of vpb_preprocess_fmt.  The host call also takes JPEG streams (VPB_PIX_JPEG), decoded on the
+ * device to R, G, B byte-equal to cv::imdecode(buf, IMREAD_COLOR_RGB | IMREAD_IGNORE_ORIENTATION); the device call
+ * rejects them. */
 int vp_autospeed_infer_frames_fmt(vp_autospeed* e, const vpb_frame_fmt* frames_host, int n, int fetch_raw);
 int vp_autospeed_infer_device_frames_fmt(vp_autospeed* e, const vpb_frame_fmt* frames_dev, int n);
 /* Lens rectification of sample `sample` in every later call, as vp_engine_set_rectify (vp_b200.h): the letterbox reads

@@ -66,17 +66,32 @@ typedef struct { const uint8_t* data; int h, w, stride; } vpb_frame;
  *         G = (4 neighbours + 2) >> 2 and the other colour = (4 diagonals + 2) >> 2, at a G site each other colour is
  *         the rounded mean of its two neighbours; the border pixels repeat the nearest interior pixel (clamp x to
  *         [1, w-2], y to [1, h-2]), reading only the crop itself.  h, w >= 3 (cv::cvtColor returns zeros below).
+ *   JPEG  data = a JFIF / MJPEG byte stream (ROS sensor_msgs/CompressedImage "jpeg", UVC MJPEG), stride = its length in
+ *         bytes, h and w = the image size of its SOF header (vpb_jpeg_info reads them), uv NULL.  Taken by the host
+ *         calls only (vp_engine_infer_frames_fmt, vp_engine_submit_frames_fmt, vp_autospeed_infer_frames_fmt; under
+ *         submit the caller keeps the bytes alive until sync); every device call rejects it.  Decoded on the device
+ *         byte-equal to cv::imdecode(buf, IMREAD_COLOR | IMREAD_IGNORE_ORIENTATION) (libjpeg-turbo: ISLOW IDCT, fancy
+ *         upsampling), to R, G, B for VPB_CONV_RGB / _RGB_UNIT and B, G, R for the BGR conventions.  Streams taken:
+ *         baseline or extended sequential (SOF0 / SOF1) Huffman, 8-bit, one interleaved scan of 3 YCbCr components
+ *         (JFIF, or Adobe transform 1), luma sampling 1x1, 2x1 or 2x2 over 1x1 chroma (4:4:4, 4:2:2, 4:2:0), optional
+ *         DRI / RSTn, missing Huffman tables replaced by the Annex K ones (MJPEG), APPn (EXIF orientation too) ignored,
+ *         at most 4800x2400.  Anything else (progressive, lossless, arithmetic, 12-bit, multi-scan, 1 or 4 components,
+ *         Adobe RGB / YCCK, other sampling, a missing SOI / SOF / SOS or a segment past `stride`, an h x w other than the
+ *         SOF's) is VPB_ERR_ARG before any device work, naming the call, the frame and the reason: cv::imdecode and the
+ *         packed call are the fall-back.  Corrupt entropy-coded data decodes to unspecified pixels of that frame only.
  * Value 4 is unassigned: it was rejected as an unknown format before the 4-channel and Bayer layouts existed, and it
  * still is (the new values start at 5). */
 enum { VPB_PIX_PACKED = 0, /* a vpb_frame: 3 interleaved channels, RGB or BGR as the convention says */
        VPB_PIX_NV12 = 1, VPB_PIX_UYVY = 2, VPB_PIX_YUYV = 3,
        VPB_PIX_BGRA = 5, VPB_PIX_RGBA = 6,
-       VPB_PIX_BAYER_RGGB = 7, VPB_PIX_BAYER_BGGR = 8, VPB_PIX_BAYER_GBRG = 9, VPB_PIX_BAYER_GRBG = 10 };
+       VPB_PIX_BAYER_RGGB = 7, VPB_PIX_BAYER_BGGR = 8, VPB_PIX_BAYER_GBRG = 9, VPB_PIX_BAYER_GRBG = 10,
+       VPB_PIX_JPEG = 11 };
 typedef struct {
   int format;                 /* VPB_PIX_* */
-  const uint8_t* data;        /* PACKED / UYVY / YUYV / BGRA / RGBA / BAYER_*: the frame; NV12: the Y plane [h][stride] */
+  const uint8_t* data;        /* PACKED / UYVY / YUYV / BGRA / RGBA / BAYER_*: the frame; NV12: the Y plane [h][stride];
+                                 JPEG: the byte stream (host memory) */
   int h, w, stride;           /* bytes per row of data: >= 3w (PACKED), >= 2w (UYVY, YUYV), >= 4w (BGRA, RGBA),
-                                 >= w (NV12, BAYER_*) */
+                                 >= w (NV12, BAYER_*); JPEG: the stream's length in bytes */
   const uint8_t* uv;          /* NV12: the interleaved U,V plane [h/2][uv_stride]; ignored otherwise */
   int uv_stride;              /* NV12: >= w */
 } vpb_frame_fmt;
@@ -252,6 +267,27 @@ void vpb_rectify_destroy(vpb_rectify* r);
  * current one. */
 int  vpb_rectify_frames(const vpb_frame_fmt* frames_dev, const vpb_rectify* const* rect, int n, int bgr,
                         uint8_t* const* out, void* stream);
+/* ---- JPEG frames (VPB_PIX_JPEG) ----
+ * Host-only header parse of a JPEG stream of `bytes` bytes: its SOF size and sampling (VPB_JPEG_444 / _422 / _420),
+ * the values a VPB_PIX_JPEG descriptor needs (sensor_msgs/CompressedImage carries no size).  VPB_ERR_ARG, the message
+ * giving the reason, for a stream the decoder does not take (see VPB_PIX_JPEG).  Opens no device. */
+enum { VPB_JPEG_444 = 0, VPB_JPEG_422 = 1, VPB_JPEG_420 = 2 };
+int vpb_jpeg_info(const uint8_t* data, size_t bytes, int* h, int* w, int* sampling);
+/* Op level: a decoder on device gpu_id for up to max_n frames of up to max_h x max_w per call (at most 4800x2400 and
+ * VP_MAX_BATCH), owning its scratch: the coefficients and planes of a full call at capacity, allocated here, and the
+ * staging of the streams (pinned and device), grown with them.  VPB_ERR_ARG before the device is opened for a capacity
+ * outside those limits. */
+typedef struct vpb_jpeg_decoder vpb_jpeg_decoder;
+int  vpb_jpeg_decoder_create(int max_h, int max_w, int max_n, int gpu_id, vpb_jpeg_decoder** out);
+void vpb_jpeg_decoder_destroy(vpb_jpeg_decoder* d);
+/* n host VPB_PIX_JPEG descriptors decoded into out_dev[k], packed [h_k][3 w_k] (device), B, G, R for bgr != 0 and
+ * R, G, B otherwise, in three launches on `stream` (jpeg_huffman_kernel, jpeg_idct_kernel, jpeg_color_kernel), equal to
+ * cv::imdecode byte for byte.  Returns once the streams are staged (the call's host work: header parse, tables and
+ * destuffing into pinned memory) and the upload and kernels are enqueued; the caller's bytes are not read afterwards.
+ * VPB_ERR_ARG before any device work for n outside 1..max_n, a NULL output, a descriptor that is not a JPEG frame the
+ * decoder takes, a frame above the capacity, or a current device other than the decoder's. */
+int  vpb_jpeg_decode(vpb_jpeg_decoder* d, const vpb_frame_fmt* frames_host, int n, int bgr, uint8_t* const* out_dev,
+                     void* stream);
 /* Host-only: the integer coefficient tables the kernel uses (bounds[out_size],
  * coeffs[out_size*ksize]); lets a CPU test pin them against Pillow / OpenCV without a GPU. */
 int vpb_resize_tables_host(int mode, int in_size, int out_size, int* bounds, int* coeffs,

@@ -529,16 +529,15 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
   return VPB_OK;
 }
 
-// The source-output jobs of the call's frames: sample k's buffers grown to its frame (outside any capture; a grown
-// buffer drops the captured graph, whose node holds the old pointer), destinations, sizes and frame pointers.
+// The source-output jobs of the call's frames: sample k's buffers grown to its frame (outside any capture),
+// destinations, sizes and frame pointers.
 static int prepare_source(vp_engine& e) {
   for (auto& so : e.src_outs) {
-    const vpb_frame_fmt& fr = e.frames[so.sample];   // packed when a job is an overlay (vp_engine::geoms)
+    const vpb_frame_fmt fr = e.chain[so.sample].pre();   // packed when a job is an overlay (vp_engine::geoms)
     vpb_src_job& j = so.job;
     const int el = j.kind == VPB_SRC_DEPTH ? 4 : j.kind == VPB_SRC_OVERLAY ? 3 : 1;
     const size_t bytes = static_cast<size_t>(fr.h) * fr.w * el;
     if (bytes > so.cap) {
-      e.frame_graph.invalidate();
       void* d = nullptr; void* h = nullptr;
       VPB_CUDA_OK(cudaMalloc(&d, bytes));
       e.dev_allocs.push_back(d);
@@ -587,10 +586,9 @@ static int build_source_outputs(vp_engine& e) {
   if (rc) return rc;
   vp_engine* ep = &e;
   e.cur_lane = -1;
-  e.add_op("source_outputs", "source_outputs_kernel",
-           [ep](cudaStream_t st) { return source_outputs_x(ep->src_jobs.data(), static_cast<int>(ep->src_jobs.size()), st); });
-  e.ops.back().repoint = [ep](cudaGraphExec_t x, cudaGraphNode_t node) {
-    return source_outputs_update_node(x, node, ep->src_jobs.data(), static_cast<int>(ep->src_jobs.size()));
+  e.add_op("source_outputs", "source_outputs_kernel", nullptr);
+  e.ops.back().describe = [ep](KernelCall& c) {
+    return source_outputs_call(ep->src_jobs.data(), static_cast<int>(ep->src_jobs.size()), c);
   };
   return VPB_OK;
 }
@@ -910,7 +908,7 @@ extern "C" int vp_engine_conv_args(vp_engine* e, int op, vpb_conv_args* out, con
 extern "C" int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flops, int* launches) {
   if (!e || !ms || reps <= 0) return VPB_ERR_ARG;
   if (!e->n_frames) { vpb_set_error("vp_engine_time_kind: run one inference first"); return VPB_ERR_STATE; }
-  return e->time_ops(e->ops, [&](const OpRec& op) { return op.gemm && op.kind == kind; }, reps, ms, flops, nullptr, launches);
+  return e->time_ops([&](const OpRec& op) { return op.gemm && op.kind == kind; }, reps, ms, flops, nullptr, launches);
 }
 
 extern "C" int vp_engine_read_resized(vp_engine* e, uint8_t* dst) { return vp_engine_read_resized_at(e, 0, dst); }
@@ -959,5 +957,5 @@ extern "C" int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, 
                                      double* bytes, int* launches) {
   if (!e || !kname || !ms || reps <= 0) return VPB_ERR_ARG;
   if (!e->n_frames) { vpb_set_error("vp_engine_time_kernel: run one inference first"); return VPB_ERR_STATE; }
-  return e->time_ops(e->ops, [&](const OpRec& op) { return op.kname == kname; }, reps, ms, flops, bytes, launches);
+  return e->time_ops([&](const OpRec& op) { return op.kname == kname; }, reps, ms, flops, bytes, launches);
 }

@@ -112,23 +112,18 @@ static bool same_geometry(const vpb_frame_fmt& a, const vpb_frame_fmt& b) {
 
 int FrameGraph::run(EngineRuntime& e) {
   const cudaStream_t st = e.stream;
-  bool same_geom = exec && n == e.n_frames, same_src = n == e.n_frames;
-  for (int k = 0; k < e.n_frames && same_geom; ++k) same_geom = same_geometry(frames[k], e.frames[k]);
-  for (int k = 0; k < e.n_frames && same_src; ++k) same_src = frames[k].data == e.frames[k].data && frames[k].uv == e.frames[k].uv;
-  for (int k = 0; k < e.n_frames && same_src; ++k)
-    same_src = rect[k] == e.rect[k] && (!rect[k] || (same_geometry(in_frames[k], e.in_frames[k]) &&
-                                                     in_frames[k].data == e.in_frames[k].data &&
-                                                     in_frames[k].uv == e.in_frames[k].uv));
-  if (e.n_jpeg) same_src = false;
-  if (same_geom && !same_src) {
-    for (const auto& [i, node] : nodes) {
-      const int rc = e.ops[i].repoint(exec, node);
+  bool same_geom = exec && n == e.n_frames;
+  for (int k = 0; k < e.n_frames && same_geom; ++k) same_geom = same_geometry(geom[k], e.chain[k].pre());
+  if (same_geom) {
+    KernelCall c;
+    for (Node& r : nodes) {
+      const int rc = e.ops[r.op].describe(c);
       if (rc) return rc;
+      if (c == r.call) continue;
+      VPB_CUDA_OK(c.set(exec, r.node));
+      std::swap(r.call, c);
     }
-    frames = e.frames; in_frames = e.in_frames; rect = e.rect;
-    same_src = true;
-  }
-  if (!same_geom || !same_src) {
+  } else {
     invalidate();
     nodes.clear();
     n = 0;
@@ -147,7 +142,8 @@ int FrameGraph::run(EngineRuntime& e) {
     if (graph) cudaGraphDestroy(graph);
     graph = g;
     if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    frames = e.frames; in_frames = e.in_frames; rect = e.rect; n = e.n_frames;
+    for (int k = 0; k < e.n_frames; ++k) geom[k] = e.chain[k].pre();
+    n = e.n_frames;
   }
   VPB_CUDA_OK(cudaGraphLaunch(exec, st));
   return VPB_OK;
@@ -267,18 +263,29 @@ void EngineRuntime::add_op(const std::string& name, const char* kname, std::func
 void EngineRuntime::add_preprocess(int convention, void* out, uint8_t* out_u8) {
   cur_lane = 0;
   rect_bgr = (convention == VPB_CONV_BGR_NOSWAP || convention == VPB_CONV_BGR_SWAP) ? 1 : 0;
-  add_op("preprocess", "preprocess", [this, convention, out, out_u8](cudaStream_t st) {
-    return pre.launch(frames.data(), convention, dtype, out, out_u8, st);
-  });
-  ops.back().repoint = [this, convention, out, out_u8](cudaGraphExec_t x, cudaGraphNode_t node) {
-    return pre.update_graph_node(x, node, frames.data(), convention, dtype, out, out_u8);
+  add_op("preprocess", "preprocess", nullptr);
+  ops.back().describe = [this, convention, out, out_u8](KernelCall& c) {
+    Frames f{};
+    for (int k = 0; k < batch; ++k) f[k] = chain[k].pre();
+    return pre.describe(f.data(), convention, dtype, out, out_u8, c);
   };
 }
 
-int EngineRuntime::rect_list(vpb_frame_fmt* f, const vpb_rectify** r, uint8_t** out) const {
+vpb_frame_fmt SampleFrames::decoded() const {
+  return given.format == VPB_PIX_JPEG ? packed_frame(vpb_frame{jpg.p, given.h, given.w, 3 * given.w}) : given;
+}
+
+vpb_frame_fmt SampleFrames::pre() const {
+  return map ? packed_frame(vpb_frame{rect.p, map->map_h, map->map_w, 3 * map->map_w}) : decoded();
+}
+
+// the samples of e with a map, in sample order: the frames the rectify op reads, their maps and outputs; the count
+static int rect_list(const EngineRuntime& e, vpb_frame_fmt* f, const vpb_rectify** r, uint8_t** out) {
   int m = 0;
-  for (int k = 0; k < batch; ++k)
-    if (rect[k]) { f[m] = in_frames[k]; r[m] = rect[k]; out[m] = d_rect[k]; ++m; }
+  for (int k = 0; k < e.batch; ++k) {
+    const SampleFrames& s = e.chain[k];
+    if (s.map) { f[m] = s.decoded(); r[m] = s.map; out[m] = s.rect.p; ++m; }
+  }
   return m;
 }
 
@@ -304,20 +311,56 @@ void EngineRuntime::erase_ops(size_t at, size_t m) {
   for (int& d : lane_dep) d -= static_cast<int>(m);
 }
 
-void EngineRuntime::sync_jpeg_ops() {
-  static const char* kOps[3][2] = {{"jpeg_huffman", "jpeg_huffman_kernel"}, {"jpeg_idct", "jpeg_idct_kernel"},
-                                   {"jpeg_color", "jpeg_color_kernel"}};
-  const bool have = op_index(kOps[0][0]) >= 0;
-  if (have == (n_jpeg > 0)) return;
-  if (have) { erase_ops(0, 3); return; }
-  std::vector<OpRec> add(3);
-  for (int k = 0; k < 3; ++k) {
-    OpRec& op = add[k];
-    op.name = kOps[k][0]; op.kname = kOps[k][1]; op.lane = 0;
-    op.launch = [this, k](cudaStream_t st) { return jpeg->launch(k, st); };
-    op.repoint = [this, k](cudaGraphExec_t x, cudaGraphNode_t node) { return jpeg->update_node(k, x, node); };
+void EngineRuntime::sync_front_ops() {
+  static const char* kJpeg[3][2] = {{"jpeg_huffman", "jpeg_huffman_kernel"}, {"jpeg_idct", "jpeg_idct_kernel"},
+                                    {"jpeg_color", "jpeg_color_kernel"}};
+  bool jpg = false, rect = false;
+  for (int k = 0; k < batch; ++k) {
+    jpg |= chain[k].given.format == VPB_PIX_JPEG;
+    rect |= chain[k].map != nullptr;
   }
-  insert_ops(0, std::move(add));
+  if (jpg != (op_index(kJpeg[0][0]) >= 0)) {
+    if (jpg) {
+      std::vector<OpRec> add(3);
+      for (int k = 0; k < 3; ++k) {
+        add[k].name = kJpeg[k][0]; add[k].kname = kJpeg[k][1]; add[k].lane = 0;
+        add[k].describe = [this, k](KernelCall& c) { jpeg->describe(k, c); return VPB_OK; };
+      }
+      insert_ops(0, std::move(add));
+    } else {
+      erase_ops(0, 3);
+    }
+  }
+  if (rect != (op_index("rectify") >= 0)) {
+    if (rect) {
+      std::vector<OpRec> add(1);
+      add[0].name = "rectify"; add[0].kname = "rectify_kernel"; add[0].lane = 0;
+      add[0].describe = [this](KernelCall& c) {
+        vpb_frame_fmt f[kMaxBatch]; const vpb_rectify* m[kMaxBatch]; uint8_t* o[kMaxBatch];
+        rectify_call(f, m, rect_list(*this, f, m, o), rect_bgr, o, c);
+        return VPB_OK;
+      };
+      insert_ops(op_index("preprocess"), std::move(add));    // after the JPEG decode: rectify reads the decoded frame
+    } else {
+      erase_ops(op_index("rectify"), 1);
+    }
+  }
+  if (jpg)
+    for (int k = 0; k < 3; ++k) ops[k].bytes = jpeg->bytes(k);
+  if (rect) {
+    vpb_frame_fmt f[kMaxBatch]; const vpb_rectify* m[kMaxBatch]; uint8_t* o[kMaxBatch];
+    const int n = rect_list(*this, f, m, o);
+    ops[op_index("rectify")].bytes = rectify_bytes(f, m, n);
+  }
+}
+
+int EngineRuntime::grow(Scratch& s, size_t bytes) {
+  if (bytes <= s.cap) return VPB_OK;
+  void* p = nullptr;
+  VPB_CUDA_OK(cudaMalloc(&p, bytes));
+  dev_allocs.push_back(p);
+  s.p = static_cast<uint8_t*>(p); s.cap = bytes;
+  return VPB_OK;
 }
 
 int EngineRuntime::set_rectify(int sample, const vpb_rectify* r, const char* who) {
@@ -326,38 +369,20 @@ int EngineRuntime::set_rectify(int sample, const vpb_rectify* r, const char* who
     vpb_set_error("%s: sample %d: the map lives on GPU %d, the engine on GPU %d", who, sample, r->gpu_id, gpu_id);
     return VPB_ERR_ARG;
   }
-  if ((rect[sample] != nullptr) != (r != nullptr)) frame_graph.invalidate();   // the rectify launch gains or loses a frame
-  rect[sample] = r;
+  chain[sample].map = r;
   n_frames = 0;                           // the last call's frames are not those the op list now reads
-  bool any = false;
-  for (int k = 0; k < batch; ++k) any |= rect[k] != nullptr;
-  if (any == rect_op()) return VPB_OK;
-  if (any) {
-    OpRec op;
-    op.name = "rectify"; op.kname = "rectify_kernel"; op.lane = 0;
-    op.launch = [this](cudaStream_t st) {
-      vpb_frame_fmt f[kMaxBatch]; const vpb_rectify* m[kMaxBatch]; uint8_t* o[kMaxBatch];
-      const int n = rect_list(f, m, o);
-      return rectify_x(f, m, n, rect_bgr, o, st);
-    };
-    op.repoint = [this](cudaGraphExec_t x, cudaGraphNode_t node) {
-      vpb_frame_fmt f[kMaxBatch]; const vpb_rectify* m[kMaxBatch]; uint8_t* o[kMaxBatch];
-      const int n = rect_list(f, m, o);
-      return rectify_update_node(x, node, f, m, n, rect_bgr, o);
-    };
-    std::vector<OpRec> add;
-    add.push_back(std::move(op));
-    insert_ops(op_index("preprocess"), std::move(add));      // after the JPEG decode: rectify reads the decoded frame
-  } else {
-    erase_ops(op_index("rectify"), 1);
-  }
+  sync_front_ops();
   return VPB_OK;
 }
 
 int EngineRuntime::launch_op(size_t i, cudaStream_t st) {
   const OpRec& op = ops[i];
-  const int rc = op.launch(st);
-  if (rc || !frame_graph.capturing || !op.repoint) return rc;
+  if (!op.describe) return op.launch(st);
+  KernelCall c;
+  const int rc = op.describe(c);
+  if (rc) return rc;
+  VPB_CUDA_OK(c.launch(st));
+  if (!frame_graph.capturing) return VPB_OK;
   // the op's launch is now the stream's only dependency; the edge data of the programmatic (PDL) edges is asked for
   // too, or the query would fail as lossy
   cudaStreamCaptureStatus cs;
@@ -371,7 +396,7 @@ int EngineRuntime::launch_op(size_t i, cudaStream_t st) {
     vpb_set_error("graph capture: op '%s' did not capture as one kernel node (%zu dependencies)", op.name.c_str(), nd);
     return VPB_ERR_CUDA;
   }
-  frame_graph.nodes.emplace_back(i, deps[0]);
+  frame_graph.nodes.push_back(FrameGraph::Node{i, deps[0], std::move(c)});
   return VPB_OK;
 }
 
@@ -484,28 +509,21 @@ bool frames_ok(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const
   return true;
 }
 
-// The frames the pre-process sees: a rectified sample's frame must have its map's source size (VPB_ERR_ARG naming who
-// and the frame otherwise) and becomes a packed descriptor of the map's size at d_rect[k], and any other JPEG sample a
-// packed descriptor of its size at d_jpg[k] (NULL until the first call grows them: host-only checks read the geometry
-// alone).
-static bool rect_frames(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who, Frames& out) {
-  out = {};
-  std::copy(frames, frames + n, out.begin());
+// Host-only checks of the call's frames: a sample with a map needs a frame of the map's source size (VPB_ERR_ARG naming
+// who and the frame otherwise); then the engine's geometries g of what the pre-process will read.
+static int pre_geoms(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who, PreGeom* g) {
+  Frames pre{};
   for (int k = 0; k < n; ++k) {
-    const vpb_rectify* r = e->rect[k];
-    if (!r) {
-      if (frames[k].format == VPB_PIX_JPEG)
-        out[k] = packed_frame(vpb_frame{e->d_jpg[k], frames[k].h, frames[k].w, 3 * frames[k].w});
-      continue;
-    }
-    if (frames[k].h != r->src_h || frames[k].w != r->src_w) {
+    SampleFrames s;
+    s.given = frames[k]; s.map = e->chain[k].map;
+    if (s.map && (frames[k].h != s.map->src_h || frames[k].w != s.map->src_w)) {
       vpb_set_error("%s: frame %d is %dx%d; the map set for sample %d rectifies %dx%d frames", who, k, frames[k].w,
-                    frames[k].h, k, r->src_w, r->src_h);
-      return false;
+                    frames[k].h, k, s.map->src_w, s.map->src_h);
+      return VPB_ERR_ARG;
     }
-    out[k] = packed_frame(vpb_frame{e->d_rect[k], r->map_h, r->map_w, 3 * r->map_w});
+    pre[k] = s.pre();
   }
-  return true;
+  return e->geoms(pre.data(), who, g);
 }
 
 // vpb_frame descriptors as VPB_PIX_PACKED ones (the first kMaxBatch; frames_ok rejects a count other than the batch)
@@ -524,42 +542,24 @@ bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int
   return frames_ok(e, out.data(), n, who);
 }
 
-// The device frames f of geometries g (a rectified sample's: its map's size) become the runtime's frames, and the
+// The call on the runtime's frames chain[0 .. n-1].given, whose pre-process geometries are g.  A rectified sample's
+// scratch buffer is grown here, outside any capture; the front ops follow the frames and maps (sync_front_ops), and the
 // pre-process op gets the algorithmic bytes of the call (SURVEY.md 8d: frame read + 3 x OH x OW 16-bit written, per
-// sample; frame_bytes).  A rectified sample's scratch buffer is grown here, outside any capture (a grown buffer drops
-// the captured graph), and the rectify op gets its bytes.  The JPEG decode ops are there exactly when the call has a
-// JPEG frame, with the bytes of the call's streams.  A failed call leaves no frames, so nothing launches the
-// pre-process on frames its tables were not built for.
-static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeom* g) {
-  e->in_frames = f;
-  Frames s = f;
+// sample; frame_bytes).  A failed call leaves no frames, so nothing launches the pre-process on frames its tables were
+// not built for.
+static int enqueue_frames(EngineRuntime* e, int n, const PreGeom* g) {
+  e->n_frames = 0;
   for (int k = 0; k < n; ++k) {
-    const vpb_rectify* r = e->rect[k];
+    const vpb_rectify* r = e->chain[k].map;
     if (!r) continue;
-    const size_t bytes = static_cast<size_t>(r->map_h) * r->map_w * 3;
-    if (bytes > e->d_rect_cap[k]) {
-      e->frame_graph.invalidate();
-      void* p = nullptr;
-      VPB_CUDA_OK(cudaMalloc(&p, bytes));
-      e->dev_allocs.push_back(p);
-      e->d_rect[k] = static_cast<uint8_t*>(p); e->d_rect_cap[k] = bytes;
-    }
-    s[k] = packed_frame(vpb_frame{e->d_rect[k], r->map_h, r->map_w, 3 * r->map_w});
+    const int rc = e->grow(e->chain[k].rect, static_cast<size_t>(r->map_h) * r->map_w * 3);
+    if (rc) return rc;
   }
-  e->frames = s;
   e->n_frames = n;
-  e->sync_jpeg_ops();
-  if (e->n_jpeg)
-    for (int k = 0; k < 3; ++k) e->ops[k].bytes = e->jpeg->bytes(k);
+  e->sync_front_ops();
   double bytes = 0;
-  for (int k = 0; k < n; ++k) bytes += frame_bytes(s[k]) + 2.0 * 3 * g[k].OH * g[k].OW;
+  for (int k = 0; k < n; ++k) bytes += frame_bytes(e->chain[k].pre()) + 2.0 * 3 * g[k].OH * g[k].OW;
   e->ops[e->op_index("preprocess")].bytes = bytes;
-  const int ri = e->op_index("rectify");
-  if (ri >= 0) {
-    vpb_frame_fmt rf[kMaxBatch]; const vpb_rectify* rm[kMaxBatch]; uint8_t* ro[kMaxBatch];
-    const int m = e->rect_list(rf, rm, ro);
-    e->ops[ri].bytes = rectify_bytes(rf, rm, m);
-  }
   const int rc = e->enqueue(g);
   if (rc) e->n_frames = 0;
   return rc;
@@ -567,15 +567,12 @@ static int enqueue_frames(EngineRuntime* e, const Frames& f, int n, const PreGeo
 
 int call_host(EngineRuntime* e, const vpb_frame_fmt* frames, int n, bool sync, bool raw, const char* who) {
   if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
-  Frames sub;
-  if (!rect_frames(e, frames, n, who, sub)) return VPB_ERR_ARG;
   PreGeom g[kMaxBatch];
-  if (e->geoms(sub.data(), who, g)) return VPB_ERR_ARG;
+  if (pre_geoms(e, frames, n, who, g)) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  Frames dev;
-  int rc = e->upload_frames(frames, n, dev);
+  int rc = e->upload_frames(frames, n);
   if (rc) return rc;
-  rc = enqueue_frames(e, dev, n, g);
+  rc = enqueue_frames(e, n, g);
   if (rc) return rc;
   rc = e->fetch(raw);
   if (rc) return rc;
@@ -586,15 +583,11 @@ int call_host(EngineRuntime* e, const vpb_frame_fmt* frames, int n, bool sync, b
 int call_device(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who) {
   if (no_jpeg(frames, n, who)) return VPB_ERR_ARG;
   if (!frames_ok(e, frames, n, who)) return VPB_ERR_ARG;
-  Frames sub;
-  if (!rect_frames(e, frames, n, who, sub)) return VPB_ERR_ARG;
   PreGeom g[kMaxBatch];
-  if (e->geoms(sub.data(), who, g)) return VPB_ERR_ARG;
-  Frames f{};
-  std::copy(frames, frames + n, f.begin());
+  if (pre_geoms(e, frames, n, who, g)) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  e->n_jpeg = 0;
-  return enqueue_frames(e, f, n, g);
+  for (int k = 0; k < n; ++k) e->chain[k].given = frames[k];
+  return enqueue_frames(e, n, g);
 }
 
 int call_host(EngineRuntime* e, const vpb_frame* frames, int n, bool sync, bool raw, const char* who) {
@@ -616,56 +609,45 @@ static int upload_plane(uint8_t* d, const uint8_t* s, int spitch, int row, int r
   return VPB_OK;
 }
 
-int EngineRuntime::upload_frames(const vpb_frame_fmt* frames, int n, Frames& dev) {
+int EngineRuntime::upload_frames(const vpb_frame_fmt* frames, int n) {
+  n_frames = 0;                           // chain[].given is rewritten: no call's frames until the enqueue
   size_t total = 0;
   for (int k = 0; k < n; ++k) {
     const vpb_frame_fmt& f = frames[k];
     if (f.format == VPB_PIX_JPEG) continue;
     total += static_cast<size_t>(f.h) * frame_row_bytes(f) + (f.format == VPB_PIX_NV12 ? static_cast<size_t>(f.h / 2) * f.w : 0);
   }
-  if (total > d_frame_cap) {
-    frame_graph.invalidate();
-    void* p = nullptr;
-    VPB_CUDA_OK(cudaMalloc(&p, total + 256));
-    dev_allocs.push_back(p);
-    d_frame = static_cast<uint8_t*>(p); d_frame_cap = total;
-  }
-  dev = {};
-  n_jpeg = 0;
+  int rc = grow(upload, total + 256);
+  if (rc) return rc;
   const vpb_frame_fmt* jf[kMaxBatch];
   uint8_t* jo[kMaxBatch];
+  int nj = 0;
   for (int k = 0; k < n; ++k) {
     const vpb_frame_fmt& f = frames[k];
+    chain[k].given = f;
     if (f.format != VPB_PIX_JPEG) continue;
-    const size_t bytes = static_cast<size_t>(f.h) * f.w * 3;
-    if (bytes > d_jpg_cap[k]) {
-      void* p = nullptr;
-      VPB_CUDA_OK(cudaMalloc(&p, bytes));
-      dev_allocs.push_back(p);
-      d_jpg[k] = static_cast<uint8_t*>(p); d_jpg_cap[k] = bytes;
-    }
-    dev[k] = packed_frame(vpb_frame{d_jpg[k], f.h, f.w, 3 * f.w});
-    jf[n_jpeg] = &f; jo[n_jpeg] = d_jpg[k]; ++n_jpeg;
+    rc = grow(chain[k].jpg, static_cast<size_t>(f.h) * f.w * 3);
+    if (rc) return rc;
+    jf[nj] = &f; jo[nj] = chain[k].jpg.p; ++nj;
   }
-  if (n_jpeg) {
+  if (nj) {
     if (!jpeg) jpeg = std::make_unique<JpegDecoder>();
-    const int rc = jpeg->stage(jf, n_jpeg, jo, rect_bgr, stream);
-    if (rc) { n_jpeg = 0; return rc; }
+    rc = jpeg->stage(jf, nj, jo, rect_bgr, stream);
+    if (rc) return rc;
   }
   size_t off = 0;
   for (int k = 0; k < n; ++k) {
     const vpb_frame_fmt& f = frames[k];
     if (f.format == VPB_PIX_JPEG) continue;
     const int dpitch = frame_row_bytes(f);
-    uint8_t* d = d_frame + off;
-    dev[k] = f;
-    dev[k].data = d; dev[k].stride = dpitch;
-    int rc = upload_plane(d, f.data, f.stride, dpitch, f.h, stream);
+    vpb_frame_fmt& dev = chain[k].given;
+    dev.data = upload.p + off; dev.stride = dpitch;
+    rc = upload_plane(upload.p + off, f.data, f.stride, dpitch, f.h, stream);
     if (rc) return rc;
     off += static_cast<size_t>(f.h) * dpitch;
     if (f.format == VPB_PIX_NV12) {
-      dev[k].uv = d_frame + off; dev[k].uv_stride = f.w;
-      rc = upload_plane(d_frame + off, f.uv, f.uv_stride, f.w, f.h / 2, stream);
+      dev.uv = upload.p + off; dev.uv_stride = f.w;
+      rc = upload_plane(upload.p + off, f.uv, f.uv_stride, f.w, f.h / 2, stream);
       if (rc) return rc;
       off += static_cast<size_t>(f.h / 2) * f.w;
     }
@@ -732,8 +714,8 @@ bool EngineRuntime::find_tap(const char* name, Tap* out) const {
   return true;
 }
 
-int EngineRuntime::time_ops(const std::vector<OpRec>& list, const std::function<bool(const OpRec&)>& keep, int reps,
-                            float* ms, double* flops, double* bytes, int* launches) {
+int EngineRuntime::time_ops(const std::function<bool(const OpRec&)>& keep, int reps, float* ms, double* flops,
+                            double* bytes, int* launches) {
   DeviceGuard guard(gpu_id);
   Event a, b;
   VPB_CUDA_OK(make_event(a));
@@ -742,9 +724,10 @@ int EngineRuntime::time_ops(const std::vector<OpRec>& list, const std::function<
   int n = 0;
   for (int r = -1; r < reps; ++r) {            // r = -1: untimed warm-up pass
     if (r == 0) VPB_CUDA_OK(cudaEventRecord(a.get(), stream));
-    for (const auto& op : list) {
+    for (size_t i = 0; i < ops.size(); ++i) {
+      const OpRec& op = ops[i];
       if (!keep(op)) continue;
-      const int rc = op.launch(stream);
+      const int rc = launch_op(i, stream);
       if (rc) return rc;
       if (r >= 0) { fl += op.flops; by += op.bytes; ++n; }
     }

@@ -70,7 +70,10 @@ struct Tap { Tens t; int channels = 0; };
 
 struct OpRec {
   std::string name;
-  std::function<int(cudaStream_t)> launch;
+  std::function<int(cudaStream_t)> launch;   // an op whose arguments are fixed when the list is built
+  // An op that reads the call's frames describes its launch from the current call instead: EngineRuntime::launch_op
+  // launches that description, and the frame graph sets it on the op's captured node where it differs.
+  std::function<int(KernelCall&)> describe;
   double flops = 0;     // 2*MAC this launch executes
   double flops_ref = -1; // 2*MAC of the reference's layers this op stands for (< 0: same as flops)
   double bytes = 0;     // algorithmic HBM bytes per launch (HBM-bound stages; SURVEY.md 8d definitions)
@@ -80,36 +83,48 @@ struct OpRec {
   int lane = 0;   // execution lane (= index of the model that owns the op); lanes run concurrently; -1: after every
                   // lane has joined the engine stream
   int conv = -1;  // index into EngineRuntime::plans / conv_list of a convolution op (append_conv), -1 otherwise
-  // Set on the ops that read the frames of the call: re-point the op's captured kernel node at the current frames.
-  std::function<int(cudaGraphExec_t, cudaGraphNode_t)> repoint;
 };
 
 // The frames of one call: descriptor k is sample k, in its own VPB_PIX_* format (entries past the batch are unused).
 using Frames = std::array<vpb_frame_fmt, kMaxBatch>;
 
 struct EngineRuntime;
-// The CUDA graph of one call of a runtime's launch list, keyed on the n (format, h, w, stride, uv_stride) tuples and the
-// frame pointers (data, uv) the pre-process reads (a rectified or JPEG sample's packed descriptor of its scratch buffer).  Frames of
-// the captured geometries and formats in other buffers only re-point the captured nodes of the ops that have repoint; a
-// new format captures again (it selects another pre-process kernel).  A rectified sample's own frame and map only
-// re-point: one rectify kernel takes every format.  A call with a JPEG frame always re-points: its streams' lengths,
-// tables and launch grids are those of the call.
+// The CUDA graph of one call of a runtime's launch list.  It is captured again when the op list changes (insert_ops,
+// erase_ops, and invalidate for op arguments that are not described) or when the geometry key does: the n (format, h,
+// w, stride, uv_stride) tuples of the frames the pre-process reads.  A new format selects another pre-process kernel;
+// the grids and tables follow the geometries.  Otherwise every described op's launch is rebuilt from the current call
+// and set on its captured node where it differs from the launch the node holds, so the captured kernels read this
+// call's frames, maps, JPEG streams and scratch buffers, whichever of them changed.
 struct FrameGraph {
   cudaGraph_t graph = nullptr;           // kept alive: the recorded nodes are handles into it
   cudaGraphExec_t exec = nullptr;
   bool capturing = false;                // inside run()'s capture: EngineRuntime::launch_op records nodes
-  std::vector<std::pair<size_t, cudaGraphNode_t>> nodes;   // (op index, its captured kernel node) of the ops with repoint
-  int n = 0;                             // the key: frames f[0 .. n-1] of the graph's last launch (0: none)
-  Frames frames{};
-  Frames in_frames{};                    // and of a rectified sample the frame the rectify op read, and its map
-  std::array<const vpb_rectify*, kMaxBatch> rect{};
+  struct Node { size_t op; cudaGraphNode_t node; KernelCall call; };   // a described op, its node, the launch it holds
+  std::vector<Node> nodes;
+  int n = 0;                             // the geometry key: geometries of geom[0 .. n-1] (0: none)
+  Frames geom{};
 
-  // Launch the graph for e's frames on e's stream.  When the key differs in more than the frame pointers: e.launch_all
-  // once outside capture (sets function attributes; its results are correct), capture e.launch_all and instantiate.
-  // When only the pointers differ: e.ops[i].repoint(exec, node) for every recorded node.
+  // Launch the graph for e's frames on e's stream.  When the key differs: e.launch_all once outside capture (sets
+  // function attributes; its results are correct), capture e.launch_all and instantiate.
   int run(EngineRuntime& e);
   void invalidate();                     // the next run() captures again
   void release();
+};
+
+// Device scratch of the front end, grown on demand outside any capture (EngineRuntime::grow)
+struct Scratch { uint8_t* p = nullptr; size_t cap = 0; };
+
+// Sample k's frame chain: the frame as given -> JPEG-decoded -> rectified -> what the pre-process reads.
+struct SampleFrames {
+  vpb_frame_fmt given{};                 // the call's frame (a host call's device copy; a JPEG frame: its host stream,
+                                         // read while the call is staged)
+  const vpb_rectify* map = nullptr;      // set_rectify; NULL: none
+  Scratch jpg, rect;                     // the decoded JPEG frame and the rectified frame, packed
+  // what the rectify op reads: a JPEG frame packed at its SOF size in jpg, any other the frame as given
+  vpb_frame_fmt decoded() const;
+  // what the pre-process (and the letterbox, the source outputs, the resized image) reads: with a map, the rectified
+  // frame packed at the map size in rect; otherwise decoded().  Host-only checks read the geometry alone.
+  vpb_frame_fmt pre() const;
 };
 
 struct ConvPlan;
@@ -138,31 +153,20 @@ struct EngineRuntime {
   size_t weight_bytes = 0, act_bytes = 0;
   std::vector<std::unique_ptr<ConvPlan>> plans;
   std::vector<vpb_conv_args> conv_list;   // [plan] the arguments each plan was built from
-  std::vector<OpRec> ops;                // every launch of a call, in order: the JPEG decode and rectify ops while they
-                                         // are needed, then the pre-process
+  std::vector<OpRec> ops;                // every launch of a call, in order: the front ops while they are needed
+                                         // (sync_front_ops), then the pre-process
   std::map<std::string, Tap> taps;
   PreprocessPlan pre;
-  Frames frames{};                        // device frames of the current / last call
-  int n_frames = 0;                       // frames of that call (0: no call has run, or the last one failed)
   FrameGraph frame_graph;
-  uint8_t* d_frame = nullptr; size_t d_frame_cap = 0;           // device copy of the host frames
-  // Lens rectification: rect[k] the map of sample k (NULL: none).  While a map is set, op 0 is "rectify": it writes
-  // sample k's rectified frame, packed, to d_rect[k] (grown on demand outside capture), and frames[k] describes that
-  // buffer, so the pre-process, the letterbox, the source outputs and the resized image see the rectified frame.
-  // in_frames are the call's device frames as given, which the rectify op reads.
-  std::array<const vpb_rectify*, kMaxBatch> rect{};
-  Frames in_frames{};
-  std::array<uint8_t*, kMaxBatch> d_rect{};
-  std::array<size_t, kMaxBatch> d_rect_cap{};
+  // The frames of the current / last call, sample by sample; n_frames of them (0: no call has run, or the last one
+  // failed).  A sample's JPEG frame is decoded by the ops "jpeg_huffman", "jpeg_idct" and "jpeg_color" from the streams
+  // upload_frames staged in `jpeg`; a sample with a map is rectified by the op "rectify".
+  std::array<SampleFrames, kMaxBatch> chain{};
+  int n_frames = 0;
+  Scratch upload;                         // device copy of a host call's frames
+  std::unique_ptr<JpegDecoder> jpeg;
   int rect_bgr = 0;                       // camera-native and JPEG frames convert to BGR (the BGR conventions of
                                           // add_preprocess)
-  // JPEG frames of host calls: upload_frames stages the call's streams in `jpeg` and gives sample k the packed
-  // descriptor of d_jpg[k] (grown on demand outside capture), which the ops "jpeg_huffman", "jpeg_idct" and
-  // "jpeg_color" (ops 0..2 while the current call has a JPEG frame, n_jpeg > 0) decode into.
-  std::unique_ptr<JpegDecoder> jpeg;
-  std::array<uint8_t*, kMaxBatch> d_jpg{};
-  std::array<size_t, kMaxBatch> d_jpg_cap{};
-  int n_jpeg = 0;
   float* d_tap_scratch = nullptr; size_t tap_scratch_cap = 0;   // read_tap staging (grown on demand)
 
   EngineRuntime() = default;
@@ -188,22 +192,21 @@ struct EngineRuntime {
   // "preprocess" on lane 0; the engines call it before their first op
   void add_preprocess(int convention, void* out, uint8_t* out_u8);
   // Map r (NULL: none) for sample `sample` of every later call: VPB_ERR_ARG (naming who) for a sample out of range or a
-  // map of another GPU.  The first map inserts the op "rectify" at index 0 and clearing the last one removes it (the
-  // lanes' producer indices follow); a sample gaining or losing its map drops the captured graph.
+  // map of another GPU; then sync_front_ops.
   int set_rectify(int sample, const vpb_rectify* r, const char* who);
-  bool rect_op() const { return op_index("rectify") >= 0; }
   int op_index(const char* name) const;   // index of the op of that name, -1 if there is none
   // insert ops at index `at` / erase m ops from `at`: the op events and the lanes' producer indices follow, and the
   // captured graph is dropped
   void insert_ops(size_t at, std::vector<OpRec> add);
   void erase_ops(size_t at, size_t m);
-  // the three JPEG decode ops at the front of the list exactly while the current call has a JPEG frame
-  void sync_jpeg_ops();
-  // the rectified samples of the current call, in sample order: their frames, maps and scratch buffers; the count
-  int rect_list(vpb_frame_fmt* f, const vpb_rectify** r, uint8_t** out) const;
+  // The front ops before "preprocess" exactly while they are needed: the three JPEG decode ops while a sample's frame
+  // is JPEG, then "rectify" while a sample has a map; with their bytes for the current frames.
+  void sync_front_ops();
+  // s grown to `bytes` (outside any capture): the new buffer joins dev_allocs, the old one is kept
+  int grow(Scratch& s, size_t bytes);
   // the ops appended next form `lane`, which starts after ops[dep_op]
   void begin_lane(int lane, int dep_op) { cur_lane = lane; lane_dep.resize(lane + 1); lane_dep[lane] = dep_op; }
-  // launch ops[i] on st; while frame_graph captures, an op with repoint records its kernel node
+  // launch ops[i] on st; while frame_graph captures, a described op records its kernel node and launch
   int launch_op(size_t i, cudaStream_t st);
   int reset_call(cudaStream_t st);        // zero call_zero on st: a memset, not an op
   // One call on st: reset_call; the ops of lanes >= 0 in list order, lane l > 0 on its own stream after waiting for
@@ -223,22 +226,22 @@ struct EngineRuntime {
   // VPB_ERR_ARG, the message prefixed with who, for an op out of range or one that is not a convolution
   int conv_args_of(int op, vpb_conv_args* out, const char** name, const char* who) const;
   void tap(const std::string& name, const Tens& t, int channels = 0) { taps[name] = Tap{t, channels > 0 ? channels : t.C}; }
-  // Copy n host frames to d_frame (grown on demand), plane after plane, frame after frame, each row with the pitch of its
-  // valid bytes (3w packed, 2w UYVY / YUYV, w for the Y and the UV rows of NV12): only those bytes of every row are read
-  // from the caller's buffer, so a cv::Mat ROI / strided view is never read past its last row.  dev[k] describes the
-  // device copy of frame k (its uv inside d_frame for NV12).  JPEG frames are staged in `jpeg` instead (n_jpeg counts
-  // them) and dev[k] is the packed descriptor of d_jpg[k], which the JPEG ops write.
-  int upload_frames(const vpb_frame_fmt* frames, int n, Frames& dev);
+  // Copy n host frames to `upload` (grown on demand), plane after plane, frame after frame, each row with the pitch of
+  // its valid bytes (3w packed, 2w UYVY / YUYV, w for the Y and the UV rows of NV12): only those bytes of every row are
+  // read from the caller's buffer, so a cv::Mat ROI / strided view is never read past its last row.  chain[k].given
+  // describes the device copy of frame k (its uv inside `upload` for NV12).  JPEG frames are staged in `jpeg` instead,
+  // to be decoded into chain[k].jpg (grown on demand), and chain[k].given is the frame as given.
+  int upload_frames(const vpb_frame_fmt* frames, int n);
   // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
   bool find_tap(const char* name, Tap* out) const;
   // tap `name` (find_tap) as fp32 [channels][H][W] into dst (NULL: size query); element count or < 0
   long read_tap(const char* name, float* dst, long cap, int* c, int* h, int* w);
-  // Device time of the ops of `list` keep() selects, launched back to back on the engine stream: one untimed warm-up
-  // pass, then `reps` passes between one event pair, then a synchronise.  flops / bytes / launches (each may be NULL)
-  // are summed over the timed passes.  No reset_call: the SE ops read whatever the accumulators hold, and their cost
-  // does not depend on it.
-  int time_ops(const std::vector<OpRec>& list, const std::function<bool(const OpRec&)>& keep, int reps, float* ms,
-               double* flops, double* bytes, int* launches);
+  // Device time of the ops keep() selects, launched back to back on the engine stream: one untimed warm-up pass, then
+  // `reps` passes between one event pair, then a synchronise.  flops / bytes / launches (each may be NULL) are summed
+  // over the timed passes.  No reset_call: the SE ops read whatever the accumulators hold, and their cost does not
+  // depend on it.
+  int time_ops(const std::function<bool(const OpRec&)>& keep, int reps, float* ms, double* flops, double* bytes,
+               int* launches);
 
   // The engine's steps of a frame call (call_host, call_device).  geoms: host-only checks of the geometries of the
   // `batch` frames (VPB_ERR_ARG naming who and the frame); enqueue: the call on the device frames `frames` of

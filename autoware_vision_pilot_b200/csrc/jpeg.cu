@@ -726,34 +726,12 @@ int JpegDecoder::stage(const vpb_frame_fmt* const* frames, int m, uint8_t* const
   return VPB_OK;
 }
 
-static void* kernel_of(int k) {
-  return k == 0 ? reinterpret_cast<void*>(jpeg_huffman_kernel)
-                : k == 1 ? reinterpret_cast<void*>(jpeg_idct_kernel) : reinterpret_cast<void*>(jpeg_color_kernel);
-}
-static dim3 block_of(int k) {
-  return k == 0 ? dim3(kHuffT) : k == 1 ? dim3(kIdctBlocks * 8) : dim3(kColTX, kColTY);
-}
-
-int JpegDecoder::launch(int k, cudaStream_t st) const {
+void JpegDecoder::describe(int k, KernelCall& c) const {
   switch (k) {
-    case 0: VPB_CUDA_OK(launch_k(jpeg_huffman_kernel, grid[0], block_of(0), 0, st, p)); break;
-    case 1: VPB_CUDA_OK(launch_k(jpeg_idct_kernel, grid[1], block_of(1), 0, st, p)); break;
-    default: VPB_CUDA_OK(launch_k(jpeg_color_kernel, grid[2], block_of(2), 0, st, p)); break;
+    case 0: c.set_kernel(jpeg_huffman_kernel, grid[0], dim3(kHuffT), 0, true, p); break;
+    case 1: c.set_kernel(jpeg_idct_kernel, grid[1], dim3(kIdctBlocks * 8), 0, true, p); break;
+    default: c.set_kernel(jpeg_color_kernel, grid[2], dim3(kColTX, kColTY), 0, true, p); break;
   }
-  return VPB_OK;
-}
-
-int JpegDecoder::update_node(int k, cudaGraphExec_t exec, cudaGraphNode_t node) const {
-  JpegParams q = p;
-  void* args[1] = {&q};
-  cudaKernelNodeParams kp{};
-  kp.func = kernel_of(k);
-  kp.gridDim = grid[k];
-  kp.blockDim = block_of(k);
-  kp.sharedMemBytes = 0;
-  kp.kernelParams = args;
-  VPB_CUDA_OK(cudaGraphExecKernelNodeSetParams(exec, node, &kp));
-  return VPB_OK;
 }
 
 double JpegDecoder::bytes(int k) const {
@@ -844,7 +822,12 @@ extern "C" int vpb_jpeg_decode(vpb_jpeg_decoder* d, const vpb_frame_fmt* frames_
   cudaGetDevice(&dev);
   if (dev != d->gpu_id) { vpb_set_error("%s: the decoder lives on GPU %d, the current device is %d", who, d->gpu_id, dev); return VPB_ERR_ARG; }
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = d->dec.stage(f, n, out_dev, bgr != 0, st);
-  for (int k = 0; k < 3 && rc == VPB_OK; ++k) rc = d->dec.launch(k, st);
-  return rc;
+  const int rc = d->dec.stage(f, n, out_dev, bgr != 0, st);
+  if (rc) return rc;
+  vpb::KernelCall c;
+  for (int k = 0; k < 3; ++k) {
+    d->dec.describe(k, c);
+    VPB_CUDA_OK(c.launch(st));
+  }
+  return VPB_OK;
 }

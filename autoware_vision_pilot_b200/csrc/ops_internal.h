@@ -2,11 +2,72 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <cstring>
 #include <vector>
 #include <mutex>
 #include "../../include/vp_b200_ops.h"
 
 namespace vpb {
+
+// One kernel launch as data: the kernel, its launch shape, whether it is launched with the programmatic-stream-
+// serialization (PDL) attribute launch_k sets, and a copy of its by-value arguments.  launch() runs it on a stream;
+// set() makes a captured kernel node of the same kernel launch it.  Two calls compare equal when every one of these,
+// argument bytes included, is equal (callers zero their parameter blocks before filling them, so padding compares
+// equal; a spurious difference only costs one node update).
+struct KernelCall {
+  const void* func = nullptr;
+  dim3 grid, block;
+  size_t smem = 0;
+  bool pdl = true;
+  std::vector<uint8_t> args;             // argument i at offs[i], at its type's alignment, the gaps zero
+  std::vector<size_t> offs;
+
+  template <class... KArgs, class... Args>
+  void set_kernel(void (*kernel)(KArgs...), dim3 g, dim3 b, size_t sm, bool use_pdl, Args&&... a) {
+    static_assert(sizeof...(KArgs) == sizeof...(Args) && sizeof...(KArgs) <= kMaxArgs, "kernel arguments");
+    func = reinterpret_cast<const void*>(kernel); grid = g; block = b; smem = sm; pdl = use_pdl;
+    args.clear(); offs.clear();
+    (push<KArgs>(a), ...);
+  }
+  cudaError_t launch(cudaStream_t st) const {
+    void* ptrs[kMaxArgs];
+    arg_ptrs(ptrs);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
+    return cudaLaunchKernelExC(&cfg, func, ptrs);
+  }
+  cudaError_t set(cudaGraphExec_t exec, cudaGraphNode_t node) const {
+    void* ptrs[kMaxArgs];
+    arg_ptrs(ptrs);
+    cudaKernelNodeParams kp{};
+    kp.func = const_cast<void*>(func);
+    kp.gridDim = grid; kp.blockDim = block; kp.sharedMemBytes = static_cast<unsigned>(smem);
+    kp.kernelParams = ptrs;
+    return cudaGraphExecKernelNodeSetParams(exec, node, &kp);
+  }
+  bool operator==(const KernelCall& o) const {
+    return func == o.func && grid.x == o.grid.x && grid.y == o.grid.y && grid.z == o.grid.z && block.x == o.block.x &&
+           block.y == o.block.y && block.z == o.block.z && smem == o.smem && pdl == o.pdl && args == o.args;
+  }
+  bool operator!=(const KernelCall& o) const { return !(*this == o); }
+
+ private:
+  static constexpr size_t kMaxArgs = 8;
+  template <class T>
+  void push(const T& v) {
+    const size_t o = (args.size() + alignof(T) - 1) / alignof(T) * alignof(T);
+    args.resize(o + sizeof(T));
+    memcpy(args.data() + o, &v, sizeof(T));
+    offs.push_back(o);
+  }
+  void arg_ptrs(void** ptrs) const {
+    for (size_t i = 0; i < offs.size(); ++i) ptrs[i] = const_cast<uint8_t*>(args.data()) + offs[i];
+  }
+};
 
 static constexpr int kNetH = 320, kNetW = 640;   // the only network input size (scene_seg_infer.py:40-42)
 static constexpr int kGapReplicas = 8;           // copies of each SE pooling accumulator (atomic spreading)
@@ -72,13 +133,13 @@ struct PreprocessPlan {
   static int check(const PreGeom& g, int mode, const char* who, int k);
   // n images (1..kMaxBatch); rebuilds the tables only when a geometry or the mode changed
   int configure(const PreGeom* g, int n, int mode);
-  // frames[0 .. n-1]: image k reads frames[k] in its format (data, stride, and uv, uv_stride for NV12; its h, w are
-  // geom[k]'s); out / out_u8 hold n images back to back (16-bit mode only for n > 1).  A call whose frames are all
-  // packed launches the packed-only kernel instantiations; one non-packed frame selects the converting ones.
+  // The launch of frames[0 .. n-1] into c: image k reads frames[k] in its format (data, stride, and uv, uv_stride for
+  // NV12; its h, w are geom[k]'s); out / out_u8 hold n images back to back (16-bit mode only for n > 1).  A call whose
+  // frames are all packed launches the packed-only kernel instantiations; one non-packed frame selects the converting
+  // ones.  launch: describe, then c.launch on stream.
+  int describe(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8, KernelCall& c) const;
   int launch(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8,
              cudaStream_t stream) const;
-  int update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames, int convention,
-                        int dtype, void* out, uint8_t* out_u8) const;
   ~PreprocessPlan();
 };
 
@@ -110,20 +171,17 @@ int fuse_pool_x(int dtype, const void* f0, const void* f1, const void* f2, const
 // vpb_final_tapsum (conv_gemm.cu)
 int final_tapsum_x(const float* P, const float* bias, int Cout, int H, int W, int final_kind, float* out, uint8_t* cls,
                    cudaStream_t st, int batch = 1);
-// vpb_source_outputs (post_ops.cu).  source_outputs_update_node re-points a captured source_outputs_kernel node at
-// another job table; source_outputs_bytes: algorithmic HBM bytes of one launch (each distinct source map read once,
-// frames read, outputs written); viz_tables_init uploads the palettes once per device (not during a stream capture).
-int source_outputs_x(const vpb_src_job* jobs, int n, cudaStream_t st);
-int source_outputs_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_src_job* jobs, int n);
+// vpb_source_outputs (post_ops.cu).  source_outputs_call: the checked launch of the n jobs (launched without PDL; the
+// palettes must be resident: viz_tables_init); source_outputs_bytes: algorithmic HBM bytes of one launch (each distinct
+// source map read once, frames read, outputs written); viz_tables_init uploads the palettes once per device (not during
+// a stream capture).
+int source_outputs_call(const vpb_src_job* jobs, int n, KernelCall& c);
 double source_outputs_bytes(const vpb_src_job* jobs, int n);
 int viz_tables_init();
 // vpb_rectify_frames (rectify.cu) without its argument checks: n frames, rect[k] their maps, out[k] the packed rectified
-// frames, one launch; rectify_update_node re-points a captured rectify_kernel node at other frames, maps of the same
-// sizes and outputs; rectify_bytes: algorithmic HBM bytes of one launch (maps and frames read, outputs written).
-int rectify_x(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out,
-              cudaStream_t st);
-int rectify_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames,
-                        const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out);
+// frames, one launch; rectify_bytes: algorithmic HBM bytes of one launch (maps and frames read, outputs written).
+void rectify_call(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out,
+                  KernelCall& c);
 double rectify_bytes(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n);
 
 // JPEG frames (jpeg.cu).  jpeg_frame_check: the host header parse of a VPB_PIX_JPEG descriptor (frame_fmt_check's JPEG
@@ -148,9 +206,8 @@ struct JpegImg {                 // one stream of a decode call (the kernels' pa
 struct JpegParams { JpegImg im[kMaxBatch]; int bgr; };
 // Device decoding of the JPEG frames of one call: stage() parses the n host streams, builds the tables, destuffs the
 // data into pinned memory, uploads it and zeroes the coefficients on st (buffers grown on demand, the stream drained
-// first); launch(k) /
-// update_node(k) run or re-point kernel k (0 Huffman, 1 IDCT, 2 colour) of the staged call, writing frame j of the call
-// packed to out[j], B, G, R for bgr, else R, G, B.
+// first); describe(k) gives the launch of kernel k (0 Huffman, 1 IDCT, 2 colour) of the staged call, which writes frame
+// j of the call packed to out[j], B, G, R for bgr, else R, G, B.
 struct JpegDecoder {
   JpegParams p{};
   dim3 grid[3];
@@ -165,8 +222,7 @@ struct JpegDecoder {
   JpegDecoder& operator=(const JpegDecoder&) = delete;
   ~JpegDecoder();
   int stage(const vpb_frame_fmt* const* frames, int n, uint8_t* const* out, int bgr, cudaStream_t st);
-  int launch(int k, cudaStream_t st) const;
-  int update_node(int k, cudaGraphExec_t exec, cudaGraphNode_t node) const;
+  void describe(int k, KernelCall& c) const;
   double bytes(int k) const;     // algorithmic HBM bytes of kernel k's launch
 };
 

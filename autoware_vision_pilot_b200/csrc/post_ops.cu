@@ -411,32 +411,12 @@ static int source_params(const vpb_src_job* jobs, int n, const char* who, SrcPar
   return VPB_OK;
 }
 
-int source_outputs_x(const vpb_src_job* jobs, int n, cudaStream_t st) {
-  SrcParams p;
-  dim3 grid;
-  int rc = source_params(jobs, n, "vpb_source_outputs", p, grid);
-  if (rc) return rc;
-  rc = viz_tables_init();
-  if (rc) return rc;
-  source_outputs_kernel<<<grid, 128, 0, st>>>(p);
-  VPB_CUDA_OK(cudaGetLastError());
-  return VPB_OK;
-}
-
-int source_outputs_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_src_job* jobs, int n) {
+int source_outputs_call(const vpb_src_job* jobs, int n, KernelCall& c) {
   SrcParams p;
   dim3 grid;
   const int rc = source_params(jobs, n, "vpb_source_outputs", p, grid);
   if (rc) return rc;
-  void* args[1] = {&p};
-  cudaKernelNodeParams kp{};
-  kp.func = reinterpret_cast<void*>(source_outputs_kernel);
-  kp.gridDim = grid;
-  kp.blockDim = dim3(128);
-  kp.sharedMemBytes = 0;
-  kp.kernelParams = args;
-  kp.extra = nullptr;
-  VPB_CUDA_OK(cudaGraphExecKernelNodeSetParams(exec, node, &kp));
+  c.set_kernel(source_outputs_kernel, grid, dim3(128), 0, false, p);
   return VPB_OK;
 }
 
@@ -507,7 +487,12 @@ extern "C" int vpb_visualize_mask(const uint8_t* mask, int mh, int mw, int viz_t
   return VPB_OK;
 }
 extern "C" int vpb_source_outputs(const vpb_src_job* jobs, int n, void* stream) {
-  return vpb::source_outputs_x(jobs, n, static_cast<cudaStream_t>(stream));
+  KernelCall c;
+  int rc = source_outputs_call(jobs, n, c);
+  if (rc == VPB_OK) rc = viz_tables_init();
+  if (rc) return rc;
+  VPB_CUDA_OK(c.launch(static_cast<cudaStream_t>(stream)));
+  return VPB_OK;
 }
 extern "C" int vpb_polyfit(const float* xs, const float* ys, const int* offsets, int n_sets, int order,
                            double* coeffs, double* yrange, void* stream) {

@@ -482,6 +482,7 @@ static int fill_params(const PreprocessPlan& pl, const vpb_frame_fmt* frames, in
     vpb_set_error("preprocess: batch %d (1..%d, 16-bit output only)", pl.n, kMaxBatch);
     return VPB_ERR_ARG;
   }
+  memset(&p, 0, sizeof(p));
   p.out_lo = pl.out_lo;
   p.out_pitch = pl.out_pitch; p.out_c = pl.out_c;
   // a non-packed image converts to the channel order the convention takes as input
@@ -523,7 +524,6 @@ template <bool CVT>
 struct PreKernel {
   void (*pil)(PreParamsOf<CVT>, int, int, int);
   void (*direct)(PreParamsOf<CVT>);
-  const void* func() const { return pil ? reinterpret_cast<const void*>(pil) : reinterpret_cast<const void*>(direct); }
 };
 template <bool CVT>
 static PreKernel<CVT> pre_kernel(int mode, int dtype, int xt) {
@@ -533,40 +533,11 @@ static PreKernel<CVT> pre_kernel(int mode, int dtype, int xt) {
     return PreKernel<CVT>{xt == 16 ? preprocess_pil_kernel<E, 16, CVT> : preprocess_pil_kernel<E, 32, CVT>, nullptr};
   });
 }
-static const void* pre_func(int mode, int dtype, int xt, bool cvt) {
-  return cvt ? pre_kernel<true>(mode, dtype, xt).func() : pre_kernel<false>(mode, dtype, xt).func();
-}
 
-// Re-point the captured pre-process node at other source frames (same geometries and formats): lets the frame graph be
-// replayed on any device buffers without re-capturing.  The node's kernel takes PreParams (packed-only call) or the
-// whole PreParamsCvt; PreParams is its first sub-object, so one pointer serves both.
-int PreprocessPlan::update_graph_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames,
-                                      int convention, int dtype, void* out, uint8_t* out_u8) const {
-  PreParamsCvt p;
-  bool cvt = false;
-  const int rc = fill_params(*this, frames, convention, out, out_u8, p, cvt);
-  if (rc) return rc;
-  int rc_ = rows_cap, pitch_ = pitch, ty_ = TY;
-  void* args[4] = {static_cast<PreParams*>(&p), &rc_, &pitch_, &ty_};
-  cudaKernelNodeParams kp{};
-  kp.func = const_cast<void*>(pre_func(mode, dtype, xt, cvt));
-  kp.kernelParams = args;
-  kp.extra = nullptr;
-  if (is_pil(mode)) {
-    kp.gridDim = dim3((OWmax + kTX - 1) / kTX, (OHmax + TY - 1) / TY, n);
-    kp.blockDim = dim3(kPreThreads);
-    kp.sharedMemBytes = static_cast<unsigned>(smem_bytes);
-  } else {
-    kp.gridDim = dim3((OWmax + 255) / 256, OHmax, n);
-    kp.blockDim = dim3(256);
-    kp.sharedMemBytes = 0;
-  }
-  VPB_CUDA_OK(cudaGraphExecKernelNodeSetParams(exec, node, &kp));
-  return VPB_OK;
-}
-
+// The launch of a call whose parameter block is p: a packed-only call passes p's PreParams sub-object, a converting
+// call the whole PreParamsCvt.
 template <bool CVT>
-static int launch_pre(const PreprocessPlan& pl, const PreParamsCvt& p, int dtype, cudaStream_t stream) {
+static int describe_pre(const PreprocessPlan& pl, const PreParamsCvt& p, int dtype, KernelCall& c) {
   const PreKernel<CVT> k = pre_kernel<CVT>(pl.mode, dtype, pl.xt);
   if (k.pil) {
     dim3 grid((pl.OWmax + kTX - 1) / kTX, (pl.OHmax + pl.TY - 1) / pl.TY, pl.n);
@@ -585,20 +556,29 @@ static int launch_pre(const PreprocessPlan& pl, const PreParamsCvt& p, int dtype
         *done = true;
       }
     }
-    VPB_CUDA_OK(launch_k(k.pil, grid, dim3(kPreThreads), pl.smem_bytes, stream, p, pl.rows_cap, pl.pitch, pl.TY));
+    c.set_kernel(k.pil, grid, dim3(kPreThreads), pl.smem_bytes, true, p, pl.rows_cap, pl.pitch, pl.TY);
   } else {
-    VPB_CUDA_OK(launch_k(k.direct, dim3((pl.OWmax + 255) / 256, pl.OHmax, pl.n), dim3(256), 0, stream, p));
+    c.set_kernel(k.direct, dim3((pl.OWmax + 255) / 256, pl.OHmax, pl.n), dim3(256), 0, true, p);
   }
   return VPB_OK;
 }
 
-int PreprocessPlan::launch(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8,
-                           cudaStream_t stream) const {
+int PreprocessPlan::describe(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8,
+                             KernelCall& c) const {
   PreParamsCvt p;
   bool cvt = false;
   const int rc = fill_params(*this, frames, convention, out, out_u8, p, cvt);
   if (rc) return rc;
-  return cvt ? launch_pre<true>(*this, p, dtype, stream) : launch_pre<false>(*this, p, dtype, stream);
+  return cvt ? describe_pre<true>(*this, p, dtype, c) : describe_pre<false>(*this, p, dtype, c);
+}
+
+int PreprocessPlan::launch(const vpb_frame_fmt* frames, int convention, int dtype, void* out, uint8_t* out_u8,
+                           cudaStream_t stream) const {
+  KernelCall c;
+  const int rc = describe(frames, convention, dtype, out, out_u8, c);
+  if (rc) return rc;
+  VPB_CUDA_OK(c.launch(stream));
+  return VPB_OK;
 }
 
 int frame_fmt_check(const vpb_frame_fmt& f, const char* who, int k) {

@@ -1,6 +1,6 @@
 // rectify.cu — lens rectification of camera frames through OpenCV's fixed-point undistortion maps, one launch for the
-// frames of a call (the map object, the kernel, the op entry point vpb_rectify_frames and the launchers the engines'
-// "rectify" op uses).
+// frames of a call (the map object, the kernel, the op entry point vpb_rectify_frames and the launch the engines'
+// "rectify" op describes).
 //
 // Replaces image_proc's rectify: cv::remap(src, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) on the 8-bit frame with the
 // CV_16SC2 + CV_16UC1 maps image_geometry builds.  That remap is integer arithmetic and is reproduced byte for byte
@@ -71,8 +71,9 @@ __global__ void __launch_bounds__(kRectTX * kRectTY) rectify_kernel(const __grid
   for (int c = 0; c < 3; ++c) o[c] = static_cast<uint8_t>(min(acc[c] >> 15, 255));
 }
 
-static void fill_params(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n, int bgr,
-                        uint8_t* const* out, RectParams& p, dim3& grid) {
+void rectify_call(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out,
+                  KernelCall& c) {
+  RectParams p;
   memset(&p, 0, sizeof(p));
   p.bgr = bgr;
   int mh = 0, mw = 0;
@@ -86,32 +87,8 @@ static void fill_params(const vpb_frame_fmt* frames, const vpb_rectify* const* r
     r.out = out[k];
     mh = std::max(mh, r.mh); mw = std::max(mw, r.mw);
   }
-  grid = dim3((mw + kRectTX - 1) / kRectTX, (mh + kRectTY - 1) / kRectTY, n);
-}
-
-int rectify_x(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out,
-              cudaStream_t st) {
-  RectParams p;
-  dim3 grid;
-  fill_params(frames, rect, n, bgr, out, p, grid);
-  VPB_CUDA_OK(launch_k(rectify_kernel, grid, dim3(kRectTX, kRectTY), 0, st, p));
-  return VPB_OK;
-}
-
-int rectify_update_node(cudaGraphExec_t exec, cudaGraphNode_t node, const vpb_frame_fmt* frames,
-                        const vpb_rectify* const* rect, int n, int bgr, uint8_t* const* out) {
-  RectParams p;
-  dim3 grid;
-  fill_params(frames, rect, n, bgr, out, p, grid);
-  void* args[1] = {&p};
-  cudaKernelNodeParams kp{};
-  kp.func = reinterpret_cast<void*>(rectify_kernel);
-  kp.gridDim = grid;
-  kp.blockDim = dim3(kRectTX, kRectTY);
-  kp.sharedMemBytes = 0;
-  kp.kernelParams = args;
-  VPB_CUDA_OK(cudaGraphExecKernelNodeSetParams(exec, node, &kp));
-  return VPB_OK;
+  const dim3 grid((mw + kRectTX - 1) / kRectTX, (mh + kRectTY - 1) / kRectTY, n);
+  c.set_kernel(rectify_kernel, grid, dim3(kRectTX, kRectTY), 0, true, p);
 }
 
 double rectify_bytes(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n) {
@@ -202,5 +179,8 @@ extern "C" int vpb_rectify_frames(const vpb_frame_fmt* frames_dev, const vpb_rec
       return VPB_ERR_ARG;
     }
   }
-  return vpb::rectify_x(frames_dev, rect, n, bgr != 0, out, static_cast<cudaStream_t>(stream));
+  vpb::KernelCall c;
+  vpb::rectify_call(frames_dev, rect, n, bgr != 0, out, c);
+  VPB_CUDA_OK(c.launch(static_cast<cudaStream_t>(stream)));
+  return VPB_OK;
 }

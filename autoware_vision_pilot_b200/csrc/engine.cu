@@ -99,6 +99,21 @@ struct vp_engine : EngineRuntime {
   std::vector<vpb_src_job> src_jobs;
   bool src_ready = false;                  // a call has run (vp_engine_source_output answers)
   bool src_host = false;                   // the last call was a host call: the pinned copies are current
+  // The lateral post-process inside the call (vp_engine_set_lateral): op "lateral" right after the final op of the
+  // EgoLanes model lat_model, on that model's lane.  States and records come in two slots of `batch` each: a call reads
+  // the states of slot lat_cur and writes the states and records of slot 1 - lat_cur, and the host flips lat_cur once
+  // the call is enqueued.  So a launch that runs again with the same arguments (a capture's eager pass, profiling,
+  // kernel timing) computes the same thing and leaves the last call's states and records alone.
+  int lat_model = -1;                      // -1: off
+  float lat_threshold = 0.f, lat_smoothing = 0.5f;
+  std::vector<double> lat_hom;             // batch x 9 orig -> BEV matrices; empty: the reference matrix
+  double steering[kMaxBatch] = {};         // vp_engine_set_steering
+  vpb_lateral_state* d_lat_state = nullptr;   // [2][batch]
+  vpb_lateral_out* d_lat_out = nullptr;       // [2][batch]
+  vpb_lateral_out* h_lat_out = nullptr;       // [batch] pinned copy of slot lat_cur's records made by a host call
+  int lat_cur = 0;
+  bool lat_ready = false;                  // a call has made records since the feature was set
+  bool lat_host = false;                   // the last call was a host call: h_lat_out is current
 
   int geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) override;
   int enqueue(const PreGeom* g) override;
@@ -623,6 +638,11 @@ static int check_source_flags(const vp_engine_config& c) {
 // callers run it before any device work.
 int vp_engine::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
   for (int k = 0; k < batch; ++k) {
+    if (lat_model >= 0 && frames[k].h > kLatMaxImgH) {
+      vpb_set_error("%s: frame %d: height %d is above the %d rows the lateral post-process takes", who, k, frames[k].h,
+                    kLatMaxImgH);
+      return VPB_ERR_ARG;
+    }
     if ((cfg.source_outputs & VP_SRC_OVERLAY) && frames[k].format != VPB_PIX_PACKED) {
       vpb_set_error("%s: frame %d: VP_SRC_OVERLAY blends the packed camera frame; this engine cannot take a non-packed frame "
                     "(format %d)", who, k, frames[k].format);
@@ -640,10 +660,12 @@ int vp_engine::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
 // unchanged).  The pinned host copies of the source outputs are stale from here on.
 int vp_engine::enqueue(const PreGeom* g) {
   src_host = false;
+  lat_host = false;
   int rc = pre.configure(g, batch, cfg.resize_mode);
   if (rc == VPB_OK && !src_outs.empty()) rc = prepare_source(*this);
   if (rc == VPB_OK) rc = run_call();
   if (rc == VPB_OK) src_ready = true;
+  if (rc == VPB_OK && lat_model >= 0) { lat_cur ^= 1; lat_ready = true; }
   return rc;
 }
 
@@ -664,6 +686,11 @@ int vp_engine::fetch(bool raw) {
   for (const auto& so : src_outs)
     VPB_CUDA_OK(cudaMemcpyAsync(so.h, so.d, static_cast<size_t>(so.job.dh) * so.job.dst_pitch, cudaMemcpyDeviceToHost, stream));
   src_host = true;
+  if (lat_model >= 0) {
+    VPB_CUDA_OK(cudaMemcpyAsync(h_lat_out, d_lat_out + static_cast<size_t>(lat_cur) * batch, sizeof(vpb_lateral_out) * batch,
+                                cudaMemcpyDeviceToHost, stream));
+    lat_host = true;
+  }
   return VPB_OK;
 }
 
@@ -814,6 +841,122 @@ extern "C" int vp_engine_set_rectify(vp_engine* e, int sample, const vpb_rectify
   if (!e) { vpb_set_error("vp_engine_set_rectify: NULL engine"); return VPB_ERR_ARG; }
   DeviceGuard guard(e->gpu_id);
   return e->set_rectify(sample, r, "vp_engine_set_rectify");
+}
+
+// ---------------------------------------------------------------- the lateral post-process inside the call
+// Op "lateral": the EgoLanes logits of model lat_model, each sample's source size (what its pre-process reads: the
+// frame as given, a JPEG frame's SOF size, a rectified frame's map size), the states of slot lat_cur -> the states and
+// records of slot 1 - lat_cur.
+static OpRec lateral_op(vp_engine& e) {
+  OpRec op;
+  op.name = "lateral"; op.kname = "lateral_kernel"; op.lane = e.lat_model;
+  const ModelOut& mo = e.outs[e.lat_model];
+  op.bytes = e.batch * (4.0 * 3 * mo.H * mo.W + 2.0 * sizeof(vpb_lateral_state) + sizeof(vpb_lateral_out));
+  vp_engine* ep = &e;
+  op.describe = [ep](KernelCall& c) {
+    const ModelOut& m = ep->outs[ep->lat_model];
+    int iw[kMaxBatch], ih[kMaxBatch];
+    for (int k = 0; k < ep->batch; ++k) {
+      const vpb_frame_fmt f = ep->chain[k].pre();
+      iw[k] = f.w; ih[k] = f.h;
+    }
+    const size_t rd = static_cast<size_t>(ep->lat_cur) * ep->batch, wr = static_cast<size_t>(1 - ep->lat_cur) * ep->batch;
+    return lateral_call("lateral", m.d_raw, ep->lat_threshold, ep->batch, m.H, m.W, iw, ih, ep->lat_smoothing,
+                        ep->lat_hom.empty() ? nullptr : ep->lat_hom.data(), ep->steering, ep->d_lat_state + rd,
+                        ep->d_lat_state + wr, ep->d_lat_out + wr, c);
+  };
+  return op;
+}
+
+// fresh states (vpb_lateral_init) for sample `sample` (-1: every sample) of slot `slot`, on the engine's stream
+static int lateral_init_slot(vp_engine& e, int slot, int sample) {
+  for (int k = sample < 0 ? 0 : sample; k < (sample < 0 ? e.batch : sample + 1); ++k) {
+    const int rc = vpb_lateral_init(e.d_lat_state + static_cast<size_t>(slot) * e.batch + k, e.stream);
+    if (rc) return rc;
+  }
+  return VPB_OK;
+}
+
+extern "C" int vp_engine_set_lateral(vp_engine* e, int model_idx, const vp_lateral_config* cfg) {
+  const char* who = "vp_engine_set_lateral";
+  if (!e) { vpb_set_error("%s: NULL engine", who); return VPB_ERR_ARG; }
+  if (cfg) {
+    if (model_idx < 0 || model_idx >= static_cast<int>(e->outs.size()) || e->outs[model_idx].kind != VP_EGO_LANES) {
+      vpb_set_error("%s: model %d is not an EgoLanes model of this engine", who, model_idx);
+      return VPB_ERR_ARG;
+    }
+    if (!(cfg->smoothing >= 0.0f && cfg->smoothing <= 1.0f)) {
+      vpb_set_error("%s: smoothing %g is outside [0, 1]", who, static_cast<double>(cfg->smoothing));
+      return VPB_ERR_ARG;
+    }
+  }
+  DeviceGuard guard(e->gpu_id);
+  if (cfg && !e->d_lat_state) {
+    void* st = nullptr; void* out = nullptr;
+    VPB_CUDA_OK(cudaMalloc(&st, sizeof(vpb_lateral_state) * 2 * e->batch));
+    e->dev_allocs.push_back(st);
+    VPB_CUDA_OK(cudaMalloc(&out, sizeof(vpb_lateral_out) * 2 * e->batch));
+    e->dev_allocs.push_back(out);
+    void* h = e->halloc(sizeof(vpb_lateral_out) * e->batch);
+    if (!h) return VPB_ERR_CUDA;
+    e->d_lat_state = static_cast<vpb_lateral_state*>(st);
+    e->d_lat_out = static_cast<vpb_lateral_out*>(out);
+    e->h_lat_out = static_cast<vpb_lateral_out*>(h);
+  }
+  const int at = e->op_index("lateral");
+  if (at >= 0) e->erase_ops(at, 1);        // drops the captured graph
+  e->lat_model = -1; e->lat_ready = false; e->lat_host = false;
+  if (!cfg) return VPB_OK;
+  e->lat_threshold = cfg->threshold; e->lat_smoothing = cfg->smoothing;
+  if (cfg->homographies) e->lat_hom.assign(cfg->homographies, cfg->homographies + 9 * e->batch);
+  else e->lat_hom.clear();
+  e->lat_cur = 0;
+  int rc = lateral_init_slot(*e, 0, -1);
+  if (rc) return rc;
+  e->lat_model = model_idx;
+  const int last = e->op_index((std::to_string(model_idx) + "/dec8sum").c_str());   // the model's final op
+  e->insert_ops(last + 1, {lateral_op(*e)});
+  return VPB_OK;
+}
+
+extern "C" int vp_engine_set_steering(vp_engine* e, const double* steering_rad) {
+  if (!e) { vpb_set_error("vp_engine_set_steering: NULL engine"); return VPB_ERR_ARG; }
+  for (int k = 0; k < e->batch; ++k) e->steering[k] = steering_rad ? steering_rad[k] : 0.0;
+  return VPB_OK;
+}
+
+extern "C" int vp_engine_lateral_reset(vp_engine* e, int sample) {
+  const char* who = "vp_engine_lateral_reset";
+  if (!e) { vpb_set_error("%s: NULL engine", who); return VPB_ERR_ARG; }
+  if (sample < -1 || sample >= e->batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch); return VPB_ERR_ARG; }
+  if (e->lat_model < 0) { vpb_set_error("%s: the lateral post-process is off (vp_engine_set_lateral)", who); return VPB_ERR_STATE; }
+  DeviceGuard guard(e->gpu_id);
+  return lateral_init_slot(*e, e->lat_cur, sample);
+}
+
+extern "C" int vp_engine_lateral(vp_engine* e, int sample, const vpb_lateral_out** host, const vpb_lateral_out** dev) {
+  const char* who = "vp_engine_lateral";
+  if (!e) { vpb_set_error("%s: NULL engine", who); return VPB_ERR_ARG; }
+  if (sample < 0 || sample >= e->batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch); return VPB_ERR_ARG; }
+  if (e->lat_model < 0) { vpb_set_error("%s: the lateral post-process is off (vp_engine_set_lateral)", who); return VPB_ERR_STATE; }
+  if (!e->lat_ready) { vpb_set_error("%s: run one call first", who); return VPB_ERR_STATE; }
+  if (host) *host = e->lat_host ? e->h_lat_out + sample : nullptr;
+  if (dev) *dev = e->d_lat_out + static_cast<size_t>(e->lat_cur) * e->batch + sample;
+  return VPB_OK;
+}
+
+const vpb_lateral_out* vpb_engine_lateral_records(const vp_engine* e, int model_idx, const char* who) {
+  if (!e || e->lat_model != model_idx || model_idx < 0) {
+    vpb_set_error("%s: model %d has no lateral post-process in the call (vp_engine_set_lateral)", who, model_idx);
+    return nullptr;
+  }
+  if (!e->lat_ready) { vpb_set_error("%s: no call has made lateral records yet", who); return nullptr; }
+  return e->d_lat_out + static_cast<size_t>(e->lat_cur) * e->batch;
+}
+
+extern "C" int vp_engine_graph_captures(const vp_engine* e) {
+  if (!e) { vpb_set_error("vp_engine_graph_captures: NULL engine"); return VPB_ERR_ARG; }
+  return e->frame_graph.captures;
 }
 
 extern "C" int vp_engine_fetch_raw(vp_engine* e, int idx) {

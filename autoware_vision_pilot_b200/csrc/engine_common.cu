@@ -138,6 +138,7 @@ int FrameGraph::run(EngineRuntime& e) {
     cudaError_t ce = cudaStreamEndCapture(st, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
     if (ce != cudaSuccess) { vpb_set_error("graph capture failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
+    ++captures;
     ce = cudaGraphInstantiate(&exec, g, 0);
     if (graph) cudaGraphDestroy(graph);
     graph = g;
@@ -301,14 +302,16 @@ void EngineRuntime::insert_ops(size_t at, std::vector<OpRec> add) {
   ops.insert(ops.begin() + at, std::make_move_iterator(add.begin()), std::make_move_iterator(add.end()));
   if (!op_events.empty())
     for (int i = 0; i < m; ++i) op_events.insert(op_events.begin() + at, Event());
-  for (int& d : lane_dep) d += m;
+  for (int& d : lane_dep)
+    if (d >= static_cast<int>(at)) d += m;
 }
 
 void EngineRuntime::erase_ops(size_t at, size_t m) {
   frame_graph.invalidate();
   ops.erase(ops.begin() + at, ops.begin() + at + m);
   if (!op_events.empty()) op_events.erase(op_events.begin() + at, op_events.begin() + at + m);
-  for (int& d : lane_dep) d -= static_cast<int>(m);
+  for (int& d : lane_dep)
+    if (d >= static_cast<int>(at + m)) d -= static_cast<int>(m);
 }
 
 void EngineRuntime::sync_front_ops() {

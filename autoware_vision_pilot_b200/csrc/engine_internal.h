@@ -103,6 +103,7 @@ struct FrameGraph {
   std::vector<Node> nodes;
   int n = 0;                             // the geometry key: geometries of geom[0 .. n-1] (0: none)
   Frames geom{};
+  int captures = 0;                      // captures so far (vp_engine_graph_captures)
 
   // Launch the graph for e's frames on e's stream.  When the key differs: e.launch_all once outside capture (sets
   // function attributes; its results are correct), capture e.launch_all and instantiate.
@@ -195,8 +196,8 @@ struct EngineRuntime {
   // map of another GPU; then sync_front_ops.
   int set_rectify(int sample, const vpb_rectify* r, const char* who);
   int op_index(const char* name) const;   // index of the op of that name, -1 if there is none
-  // insert ops at index `at` / erase m ops from `at`: the op events and the lanes' producer indices follow, and the
-  // captured graph is dropped
+  // insert ops at index `at` / erase m ops from `at`: the op events and the lanes' producer indices past `at` follow,
+  // and the captured graph is dropped
   void insert_ops(size_t at, std::vector<OpRec> add);
   void erase_ops(size_t at, size_t m);
   // The front ops before "preprocess" exactly while they are needed: the three JPEG decode ops while a sample's frame
@@ -272,3 +273,6 @@ bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int
 // frames per call of a segmentation engine (engine.cu), for callers that see vp_engine only as an opaque type
 struct vp_engine;
 int vpb_engine_batch(const vp_engine* e);
+// the device records of e's last call made by its in-call lateral post-process on model model_idx (vp_engine_set_lateral);
+// NULL, with the error set naming who, when that model has none or no call has made them
+const vpb_lateral_out* vpb_engine_lateral_records(const vp_engine* e, int model_idx, const char* who);

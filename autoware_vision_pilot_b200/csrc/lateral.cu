@@ -30,7 +30,7 @@ static constexpr int kMaxPts = 2 * (kMaxH / 4) * 48;
 // Points generated from one polynomial: y from min_y to max_y in steps of 5 source rows.  The fitted y-limits are
 // mask rows (at most H - 1, smoothing keeps them there), so the count is at most (H-1)/H * img_h / 5 + 1, one more
 // for the rounding of the accumulated y: this bounds the source height the launcher accepts.
-static constexpr int kMaxImgH = 4320;
+static constexpr int kMaxImgH = kLatMaxImgH;
 static constexpr int kMaxGen = 896;
 static_assert(kMaxGen >= kMaxImgH / 5 + 2, "generated-point buffers too small for the tallest accepted source");
 
@@ -256,6 +256,7 @@ struct LatCam {               // what differs between the cameras of one launch
 struct LatParams {          // by value: 1.4 KB at kMaxBatch cameras, under the 4 KB kernel-parameter limit
   int H, W;
   float smoothing;
+  float threshold;          // a mask bit is set where the input is > threshold
   LatCam cam[kMaxBatch];    // camera k = blockIdx.x
 };
 
@@ -322,20 +323,31 @@ __device__ __forceinline__ double f_curv(const double* c, double y) {
   return fabs(den) < 1e-6 ? 0.0 : fabs(2 * c[1]) / den;
 }
 
-// One CTA per camera: camera k = blockIdx.x reads masks [k][3][H][W] and owns st[k], out[k] and p.cam[k].
+// One CTA per camera: camera k = blockIdx.x reads masks [k][3][H][W] and st_in[k], and owns st[k], out[k] and
+// p.cam[k].  masks are vpb_lane_masks' 0 / 1 output with threshold 0.5f (every test in lane_filter.cpp is > 0.5f), or
+// the EgoLanes logits themselves with the engine's threshold: both set the same bits.  With st_in != st the CTA first
+// copies st_in[k] to st[k] and then updates st[k], so a launch that is repeated (a graph capture after its eager run, a
+// timing pass) leaves the same state; with st_in == st it updates st[k] in place.
 // At most 8 CTAs on 132 SMs, so each has an SM to itself: the minimum of one CTA per SM lets ptxas keep the fp64
 // scalars in registers (0 spill bytes; with the default bound it spills about 2 KB per thread).
 __global__ void __launch_bounds__(256, 1) lateral_kernel(const float* __restrict__ masks,
                                                          const __grid_constant__ LatParams p,
+                                                         const vpb_lateral_state* __restrict__ st_in,
                                                          vpb_lateral_state* __restrict__ st,
                                                          vpb_lateral_out* __restrict__ out) {
   __shared__ LatShared s;
   const int H = p.H, W = p.W, words = (W + 31) >> 5;
   const LatCam& cam = p.cam[blockIdx.x];
   masks += static_cast<size_t>(blockIdx.x) * 3 * H * W;
+  if (st_in != st) {          // made visible to the CTA by the __syncthreads below
+    static_assert(sizeof(vpb_lateral_state) % 8 == 0, "the state is copied as 8-byte words");
+    const uint64_t* a = reinterpret_cast<const uint64_t*>(st_in + blockIdx.x);
+    uint64_t* d = reinterpret_cast<uint64_t*>(st + blockIdx.x);
+    for (int i = threadIdx.x; i < static_cast<int>(sizeof(vpb_lateral_state) / 8); i += blockDim.x) d[i] = a[i];
+  }
   st += blockIdx.x;
   out += blockIdx.x;
-  // ---- masks -> bit rows (> 0.5f, as every test in lane_filter.cpp)
+  // ---- masks -> bit rows
   for (int i = threadIdx.x; i < 3 * kMaxH * kMaxWords; i += blockDim.x) (&s.bits[0][0][0])[i] = 0u;
   __syncthreads();
   for (int i = threadIdx.x; i < 3 * H * words; i += blockDim.x) {
@@ -344,7 +356,7 @@ __global__ void __launch_bounds__(256, 1) lateral_kernel(const float* __restrict
     const float* row = masks + (static_cast<size_t>(ch) * H + y) * W;
     for (int b = 0; b < 32; ++b) {
       const int x = w * 32 + b;
-      if (x < W && row[x] > 0.5f) bitsv |= 1u << b;
+      if (x < W && row[x] > p.threshold) bitsv |= 1u << b;
     }
     s.bits[ch][y][w] = bitsv;
   }
@@ -588,16 +600,16 @@ extern "C" int vpb_lateral_init(vpb_lateral_state* state, void* stream) {
 }
 
 // n cameras in one launch, camera k with source size img_w[k] x img_h[k] (vpb_lateral_update is n = 1,
-// vpb_lateral_update_batch n equal sizes).  Everything is checked before device work.
-static int lateral_launch(const char* who, const float* masks, int n, int H, int W, const int* img_w, const int* img_h,
-                          float smoothing, const double* homographies, const double* steering,
-                          vpb_lateral_state* states, vpb_lateral_out* outs, void* stream) {
+// vpb_lateral_update_batch n equal sizes).  Everything is checked before the launch is described.
+int vpb::lateral_call(const char* who, const float* masks, float threshold, int n, int H, int W, const int* img_w,
+                      const int* img_h, float smoothing, const double* homographies, const double* steering,
+                      const vpb_lateral_state* st_in, vpb_lateral_state* states, vpb_lateral_out* outs, KernelCall& c) {
   if (n < 1 || n > vpb::kMaxBatch) {
     vpb_set_error("%s: %d cameras (1..%d)", who, n, vpb::kMaxBatch);
     return VPB_ERR_ARG;
   }
   static const char* kNeed = "need masks [3][H<=128][W<=256] (H >= 41), state and out";
-  if (!masks || !states || !outs || H < 41 || H > vpb::kMaxH || W < 2 || W > vpb::kMaxWords * 32) {
+  if (!masks || !st_in || !states || !outs || H < 41 || H > vpb::kMaxH || W < 2 || W > vpb::kMaxWords * 32) {
     vpb_set_error("%s: %s", who, kNeed);
     return VPB_ERR_ARG;
   }
@@ -605,13 +617,13 @@ static int lateral_launch(const char* who, const float* masks, int n, int H, int
     vpb_set_error("%s: %s, and img_w / img_h arrays (NULL)", who, kNeed);
     return VPB_ERR_ARG;
   }
-  for (int c = 0; c < n; ++c) {
-    if (img_w[c] <= 0 || img_h[c] <= 0) {
-      vpb_set_error("%s: %s; camera %d: image size %dx%d is not positive", who, kNeed, c, img_w[c], img_h[c]);
+  for (int k = 0; k < n; ++k) {
+    if (img_w[k] <= 0 || img_h[k] <= 0) {
+      vpb_set_error("%s: %s; camera %d: image size %dx%d is not positive", who, kNeed, k, img_w[k], img_h[k]);
       return VPB_ERR_ARG;
     }
-    if (img_h[c] > vpb::kMaxImgH) {
-      vpb_set_error("%s: camera %d: image height %d is above %d", who, c, img_h[c], vpb::kMaxImgH);
+    if (img_h[k] > vpb::kMaxImgH) {
+      vpb_set_error("%s: camera %d: image height %d is above %d", who, k, img_h[k], vpb::kMaxImgH);
       return VPB_ERR_ARG;
     }
   }
@@ -625,16 +637,28 @@ static int lateral_launch(const char* who, const float* masks, int n, int H, int
                                1.85824549e-14,  -1.28170839e+00, 8.63871455e+02,
                                2.95628463e-17,  -1.76125061e-03, 1.00000000e+00};
   vpb::LatParams p;
-  p.H = H; p.W = W; p.smoothing = smoothing;
-  for (int c = 0; c < n; ++c) {
-    vpb::LatCam& cam = p.cam[c];
-    for (int k = 0; k < 9; ++k) cam.Hm[k] = homographies ? homographies[9 * c + k] : kH[k];
+  memset(&p, 0, sizeof(p));
+  p.H = H; p.W = W; p.smoothing = smoothing; p.threshold = threshold;
+  for (int k = 0; k < n; ++k) {
+    vpb::LatCam& cam = p.cam[k];
+    for (int i = 0; i < 9; ++i) cam.Hm[i] = homographies ? homographies[9 * k + i] : kH[i];
     vpb::inv3(cam.Hm, cam.Hi);
-    cam.steering = steering ? steering[c] : 0.0;
-    cam.sx = static_cast<double>(img_w[c]) / W; cam.sy = static_cast<double>(img_h[c]) / H;
+    cam.steering = steering ? steering[k] : 0.0;
+    cam.sx = static_cast<double>(img_w[k]) / W; cam.sy = static_cast<double>(img_h[k]) / H;
   }
-  vpb::lateral_kernel<<<n, 256, 0, static_cast<cudaStream_t>(stream)>>>(masks, p, states, outs);
-  VPB_CUDA_OK(cudaGetLastError());
+  c.set_kernel(vpb::lateral_kernel, dim3(n), dim3(256), 0, false, masks, p, st_in, states, outs);
+  return VPB_OK;
+}
+
+// The launch of lateral_call, in place (st_in == states)
+static int lateral_launch(const char* who, const float* masks, float threshold, int n, int H, int W, const int* img_w,
+                          const int* img_h, float smoothing, const double* homographies, const double* steering,
+                          vpb_lateral_state* states, vpb_lateral_out* outs, void* stream) {
+  vpb::KernelCall c;
+  const int rc = vpb::lateral_call(who, masks, threshold, n, H, W, img_w, img_h, smoothing, homographies, steering,
+                                   states, states, outs, c);
+  if (rc) return rc;
+  VPB_CUDA_OK(c.launch(static_cast<cudaStream_t>(stream)));
   return VPB_OK;
 }
 
@@ -644,7 +668,7 @@ static int lateral_launch_one_size(const char* who, const float* masks, int n, i
                                    vpb_lateral_state* states, vpb_lateral_out* outs, void* stream) {
   int ws[vpb::kMaxBatch], hs[vpb::kMaxBatch];
   for (int c = 0; c < vpb::kMaxBatch; ++c) { ws[c] = img_w; hs[c] = img_h; }
-  return lateral_launch(who, masks, n, H, W, ws, hs, smoothing, homographies, steering, states, outs, stream);
+  return lateral_launch(who, masks, 0.5f, n, H, W, ws, hs, smoothing, homographies, steering, states, outs, stream);
 }
 
 extern "C" int vpb_lateral_update(const float* masks, int H, int W, int img_w, int img_h, float smoothing,
@@ -664,6 +688,14 @@ extern "C" int vpb_lateral_update_batch(const float* masks, int n, int H, int W,
 extern "C" int vpb_lateral_update_cameras(const float* masks, int n, int H, int W, const int* img_w, const int* img_h,
                                           float smoothing, const double* homographies, const double* steering_rad,
                                           vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream) {
-  return lateral_launch("vpb_lateral_update_cameras", masks, n, H, W, img_w, img_h, smoothing, homographies,
+  return lateral_launch("vpb_lateral_update_cameras", masks, 0.5f, n, H, W, img_w, img_h, smoothing, homographies,
+                        steering_rad, states_dev, outs_dev, stream);
+}
+
+extern "C" int vpb_lateral_update_logits(const float* raw, int n, int H, int W, float threshold, const int* img_w,
+                                         const int* img_h, float smoothing, const double* homographies,
+                                         const double* steering_rad, vpb_lateral_state* states_dev,
+                                         vpb_lateral_out* outs_dev, void* stream) {
+  return lateral_launch("vpb_lateral_update_logits", raw, threshold, n, H, W, img_w, img_h, smoothing, homographies,
                         steering_rad, states_dev, outs_dev, stream);
 }

@@ -289,7 +289,8 @@ extern "C" int vp_multicam_step(vp_multicam* mc, const void* feat_dev, const dou
 
 extern "C" int vp_multicam_step_engine(vp_multicam* mc, vp_engine* e, int model_idx, const vpb_lateral_out* lat,
                                        int predict) {
-  if (!mc || !e || !lat) { vpb_set_error("vp_multicam_step_engine: bad arguments"); return VPB_ERR_ARG; }
+  if (!mc || !e) { vpb_set_error("vp_multicam_step_engine: bad arguments"); return VPB_ERR_ARG; }
+  if (!lat && !(lat = vpb_engine_lateral_records(e, model_idx, "vp_multicam_step_engine"))) return VPB_ERR_ARG;
   if (mc->local && vpb_engine_batch(e) != mc->world) {
     vpb_set_error("vp_multicam_step_engine: engine of batch %d for %d cameras", vpb_engine_batch(e), mc->world);
     return VPB_ERR_ARG;

@@ -184,6 +184,16 @@ void rectify_call(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, i
                   KernelCall& c);
 double rectify_bytes(const vpb_frame_fmt* frames, const vpb_rectify* const* rect, int n);
 
+// The lateral post-process (lateral.cu).  lateral_call: the checked launch of vpb_lateral_update_cameras (threshold
+// 0.5f on vpb_lane_masks' output) and of vpb_lateral_update_logits (the EgoLanes logits with the engine's threshold):
+// camera k reads st_in[k] and writes states[k] (st_in == states: in place) and outs[k]; launched without PDL.
+// VPB_ERR_ARG, the message prefixed with who, as those entry points document.  kLatMaxImgH: the tallest source frame it
+// takes.
+static constexpr int kLatMaxImgH = 4320;
+int lateral_call(const char* who, const float* masks, float threshold, int n, int H, int W, const int* img_w,
+                 const int* img_h, float smoothing, const double* homographies, const double* steering,
+                 const vpb_lateral_state* st_in, vpb_lateral_state* states, vpb_lateral_out* outs, KernelCall& c);
+
 // JPEG frames (jpeg.cu).  jpeg_frame_check: the host header parse of a VPB_PIX_JPEG descriptor (frame_fmt_check's JPEG
 // case): VPB_ERR_ARG "<who>: frame <k>: ..." for a stream the decoder does not take or an h x w other than the SOF's.
 // no_jpeg: VPB_ERR_ARG for a JPEG descriptor among device frames (their headers cannot be parsed on the host).

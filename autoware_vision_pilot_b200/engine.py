@@ -56,6 +56,12 @@ class _Stats(C.Structure):
                 ("shared_encoders", C.c_int), ("shared_trunks", C.c_int), ("reference_flops", C.c_double)]
 
 
+class LateralConfig(C.Structure):
+    """Mirror of vp_lateral_config (include/vp_b200.h)."""
+
+    _fields_ = [("threshold", C.c_float), ("smoothing", C.c_float), ("homographies", C.POINTER(C.c_double))]
+
+
 class _TapView(C.Structure):
     _fields_ = [("data", C.c_void_p), ("height", C.c_int), ("width", C.c_int), ("channels", C.c_int),
                 ("ld", C.c_int), ("pad", C.c_int), ("dtype", C.c_int)]
@@ -108,6 +114,11 @@ def _bind():
     lib.vp_engine_kernel_names.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int)]
     lib.vp_engine_time_kernel.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_double),
                                           C.POINTER(C.c_double), C.POINTER(C.c_int)]
+    lib.vp_engine_set_lateral.argtypes = [C.c_void_p, C.c_int, C.POINTER(LateralConfig)]
+    lib.vp_engine_set_steering.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+    lib.vp_engine_lateral_reset.argtypes = [C.c_void_p, C.c_int]
+    lib.vp_engine_lateral.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.vp_engine_graph_captures.argtypes = [C.c_void_p]
     _bound = True
     return lib
 
@@ -159,6 +170,72 @@ class Engine:
         L.check(self._lib.vp_engine_set_rectify(self._h, sample, r.handle if r is not None else None),
                 "vp_engine_set_rectify")
         self._rectify[sample] = r
+
+    # ---- the lateral post-process inside the call
+    def set_lateral(self, model_idx: Optional[int], threshold: float = 0.0, smoothing: float = 0.5,
+                    homographies=None) -> None:
+        """Run LaneFilter -> LaneTracker -> PathFinder on EgoLanes model model_idx's logits inside every later call, one
+        state per sample, each sample with its own source size (fresh states; model_idx None: off).  threshold: the
+        EgoLanes inference threshold on the logits; smoothing: LaneFilter's factor in [0, 1]; homographies: None (the
+        reference matrix) or one 3x3 / 9-value orig -> BEV matrix per sample.  Results: lateral(k) / lateral_dev(k)."""
+        if model_idx is None:
+            L.check(self._lib.vp_engine_set_lateral(self._h, 0, None), "vp_engine_set_lateral")
+            return
+        if not 0 <= model_idx < len(self.kinds) or self.kinds[model_idx] != EGO_LANES:
+            raise ValueError(f"model {model_idx} is not an EgoLanes model of this engine (kinds {self.kinds})")
+        if not 0.0 <= smoothing <= 1.0:
+            raise ValueError(f"smoothing {smoothing} is outside [0, 1]")
+        cfg = LateralConfig(float(threshold), float(smoothing), None)
+        if homographies is not None:
+            h = np.asarray(homographies, dtype=np.float64)
+            if h.size != 9 * self.batch:
+                raise ValueError(f"need {self.batch} homographies of 9 values, got shape {h.shape}")
+            hom = (C.c_double * h.size)(*h.reshape(-1).tolist())
+            cfg.homographies = C.cast(hom, C.POINTER(C.c_double))
+        L.check(self._lib.vp_engine_set_lateral(self._h, model_idx, C.byref(cfg)), "vp_engine_set_lateral")
+
+    def set_steering(self, values: Optional[Sequence[float]]) -> None:
+        """The AutoSteer steering angle (rad) of each of the `batch` samples for every later call (None: 0)."""
+        arr = None
+        if values is not None:
+            values = list(values)
+            if len(values) != self.batch:
+                raise ValueError(f"{len(values)} steering values for an engine of batch {self.batch}")
+            arr = (C.c_double * self.batch)(*[float(v) for v in values])
+        L.check(self._lib.vp_engine_set_steering(self._h, arr), "vp_engine_set_steering")
+
+    def lateral_reset(self, sample: Optional[int] = None) -> None:
+        """A fresh lateral state for sample `sample` (None: every sample) from the next call on."""
+        s = -1 if sample is None else int(sample)
+        if not -1 <= s < self.batch:
+            raise ValueError(f"sample {sample} of a batch of {self.batch}")
+        L.check(self._lib.vp_engine_lateral_reset(self._h, s), "vp_engine_lateral_reset")
+
+    def _lateral(self, sample: int):
+        if not 0 <= sample < self.batch:
+            raise ValueError(f"sample {sample} of a batch of {self.batch}")
+        host, dev = C.c_void_p(), C.c_void_p()
+        L.check(self._lib.vp_engine_lateral(self._h, sample, C.byref(host), C.byref(dev)), "vp_engine_lateral")
+        return host.value, dev.value
+
+    def lateral(self, sample: int = 0) -> dict:
+        """Sample `sample`'s vpb_lateral_out record of the last host call as a dict (after sync() for a submit)."""
+        from .lateral import _record
+        host, _ = self._lateral(sample)
+        if not host:
+            raise RuntimeError("lateral record: the last call was a device call, use lateral_dev()")
+        return _record(C.string_at(host, C.sizeof(L.LateralOut)))
+
+    def lateral_dev(self, sample: int = 0) -> int:
+        """Device address of sample `sample`'s vpb_lateral_out record of the last call."""
+        return self._lateral(sample)[1]
+
+    def graph_captures(self) -> int:
+        """How many times the frame graph has been captured."""
+        n = self._lib.vp_engine_graph_captures(self._h)
+        if n < 0:
+            raise RuntimeError(L.last_error())
+        return n
 
     # ---- inference
     @staticmethod

@@ -170,8 +170,10 @@ class MultiCamera:
         """Enqueue pack -> ncclAllGather -> Estimator::update (device pointers; asynchronous)."""
         L.check(self._lib.vp_multicam_step(self._h, feat_ptr, meas_ptr, int(predict)), "vp_multicam_step")
 
-    def step_engine(self, engine, model_idx: int, lateral_out_ptr: int, predict: bool = True) -> None:
-        """feat = the engine's "<model_idx>/fused" tensor, meas = vpb_lateral_out.pf_meas (device)."""
+    def step_engine(self, engine, model_idx: int, lateral_out_ptr: Optional[int] = None, predict: bool = True) -> None:
+        """feat = the engine's "<model_idx>/fused" tensor, meas = vpb_lateral_out.pf_meas (device) of the records at
+        lateral_out_ptr, or (None) of those the engine's own lateral post-process made in its last call
+        (Engine.set_lateral on model_idx)."""
         L.check(self._lib.vp_multicam_step_engine(self._h, engine.handle, model_idx, lateral_out_ptr, int(predict)),
                 "vp_multicam_step_engine")
 

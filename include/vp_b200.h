@@ -167,8 +167,42 @@ int vp_engine_infer_device_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_
  * whose h x w is not the map's source size returns VPB_ERR_ARG naming the call and the frame, before any device work.
  * r NULL clears the sample's map.  VPB_ERR_ARG for a sample outside 0 .. batch-1 or a map created on another GPU.  The
  * engine keeps the pointer: r must outlive every call that uses it.  The lateral post-process of a rectified camera
- * takes the map's size as its image size. */
+ * takes the map's size as its image size: the in-call one (vp_engine_set_lateral) does so by itself. */
 int vp_engine_set_rectify(vp_engine* e, int sample, const vpb_rectify* r);
+
+/* The lateral post-process inside the call (production_release/main.cpp:505-577: EgoLanes -> LaneFilter ->
+ * LaneTracker -> PathFinder, per camera).  With it set on EgoLanes model model_idx, every later call of every form
+ * appends the op "lateral" (kernel lateral_kernel) right after that model's final op, on its lane: sample k's logits
+ * are thresholded (raw > threshold) as they are read, and sample k's vpb_lateral_state advances exactly once per call.
+ * Sample k's image size is its source size: the frame's h x w, a JPEG frame's SOF size, a rectified sample's map size.
+ * Sample k's record is byte-identical to vpb_lane_masks + vpb_lateral_update_cameras on the call's raw tensor
+ * (vp_output.raw_dev) with that size, on a state of its own.  Launches that repeat the op outside a call
+ * (vp_engine_profile, vp_engine_time_kernel) leave the states and records of the last call as they were.
+ *   vp_engine_set_lateral   cfg NULL: off (model_idx is not read); otherwise on, or reconfigured, with every sample's
+ *                           state fresh (LaneFilter::reset, a new LaneTracker and PathFinder).  Either way the captured
+ *                           graph is dropped.  VPB_ERR_ARG for a NULL engine, a model that is not EgoLanes or smoothing
+ *                           outside [0, 1].
+ *   vp_engine_set_steering  the AutoSteer steering angle (rad) PathFinder takes for each of the `batch` samples in
+ *                           every later call (NULL: 0); the frame graph re-points the op, it does not capture again.
+ *   vp_engine_lateral_reset sample `sample`'s state (-1: every sample) fresh before the next call.  VPB_ERR_ARG for a
+ *                           sample outside -1 .. batch-1, VPB_ERR_STATE while the feature is off.
+ *   vp_engine_lateral       sample `sample`'s record of the last call: host = an engine-owned pinned copy made by the
+ *                           host calls (valid after the call, or after vp_engine_sync for submit), NULL after a device
+ *                           call; dev = the device record.  Both stay valid until the next call.  Either out pointer
+ *                           may be NULL.  VPB_ERR_ARG for a NULL engine or a sample out of range, VPB_ERR_STATE while
+ *                           the feature is off or before its first call.
+ * Every call then checks, before any device work, that no sample's source is taller than 4320 rows (VPB_ERR_ARG naming
+ * the call and the frame).  With the feature off the launch list, the graph and every launch are as without it.  The
+ * split-fp16 engine (batch 1) takes it too. */
+typedef struct {
+  float threshold;                  /* EgoLanes*Engine::inference threshold (reference default 0.0) */
+  float smoothing;                  /* LaneFilter smoothing factor, [0, 1] */
+  const double* homographies;       /* host, batch*9 orig -> BEV, copied; NULL = the reference matrix for every sample */
+} vp_lateral_config;
+int vp_engine_set_lateral(vp_engine* e, int model_idx, const vp_lateral_config* cfg);
+int vp_engine_set_steering(vp_engine* e, const double* steering_rad);
+int vp_engine_lateral_reset(vp_engine* e, int sample);
+int vp_engine_lateral(vp_engine* e, int sample, const vpb_lateral_out** host, const vpb_lateral_out** dev);
 /* Copy the raw fp32 tensor of one model to its host buffer (after a device/async inference). */
 int vp_engine_fetch_raw(vp_engine* e, int model_idx);
 
@@ -239,6 +273,9 @@ int vp_engine_time_kind(vp_engine* e, int kind, int reps, float* ms, double* flo
 int vp_engine_kernel_names(vp_engine* e, const char** names, int cap, int* n);
 int vp_engine_time_kernel(vp_engine* e, const char* kname, int reps, float* ms, double* flops, double* bytes,
                           int* launches);
+/* How many times the frame graph has been captured since the engine was created (a call that only re-points captured
+ * nodes does not count); VPB_ERR_ARG for a NULL engine. */
+int vp_engine_graph_captures(const vp_engine* e);
 
 /* Intermediate activations for the per-tap parity tests: copies tensor `name`
  * ("<model_idx>/f0".."f4", "context", "neck", "pre") to host as fp32 NCHW. Returns element count.

@@ -67,7 +67,8 @@ int vp_multicam_reset(vp_multicam* mc);
  * [n][14][2]; all n are packed by one launch and fused in camera order, without a collective. */
 int vp_multicam_step(vp_multicam* mc, const void* feat_dev, const double* meas_dev, int predict);
 /* Convenience for the engine: feat = tensor "<model_idx>/fused" of an EgoLanes model, meas =
- * lat_out_dev->pf_meas (vpb_lateral_update's output record, device).
+ * lat_out_dev->pf_meas (vpb_lateral_update's output record, device).  lat_out_dev NULL: the records the engine's own
+ * lateral post-process made in its last call (vp_engine_set_lateral on model_idx; VPB_ERR_ARG without it).
  * Local mode: the engine's batch must equal n; camera k's features are tensor "<model_idx>/fused@k" and its
  * measurement is lat_out_dev[k].pf_meas (the n records of vpb_lateral_update_batch).  A batch mismatch or a model
  * without a "fused" tensor is VPB_ERR_ARG. */

@@ -490,6 +490,14 @@ int vpb_lateral_update_batch(const float* masks, int n, int H, int W, int img_w,
 int vpb_lateral_update_cameras(const float* masks, int n, int H, int W, const int* img_w, const int* img_h,
                                float smoothing, const double* homographies, const double* steering_rad,
                                vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream);
+/* vpb_lateral_update_cameras on the EgoLanes logits themselves: raw is the model's fp32 output [n][3][H][W] and a mask
+ * pixel is set where raw > threshold (EgoLanes*Engine::inference's threshold).  States and records are byte-identical
+ * to vpb_lane_masks(raw, n*3*H*W, threshold) followed by vpb_lateral_update_cameras on its output, for every float
+ * (NaN and -0.0 included), without the float mask buffer and its launch.  Same checks and messages as
+ * vpb_lateral_update_cameras.  This is the launch the engine's in-call lateral op makes (vp_engine_set_lateral). */
+int vpb_lateral_update_logits(const float* raw, int n, int H, int W, float threshold, const int* img_w,
+                              const int* img_h, float smoothing, const double* homographies, const double* steering_rad,
+                              vpb_lateral_state* states_dev, vpb_lateral_out* outs_dev, void* stream);
 
 /* ---- AutoSteer boundary (SURVEY.md 8f rank 2) ----
  * The AutoSteer v1 network itself (ONNX [1,6,80,160] -> 2 x [1,61]) is not in the reference repository

@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -60,8 +61,13 @@ class AutoSpeedEngine:
                                                     C.byref(self._h)), "vp_autospeed_create_batch")
         self.batch = batch
         self._rectify = {}
+        self._engines = weakref.WeakSet()    # segmentation engines this detector is attached to (Engine.set_detector)
 
     def close(self):
+        """Detach from every engine that runs this detector in its call, then free it."""
+        for eng in list(getattr(self, "_engines", ())):
+            if eng._h.value and eng._detector is self:
+                eng.set_detector(None)
         if getattr(self, "_h", None) and self._h.value:
             self._lib.vp_autospeed_destroy(self._h)
             self._h = C.c_void_p()
@@ -191,6 +197,10 @@ class AutoSpeedEngine:
         L.check(self._lib.vp_autospeed_raw_at(self._h, sample, C.byref(rh), None, C.byref(ch), C.byref(na)),
                 "vp_autospeed_raw_at")
         return np.ctypeslib.as_array(rh, shape=(ch.value, na.value)).copy()
+
+    @property
+    def handle(self) -> C.c_void_p:
+        return self._h
 
     def stats(self) -> dict:
         n, f = C.c_int(), C.c_double()

@@ -473,14 +473,16 @@ static int as_decode_x(int dt, const void* lvl, int h, int w, int ld, float stri
 }
 
 // Every buffer holds NA entries per image, so no candidate and no detection is ever cut; the dead flags (one byte per
-// candidate) live in shared memory, NA <= kNA keeps them under the 48 KB default.
-static int as_postprocess_x(const float* raw, int NA, int nb, float conf, float iou, const float* scale, const int* pad_x,
-                            const int* pad_y, const int* orig_w, const int* orig_h, float* cand, int* order, float* det,
-                            int* counts, cudaStream_t st) {
+// candidate) live in shared memory, NA <= kNA keeps them under the 48 KB default.  as_postprocess_call describes the
+// launch, as_postprocess_x launches it.
+static int as_postprocess_call(const float* raw, int NA, int nb, float conf, float iou, const float* scale,
+                               const int* pad_x, const int* pad_y, const int* orig_w, const int* orig_h, float* cand,
+                               int* order, float* det, int* counts, KernelCall& c) {
   const char* op = "as_postprocess";
   if (!batch_ok(op, nb) || !ptrs_ok(op, {raw, scale, pad_x, pad_y, orig_w, orig_h, cand, order, det, counts})) return VPB_ERR_ARG;
   if (NA < 1 || NA > kNA) { vpb_set_error("%s: NA=%d (1..%d)", op, NA, kNA); return VPB_ERR_ARG; }
-  PostParams pp{};
+  PostParams pp;
+  memset(&pp, 0, sizeof(pp));              // the padding compares equal (KernelCall)
   pp.raw = raw; pp.NA = NA; pp.conf = conf; pp.iou = iou;
   for (int k = 0; k < nb; ++k) {
     if (!(scale[k] > 0.f)) { vpb_set_error("%s: image %d: scale %g", op, k, scale[k]); return VPB_ERR_ARG; }
@@ -489,8 +491,19 @@ static int as_postprocess_x(const float* raw, int NA, int nb, float conf, float 
   pp.max_cand = NA; pp.max_det = NA;
   pp.cand = cand; pp.order = order; pp.det = det; pp.counts = counts;
   const size_t smem = NA;                      // s_dead
-  if (nb > 1) VPB_CUDA_OK(launch_k(postprocess_kernel<true>, dim3(nb), dim3(1024), smem, st, pp));
-  else VPB_CUDA_OK(launch_k(postprocess_kernel<false>, dim3(1), dim3(1024), smem, st, pp));
+  if (nb > 1) c.set_kernel(postprocess_kernel<true>, dim3(nb), dim3(1024), smem, true, pp);
+  else c.set_kernel(postprocess_kernel<false>, dim3(1), dim3(1024), smem, true, pp);
+  return VPB_OK;
+}
+
+static int as_postprocess_x(const float* raw, int NA, int nb, float conf, float iou, const float* scale, const int* pad_x,
+                            const int* pad_y, const int* orig_w, const int* orig_h, float* cand, int* order, float* det,
+                            int* counts, cudaStream_t st) {
+  KernelCall c;
+  const int rc = as_postprocess_call(raw, NA, nb, conf, iou, scale, pad_x, pad_y, orig_w, orig_h, cand, order, det,
+                                     counts, c);
+  if (rc) return rc;
+  VPB_CUDA_OK(c.launch(st));
   return VPB_OK;
 }
 
@@ -515,9 +528,11 @@ struct vp_autospeed : EngineRuntime {
   // others of a sample that has more, after the call has completed.
   static constexpr int kDetFetch = 1024;
 
-  int geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) override;
+  int geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, const char* who, PreGeom* g) override;
   int enqueue(const PreGeom* g) override;
-  int fetch(bool raw) override;
+  int fetch(bool raw) override { return fetch_on(raw, stream); }
+  int letterbox(const PreGeom* g, cudaStream_t st);
+  int fetch_on(bool raw, cudaStream_t st);
   int fetch_rest();
 };
 
@@ -716,6 +731,17 @@ struct ASBuilder {
   }
 };
 
+// The NMS launch of a call: the thresholds and the letterboxes (pre.geom, scale) as they are when it is described
+static int as_post_describe(const vp_autospeed* ep, KernelCall& c) {
+  int pad_x[kMaxBatch], pad_y[kMaxBatch], orig_w[kMaxBatch], orig_h[kMaxBatch];
+  for (int k = 0; k < ep->batch; ++k) {
+    const PreGeom& g = ep->pre.geom[k];
+    pad_x[k] = g.x0; pad_y[k] = g.y0; orig_w[k] = g.w; orig_h[k] = g.h;
+  }
+  return as_postprocess_call(ep->d_raw, kNA, ep->batch, ep->conf, ep->iou, ep->scale, pad_x, pad_y, orig_w, orig_h,
+                             ep->d_cand, ep->d_order, ep->d_det, ep->d_counts, c);
+}
+
 static int as_build(vp_autospeed& e, const WeightMap& w) {
   ASBuilder b{e, w};
   const int W0 = kASW, H0 = kASH;
@@ -808,14 +834,12 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   // ---- NMS and the map back to each source frame, with the thresholds and letterboxes of the call
   {
     vp_autospeed* ep = &e;
-    e.add_op("postprocess", "postprocess_kernel", [ep](cudaStream_t st) {
-      int pad_x[kMaxBatch], pad_y[kMaxBatch], orig_w[kMaxBatch], orig_h[kMaxBatch];
-      for (int k = 0; k < ep->batch; ++k) {
-        const PreGeom& g = ep->pre.geom[k];
-        pad_x[k] = g.x0; pad_y[k] = g.y0; orig_w[k] = g.w; orig_h[k] = g.h;
-      }
-      return as_postprocess_x(ep->d_raw, kNA, ep->batch, ep->conf, ep->iou, ep->scale, pad_x, pad_y, orig_w, orig_h,
-                              ep->d_cand, ep->d_order, ep->d_det, ep->d_counts, st);
+    e.add_op("postprocess", "postprocess_kernel", [ep](cudaStream_t st) -> int {
+      KernelCall c;
+      const int rc = as_post_describe(ep, c);
+      if (rc) return rc;
+      VPB_CUDA_OK(c.launch(st));
+      return VPB_OK;
     });
   }
   e.tap("p1", p1); e.tap("p2", p2); e.tap("p3", p3); e.tap("p4", p4); e.tap("p5_ctx", q5); e.tap("p5_sppf", s5);
@@ -831,7 +855,7 @@ static double as_scale(int h, int w) { return std::min(static_cast<double>(kASW)
 }  // namespace vpb
 
 // letterbox geometry of every frame; VPB_ERR_ARG (naming `who` and the frame) if one cannot be resized.  Host-only.
-int vp_autospeed::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
+int vp_autospeed::geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt*, const char* who, PreGeom* g) {
   for (int k = 0; k < batch; ++k) {
     const int h = frames[k].h, w = frames[k].w;
     const double sc = as_scale(h, w);
@@ -845,10 +869,9 @@ int vp_autospeed::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g
   return VPB_OK;
 }
 
-// Enqueue one call for the batch frames f[0 .. batch-1]: tables for the call's letterboxes; the gray border of a
-// sample's canvas is refilled only when its letterbox changed (the pre-process overwrites the pasted region on every
-// call).
-int vp_autospeed::enqueue(const PreGeom* g) {
+// Tables for the call's letterboxes g; the gray border of a sample's canvas is refilled on st only when its letterbox
+// changed (the pre-process overwrites the pasted region on every call).
+int vp_autospeed::letterbox(const PreGeom* g, cudaStream_t st) {
   int rc = pre.configure(g, batch, VPB_RESIZE_PIL_BILINEAR);
   if (rc) return rc;
   const int npix = kASW * kASH;
@@ -858,21 +881,27 @@ int vp_autospeed::enqueue(const PreGeom* g) {
     void* c = static_cast<uint8_t*>(d_canvas) + static_cast<size_t>(npix) * 8 * 2 * k;
     dispatch_dtype(dtype, [&](auto tag) {
       using E = decltype(tag);
-      fill_canvas_kernel<E><<<(npix + 255) / 256, 256, 0, stream>>>(static_cast<typename E::T*>(c), npix);
+      fill_canvas_kernel<E><<<(npix + 255) / 256, 256, 0, st>>>(static_cast<typename E::T*>(c), npix);
     });
     VPB_CUDA_OK(cudaGetLastError());
     canvas_geom[k] = g[k];
   }
-  return run_call();
+  return VPB_OK;
 }
 
-// detections (and with raw the raw tensors) of every sample to the host buffers
-int vp_autospeed::fetch(bool raw) {
+// Enqueue one call for the batch frames: the letterboxes, then the launch list
+int vp_autospeed::enqueue(const PreGeom* g) {
+  const int rc = letterbox(g, stream);
+  return rc ? rc : run_call();
+}
+
+// detections (and with raw the raw tensors) of every sample to the host buffers, on st
+int vp_autospeed::fetch_on(bool raw, cudaStream_t st) {
   const size_t nb = batch;
-  VPB_CUDA_OK(cudaMemcpyAsync(h_counts, d_counts, 8 * nb, cudaMemcpyDeviceToHost, stream));
+  VPB_CUDA_OK(cudaMemcpyAsync(h_counts, d_counts, 8 * nb, cudaMemcpyDeviceToHost, st));
   const size_t pitch = static_cast<size_t>(kNA) * 6 * 4;
-  VPB_CUDA_OK(cudaMemcpy2DAsync(h_det, pitch, d_det, pitch, static_cast<size_t>(kDetFetch) * 6 * 4, nb, cudaMemcpyDeviceToHost, stream));
-  if (raw) VPB_CUDA_OK(cudaMemcpyAsync(h_raw, d_raw, static_cast<size_t>(8) * kNA * 4 * nb, cudaMemcpyDeviceToHost, stream));
+  VPB_CUDA_OK(cudaMemcpy2DAsync(h_det, pitch, d_det, pitch, static_cast<size_t>(kDetFetch) * 6 * 4, nb, cudaMemcpyDeviceToHost, st));
+  if (raw) VPB_CUDA_OK(cudaMemcpyAsync(h_raw, d_raw, static_cast<size_t>(8) * kNA * 4 * nb, cudaMemcpyDeviceToHost, st));
   return VPB_OK;
 }
 
@@ -892,6 +921,37 @@ int vp_autospeed::fetch_rest() {
 }
 
 namespace vpb {
+
+const EngineRuntime* autospeed_runtime(const vp_autospeed* d) { return d; }
+
+int autospeed_geoms(vp_autospeed* d, const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
+  return d->geoms(frames, frames, who, g);
+}
+
+int autospeed_prepare(vp_autospeed* d, const PreGeom* g, cudaStream_t st) { return d->letterbox(g, st); }
+
+int autospeed_letterbox(const vp_autospeed* d, const vpb_frame_fmt* frames, int bgr, KernelCall& c) {
+  return d->pre.describe(frames, bgr ? kConvBgrUnit : VPB_CONV_RGB_UNIT, d->dtype, d->d_canvas, nullptr, c);
+}
+
+std::vector<OpRec> autospeed_net_ops(const vp_autospeed* d) {
+  std::vector<OpRec> v;
+  for (size_t i = d->op_index("preprocess") + 1; i < d->ops.size(); ++i) {
+    OpRec op = d->ops[i];
+    op.name = "det/" + op.name;
+    op.conv = -1;                          // its plan is the detector's
+    if (d->ops[i].name == "postprocess") {
+      op.launch = nullptr;
+      op.describe = [d](KernelCall& c) { return as_post_describe(d, c); };
+    }
+    v.push_back(std::move(op));
+  }
+  return v;
+}
+
+int autospeed_fetch(vp_autospeed* d, bool raw, cudaStream_t st) { return d->fetch_on(raw, st); }
+
+int autospeed_fetch_rest(vp_autospeed* d) { return d->fetch_rest(); }
 
 static int as_create(const char* who, const char* weights_vpw, int gpu_id, int dtype, void* stream, int batch,
                      vp_autospeed** out) {

@@ -114,8 +114,12 @@ struct vp_engine : EngineRuntime {
   int lat_cur = 0;
   bool lat_ready = false;                  // a call has made records since the feature was set
   bool lat_host = false;                   // the last call was a host call: h_lat_out is current
+  // The detector inside the call (vp_engine_set_detector): op "det/letterbox" and copies of det's ops on lane
+  // front_lane, before the lanes' join; det_geom are its letterboxes of the current call.
+  vp_autospeed* det = nullptr;
+  PreGeom det_geom[kMaxBatch];
 
-  int geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) override;
+  int geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, const char* who, PreGeom* g) override;
   int enqueue(const PreGeom* g) override;
   int fetch(bool raw) override;
 };
@@ -634,9 +638,9 @@ static int check_source_flags(const vp_engine_config& c) {
 
 // Every frame resizes to the 640 x 320 network input: VPB_ERR_ARG (naming `who` and the frame) if one cannot in the
 // engine's resize mode, or if the engine makes overlays and the frame is not packed (the overlay blends the camera
-// frame's pixels as vpb_src_job reads them; a rectified sample's frame here is the packed rectified frame).  Host-only:
-// callers run it before any device work.
-int vp_engine::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
+// frame's pixels as vpb_src_job reads them; a rectified sample's frame here is the packed rectified frame).  With a
+// detector, its letterboxes of the full frames.  Host-only: callers run it before any device work.
+int vp_engine::geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, const char* who, PreGeom* g) {
   for (int k = 0; k < batch; ++k) {
     if (lat_model >= 0 && frames[k].h > kLatMaxImgH) {
       vpb_set_error("%s: frame %d: height %d is above the %d rows the lateral post-process takes", who, k, frames[k].h,
@@ -653,7 +657,7 @@ int vp_engine::geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) {
     const int rc = PreprocessPlan::check(g[k], cfg.resize_mode, who, k);
     if (rc) return rc;
   }
-  return VPB_OK;
+  return det ? autospeed_geoms(det, full, who, det_geom) : VPB_OK;
 }
 
 // Enqueue one call's kernels for the batch frames of the call (graph replay when enabled and the geometries are
@@ -663,6 +667,12 @@ int vp_engine::enqueue(const PreGeom* g) {
   lat_host = false;
   int rc = pre.configure(g, batch, cfg.resize_mode);
   if (rc == VPB_OK && !src_outs.empty()) rc = prepare_source(*this);
+  if (rc == VPB_OK && det) {
+    rc = autospeed_prepare(det, det_geom, stream);
+    double bytes = 0;   // as the detector's own pre-process: frame read + 3 x OH x OW 16-bit written, per sample
+    for (int k = 0; k < batch; ++k) bytes += frame_bytes(chain[k].full()) + 2.0 * 3 * det_geom[k].OH * det_geom[k].OW;
+    ops[op_index("det/letterbox")].bytes = bytes;
+  }
   if (rc == VPB_OK) rc = run_call();
   if (rc == VPB_OK) src_ready = true;
   if (rc == VPB_OK && lat_model >= 0) { lat_cur ^= 1; lat_ready = true; }
@@ -691,7 +701,7 @@ int vp_engine::fetch(bool raw) {
                                 cudaMemcpyDeviceToHost, stream));
     lat_host = true;
   }
-  return VPB_OK;
+  return det ? autospeed_fetch(det, raw || cfg.fetch_raw, stream) : VPB_OK;
 }
 
 // ====================================================================== C-ABI
@@ -794,11 +804,18 @@ extern "C" int vp_engine_sync(vp_engine* e) {
   return VPB_OK;
 }
 
+// A host call; a synchronous one also copies an attached detector's detections past the first 1024 of a sample
+template <class F>
+static int host_call(vp_engine* e, const F* frames, int n, bool sync, const char* who) {
+  const int rc = call_host(e, frames, n, sync, false, who);
+  return rc || !sync || !e->det ? rc : autospeed_fetch_rest(e->det);
+}
+
 static int submit_host_batch(vp_engine* e, const uint8_t* const* frames, int n, int h, int w, int stride, bool sync) {
   const char* who = sync ? "vp_engine_infer" : "vp_engine_submit";
   Frames f;
   if (!batch_frames(e, frames, n, h, w, stride, who, f)) return VPB_ERR_ARG;
-  return call_host(e, f.data(), n, sync, false, who);
+  return host_call(e, f.data(), n, sync, who);
 }
 
 extern "C" int vp_engine_infer(vp_engine* e, const uint8_t* frame_host, int h, int w, int stride) {
@@ -818,19 +835,19 @@ extern "C" int vp_engine_submit_batch(vp_engine* e, const uint8_t* const* frames
 }
 
 extern "C" int vp_engine_infer_frames(vp_engine* e, const vpb_frame* frames_host, int n) {
-  return call_host(e, frames_host, n, true, false, "vp_engine_infer_frames");
+  return host_call(e, frames_host, n, true, "vp_engine_infer_frames");
 }
 
 extern "C" int vp_engine_submit_frames(vp_engine* e, const vpb_frame* frames_host, int n) {
-  return call_host(e, frames_host, n, false, false, "vp_engine_submit_frames");
+  return host_call(e, frames_host, n, false, "vp_engine_submit_frames");
 }
 
 extern "C" int vp_engine_infer_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n) {
-  return call_host(e, frames_host, n, true, false, "vp_engine_infer_frames_fmt");
+  return host_call(e, frames_host, n, true, "vp_engine_infer_frames_fmt");
 }
 
 extern "C" int vp_engine_submit_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_host, int n) {
-  return call_host(e, frames_host, n, false, false, "vp_engine_submit_frames_fmt");
+  return host_call(e, frames_host, n, false, "vp_engine_submit_frames_fmt");
 }
 
 extern "C" int vp_engine_infer_device_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_dev, int n) {
@@ -841,6 +858,67 @@ extern "C" int vp_engine_set_rectify(vp_engine* e, int sample, const vpb_rectify
   if (!e) { vpb_set_error("vp_engine_set_rectify: NULL engine"); return VPB_ERR_ARG; }
   DeviceGuard guard(e->gpu_id);
   return e->set_rectify(sample, r, "vp_engine_set_rectify");
+}
+
+extern "C" int vp_engine_set_roi(vp_engine* e, int sample, int x, int y, int w, int h) {
+  if (!e) { vpb_set_error("vp_engine_set_roi: NULL engine"); return VPB_ERR_ARG; }
+  return e->set_roi(sample, x, y, w, h, "vp_engine_set_roi");
+}
+
+// ---------------------------------------------------------------- the detector inside the call
+// Op "det/letterbox": the detector's letterbox of every sample's full() frame, B, G, R under the BGR conventions.
+static OpRec letterbox_op(vp_engine& e) {
+  OpRec op;
+  op.name = "det/letterbox"; op.kname = "preprocess"; op.lane = e.front_lane;
+  vp_engine* ep = &e;
+  op.describe = [ep](KernelCall& c) {
+    Frames f{};
+    for (int k = 0; k < ep->batch; ++k) f[k] = ep->chain[k].full();
+    return autospeed_letterbox(ep->det, f.data(), ep->rect_bgr, c);
+  };
+  return op;
+}
+
+extern "C" int vp_engine_set_detector(vp_engine* e, vp_autospeed* det) {
+  const char* who = "vp_engine_set_detector";
+  if (!e) { vpb_set_error("%s: NULL engine", who); return VPB_ERR_ARG; }
+  if (det) {
+    const EngineRuntime* d = autospeed_runtime(det);
+    if (d->batch != e->batch) {
+      vpb_set_error("%s: the detector has batch %d, the engine batch %d", who, d->batch, e->batch);
+      return VPB_ERR_ARG;
+    }
+    if (d->gpu_id != e->gpu_id) {
+      vpb_set_error("%s: the detector lives on GPU %d, the engine on GPU %d", who, d->gpu_id, e->gpu_id);
+      return VPB_ERR_ARG;
+    }
+  }
+  DeviceGuard guard(e->gpu_id);
+  const int at = e->op_index("det/letterbox");
+  if (at >= 0) {                           // detach: the detector's ops and its lane go
+    size_t m = 0;
+    while (at + m < e->ops.size() && e->ops[at + m].name.compare(0, 4, "det/") == 0) ++m;
+    e->set_lane_dep(e->front_lane, -1);   // drops the event of its fork op
+    e->erase_ops(at, m);
+    e->lane_dep.pop_back();
+    e->call_start.reset();
+    e->front_lane = 0;
+  }
+  e->det = nullptr;
+  e->n_frames = 0;                         // profiling and timing wait for a call on the new op list
+  if (!det) return VPB_OK;
+  e->det = det;
+  e->front_lane = static_cast<int>(e->lane_dep.size());
+  e->lane_dep.push_back(-1);
+  std::vector<OpRec> add{letterbox_op(*e)};
+  for (OpRec& op : autospeed_net_ops(det)) {
+    op.lane = e->front_lane;
+    add.push_back(std::move(op));
+  }
+  const int src = e->op_index("source_outputs");   // the only op after the lanes' join
+  e->insert_ops(src >= 0 ? src : e->ops.size(), std::move(add));
+  e->sync_front_ops();                     // the lane's fork
+  return VPB_OK;
 }
 
 // ---------------------------------------------------------------- the lateral post-process inside the call

@@ -113,7 +113,8 @@ static bool same_geometry(const vpb_frame_fmt& a, const vpb_frame_fmt& b) {
 int FrameGraph::run(EngineRuntime& e) {
   const cudaStream_t st = e.stream;
   bool same_geom = exec && n == e.n_frames;
-  for (int k = 0; k < e.n_frames && same_geom; ++k) same_geom = same_geometry(geom[k], e.chain[k].pre());
+  for (int k = 0; k < e.n_frames && same_geom; ++k)
+    same_geom = same_geometry(geom[k], e.chain[k].pre()) && same_geometry(geom_full[k], e.chain[k].full());
   if (same_geom) {
     KernelCall c;
     for (Node& r : nodes) {
@@ -143,7 +144,7 @@ int FrameGraph::run(EngineRuntime& e) {
     if (graph) cudaGraphDestroy(graph);
     graph = g;
     if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    for (int k = 0; k < e.n_frames; ++k) geom[k] = e.chain[k].pre();
+    for (int k = 0; k < e.n_frames; ++k) { geom[k] = e.chain[k].pre(); geom_full[k] = e.chain[k].full(); }
     n = e.n_frames;
   }
   VPB_CUDA_OK(cudaGraphLaunch(exec, st));
@@ -276,8 +277,18 @@ vpb_frame_fmt SampleFrames::decoded() const {
   return given.format == VPB_PIX_JPEG ? packed_frame(vpb_frame{jpg.p, given.h, given.w, 3 * given.w}) : given;
 }
 
-vpb_frame_fmt SampleFrames::pre() const {
+vpb_frame_fmt SampleFrames::full() const {
   return map ? packed_frame(vpb_frame{rect.p, map->map_h, map->map_w, 3 * map->map_w}) : decoded();
+}
+
+vpb_frame_fmt SampleFrames::pre() const {
+  vpb_frame_fmt f = full();
+  if (!roi[2]) return f;
+  const int bpp = f.w > 0 ? frame_row_bytes(f) / f.w : 0;    // bytes per pixel of the main plane (NV12: the Y plane)
+  if (f.data) f.data += static_cast<size_t>(roi[1]) * f.stride + static_cast<size_t>(roi[0]) * bpp;
+  if (f.format == VPB_PIX_NV12 && f.uv) f.uv += static_cast<size_t>(roi[1] / 2) * f.uv_stride + roi[0];
+  f.w = roi[2]; f.h = roi[3];
+  return f;
 }
 
 // the samples of e with a map, in sample order: the frames the rectify op reads, their maps and outputs; the count
@@ -312,6 +323,20 @@ void EngineRuntime::erase_ops(size_t at, size_t m) {
   if (!op_events.empty()) op_events.erase(op_events.begin() + at, op_events.begin() + at + m);
   for (int& d : lane_dep)
     if (d >= static_cast<int>(at + m)) d -= static_cast<int>(m);
+}
+
+int EngineRuntime::set_roi(int sample, int x, int y, int w, int h, const char* who) {
+  if (sample < 0 || sample >= batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, batch); return VPB_ERR_ARG; }
+  const bool clear = w == 0 && h == 0;
+  if (!clear && (x < 0 || y < 0 || w <= 0 || h <= 0)) {
+    vpb_set_error("%s: sample %d: region %dx%d at (%d, %d) (need x, y >= 0 and w, h > 0, or w = h = 0 to clear)", who,
+                  sample, w, h, x, y);
+    return VPB_ERR_ARG;
+  }
+  int* r = chain[sample].roi;
+  r[0] = clear ? 0 : x; r[1] = clear ? 0 : y; r[2] = clear ? 0 : w; r[3] = clear ? 0 : h;
+  n_frames = 0;                           // the last call's frames are not those the pre-process now reads
+  return VPB_OK;
 }
 
 void EngineRuntime::sync_front_ops() {
@@ -355,6 +380,16 @@ void EngineRuntime::sync_front_ops() {
     const int n = rect_list(*this, f, m, o);
     ops[op_index("rectify")].bytes = rectify_bytes(f, m, n);
   }
+  if (front_lane > 0) set_lane_dep(front_lane, op_index("preprocess") - 1);   // the last front op, -1: none
+}
+
+void EngineRuntime::set_lane_dep(int lane, int dep) {
+  const int old = lane_dep[lane];
+  lane_dep[lane] = dep;
+  if (old < 0 || old == dep || old >= static_cast<int>(op_events.size())) return;
+  for (size_t l = 1; l < lane_dep.size(); ++l)
+    if (lane_dep[l] == old) return;
+  op_events[old].reset();
 }
 
 int EngineRuntime::grow(Scratch& s, size_t bytes) {
@@ -408,16 +443,24 @@ int EngineRuntime::reset_call(cudaStream_t st) {
   return VPB_OK;
 }
 
+// The lanes' streams and join events, and the event of each lane's fork (a lane added or removed after the first call,
+// front_lane's fork moving: the missing ones are made, a removed lane's stream is destroyed)
 static int prepare_lanes(EngineRuntime& e) {
   const size_t nl = e.lane_dep.size();
-  if (e.lane_streams.size() == nl) return VPB_OK;
-  e.lane_streams.assign(nl, nullptr);
+  while (e.lane_streams.size() > nl) {
+    if (e.lane_streams.back()) cudaStreamDestroy(e.lane_streams.back());
+    e.lane_streams.pop_back();
+    e.lane_done.pop_back();
+  }
+  e.lane_streams.resize(nl, nullptr);
   e.lane_done.resize(nl);
   e.op_events.resize(e.ops.size());
   for (size_t l = 1; l < nl; ++l) {
-    VPB_CUDA_OK(cudaStreamCreateWithFlags(&e.lane_streams[l], cudaStreamNonBlocking));
-    VPB_CUDA_OK(make_event(e.lane_done[l], cudaEventDisableTiming));
-    Event& dep = e.op_events[e.lane_dep[l]];
+    if (!e.lane_streams[l]) {
+      VPB_CUDA_OK(cudaStreamCreateWithFlags(&e.lane_streams[l], cudaStreamNonBlocking));
+      VPB_CUDA_OK(make_event(e.lane_done[l], cudaEventDisableTiming));
+    }
+    Event& dep = e.lane_dep[l] >= 0 ? e.op_events[e.lane_dep[l]] : e.call_start;
     if (!dep) VPB_CUDA_OK(make_event(dep, cudaEventDisableTiming));
   }
   return VPB_OK;
@@ -432,13 +475,15 @@ int EngineRuntime::launch_all(cudaStream_t st) {
     for (size_t i = 0; i < ops.size() && rc == VPB_OK; ++i) rc = launch_op(i, st);
     return rc;
   }
+  for (size_t l = 1; l < nl; ++l)
+    if (lane_dep[l] < 0) { VPB_CUDA_OK(cudaEventRecord(call_start.get(), st)); break; }
   std::vector<char> started(nl, 0);
   for (size_t i = 0; i < ops.size(); ++i) {
     const int lane = ops[i].lane;
     if (lane < 0) continue;                   // after the join
     cudaStream_t s = lane == 0 ? st : lane_streams[lane];
     if (lane > 0 && !started[lane]) {         // fork: wait for the producer of this lane's input
-      VPB_CUDA_OK(cudaStreamWaitEvent(s, op_events[lane_dep[lane]].get(), 0));
+      VPB_CUDA_OK(cudaStreamWaitEvent(s, lane_dep[lane] >= 0 ? op_events[lane_dep[lane]].get() : call_start.get(), 0));
       started[lane] = 1;
     }
     rc = launch_op(i, s);
@@ -512,21 +557,39 @@ bool frames_ok(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const
   return true;
 }
 
-// Host-only checks of the call's frames: a sample with a map needs a frame of the map's source size (VPB_ERR_ARG naming
-// who and the frame otherwise); then the engine's geometries g of what the pre-process will read.
+// Host-only checks of the call's frames (VPB_ERR_ARG naming who and the frame): a sample with a map needs a frame of the
+// map's source size; a sample's region must lie inside its full() frame, start at an even x and y on an unrectified
+// YUV or Bayer frame (an odd offset would change the chroma phase or the Bayer pattern), and, cropped, still be a
+// frame frame_fmt_check takes.  Then the engine's geometries g of what the pre-process will read.
 static int pre_geoms(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who, PreGeom* g) {
-  Frames pre{};
+  Frames pre{}, full{};
   for (int k = 0; k < n; ++k) {
     SampleFrames s;
     s.given = frames[k]; s.map = e->chain[k].map;
+    memcpy(s.roi, e->chain[k].roi, sizeof(s.roi));
     if (s.map && (frames[k].h != s.map->src_h || frames[k].w != s.map->src_w)) {
       vpb_set_error("%s: frame %d is %dx%d; the map set for sample %d rectifies %dx%d frames", who, k, frames[k].w,
                     frames[k].h, k, s.map->src_w, s.map->src_h);
       return VPB_ERR_ARG;
     }
+    full[k] = s.full();
     pre[k] = s.pre();
+    const int* r = s.roi;
+    if (!r[2]) continue;
+    if (static_cast<long long>(r[0]) + r[2] > full[k].w || static_cast<long long>(r[1]) + r[3] > full[k].h) {
+      vpb_set_error("%s: frame %d: the region %dx%d at (%d, %d) set for sample %d does not lie inside its %dx%d frame",
+                    who, k, r[2], r[3], r[0], r[1], k, full[k].w, full[k].h);
+      return VPB_ERR_ARG;
+    }
+    const int fmt = full[k].format;
+    if (fmt != VPB_PIX_PACKED && fmt != VPB_PIX_BGRA && fmt != VPB_PIX_RGBA && ((r[0] | r[1]) & 1)) {
+      vpb_set_error("%s: frame %d: the region set for sample %d starts at (%d, %d); a YUV or Bayer frame needs an even x "
+                    "and y", who, k, k, r[0], r[1]);
+      return VPB_ERR_ARG;
+    }
+    if (fmt != VPB_PIX_PACKED && frame_fmt_check(pre[k], who, k)) return VPB_ERR_ARG;
   }
-  return e->geoms(pre.data(), who, g);
+  return e->geoms(pre.data(), full.data(), who, g);
 }
 
 // vpb_frame descriptors as VPB_PIX_PACKED ones (the first kMaxBatch; frames_ok rejects a count other than the batch)

@@ -16,6 +16,8 @@
 #include <vector>
 #include "ops_internal.h"
 
+struct vp_autospeed;
+
 namespace vpb {
 
 struct HostTensor {
@@ -91,7 +93,7 @@ using Frames = std::array<vpb_frame_fmt, kMaxBatch>;
 struct EngineRuntime;
 // The CUDA graph of one call of a runtime's launch list.  It is captured again when the op list changes (insert_ops,
 // erase_ops, and invalidate for op arguments that are not described) or when the geometry key does: the n (format, h,
-// w, stride, uv_stride) tuples of the frames the pre-process reads.  A new format selects another pre-process kernel;
+// w, stride, uv_stride) tuples of the frames the pre-process reads and of the uncropped frames they are regions of.  A new format selects another pre-process kernel;
 // the grids and tables follow the geometries.  Otherwise every described op's launch is rebuilt from the current call
 // and set on its captured node where it differs from the launch the node holds, so the captured kernels read this
 // call's frames, maps, JPEG streams and scratch buffers, whichever of them changed.
@@ -103,6 +105,7 @@ struct FrameGraph {
   std::vector<Node> nodes;
   int n = 0;                             // the geometry key: geometries of geom[0 .. n-1] (0: none)
   Frames geom{};
+  Frames geom_full{};                    // ... and of geom_full[0 .. n-1], the uncropped frames (SampleFrames::full)
   int captures = 0;                      // captures so far (vp_engine_graph_captures)
 
   // Launch the graph for e's frames on e's stream.  When the key differs: e.launch_all once outside capture (sets
@@ -115,16 +118,21 @@ struct FrameGraph {
 // Device scratch of the front end, grown on demand outside any capture (EngineRuntime::grow)
 struct Scratch { uint8_t* p = nullptr; size_t cap = 0; };
 
-// Sample k's frame chain: the frame as given -> JPEG-decoded -> rectified -> what the pre-process reads.
+// Sample k's frame chain: the frame as given -> JPEG-decoded -> rectified -> its region -> what the pre-process reads.
 struct SampleFrames {
   vpb_frame_fmt given{};                 // the call's frame (a host call's device copy; a JPEG frame: its host stream,
                                          // read while the call is staged)
   const vpb_rectify* map = nullptr;      // set_rectify; NULL: none
   Scratch jpg, rect;                     // the decoded JPEG frame and the rectified frame, packed
+  int roi[4] = {0, 0, 0, 0};             // set_roi: x, y, w, h of the region of full() the pre-process reads; w = 0: none
   // what the rectify op reads: a JPEG frame packed at its SOF size in jpg, any other the frame as given
   vpb_frame_fmt decoded() const;
-  // what the pre-process (and the letterbox, the source outputs, the resized image) reads: with a map, the rectified
-  // frame packed at the map size in rect; otherwise decoded().  Host-only checks read the geometry alone.
+  // the whole frame of the sample: with a map, the rectified frame packed at the map size in rect; otherwise decoded()
+  // (what an attached detector's letterbox reads)
+  vpb_frame_fmt full() const;
+  // what the pre-process (and the letterbox, the source outputs, the resized image, the lateral op) reads: full(), or
+  // with a region its view (the data pointer, and NV12's uv, offset to (x, y), the same strides, the region's size).
+  // Host-only checks read the geometry alone.
   vpb_frame_fmt pre() const;
 };
 
@@ -140,6 +148,11 @@ struct EngineRuntime {
   std::vector<int> lane_dep;              // [lane] producer op index; empty: no lanes were opened
   std::vector<cudaStream_t> lane_streams; // [lane] for the lanes > 0; lane 0 is the engine stream
   std::vector<Event> op_events, lane_done;   // [op], only for ops some lane waits on; [lane] its join
+  // A lane that forks after the last front op (the JPEG decode or "rectify"), or at the call's start while there is
+  // none (lane_dep -1: it waits on call_start, recorded on the engine stream after the per-call reset); 0: none.
+  // sync_front_ops keeps its lane_dep right.
+  int front_lane = 0;
+  Event call_start;
   bool single_stream = false;             // the lanes run one after another on the engine stream
   bool use_graph = true;                  // run_call replays the frame graph
   void* call_zero = nullptr; size_t call_zero_bytes = 0;   // what a call zeroes before its first op
@@ -201,12 +214,18 @@ struct EngineRuntime {
   void insert_ops(size_t at, std::vector<OpRec> add);
   void erase_ops(size_t at, size_t m);
   // The front ops before "preprocess" exactly while they are needed: the three JPEG decode ops while a sample's frame
-  // is JPEG, then "rectify" while a sample has a map; with their bytes for the current frames.
+  // is JPEG, then "rectify" while a sample has a map; with their bytes for the current frames; and front_lane's fork.
   void sync_front_ops();
+  // Region (x, y, w, h) of sample `sample`'s full() frame for the pre-process of every later call; w == h == 0 clears
+  // it.  VPB_ERR_ARG (naming who) for a sample out of range, x or y < 0, or w, h <= 0 other than the clearing pair.
+  int set_roi(int sample, int x, int y, int w, int h, const char* who);
   // s grown to `bytes` (outside any capture): the new buffer joins dev_allocs, the old one is kept
   int grow(Scratch& s, size_t bytes);
   // the ops appended next form `lane`, which starts after ops[dep_op]
   void begin_lane(int lane, int dep_op) { cur_lane = lane; lane_dep.resize(lane + 1); lane_dep[lane] = dep_op; }
+  // `lane` forks after ops[dep] from now on (-1: at the call's start); the event of its former fork op is dropped
+  // unless another lane forks there, so no op records an event nothing waits on
+  void set_lane_dep(int lane, int dep);
   // launch ops[i] on st; while frame_graph captures, a described op records its kernel node and launch
   int launch_op(size_t i, cudaStream_t st);
   int reset_call(cudaStream_t st);        // zero call_zero on st: a memset, not an op
@@ -245,10 +264,10 @@ struct EngineRuntime {
                int* launches);
 
   // The engine's steps of a frame call (call_host, call_device).  geoms: host-only checks of the geometries of the
-  // `batch` frames (VPB_ERR_ARG naming who and the frame); enqueue: the call on the device frames `frames` of
-  // geometries g; fetch: copies of the outputs to the pinned host buffers (raw: also the raw tensors the engine does
-  // not copy by default).
-  virtual int geoms(const vpb_frame_fmt* frames, const char* who, PreGeom* g) = 0;
+  // `batch` frames the pre-process reads, `full` the uncropped frames they are regions of (VPB_ERR_ARG naming who and
+  // the frame); enqueue: the call on the device frames of geometries g; fetch: copies of the outputs to the pinned
+  // host buffers (raw: also the raw tensors the engine does not copy by default).
+  virtual int geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, const char* who, PreGeom* g) = 0;
   virtual int enqueue(const PreGeom* g) = 0;
   virtual int fetch(bool raw) = 0;
 };
@@ -267,6 +286,24 @@ bool frames_ok(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const
 // n frames of one geometry (the *_batch calls) as descriptors; false (error set as frames_ok does) on bad arguments
 bool batch_frames(const EngineRuntime* e, const uint8_t* const* ptrs, int n, int h, int w, int stride, const char* who,
                   Frames& out);
+
+// The AutoSpeed detector (autospeed.cu) as a segmentation engine's call runs it (vp_engine_set_detector), on the
+// detector's own weights and buffers:
+//   autospeed_runtime    the detector's runtime (batch, device)
+//   autospeed_geoms      the letterbox geometries of the frames (VPB_ERR_ARG naming who and the frame), host-only
+//   autospeed_prepare    the letterbox tables and scales for g, and the canvas borders refilled on st where they changed
+//   autospeed_letterbox  the launch of the letterbox of the frames into the canvases; bgr: the frames are B, G, R
+//   autospeed_net_ops    copies of the ops after the detector's pre-process, named "det/<name>", the NMS described
+//                        (it reads the thresholds and letterboxes when it launches)
+//   autospeed_fetch      the detections (raw: and the raw tensors) to the detector's pinned buffers on st
+//   autospeed_fetch_rest after a synchronise: the detections past the first 1024 of a sample that has more
+const EngineRuntime* autospeed_runtime(const vp_autospeed* d);
+int autospeed_geoms(vp_autospeed* d, const vpb_frame_fmt* frames, const char* who, PreGeom* g);
+int autospeed_prepare(vp_autospeed* d, const PreGeom* g, cudaStream_t st);
+int autospeed_letterbox(const vp_autospeed* d, const vpb_frame_fmt* frames, int bgr, KernelCall& c);
+std::vector<OpRec> autospeed_net_ops(const vp_autospeed* d);
+int autospeed_fetch(vp_autospeed* d, bool raw, cudaStream_t st);
+int autospeed_fetch_rest(vp_autospeed* d);
 
 }  // namespace vpb
 

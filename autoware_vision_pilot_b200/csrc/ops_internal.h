@@ -73,6 +73,10 @@ static constexpr int kNetH = 320, kNetW = 640;   // the only network input size 
 static constexpr int kGapReplicas = 8;           // copies of each SE pooling accumulator (atomic spreading)
 static constexpr int kMaxBatch = 8;              // VP_MAX_BATCH (vp_b200.h): frames per engine call
 static constexpr int kMaxSrcJobs = 64;           // vpb_source_outputs: 8 samples x 4 models x 2 outputs
+// A pre-process convention of the library only (the public entry points reject it): B, G, R in, swapped to R, G, B,
+// x/255 only -- VPB_CONV_RGB_UNIT on the frames of a BGR engine (the AutoSpeed letterbox inside a segmentation call,
+// vp_engine_set_detector).  Its fields are run-time parameters of the existing kernels.
+static constexpr int kConvBgrUnit = VPB_CONV_RGB_UNIT + 1;
 
 void resize_tables_host(int mode, int in_size, int out_size, std::vector<int>& bounds,
                         std::vector<int>& coeffs, int& ksize);

@@ -486,7 +486,7 @@ static int fill_params(const PreprocessPlan& pl, const vpb_frame_fmt* frames, in
   p.out_lo = pl.out_lo;
   p.out_pitch = pl.out_pitch; p.out_c = pl.out_c;
   // a non-packed image converts to the channel order the convention takes as input
-  const int bgr = (convention == VPB_CONV_BGR_NOSWAP || convention == VPB_CONV_BGR_SWAP) ? 1 : 0;
+  const int bgr = (convention == VPB_CONV_BGR_NOSWAP || convention == VPB_CONV_BGR_SWAP || convention == kConvBgrUnit) ? 1 : 0;
   cvt = false;
   for (int i = 0; i < kMaxBatch; ++i) {
     const int k = i < pl.n ? i : 0;
@@ -507,12 +507,13 @@ static int fill_params(const PreprocessPlan& pl, const vpb_frame_fmt* frames, in
   p.out_img = static_cast<size_t>(pl.out_rows) * p.out_pitch * pl.out_c;   // whole canvases
   // conventions: see include/vp_b200_ops.h
   static const float kMeanRGB[3] = {0.485f, 0.456f, 0.406f}, kStdRGB[3] = {0.229f, 0.224f, 0.225f};
-  p.swap_rb = convention == VPB_CONV_BGR_SWAP ? 1 : 0;
-  p.mul_inv255 = (convention == VPB_CONV_RGB || convention == VPB_CONV_RGB_UNIT) ? 0 : 1;
+  const bool unit = convention == VPB_CONV_RGB_UNIT || convention == kConvBgrUnit;   // ToTensor only (auto_speed_infer.py:50)
+  p.swap_rb = (convention == VPB_CONV_BGR_SWAP || convention == kConvBgrUnit) ? 1 : 0;
+  p.mul_inv255 = (convention == VPB_CONV_RGB || unit) ? 0 : 1;
   for (int c = 0; c < 3; ++c) {
     const int s = convention == VPB_CONV_BGR_NOSWAP ? 2 - c : c;   // BGR-ordered stats (tensorrt_backend.cpp:167-168)
-    p.mean[c] = convention == VPB_CONV_RGB_UNIT ? 0.f : kMeanRGB[s];   // ToTensor only (auto_speed_infer.py:50)
-    p.stdv[c] = convention == VPB_CONV_RGB_UNIT ? 1.f : kStdRGB[s];
+    p.mean[c] = unit ? 0.f : kMeanRGB[s];
+    p.stdv[c] = unit ? 1.f : kStdRGB[s];
   }
   p.out = out; p.out_u8 = out_u8;
   return VPB_OK;

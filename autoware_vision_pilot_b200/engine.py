@@ -119,6 +119,8 @@ def _bind():
     lib.vp_engine_lateral_reset.argtypes = [C.c_void_p, C.c_int]
     lib.vp_engine_lateral.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     lib.vp_engine_graph_captures.argtypes = [C.c_void_p]
+    lib.vp_engine_set_roi.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.vp_engine_set_detector.argtypes = [C.c_void_p, C.c_void_p]
     _bound = True
     return lib
 
@@ -155,6 +157,7 @@ class Engine:
         self.kinds = list(kinds)
         self.batch = max(1, batch)
         self._rectify = {}
+        self._detector = None
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -170,6 +173,37 @@ class Engine:
         L.check(self._lib.vp_engine_set_rectify(self._h, sample, r.handle if r is not None else None),
                 "vp_engine_set_rectify")
         self._rectify[sample] = r
+
+    def set_roi(self, sample: int, roi: Optional[Sequence[int]]) -> None:
+        """Read only the region roi = (x, y, w, h) of sample `sample`'s frame (after its JPEG decode and rectify) in the
+        pre-process of every later call, or the whole frame again (roi None).  The outputs, the resized image, the source
+        outputs and the lateral image size are then the region's; an attached detector still reads the whole frame.
+        A region outside a call's frame, or at an odd x / y of an unrectified YUV or Bayer frame, fails that call."""
+        if not 0 <= sample < self.batch:
+            raise ValueError(f"sample {sample} of a batch of {self.batch}")
+        x, y, w, h = (0, 0, 0, 0) if roi is None else (int(v) for v in roi)
+        if roi is not None and (x < 0 or y < 0 or w <= 0 or h <= 0):
+            raise ValueError(f"region {tuple(roi)}: need x, y >= 0 and w, h > 0")
+        L.check(self._lib.vp_engine_set_roi(self._h, sample, x, y, w, h), "vp_engine_set_roi")
+
+    def set_detector(self, det) -> None:
+        """Run the AutoSpeedEngine det (of this engine's batch and GPU) on every sample's whole frame inside every later
+        call, on a lane of its own (det None: detach).  After a host call det.detections(k) holds sample k's detections;
+        after a submit or device call: sync(), then det.sync().  The engine keeps det alive while it is attached, and
+        det.close() detaches it first."""
+        from .autospeed import AutoSpeedEngine
+        if det is not None:
+            if not isinstance(det, AutoSpeedEngine):
+                raise TypeError(f"set_detector takes an AutoSpeedEngine or None, not {type(det).__name__}")
+            if det.batch != self.batch:
+                raise ValueError(f"the detector has batch {det.batch}, the engine batch {self.batch}")
+        L.check(self._lib.vp_engine_set_detector(self._h, det.handle if det is not None else None),
+                "vp_engine_set_detector")
+        if self._detector is not None:
+            self._detector._engines.discard(self)
+        if det is not None:
+            det._engines.add(self)
+        self._detector = det
 
     # ---- the lateral post-process inside the call
     def set_lateral(self, model_idx: Optional[int], threshold: float = 0.0, smoothing: float = 0.5,

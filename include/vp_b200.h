@@ -53,6 +53,7 @@ enum { VP_SCENE_SEG = 0, VP_SCENE_3D = 1, VP_DOMAIN_SEG = 2, VP_EGO_LANES = 3 };
 enum { VP_PREC_16 = 0, VP_PREC_SPLIT = 1 };
 
 typedef struct vp_engine vp_engine;
+struct vp_autospeed;                /* the AutoSpeed detector, vp_b200_autospeed.h (vp_engine_set_detector) */
 
 typedef struct {
   int gpu_id;                       /* cudaSetDevice target (tensorrt_backend.cpp:38) */
@@ -169,6 +170,32 @@ int vp_engine_infer_device_frames_fmt(vp_engine* e, const vpb_frame_fmt* frames_
  * engine keeps the pointer: r must outlive every call that uses it.  The lateral post-process of a rectified camera
  * takes the map's size as its image size: the in-call one (vp_engine_set_lateral) does so by itself. */
 int vp_engine_set_rectify(vp_engine* e, int sample, const vpb_rectify* r);
+
+/* A region of interest per sample: every later call's pre-process reads the w x h region at (x, y) of sample `sample`'s
+ * frame after its JPEG decode and rectify (the production lateral view: rows >= 420 of a 1080p camera).  The outputs,
+ * the resized image, the source outputs (at the region's size; the overlay blends the region) and the in-call lateral
+ * op's image size are then those of the region; an attached detector (vp_engine_set_detector) still reads the whole
+ * frame.  w == h == 0 clears it.  VPB_ERR_ARG for a NULL engine, a sample outside 0 .. batch-1, x or y < 0, or w, h <= 0
+ * other than the clearing pair.  A call returns VPB_ERR_ARG, naming the call and the frame, before any device work when
+ * the region does not lie inside the (decoded, rectified) frame, when the cropped frame fails the checks a frame of
+ * its own would (the format's size rules, VPB_RESIZE_NONE's 640 x 320, the 32-tap limit), or when x or y is odd on an
+ * unrectified YUV or Bayer frame (it would change the chroma phase or the Bayer pattern).  A new offset re-points the
+ * frame graph; a new size captures it again. */
+int vp_engine_set_roi(vp_engine* e, int sample, int x, int y, int w, int h);
+
+/* The AutoSpeed detector (vp_b200_autospeed.h) inside every later call of every form: "det/letterbox" (its Pillow-
+ * bilinear letterbox of each sample's whole decoded and rectified frame, never the region) and copies of its network,
+ * decode and NMS ops ("det/<name>") on a lane of their own, which forks after the JPEG decode / rectify ops (at the
+ * call's start without them) and joins before the source outputs.  The frames are read as R, G, B under VPB_CONV_RGB
+ * and as B, G, R under the BGR conventions.  det keeps its weights, buffers and thresholds, and it stays usable on its
+ * own: the caller serialises its calls with the engine's.  A threshold change reaches the engine's next call (the frame
+ * graph re-points the NMS node; it does not capture again).  Results: vp_autospeed_detections_at / _raw_at.  A host
+ * infer call copies the detections (every one of them) to det's host buffers, and the raw tensors with
+ * vp_engine_config.fetch_raw; after a submit or a device call: vp_engine_sync, then vp_autospeed_sync(det, fetch).
+ * vp_engine_profile, _kernel_names, _time_kernel and _get_stats include the detector's ops.  det NULL detaches.  The
+ * engine does not own det, which must outlive the attachment.  VPB_ERR_ARG for a NULL engine, or a detector of
+ * another batch or GPU. */
+int vp_engine_set_detector(vp_engine* e, struct vp_autospeed* det);
 
 /* The lateral post-process inside the call (production_release/main.cpp:505-577: EgoLanes -> LaneFilter ->
  * LaneTracker -> PathFinder, per camera).  With it set on EgoLanes model model_idx, every later call of every form

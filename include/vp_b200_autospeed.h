@@ -46,6 +46,8 @@ int vp_autospeed_create_batch(const char* weights_vpw, int gpu_id, int dtype, vo
 void vp_autospeed_destroy(vp_autospeed* e);
 /* conf_thres / iou_thres of post_process_predictions (defaults 0.6 / 0.45, auto_speed_infer.py:71) */
 int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float iou);
+/* A detector may also run inside a segmentation engine's call on that engine's frames (vp_engine_set_detector,
+ * vp_b200.h); its results are then read here as after its own calls. */
 
 /* Host RGB frame (uint8, 3 interleaved channels, any size), results on the host when it returns:
  * H2D + letterbox + network + decode + NMS + D2H + sync.  fetch_raw != 0 also copies the raw tensor. */

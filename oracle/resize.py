@@ -1,4 +1,4 @@
-"""ORACLE (test infrastructure): integer restatements of the two caller-side resize conventions.
+"""ORACLE (test infrastructure): integer restatements of the caller-side resize conventions.
 
 * `pil_bicubic_resize`  — Pillow `Image.resize((640,320))` default filter = BICUBIC with antialias
   (Models/visualizations/SceneSeg/image_visualization.py:108-109).  Pillow (>=11.3.0,
@@ -6,12 +6,15 @@
   /root/reference; its published algorithm (libImaging/Resample.c: precompute_coeffs,
   normalize_coeffs_8bpc, ImagingResampleHorizontal/Vertical_8bpc) is restated here in numpy:
   separable, horizontal pass first, 22-bit fixed-point coefficients, uint8 clip after each pass.
+* `pil_bilinear_resize` — Pillow `Image.resize(size, Image.BILINEAR)` (antialias: a triangle filter of support 1
+  scaled by the downscale factor), the AutoSpeed letterbox (Models/inference/auto_speed_infer.py:38); the same
+  Resample.c passes as BICUBIC with the other filter.
 * `cv_linear_resize`    — OpenCV `cv::resize` default INTER_LINEAR on uint8
   (VisionPilot/middleware_recipes/common/backends/tensorrt_backend.cpp:163,
   production_release/src/inference/tensorrt_engine.cpp:194-195): 11-bit fixed-point weights,
   two-stage integer rounding (imgproc/resize.cpp HResizeLinear / VResizeLinear<uchar>).
 
-Both are pinned bit-exact against the installed libraries in tests/test_oracle_resize.py (PIL /
+All are pinned bit-exact against the installed libraries in tests/test_oracle_resize.py (PIL /
 cv2 are present in the image, on the GPU box too).
 """
 from __future__ import annotations
@@ -32,12 +35,21 @@ def _bicubic(x: float, a: float = -0.5) -> float:
     return 0.0
 
 
-def pil_coeffs(in_size: int, out_size: int):
+def _bilinear(x: float) -> float:
+    x = abs(x)
+    return 1.0 - x if x < 1.0 else 0.0
+
+
+_FILTERS = {"bicubic": (_bicubic, 2.0), "bilinear": (_bilinear, 1.0)}   # Resample.c: filter, support
+
+
+def pil_coeffs(in_size: int, out_size: int, filter: str = "bicubic"):
     """Per output index: (xmin, int32 coefficient vector).  Resample.c precompute_coeffs +
     normalize_coeffs_8bpc."""
+    fn, base_support = _FILTERS[filter]
     scale = in_size / out_size
     filterscale = max(scale, 1.0)
-    support = 2.0 * filterscale
+    support = base_support * filterscale
     ss = 1.0 / filterscale
     bounds, coeffs = [], []
     for xx in range(out_size):
@@ -49,7 +61,7 @@ def pil_coeffs(in_size: int, out_size: int):
         if xmax > in_size:
             xmax = in_size
         n = xmax - xmin
-        k = [_bicubic((x + xmin - center + 0.5) * ss) for x in range(n)]
+        k = [fn((x + xmin - center + 0.5) * ss) for x in range(n)]
         ww = sum(k)
         k = [v / ww for v in k] if ww != 0.0 else k
         kk = [int(v * (1 << PRECISION_BITS) - 0.5) if v < 0 else int(v * (1 << PRECISION_BITS) + 0.5)
@@ -59,10 +71,10 @@ def pil_coeffs(in_size: int, out_size: int):
     return bounds, coeffs
 
 
-def _pil_pass(img: np.ndarray, out_size: int, axis: int) -> np.ndarray:
+def _pil_pass(img: np.ndarray, out_size: int, axis: int, filter: str) -> np.ndarray:
     """One separable pass along `axis` (0 = vertical, 1 = horizontal) on uint8 HWC."""
     in_size = img.shape[axis]
-    bounds, coeffs = pil_coeffs(in_size, out_size)
+    bounds, coeffs = pil_coeffs(in_size, out_size, filter)
     src = np.moveaxis(img, axis, 0).astype(np.int64)
     out = np.empty((out_size,) + src.shape[1:], dtype=np.uint8)
     for o in range(out_size):
@@ -73,14 +85,22 @@ def _pil_pass(img: np.ndarray, out_size: int, axis: int) -> np.ndarray:
     return np.moveaxis(out, 0, axis)
 
 
-def pil_bicubic_resize(img_u8_hwc: np.ndarray, out_w: int, out_h: int) -> np.ndarray:
+def _pil_resize(img_u8_hwc: np.ndarray, out_w: int, out_h: int, filter: str) -> np.ndarray:
     h, w = img_u8_hwc.shape[:2]
     x = img_u8_hwc
     if w != out_w:
-        x = _pil_pass(x, out_w, axis=1)   # horizontal first (ImagingResample)
+        x = _pil_pass(x, out_w, axis=1, filter=filter)   # horizontal first (ImagingResample)
     if h != out_h:
-        x = _pil_pass(x, out_h, axis=0)
+        x = _pil_pass(x, out_h, axis=0, filter=filter)
     return np.ascontiguousarray(x)
+
+
+def pil_bicubic_resize(img_u8_hwc: np.ndarray, out_w: int, out_h: int) -> np.ndarray:
+    return _pil_resize(img_u8_hwc, out_w, out_h, "bicubic")
+
+
+def pil_bilinear_resize(img_u8_hwc: np.ndarray, out_w: int, out_h: int) -> np.ndarray:
+    return _pil_resize(img_u8_hwc, out_w, out_h, "bilinear")
 
 
 def cv_linear_coeffs(in_size: int, out_size: int):

@@ -36,6 +36,25 @@ def test_ragged_sizes(h, w):
     assert np.array_equal(resize.cv_linear_resize(f, 640, 320), cv2.resize(f, (640, 320)))
 
 
+@pytest.mark.parametrize("h,w,oh,ow", [
+    (1080, 1920, 512, 910),      # downscale: the 1080p letterbox
+    (333, 517, 320, 640),        # one axis down, one up
+    (100, 130, 256, 333),        # upscale
+    (5, 8, 320, 640),            # upscale from a few pixels
+    (270, 480, 270, 480),        # identity
+    (1, 4800, 1, 640),           # 1-pixel axis kept, the other down
+    (1, 1, 320, 640),            # a 1x1 frame
+    (7, 1, 512, 3),              # a 1-pixel column
+    (2400, 4800, 320, 640),      # a 7.5x downscale (17 taps)
+])
+def test_pil_bilinear_matches_pillow(h, w, oh, ow):
+    from PIL import Image
+    rng = np.random.default_rng(h * 31 + w)
+    f = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+    exp = np.asarray(Image.fromarray(f).resize((ow, oh), Image.BILINEAR))
+    assert np.array_equal(resize.pil_bilinear_resize(f, ow, oh), exp)
+
+
 def test_identity_size_is_passthrough():
     f = synth.synth_frame(1, 320, 640)
     assert np.array_equal(resize.pil_bicubic_resize(f, 640, 320), f)

@@ -11,7 +11,18 @@ from . import _lib as L
 
 NUM_ANCHORS, NUM_OUT = 10752, 8
 MAX_BATCH = 8   # VP_MAX_BATCH
+PREC_16, PREC_SPLIT = 0, 1   # VP_PREC_*
+# dtype name -> (dtype, precision) of vp_autospeed_create_precision; "fp32" (the reference's precision="fp32") is the
+# split-fp16 fp32-grade detector
+PRECISION_BY_DTYPE = {"fp16": (L.VPB_F16, PREC_16), "bf16": (L.VPB_BF16, PREC_16), "fp32": (L.VPB_F16, PREC_SPLIT)}
 _bound = False
+
+
+def precision_args(dtype: str):
+    """(dtype, precision) of vp_autospeed_create_precision for a dtype name; ValueError for any other name."""
+    if dtype not in PRECISION_BY_DTYPE:
+        raise ValueError(f"dtype {dtype!r}: one of {sorted(PRECISION_BY_DTYPE)}")
+    return PRECISION_BY_DTYPE[dtype]
 
 
 def _bind():
@@ -21,6 +32,8 @@ def _bind():
         return lib
     lib.vp_autospeed_create.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
     lib.vp_autospeed_create_batch.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]
+    lib.vp_autospeed_create_precision.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                                  C.POINTER(C.c_void_p)]
     lib.vp_autospeed_destroy.argtypes = [C.c_void_p]
     lib.vp_autospeed_destroy.restype = None
     lib.vp_autospeed_set_thresholds.argtypes = [C.c_void_p, C.c_float, C.c_float]
@@ -52,13 +65,15 @@ def _bind():
 class AutoSpeedEngine:
     def __init__(self, weights_vpw: str, *, gpu_id: int = 0, dtype: str = "fp16", stream: Optional[int] = None,
                  batch: int = 1):
-        """batch > 1: every call takes exactly `batch` frames of one shape (infer_batch / infer_device_batch); sample k's
-        results are detections(k) / raw(k) / read_tap("<name>@k")."""
+        """dtype "fp16" | "bf16": 16-bit operands; "fp32" (the reference's precision="fp32"): the split-fp16
+        fp32-grade detector (batch 1); any other name raises ValueError.  batch > 1: every call takes exactly `batch`
+        frames of one shape (infer_batch / infer_device_batch); sample k's results are detections(k) / raw(k) /
+        read_tap("<name>@k")."""
+        dt, prec = precision_args(dtype)
         self._lib = _bind()
         self._h = C.c_void_p()
-        L.check(self._lib.vp_autospeed_create_batch(weights_vpw.encode(), gpu_id,
-                                                    L.VPB_BF16 if dtype == "bf16" else L.VPB_F16, stream, batch,
-                                                    C.byref(self._h)), "vp_autospeed_create_batch")
+        L.check(self._lib.vp_autospeed_create_precision(weights_vpw.encode(), gpu_id, dt, prec, stream, batch,
+                                                        C.byref(self._h)), "vp_autospeed_create_precision")
         self.batch = batch
         self._rectify = {}
         self._engines = weakref.WeakSet()    # segmentation engines this detector is attached to (Engine.set_detector)

@@ -45,11 +45,14 @@ static constexpr float kBnEps = 1e-3f;                        // common_layers.p
 // ------------------------------------------------------------------ SIMT kernels
 // kB / kBatch = false (batch 1, a grid without images) compiles each kernel to its single-image code: these kernels are
 // latency-bound, and the per-image addressing on the critical path slowed a batch-1 frame by about 1 % on the H100.
+// kS = true is the split-fp16 form of a kernel (batch 1): every 16-bit tensor is a (hi, lo) pair of one layout, the low
+// halves passed after the kernel's other arguments, so the 16-bit instantiations keep their parameter layout and code.
 // mean over H*W per channel, two deterministic stages (CTX block, common_layers.py:214); blockIdx.y = image:
 // in [N][HW][ld], part [N][nblk][C], out [N][C]
-template <class E, bool kB>
+template <class E, bool kB, bool kS = false>
 __global__ void __launch_bounds__(256) mean_part_kernel(const typename E::T* __restrict__ in, int HW, int C, int ld,
-                                                        float* __restrict__ part) {
+                                                        float* __restrict__ part,
+                                                        const typename E::T* __restrict__ in_lo = nullptr) {
   pdl_launch_dependents();
   pdl_wait();
   if (kB) {
@@ -63,7 +66,10 @@ __global__ void __launch_bounds__(256) mean_part_kernel(const typename E::T* __r
   const int p0 = blockIdx.x * chunk, p1 = min(HW, p0 + chunk);
   float s = 0.f;
   if (pl < ppb)
-    for (int p = p0 + pl; p < p1; p += ppb) s += to_f32<E>(in[static_cast<size_t>(p) * ld + c]);
+    for (int p = p0 + pl; p < p1; p += ppb) {
+      const size_t i = static_cast<size_t>(p) * ld + c;
+      s += kS ? to_f32<E>(in[i]) + to_f32<E>(in_lo[i]) : to_f32<E>(in[i]);   // hi + lo is exact in fp32
+    }
   __shared__ float red[256];
   red[threadIdx.x] = s;
   __syncthreads();
@@ -107,9 +113,14 @@ __global__ void upsample2_kernel(const uint4* __restrict__ in, int H, int W, int
   out[pix * ld8_out + g] = __ldg(in + (static_cast<long>(oy >> 1) * W + (ox >> 1)) * ld8_in + g);
 }
 
-// MaxPool2d(5, stride 1, padding 2) (SPPF, common_layers.py:249), slice in -> slice out; blockIdx.y = image
-template <class E, bool kB>
-__global__ void maxpool5_kernel(const uint4* __restrict__ in, int H, int W, int C8, int ld8, uint4* __restrict__ out) {
+// MaxPool2d(5, stride 1, padding 2) (SPPF, common_layers.py:249), slice in -> slice out; blockIdx.y = image.
+// kS: the (hi, lo) pair of the largest hi + lo.  Every producer stores hi = round(v), lo = round(v - hi), so
+// |lo| <= ulp(hi) / 2 and the lexicographic order of the pairs is the order of hi + lo (pairs tie only when their values
+// are equal); the output pair is an input pair, bit for bit.  A NaN hi fails both comparisons and is dropped, as fmaxf
+// drops it in the 16-bit form.
+template <class E, bool kB, bool kS = false>
+__global__ void maxpool5_kernel(const uint4* __restrict__ in, int H, int W, int C8, int ld8, uint4* __restrict__ out,
+                                const uint4* __restrict__ in_lo = nullptr, uint4* __restrict__ out_lo = nullptr) {
   pdl_launch_dependents();
   pdl_wait();
   if (kB) {
@@ -120,27 +131,48 @@ __global__ void maxpool5_kernel(const uint4* __restrict__ in, int H, int W, int 
   if (i >= H * W * C8) return;
   const int g = i % C8, pix = i / C8;
   const int x = pix % W, y = pix / W;
-  float m[8];
+  float m[8], ml[8];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) m[k] = -INFINITY;
+  for (int k = 0; k < 8; ++k) { m[k] = -INFINITY; ml[k] = 0.f; }
   for (int dy = -2; dy <= 2; ++dy) {
     const int yy = y + dy;
     if (yy < 0 || yy >= H) continue;
     for (int dx = -2; dx <= 2; ++dx) {
       const int xx = x + dx;
       if (xx < 0 || xx >= W) continue;
-      const uint4 v = __ldg(in + static_cast<size_t>(yy * W + xx) * ld8 + g);
+      const size_t at = static_cast<size_t>(yy * W + xx) * ld8 + g;
+      const uint4 v = __ldg(in + at);
       const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+      if (kS) {
+        const uint4 vl = __ldg(in_lo + at);
+        const uint32_t wl[4] = {vl.x, vl.y, vl.z, vl.w};
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float2 f = unpack2<E>(w[k]);
-        m[2 * k] = fmaxf(m[2 * k], f.x); m[2 * k + 1] = fmaxf(m[2 * k + 1], f.y);
+        for (int k = 0; k < 4; ++k) {
+          const float2 f = unpack2<E>(w[k]), fl = unpack2<E>(wl[k]);
+          const float h[2] = {f.x, f.y}, l[2] = {fl.x, fl.y};
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            float& mh = m[2 * k + j];
+            float& mlo = ml[2 * k + j];
+            if (h[j] > mh || (h[j] == mh && l[j] > mlo)) { mh = h[j]; mlo = l[j]; }
+          }
+        }
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float2 f = unpack2<E>(w[k]);
+          m[2 * k] = fmaxf(m[2 * k], f.x); m[2 * k + 1] = fmaxf(m[2 * k + 1], f.y);
+        }
       }
     }
   }
   uint4 o;
   o.x = pack2<E>(m[0], m[1]); o.y = pack2<E>(m[2], m[3]); o.z = pack2<E>(m[4], m[5]); o.w = pack2<E>(m[6], m[7]);
   out[static_cast<size_t>(pix) * ld8 + g] = o;
+  if (kS) {     // 16-bit values convert to fp32 and back exactly
+    o.x = pack2<E>(ml[0], ml[1]); o.y = pack2<E>(ml[2], ml[3]); o.z = pack2<E>(ml[4], ml[5]); o.w = pack2<E>(ml[6], ml[7]);
+    out_lo[static_cast<size_t>(pix) * ld8 + g] = o;
+  }
 }
 
 // qkv [T][nh*(2dk+dh)] -> Vc [T][nh*dh] (token-major, for the depthwise conv on v, common_layers.py:102) and
@@ -165,21 +197,24 @@ __global__ void split_v_kernel(const typename E::T* __restrict__ qkv, int T, int
 }
 
 // softmax over the key axis of S * scale (common_layers.py:99-100): one warp per query row, fp32 math (a batch is
-// [N * T] independent rows)
-template <class E>
+// [N * T] independent rows); kS: reads hi + lo of S and writes the split of P
+template <class E, bool kS = false>
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const typename E::T* __restrict__ s, int rows, int cols,
-                                                           float scale, typename E::T* __restrict__ p) {
+                                                           float scale, typename E::T* __restrict__ p,
+                                                           const typename E::T* __restrict__ s_lo = nullptr,
+                                                           typename E::T* __restrict__ p_lo = nullptr) {
   pdl_launch_dependents();
   pdl_wait();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= rows) return;
   const typename E::T* sr = s + static_cast<size_t>(row) * cols;
+  const typename E::T* sl = kS ? s_lo + static_cast<size_t>(row) * cols : nullptr;
   float v[16];                                   // cols <= 512
   float mx = -INFINITY;
 #pragma unroll
   for (int k = 0; k < 16; ++k) {
     const int c = lane + 32 * k;
-    v[k] = c < cols ? to_f32<E>(sr[c]) * scale : -INFINITY;
+    v[k] = c < cols ? (kS ? to_f32<E>(sr[c]) + to_f32<E>(sl[c]) : to_f32<E>(sr[c])) * scale : -INFINITY;
     mx = fmaxf(mx, v[k]);
   }
 #pragma unroll
@@ -193,17 +228,21 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const typename E::T* 
 #pragma unroll
   for (int k = 0; k < 16; ++k) {
     const int c = lane + 32 * k;
-    if (c < cols) p[static_cast<size_t>(row) * cols + c] = from_f32<E>(v[k] * inv);
+    if (c >= cols) continue;
+    const float x = v[k] * inv;
+    const typename E::T hi = from_f32<E>(x);
+    p[static_cast<size_t>(row) * cols + c] = hi;
+    if (kS) p_lo[static_cast<size_t>(row) * cols + c] = from_f32<E>(x - to_f32<E>(hi));
   }
 }
 
 // AutoSpeedHead decode (auto_speed_head.py:53-63): DFL expectation over 16 bins x 4 sides, anchors, stride,
 // class sigmoid.  lvl [hw][ld] 16-bit: channels 0..63 box logits (side-major: side*16 + bin), 64..67 class logits.
 // out fp32 planar [8][NA]: cx, cy, w, h (pixels of the 1024x512 canvas), 4 class probabilities.  blockIdx.y = image
-// (lvl [N][hw][ld], out [N][8][NA]).
-template <class E, bool kB>
+// (lvl [N][hw][ld], out [N][8][NA]).  kS: the logits are hi + lo.
+template <class E, bool kB, bool kS = false>
 __global__ void decode_kernel(const typename E::T* __restrict__ lvl, int h, int w, int ld, float stride, int a0, int NA,
-                              float* __restrict__ out) {
+                              float* __restrict__ out, const typename E::T* __restrict__ lvl_lo = nullptr) {
   pdl_launch_dependents();
   pdl_wait();
   if (kB) {
@@ -213,12 +252,14 @@ __global__ void decode_kernel(const typename E::T* __restrict__ lvl, int h, int 
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= h * w) return;
   const typename E::T* r = lvl + static_cast<size_t>(i) * ld;
+  const typename E::T* rl = kS ? lvl_lo + static_cast<size_t>(i) * ld : nullptr;
+  auto logit = [&](int c) { return kS ? to_f32<E>(r[c]) + to_f32<E>(rl[c]) : to_f32<E>(r[c]); };
   float d[4];
 #pragma unroll
   for (int s = 0; s < 4; ++s) {
     float l[16], mx = -INFINITY;
 #pragma unroll
-    for (int k = 0; k < 16; ++k) { l[k] = to_f32<E>(r[s * 16 + k]); mx = fmaxf(mx, l[k]); }
+    for (int k = 0; k < 16; ++k) { l[k] = logit(s * 16 + k); mx = fmaxf(mx, l[k]); }
     float sum = 0.f, ex = 0.f;
 #pragma unroll
     for (int k = 0; k < 16; ++k) { const float e = expf(l[k] - mx); sum += e; ex += e * static_cast<float>(k); }
@@ -232,7 +273,7 @@ __global__ void decode_kernel(const typename E::T* __restrict__ lvl, int h, int 
   out[2 * NA + a] = (x2 - x1) * stride;
   out[3 * NA + a] = (y2 - y1) * stride;
 #pragma unroll
-  for (int c = 0; c < kNC; ++c) out[(4 + c) * NA + a] = 1.0f / (1.0f + expf(-to_f32<E>(r[64 + c])));
+  for (int c = 0; c < kNC; ++c) out[(4 + c) * NA + a] = 1.0f / (1.0f + expf(-logit(64 + c)));
 }
 
 // AutoSpeedNetworkInfer.post_process_predictions + un-letterbox (auto_speed_infer.py:71-106), one block:
@@ -354,14 +395,21 @@ __global__ void __launch_bounds__(1024) postprocess_kernel(const __grid_constant
   if (tid == 0) { p.counts[0] = s_keep_n; p.counts[1] = ncand_all; }
 }
 
-// gray (114, 114, 114) / 255 letterbox canvas with zero channels 3..7 (auto_speed_infer.py:39); npix covers all canvases
-template <class E>
-__global__ void fill_canvas_kernel(typename E::T* __restrict__ x, int npix) {
+// gray (114, 114, 114) / 255 letterbox canvas with zero channels 3..7 (auto_speed_infer.py:39); npix covers all canvases.
+// kS: also the low half x_lo of the canvas, round(114/255 - hi).
+template <class E, bool kS = false>
+__global__ void fill_canvas_kernel(typename E::T* __restrict__ x, int npix, typename E::T* __restrict__ x_lo = nullptr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npix) return;
-  const typename E::T g = from_f32<E>(__fdiv_rn(114.0f, 255.0f)), z = from_f32<E>(0.f);
+  const float gray = __fdiv_rn(114.0f, 255.0f);
+  const typename E::T g = from_f32<E>(gray), z = from_f32<E>(0.f);
 #pragma unroll
   for (int c = 0; c < 8; ++c) x[static_cast<size_t>(i) * 8 + c] = c < 3 ? g : z;
+  if (kS) {
+    const typename E::T gl = from_f32<E>(gray - to_f32<E>(g));
+#pragma unroll
+    for (int c = 0; c < 8; ++c) x_lo[static_cast<size_t>(i) * 8 + c] = c < 3 ? gl : z;
+  }
 }
 
 // ------------------------------------------------------------------ launchers
@@ -391,15 +439,32 @@ static bool vec8_ok(const char* op, int C, std::initializer_list<int> lds, std::
 // block, not tuned for the H100)
 static int as_mean_blocks(int HW) { return std::min(148, std::max(1, HW / 64)); }
 
-static int as_mean_x(int dt, const void* in, int HW, int C, int ld, float* part, float* out, int nb, cudaStream_t st) {
-  const char* op = "as_mean";
+// The split-fp16 forms (a non-NULL low half): fp16, batch 1, every low half of the op given
+static bool split_ok(const char* op, int dt, int nb, std::initializer_list<const void*> los) {
+  if (dt != VPB_F16 || nb != 1) {
+    vpb_set_error("%s: the split-fp16 form takes dtype VPB_F16 and batch 1 (dtype %d, batch %d)", op, dt, nb);
+    return false;
+  }
+  for (const void* p : los)
+    if (!p) { vpb_set_error("%s: split-fp16 form: NULL low half", op); return false; }
+  return true;
+}
+
+static int as_mean_x(int dt, const void* in, const void* in_lo, int HW, int C, int ld, float* part, float* out, int nb,
+                     cudaStream_t st) {
+  const char* op = in_lo ? "as_mean_split" : "as_mean";
   if (!batch_ok(op, nb) || !ptrs_ok(op, {in, part, out})) return VPB_ERR_ARG;
+  if (in_lo && !split_ok(op, dt, nb, {in_lo})) return VPB_ERR_ARG;
   // ppb = 256 / C pixels per pass: C > 256 would make it 0 and the mean silently zero
   if (C < 1 || C > 256 || HW < 1 || ld < C) { vpb_set_error("%s: HW=%d C=%d ld=%d (C 1..256, ld >= C)", op, HW, C, ld); return VPB_ERR_ARG; }
   const int nblk = as_mean_blocks(HW);
-  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+  using H16 = F16::T;
+  if (in_lo)
+    VPB_CUDA_OK(launch_k(mean_part_kernel<F16, false, true>, dim3(nblk), dim3(256), 0, st, static_cast<const H16*>(in), HW, C, ld, part, static_cast<const H16*>(in_lo)));
+  else VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
     using E = decltype(tag);
-    return launch_k(nb > 1 ? mean_part_kernel<E, true> : mean_part_kernel<E, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const typename E::T*>(in), HW, C, ld, part);
+    using T16 = typename E::T;
+    return launch_k(nb > 1 ? mean_part_kernel<E, true> : mean_part_kernel<E, false>, dim3(nblk, nb), dim3(256), 0, st, static_cast<const T16*>(in), HW, C, ld, part, static_cast<const T16*>(nullptr));
   }));
   VPB_CUDA_OK(launch_k(nb > 1 ? mean_final_kernel<true> : mean_final_kernel<false>, dim3((C + 127) / 128, nb), dim3(128), 0, st, static_cast<const float*>(part), nblk, C, 1.0f / HW, out));
   return VPB_OK;
@@ -418,14 +483,22 @@ static int as_upsample2_x(int dt, const void* in, int H, int W, int C, int ld_in
   return VPB_OK;
 }
 
-static int as_maxpool5_x(int dt, const void* in, int H, int W, int C, int ld, void* out, int nb, cudaStream_t st) {
-  const char* op = "as_maxpool5";
-  if (!batch_ok(op, nb) || !ptrs_ok(op, {in, out}) || !vec8_ok(op, C, {ld}, {in, out})) return VPB_ERR_ARG;
+static int as_maxpool5_x(int dt, const void* in, const void* in_lo, int H, int W, int C, int ld, void* out, void* out_lo,
+                         int nb, cudaStream_t st) {
+  const bool sp = in_lo || out_lo;
+  const char* op = sp ? "as_maxpool5_split" : "as_maxpool5";
+  if (!batch_ok(op, nb) || !ptrs_ok(op, {in, out})) return VPB_ERR_ARG;
+  if (sp && !split_ok(op, dt, nb, {in_lo, out_lo})) return VPB_ERR_ARG;
+  if (!vec8_ok(op, C, {ld}, {in, out, in_lo, out_lo})) return VPB_ERR_ARG;
   if (H < 1 || W < 1) { vpb_set_error("%s: H=%d W=%d", op, H, W); return VPB_ERR_ARG; }
   const dim3 g((H * W * (C / 8) + 255) / 256, nb), b(256);
-  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+  const uint4* il = static_cast<const uint4*>(in_lo);
+  uint4* ol = static_cast<uint4*>(out_lo);
+  if (sp)
+    VPB_CUDA_OK(launch_k(maxpool5_kernel<F16, false, true>, g, b, 0, st, static_cast<const uint4*>(in), H, W, C / 8, ld / 8, static_cast<uint4*>(out), il, ol));
+  else VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
     using E = decltype(tag);
-    return launch_k(nb > 1 ? maxpool5_kernel<E, true> : maxpool5_kernel<E, false>, g, b, 0, st, static_cast<const uint4*>(in), H, W, C / 8, ld / 8, static_cast<uint4*>(out));
+    return launch_k(nb > 1 ? maxpool5_kernel<E, true> : maxpool5_kernel<E, false>, g, b, 0, st, static_cast<const uint4*>(in), H, W, C / 8, ld / 8, static_cast<uint4*>(out), il, ol);
   }));
   return VPB_OK;
 }
@@ -443,31 +516,43 @@ static int as_split_v_x(int dt, const void* qkv, int T, int nh, int dk, int dh, 
   return VPB_OK;
 }
 
-static int as_softmax_rows_x(int dt, const void* s, int rows, int cols, float scale, void* p, cudaStream_t st) {
-  const char* op = "as_softmax_rows";
+static int as_softmax_rows_x(int dt, const void* s, const void* s_lo, int rows, int cols, float scale, void* p, void* p_lo,
+                             cudaStream_t st) {
+  const bool sp = s_lo || p_lo;
+  const char* op = sp ? "as_softmax_rows_split" : "as_softmax_rows";
   if (!ptrs_ok(op, {s, p})) return VPB_ERR_ARG;
+  if (sp && !split_ok(op, dt, 1, {s_lo, p_lo})) return VPB_ERR_ARG;
   // one warp holds a row in 16 registers per lane
   if (rows < 1 || cols < 1 || cols > 512) { vpb_set_error("%s: rows=%d cols=%d (cols 1..512)", op, rows, cols); return VPB_ERR_ARG; }
   const dim3 g((rows + 7) / 8), b(256);
-  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+  using H16 = F16::T;
+  if (sp)
+    VPB_CUDA_OK(launch_k(softmax_rows_kernel<F16, true>, g, b, 0, st, static_cast<const H16*>(s), rows, cols, scale, static_cast<H16*>(p), static_cast<const H16*>(s_lo), static_cast<H16*>(p_lo)));
+  else VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
     using E = decltype(tag);
-    return launch_k(softmax_rows_kernel<E>, g, b, 0, st, static_cast<const typename E::T*>(s), rows, cols, scale, static_cast<typename E::T*>(p));
+    using T16 = typename E::T;
+    return launch_k(softmax_rows_kernel<E>, g, b, 0, st, static_cast<const T16*>(s), rows, cols, scale, static_cast<T16*>(p), static_cast<const T16*>(nullptr), static_cast<T16*>(nullptr));
   }));
   return VPB_OK;
 }
 
-static int as_decode_x(int dt, const void* lvl, int h, int w, int ld, float stride, int a0, int NA, float* out, int nb,
-                       cudaStream_t st) {
-  const char* op = "as_decode";
+static int as_decode_x(int dt, const void* lvl, const void* lvl_lo, int h, int w, int ld, float stride, int a0, int NA,
+                       float* out, int nb, cudaStream_t st) {
+  const char* op = lvl_lo ? "as_decode_split" : "as_decode";
   if (!batch_ok(op, nb) || !ptrs_ok(op, {lvl, out})) return VPB_ERR_ARG;
+  if (lvl_lo && !split_ok(op, dt, nb, {lvl_lo})) return VPB_ERR_ARG;
   if (h < 1 || w < 1 || ld < 4 * kDfl + kNC || a0 < 0 || a0 + h * w > NA) {
     vpb_set_error("%s: h=%d w=%d ld=%d a0=%d NA=%d (ld >= %d, a0 + h*w <= NA)", op, h, w, ld, a0, NA, 4 * kDfl + kNC);
     return VPB_ERR_ARG;
   }
   const dim3 g((h * w + 127) / 128, nb), bb(128);
-  VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
+  using H16 = F16::T;
+  if (lvl_lo)
+    VPB_CUDA_OK(launch_k(decode_kernel<F16, false, true>, g, bb, 0, st, static_cast<const H16*>(lvl), h, w, ld, stride, a0, NA, out, static_cast<const H16*>(lvl_lo)));
+  else VPB_CUDA_OK(dispatch_dtype(dt, [&](auto tag) {
     using E = decltype(tag);
-    return launch_k(nb > 1 ? decode_kernel<E, true> : decode_kernel<E, false>, g, bb, 0, st, static_cast<const typename E::T*>(lvl), h, w, ld, stride, a0, NA, out);
+    using T16 = typename E::T;
+    return launch_k(nb > 1 ? decode_kernel<E, true> : decode_kernel<E, false>, g, bb, 0, st, static_cast<const T16*>(lvl), h, w, ld, stride, a0, NA, out, static_cast<const T16*>(nullptr));
   }));
   return VPB_OK;
 }
@@ -605,8 +690,8 @@ struct ASBuilder {
     if (!fold(p, in.C, 1, 3, wt, bias, true)) return;
     float *dwt = e.upload_f32(wt), *db = e.upload_f32(bias);
     const int dt = e.dtype, H = in.H, W = in.W, C = in.C, nb = e.batch;
-    const void* ip = in.p; void* op_ = out.p; long long* gap = e.d_gap_scratch;
-    e.add_op(p, "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, ip, nullptr, H, W, C, 3, 1, dwt, db, op_, nullptr, gap, st, act ? VPB_ACT_SILU : VPB_ACT_NONE, nb); },
+    const void* ip = in.p; const void* il = in.lo; void* op_ = out.p; void* ol = out.lo; long long* gap = e.d_gap_scratch;
+    e.add_op(p, "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, ip, il, H, W, C, 3, 1, dwt, db, op_, ol, gap, st, act ? VPB_ACT_SILU : VPB_ACT_NONE, nb); },
              2.0 * H * W * C * 9, nb * 4.0 * H * W * C);
   }
   // CTX (common_layers.py:194-239): x [h][w][C] -> out [h][w][Cout]
@@ -620,9 +705,9 @@ struct ASBuilder {
     float* d_part = static_cast<float*>(e.dalloc(static_cast<size_t>(as_mean_blocks(HW)) * C * 4 * nb));
     float* d_mean = static_cast<float*>(e.dalloc(static_cast<size_t>(C) * 4 * nb));
     {
-      const void* ip = x.p; const int ld = x.ld;
+      const void* ip = x.p; const void* il = x.lo; const int ld = x.ld;
       // two launches; the partial sums and the means are small next to the activation read
-      e.add_op(p + ".mean", "mean_part_kernel", [=](cudaStream_t st) { return as_mean_x(dt, ip, HW, C, ld, d_part, d_mean, nb, st); },
+      e.add_op(p + ".mean", "mean_part_kernel", [=](cudaStream_t st) { return as_mean_x(dt, ip, il, HW, C, ld, d_part, d_mean, nb, st); },
                0.0, nb * 2.0 * HW * C);
     }
     // exp0: Conv1d(k=3, pad 1) on a length-1 sequence == the centre tap as a Linear(C -> h*w); SiLU twice (:218-221)
@@ -637,8 +722,8 @@ struct ASBuilder {
     Tens c2 = e.act_alloc(H, W, C / 2);
     float *d_c0w = e.upload_f32(c0w->f), *d_c0b = e.upload_f32(c0b->f);
     {
-      void* op_ = c2.p; const int co = C / 2;
-      e.add_op(p + ".ctx0", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, nullptr, 0, st, ACT_SILU, nb); },
+      void* op_ = c2.p; void* ol = c2.lo; const int co = C / 2;
+      e.add_op(p + ".ctx0", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, ol, 0, st, ACT_SILU, nb); },
                2.0 * HW * co * 9, nb * 2.0 * HW * co);
     }
     // ctx1: SiLU(conv) * x + x, then SiLU (:224-232) — one wgmma conv with the MULADD epilogue and a post activation
@@ -672,17 +757,20 @@ struct ASBuilder {
     }
     cbs(p + ".conv2", cat, out, cout, 1, 1, true);
   }
+  // a pure copy: the split-fp16 mode runs the same kernel once more on the low halves
   void upsample(const std::string& name, const Tens& in, const Tens& out) {
     const int dt = e.dtype, H = in.H, W = in.W, C = in.C, li = in.ld, lo = out.ld, nb = e.batch;
-    const void* ip = in.p; void* op_ = out.p;
-    e.add_op(name, "upsample2_kernel", [=](cudaStream_t st) { return as_upsample2_x(dt, ip, H, W, C, li, op_, lo, nb, st); },
-             0.0, nb * 10.0 * H * W * C);
+    const void* ip = in.p; void* op_ = out.p; const void* il = in.lo; void* ol = out.lo;
+    e.add_op(name, "upsample2_kernel", [=](cudaStream_t st) {
+      const int rc = as_upsample2_x(dt, ip, H, W, C, li, op_, lo, nb, st);
+      return rc || !il ? rc : as_upsample2_x(dt, il, H, W, C, li, ol, lo, nb, st);
+    }, 0.0, (il ? 2 : 1) * nb * 10.0 * H * W * C);
   }
   void maxpool(const std::string& name, const Tens& in, const Tens& out) {
     const int dt = e.dtype, H = in.H, W = in.W, C = in.C, ld = in.ld, nb = e.batch;
-    const void* ip = in.p; void* op_ = out.p;
-    e.add_op(name, "maxpool5_kernel", [=](cudaStream_t st) { return as_maxpool5_x(dt, ip, H, W, C, ld, op_, nb, st); },
-             0.0, nb * 4.0 * H * W * C);
+    const void* ip = in.p; void* op_ = out.p; const void* il = in.lo; void* ol = out.lo;
+    e.add_op(name, "maxpool5_kernel", [=](cudaStream_t st) { return as_maxpool5_x(dt, ip, il, H, W, C, ld, op_, ol, nb, st); },
+             0.0, (il ? 2 : 1) * nb * 4.0 * H * W * C);
   }
   // PSABlock on y (in place): y += attention(y); y += ffn(y)   (common_layers.py:77-118)
   void psablock(const std::string& p, const Tens& y, int nh) {
@@ -691,11 +779,17 @@ struct ASBuilder {
     Tens qkv = e.act_alloc(y.H, y.W, nh * per);
     cbs(p + ".conv1.qkv", y, qkv, nh * per, 1, 1, false);
     Tens vc = e.act_alloc(y.H, y.W, C);
-    void* vt = e.dalloc(static_cast<size_t>(nh) * dh * T * 2 * nb);          // [N][nh][dh][T]
+    // [N][nh][dh][T]; split-fp16 mode (batch 1): the low half follows
+    const size_t vt_bytes = static_cast<size_t>(nh) * dh * T * 2;
+    void* vt = e.dalloc(vt_bytes * nb * (e.split ? 2 : 1));
+    void* vt_lo = e.split && vt ? static_cast<uint8_t*>(vt) + vt_bytes : nullptr;
     {
-      const void* q = qkv.p; void* vcp = vc.p;
-      e.add_op(p + ".split_v", "split_v_kernel", [=](cudaStream_t st) { return as_split_v_x(dt, q, T, nh, dk, dh, vcp, vt, nb, st); },
-               0.0, nb * 6.0 * T * nh * dh);
+      // a pure copy: the split-fp16 mode runs the same kernel once more on the low halves
+      const void* q = qkv.p; void* vcp = vc.p; const void* ql = qkv.lo; void* vcl = vc.lo;
+      e.add_op(p + ".split_v", "split_v_kernel", [=](cudaStream_t st) {
+        const int rc = as_split_v_x(dt, q, T, nh, dk, dh, vcp, vt, nb, st);
+        return rc || !ql ? rc : as_split_v_x(dt, ql, T, nh, dk, dh, vcl, vt_lo, nb, st);
+      }, 0.0, (ql ? 2 : 1) * nb * 6.0 * T * nh * dh);
     }
     Tens dwv = e.act_alloc(y.H, y.W, C);
     dw(p + ".conv1.conv1", vc, dwv, false);                     // positional term: depthwise 3x3 on v, no activation
@@ -707,21 +801,29 @@ struct ASBuilder {
       Tens s = e.act_alloc(1, T, T), pm = e.act_alloc(1, T, T);
       Tens q = qkv.slice(h * per, dk);
       Tens qv = q; qv.H = 1; qv.W = T;
-      const void* kmat = static_cast<const uint8_t*>(qkv.p) + static_cast<size_t>(h * per + dk) * 2;
-      vpb_conv_args a = conv(qv, s, T, 1, 1, kmat, nullptr, ACT_NONE, VPB_EPI_STORE, nullptr);
-      a.ldw = qkv.ld; a.w_img = T * qkv.ld;
+      // The activation "weights" carry their low halves themselves (conv_args finds only uploaded weights' halves).  The
+      // split-fp16 mode (batch 1) leaves w_img at 0: the convolution takes no per-image weights with split operands, and
+      // one image needs none.
+      const size_t koff = static_cast<size_t>(h * per + dk) * 2;
+      vpb_conv_args a = conv(qv, s, T, 1, 1, static_cast<const uint8_t*>(qkv.p) + koff, nullptr, ACT_NONE, VPB_EPI_STORE, nullptr);
+      a.ldw = qkv.ld;
+      if (!e.split) a.w_img = T * qkv.ld;
+      if (qkv.lo) a.w_lo = static_cast<const uint8_t*>(qkv.lo) + koff;
       rc = e.append_conv(p + ".attn.qk" + std::to_string(h), a);
       if (!ok()) return;
       {
-        const void* sp = s.p; void* pp = pm.p;
+        const void* sp = s.p; void* pp = pm.p; const void* sl = s.lo; void* pl = pm.lo;
         e.add_op(p + ".attn.softmax" + std::to_string(h), "softmax_rows_kernel",
-                 [=](cudaStream_t st) { return as_softmax_rows_x(dt, sp, nb * T, T, scale, pp, st); }, 0.0, nb * 4.0 * T * T);
+                 [=](cudaStream_t st) { return as_softmax_rows_x(dt, sp, sl, nb * T, T, scale, pp, pl, st); }, 0.0, nb * 4.0 * T * T);
       }
       // O = P V^T (+ depthwise term): Cin = key tokens, "weights" = Vt[h] [dh][T] of the same sample
       Tens o = att.slice(h * dh, dh); o.H = 1; o.W = T;
       Tens r = dwv.slice(h * dh, dh); r.H = 1; r.W = T;
-      a = conv(pm, o, dh, 1, 1, static_cast<const uint8_t*>(vt) + static_cast<size_t>(h) * dh * T * 2, nullptr, ACT_NONE, VPB_EPI_ADD, &r);
-      a.ldw = T; a.w_img = nh * dh * T;
+      const size_t voff = static_cast<size_t>(h) * dh * T * 2;
+      a = conv(pm, o, dh, 1, 1, static_cast<const uint8_t*>(vt) + voff, nullptr, ACT_NONE, VPB_EPI_ADD, &r);
+      a.ldw = T;
+      if (!e.split) a.w_img = nh * dh * T;
+      if (vt_lo) a.w_lo = static_cast<const uint8_t*>(vt_lo) + voff;
       rc = e.append_conv(p + ".attn.pv" + std::to_string(h), a);
     }
     cbs(p + ".conv1.conv2", att, y, C, 1, 1, false, 0, VPB_EPI_ADD, &y);          // y = y + proj(attention)
@@ -747,7 +849,7 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   const int W0 = kASW, H0 = kASH;
   e.d_gap_scratch = static_cast<long long*>(e.dalloc(static_cast<size_t>(kGapReplicas) * 256 * 8 * e.batch + 64));
   e.add_preprocess(VPB_CONV_RGB_UNIT, e.d_canvas, nullptr);
-  Tens x0; x0.p = e.d_canvas; x0.H = H0; x0.W = W0; x0.C = 8; x0.ld = 8;
+  Tens x0; x0.p = e.d_canvas; x0.lo = e.pre.out_lo; x0.H = H0; x0.W = W0; x0.C = 8; x0.ld = 8;
   // ---- backbone (auto_speed_backbone.py:9-48)
   Tens p1 = e.act_alloc(H0 / 2, W0 / 2, 16);
   b.cbs("net.p1", x0, p1, 16, 3, 2, true, /*cin_pad=*/8);
@@ -823,10 +925,11 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
     int a0 = 0;
     const float strides[3] = {8.f, 16.f, 32.f};
     for (int i = 0; i < 3; ++i) {
-      const void* lp = lv[i].p; const int h = lv[i].H, wd = lv[i].W, ld = lv[i].ld, off = a0; const float st_ = strides[i];
+      const void* lp = lv[i].p; const void* ll = lv[i].lo; const int h = lv[i].H, wd = lv[i].W, ld = lv[i].ld, off = a0;
+      const float st_ = strides[i];
       // 4 * kDfl box and kNC class logits read, 8 fp32 written per anchor
       e.add_op("head.decode" + std::to_string(i), "decode_kernel",
-               [=](cudaStream_t st) { return as_decode_x(dt, lp, h, wd, ld, st_, off, kNA, raw, nb, st); }, 0.0,
+               [=](cudaStream_t st) { return as_decode_x(dt, lp, ll, h, wd, ld, st_, off, kNA, raw, nb, st); }, 0.0,
                nb * (2.0 * (4 * kDfl + kNC) + 32.0) * h * wd);
       a0 += h * wd;
     }
@@ -879,9 +982,11 @@ int vp_autospeed::letterbox(const PreGeom* g, cudaStream_t st) {
     scale[k] = static_cast<float>(as_scale(g[k].h, g[k].w));
     if (canvas_geom[k] == g[k]) continue;
     void* c = static_cast<uint8_t*>(d_canvas) + static_cast<size_t>(npix) * 8 * 2 * k;
-    dispatch_dtype(dtype, [&](auto tag) {
+    if (pre.out_lo)
+      fill_canvas_kernel<F16, true><<<(npix + 255) / 256, 256, 0, st>>>(static_cast<__half*>(c), npix, static_cast<__half*>(pre.out_lo));
+    else dispatch_dtype(dtype, [&](auto tag) {
       using E = decltype(tag);
-      fill_canvas_kernel<E><<<(npix + 255) / 256, 256, 0, st>>>(static_cast<typename E::T*>(c), npix);
+      fill_canvas_kernel<E><<<(npix + 255) / 256, 256, 0, st>>>(static_cast<typename E::T*>(c), npix, nullptr);
     });
     VPB_CUDA_OK(cudaGetLastError());
     canvas_geom[k] = g[k];
@@ -953,20 +1058,32 @@ int autospeed_fetch(vp_autospeed* d, bool raw, cudaStream_t st) { return d->fetc
 
 int autospeed_fetch_rest(vp_autospeed* d) { return d->fetch_rest(); }
 
-static int as_create(const char* who, const char* weights_vpw, int gpu_id, int dtype, void* stream, int batch,
-                     vp_autospeed** out) {
+static int as_create(const char* who, const char* weights_vpw, int gpu_id, int dtype, int precision, void* stream,
+                     int batch, vp_autospeed** out) {
   if (!out) return VPB_ERR_ARG;
   *out = nullptr;
   if (batch < 1 || batch > kMaxBatch) { vpb_set_error("%s: batch %d out of range (1..%d)", who, batch, kMaxBatch); return VPB_ERR_ARG; }
+  if (precision != VP_PREC_16 && precision != VP_PREC_SPLIT) { vpb_set_error("%s: unknown precision %d", who, precision); return VPB_ERR_ARG; }
+  const bool split = precision == VP_PREC_SPLIT;
+  if (split && batch != 1) {
+    vpb_set_error("%s: batch %d needs the 16-bit precision (the split-fp16 mode runs one frame per call)", who, batch);
+    return VPB_ERR_ARG;
+  }
+  if (split && dtype != VPB_F16) {
+    vpb_set_error("%s: the split-fp16 mode takes dtype VPB_F16 (fp16 pairs), got %d", who, dtype);
+    return VPB_ERR_ARG;
+  }
   if (!weights_vpw || !weights_vpw[0]) { vpb_set_error("%s: no checkpoint path", who); return VPB_ERR_ARG; }
   std::unique_ptr<vp_autospeed> e(new vp_autospeed());
   int rc = e->open(who, gpu_id, stream);
   if (rc) return rc;
   DeviceGuard guard(gpu_id);
   e->dtype = dtype == VPB_BF16 ? VPB_BF16 : VPB_F16;
+  e->split = split;
   e->batch = batch;
-  const size_t nb = batch;
-  e->d_canvas = e->dalloc(static_cast<size_t>(kASW) * kASH * 8 * 2 * nb);
+  const size_t nb = batch, canvas_bytes = static_cast<size_t>(kASW) * kASH * 8 * 2;
+  e->d_canvas = e->dalloc(canvas_bytes * nb * (split ? 2 : 1));     // split: the low half follows the canvas
+  if (split && e->d_canvas) e->pre.out_lo = static_cast<uint8_t*>(e->d_canvas) + canvas_bytes;
   e->pre.out_pitch = kASW; e->pre.out_rows = kASH; e->pre.out_c = 8;
   for (int k = 0; k < batch; ++k) e->canvas_geom[k].h = -1;   // no border filled yet
   e->d_raw = static_cast<float*>(e->dalloc(static_cast<size_t>(8) * kNA * 4 * nb));
@@ -1007,12 +1124,17 @@ static bool sample_ok(const vp_autospeed* e, int sample, const char* who) {
 
 // ====================================================================== C-ABI
 extern "C" int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtype, void* stream, vp_autospeed** out) {
-  return as_create("vp_autospeed_create", weights_vpw, gpu_id, dtype, stream, 1, out);
+  return as_create("vp_autospeed_create", weights_vpw, gpu_id, dtype, VP_PREC_16, stream, 1, out);
 }
 
 extern "C" int vp_autospeed_create_batch(const char* weights_vpw, int gpu_id, int dtype, void* stream, int batch,
                                          vp_autospeed** out) {
-  return as_create("vp_autospeed_create_batch", weights_vpw, gpu_id, dtype, stream, batch, out);
+  return as_create("vp_autospeed_create_batch", weights_vpw, gpu_id, dtype, VP_PREC_16, stream, batch, out);
+}
+
+extern "C" int vp_autospeed_create_precision(const char* weights_vpw, int gpu_id, int dtype, int precision, void* stream,
+                                             int batch, vp_autospeed** out) {
+  return as_create("vp_autospeed_create_precision", weights_vpw, gpu_id, dtype, precision, stream, batch, out);
 }
 
 extern "C" void vp_autospeed_destroy(vp_autospeed* e) { delete e; }
@@ -1130,7 +1252,13 @@ extern "C" long vp_autospeed_read_tap(vp_autospeed* e, const char* name, float* 
 extern "C" int vpb_as_mean_blocks(int HW) { return as_mean_blocks(HW); }
 
 extern "C" int vpb_as_mean(int dtype, const void* in, int HW, int C, int ld, float* part, float* out, int batch, void* stream) {
-  return as_mean_x(dtype, in, HW, C, ld, part, out, batch, static_cast<cudaStream_t>(stream));
+  return as_mean_x(dtype, in, nullptr, HW, C, ld, part, out, batch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_mean_split(const void* in, const void* in_lo, int HW, int C, int ld, float* part, float* out,
+                                 void* stream) {
+  if (!in_lo) { vpb_set_error("as_mean_split: NULL low half"); return VPB_ERR_ARG; }
+  return as_mean_x(VPB_F16, in, in_lo, HW, C, ld, part, out, 1, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_as_upsample2(int dtype, const void* in, int H, int W, int C, int ld_in, void* out, int ld_out, int batch,
@@ -1139,7 +1267,13 @@ extern "C" int vpb_as_upsample2(int dtype, const void* in, int H, int W, int C, 
 }
 
 extern "C" int vpb_as_maxpool5(int dtype, const void* in, int H, int W, int C, int ld, void* out, int batch, void* stream) {
-  return as_maxpool5_x(dtype, in, H, W, C, ld, out, batch, static_cast<cudaStream_t>(stream));
+  return as_maxpool5_x(dtype, in, nullptr, H, W, C, ld, out, nullptr, batch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_maxpool5_split(const void* in, const void* in_lo, int H, int W, int C, int ld, void* out,
+                                     void* out_lo, void* stream) {
+  if (!in_lo || !out_lo) { vpb_set_error("as_maxpool5_split: NULL low half"); return VPB_ERR_ARG; }
+  return as_maxpool5_x(VPB_F16, in, in_lo, H, W, C, ld, out, out_lo, 1, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_as_split_v(int dtype, const void* qkv, int T, int nh, int dk, int dh, void* vc, void* vt, int batch,
@@ -1148,12 +1282,24 @@ extern "C" int vpb_as_split_v(int dtype, const void* qkv, int T, int nh, int dk,
 }
 
 extern "C" int vpb_as_softmax_rows(int dtype, const void* s, int rows, int cols, float scale, void* p, void* stream) {
-  return as_softmax_rows_x(dtype, s, rows, cols, scale, p, static_cast<cudaStream_t>(stream));
+  return as_softmax_rows_x(dtype, s, nullptr, rows, cols, scale, p, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_softmax_rows_split(const void* s, const void* s_lo, int rows, int cols, float scale, void* p,
+                                         void* p_lo, void* stream) {
+  if (!s_lo || !p_lo) { vpb_set_error("as_softmax_rows_split: NULL low half"); return VPB_ERR_ARG; }
+  return as_softmax_rows_x(VPB_F16, s, s_lo, rows, cols, scale, p, p_lo, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_as_decode(int dtype, const void* lvl, int h, int w, int ld, float stride, int a0, int NA, float* out,
                              int batch, void* stream) {
-  return as_decode_x(dtype, lvl, h, w, ld, stride, a0, NA, out, batch, static_cast<cudaStream_t>(stream));
+  return as_decode_x(dtype, lvl, nullptr, h, w, ld, stride, a0, NA, out, batch, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_as_decode_split(const void* lvl, const void* lvl_lo, int h, int w, int ld, float stride, int a0, int NA,
+                                   float* out, void* stream) {
+  if (!lvl_lo) { vpb_set_error("as_decode_split: NULL low half"); return VPB_ERR_ARG; }
+  return as_decode_x(VPB_F16, lvl, lvl_lo, h, w, ld, stride, a0, NA, out, 1, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_as_postprocess(const float* raw, int NA, int batch, float conf, float iou, const float* scale,

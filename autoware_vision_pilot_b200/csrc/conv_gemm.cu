@@ -625,7 +625,8 @@ int conv_plan_build(const vpb_conv_args* a, ConvPlan* plan) {
   }
   const int cstride = a->stride == 2 ? 2 : 1;
   if (a->stride != 0 && a->stride != 1 && a->stride != 2) { vpb_set_error("conv: stride %d unsupported", a->stride); return VPB_ERR_ARG; }
-  if (cstride == 2 && (a->algo == VPB_ALGO_LINEAR || a->phases != 1 || a->in_pad || a->in2 || a->in_lo)) {
+  // the split-fp16 mode's low half (map Alo) is encoded and loaded like the first input's, element stride included
+  if (cstride == 2 && (a->algo == VPB_ALGO_LINEAR || a->phases != 1 || a->in_pad || a->in2)) {
     vpb_set_error("conv: stride 2 needs the TILE algorithm on an unpadded input, phases = 1, no second input");
     return VPB_ERR_ARG;
   }

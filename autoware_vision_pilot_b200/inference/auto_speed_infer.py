@@ -33,7 +33,8 @@ def _resolve(path: str) -> str:
 class AutoSpeedNetworkInfer:
     """Same boundary as the reference helper: `AutoSpeedNetworkInfer(checkpoint_path)`, `.inference(PIL image)` ->
     `[[x1, y1, x2, y2, score, class], ...]` in original-image coordinates (auto_speed_infer.py:88-108).  Letterbox,
-    network, decode, the second sigmoid + 0.6 filter and the NMS all run on the GPU inside one C-ABI call."""
+    network, decode, the second sigmoid + 0.6 filter and the NMS all run on the GPU inside one C-ABI call.
+    precision "fp16" (the helper's `.half()`), "bf16", or "fp32": the split-fp16 fp32-grade detector."""
 
     def __init__(self, checkpoint_path: str = "", *, gpu_id: int = 0, precision: str = "fp16"):
         self.train_size = (1024, 512)

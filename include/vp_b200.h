@@ -50,7 +50,6 @@ extern "C" {
 
 /* network kinds (the four Models/model_components network modules, e.g. scene_seg_network.py) */
 enum { VP_SCENE_SEG = 0, VP_SCENE_3D = 1, VP_DOMAIN_SEG = 2, VP_EGO_LANES = 3 };
-enum { VP_PREC_16 = 0, VP_PREC_SPLIT = 1 };
 
 typedef struct vp_engine vp_engine;
 struct vp_autospeed;                /* the AutoSpeed detector, vp_b200_autospeed.h (vp_engine_set_detector) */
@@ -193,8 +192,9 @@ int vp_engine_set_roi(vp_engine* e, int sample, int x, int y, int w, int h);
  * infer call copies the detections (every one of them) to det's host buffers, and the raw tensors with
  * vp_engine_config.fetch_raw; after a submit or a device call: vp_engine_sync, then vp_autospeed_sync(det, fetch).
  * vp_engine_profile, _kernel_names, _time_kernel and _get_stats include the detector's ops.  det NULL detaches.  The
- * engine does not own det, which must outlive the attachment.  VPB_ERR_ARG for a NULL engine, or a detector of
- * another batch or GPU. */
+ * engine does not own det, which must outlive the attachment.  A split-fp16 detector (vp_autospeed_create_precision,
+ * batch 1) attaches to any batch-1 engine, 16-bit or split; its copied ops are its split launches and det/letterbox
+ * writes its canvas low half.  VPB_ERR_ARG for a NULL engine, or a detector of another batch or GPU. */
 int vp_engine_set_detector(vp_engine* e, struct vp_autospeed* det);
 
 /* The lateral post-process inside the call (production_release/main.cpp:505-577: EgoLanes -> LaneFilter ->

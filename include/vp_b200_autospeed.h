@@ -25,6 +25,7 @@
  * The checkpoint is a .vpw file holding the module's state_dict (python -m autoware_vision_pilot_b200.convert);
  * BatchNorm (eps 1e-3) is folded at load.  16-bit operands on the wgmma tensor cores, fp32 accumulation, exactly
  * like the reference helper's own half-precision inference (auto_speed_infer.py:50 `.half()`).
+ * vp_autospeed_create_precision(..., VP_PREC_SPLIT, ...) builds the split-fp16 detector instead (see there).
  * No CPU fallback: creation fails with VPB_ERR_CUDA without an sm_90 device.
  */
 #ifndef VP_B200_AUTOSPEED_H_
@@ -43,6 +44,19 @@ int vp_autospeed_create(const char* weights_vpw, int gpu_id, int dtype /* VPB_F1
                         vp_autospeed** out);
 /* batch 1..VP_MAX_BATCH (vp_b200.h) frames per call; VPB_ERR_ARG otherwise, before the device is opened */
 int vp_autospeed_create_batch(const char* weights_vpw, int gpu_id, int dtype, void* stream, int batch, vp_autospeed** out);
+/* precision VP_PREC_16 (vp_b200_ops.h): exactly vp_autospeed_create_batch.  VP_PREC_SPLIT: the split-fp16 "fp32-grade"
+ * detector for the reference's precision="fp32" (run_model_node.cpp:29-36, tensorrt_backend.cpp:129-131), as the
+ * segmentation engine's VP_PREC_SPLIT: every 16-bit tensor (the letterbox canvas, every activation, the attention's
+ * qkv, S, P and V^T) is an fp16 (hi, lo) pair of one layout, hi = round(x), lo = round(x - hi) (~22 significant bits),
+ * and every wgmma convolution accumulates A_hi W_hi + A_lo W_hi + A_hi W_lo in fp32.  The raw tensor, the candidates
+ * and the detections stay fp32, and the confidence filter and NMS are those of the 16-bit mode.  Every output has the
+ * same shape and meaning as in the 16-bit mode; vp_autospeed_read_tap returns hi + lo; vp_autospeed_stats reports the
+ * same algorithmic FLOPs, while the split GEMMs execute about 3x that tensor work.  The split detector runs one frame
+ * per call and may be attached to any batch-1 engine, 16-bit or split (vp_engine_set_detector).
+ * VPB_ERR_ARG, naming the call, before the device is opened or the file read, for a precision other than these two,
+ * VP_PREC_SPLIT with batch != 1, or VP_PREC_SPLIT with a dtype other than VPB_F16. */
+int vp_autospeed_create_precision(const char* weights_vpw, int gpu_id, int dtype, int precision, void* stream, int batch,
+                                  vp_autospeed** out);
 void vp_autospeed_destroy(vp_autospeed* e);
 /* conf_thres / iou_thres of post_process_predictions (defaults 0.6 / 0.45, auto_speed_infer.py:71) */
 int vp_autospeed_set_thresholds(vp_autospeed* e, float conf, float iou);
@@ -138,6 +152,21 @@ int vpb_as_decode(int dtype, const void* lvl, int h, int w, int ld, float stride
 int vpb_as_postprocess(const float* raw, int NA, int batch, float conf, float iou, const float* scale, const int* pad_x,
                        const int* pad_y, const int* orig_w, const int* orig_h, float* cand, int* order, float* det,
                        int* counts, void* stream);
+/* The split-fp16 forms the VP_PREC_SPLIT detector launches: fp16, batch 1, each 16-bit tensor an (hi, lo) pair of one
+ * layout (every *_lo pointer non-NULL, with the alignment its hi partner needs), otherwise the contract of the op above.
+ *   mean      sums hi + lo (exact in fp32)
+ *   maxpool5  out, out_lo = the input pair of the largest hi + lo of each window (the pairs compared lexicographically;
+ *             a NaN hi is dropped)
+ *   softmax   reads hi + lo of s * scale, writes p = hi + lo split (hi = round(p), lo = round(p - hi))
+ *   decode    reads hi + lo of the logits
+ * Upsample and the V split are pure copies: the detector runs vpb_as_upsample2 / vpb_as_split_v once per half. */
+int vpb_as_mean_split(const void* in, const void* in_lo, int HW, int C, int ld, float* part, float* out, void* stream);
+int vpb_as_maxpool5_split(const void* in, const void* in_lo, int H, int W, int C, int ld, void* out, void* out_lo,
+                          void* stream);
+int vpb_as_softmax_rows_split(const void* s, const void* s_lo, int rows, int cols, float scale, void* p, void* p_lo,
+                              void* stream);
+int vpb_as_decode_split(const void* lvl, const void* lvl_lo, int h, int w, int ld, float stride, int a0, int NA,
+                        float* out, void* stream);
 
 #ifdef __cplusplus
 }

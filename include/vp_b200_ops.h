@@ -23,6 +23,9 @@ extern "C" {
 
 enum { VPB_OK = 0, VPB_ERR_ARG = -1, VPB_ERR_CUDA = -2, VPB_ERR_STATE = -3, VPB_ERR_IO = -4 };
 enum { VPB_F16 = 0, VPB_BF16 = 1 };
+/* precision of an engine (vp_engine_config.precision, vp_b200.h) or a detector (vp_autospeed_create_precision,
+ * vp_b200_autospeed.h): 16-bit operands, or split-fp16 (hi, lo) pairs for the reference's precision="fp32" */
+enum { VP_PREC_16 = 0, VP_PREC_SPLIT = 1 };
 enum { VPB_ACT_NONE = 0, VPB_ACT_GELU = 1, VPB_ACT_SILU = 2, VPB_ACT_SIGMOID = 3, VPB_ACT_SILU2 = 4 /* SiLU(SiLU(x)) */ };
 /* conv epilogue modes */
 enum {
@@ -152,7 +155,8 @@ typedef struct {
   /* Widening for the AutoSpeed detector (SURVEY.md 8f.4), TILE algorithm:
    *   stride   1 (default when 0) or 2: Conv2d 3x3 / 1x1 with stride 2, padding 1 (common_layers.py:8 with s=2);
    *            H, W are the OUTPUT size, in_h x in_w the input size (0 = H x W); the input is sampled through the
-   *            tensor map's traversal stride, zero padding stays the TMA unit's out-of-bounds fill;
+   *            tensor map's traversal stride, zero padding stays the TMA unit's out-of-bounds fill (the split-fp16
+   *            mode's in_lo alike);
    *   ldw      elements between consecutive output-channel rows of w (0 = Cin): lets a [tokens][channels] activation
    *            slice act as the weight matrix (attention: S = Q K^T, O = P V^T as 1x1 "convolutions");
    *   act2     activation applied AFTER the residual step of modes ADD / MULADD (CTX block: SiLU(SiLU(conv) * x + x),

@@ -604,7 +604,6 @@ struct vp_autospeed : EngineRuntime {
   float* d_raw = nullptr; float* h_raw = nullptr;
   float* d_cand = nullptr; int* d_order = nullptr; float* d_det = nullptr; int* d_counts = nullptr;
   float* h_det = nullptr; int* h_counts = nullptr;
-  long long* d_gap_scratch = nullptr;
   float scale[kMaxBatch] = {};             // letterbox of each sample of the last call (geometry in pre.geom)
   PreGeom canvas_geom[kMaxBatch];          // the letterbox each sample's canvas border was last filled for
   float conf = 0.6f, iou = 0.45f;
@@ -623,39 +622,18 @@ struct vp_autospeed : EngineRuntime {
 
 namespace vpb {
 
-struct ASBuilder {
-  vp_autospeed& e;
-  const WeightMap& w;
-  int rc = VPB_OK;
-  bool ok() const { return rc == VPB_OK && !e.oom; }
+// The detector's layers on the shared NetBuilder
+struct ASBuilder : NetBuilder {
+  long long* gap;   // the depthwise kernel's SE partial sums, which no AutoSpeed layer reads
 
   // vpb_conv_args of one wgmma convolution in -> out, a channel slice; H x W is the output's size (stride 1 or 2)
-  vpb_conv_args conv(const Tens& in, const Tens& out, int cout, int taps, int stride, const void* wt, const float* bias,
+  vpb_conv_args args(const Tens& in, const Tens& out, int cout, int taps, int stride, const void* wt, const float* bias,
                      int act, int mode, const Tens* res) const {
     vpb_conv_args a = e.conv_args(in, &out, res, cout, taps, 1, wt, bias, act, mode);
     a.H = out.H; a.W = out.W; a.stride = stride; a.in_h = in.H; a.in_w = in.W; a.out_slice = 1;
     return a;
   }
 
-  // Conv = Conv2d(bias=False) + BatchNorm2d(eps 1e-3) [+ SiLU] (common_layers.py:5-17), folded
-  bool fold(const std::string& p, int cout, int cin_per_g, int k, std::vector<float>& wt, std::vector<float>& bias,
-            bool depthwise) {
-    const HostTensor* cw = find_w_shaped(w, p + ".conv.weight", {cout, cin_per_g, k, k});
-    const HostTensor *g = find_w_shaped(w, p + ".norm.weight", {cout}), *b = find_w_shaped(w, p + ".norm.bias", {cout}),
-                     *m = find_w_shaped(w, p + ".norm.running_mean", {cout}), *v = find_w_shaped(w, p + ".norm.running_var", {cout});
-    if (!cw || !g || !b || !m || !v) { rc = VPB_ERR_IO; return false; }
-    std::vector<float> s(cout);
-    bias.resize(cout);
-    for (int c = 0; c < cout; ++c) { s[c] = g->f[c] / std::sqrt(v->f[c] + kBnEps); bias[c] = b->f[c] - m->f[c] * s[c]; }
-    if (depthwise) {                                   // [C][1][k][k] -> [k*k][C]
-      wt.assign(static_cast<size_t>(k) * k * cout, 0.f);
-      for (int c = 0; c < cout; ++c)
-        for (int t = 0; t < k * k; ++t) wt[static_cast<size_t>(t) * cout + c] = cw->f[static_cast<size_t>(c) * k * k + t] * s[c];
-    } else {
-      wt = pack_conv(*cw, &s);
-    }
-    return true;
-  }
   // input channels padded with zero weights (network input: 3 -> 8)
   static std::vector<float> pad_cin(const std::vector<float>& wt, int taps, int cout, int cin, int cin_pad) {
     std::vector<float> o(static_cast<size_t>(taps) * cout * cin_pad, 0.f);
@@ -664,68 +642,61 @@ struct ASBuilder {
         for (int ci = 0; ci < cin; ++ci) o[(static_cast<size_t>(t) * cout + co) * cin_pad + ci] = wt[(static_cast<size_t>(t) * cout + co) * cin + ci];
     return o;
   }
+  // Conv = Conv2d(bias=False) + BatchNorm2d(eps 1e-3) [+ SiLU] (common_layers.py:5-17), folded
   void cbs(const std::string& p, const Tens& in, const Tens& out, int cout, int k, int stride, bool act, int cin_pad = 0,
            int mode = VPB_EPI_STORE, const Tens* res = nullptr) {
-    if (!ok()) return;
-    const int cin = cin_pad ? 3 : in.C;
-    std::vector<float> wt, bias;
-    if (!fold(p, cout, cin, k, wt, bias, false)) return;
-    if (cin_pad) wt = pad_cin(wt, k * k, cout, cin, cin_pad);
-    rc = e.append_conv(p, conv(in, out, cout, k * k, stride, e.upload_16(wt), e.upload_f32(bias), act ? ACT_SILU : ACT_NONE, mode, res));
+    Params f;
+    if (!cin_pad) {
+      f = folded(p + ".conv.weight", {cout, in.C, k, k}, p + ".norm.", kBnEps);
+    } else {
+      std::vector<float> s, t;
+      const HostTensor* cw = get(p + ".conv.weight", {cout, 3, k, k});
+      if (!bn(p + ".norm.", cout, kBnEps, s, t)) return;
+      f = {e.upload_16(pad_cin(pack_conv(*cw, &s), k * k, cout, 3, cin_pad)), e.upload_f32(t)};
+    }
+    conv(p, args(in, out, cout, k * k, stride, f.w, f.b, act ? ACT_SILU : ACT_NONE, mode, res));
   }
   // plain nn.Conv2d with bias (CTX convs, head output convs)
   void plain(const std::string& p, const Tens& in, const Tens& out, int cout, int k, int act, int mode = VPB_EPI_STORE,
              const Tens* res = nullptr, int act2 = ACT_NONE) {
-    if (!ok()) return;
-    const HostTensor* cw = find_w_shaped(w, p + ".weight", {cout, in.C, k, k});
-    const HostTensor* cb = find_w_shaped(w, p + ".bias", {cout});
-    if (!cw || !cb) { rc = VPB_ERR_IO; return; }
-    vpb_conv_args a = conv(in, out, cout, k * k, 1, e.upload_16(pack_conv(*cw, nullptr)), e.upload_f32(cb->f), act, mode, res);
+    const Params c = NetBuilder::plain(p, {cout, in.C, k, k});
+    vpb_conv_args a = args(in, out, cout, k * k, 1, c.w, c.b, act, mode, res);
     a.act2 = act2;
-    rc = e.append_conv(p, a);
+    conv(p, a);
   }
   void dw(const std::string& p, const Tens& in, const Tens& out, bool act) {
-    if (!ok()) return;
-    std::vector<float> wt, bias;
-    if (!fold(p, in.C, 1, 3, wt, bias, true)) return;
-    float *dwt = e.upload_f32(wt), *db = e.upload_f32(bias);
-    const int dt = e.dtype, H = in.H, W = in.W, C = in.C, nb = e.batch;
-    const void* ip = in.p; const void* il = in.lo; void* op_ = out.p; void* ol = out.lo; long long* gap = e.d_gap_scratch;
-    e.add_op(p, "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, ip, il, H, W, C, 3, 1, dwt, db, op_, ol, gap, st, act ? VPB_ACT_SILU : VPB_ACT_NONE, nb); },
-             2.0 * H * W * C * 9, nb * 4.0 * H * W * C);
+    const Params f = depthwise(p + ".conv.weight", in.C, 3, p + ".norm.", kBnEps);
+    const float *dwt = static_cast<const float*>(f.w), *db = f.b;
+    const int dt = e.dtype, nb = e.batch;
+    long long* part = gap;
+    op(p, "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, in.p, in.lo, in.H, in.W, in.C, 3, 1, dwt, db, out.p, out.lo, part, st, act ? VPB_ACT_SILU : VPB_ACT_NONE, nb); },
+       2.0 * in.H * in.W * in.C * 9, nb * 4.0 * in.H * in.W * in.C);
   }
   // CTX (common_layers.py:194-239): x [h][w][C] -> out [h][w][Cout]
   void ctx(const std::string& p, const Tens& x, const Tens& out, int cout) {
-    if (!ok()) return;
     const int C = x.C, H = x.H, W = x.W, HW = H * W, dt = e.dtype, nb = e.batch;
-    const HostTensor *ew = find_w_shaped(w, p + ".exp0.weight", {HW, C, 3}), *eb = find_w_shaped(w, p + ".exp0.bias", {HW});
-    const HostTensor *c0w = find_w_shaped(w, p + ".ctx0.weight", {C / 2, 1, 3, 3}), *c0b = find_w_shaped(w, p + ".ctx0.bias", {C / 2});
-    if (!ew || !eb || !c0w || !c0b) { rc = VPB_ERR_IO; return; }
+    const HostTensor *ew = get(p + ".exp0.weight", {HW, C, 3}), *eb = get(p + ".exp0.bias", {HW});
+    const HostTensor *c0w = get(p + ".ctx0.weight", {C / 2, 1, 3, 3}), *c0b = get(p + ".ctx0.bias", {C / 2});
+    if (!ok()) return;
     // mean over H x W
     float* d_part = static_cast<float*>(e.dalloc(static_cast<size_t>(as_mean_blocks(HW)) * C * 4 * nb));
     float* d_mean = static_cast<float*>(e.dalloc(static_cast<size_t>(C) * 4 * nb));
-    {
-      const void* ip = x.p; const void* il = x.lo; const int ld = x.ld;
-      // two launches; the partial sums and the means are small next to the activation read
-      e.add_op(p + ".mean", "mean_part_kernel", [=](cudaStream_t st) { return as_mean_x(dt, ip, il, HW, C, ld, d_part, d_mean, nb, st); },
-               0.0, nb * 2.0 * HW * C);
-    }
+    // two launches; the partial sums and the means are small next to the activation read
+    op(p + ".mean", "mean_part_kernel", [=](cudaStream_t st) { return as_mean_x(dt, x.p, x.lo, HW, C, x.ld, d_part, d_mean, nb, st); },
+       0.0, nb * 2.0 * HW * C);
     // exp0: Conv1d(k=3, pad 1) on a length-1 sequence == the centre tap as a Linear(C -> h*w); SiLU twice (:218-221)
     std::vector<float> lw(static_cast<size_t>(HW) * C);
     for (int o = 0; o < HW; ++o)
       for (int c = 0; c < C; ++c) lw[static_cast<size_t>(o) * C + c] = ew->f[(static_cast<size_t>(o) * C + c) * 3 + 1];
     float *d_lw = e.upload_f32(lw), *d_lb = e.upload_f32(eb->f);
     float* d_map = static_cast<float*>(e.dalloc(static_cast<size_t>(HW) * 4 * nb));
-    e.add_op(p + ".exp0", "linear_kernel", [=](cudaStream_t st) { return linear_x(d_mean, d_lw, d_lb, C, HW, VPB_ACT_SILU2, d_map, st, nb); },
-             2.0 * HW * C, 4.0 * HW * C);
+    op(p + ".exp0", "linear_kernel", [=](cudaStream_t st) { return linear_x(d_mean, d_lw, d_lb, C, HW, VPB_ACT_SILU2, d_map, st, nb); },
+       2.0 * HW * C, 4.0 * HW * C);
     // ctx0: Conv2d(1 -> C/2, 3x3) + SiLU
-    Tens c2 = e.act_alloc(H, W, C / 2);
+    const Tens c2 = e.act_alloc(H, W, C / 2);
     float *d_c0w = e.upload_f32(c0w->f), *d_c0b = e.upload_f32(c0b->f);
-    {
-      void* op_ = c2.p; void* ol = c2.lo; const int co = C / 2;
-      e.add_op(p + ".ctx0", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, co, op_, ol, 0, st, ACT_SILU, nb); },
-               2.0 * HW * co * 9, nb * 2.0 * HW * co);
-    }
+    op(p + ".ctx0", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, d_map, H, W, d_c0w, d_c0b, c2.C, c2.p, c2.lo, 0, st, ACT_SILU, nb); },
+       2.0 * HW * c2.C * 9, nb * 2.0 * HW * c2.C);
     // ctx1: SiLU(conv) * x + x, then SiLU (:224-232) — one wgmma conv with the MULADD epilogue and a post activation
     Tens c4 = e.act_alloc(H, W, C);
     plain(p + ".ctx1", c2, c4, C, 3, ACT_SILU, VPB_EPI_MULADD, &x, ACT_SILU);
@@ -759,18 +730,16 @@ struct ASBuilder {
   }
   // a pure copy: the split-fp16 mode runs the same kernel once more on the low halves
   void upsample(const std::string& name, const Tens& in, const Tens& out) {
-    const int dt = e.dtype, H = in.H, W = in.W, C = in.C, li = in.ld, lo = out.ld, nb = e.batch;
-    const void* ip = in.p; void* op_ = out.p; const void* il = in.lo; void* ol = out.lo;
-    e.add_op(name, "upsample2_kernel", [=](cudaStream_t st) {
-      const int rc = as_upsample2_x(dt, ip, H, W, C, li, op_, lo, nb, st);
-      return rc || !il ? rc : as_upsample2_x(dt, il, H, W, C, li, ol, lo, nb, st);
-    }, 0.0, (il ? 2 : 1) * nb * 10.0 * H * W * C);
+    const int dt = e.dtype, nb = e.batch;
+    op(name, "upsample2_kernel", [=](cudaStream_t st) {
+      const int rc = as_upsample2_x(dt, in.p, in.H, in.W, in.C, in.ld, out.p, out.ld, nb, st);
+      return rc || !in.lo ? rc : as_upsample2_x(dt, in.lo, in.H, in.W, in.C, in.ld, out.lo, out.ld, nb, st);
+    }, 0.0, (in.lo ? 2 : 1) * nb * 10.0 * in.H * in.W * in.C);
   }
   void maxpool(const std::string& name, const Tens& in, const Tens& out) {
-    const int dt = e.dtype, H = in.H, W = in.W, C = in.C, ld = in.ld, nb = e.batch;
-    const void* ip = in.p; void* op_ = out.p; const void* il = in.lo; void* ol = out.lo;
-    e.add_op(name, "maxpool5_kernel", [=](cudaStream_t st) { return as_maxpool5_x(dt, ip, il, H, W, C, ld, op_, ol, nb, st); },
-             0.0, (il ? 2 : 1) * nb * 4.0 * H * W * C);
+    const int dt = e.dtype, nb = e.batch;
+    op(name, "maxpool5_kernel", [=](cudaStream_t st) { return as_maxpool5_x(dt, in.p, in.lo, in.H, in.W, in.C, in.ld, out.p, out.lo, nb, st); },
+       0.0, (in.lo ? 2 : 1) * nb * 4.0 * in.H * in.W * in.C);
   }
   // PSABlock on y (in place): y += attention(y); y += ffn(y)   (common_layers.py:77-118)
   void psablock(const std::string& p, const Tens& y, int nh) {
@@ -783,14 +752,11 @@ struct ASBuilder {
     const size_t vt_bytes = static_cast<size_t>(nh) * dh * T * 2;
     void* vt = e.dalloc(vt_bytes * nb * (e.split ? 2 : 1));
     void* vt_lo = e.split && vt ? static_cast<uint8_t*>(vt) + vt_bytes : nullptr;
-    {
-      // a pure copy: the split-fp16 mode runs the same kernel once more on the low halves
-      const void* q = qkv.p; void* vcp = vc.p; const void* ql = qkv.lo; void* vcl = vc.lo;
-      e.add_op(p + ".split_v", "split_v_kernel", [=](cudaStream_t st) {
-        const int rc = as_split_v_x(dt, q, T, nh, dk, dh, vcp, vt, nb, st);
-        return rc || !ql ? rc : as_split_v_x(dt, ql, T, nh, dk, dh, vcl, vt_lo, nb, st);
-      }, 0.0, (ql ? 2 : 1) * nb * 6.0 * T * nh * dh);
-    }
+    // a pure copy: the split-fp16 mode runs the same kernel once more on the low halves
+    op(p + ".split_v", "split_v_kernel", [=](cudaStream_t st) {
+      const int rc = as_split_v_x(dt, qkv.p, T, nh, dk, dh, vc.p, vt, nb, st);
+      return rc || !qkv.lo ? rc : as_split_v_x(dt, qkv.lo, T, nh, dk, dh, vc.lo, vt_lo, nb, st);
+    }, 0.0, (qkv.lo ? 2 : 1) * nb * 6.0 * T * nh * dh);
     Tens dwv = e.act_alloc(y.H, y.W, C);
     dw(p + ".conv1.conv1", vc, dwv, false);                     // positional term: depthwise 3x3 on v, no activation
     Tens att = e.act_alloc(y.H, y.W, C);
@@ -805,26 +771,22 @@ struct ASBuilder {
       // split-fp16 mode (batch 1) leaves w_img at 0: the convolution takes no per-image weights with split operands, and
       // one image needs none.
       const size_t koff = static_cast<size_t>(h * per + dk) * 2;
-      vpb_conv_args a = conv(qv, s, T, 1, 1, static_cast<const uint8_t*>(qkv.p) + koff, nullptr, ACT_NONE, VPB_EPI_STORE, nullptr);
+      vpb_conv_args a = args(qv, s, T, 1, 1, static_cast<const uint8_t*>(qkv.p) + koff, nullptr, ACT_NONE, VPB_EPI_STORE, nullptr);
       a.ldw = qkv.ld;
       if (!e.split) a.w_img = T * qkv.ld;
       if (qkv.lo) a.w_lo = static_cast<const uint8_t*>(qkv.lo) + koff;
-      rc = e.append_conv(p + ".attn.qk" + std::to_string(h), a);
-      if (!ok()) return;
-      {
-        const void* sp = s.p; void* pp = pm.p; const void* sl = s.lo; void* pl = pm.lo;
-        e.add_op(p + ".attn.softmax" + std::to_string(h), "softmax_rows_kernel",
-                 [=](cudaStream_t st) { return as_softmax_rows_x(dt, sp, sl, nb * T, T, scale, pp, pl, st); }, 0.0, nb * 4.0 * T * T);
-      }
+      conv(p + ".attn.qk" + std::to_string(h), a);
+      op(p + ".attn.softmax" + std::to_string(h), "softmax_rows_kernel",
+         [=](cudaStream_t st) { return as_softmax_rows_x(dt, s.p, s.lo, nb * T, T, scale, pm.p, pm.lo, st); }, 0.0, nb * 4.0 * T * T);
       // O = P V^T (+ depthwise term): Cin = key tokens, "weights" = Vt[h] [dh][T] of the same sample
       Tens o = att.slice(h * dh, dh); o.H = 1; o.W = T;
       Tens r = dwv.slice(h * dh, dh); r.H = 1; r.W = T;
       const size_t voff = static_cast<size_t>(h) * dh * T * 2;
-      a = conv(pm, o, dh, 1, 1, static_cast<const uint8_t*>(vt) + voff, nullptr, ACT_NONE, VPB_EPI_ADD, &r);
+      a = args(pm, o, dh, 1, 1, static_cast<const uint8_t*>(vt) + voff, nullptr, ACT_NONE, VPB_EPI_ADD, &r);
       a.ldw = T;
       if (!e.split) a.w_img = nh * dh * T;
       if (vt_lo) a.w_lo = static_cast<const uint8_t*>(vt_lo) + voff;
-      rc = e.append_conv(p + ".attn.pv" + std::to_string(h), a);
+      conv(p + ".attn.pv" + std::to_string(h), a);
     }
     cbs(p + ".conv1.conv2", att, y, C, 1, 1, false, 0, VPB_EPI_ADD, &y);          // y = y + proj(attention)
     Tens f = e.act_alloc(y.H, y.W, 2 * C);
@@ -845,9 +807,8 @@ static int as_post_describe(const vp_autospeed* ep, KernelCall& c) {
 }
 
 static int as_build(vp_autospeed& e, const WeightMap& w) {
-  ASBuilder b{e, w};
   const int W0 = kASW, H0 = kASH;
-  e.d_gap_scratch = static_cast<long long*>(e.dalloc(static_cast<size_t>(kGapReplicas) * 256 * 8 * e.batch + 64));
+  ASBuilder b{{e, w}, static_cast<long long*>(e.dalloc(static_cast<size_t>(kGapReplicas) * 256 * 8 * e.batch + 64))};
   e.add_preprocess(VPB_CONV_RGB_UNIT, e.d_canvas, nullptr);
   Tens x0; x0.p = e.d_canvas; x0.lo = e.pre.out_lo; x0.H = H0; x0.W = W0; x0.C = 8; x0.ld = 8;
   // ---- backbone (auto_speed_backbone.py:9-48)
@@ -873,11 +834,9 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   b.ctx("net.p5.1", a5, q5, 256);
   Tens sp = e.act_alloc(H0 / 32, W0 / 32, 512);                 // SPPF cat (common_layers.py:242-254)
   b.cbs("net.p5.2.cv1", q5, sp.slice(0, 128), 128, 1, 1, true);
-  if (b.ok()) {
-    b.maxpool("net.p5.2.pool1", sp.slice(0, 128), sp.slice(128, 128));
-    b.maxpool("net.p5.2.pool2", sp.slice(128, 128), sp.slice(256, 128));
-    b.maxpool("net.p5.2.pool3", sp.slice(256, 128), sp.slice(384, 128));
-  }
+  b.maxpool("net.p5.2.pool1", sp.slice(0, 128), sp.slice(128, 128));
+  b.maxpool("net.p5.2.pool2", sp.slice(128, 128), sp.slice(256, 128));
+  b.maxpool("net.p5.2.pool3", sp.slice(256, 128), sp.slice(384, 128));
   Tens s5 = e.act_alloc(H0 / 32, W0 / 32, 256);
   b.cbs("net.p5.2.cv2", sp, s5, 256, 1, 1, true);
   Tens cp = e.act_alloc(H0 / 32, W0 / 32, 256);                 // C2PSA cat (common_layers.py:257-269)
@@ -887,11 +846,11 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
   Tens p5 = h6cat.slice(128, 256);
   b.cbs("net.p5.3.cv2", cp, p5, 256, 1, 1, true);
   // ---- neck (auto_speed_neck.py:17-24)
-  if (b.ok()) b.upsample("fpn.up_p5", p5, h1cat.slice(0, 256));
+  b.upsample("fpn.up_p5", p5, h1cat.slice(0, 256));
   Tens h4cat = e.act_alloc(H0 / 16, W0 / 16, 192);              // cat(h3(p3'), p4')
   Tens p4n = h4cat.slice(64, 128);
   b.c3k2("fpn.h1", h1cat, p4n, 128, false);
-  if (b.ok()) b.upsample("fpn.up_p4", p4n, h2cat.slice(0, 128));
+  b.upsample("fpn.up_p4", p4n, h2cat.slice(0, 128));
   Tens n3 = e.act_alloc(H0 / 8, W0 / 8, 64);
   b.c3k2("fpn.h2", h2cat, n3, 64, false);
   b.cbs("fpn.h3", n3, h4cat.slice(0, 64), 64, 3, 2, true);
@@ -918,20 +877,21 @@ static int as_build(vp_autospeed& e, const WeightMap& w) {
     b.cbs(ci + ".3", c3, c4, 80, 1, 1, true);
     b.plain(ci + ".4", c4, lv[i].slice(64, 8), kNC, 1, ACT_NONE);
   }
-  if (!b.ok()) return b.rc != VPB_OK ? b.rc : VPB_ERR_CUDA;
+  if (!b.ok()) return b.status();
   // ---- decode (auto_speed_head.py:53-63)
   {
     const int dt = e.dtype, nb = e.batch; float* raw = e.d_raw;
     int a0 = 0;
     const float strides[3] = {8.f, 16.f, 32.f};
     for (int i = 0; i < 3; ++i) {
-      const void* lp = lv[i].p; const void* ll = lv[i].lo; const int h = lv[i].H, wd = lv[i].W, ld = lv[i].ld, off = a0;
+      const Tens& l = lv[i];
+      const int off = a0;
       const float st_ = strides[i];
       // 4 * kDfl box and kNC class logits read, 8 fp32 written per anchor
       e.add_op("head.decode" + std::to_string(i), "decode_kernel",
-               [=](cudaStream_t st) { return as_decode_x(dt, lp, ll, h, wd, ld, st_, off, kNA, raw, nb, st); }, 0.0,
-               nb * (2.0 * (4 * kDfl + kNC) + 32.0) * h * wd);
-      a0 += h * wd;
+               [=](cudaStream_t st) { return as_decode_x(dt, l.p, l.lo, l.H, l.W, l.ld, st_, off, kNA, raw, nb, st); }, 0.0,
+               nb * (2.0 * (4 * kDfl + kNC) + 32.0) * l.H * l.W);
+      a0 += l.H * l.W;
     }
   }
   // ---- NMS and the map back to each source frame, with the thresholds and letterboxes of the call

@@ -126,18 +126,7 @@ struct vp_engine : EngineRuntime {
 
 namespace vpb {
 
-// BatchNorm folding (eval mode, eps 1e-5 — torchvision EfficientNet-B0): y = conv(x)*s + t
-static bool bn_fold(const WeightMap& w, const std::string& p, int C, std::vector<float>& s, std::vector<float>& t) {
-  const HostTensor *g = find_w_shaped(w, p + "weight", {C}), *b = find_w_shaped(w, p + "bias", {C}),
-                   *m = find_w_shaped(w, p + "running_mean", {C}), *v = find_w_shaped(w, p + "running_var", {C});
-  if (!g || !b || !m || !v) return false;
-  s.resize(C); t.resize(C);
-  for (int c = 0; c < C; ++c) {
-    const float sc = g->f[c] / std::sqrt(v->f[c] + 1e-5f);
-    s[c] = sc; t[c] = b->f[c] - m->f[c] * sc;
-  }
-  return true;
-}
+static constexpr float kBnEps = 1e-5f;   // BatchNorm eps of torchvision's EfficientNet-B0
 
 // ConvTranspose2d weight [Cin][Cout][2][2] -> [a*2+b][Cout][Cin]
 static std::vector<float> pack_convT(const HostTensor& t) {
@@ -155,13 +144,13 @@ static const int kStages[7][6] = {  // expand, kernel, stride, cin, cout, repeat
     {6, 5, 1, 80, 112, 3}, {6, 5, 2, 112, 192, 4}, {6, 3, 1, 192, 320, 1}};
 
 // ---------------------------------------------------------------- encoder (backbone.py:11-22)
-static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p, const std::string& tag,
-                         vp_engine::EncOut& out) {
+static void build_encoder(vp_engine& e, NetBuilder& b, const std::string& p, const std::string& tag,
+                          vp_engine::EncOut& out) {
   const int dt = e.dtype, nb = e.batch;
-  std::vector<float> s, t;
   // stem
-  const HostTensor* sw = find_w_shaped(w, p + "0.0.weight", {32, 3, 3, 3});
-  if (!sw || !bn_fold(w, p + "0.1.", 32, s, t)) return VPB_ERR_IO;
+  std::vector<float> s, t;
+  const HostTensor* sw = b.get(p + "0.0.weight", {32, 3, 3, 3});
+  if (!b.bn(p + "0.1.", 32, kBnEps, s, t)) return;
   std::vector<float> stem(27 * 32);
   for (int co = 0; co < 32; ++co)
     for (int c = 0; c < 3; ++c)
@@ -169,12 +158,9 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
   float* d_stem = e.upload_f32(stem);
   float* d_stem_b = e.upload_f32(t);
   Tens x = e.act_alloc(kNetH / 2, kNetW / 2, 32);
-  {
-    const void* in = e.d_pre; void* o = x.p;
-    const void* in_lo = e.d_pre_lo; void* o_lo = x.lo;
-    e.add_op(tag + "stem", "stem_conv_kernel", [=](cudaStream_t st) { return stem_conv_x(dt, in, in_lo, kNetH, kNetW, d_stem, d_stem_b, o, o_lo, st, nb); },
-             2.0 * x.H * x.W * 32 * 27, nb * (2.0 * kNetH * kNetW * 4 + 2.0 * x.H * x.W * 32));
-  }
+  const void *in = e.d_pre, *in_lo = e.d_pre_lo;
+  b.op(tag + "stem", "stem_conv_kernel", [=](cudaStream_t st) { return stem_conv_x(dt, in, in_lo, kNetH, kNetW, d_stem, d_stem_b, x.p, x.lo, st, nb); },
+       2.0 * x.H * x.W * 32 * 27, nb * (2.0 * kNetH * kNetW * 4 + 2.0 * x.H * x.W * 32));
   Tens stage_out[9];
   stage_out[0] = x;
   for (int si = 0; si < 7; ++si) {
@@ -187,142 +173,114 @@ static int build_encoder(vp_engine& e, const WeightMap& w, const std::string& p,
       int bi = 0;
       Tens cur = x;
       if (exp != 1) {  // 1x1 expand + BN + SiLU -> wgmma GEMM
-        const HostTensor* ew = find_w_shaped(w, bp + "0.0.weight", {ce, ci, 1, 1});
-        if (!ew || !bn_fold(w, bp + "0.1.", ce, s, t)) return VPB_ERR_IO;
-        void* dw_ = e.upload_16(pack_conv(*ew, &s));
-        float* db = e.upload_f32(t);
-        Tens ex = e.act_alloc(x.H, x.W, ce);
-        int rc = e.append_conv(nm + "expand", e.conv_args(x, &ex, nullptr, ce, 1, 1, dw_, db, ACT_SILU, VPB_EPI_STORE));
-        if (rc) return rc;
-        cur = ex; bi = 1;
+        const NetBuilder::Params ex = b.folded(bp + "0.0.weight", {ce, ci, 1, 1}, bp + "0.1.", kBnEps);
+        cur = e.act_alloc(x.H, x.W, ce);
+        b.conv(nm + "expand", e.conv_args(x, &cur, nullptr, ce, 1, 1, ex.w, ex.b, ACT_SILU, VPB_EPI_STORE));
+        bi = 1;
       }
       // depthwise + BN + SiLU (+ SE pooling partial sums)
-      const HostTensor* dwt = find_w_shaped(w, bp + std::to_string(bi) + ".0.weight", {ce, 1, k, k});
-      if (!dwt || !bn_fold(w, bp + std::to_string(bi) + ".1.", ce, s, t)) return VPB_ERR_IO;
-      std::vector<float> dwp(static_cast<size_t>(k) * k * ce);
-      for (int c = 0; c < ce; ++c)
-        for (int kk = 0; kk < k * k; ++kk) dwp[static_cast<size_t>(kk) * ce + c] = dwt->f[static_cast<size_t>(c) * k * k + kk] * s[c];
-      float* d_dw = e.upload_f32(dwp);
-      float* d_dwb = e.upload_f32(t);
+      const NetBuilder::Params dw = b.depthwise(bp + std::to_string(bi) + ".0.weight", ce, k, bp + std::to_string(bi) + ".1.", kBnEps);
+      const float *d_dw = static_cast<const float*>(dw.w), *d_dwb = dw.b;
       const DwGeom g = dw_geometry(cur.H, cur.W, ce, k, s_);
-      Tens dwo = e.act_alloc(g.Ho, g.Wo, ce);
+      const Tens dwo = e.act_alloc(g.Ho, g.Wo, ce);
       long long* d_part = e.gap_alloc(ce);
-      {
-        const void* in = cur.p; void* o = dwo.p; const int H = cur.H, W = cur.W;
-        const void* in_lo = cur.lo; void* o_lo = dwo.lo;
-        e.add_op(nm + "dw", "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, in, in_lo, H, W, ce, k, s_, d_dw, d_dwb, o, o_lo, d_part, st, VPB_ACT_SILU, nb); },
-                 2.0 * g.Ho * g.Wo * ce * k * k, nb * (2.0 * H * W * ce + 2.0 * g.Ho * g.Wo * ce));
-      }
+      b.op(nm + "dw", "depthwise_kernel", [=](cudaStream_t st) { return depthwise_x(dt, cur.p, cur.lo, cur.H, cur.W, ce, k, s_, d_dw, d_dwb, dwo.p, dwo.lo, d_part, st, VPB_ACT_SILU, nb); },
+           2.0 * g.Ho * g.Wo * ce * k * k, nb * (2.0 * cur.H * cur.W * ce + 2.0 * g.Ho * g.Wo * ce));
       // SE gate applied to the depthwise output in place (where the reference graph applies it), then a plain 1x1
-      const std::string sp = bp + std::to_string(bi + 1) + ".";
-      const HostTensor *f1 = find_w_shaped(w, sp + "fc1.weight", {sq, ce, 1, 1}), *b1 = find_w_shaped(w, sp + "fc1.bias", {sq}),
-                       *f2 = find_w_shaped(w, sp + "fc2.weight", {ce, sq, 1, 1}), *b2 = find_w_shaped(w, sp + "fc2.bias", {ce});
-      const HostTensor* pw = find_w_shaped(w, bp + std::to_string(bi + 2) + ".0.weight", {cout, ce, 1, 1});
-      if (!f1 || !b1 || !f2 || !b2 || !pw || !bn_fold(w, bp + std::to_string(bi + 2) + ".1.", cout, s, t)) return VPB_ERR_IO;
+      const std::string sp = bp + std::to_string(bi + 1) + ".", pp = bp + std::to_string(bi + 2) + ".";
+      const HostTensor *f1 = b.get(sp + "fc1.weight", {sq, ce, 1, 1}), *b1 = b.get(sp + "fc1.bias", {sq}),
+                       *f2 = b.get(sp + "fc2.weight", {ce, sq, 1, 1}), *b2 = b.get(sp + "fc2.bias", {ce});
+      const NetBuilder::Params proj = b.folded(pp + "0.weight", {cout, ce, 1, 1}, pp + "1.", kBnEps);   // BatchNorm folded, static
+      if (!b.ok()) return;
       std::vector<float> f2t(f2->f.size());   // fc2 [C][sq] -> [sq][C] so the gate kernel reads it coalesced
       for (int c = 0; c < ce; ++c)
         for (int j = 0; j < sq; ++j) f2t[static_cast<size_t>(j) * ce + c] = f2->f[static_cast<size_t>(c) * sq + j];
       float *d_f1 = e.upload_f32(f1->f), *d_b1 = e.upload_f32(b1->f), *d_f2 = e.upload_f32(f2t), *d_b2 = e.upload_f32(b2->f);
-      if (!d_part) { vpb_set_error("SE accumulator arena exhausted"); return VPB_ERR_STATE; }
-      void* d_wproj = e.upload_16(pack_conv(*pw, &s));            // BatchNorm folded, static
-      float* d_pb = e.upload_f32(t);
-      {
-        const int HW = g.Ho * g.Wo;
-        void* act = dwo.p; void* act_lo = dwo.lo;
-        e.add_op(nm + "se", "se_scale_kernel", [=](cudaStream_t st) {
-          return se_scale_x(dt, d_part, HW, ce, sq, d_f1, d_b1, d_f2, d_b2, act, act_lo, nullptr, st, nb);
-        }, 2.0 * (2.0 * ce * sq), nb * (8.0 * ce * kGapReplicas + 4.0 * HW * ce) + 8.0 * ce * sq);
-      }
+      if (!d_part) b.fail(VPB_ERR_STATE, "SE accumulator arena exhausted");
+      const int HW = g.Ho * g.Wo;
+      b.op(nm + "se", "se_scale_kernel", [=](cudaStream_t st) {
+        return se_scale_x(dt, d_part, HW, ce, sq, d_f1, d_b1, d_f2, d_b2, dwo.p, dwo.lo, nullptr, st, nb);
+      }, 2.0 * (2.0 * ce * sq), nb * (8.0 * ce * kGapReplicas + 4.0 * HW * ce) + 8.0 * ce * sq);
       // 1x1 project + BN (+ residual; StochasticDepth is identity in eval)
       const bool residual = (s_ == 1 && ci == cout);
-      Tens po = e.act_alloc(dwo.H, dwo.W, cout);
-      int rc = e.append_conv(nm + "project", e.conv_args(dwo, &po, residual ? &x : nullptr, cout, 1, 1, d_wproj, d_pb, ACT_NONE,
-                                                         residual ? VPB_EPI_ADD : VPB_EPI_STORE));
-      if (rc) return rc;
+      const Tens po = e.act_alloc(dwo.H, dwo.W, cout);
+      b.conv(nm + "project", e.conv_args(dwo, &po, residual ? &x : nullptr, cout, 1, 1, proj.w, proj.b, ACT_NONE,
+                                         residual ? VPB_EPI_ADD : VPB_EPI_STORE));
       x = po;
     }
     stage_out[si + 1] = x;
   }
   // encoder[8]: 1x1 320 -> 1280 + BN + SiLU
-  const HostTensor* hw = find_w_shaped(w, p + "8.0.weight", {1280, 320, 1, 1});
-  if (!hw || !bn_fold(w, p + "8.1.", 1280, s, t)) return VPB_ERR_IO;
-  void* d_hw = e.upload_16(pack_conv(*hw, &s));
-  float* d_hb = e.upload_f32(t);
-  Tens f4 = e.act_alloc(x.H, x.W, 1280);
-  int rc = e.append_conv(tag + "enc8", e.conv_args(x, &f4, nullptr, 1280, 1, 1, d_hw, d_hb, ACT_SILU, VPB_EPI_STORE));
-  if (rc) return rc;
+  const NetBuilder::Params hd = b.folded(p + "8.0.weight", {1280, 320, 1, 1}, p + "8.1.", kBnEps);
+  const Tens f4 = e.act_alloc(x.H, x.W, 1280);
+  b.conv(tag + "enc8", e.conv_args(x, &f4, nullptr, 1280, 1, 1, hd.w, hd.b, ACT_SILU, VPB_EPI_STORE));
   out.f[0] = stage_out[0]; out.f[1] = stage_out[2]; out.f[2] = stage_out[3]; out.f[3] = stage_out[4]; out.f[4] = f4;
-  return VPB_OK;
 }
 
-static int conv_layer(vp_engine& e, const WeightMap& w, const std::string& key, const std::string& name,
-                      const Tens& in, int taps, int act, int mode, Tens* out, const Tens* res) {
-  const HostTensor* wt = find_w_shaped(w, key + ".weight", {-1, -1, 3, 3});
-  const HostTensor* bt = wt ? find_w_shaped(w, key + ".bias", {wt->dims[0]}) : nullptr;
-  if (!wt || !bt || taps != 9) return VPB_ERR_IO;
+// Conv2d 3x3 with bias + GELU: in -> *out (allocated zero-bordered unless given)
+static void conv_layer(vp_engine& e, NetBuilder& b, const std::string& key, const std::string& name, const Tens& in,
+                       Tens* out, int mode = VPB_EPI_STORE, const Tens* res = nullptr) {
+  const HostTensor* wt;
+  const NetBuilder::Params c = b.plain(key, {-1, -1, 3, 3}, &wt);
+  if (!b.ok()) return;
+  if (wt->dims[1] != in.C) return b.fail(VPB_ERR_ARG, "%s: Cin %d != input channels %d", key.c_str(), wt->dims[1], in.C);
   const int Cout = wt->dims[0];
-  if (wt->dims[1] != in.C) { vpb_set_error("%s: Cin %d != input channels %d", key.c_str(), wt->dims[1], in.C); return VPB_ERR_ARG; }
-  void* dw_ = e.upload_16(pack_conv(*wt, nullptr));
-  float* db = e.upload_f32(bt->f);
   if (!out->p) *out = e.act_alloc(in.H, in.W, (Cout + 7) / 8 * 8, /*pad=*/1);
-  return e.append_conv(name, e.conv_args(in, out, res, Cout, taps, 1, dw_, db, act, mode));
+  b.conv(name, e.conv_args(in, out, res, Cout, 9, 1, c.w, c.b, ACT_GELU, mode));
 }
 
 // ConvTranspose2d(k2,s2) [+ Conv1x1(skip)] summed before any activation (scene_neck.py:30-32)
-static int up_skip(vp_engine& e, const WeightMap& w, const std::string& p, int i, const std::string& tag,
-                   const Tens& in, const Tens* skip, Tens* out) {
+static void up_skip(vp_engine& e, NetBuilder& b, const std::string& p, int i, const std::string& tag, const Tens& in,
+                    const Tens* skip, Tens* out) {
   const std::string uk = p + "upsample_layer_" + std::to_string(i);
-  const HostTensor* ut = find_w_shaped(w, uk + ".weight", {in.C, -1, 2, 2});
-  const HostTensor* ub = ut ? find_w_shaped(w, uk + ".bias", {ut->dims[1]}) : nullptr;
-  if (!ut || !ub) return VPB_ERR_IO;
+  const HostTensor* ut = b.get(uk + ".weight", {in.C, -1, 2, 2});
+  const HostTensor* ub = ut ? b.get(uk + ".bias", {ut->dims[1]}) : nullptr;
+  if (!b.ok()) return;
   const int Cout = ut->dims[1];
   *out = e.act_alloc(in.H * 2, in.W * 2, Cout, /*pad=*/1);
   void* dw_ = e.upload_16(pack_convT(*ut));
   if (!skip)
-    return e.append_conv(tag + "up" + std::to_string(i),
-                         e.conv_args(in, out, nullptr, Cout, 1, 4, dw_, e.upload_f32(ub->f), ACT_NONE, VPB_EPI_STORE));
+    return b.conv(tag + "up" + std::to_string(i),
+                  e.conv_args(in, out, nullptr, Cout, 1, 4, dw_, e.upload_f32(ub->f), ACT_NONE, VPB_EPI_STORE));
   // the skip link's 1x1 conv is a second K segment of the same GEMM: both layers accumulate in the
   // fp32 accumulator and the sum is rounded and written once (no intermediate tensor)
   const std::string sk = p + "skip_link_layer_" + std::to_string(i);
-  const HostTensor *st = find_w_shaped(w, sk + ".weight", {Cout, -1, 1, 1}), *sb = find_w_shaped(w, sk + ".bias", {Cout});
-  if (!st || !sb) return VPB_ERR_IO;
-  if (st->dims[0] != Cout || st->dims[1] != skip->C || (skip->C & 7)) {
-    vpb_set_error("%s: skip link [%d,%d] does not match Cout=%d / skip channels %d", sk.c_str(), st->dims[0],
-                  st->dims[1], Cout, skip->C);
-    return VPB_ERR_ARG;
-  }
+  const HostTensor *st = b.get(sk + ".weight", {Cout, -1, 1, 1}), *sb = b.get(sk + ".bias", {Cout});
+  if (!b.ok()) return;
+  if (st->dims[0] != Cout || st->dims[1] != skip->C || (skip->C & 7))
+    return b.fail(VPB_ERR_ARG, "%s: skip link [%d,%d] does not match Cout=%d / skip channels %d", sk.c_str(),
+                  st->dims[0], st->dims[1], Cout, skip->C);
   void* dw2 = e.upload_16(pack_conv(*st, nullptr));
   std::vector<float> bsum(ub->f);
   for (int c = 0; c < Cout; ++c) bsum[c] += sb->f[c];
-  return e.append_conv(tag + "up" + std::to_string(i),
-                       e.conv_args(in, out, nullptr, Cout, 1, 4, dw_, e.upload_f32(bsum), ACT_NONE, VPB_EPI_STORE, skip, dw2));
+  b.conv(tag + "up" + std::to_string(i),
+         e.conv_args(in, out, nullptr, Cout, 1, 4, dw_, e.upload_f32(bsum), ACT_NONE, VPB_EPI_STORE, skip, dw2));
 }
 
 // ConvTranspose2d(k2,s2) [+ Conv1x1(skip)] and the Conv3x3 + GELU that follows it (scene_neck.py:30-37,
 // scene_seg_head.py:25-33) as ONE GEMM over the low-resolution tensor: no activation separates the layers, so their
 // weights are composed once at load time (vpb_upconv_compose, upconv_compose.cu) and the upsampled tensor is never
 // materialised.  16-bit mode only — the split-fp16 mode keeps the reference's layer-by-layer graph.
-static int upconv_layer(vp_engine& e, const WeightMap& w, const std::string& p, int i, int dec, const std::string& tag,
-                        const Tens& in, const Tens* skip, Tens* out) {
+static void upconv_layer(vp_engine& e, NetBuilder& b, const std::string& p, int i, int dec, const std::string& tag,
+                         const Tens& in, const Tens* skip, Tens* out) {
   const std::string uk = p + "upsample_layer_" + std::to_string(i), dk = p + "decode_layer_" + std::to_string(dec);
-  const HostTensor* ut = find_w_shaped(w, uk + ".weight", {in.C, -1, 2, 2});
-  const HostTensor* ub = ut ? find_w_shaped(w, uk + ".bias", {ut->dims[1]}) : nullptr;
-  if (!ut || !ub) return VPB_ERR_IO;
-  const int Cin = in.C, Cmid = ut->dims[1];
-  const HostTensor* w3 = find_w_shaped(w, dk + ".weight", {-1, Cmid, 3, 3});
-  const HostTensor* b3 = w3 ? find_w_shaped(w, dk + ".bias", {w3->dims[0]}) : nullptr;
-  if (!w3 || !b3) return VPB_ERR_IO;
+  const HostTensor* ut = b.get(uk + ".weight", {in.C, -1, 2, 2});
+  const HostTensor* ub = ut ? b.get(uk + ".bias", {ut->dims[1]}) : nullptr;
+  const int Cin = in.C, Cmid = ut ? ut->dims[1] : 0;
+  const HostTensor* w3 = b.get(dk + ".weight", {-1, Cmid, 3, 3});
+  const HostTensor* b3 = w3 ? b.get(dk + ".bias", {w3->dims[0]}) : nullptr;
+  if (!b.ok()) return;
   const int Cout = w3->dims[0];
   const HostTensor *st = nullptr, *sb = nullptr;
   int C2 = 0;
   if (skip) {
     const std::string sk = p + "skip_link_layer_" + std::to_string(i);
-    st = find_w_shaped(w, sk + ".weight", {Cmid, skip->C, 1, 1}); sb = find_w_shaped(w, sk + ".bias", {Cmid});
-    if (!st || !sb) return VPB_ERR_IO;
-    if (skip->C & 7) { vpb_set_error("%s: skip channels %d not a multiple of 8", sk.c_str(), skip->C); return VPB_ERR_ARG; }
+    st = b.get(sk + ".weight", {Cmid, skip->C, 1, 1}); sb = b.get(sk + ".bias", {Cmid});
+    if (b.ok() && (skip->C & 7)) b.fail(VPB_ERR_ARG, "%s: skip channels %d not a multiple of 8", sk.c_str(), skip->C);
     C2 = skip->C;
   }
-  if (Cout & 15) { vpb_set_error("%s: Cout %d not a multiple of 16", dk.c_str(), Cout); return VPB_ERR_ARG; }
+  if (Cout & 15) b.fail(VPB_ERR_ARG, "%s: Cout %d not a multiple of 16", dk.c_str(), Cout);
+  if (!b.ok()) return;
   // fp32 parameters -> device scratch, composed operands in fp32, then rounded to the 16-bit storage type
   std::vector<void*> tmp;
   auto put = [&](const std::vector<float>& v) -> float* {
@@ -338,7 +296,7 @@ static int upconv_layer(vp_engine& e, const WeightMap& w, const std::string& p, 
     tmp.push_back(d);
     return static_cast<float*>(d);
   };
-  auto done = [&](int rc) { for (void* d : tmp) cudaFree(d); return rc; };
+  auto done = [&](int rc) { for (void* d : tmp) cudaFree(d); if (rc) b.fail(rc); };
   const size_t nwf = static_cast<size_t>(16) * Cout * Cin, nw2 = static_cast<size_t>(9) * Cout * C2;
   float *d_w3 = put(w3->f), *d_b3 = put(b3->f), *d_wt = put(ut->f), *d_bt = put(ub->f);
   float *d_ws = st ? put(st->f) : nullptr, *d_bs = sb ? put(sb->f) : nullptr;
@@ -358,95 +316,80 @@ static int upconv_layer(vp_engine& e, const WeightMap& w, const std::string& p, 
   if (rc == VPB_OK) rc = vpb_f32_to_16(e.dtype, d_wf, d_wf16, static_cast<long long>(nwf), e.stream);
   if (rc == VPB_OK && C2) rc = vpb_f32_to_16(e.dtype, d_w2f, d_w216, static_cast<long long>(nw2), e.stream);
   if (cudaStreamSynchronize(e.stream) != cudaSuccess && rc == VPB_OK) { vpb_set_error("%s: weight composition failed", dk.c_str()); rc = VPB_ERR_CUDA; }
-  if (rc != VPB_OK) return done(rc);
-  done(VPB_OK);
+  done(rc);
+  if (!b.ok()) return;
   *out = e.act_alloc(in.H * 2, in.W * 2, (Cout + 7) / 8 * 8, /*pad=*/1);
   vpb_conv_args a = e.conv_args(in, out, nullptr, Cout, 4, 4, d_wf16, d_b9, ACT_GELU, VPB_EPI_STORE, skip, d_w216);
   a.taps2 = C2 ? 9 : 0;
-  rc = e.append_conv(tag + "up" + std::to_string(i) + "dec" + std::to_string(dec), a);
-  if (rc == VPB_OK)   // what the reference's three layers cost: ConvTranspose + skip 1x1 at 4 phases, then the 3x3 at 2H x 2W
+  b.conv(tag + "up" + std::to_string(i) + "dec" + std::to_string(dec), a);
+  if (b.ok())   // what the reference's three layers cost: ConvTranspose + skip 1x1 at 4 phases, then the 3x3 at 2H x 2W
     e.ops.back().flops_ref = e.batch * (2.0 * in.H * in.W * 4.0 * Cmid * (Cin + C2) + 2.0 * (4.0 * in.H * in.W) * Cout * 9.0 * Cmid);
-  return rc;
 }
 
 // SceneContext / DepthContext / AutoSteerContext (scene_context.py:25-57)
-static int build_context(vp_engine& e, const WeightMap& w, const std::string& p, const std::string& tag,
-                         const Tens& feat, Tens* ctx) {
+static void build_context(vp_engine& e, NetBuilder& b, const std::string& p, const std::string& tag, const Tens& feat,
+                          Tens* ctx) {
   const int dt = e.dtype, C = feat.C, HW = feat.H * feat.W, nb = e.batch;
   float* d_v = static_cast<float*>(e.dalloc(static_cast<size_t>(C) * 4 * nb, false));   // [batch][C]: per-sample context vectors
-  {
-    const void* in = feat.p; const void* in_lo = feat.lo;
-    e.add_op(tag + "gap", "gap_kernel", [=](cudaStream_t st) { return gap_x(dt, in, in_lo, HW, C, C, d_v, st, nb); }, 0.0, nb * 2.0 * HW * C);
-  }
+  b.op(tag + "gap", "gap_kernel", [=](cudaStream_t st) { return gap_x(dt, feat.p, feat.lo, HW, C, C, d_v, st, nb); }, 0.0, nb * 2.0 * HW * C);
   const int dims[4] = {C, 800, 800, 200};
   const int acts[3] = {ACT_GELU, ACT_GELU, ACT_SIGMOID};
   float* cur = d_v;
   for (int i = 0; i < 3; ++i) {
     const std::string k = p + "context_layer_" + std::to_string(i);
-    const HostTensor *wt = find_w_shaped(w, k + ".weight", {dims[i + 1], dims[i]}), *bt = find_w_shaped(w, k + ".bias", {dims[i + 1]});
-    if (!wt || !bt) return VPB_ERR_IO;
+    const HostTensor *wt = b.get(k + ".weight", {dims[i + 1], dims[i]}), *bt = b.get(k + ".bias", {dims[i + 1]});
+    if (!b.ok()) return;
     float *dw_ = e.upload_f32(wt->f), *db = e.upload_f32(bt->f);
     float* y = static_cast<float*>(e.dalloc(static_cast<size_t>(dims[i + 1]) * 4 * nb, false));
     const int in_f = dims[i], out_f = dims[i + 1], a = acts[i];
     const float* xin = cur;
-    e.add_op(tag + "mlp" + std::to_string(i), "linear_kernel", [=](cudaStream_t st) { return linear_x(xin, dw_, db, in_f, out_f, a, y, st, nb); },
-             2.0 * in_f * out_f, 4.0 * in_f * out_f);
+    b.op(tag + "mlp" + std::to_string(i), "linear_kernel", [=](cudaStream_t st) { return linear_x(xin, dw_, db, in_f, out_f, a, y, st, nb); },
+         2.0 * in_f * out_f, 4.0 * in_f * out_f);
     cur = y;
   }
-  const HostTensor *w3 = find_w_shaped(w, p + "context_layer_3.weight", {128, 1, 3, 3}), *b3 = find_w_shaped(w, p + "context_layer_3.bias", {128});
-  if (!w3 || !b3) return VPB_ERR_IO;
+  const HostTensor *w3 = b.get(p + "context_layer_3.weight", {128, 1, 3, 3}), *b3 = b.get(p + "context_layer_3.bias", {128});
+  if (!b.ok()) return;
   float *d_w3 = e.upload_f32(w3->f), *d_b3 = e.upload_f32(b3->f);
-  Tens c4 = e.act_alloc(feat.H, feat.W, 128, /*pad=*/1);
-  {
-    const float* xin = cur; void* o = c4.p; void* o_lo = c4.lo; const int H = feat.H, W = feat.W;
-    e.add_op(tag + "ctx3", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, xin, H, W, d_w3, d_b3, 128, o, o_lo, 1, st, VPB_ACT_GELU, nb); },
-             2.0 * HW * 128 * 9, nb * 2.0 * (H + 2) * (W + 2) * 128);
-  }
+  const Tens c4 = e.act_alloc(feat.H, feat.W, 128, /*pad=*/1);
+  const float* xin = cur;
+  b.op(tag + "ctx3", "ctx_conv1_kernel", [=](cudaStream_t st) { return ctx_conv1_x(dt, xin, c4.H, c4.W, d_w3, d_b3, 128, c4.p, c4.lo, 1, st, VPB_ACT_GELU, nb); },
+       2.0 * HW * 128 * 9, nb * 2.0 * (c4.H + 2) * (c4.W + 2) * 128);
   Tens c5, c6;
-  int rc = conv_layer(e, w, p + "context_layer_4", tag + "ctx4", c4, 9, ACT_GELU, VPB_EPI_STORE, &c5, nullptr);
-  if (rc) return rc;
-  rc = conv_layer(e, w, p + "context_layer_5", tag + "ctx5", c5, 9, ACT_GELU, VPB_EPI_STORE, &c6, nullptr);
-  if (rc) return rc;
+  conv_layer(e, b, p + "context_layer_4", tag + "ctx4", c4, &c5);
+  conv_layer(e, b, p + "context_layer_5", tag + "ctx5", c5, &c6);
   *ctx = e.act_alloc(feat.H, feat.W, C, /*pad=*/1);
-  return conv_layer(e, w, p + "context_layer_6", tag + "ctx6", c6, 9, ACT_GELU, VPB_EPI_MULADD, ctx, &feat);
+  conv_layer(e, b, p + "context_layer_6", tag + "ctx6", c6, ctx, VPB_EPI_MULADD, &feat);
 }
 
 // SceneNeck / Scene3DNeck / EgoPathNeck (scene_neck.py:26-60)
-static int build_neck(vp_engine& e, const WeightMap& w, const std::string& p, const std::string& tag,
-                      const Tens& ctx, const vp_engine::EncOut& enc, Tens* neck) {
+static void build_neck(vp_engine& e, NetBuilder& b, const std::string& p, const std::string& tag, const Tens& ctx,
+                       const vp_engine::EncOut& enc, Tens* neck) {
   Tens d = ctx, u;
   const int skip_src[3] = {3, 2, 1};
-  for (int b = 0; b < 3; ++b) {
+  for (int i = 0; i < 3; ++i) {
+    const std::string d0 = std::to_string(2 * i), d1 = std::to_string(2 * i + 1);
     Tens a, c;
-    int rc;
     if (!e.split) {
-      rc = upconv_layer(e, w, p, b, 2 * b, tag, d, &enc.f[skip_src[b]], &a);
-      if (rc) return rc;
+      upconv_layer(e, b, p, i, 2 * i, tag, d, &enc.f[skip_src[i]], &a);
     } else {
-      rc = up_skip(e, w, p, b, tag, d, &enc.f[skip_src[b]], &u);
-      if (rc) return rc;
-      rc = conv_layer(e, w, p + "decode_layer_" + std::to_string(2 * b), tag + "dec" + std::to_string(2 * b), u, 9, ACT_GELU, VPB_EPI_STORE, &a, nullptr);
-      if (rc) return rc;
+      up_skip(e, b, p, i, tag, d, &enc.f[skip_src[i]], &u);
+      conv_layer(e, b, p + "decode_layer_" + d0, tag + "dec" + d0, u, &a);
     }
-    rc = conv_layer(e, w, p + "decode_layer_" + std::to_string(2 * b + 1), tag + "dec" + std::to_string(2 * b + 1), a, 9, ACT_GELU, VPB_EPI_STORE, &c, nullptr);
-    if (rc) return rc;
+    conv_layer(e, b, p + "decode_layer_" + d1, tag + "dec" + d1, a, &c);
     d = c;
   }
   *neck = d;
-  return VPB_OK;
 }
 
 // A head's output layer (3x3 to Cout <= 3 channels) as two ops (DESIGN.md §3f): a 1x1 GEMM onto the 9*Cout tap
 // products P — the activation tensor is read once instead of once per tap — and the nine-point shifted sum + bias +
 // class map (final_tapsum_kernel).
-static int final_conv(vp_engine& e, const WeightMap& w, const std::string& key, const std::string& name,
-                      const Tens& in, int final_kind, ModelOut& mo) {
-  const HostTensor* wt = find_w_shaped(w, key + ".weight", {-1, in.C, 3, 3});
-  const HostTensor* bt = wt ? find_w_shaped(w, key + ".bias", {wt->dims[0]}) : nullptr;
-  if (!wt || !bt) return VPB_ERR_IO;
+static void final_conv(vp_engine& e, NetBuilder& b, const std::string& key, const std::string& name, const Tens& in,
+                       int final_kind, ModelOut& mo) {
+  const HostTensor* wt;
+  const NetBuilder::Params c = b.plain(key, {-1, in.C, 3, 3}, &wt);   // [9][Cout][Cin] == [9*Cout][Cin], row t*Cout + o
+  if (!b.ok()) return;
   const int Cout = wt->dims[0], H = in.H, W = in.W, nb = e.batch;
-  void* dw_ = e.upload_16(pack_conv(*wt, nullptr));     // [9][Cout][Cin] == [9*Cout][Cin], row t*Cout + o
-  float* db = e.upload_f32(bt->f);
   mo.C = Cout; mo.H = H; mo.W = W;
   const size_t plane = static_cast<size_t>(H) * W;
   // [batch][C][H][W] fp32 and [batch][H][W] uint8
@@ -455,53 +398,50 @@ static int final_conv(vp_engine& e, const WeightMap& w, const std::string& key, 
   if (mo.has_cls) mo.d_cls = static_cast<uint8_t*>(e.dalloc(plane * nb, false));
   mo.h_raw = static_cast<float*>(e.halloc(plane * Cout * 4 * nb));
   if (mo.has_cls) mo.h_cls = static_cast<uint8_t*>(e.halloc(plane * nb));
-  if (!mo.h_raw || (mo.has_cls && !mo.h_cls)) return VPB_ERR_CUDA;
+  if (!mo.h_raw || (mo.has_cls && !mo.h_cls)) return b.fail(VPB_ERR_CUDA);
   float* d_taps = static_cast<float*>(e.dalloc(plane * 9 * Cout * 4 * nb, false));   // P [batch][9*Cout][H][W]
-  vpb_conv_args a = e.conv_args(in, nullptr, nullptr, 9 * Cout, 1, 1, dw_, nullptr, ACT_NONE, VPB_EPI_FINAL);
+  vpb_conv_args a = e.conv_args(in, nullptr, nullptr, 9 * Cout, 1, 1, c.w, nullptr, ACT_NONE, VPB_EPI_FINAL);
   a.final_kind = VPB_FINAL_NONE; a.out_f32 = d_taps;
-  int rc = e.append_conv(name + "taps", a);
-  if (rc) return rc;
-  float* raw = mo.d_raw; uint8_t* cls = mo.d_cls;
-  e.add_op(name + "sum", "final_tapsum_kernel",
-           [=](cudaStream_t st) { return final_tapsum_x(d_taps, db, Cout, H, W, final_kind, raw, cls, st, nb); },
-           0.0, nb * (4.0 * 10 * Cout * plane + (cls ? plane : 0)));
-  return VPB_OK;
+  b.conv(name + "taps", a);
+  const float* db = c.b; float* raw = mo.d_raw; uint8_t* cls = mo.d_cls;
+  b.op(name + "sum", "final_tapsum_kernel",
+       [=](cudaStream_t st) { return final_tapsum_x(d_taps, db, Cout, H, W, final_kind, raw, cls, st, nb); },
+       0.0, nb * (4.0 * 10 * Cout * plane + (cls ? plane : 0)));
 }
 
 // SceneSegHead / Scene3DHead / DomainSegHead (scene_seg_head.py:21-44) and EgoLanesHead
-static int build_head(vp_engine& e, const WeightMap& w, const std::string& p, const std::string& tag, int kind,
-                      const Tens& neck, const vp_engine::EncOut& enc, ModelOut& mo) {
-  int rc;
+static void build_head(vp_engine& e, NetBuilder& b, const std::string& p, const std::string& tag, int kind,
+                       const Tens& neck, const vp_engine::EncOut& enc, ModelOut& mo) {
   if (kind == VP_EGO_LANES) {  // ego_lanes_head.py:17-26
-    Tens a, b;
-    rc = conv_layer(e, w, p + "decode_layer_6", tag + "dec6", neck, 9, ACT_GELU, VPB_EPI_STORE, &a, nullptr); if (rc) return rc;
-    rc = conv_layer(e, w, p + "decode_layer_7", tag + "dec7", a, 9, ACT_GELU, VPB_EPI_STORE, &b, nullptr); if (rc) return rc;
-    return final_conv(e, w, p + "decode_layer_8", tag + "dec8", b, VPB_FINAL_EGOLANES, mo);
+    Tens a, c;
+    conv_layer(e, b, p + "decode_layer_6", tag + "dec6", neck, &a);
+    conv_layer(e, b, p + "decode_layer_7", tag + "dec7", a, &c);
+    return final_conv(e, b, p + "decode_layer_8", tag + "dec8", c, VPB_FINAL_EGOLANES, mo);
   }
-  Tens u3, a, b, u4, c, d;
+  Tens u3, a, c, u4, d, f;
   if (!e.split) {
-    rc = upconv_layer(e, w, p, 3, 6, tag, neck, &enc.f[0], &a); if (rc) return rc;
-    rc = conv_layer(e, w, p + "decode_layer_7", tag + "dec7", a, 9, ACT_GELU, VPB_EPI_STORE, &b, nullptr); if (rc) return rc;
-    rc = upconv_layer(e, w, p, 4, 8, tag, b, nullptr, &c); if (rc) return rc;
+    upconv_layer(e, b, p, 3, 6, tag, neck, &enc.f[0], &a);
+    conv_layer(e, b, p + "decode_layer_7", tag + "dec7", a, &c);
+    upconv_layer(e, b, p, 4, 8, tag, c, nullptr, &d);
   } else {
-    rc = up_skip(e, w, p, 3, tag, neck, &enc.f[0], &u3); if (rc) return rc;
-    rc = conv_layer(e, w, p + "decode_layer_6", tag + "dec6", u3, 9, ACT_GELU, VPB_EPI_STORE, &a, nullptr); if (rc) return rc;
-    rc = conv_layer(e, w, p + "decode_layer_7", tag + "dec7", a, 9, ACT_GELU, VPB_EPI_STORE, &b, nullptr); if (rc) return rc;
-    rc = up_skip(e, w, p, 4, tag, b, nullptr, &u4); if (rc) return rc;
-    rc = conv_layer(e, w, p + "decode_layer_8", tag + "dec8", u4, 9, ACT_GELU, VPB_EPI_STORE, &c, nullptr); if (rc) return rc;
+    up_skip(e, b, p, 3, tag, neck, &enc.f[0], &u3);
+    conv_layer(e, b, p + "decode_layer_6", tag + "dec6", u3, &a);
+    conv_layer(e, b, p + "decode_layer_7", tag + "dec7", a, &c);
+    up_skip(e, b, p, 4, tag, c, nullptr, &u4);
+    conv_layer(e, b, p + "decode_layer_8", tag + "dec8", u4, &d);
   }
-  rc = conv_layer(e, w, p + "decode_layer_9", tag + "dec9", c, 9, ACT_GELU, VPB_EPI_STORE, &d, nullptr); if (rc) return rc;
-  e.tap(tag + "d9", d);
+  conv_layer(e, b, p + "decode_layer_9", tag + "dec9", d, &f);
+  e.tap(tag + "d9", f);
   const int fk = kind == VP_SCENE_SEG ? VPB_FINAL_ARGMAX : kind == VP_DOMAIN_SEG ? VPB_FINAL_THRESH : VPB_FINAL_NONE;
-  return final_conv(e, w, p + "decode_layer_10", tag + "dec10", d, fk, mo);
+  final_conv(e, b, p + "decode_layer_10", tag + "dec10", f, fk, mo);
 }
 
-static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
+static void build_model(vp_engine& e, NetBuilder& b, int idx, int kind) {
   const Prefixes pf = prefixes_for(kind);
   const std::string tag = std::to_string(idx) + "/";
-  const uint64_t h_enc = hash_prefix(w, pf.enc);
+  const uint64_t h_enc = hash_prefix(b.w, pf.enc);
   uint64_t h_trunk = h_enc;
-  { const uint64_t a = hash_prefix(w, pf.ctx), b = hash_prefix(w, pf.neck); h_trunk = fnv1a(fnv1a(h_trunk, &a, 8), &b, 8); }
+  { const uint64_t x = hash_prefix(b.w, pf.ctx), y = hash_prefix(b.w, pf.neck); h_trunk = fnv1a(fnv1a(h_trunk, &x, 8), &y, 8); }
   const auto ie = e.enc_cache.find(h_enc);
   const auto it = e.trunk_cache.find(h_trunk);
   // the model's lane starts after the op producing its input: a shared neck, a shared encoder, or the pre-process (op 0)
@@ -509,8 +449,7 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
   vp_engine::EncOut enc;
   if (ie != e.enc_cache.end()) { enc = ie->second; ++e.shared_encoders; }
   else {
-    int rc = build_encoder(e, w, pf.enc, tag, enc);
-    if (rc) return rc;
+    build_encoder(e, b, pf.enc, tag, enc);
     e.enc_cache[h_enc] = enc;
     e.enc_last_op[h_enc] = static_cast<int>(e.ops.size()) - 1;
   }
@@ -521,31 +460,25 @@ static int build_model(vp_engine& e, int idx, int kind, const WeightMap& w) {
     Tens feat = enc.f[4];
     if (kind == VP_EGO_LANES) {  // BackboneFeatureFusion (backbone_feature_fusion.py:13-38)
       feat = e.act_alloc(enc.f[4].H, enc.f[4].W, 1456);
-      const int dt = e.dtype; const void *f0 = enc.f[0].p, *f1 = enc.f[1].p, *f2 = enc.f[2].p, *f3 = enc.f[3].p, *f4 = enc.f[4].p;
-      void* o = feat.p; void* o_lo = feat.lo; const int H4 = feat.H, W4 = feat.W;
+      const int dt = e.dtype, nb = e.batch;
       struct LoOff { size_t v[5]; } lo{};
       for (int i = 0; i < 5; ++i)
         lo.v[i] = enc.f[i].lo ? static_cast<size_t>(static_cast<const uint8_t*>(enc.f[i].lo) - static_cast<const uint8_t*>(enc.f[i].p)) : 0;
-      const int nb = e.batch;
-      e.add_op(tag + "fuse", "fuse_pool_kernel", [=](cudaStream_t st) { return fuse_pool_x(dt, f0, f1, f2, f3, f4, lo.v, H4, W4, o, o_lo, st, nb); },
-               0.0, nb * 2.0 * (160.0 * 320 * 32 + 80.0 * 160 * 24 + 40.0 * 80 * 40 + 20.0 * 40 * 80 + 200.0 * 1280 + 200.0 * 1456));
+      b.op(tag + "fuse", "fuse_pool_kernel", [=](cudaStream_t st) { return fuse_pool_x(dt, enc.f[0].p, enc.f[1].p, enc.f[2].p, enc.f[3].p, enc.f[4].p, lo.v, feat.H, feat.W, feat.p, feat.lo, st, nb); },
+           0.0, nb * 2.0 * (160.0 * 320 * 32 + 80.0 * 160 * 24 + 40.0 * 80 * 40 + 20.0 * 40 * 80 + 200.0 * 1280 + 200.0 * 1456));
       e.tap(tag + "fused", feat);
     }
     Tens ctx;
-    int rc = build_context(e, w, pf.ctx, tag, feat, &ctx);
-    if (rc) return rc;
+    build_context(e, b, pf.ctx, tag, feat, &ctx);
     e.tap(tag + "context", ctx);
-    rc = build_neck(e, w, pf.neck, tag, ctx, enc, &neck);
-    if (rc) return rc;
+    build_neck(e, b, pf.neck, tag, ctx, enc, &neck);
     e.trunk_cache[h_trunk] = neck;
     e.trunk_last_op[h_trunk] = static_cast<int>(e.ops.size()) - 1;
   }
   e.tap(tag + "neck", neck);
   ModelOut mo; mo.kind = kind;
-  int rc = build_head(e, w, pf.head, tag, kind, neck, enc, mo);
-  if (rc) return rc;
+  build_head(e, b, pf.head, tag, kind, neck, enc, mo);
   e.outs.push_back(mo);
-  return VPB_OK;
 }
 
 // The source-output jobs of the call's frames: sample k's buffers grown to its frame (outside any capture),
@@ -755,9 +688,9 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
     WeightMap w;
     rc = load_vpw(cfg->weights[i], w);
     if (rc) return rc;
-    rc = build_model(*e, i, cfg->kinds[i], w);
-    if (e->oom) return VPB_ERR_CUDA;       // message set by the failing allocation
-    if (rc) return rc;
+    NetBuilder b{*e, w};
+    build_model(*e, b, i, cfg->kinds[i]);
+    if (b.status()) return b.status();     // an oom first (VPB_ERR_CUDA), with the failing allocation's message
   }
   if (e->oom) return VPB_ERR_CUDA;
   rc = build_source_outputs(*e);

@@ -4,6 +4,7 @@
 #include "engine_internal.h"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -88,6 +89,52 @@ std::vector<float> pack_conv(const HostTensor& t, const std::vector<float>* scal
         o[(static_cast<size_t>(tt) * Cout + co) * Cin + ci] =
             t.f[(static_cast<size_t>(co) * Cin + ci) * k * k + tt] * (scale ? (*scale)[co] : 1.0f);
   return o;
+}
+
+// =============================================================== network builder
+const HostTensor* NetBuilder::get(const std::string& key, std::initializer_list<int> dims) {
+  if (!ok()) return nullptr;
+  const HostTensor* t = find_w_shaped(w, key, dims);
+  if (!t) rc = VPB_ERR_IO;
+  return t;
+}
+
+bool NetBuilder::bn(const std::string& p, int C, float eps, std::vector<float>& s, std::vector<float>& t) {
+  const HostTensor *g = get(p + "weight", {C}), *b = get(p + "bias", {C}), *m = get(p + "running_mean", {C}),
+                   *v = get(p + "running_var", {C});
+  if (!ok()) return false;
+  s.resize(C); t.resize(C);
+  for (int c = 0; c < C; ++c) {
+    const float sc = g->f[c] / std::sqrt(v->f[c] + eps);
+    s[c] = sc; t[c] = b->f[c] - m->f[c] * sc;
+  }
+  return true;
+}
+
+NetBuilder::Params NetBuilder::folded(const std::string& key, std::initializer_list<int> dims, const std::string& bn_p,
+                                      float eps) {
+  std::vector<float> s, t;
+  const HostTensor* wt = get(key, dims);
+  if (!bn(bn_p, dims.begin()[0], eps, s, t)) return {};
+  return {e.upload_16(pack_conv(*wt, &s)), e.upload_f32(t)};
+}
+
+NetBuilder::Params NetBuilder::depthwise(const std::string& key, int C, int k, const std::string& bn_p, float eps) {
+  std::vector<float> s, t;
+  const HostTensor* wt = get(key, {C, 1, k, k});
+  if (!bn(bn_p, C, eps, s, t)) return {};
+  std::vector<float> o(static_cast<size_t>(k) * k * C);
+  for (int c = 0; c < C; ++c)
+    for (int kk = 0; kk < k * k; ++kk) o[static_cast<size_t>(kk) * C + c] = wt->f[static_cast<size_t>(c) * k * k + kk] * s[c];
+  return {e.upload_f32(o), e.upload_f32(t)};
+}
+
+NetBuilder::Params NetBuilder::plain(const std::string& key, std::initializer_list<int> dims, const HostTensor** wt) {
+  const HostTensor* cw = get(key + ".weight", dims);
+  const HostTensor* cb = cw ? get(key + ".bias", {cw->dims[0]}) : nullptr;
+  if (wt) *wt = cw;
+  if (!ok()) return {};
+  return {e.upload_16(pack_conv(*cw, nullptr)), e.upload_f32(cb->f)};
 }
 
 }  // namespace vpb

@@ -1,6 +1,6 @@
 // engine_internal.h — host-side runtime shared by the engines (engine.cu: the four segmentation / depth / lane
 // networks; autospeed.cu: the AutoSpeed detector), defined in engine_common.cu: the .vpw weight-file reader,
-// shape-checked lookups, K-major repacking, the device guard, the event owner, and EngineRuntime (device and stream
+// shape-checked lookups, K-major repacking, the network builder (NetBuilder), the device guard, the event owner, and EngineRuntime (device and stream
 // set-up, device / pinned allocations, weight uploads, activation tensors, the op list and its convolutions, the
 // launcher of a call with its lanes and per-call reset, the frame graph, the frame calls, kernel timing, tap read-back).
 #pragma once
@@ -270,6 +270,41 @@ struct EngineRuntime {
   virtual int geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, const char* who, PreGeom* g) = 0;
   virtual int enqueue(const PreGeom* g) = 0;
   virtual int fetch(bool raw) = 0;
+};
+
+// Builds a network's ops from its checkpoint w.  The first failure is kept (a missing or mis-shaped weight:
+// VPB_ERR_IO; a failed check of the network's own; a convolution the kernel cannot run; a device allocation, e.oom),
+// and every later step does nothing, so the create call reports the first vpb_last_error message.
+struct NetBuilder {
+  EngineRuntime& e;
+  const WeightMap& w;
+  int rc = VPB_OK;
+  struct Params { void* w = nullptr; float* b = nullptr; };   // a layer's device weight and fp32 bias
+
+  bool ok() const { return rc == VPB_OK && !e.oom; }
+  int status() const { return e.oom ? VPB_ERR_CUDA : rc; }
+  // keep code (the failing call has set the message) / keep code with the message fmt, unless a step failed before
+  void fail(int code) { if (ok()) rc = code; }
+  template <class... A> void fail(int code, const char* fmt, A... a) {
+    if (ok()) { rc = code; vpb_set_error(fmt, a...); }
+  }
+  // find_w_shaped; NULL (VPB_ERR_IO) for a missing or mis-shaped weight, and after any failure
+  const HostTensor* get(const std::string& key, std::initializer_list<int> dims);
+  // eval-mode BatchNorm of C channels (<p>weight, <p>bias, <p>running_mean, <p>running_var) as y * s + t:
+  // s = weight / sqrt(running_var + eps), t = bias - running_mean * s
+  bool bn(const std::string& p, int C, float eps, std::vector<float>& s, std::vector<float>& t);
+  // Conv2d(bias=False) weight `key` of shape dims, then the BatchNorm at bn_p: the weight scaled by s and packed
+  // (pack_conv) in 16 bits, t in fp32
+  Params folded(const std::string& key, std::initializer_list<int> dims, const std::string& bn_p, float eps);
+  // the same for a depthwise k x k weight [C][1][k][k]: the weight scaled by s as [k*k][C] and t, both fp32
+  Params depthwise(const std::string& key, int C, int k, const std::string& bn_p, float eps);
+  // nn.Conv2d with bias: <key>.weight of shape dims packed in 16 bits, <key>.bias [Cout] in fp32; *wt: the weight
+  Params plain(const std::string& key, std::initializer_list<int> dims, const HostTensor** wt = nullptr);
+  void conv(const std::string& name, const vpb_conv_args& a) { if (ok()) rc = e.append_conv(name, a); }
+  void op(const std::string& name, const char* kname, std::function<int(cudaStream_t)> fn, double flops = 0,
+          double bytes = 0) {
+    if (ok()) e.add_op(name, kname, std::move(fn), flops, bytes);
+  }
 };
 
 // A call on n host frames: frames_ok, the engine's geometries, its device, the upload of the frames, enqueue, fetch and

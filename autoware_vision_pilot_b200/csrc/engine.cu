@@ -14,6 +14,8 @@
 #include "../../include/vp_b200.h"
 #include "engine_internal.h"
 
+#include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstring>
 #include <functional>
@@ -118,10 +120,37 @@ struct vp_engine : EngineRuntime {
   // front_lane, before the lanes' join; det_geom are its letterboxes of the current call.
   vp_autospeed* det = nullptr;
   PreGeom det_geom[kMaxBatch];
+  // The network input each model's stem reads: d_pre, or its view's.  The stem op reads it when it launches; setting or
+  // clearing a view changes the op list, so the captured graph is dropped with it.
+  struct Input { const void* p = nullptr; const void* lo = nullptr; };
+  std::array<Input, VP_MAX_MODELS> input{};
+  std::vector<uint64_t> enc_hash;          // [model] hash of its encoder's weights (equal: the encoder is shared)
+  // A model's own region and convention of every sample's full() frame (vp_engine_set_view): op "preprocess/<m>" before
+  // the model's stem, on its lane, into its own network input and resized image (allocated on the first set, kept).
+  struct View {
+    bool on = false;
+    int convention = 0;
+    int roi[kMaxBatch][4] = {};
+    PreprocessPlan plan;
+    void* pre = nullptr; void* pre_lo = nullptr;
+    uint8_t* resized = nullptr;
+    PreGeom geom[kMaxBatch];               // of the current call
+  };
+  std::array<View, VP_MAX_MODELS> views;
 
+  // what model m reads of sample k: its view of full(), or the engine's pre()
+  vpb_frame_fmt input_frame(int m, int k) const {
+    return views[m].on ? crop_frame(chain[k].full(), views[m].roi[k]) : chain[k].pre();
+  }
   int geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, const char* who, PreGeom* g) override;
   int enqueue(const PreGeom* g) override;
   int fetch(bool raw) override;
+  void frame_key(std::vector<vpb_frame_fmt>& key) const override {
+    EngineRuntime::frame_key(key);
+    for (const View& v : views)
+      if (v.on)
+        for (int k = 0; k < n_frames; ++k) key.push_back(crop_frame(chain[k].full(), v.roi[k]));
+  }
 };
 
 namespace vpb {
@@ -145,7 +174,7 @@ static const int kStages[7][6] = {  // expand, kernel, stride, cin, cout, repeat
 
 // ---------------------------------------------------------------- encoder (backbone.py:11-22)
 static void build_encoder(vp_engine& e, NetBuilder& b, const std::string& p, const std::string& tag,
-                          vp_engine::EncOut& out) {
+                          const vp_engine::Input* in, vp_engine::EncOut& out) {
   const int dt = e.dtype, nb = e.batch;
   // stem
   std::vector<float> s, t;
@@ -158,8 +187,7 @@ static void build_encoder(vp_engine& e, NetBuilder& b, const std::string& p, con
   float* d_stem = e.upload_f32(stem);
   float* d_stem_b = e.upload_f32(t);
   Tens x = e.act_alloc(kNetH / 2, kNetW / 2, 32);
-  const void *in = e.d_pre, *in_lo = e.d_pre_lo;
-  b.op(tag + "stem", "stem_conv_kernel", [=](cudaStream_t st) { return stem_conv_x(dt, in, in_lo, kNetH, kNetW, d_stem, d_stem_b, x.p, x.lo, st, nb); },
+  b.op(tag + "stem", "stem_conv_kernel", [=](cudaStream_t st) { return stem_conv_x(dt, in->p, in->lo, kNetH, kNetW, d_stem, d_stem_b, x.p, x.lo, st, nb); },
        2.0 * x.H * x.W * 32 * 27, nb * (2.0 * kNetH * kNetW * 4 + 2.0 * x.H * x.W * 32));
   Tens stage_out[9];
   stage_out[0] = x;
@@ -446,10 +474,13 @@ static void build_model(vp_engine& e, NetBuilder& b, int idx, int kind) {
   const auto it = e.trunk_cache.find(h_trunk);
   // the model's lane starts after the op producing its input: a shared neck, a shared encoder, or the pre-process (op 0)
   e.begin_lane(idx, it != e.trunk_cache.end() ? e.trunk_last_op[h_trunk] : ie != e.enc_cache.end() ? e.enc_last_op[h_enc] : 0);
+  e.enc_hash.push_back(h_enc);
+  e.input[idx] = {e.d_pre, e.d_pre_lo};
+  e.tap(tag + "pre", e.taps["pre"].t, 3);
   vp_engine::EncOut enc;
   if (ie != e.enc_cache.end()) { enc = ie->second; ++e.shared_encoders; }
   else {
-    build_encoder(e, b, pf.enc, tag, enc);
+    build_encoder(e, b, pf.enc, tag, &e.input[idx], enc);
     e.enc_cache[h_enc] = enc;
     e.enc_last_op[h_enc] = static_cast<int>(e.ops.size()) - 1;
   }
@@ -485,7 +516,7 @@ static void build_model(vp_engine& e, NetBuilder& b, int idx, int kind) {
 // destinations, sizes and frame pointers.
 static int prepare_source(vp_engine& e) {
   for (auto& so : e.src_outs) {
-    const vpb_frame_fmt fr = e.chain[so.sample].pre();   // packed when a job is an overlay (vp_engine::geoms)
+    const vpb_frame_fmt fr = e.input_frame(so.model, so.sample);   // packed when a job is an overlay (vp_engine::geoms)
     vpb_src_job& j = so.job;
     const int el = j.kind == VPB_SRC_DEPTH ? 4 : j.kind == VPB_SRC_OVERLAY ? 3 : 1;
     const size_t bytes = static_cast<size_t>(fr.h) * fr.w * el;
@@ -572,11 +603,24 @@ static int check_source_flags(const vp_engine_config& c) {
 // Every frame resizes to the 640 x 320 network input: VPB_ERR_ARG (naming `who` and the frame) if one cannot in the
 // engine's resize mode, or if the engine makes overlays and the frame is not packed (the overlay blends the camera
 // frame's pixels as vpb_src_job reads them; a rectified sample's frame here is the packed rectified frame).  With a
-// detector, its letterboxes of the full frames.  Host-only: callers run it before any device work.
+// detector, its letterboxes of the full frames.  Each view's regions pass region_check and resize likewise (the view
+// geometries of the call).  Host-only: callers run it before any device work.
 int vp_engine::geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, const char* who, PreGeom* g) {
+  for (int m = 0; m < static_cast<int>(outs.size()); ++m) {
+    View& v = views[m];
+    for (int k = 0; k < batch && v.on; ++k) {
+      if (region_check(full[k], v.roi[k], m, who, k)) return VPB_ERR_ARG;
+      const vpb_frame_fmt f = crop_frame(full[k], v.roi[k]);
+      v.geom[k] = PreGeom{};
+      v.geom[k].h = f.h; v.geom[k].w = f.w;
+      const int rc = PreprocessPlan::check(v.geom[k], cfg.resize_mode, who, k);
+      if (rc) return rc;
+    }
+  }
   for (int k = 0; k < batch; ++k) {
-    if (lat_model >= 0 && frames[k].h > kLatMaxImgH) {
-      vpb_set_error("%s: frame %d: height %d is above the %d rows the lateral post-process takes", who, k, frames[k].h,
+    const int lat_h = lat_model < 0 ? 0 : views[lat_model].on ? views[lat_model].geom[k].h : frames[k].h;
+    if (lat_h > kLatMaxImgH) {
+      vpb_set_error("%s: frame %d: height %d is above the %d rows the lateral post-process takes", who, k, lat_h,
                     kLatMaxImgH);
       return VPB_ERR_ARG;
     }
@@ -599,6 +643,14 @@ int vp_engine::enqueue(const PreGeom* g) {
   src_host = false;
   lat_host = false;
   int rc = pre.configure(g, batch, cfg.resize_mode);
+  for (int m = 0; m < static_cast<int>(outs.size()) && rc == VPB_OK; ++m) {
+    View& v = views[m];
+    if (!v.on) continue;
+    rc = v.plan.configure(v.geom, batch, cfg.resize_mode);
+    double bytes = 0;   // as "preprocess": frame read + 3 x OH x OW 16-bit written, per sample
+    for (int k = 0; k < batch; ++k) bytes += frame_bytes(input_frame(m, k)) + 2.0 * 3 * v.geom[k].OH * v.geom[k].OW;
+    ops[op_index(("preprocess/" + std::to_string(m)).c_str())].bytes = bytes;
+  }
   if (rc == VPB_OK && !src_outs.empty()) rc = prepare_source(*this);
   if (rc == VPB_OK && det) {
     rc = autospeed_prepare(det, det_geom, stream);
@@ -798,6 +850,126 @@ extern "C" int vp_engine_set_roi(vp_engine* e, int sample, int x, int y, int w, 
   return e->set_roi(sample, x, y, w, h, "vp_engine_set_roi");
 }
 
+// ---------------------------------------------------------------- per-model input views
+// sample `sample` of the [batch][320][640][3] resized images at src to dst (host), synchronously
+static int read_resized(vp_engine* e, const uint8_t* src, int sample, uint8_t* dst, const char* who) {
+  if (sample < 0 || sample >= e->batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch); return VPB_ERR_ARG; }
+  DeviceGuard guard(e->gpu_id);
+  const size_t bytes = static_cast<size_t>(kNetH) * kNetW * 3;
+  VPB_CUDA_OK(cudaMemcpyAsync(dst, src + bytes * sample, bytes, cudaMemcpyDeviceToHost, e->stream));
+  VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
+  return VPB_OK;
+}
+
+static bool reads_bgr(int convention) { return convention == VPB_CONV_BGR_NOSWAP || convention == VPB_CONV_BGR_SWAP; }
+
+// Op "preprocess/<m>": the pre-process of model m's view of every sample's full() frame into the view's buffers
+static OpRec view_op(vp_engine& e, int m) {
+  OpRec op;
+  op.name = "preprocess/" + std::to_string(m); op.kname = "preprocess"; op.lane = m;
+  vp_engine* ep = &e;
+  op.describe = [ep, m](KernelCall& c) {
+    const vp_engine::View& v = ep->views[m];
+    Frames f{};
+    for (int k = 0; k < ep->batch; ++k) f[k] = ep->input_frame(m, k);
+    return v.plan.describe(f.data(), v.convention, ep->dtype, v.pre, v.resized, c);
+  };
+  return op;
+}
+
+// model m's stem, its "<m>/pre" tap and its lane's fork follow its view (on) or the engine's input
+static void route_input(vp_engine& e, int m, bool on) {
+  vp_engine::View& v = e.views[m];
+  e.input[m] = on ? vp_engine::Input{v.pre, v.pre_lo} : vp_engine::Input{e.d_pre, e.d_pre_lo};
+  Tens t = e.taps["pre"].t;
+  t.p = const_cast<void*>(e.input[m].p); t.lo = const_cast<void*>(e.input[m].lo);
+  e.tap(std::to_string(m) + "/pre", t, 3);
+  if (m == 0) return;                      // lane 0 is the engine stream: its ops already follow the front ops
+  auto& ff = e.front_forks;
+  ff.erase(std::remove(ff.begin(), ff.end(), m), ff.end());
+  if (on) ff.push_back(m);
+  e.set_lane_dep(m, on ? e.op_index("preprocess") - 1 : e.op_index("preprocess"));
+}
+
+extern "C" int vp_engine_set_view(vp_engine* e, int model_idx, const vp_view* v) {
+  const char* who = "vp_engine_set_view";
+  if (!e) { vpb_set_error("%s: NULL engine", who); return VPB_ERR_ARG; }
+  const int nm = static_cast<int>(e->outs.size());
+  if (model_idx < 0 || model_idx >= nm) {
+    vpb_set_error("%s: model %d out of range (the engine has %d models)", who, model_idx, nm);
+    return VPB_ERR_ARG;
+  }
+  if (v) {
+    const int conv = v->convention == -1 ? e->cfg.convention : v->convention;
+    if (conv < VPB_CONV_RGB || conv > VPB_CONV_RGB_UNIT) {
+      vpb_set_error("%s: unknown convention %d", who, v->convention);
+      return VPB_ERR_ARG;
+    }
+    if (reads_bgr(conv) != (e->rect_bgr != 0)) {
+      vpb_set_error("%s: convention %d reads %s, the engine's convention %d reads %s: the decoded and rectified frames "
+                    "are written in the engine's channel order", who, conv, reads_bgr(conv) ? "B, G, R" : "R, G, B",
+                    e->cfg.convention, e->rect_bgr ? "B, G, R" : "R, G, B");
+      return VPB_ERR_ARG;
+    }
+    for (int k = 0; k < e->batch; ++k) {
+      const int* r = v->roi[k];
+      if (region_args_check(k, r[0], r[1], r[2], r[3], who)) return VPB_ERR_ARG;
+    }
+    for (int j = 0; j < nm; ++j)
+      if (j != model_idx && e->enc_hash[j] == e->enc_hash[model_idx]) {
+        vpb_set_error("%s: model %d shares its encoder with model %d; a view needs a model with an encoder of its own",
+                      who, model_idx, j);
+        return VPB_ERR_ARG;
+      }
+  }
+  DeviceGuard guard(e->gpu_id);
+  vp_engine::View& view = e->views[model_idx];
+  e->n_frames = 0;                         // the last call's frames are not those the model now reads
+  if (!v) {
+    if (!view.on) return VPB_OK;
+    e->erase_ops(e->op_index(("preprocess/" + std::to_string(model_idx)).c_str()), 1);
+    view.on = false;
+    route_input(*e, model_idx, false);
+    return VPB_OK;
+  }
+  if (!view.pre) {
+    const size_t in = static_cast<size_t>(kNetH) * kNetW * 4 * 2 * e->batch * (e->split ? 2 : 1),
+                 rs = static_cast<size_t>(kNetH) * kNetW * 3 * e->batch;
+    void* p = nullptr; void* q = nullptr;
+    VPB_CUDA_OK(cudaMalloc(&p, in));
+    e->dev_allocs.push_back(p);
+    VPB_CUDA_OK(cudaMalloc(&q, rs));
+    e->dev_allocs.push_back(q);
+    VPB_CUDA_OK(cudaMemsetAsync(p, 0, in, e->stream));   // the fourth channel stays zero, as d_pre's
+    view.pre = p;
+    if (e->split) view.pre_lo = static_cast<uint8_t*>(p) + static_cast<size_t>(kNetH) * kNetW * 4 * 2;
+    view.plan.out_lo = view.pre_lo;
+    view.resized = static_cast<uint8_t*>(q);
+  }
+  view.convention = v->convention == -1 ? e->cfg.convention : v->convention;
+  for (int k = 0; k < e->batch; ++k) {
+    const int* r = v->roi[k];
+    const bool whole = r[2] == 0 && r[3] == 0;
+    for (int i = 0; i < 4; ++i) view.roi[k][i] = whole ? 0 : r[i];
+  }
+  if (view.on) return VPB_OK;              // a new region or convention: the next call re-points or captures again
+  view.on = true;
+  e->insert_ops(e->op_index((std::to_string(model_idx) + "/stem").c_str()), {view_op(*e, model_idx)});
+  route_input(*e, model_idx, true);
+  return VPB_OK;
+}
+
+extern "C" int vp_engine_read_resized_view(vp_engine* e, int model_idx, int sample, uint8_t* dst) {
+  const char* who = "vp_engine_read_resized_view";
+  if (!e || !dst) { vpb_set_error("%s: bad arguments", who); return VPB_ERR_ARG; }
+  if (model_idx < 0 || model_idx >= static_cast<int>(e->outs.size())) {
+    vpb_set_error("%s: model %d out of range (the engine has %d models)", who, model_idx, static_cast<int>(e->outs.size()));
+    return VPB_ERR_ARG;
+  }
+  const vp_engine::View& v = e->views[model_idx];
+  return read_resized(e, v.on ? v.resized : e->d_resized, sample, dst, who);
+}
+
 // ---------------------------------------------------------------- the detector inside the call
 // Op "det/letterbox": the detector's letterbox of every sample's full() frame, B, G, R under the BGR conventions.
 static OpRec letterbox_op(vp_engine& e) {
@@ -868,7 +1040,7 @@ static OpRec lateral_op(vp_engine& e) {
     const ModelOut& m = ep->outs[ep->lat_model];
     int iw[kMaxBatch], ih[kMaxBatch];
     for (int k = 0; k < ep->batch; ++k) {
-      const vpb_frame_fmt f = ep->chain[k].pre();
+      const vpb_frame_fmt f = ep->input_frame(ep->lat_model, k);
       iw[k] = f.w; ih[k] = f.h;
     }
     const size_t rd = static_cast<size_t>(ep->lat_cur) * ep->batch, wr = static_cast<size_t>(1 - ep->lat_cur) * ep->batch;
@@ -1069,12 +1241,7 @@ extern "C" int vp_engine_read_resized(vp_engine* e, uint8_t* dst) { return vp_en
 
 extern "C" int vp_engine_read_resized_at(vp_engine* e, int sample, uint8_t* dst) {
   if (!e || !dst) return VPB_ERR_ARG;
-  if (sample < 0 || sample >= e->batch) { vpb_set_error("vp_engine_read_resized: sample %d of a batch of %d", sample, e->batch); return VPB_ERR_ARG; }
-  DeviceGuard guard(e->gpu_id);
-  const size_t bytes = static_cast<size_t>(kNetH) * kNetW * 3;
-  VPB_CUDA_OK(cudaMemcpyAsync(dst, e->d_resized + bytes * sample, bytes, cudaMemcpyDeviceToHost, e->stream));
-  VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
-  return VPB_OK;
+  return read_resized(e, e->d_resized, sample, dst, "vp_engine_read_resized");
 }
 
 extern "C" long vp_engine_read_tap(vp_engine* e, const char* name, float* dst, long cap, int* c, int* h, int* w) {

@@ -159,9 +159,10 @@ static bool same_geometry(const vpb_frame_fmt& a, const vpb_frame_fmt& b) {
 
 int FrameGraph::run(EngineRuntime& e) {
   const cudaStream_t st = e.stream;
-  bool same_geom = exec && n == e.n_frames;
-  for (int k = 0; k < e.n_frames && same_geom; ++k)
-    same_geom = same_geometry(geom[k], e.chain[k].pre()) && same_geometry(geom_full[k], e.chain[k].full());
+  std::vector<vpb_frame_fmt> now;
+  e.frame_key(now);
+  bool same_geom = exec && now.size() == key.size();
+  for (size_t i = 0; i < now.size() && same_geom; ++i) same_geom = same_geometry(key[i], now[i]);
   if (same_geom) {
     KernelCall c;
     for (Node& r : nodes) {
@@ -174,7 +175,7 @@ int FrameGraph::run(EngineRuntime& e) {
   } else {
     invalidate();
     nodes.clear();
-    n = 0;
+    key.clear();
     int rc = e.launch_all(st);
     if (rc) return rc;
     VPB_CUDA_OK(cudaStreamSynchronize(st));
@@ -191,8 +192,7 @@ int FrameGraph::run(EngineRuntime& e) {
     if (graph) cudaGraphDestroy(graph);
     graph = g;
     if (ce != cudaSuccess) { vpb_set_error("graph instantiate failed: %s", cudaGetErrorString(ce)); return VPB_ERR_CUDA; }
-    for (int k = 0; k < e.n_frames; ++k) { geom[k] = e.chain[k].pre(); geom_full[k] = e.chain[k].full(); }
-    n = e.n_frames;
+    key = std::move(now);
   }
   VPB_CUDA_OK(cudaGraphLaunch(exec, st));
   return VPB_OK;
@@ -328,14 +328,39 @@ vpb_frame_fmt SampleFrames::full() const {
   return map ? packed_frame(vpb_frame{rect.p, map->map_h, map->map_w, 3 * map->map_w}) : decoded();
 }
 
-vpb_frame_fmt SampleFrames::pre() const {
-  vpb_frame_fmt f = full();
-  if (!roi[2]) return f;
+vpb_frame_fmt crop_frame(vpb_frame_fmt f, const int* r) {
+  if (!r[2]) return f;
   const int bpp = f.w > 0 ? frame_row_bytes(f) / f.w : 0;    // bytes per pixel of the main plane (NV12: the Y plane)
-  if (f.data) f.data += static_cast<size_t>(roi[1]) * f.stride + static_cast<size_t>(roi[0]) * bpp;
-  if (f.format == VPB_PIX_NV12 && f.uv) f.uv += static_cast<size_t>(roi[1] / 2) * f.uv_stride + roi[0];
-  f.w = roi[2]; f.h = roi[3];
+  if (f.data) f.data += static_cast<size_t>(r[1]) * f.stride + static_cast<size_t>(r[0]) * bpp;
+  if (f.format == VPB_PIX_NV12 && f.uv) f.uv += static_cast<size_t>(r[1] / 2) * f.uv_stride + r[0];
+  f.w = r[2]; f.h = r[3];
   return f;
+}
+
+int region_check(const vpb_frame_fmt& full, const int* r, int model, const char* who, int k) {
+  if (!r[2]) return VPB_OK;
+  char by[48] = "";
+  if (model >= 0) snprintf(by, sizeof(by), " in the view of model %d", model);
+  if (static_cast<long long>(r[0]) + r[2] > full.w || static_cast<long long>(r[1]) + r[3] > full.h) {
+    vpb_set_error("%s: frame %d: the region %dx%d at (%d, %d) set for sample %d%s does not lie inside its %dx%d frame",
+                  who, k, r[2], r[3], r[0], r[1], k, by, full.w, full.h);
+    return VPB_ERR_ARG;
+  }
+  const int fmt = full.format;
+  if (fmt != VPB_PIX_PACKED && fmt != VPB_PIX_BGRA && fmt != VPB_PIX_RGBA && ((r[0] | r[1]) & 1)) {
+    vpb_set_error("%s: frame %d: the region set for sample %d%s starts at (%d, %d); a YUV or Bayer frame needs an even x "
+                  "and y", who, k, k, by, r[0], r[1]);
+    return VPB_ERR_ARG;
+  }
+  if (fmt != VPB_PIX_PACKED && frame_fmt_check(crop_frame(full, r), who, k)) return VPB_ERR_ARG;
+  return VPB_OK;
+}
+
+int region_args_check(int sample, int x, int y, int w, int h, const char* who) {
+  if ((w == 0 && h == 0) || (x >= 0 && y >= 0 && w > 0 && h > 0)) return VPB_OK;
+  vpb_set_error("%s: sample %d: region %dx%d at (%d, %d) (need x, y >= 0 and w, h > 0, or w = h = 0 to clear)", who,
+                sample, w, h, x, y);
+  return VPB_ERR_ARG;
 }
 
 // the samples of e with a map, in sample order: the frames the rectify op reads, their maps and outputs; the count
@@ -374,12 +399,8 @@ void EngineRuntime::erase_ops(size_t at, size_t m) {
 
 int EngineRuntime::set_roi(int sample, int x, int y, int w, int h, const char* who) {
   if (sample < 0 || sample >= batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, batch); return VPB_ERR_ARG; }
+  if (region_args_check(sample, x, y, w, h, who)) return VPB_ERR_ARG;
   const bool clear = w == 0 && h == 0;
-  if (!clear && (x < 0 || y < 0 || w <= 0 || h <= 0)) {
-    vpb_set_error("%s: sample %d: region %dx%d at (%d, %d) (need x, y >= 0 and w, h > 0, or w = h = 0 to clear)", who,
-                  sample, w, h, x, y);
-    return VPB_ERR_ARG;
-  }
   int* r = chain[sample].roi;
   r[0] = clear ? 0 : x; r[1] = clear ? 0 : y; r[2] = clear ? 0 : w; r[3] = clear ? 0 : h;
   n_frames = 0;                           // the last call's frames are not those the pre-process now reads
@@ -427,7 +448,16 @@ void EngineRuntime::sync_front_ops() {
     const int n = rect_list(*this, f, m, o);
     ops[op_index("rectify")].bytes = rectify_bytes(f, m, n);
   }
-  if (front_lane > 0) set_lane_dep(front_lane, op_index("preprocess") - 1);   // the last front op, -1: none
+  const int front = op_index("preprocess") - 1;   // the last front op, -1: none
+  if (front_lane > 0) set_lane_dep(front_lane, front);
+  for (int l : front_forks) set_lane_dep(l, front);
+}
+
+void EngineRuntime::frame_key(std::vector<vpb_frame_fmt>& key) const {
+  for (int k = 0; k < n_frames; ++k) {
+    key.push_back(chain[k].pre());
+    key.push_back(chain[k].full());
+  }
 }
 
 void EngineRuntime::set_lane_dep(int lane, int dep) {
@@ -605,9 +635,8 @@ bool frames_ok(const EngineRuntime* e, const vpb_frame_fmt* frames, int n, const
 }
 
 // Host-only checks of the call's frames (VPB_ERR_ARG naming who and the frame): a sample with a map needs a frame of the
-// map's source size; a sample's region must lie inside its full() frame, start at an even x and y on an unrectified
-// YUV or Bayer frame (an odd offset would change the chroma phase or the Bayer pattern), and, cropped, still be a
-// frame frame_fmt_check takes.  Then the engine's geometries g of what the pre-process will read.
+// map's source size; a sample's region must pass region_check.  Then the engine's geometries g of what the pre-process
+// will read.
 static int pre_geoms(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const char* who, PreGeom* g) {
   Frames pre{}, full{};
   for (int k = 0; k < n; ++k) {
@@ -621,20 +650,7 @@ static int pre_geoms(EngineRuntime* e, const vpb_frame_fmt* frames, int n, const
     }
     full[k] = s.full();
     pre[k] = s.pre();
-    const int* r = s.roi;
-    if (!r[2]) continue;
-    if (static_cast<long long>(r[0]) + r[2] > full[k].w || static_cast<long long>(r[1]) + r[3] > full[k].h) {
-      vpb_set_error("%s: frame %d: the region %dx%d at (%d, %d) set for sample %d does not lie inside its %dx%d frame",
-                    who, k, r[2], r[3], r[0], r[1], k, full[k].w, full[k].h);
-      return VPB_ERR_ARG;
-    }
-    const int fmt = full[k].format;
-    if (fmt != VPB_PIX_PACKED && fmt != VPB_PIX_BGRA && fmt != VPB_PIX_RGBA && ((r[0] | r[1]) & 1)) {
-      vpb_set_error("%s: frame %d: the region set for sample %d starts at (%d, %d); a YUV or Bayer frame needs an even x "
-                    "and y", who, k, k, r[0], r[1]);
-      return VPB_ERR_ARG;
-    }
-    if (fmt != VPB_PIX_PACKED && frame_fmt_check(pre[k], who, k)) return VPB_ERR_ARG;
+    if (region_check(full[k], s.roi, -1, who, k)) return VPB_ERR_ARG;
   }
   return e->geoms(pre.data(), full.data(), who, g);
 }

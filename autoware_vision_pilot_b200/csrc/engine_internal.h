@@ -92,8 +92,8 @@ using Frames = std::array<vpb_frame_fmt, kMaxBatch>;
 
 struct EngineRuntime;
 // The CUDA graph of one call of a runtime's launch list.  It is captured again when the op list changes (insert_ops,
-// erase_ops, and invalidate for op arguments that are not described) or when the geometry key does: the n (format, h,
-// w, stride, uv_stride) tuples of the frames the pre-process reads and of the uncropped frames they are regions of.  A new format selects another pre-process kernel;
+// erase_ops, and invalidate for op arguments that are not described) or when the geometry key does: the (format, h,
+// w, stride, uv_stride) tuples of the frames EngineRuntime::frame_key lists.  A new format selects another pre-process kernel;
 // the grids and tables follow the geometries.  Otherwise every described op's launch is rebuilt from the current call
 // and set on its captured node where it differs from the launch the node holds, so the captured kernels read this
 // call's frames, maps, JPEG streams and scratch buffers, whichever of them changed.
@@ -103,9 +103,7 @@ struct FrameGraph {
   bool capturing = false;                // inside run()'s capture: EngineRuntime::launch_op records nodes
   struct Node { size_t op; cudaGraphNode_t node; KernelCall call; };   // a described op, its node, the launch it holds
   std::vector<Node> nodes;
-  int n = 0;                             // the geometry key: geometries of geom[0 .. n-1] (0: none)
-  Frames geom{};
-  Frames geom_full{};                    // ... and of geom_full[0 .. n-1], the uncropped frames (SampleFrames::full)
+  std::vector<vpb_frame_fmt> key;        // the geometry key: the frames of frame_key at the capture (empty: none)
   int captures = 0;                      // captures so far (vp_engine_graph_captures)
 
   // Launch the graph for e's frames on e's stream.  When the key differs: e.launch_all once outside capture (sets
@@ -117,6 +115,18 @@ struct FrameGraph {
 
 // Device scratch of the front end, grown on demand outside any capture (EngineRuntime::grow)
 struct Scratch { uint8_t* p = nullptr; size_t cap = 0; };
+
+// The w x h region at (x, y) = r[0..3] of f: the data pointer, and NV12's uv, offset to (x, y), the same strides, the
+// region's size; f itself for w = 0.  Host-only checks read the geometry alone (the pointers may be NULL).
+vpb_frame_fmt crop_frame(vpb_frame_fmt f, const int* r);
+// Call-time checks of region r of the frame `full` (VPB_ERR_ARG naming who and frame k; model >= 0: the region is that
+// model's view, otherwise the sample's set_roi region): it lies inside the frame, starts at an even x and y on an
+// unrectified YUV or Bayer frame (an odd offset would change the chroma phase or the Bayer pattern), and, cropped, still
+// is a frame frame_fmt_check takes.  r[2] = 0 (the whole frame) passes.
+int region_check(const vpb_frame_fmt& full, const int* r, int model, const char* who, int k);
+// Set-time check of a region (x, y, w, h) of sample `sample`: VPB_ERR_ARG naming who unless x, y >= 0 and w, h > 0, or
+// w = h = 0 (no region)
+int region_args_check(int sample, int x, int y, int w, int h, const char* who);
 
 // Sample k's frame chain: the frame as given -> JPEG-decoded -> rectified -> its region -> what the pre-process reads.
 struct SampleFrames {
@@ -130,10 +140,9 @@ struct SampleFrames {
   // the whole frame of the sample: with a map, the rectified frame packed at the map size in rect; otherwise decoded()
   // (what an attached detector's letterbox reads)
   vpb_frame_fmt full() const;
-  // what the pre-process (and the letterbox, the source outputs, the resized image, the lateral op) reads: full(), or
-  // with a region its view (the data pointer, and NV12's uv, offset to (x, y), the same strides, the region's size).
-  // Host-only checks read the geometry alone.
-  vpb_frame_fmt pre() const;
+  // what the pre-process (and the source outputs, the resized image, the lateral op) reads: full(), or with a region
+  // crop_frame(full(), roi)
+  vpb_frame_fmt pre() const { return crop_frame(full(), roi); }
 };
 
 struct ConvPlan;
@@ -152,6 +161,7 @@ struct EngineRuntime {
   // none (lane_dep -1: it waits on call_start, recorded on the engine stream after the per-call reset); 0: none.
   // sync_front_ops keeps its lane_dep right.
   int front_lane = 0;
+  std::vector<int> front_forks;           // other lanes that fork where front_lane does (a model reading a view of its own)
   Event call_start;
   bool single_stream = false;             // the lanes run one after another on the engine stream
   bool use_graph = true;                  // run_call replays the frame graph
@@ -214,7 +224,8 @@ struct EngineRuntime {
   void insert_ops(size_t at, std::vector<OpRec> add);
   void erase_ops(size_t at, size_t m);
   // The front ops before "preprocess" exactly while they are needed: the three JPEG decode ops while a sample's frame
-  // is JPEG, then "rectify" while a sample has a map; with their bytes for the current frames; and front_lane's fork.
+  // is JPEG, then "rectify" while a sample has a map; with their bytes for the current frames; and the forks of
+  // front_lane and front_forks.
   void sync_front_ops();
   // Region (x, y, w, h) of sample `sample`'s full() frame for the pre-process of every later call; w == h == 0 clears
   // it.  VPB_ERR_ARG (naming who) for a sample out of range, x or y < 0, or w, h <= 0 other than the clearing pair.
@@ -234,6 +245,9 @@ struct EngineRuntime {
   int launch_all(cudaStream_t st);
   // launch_all through the frame graph (use_graph) or on the engine stream
   int run_call() { return use_graph ? frame_graph.run(*this) : launch_all(stream); }
+  // The frames whose geometries key the frame graph: each sample's pre() and full() of the current call; an engine
+  // whose ops read other frames adds them.
+  virtual void frame_key(std::vector<vpb_frame_fmt>& key) const;
   // vpb_conv_args of a convolution in -> out (+ res, + the second input in2 with weights w2) from the views: shapes,
   // ld, pad, the split low halves and the batch.  3x3 on a zero-bordered input runs LINEAR (the layer also writes its
   // output's zero border, so the next 3x3 layer reads it as it stands), everything else and the split-fp16 mode

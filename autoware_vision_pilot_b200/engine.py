@@ -11,7 +11,7 @@ from . import _lib as L
 SCENE_SEG, SCENE_3D, DOMAIN_SEG, EGO_LANES = 0, 1, 2, 3
 KIND_BY_NAME = {"scene_seg": SCENE_SEG, "scene_3d": SCENE_3D, "domain_seg": DOMAIN_SEG, "ego_lanes": EGO_LANES}
 RESIZE_NONE, RESIZE_PIL_BICUBIC, RESIZE_CV_LINEAR = 0, 1, 2
-CONV_RGB, CONV_BGR_NOSWAP, CONV_BGR_SWAP = 0, 1, 2
+CONV_RGB, CONV_BGR_NOSWAP, CONV_BGR_SWAP, CONV_RGB_UNIT = 0, 1, 2, 3
 RESIZE_BY_NAME = {"none": RESIZE_NONE, "pil_bicubic": RESIZE_PIL_BICUBIC, "cv_linear": RESIZE_CV_LINEAR}
 DTYPE_BY_NAME = {"fp16": L.VPB_F16, "bf16": L.VPB_BF16, "fp32": L.VPB_F16}
 PREC_16, PREC_SPLIT = 0, 1
@@ -60,6 +60,12 @@ class LateralConfig(C.Structure):
     """Mirror of vp_lateral_config (include/vp_b200.h)."""
 
     _fields_ = [("threshold", C.c_float), ("smoothing", C.c_float), ("homographies", C.POINTER(C.c_double))]
+
+
+class View(C.Structure):
+    """Mirror of vp_view (include/vp_b200.h)."""
+
+    _fields_ = [("convention", C.c_int), ("roi", (C.c_int * 4) * MAX_BATCH)]
 
 
 class _TapView(C.Structure):
@@ -121,6 +127,8 @@ def _bind():
     lib.vp_engine_graph_captures.argtypes = [C.c_void_p]
     lib.vp_engine_set_roi.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     lib.vp_engine_set_detector.argtypes = [C.c_void_p, C.c_void_p]
+    lib.vp_engine_set_view.argtypes = [C.c_void_p, C.c_int, C.POINTER(View)]
+    lib.vp_engine_read_resized_view.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     _bound = True
     return lib
 
@@ -156,6 +164,7 @@ class Engine:
         L.check(self._lib.vp_engine_create(C.byref(cfg), C.byref(self._h)), "vp_engine_create")
         self.kinds = list(kinds)
         self.batch = max(1, batch)
+        self.convention = convention
         self._rectify = {}
         self._detector = None
 
@@ -185,6 +194,40 @@ class Engine:
         if roi is not None and (x < 0 or y < 0 or w <= 0 or h <= 0):
             raise ValueError(f"region {tuple(roi)}: need x, y >= 0 and w, h > 0")
         L.check(self._lib.vp_engine_set_roi(self._h, sample, x, y, w, h), "vp_engine_set_roi")
+
+    def set_view(self, model_idx: int, rois: Optional[Sequence[Optional[Sequence[int]]]] = None,
+                 convention: Optional[int] = None) -> None:
+        """Give model model_idx an input of its own in every later call: sample k's region rois[k] = (x, y, w, h) of its
+        frame after JPEG decode and rectify (None, or rois None: the whole frame), in `convention` (None: the engine's).
+        The model's outputs, taps ("<m>/pre"), source outputs, lateral image size and read_resized(k, model_idx) follow
+        the view; the other models keep the engine's input.  rois and convention both None: no view (the engine's input
+        again).  The convention must read the engine's channel order (R, G, B: CONV_RGB; B, G, R: the BGR conventions),
+        and the model must have an encoder of its own."""
+        if not 0 <= model_idx < len(self.kinds):
+            raise ValueError(f"model {model_idx} out of range (the engine has {len(self.kinds)} models)")
+        if rois is None and convention is None:
+            L.check(self._lib.vp_engine_set_view(self._h, model_idx, None), "vp_engine_set_view")
+            return
+        v = View()
+        v.convention = -1 if convention is None else int(convention)
+        if convention is not None:
+            if convention not in (CONV_RGB, CONV_BGR_NOSWAP, CONV_BGR_SWAP, CONV_RGB_UNIT):
+                raise ValueError(f"unknown convention {convention}")
+            if (convention in (CONV_BGR_NOSWAP, CONV_BGR_SWAP)) != (self.convention in (CONV_BGR_NOSWAP, CONV_BGR_SWAP)):
+                raise ValueError(f"convention {convention} reads another channel order than the engine's convention "
+                                 f"{self.convention}")
+        if rois is not None:
+            rois = list(rois)
+            if len(rois) != self.batch:
+                raise ValueError(f"{len(rois)} region(s) for an engine of batch {self.batch}")
+            for k, r in enumerate(rois):
+                if r is None:
+                    continue
+                x, y, w, h = (int(a) for a in r)
+                if x < 0 or y < 0 or w <= 0 or h <= 0:
+                    raise ValueError(f"region {tuple(r)} of sample {k}: need x, y >= 0 and w, h > 0")
+                v.roi[k][:] = [x, y, w, h]
+        L.check(self._lib.vp_engine_set_view(self._h, model_idx, C.byref(v)), "vp_engine_set_view")
 
     def set_detector(self, det) -> None:
         """Run the AutoSpeedEngine det (of this engine's batch and GPU) on every sample's whole frame inside every later
@@ -549,10 +592,19 @@ class Engine:
     def handle(self) -> C.c_void_p:
         return self._h
 
-    def read_resized(self, sample: int = 0) -> np.ndarray:
-        """The 640x320 uint8 image the fused resize produced for sample `sample` of the last call."""
+    def read_resized(self, sample: int = 0, model: Optional[int] = None) -> np.ndarray:
+        """The 640x320 uint8 image the fused resize produced for sample `sample` of the last call: the engine's, or with
+        `model` the one that model read (its view's, set_view)."""
         buf = np.empty((320, 640, 3), dtype=np.uint8)
-        L.check(self._lib.vp_engine_read_resized_at(self._h, sample, buf.ctypes.data), "vp_engine_read_resized_at")
+        if model is None:
+            L.check(self._lib.vp_engine_read_resized_at(self._h, sample, buf.ctypes.data), "vp_engine_read_resized_at")
+            return buf
+        if not 0 <= model < len(self.kinds):
+            raise ValueError(f"model {model} out of range (the engine has {len(self.kinds)} models)")
+        if not 0 <= sample < self.batch:
+            raise ValueError(f"sample {sample} of a batch of {self.batch}")
+        L.check(self._lib.vp_engine_read_resized_view(self._h, model, sample, buf.ctypes.data),
+                "vp_engine_read_resized_view")
         return buf
 
     def read_tap(self, name: str) -> np.ndarray:

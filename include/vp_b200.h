@@ -182,6 +182,31 @@ int vp_engine_set_rectify(vp_engine* e, int sample, const vpb_rectify* r);
  * frame graph; a new size captures it again. */
 int vp_engine_set_roi(vp_engine* e, int sample, int x, int y, int w, int h);
 
+/* A view of its own for model model_idx: every later call's pre-process of that model reads region roi[k] of sample k's
+ * frame after its JPEG decode and rectify, in convention `convention`, into the model's own network input (op
+ * "preprocess/<model_idx>", on the model's lane, which then forks after the JPEG decode / rectify ops or at the call's
+ * start).  So one engine gives each network the input its reference deployment gives it: the ROS2 scene nodes the
+ * whole frame in VPB_CONV_BGR_NOSWAP, the production EgoLanes engine rows >= 420 in VPB_CONV_BGR_SWAP.  A view does not
+ * read the vp_engine_set_roi region.  The model's raw tensor, class map and taps (with "<model_idx>/pre", its network
+ * input), its source outputs (at the view's size; the overlay blends the view's region), the in-call lateral op's
+ * image size when it is the lateral's model, and vp_engine_read_resized_view follow the view; the other models and an
+ * attached detector read what they read without it.  v NULL: the model reads the engine's input again.  Setting or
+ * clearing a view captures the frame graph again; a moved region re-points it, a resized one captures it again.
+ * VPB_ERR_ARG, before anything changes, for a NULL engine, a model out of range, a region with x or y < 0 or w, h <= 0
+ * other than the whole-frame pair 0, 0, an unknown convention, a convention whose input channel order (R, G, B for
+ * VPB_CONV_RGB / _RGB_UNIT, B, G, R for the BGR conventions) differs from the engine's (decoded and rectified frames
+ * are written in the engine's order), or a model whose encoder another model of the engine shares.  A call checks
+ * every view's regions as vp_engine_set_roi's (inside the frame, the frame checks of the cropped frame, an even x and y
+ * on an unrectified YUV or Bayer frame) before any device work.  The split-fp16 engine (batch 1) takes views too. */
+typedef struct {
+  int convention;                   /* VPB_CONV_*, or -1: the engine's vp_engine_config.convention */
+  int roi[VP_MAX_BATCH][4];         /* x, y, w, h of sample k's frame; w = h = 0: the whole frame */
+} vp_view;
+int vp_engine_set_view(vp_engine* e, int model_idx, const vp_view* v);
+/* The 640x320 uint8 image model model_idx's pre-process produced for sample `sample` of the last call: its view's
+ * (vp_engine_set_view), or the engine's (vp_engine_read_resized_at) for a model without one. */
+int vp_engine_read_resized_view(vp_engine* e, int model_idx, int sample, uint8_t* dst);
+
 /* The AutoSpeed detector (vp_b200_autospeed.h) inside every later call of every form: "det/letterbox" (its Pillow-
  * bilinear letterbox of each sample's whole decoded and rectified frame, never the region) and copies of its network,
  * decode and NMS ops ("det/<name>") on a lane of their own, which forks after the JPEG decode / rectify ops (at the

@@ -76,14 +76,24 @@ void std_table(int cls, int slot, HuffSpec& t) {
   t.set = true;
 }
 
-// canonical codes of t fit their lengths (libjpeg's "Bogus Huffman table definition" otherwise)
-bool table_ok(const HuffSpec& t) {
+// jpeg_make_d_derived_tbl (jdhuff.c), which libjpeg runs on the tables a scan uses: the canonical codes fit their
+// lengths with no code of all ones, and a DC table's symbols are categories 0..15.  true, or false with why set.
+bool table_ok(const HuffSpec& t, int cls, int th, char* why, size_t n) {
   long code = 0;
   for (int l = 1; l <= 16; ++l) {
     code += t.bits[l - 1];
-    if (code > (1L << l)) return false;
+    if (code >= (1L << l)) {
+      snprintf(why, n, "Huffman table %d of class %d has more codes of up to %d bits than fit without an all-ones code",
+               th, cls, l);
+      return false;
+    }
     code <<= 1;
   }
+  for (int i = 0; cls == 0 && i < t.count; ++i)
+    if (t.vals[i] > 15) {
+      snprintf(why, n, "DC Huffman table %d has symbol %d (DC categories are 0..15)", th, t.vals[i]);
+      return false;
+    }
   return true;
 }
 }  // namespace
@@ -110,7 +120,7 @@ static bool parse_jpeg(const uint8_t* b, size_t n, JpegInfo& J) {
   for (auto& c : ht) for (auto& t : c) t.set = false;
   bool qset[4] = {false, false, false, false};
   uint8_t qt[4][64];
-  bool sof = false;
+  bool sof = false, jfif = false;
   int adobe = -1, comp_id[3] = {0, 0, 0}, comp_tq[3] = {0, 0, 0}, samp[3][2] = {};
   size_t pos = 2;
   for (;;) {
@@ -162,12 +172,13 @@ static bool parse_jpeg(const uint8_t* b, size_t n, JpegInfo& J) {
         memcpy(t.vals, b + p + 17, cnt);
         t.count = cnt;
         t.set = true;
-        if (!table_ok(t)) return fail("Huffman table %d of class %d is not a prefix code", th, tc);
         p += 17 + cnt;
       }
     } else if (m == 0xDD) {
       if (seg != 4) return fail("DRI segment is malformed");
       J.ri = (b[p] << 8) | b[p + 1];
+    } else if (m == 0xE0) {
+      if (seg >= 16 && memcmp(b + p, "JFIF", 5) == 0) jfif = true;
     } else if (m == 0xEE) {
       if (seg >= 14 && memcmp(b + p, "Adobe", 5) == 0) adobe = b[p + 11];
     } else if (m == 0xDA) {
@@ -176,7 +187,11 @@ static bool parse_jpeg(const uint8_t* b, size_t n, JpegInfo& J) {
       if (ns != 3 || seg != 6 + 2 * static_cast<size_t>(ns))
         return fail("a scan of %d component(s); only one interleaved scan of 3 is taken", ns);
       if (b[p + 7] != 0 || b[p + 8] != 63 || b[p + 9] != 0) return fail("scan is not sequential (Ss 0, Se 63, Ah Al 0)");
-      if (adobe >= 0 && adobe != 1) return fail("Adobe colour transform %d (RGB or YCCK); only YCbCr is taken", adobe);
+      // libjpeg's colour space of three components (default_decompress_parms): JFIF means YCbCr, then an Adobe
+      // transform decides (0 RGB, anything else YCbCr), then the ids ('R', 'G', 'B' RGB, anything else YCbCr)
+      if (!jfif && adobe == 0) return fail("RGB colour space (Adobe transform 0); only YCbCr is taken");
+      if (!jfif && adobe < 0 && comp_id[0] == 'R' && comp_id[1] == 'G' && comp_id[2] == 'B')
+        return fail("RGB colour space (component ids R, G, B); only YCbCr is taken");
       if (J.h == 0 || J.w == 0) return fail("image size 0 in the SOF");
       if (J.h > 2400 || J.w > 4800)
         return fail("a %dx%d image is larger than the pre-process takes (4800x2400)", J.w, J.h);
@@ -198,6 +213,7 @@ static bool parse_jpeg(const uint8_t* b, size_t n, JpegInfo& J) {
           if (ht[cls][th].set) dst = ht[cls][th];
           else if (th < 2) std_table(cls, th, dst);
           else return fail("Huffman table %d is missing", th);
+          if (!table_ok(dst, cls, th, J.why, sizeof(J.why))) return false;
         }
       }
       J.data = end;

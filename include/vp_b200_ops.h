@@ -75,13 +75,18 @@ typedef struct { const uint8_t* data; int h, w, stride; } vpb_frame;
  *         submit the caller keeps the bytes alive until sync); every device call rejects it.  Decoded on the device
  *         byte-equal to cv::imdecode(buf, IMREAD_COLOR | IMREAD_IGNORE_ORIENTATION) (libjpeg-turbo: ISLOW IDCT, fancy
  *         upsampling), to R, G, B for VPB_CONV_RGB / _RGB_UNIT and B, G, R for the BGR conventions.  Streams taken:
- *         baseline or extended sequential (SOF0 / SOF1) Huffman, 8-bit, one interleaved scan of 3 YCbCr components
- *         (JFIF, or Adobe transform 1), luma sampling 1x1, 2x1 or 2x2 over 1x1 chroma (4:4:4, 4:2:2, 4:2:0), optional
- *         DRI / RSTn, missing Huffman tables replaced by the Annex K ones (MJPEG), APPn (EXIF orientation too) ignored,
- *         at most 4800x2400.  Anything else (progressive, lossless, arithmetic, 12-bit, multi-scan, 1 or 4 components,
- *         Adobe RGB / YCCK, other sampling, a missing SOI / SOF / SOS or a segment past `stride`, an h x w other than the
- *         SOF's) is VPB_ERR_ARG before any device work, naming the call, the frame and the reason: cv::imdecode and the
- *         packed call are the fall-back.  Corrupt entropy-coded data decodes to unspecified pixels of that frame only.
+ *         baseline or extended sequential (SOF0 / SOF1) Huffman, 8-bit, one interleaved scan of 3 components that
+ *         libjpeg reads as YCbCr (a JFIF APP0; else an Adobe APP14 transform other than 0; else any component ids but
+ *         'R', 'G', 'B'), luma sampling 1x1, 2x1 or 2x2 over 1x1 chroma (4:4:4, 4:2:2, 4:2:0), optional DRI / RSTn,
+ *         missing Huffman tables replaced by the Annex K ones (MJPEG), APPn (EXIF orientation too) ignored, at most
+ *         4800x2400.  Anything else (progressive, lossless, arithmetic, 12-bit, multi-scan, 1 or 4 components, an RGB
+ *         colour space by those rules, a Huffman table of the scan that libjpeg rejects (a code of all ones, a DC symbol
+ *         above 15), other sampling, a missing SOI / SOF / SOS or a segment past `stride`, an h x w other than the SOF's)
+ *         is VPB_ERR_ARG before any device work, naming the call, the frame and the reason: cv::imdecode and the packed
+ *         call are the fall-back.  Byte-equality holds while every IDCT output sample stays within the range limit's
+ *         [-512, 511] around 128 (any stream an 8-bit image encodes to): past it jidctint.c's table wraps while
+ *         libjpeg-turbo's SIMD IDCT saturates, so cv::imdecode itself depends on the CPU.  Corrupt entropy-coded data
+ *         decodes to unspecified pixels of that frame only.
  * Value 4 is unassigned: it was rejected as an unknown format before the 4-channel and Bayer layouts existed, and it
  * still is (the new values start at 5). */
 enum { VPB_PIX_PACKED = 0, /* a vpb_frame: 3 interleaved channels, RGB or BGR as the convention says */

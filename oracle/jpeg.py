@@ -44,7 +44,7 @@ def parse(buf) -> dict:
     n = len(b)
     if n < 4 or b[0] != 0xFF or b[1] != 0xD8:
         raise JpegError("no SOI marker")
-    pos, qt, ht, ri, sof, adobe = 2, {}, {}, 0, None, None
+    pos, qt, ht, ri, sof, adobe, jfif = 2, {}, {}, 0, None, None, False
     while True:
         while pos < n and b[pos] == 0xFF and pos + 1 < n and b[pos + 1] == 0xFF:
             pos += 1                                     # fill bytes
@@ -95,6 +95,9 @@ def parse(buf) -> dict:
             if seg != 4:
                 raise JpegError("DRI segment is malformed")
             ri = (b[p] << 8) | b[p + 1]
+        elif m == 0xE0:
+            if seg >= 16 and b[p:p + 5] == b"JFIF\0":
+                jfif = True
         elif m == 0xEE:
             if seg >= 14 and b[p:p + 5] == b"Adobe":
                 adobe = b[p + 11]
@@ -108,14 +111,40 @@ def parse(buf) -> dict:
             ss, se, ahal = b[p + 7], b[p + 8], b[p + 9]
             if ss != 0 or se != 63 or ahal != 0:
                 raise JpegError("scan is not sequential (Ss 0, Se 63, Ah Al 0)")
-            return _finish(sof, sel, qt, ht, ri, adobe, end)
+            return _finish(sof, sel, qt, ht, ri, jfif, adobe, end)
         pos = end
 
 
-def _finish(sof, sel, qt, ht, ri, adobe, data):
+def table_fault(bits, vals, cls, slot):
+    """why libjpeg's jpeg_make_d_derived_tbl rejects a table a scan uses ("Bogus Huffman table definition"), or None:
+    more codes than fit their lengths without a code of all ones, or a DC symbol above 15"""
+    code = 0
+    for L in range(1, 17):
+        code += bits[L - 1]
+        if code >= 1 << L:
+            return (f"Huffman table {slot} of class {cls} has more codes of up to {L} bits than fit without an all-ones "
+                    "code")
+        code <<= 1
+    bad = [v for v in vals if v > 15] if cls == 0 else []
+    return f"DC Huffman table {slot} has symbol {bad[0]} (DC categories are 0..15)" if bad else None
+
+
+def colour_space(jfif, adobe, ids):
+    """"YCbCr" or "RGB": libjpeg-turbo's guess for three components (jdapimin.c default_decompress_parms): a JFIF APP0
+    means YCbCr; otherwise an Adobe APP14 transform decides (0 RGB, 1 YCbCr, anything else YCbCr with a warning);
+    otherwise the component ids ('R', 'G', 'B' RGB, anything else YCbCr)"""
+    if jfif:
+        return "YCbCr"
+    if adobe is not None:
+        return "RGB" if adobe == 0 else "YCbCr"
+    return "RGB" if list(ids) == [82, 71, 66] else "YCbCr"
+
+
+def _finish(sof, sel, qt, ht, ri, jfif, adobe, data):
     h, w, comps = sof
-    if adobe is not None and adobe != 1:
-        raise JpegError(f"Adobe colour transform {adobe} (RGB or YCCK); only YCbCr is taken")
+    if colour_space(jfif, adobe, [c[0] for c in comps]) == "RGB":
+        why = "Adobe transform 0" if not jfif and adobe == 0 else "component ids R, G, B"
+        raise JpegError(f"RGB colour space ({why}); only YCbCr is taken")
     if h == 0 or w == 0:
         raise JpegError("image size 0 in the SOF")
     if h > MAX_H or w > MAX_W:
@@ -136,8 +165,12 @@ def _finish(sof, sel, qt, ht, ri, adobe, data):
             t = ht.get((tc, th)) or STD_TABLES.get((tc, th))
             if t is None:
                 raise JpegError(f"Huffman table {th} is missing")
+            why = table_fault(*t, tc, th)
+            if why:
+                raise JpegError(why)
             lst.append(t)
-    return dict(h=h, w=w, sampling=SAMPLING[samp], hs=samp[0], vs=samp[1], q=q, dc=dc, ac=ac, ri=ri, data=data)
+    return dict(h=h, w=w, sampling=SAMPLING[samp], hs=samp[0], vs=samp[1], q=q, dc=dc, ac=ac, ri=ri, data=data,
+                ids=ids, slots=[(c[3], s[1], s[2]) for c, s in zip(comps, sel)], qt=qt, ht=ht)
 
 
 def destuff(buf, start: int):
@@ -183,9 +216,10 @@ def _lut(bits, vals):
     return ln, sym
 
 
-def huffman(info: dict, buf) -> np.ndarray:
+def huffman(info: dict, buf, trace=None) -> np.ndarray:
     """Coefficients int64 [blocks][64] (zig-zag order, DC as decoded differences) in MCU order, the blocks of an MCU in
-    the scan's order (hs*vs luma blocks row-major, then Cb, Cr).  Bits past the data read as 0."""
+    the scan's order (hs*vs luma blocks row-major, then Cb, Cr).  Bits past the data read as 0.  trace: a list that
+    gets (class, code length, symbol, zig-zag index before the symbol) of every code decoded."""
     data, segs = destuff(buf, info["data"])
     bpm = info["hs"] * info["vs"] + 2
     mx, my = -(-info["w"] // (8 * info["hs"])), -(-info["h"] // (8 * info["vs"]))
@@ -220,6 +254,8 @@ def huffman(info: dict, buf) -> np.ndarray:
                 L = int(dl[v])
                 s = int(ds[v]) if L else 0
                 p += L if L else 16
+                if trace is not None:
+                    trace.append((0, L, s, 0))
                 blk[0] = extend(get(p, s), s)
                 p += s
                 k = 1
@@ -228,6 +264,8 @@ def huffman(info: dict, buf) -> np.ndarray:
                     L = int(al[v])
                     rs = int(asym[v]) if L else 0
                     p += L if L else 16
+                    if trace is not None:
+                        trace.append((1, L, rs, k))
                     r, s = rs >> 4, rs & 15
                     if s:
                         k += r
@@ -374,10 +412,10 @@ def color_tables():
 _CT = color_tables()
 
 
-def decode(buf, bgr: bool = True) -> np.ndarray:
-    """uint8 [h, w, 3] in B, G, R (cv2.imdecode's order) or R, G, B"""
+def decode(buf, bgr: bool = True, trace=None) -> np.ndarray:
+    """uint8 [h, w, 3] in B, G, R (cv2.imdecode's order) or R, G, B; trace as huffman() takes it"""
     info = parse(buf)
-    coef = dc_values(info, huffman(info, buf))
+    coef = dc_values(info, huffman(info, buf, trace))
     y, cb, cr = planes(info, coef)
     h, w = info["h"], info["w"]
     Y = y[:h, :w].astype(np.int64)
@@ -403,3 +441,124 @@ def strip_dht(buf) -> bytes:
             out += b[pos:]
             break
     return bytes(out)
+
+
+# ------------------------------------------------------------------------------------------------ writer
+JFIF_APP0 = b"\xff\xe0\x00\x10JFIF\x00\x01\x01\x00\x00\x01\x00\x01\x00\x00"    # what libjpeg writes
+
+
+def huff_table(lengths, cls: int) -> tuple:
+    """(bits, vals) of the canonical Huffman table giving each symbol of `lengths` (symbol, code length) pairs a code of
+    that length; symbols of one length take codes in the order given.  ValueError for a table libjpeg would reject
+    (table_fault) or could not hold: lengths outside 1..16, a symbol twice or outside 0..255, more than 256 symbols."""
+    lengths = list(lengths)
+    syms = [s for s, _ in lengths]
+    if len(set(syms)) != len(syms) or len(syms) > 256 or any(not 0 <= s <= 255 for s in syms):
+        raise ValueError("a symbol twice, outside 0..255 or more than 256 symbols")
+    if any(not 1 <= L <= 16 for _, L in lengths):
+        raise ValueError("code lengths are 1..16")
+    bits = [sum(1 for _, L in lengths if L == n) for n in range(1, 17)]
+    vals = bytes(s for n in range(1, 17) for s, L in lengths if L == n)
+    why = table_fault(bits, vals, cls, 0)
+    if why:
+        raise ValueError(why)
+    return bits, vals
+
+
+def _codes(bits, vals):
+    """symbol -> (code, length) of a table"""
+    out, code, k = {}, 0, 0
+    for L in range(1, 17):
+        for _ in range(bits[L - 1]):
+            out.setdefault(vals[k], (code, L))
+            code += 1
+            k += 1
+        code <<= 1
+    return out
+
+
+def _segment(marker: int, payload: bytes, fill: int) -> bytes:
+    return b"\xff" * fill + bytes([0xFF, marker]) + (len(payload) + 2).to_bytes(2, "big") + payload
+
+
+def write(coef, h, w, sampling, qt, ht, slots=((0, 0, 0), (1, 1, 1), (1, 1, 1)), ids=(1, 2, 3), ri=0,
+          app=(JFIF_APP0,), merged=False, fill=0, sof=0xC0, zrl_end=False) -> bytes:
+    """A sequential Huffman JPEG stream of quantised coefficients as huffman() returns them ([blocks][64], zig-zag
+    order, DC as differences, MCU order), laid out as libjpeg writes one: SOI, `app` (whole segments, e.g. APPn or COM),
+    DQT, SOF, DHT, DRI, SOS, the entropy-coded data (1-padded to a byte at each RSTn and the end, 0xFF stuffed), EOI.
+    qt {slot: 64 zig-zag entries} and ht {(class, slot): (bits, vals)} are written in their order, one table per
+    segment or, merged, all in one DQT and one DHT; a slot the scan uses that ht leaves out is coded with its Annex K
+    table (STD_TABLES) and written nowhere, as in an MJPEG frame.  slots: (quantisation, DC, AC) slot of each component.
+    fill: 0xFF fill bytes before every marker after SOI.  sof: 0xC0 baseline or 0xC1 extended sequential.  zrl_end:
+    code each block's trailing zeros as ZRLs instead of an EOB (a ZRL then runs to or past z = 63)."""
+    hs, vs = {"444": (1, 1), "422": (2, 1), "420": (2, 2)}[sampling]
+    bpm = hs * vs + 2
+    mcus = -(-w // (8 * hs)) * -(-h // (8 * vs))
+    coef = np.asarray(coef, np.int64)
+    assert coef.shape == (mcus * bpm, 64), (coef.shape, mcus * bpm)
+    out = bytearray(b"\xff\xd8")
+    for a in app:
+        out += b"\xff" * fill + a
+    dqt = [bytes([t]) + bytes(int(v) for v in q) for t, q in qt.items()]
+    dht = [bytes([16 * c + t]) + bytes(bits) + bytes(vals) for (c, t), (bits, vals) in ht.items()]
+    for seg in ([b"".join(dqt)] if merged else dqt):
+        out += _segment(0xDB, seg, fill)
+    out += _segment(sof, bytes([8]) + h.to_bytes(2, "big") + w.to_bytes(2, "big") + bytes([3]) +
+                    b"".join(bytes([i, 16 * f[0] + f[1], s[0]]) for i, s, f in zip(ids, slots, ((hs, vs), (1, 1), (1, 1)))),
+                    fill)
+    for seg in ([b"".join(dht)] if merged and dht else dht):
+        out += _segment(0xC4, seg, fill)
+    if ri:
+        out += _segment(0xDD, ri.to_bytes(2, "big"), fill)
+    out += _segment(0xDA, bytes([3]) + b"".join(bytes([i, 16 * s[1] + s[2]]) for i, s in zip(ids, slots)) +
+                    bytes([0, 63, 0]), fill)
+    tables = {key: _codes(*(ht.get(key) or STD_TABLES[key])) for key in
+              {(c, s[1 + c]) for s in slots for c in (0, 1)}}
+    comp = [0] * (bpm - 2) + [1, 2]
+    acc, nacc, rst = 0, 0, 0
+
+    def put(code, n):
+        nonlocal acc, nacc
+        acc, nacc = (acc << n) | code, nacc + n
+        while nacc >= 8:
+            nacc -= 8
+            byte = (acc >> nacc) & 255
+            out.append(byte)
+            if byte == 0xFF:
+                out.append(0)
+        acc &= (1 << nacc) - 1
+
+    def flush():
+        if nacc:
+            put((1 << (8 - nacc)) - 1, 8 - nacc)
+
+    for m in range(mcus):
+        if ri and m and m % ri == 0:
+            flush()
+            out += b"\xff" * fill + bytes([0xFF, 0xD0 + rst])
+            rst = (rst + 1) & 7
+        for c in range(bpm):
+            dc_t, ac_t = (tables[(0, slots[comp[c]][1])], tables[(1, slots[comp[c]][2])])
+            blk = coef[m * bpm + c].tolist()
+            for k, v in enumerate(blk):
+                s = abs(v).bit_length()
+                if k == 0:
+                    put(*dc_t[s])
+                elif v == 0:
+                    run += 1
+                    continue
+                else:
+                    while run > 15:
+                        put(*ac_t[0xF0])
+                        run -= 16
+                    put(*ac_t[(run << 4) | s])
+                if s:
+                    put(v if v > 0 else v + (1 << s) - 1, s)
+                run = 0
+            if run and zrl_end:
+                for _ in range(-(-run // 16)):
+                    put(*ac_t[0xF0])
+            elif run:
+                put(*ac_t[0x00])
+    flush()
+    return bytes(out + b"\xff" * fill + b"\xff\xd9")

@@ -130,7 +130,22 @@ def rejected_streams():
     bad_samp[s + 11] = 0x41                              # luma 4x1
     big = bytearray(base)
     big[s + 5:s + 7] = (2401).to_bytes(2, "big")
+    info = J.parse(base)
+    coef = J.huffman(info, base)
+    bits, vals = info["ht"][(0, 0)]
+    full = list(bits)
+    full[8] += 1                                         # one more 9-bit DC code: the last code is all ones
+
+    def rewrite(ht=info["ht"], ids=(1, 2, 3), app=(J.JFIF_APP0,)):
+        return J.write(coef, 40, 64, "420", info["qt"], ht, info["slots"], ids, app=app)
     return {
+        "all-ones code": (rewrite({**info["ht"], (0, 0): (full, bytes(vals) + b"\x0b")}),
+                          "Huffman table 0 of class 0 has more codes of up to 9 bits than fit"),
+        "DC symbol 27": (rewrite({**info["ht"], (0, 0): (bits, bytes(vals[:-1]) + b"\x1b")}),
+                         "DC Huffman table 0 has symbol 27"),
+        "RGB by Adobe": (rewrite(app=(b"\xff\xee\x00\x0eAdobe\x00\x64\x00\x00\x00\x00\x00",)),
+                         "RGB colour space (Adobe transform 0)"),
+        "RGB by ids": (rewrite(ids=(82, 71, 66), app=()), "RGB colour space (component ids R, G, B)"),
         "progressive": (encode(img, 75, "420", cv2.IMWRITE_JPEG_PROGRESSIVE, 1), "progressive stream"),
         "grayscale": (cv2.imencode(".jpg", img[:, :, 0])[1].tobytes(), "1 component(s)"),
         "sampling": (bytes(bad_samp), "sampling 4x1,1x1,1x1"),

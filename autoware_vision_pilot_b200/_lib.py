@@ -204,11 +204,9 @@ class JPEG:
             raise ValueError("JPEG: bytes or a 1-D uint8 array expected")
         self.data = np.ascontiguousarray(data)
         h, w, s = C.c_int(), C.c_int(), C.c_int()
-        lib_ = lib()
-        lib_.vpb_jpeg_info.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                       C.POINTER(C.c_int)]
-        check(lib_.vpb_jpeg_info(self.data.ctypes.data, self.data.size, C.byref(h), C.byref(w), C.byref(s)),
-              "vpb_jpeg_info")
+        # the stream as a c_char_p, which the table's c_void_p takes as well as a caller's c_char_p declaration
+        data = self.data.ctypes.data_as(C.c_char_p)
+        check(lib().vpb_jpeg_info(data, self.data.size, C.byref(h), C.byref(w), C.byref(s)), "vpb_jpeg_info")
         self.h, self.w, self.sampling = h.value, w.value, JPEG_SAMPLING[s.value]
 
     def desc(self, allow_copy: bool = True):
@@ -223,14 +221,9 @@ class JpegDecoder:
     """The op-level decoder (vpb_jpeg_decoder_create): up to n frames of up to h x w per decode() call on one GPU."""
 
     def __init__(self, max_h: int, max_w: int, max_n: int = 1, gpu_id: int = 0):
-        lib_ = lib()
-        lib_.vpb_jpeg_decoder_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
-        lib_.vpb_jpeg_decoder_destroy.argtypes = [C.c_void_p]
-        lib_.vpb_jpeg_decoder_destroy.restype = None
-        lib_.vpb_jpeg_decode.argtypes = [C.c_void_p, C.POINTER(FrameFmt), C.c_int, C.c_int, C.POINTER(C.c_void_p),
-                                         C.c_void_p]
-        self._lib, self._h = lib_, C.c_void_p()
-        check(lib_.vpb_jpeg_decoder_create(max_h, max_w, max_n, gpu_id, C.byref(self._h)), "vpb_jpeg_decoder_create")
+        self._lib, self._h = lib(), C.c_void_p()
+        check(self._lib.vpb_jpeg_decoder_create(max_h, max_w, max_n, gpu_id, C.byref(self._h)),
+              "vpb_jpeg_decoder_create")
 
     def decode(self, frames, out_ptrs, bgr: bool = True, stream: int = 0) -> None:
         """JPEG objects -> device packed frames at out_ptrs (asynchronous on `stream`)"""
@@ -262,17 +255,12 @@ class Rectify:
             raise ValueError(f"Rectify: map1 must be int16 [h, w, 2], got {map1.dtype} {map1.shape}")
         if map2.dtype != np.uint16 or map2.shape != map1.shape[:2]:
             raise ValueError(f"Rectify: map2 must be uint16 {map1.shape[:2]}, got {map2.dtype} {map2.shape}")
-        lib_ = lib()
-        lib_.vpb_rectify_create.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                            C.POINTER(C.c_void_p)]
-        lib_.vpb_rectify_destroy.argtypes = [C.c_void_p]
-        lib_.vpb_rectify_destroy.restype = None
-        self._lib, self._h = lib_, C.c_void_p()
+        self._lib, self._h = lib(), C.c_void_p()
         self.h, self.w = map1.shape[:2]
         self.src_h, self.src_w = (int(v) for v in src_size)
         self.gpu_id = gpu_id
-        check(lib_.vpb_rectify_create(map1.ctypes.data, map2.ctypes.data, self.h, self.w, self.src_h, self.src_w,
-                                      gpu_id, C.byref(self._h)), "vpb_rectify_create")
+        check(self._lib.vpb_rectify_create(map1.ctypes.data, map2.ctypes.data, self.h, self.w, self.src_h,
+                                           self.src_w, gpu_id, C.byref(self._h)), "vpb_rectify_create")
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -349,21 +337,231 @@ class LateralOut(C.Structure):
                 ("pf_meas", (C.c_double * 2) * 14)]
 
 
+MAX_BATCH = 8   # VP_MAX_BATCH
+
+
+class EngineConfig(C.Structure):
+    """Mirror of vp_engine_config (include/vp_b200.h)."""
+
+    _fields_ = [("gpu_id", C.c_int), ("dtype", C.c_int), ("resize_mode", C.c_int), ("convention", C.c_int),
+                ("n_models", C.c_int), ("kinds", C.c_int * 4), ("weights", C.c_char_p * 4),
+                ("fetch_raw", C.c_int), ("use_graph", C.c_int), ("stream", C.c_void_p),
+                ("single_stream", C.c_int), ("precision", C.c_int), ("batch", C.c_int), ("source_outputs", C.c_int)]
+
+
+class Output(C.Structure):
+    """Mirror of vp_output (include/vp_b200.h)."""
+
+    _fields_ = [("kind", C.c_int), ("channels", C.c_int), ("height", C.c_int), ("width", C.c_int),
+                ("raw_host", C.POINTER(C.c_float)), ("cls_host", C.POINTER(C.c_uint8)),
+                ("raw_dev", C.c_void_p), ("cls_dev", C.c_void_p)]
+
+
+class SourceOutput(C.Structure):
+    """Mirror of vp_source_output (include/vp_b200.h)."""
+
+    _fields_ = [("kind", C.c_int), ("height", C.c_int), ("width", C.c_int), ("channels", C.c_int), ("pitch", C.c_int),
+                ("is_f32", C.c_int), ("host", C.c_void_p), ("dev", C.c_void_p)]
+
+
+class EngineStats(C.Structure):
+    """Mirror of vp_engine_stats (include/vp_b200.h)."""
+
+    _fields_ = [("n_launches", C.c_int), ("n_gemm_launches", C.c_int), ("gemm_flops", C.c_double),
+                ("total_flops", C.c_double), ("weight_bytes", C.c_size_t), ("act_bytes", C.c_size_t),
+                ("shared_encoders", C.c_int), ("shared_trunks", C.c_int), ("reference_flops", C.c_double)]
+
+
+class LateralConfig(C.Structure):
+    """Mirror of vp_lateral_config (include/vp_b200.h)."""
+
+    _fields_ = [("threshold", C.c_float), ("smoothing", C.c_float), ("homographies", C.POINTER(C.c_double))]
+
+
+class View(C.Structure):
+    """Mirror of vp_view (include/vp_b200.h)."""
+
+    _fields_ = [("convention", C.c_int), ("roi", (C.c_int * 4) * MAX_BATCH)]
+
+
+class TapView(C.Structure):
+    """Mirror of vp_tap_view (include/vp_b200.h)."""
+
+    _fields_ = [("data", C.c_void_p), ("height", C.c_int), ("width", C.c_int), ("channels", C.c_int),
+                ("ld", C.c_int), ("pad", C.c_int), ("dtype", C.c_int)]
+
+
+class MulticamView(C.Structure):
+    """Mirror of vp_multicam_view (include/vp_b200_multicam.h)."""
+
+    _fields_ = [("world", C.c_int), ("rank", C.c_int), ("payload_bytes", C.c_size_t),
+                ("gathered_dev", C.c_void_p), ("state_dev", C.c_void_p)]
+
+
+# The C-ABI of include/vp_b200*.h as ctypes sees it: name -> (restype, argtypes), every function in header order except
+# the variadic vpb_set_error.  lib() applies it once, so every caller gets the same signature.  Data pointers (device or
+# host, out-parameters, arrays of pointers) are c_void_p, which takes an address, a ctypes array, a pointer or byref();
+# a host struct is POINTER(its mirror); a C string is c_char_p.  tests/test_cabi_cpu.py checks it against the headers.
+vp, s, i, f, d, sz, P = C.c_void_p, C.c_char_p, C.c_int, C.c_float, C.c_double, C.c_size_t, C.POINTER
+SIGNATURES = {
+    # include/vp_b200.h
+    "vp_last_error": (s, []),
+    "vp_engine_create": (i, [P(EngineConfig), vp]),
+    "vp_engine_destroy": (None, [vp]),
+    "vp_engine_infer": (i, [vp, vp, i, i, i]),
+    "vp_engine_submit": (i, [vp, vp, i, i, i]),
+    "vp_engine_infer_device": (i, [vp, vp, i, i, i]),
+    "vp_engine_sync": (i, [vp]),
+    "vp_engine_infer_batch": (i, [vp, vp, i, i, i, i]),
+    "vp_engine_submit_batch": (i, [vp, vp, i, i, i, i]),
+    "vp_engine_infer_device_batch": (i, [vp, vp, i, i, i, i]),
+    "vp_engine_infer_frames": (i, [vp, P(Frame), i]),
+    "vp_engine_submit_frames": (i, [vp, P(Frame), i]),
+    "vp_engine_infer_device_frames": (i, [vp, P(Frame), i]),
+    "vp_engine_infer_frames_fmt": (i, [vp, P(FrameFmt), i]),
+    "vp_engine_submit_frames_fmt": (i, [vp, P(FrameFmt), i]),
+    "vp_engine_infer_device_frames_fmt": (i, [vp, P(FrameFmt), i]),
+    "vp_engine_set_rectify": (i, [vp, i, vp]),
+    "vp_engine_set_roi": (i, [vp, i, i, i, i, i]),
+    "vp_engine_set_view": (i, [vp, i, P(View)]),
+    "vp_engine_read_resized_view": (i, [vp, i, i, vp]),
+    "vp_engine_set_detector": (i, [vp, vp]),
+    "vp_engine_set_lateral": (i, [vp, i, P(LateralConfig)]),
+    "vp_engine_set_steering": (i, [vp, vp]),
+    "vp_engine_lateral_reset": (i, [vp, i]),
+    "vp_engine_lateral": (i, [vp, i, vp, vp]),
+    "vp_engine_fetch_raw": (i, [vp, i]),
+    "vp_engine_output": (i, [vp, i, P(Output)]),
+    "vp_engine_output_at": (i, [vp, i, i, P(Output)]),
+    "vp_engine_num_models": (i, [vp]),
+    "vp_engine_source_output": (i, [vp, i, i, i, P(SourceOutput)]),
+    "vp_engine_pinned_frame": (vp, [vp, sz]),
+    "vp_engine_get_stats": (i, [vp, P(EngineStats)]),
+    "vp_engine_profile": (i, [vp, i, vp, vp, vp, vp, vp]),
+    "vp_engine_conv_args": (i, [vp, i, P(ConvArgs), vp]),
+    "vp_engine_time_kind": (i, [vp, i, i, vp, vp, vp]),
+    "vp_engine_kernel_names": (i, [vp, vp, i, vp]),
+    "vp_engine_time_kernel": (i, [vp, s, i, vp, vp, vp, vp]),
+    "vp_engine_graph_captures": (i, [vp]),
+    "vp_engine_read_tap": (C.c_long, [vp, s, vp, C.c_long, vp, vp, vp]),
+    "vp_engine_tap_dev": (i, [vp, s, P(TapView)]),
+    "vp_engine_stream": (vp, [vp]),
+    "vp_engine_read_resized": (i, [vp, vp]),
+    "vp_engine_read_resized_at": (i, [vp, i, vp]),
+    # include/vp_b200_ops.h
+    "vpb_last_error": (s, []),
+    "vpb_conv_gemm": (i, [P(ConvArgs), vp]),
+    "vpb_final_tapsum": (i, [vp, vp, i, i, i, i, vp, vp, i, vp]),
+    "vpb_final_conv_weights_host": (i, [vp, i, i, vp]),
+    "vpb_upconv_compose": (i, [vp, vp, vp, vp, vp, vp, i, i, i, i, vp, vp, vp, vp]),
+    "vpb_f32_to_16": (i, [i, vp, vp, C.c_longlong, vp]),
+    "vpb_preprocess": (i, [vp, i, i, i, i, i, i, vp, vp, vp]),
+    "vpb_preprocess_fmt": (i, [P(FrameFmt), i, i, i, vp, vp, vp]),
+    "vpb_rectify_create": (i, [vp, vp, i, i, i, i, i, vp]),
+    "vpb_rectify_destroy": (None, [vp]),
+    "vpb_rectify_frames": (i, [P(FrameFmt), vp, i, i, vp, vp]),
+    "vpb_jpeg_info": (i, [vp, sz, vp, vp, vp]),
+    "vpb_jpeg_decoder_create": (i, [i, i, i, i, vp]),
+    "vpb_jpeg_decoder_destroy": (None, [vp]),
+    "vpb_jpeg_decode": (i, [vp, P(FrameFmt), i, i, vp, vp]),
+    "vpb_resize_tables_host": (i, [i, i, i, vp, vp, i, vp]),
+    "vpb_stem_conv": (i, [i, vp, i, i, vp, vp, vp, vp]),
+    "vpb_depthwise": (i, [i, vp, i, i, i, i, i, vp, vp, vp, vp, vp]),
+    "vpb_se_scale": (i, [i, vp, i, i, i, vp, vp, vp, vp, vp, vp, vp]),
+    "vpb_gap": (i, [i, vp, i, i, i, vp, vp]),
+    "vpb_linear": (i, [vp, vp, vp, i, i, i, vp, vp]),
+    "vpb_ctx_conv1": (i, [i, vp, i, i, vp, vp, i, vp, i, vp]),
+    "vpb_fuse_pool_concat": (i, [i, vp, vp, vp, vp, vp, i, i, vp, vp]),
+    "vpb_stem_conv_ex": (i, [i, vp, vp, i, i, vp, vp, vp, vp, i, vp]),
+    "vpb_depthwise_ex": (i, [i, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp, i, i, vp]),
+    "vpb_se_scale_ex": (i, [i, vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, i, vp]),
+    "vpb_gap_ex": (i, [i, vp, vp, i, i, i, vp, i, vp]),
+    "vpb_linear_ex": (i, [vp, vp, vp, i, i, i, vp, i, vp]),
+    "vpb_ctx_conv1_ex": (i, [i, vp, i, i, vp, vp, i, vp, vp, i, i, i, vp]),
+    "vpb_fuse_pool_concat_ex": (i, [i, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i, i, vp, vp, i, vp]),
+    "vpb_mask255": (i, [vp, i, i, i, vp, vp]),
+    "vpb_egolanes_ids": (i, [vp, i, i, i, vp, vp]),
+    "vpb_lane_masks": (i, [vp, i, f, vp, vp]),
+    "vpb_resize_nearest_u8": (i, [vp, i, i, vp, i, i, vp]),
+    "vpb_resize_linear_f32": (i, [vp, i, i, vp, i, i, vp]),
+    "vpb_visualize_mask": (i, [vp, i, i, i, vp, i, i, i, vp, i, vp]),
+    "vpb_source_outputs": (i, [P(SrcJob), i, vp]),
+    "vpb_polyfit": (i, [vp, vp, vp, i, i, vp, vp, vp]),
+    "vpb_bayes_fuse": (i, [vp, vp, i, vp]),
+    "vpb_lateral_init": (i, [vp, vp]),
+    "vpb_lateral_update": (i, [vp, i, i, i, i, f, vp, d, vp, vp, vp]),
+    "vpb_lateral_update_batch": (i, [vp, i, i, i, i, i, f, vp, vp, vp, vp, vp]),
+    "vpb_lateral_update_cameras": (i, [vp, i, i, i, vp, vp, f, vp, vp, vp, vp, vp]),
+    "vpb_lateral_update_logits": (i, [vp, i, i, i, f, vp, vp, f, vp, vp, vp, vp, vp]),
+    "vpb_autosteer_pack": (i, [vp, vp, vp, vp]),
+    "vpb_autosteer_decode": (i, [vp, i, vp, vp, vp]),
+    # include/vp_b200_autospeed.h
+    "vp_autospeed_create": (i, [s, i, i, vp, vp]),
+    "vp_autospeed_create_batch": (i, [s, i, i, vp, i, vp]),
+    "vp_autospeed_create_precision": (i, [s, i, i, i, vp, i, vp]),
+    "vp_autospeed_destroy": (None, [vp]),
+    "vp_autospeed_set_thresholds": (i, [vp, f, f]),
+    "vp_autospeed_infer": (i, [vp, vp, i, i, i, i]),
+    "vp_autospeed_infer_device": (i, [vp, vp, i, i, i]),
+    "vp_autospeed_infer_batch": (i, [vp, vp, i, i, i, i, i]),
+    "vp_autospeed_infer_device_batch": (i, [vp, vp, i, i, i, i]),
+    "vp_autospeed_infer_frames": (i, [vp, P(Frame), i, i]),
+    "vp_autospeed_infer_device_frames": (i, [vp, P(Frame), i]),
+    "vp_autospeed_infer_frames_fmt": (i, [vp, P(FrameFmt), i, i]),
+    "vp_autospeed_infer_device_frames_fmt": (i, [vp, P(FrameFmt), i]),
+    "vp_autospeed_set_rectify": (i, [vp, i, vp]),
+    "vp_autospeed_sync": (i, [vp, i]),
+    "vp_autospeed_detections": (i, [vp, vp, vp, vp]),
+    "vp_autospeed_raw": (i, [vp, vp, vp, vp, vp]),
+    "vp_autospeed_detections_at": (i, [vp, i, vp, vp, vp]),
+    "vp_autospeed_raw_at": (i, [vp, i, vp, vp, vp, vp]),
+    "vp_autospeed_stats": (i, [vp, vp, vp]),
+    "vp_autospeed_conv_args": (i, [vp, i, P(ConvArgs), vp]),
+    "vp_autospeed_read_tap": (C.c_long, [vp, s, vp, C.c_long, vp, vp, vp]),
+    "vpb_as_mean_blocks": (i, [i]),
+    "vpb_as_mean": (i, [i, vp, i, i, i, vp, vp, i, vp]),
+    "vpb_as_upsample2": (i, [i, vp, i, i, i, i, vp, i, i, vp]),
+    "vpb_as_maxpool5": (i, [i, vp, i, i, i, i, vp, i, vp]),
+    "vpb_as_split_v": (i, [i, vp, i, i, i, i, vp, vp, i, vp]),
+    "vpb_as_softmax_rows": (i, [i, vp, i, i, f, vp, vp]),
+    "vpb_as_decode": (i, [i, vp, i, i, i, f, i, i, vp, i, vp]),
+    "vpb_as_postprocess": (i, [vp, i, i, f, f, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "vpb_as_mean_split": (i, [vp, vp, i, i, i, vp, vp, vp]),
+    "vpb_as_maxpool5_split": (i, [vp, vp, i, i, i, i, vp, vp, vp]),
+    "vpb_as_softmax_rows_split": (i, [vp, vp, i, i, f, vp, vp, vp]),
+    "vpb_as_decode_split": (i, [vp, vp, i, i, i, f, i, i, vp, vp]),
+    # include/vp_b200_multicam.h
+    "vp_multicam_unique_id": (i, [vp]),
+    "vp_multicam_create": (i, [vp, i, i, i, vp, vp]),
+    "vp_multicam_create_with_comm": (i, [vp, i, i, i, vp, vp]),
+    "vp_multicam_create_local": (i, [i, i, vp, vp]),
+    "vp_multicam_destroy": (None, [vp]),
+    "vp_multicam_reset": (i, [vp]),
+    "vp_multicam_step": (i, [vp, vp, vp, i]),
+    "vp_multicam_step_engine": (i, [vp, vp, i, vp, i]),
+    "vp_multicam_sync": (i, [vp]),
+    "vp_multicam_get_view": (i, [vp, P(MulticamView)]),
+    "vp_multicam_read": (i, [vp, vp, vp, vp]),
+    "vp_multicam_time_allgather": (i, [vp, i, vp]),
+}
+del vp, s, i, f, d, sz, P
+
 _lib = None
 
 
 def lib() -> C.CDLL:
-    """Load (once) and return the shared library; raise loudly if it is not built."""
+    """Load (once) and return the shared library with SIGNATURES applied; raise loudly if it is not built."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing — run `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(there is no CPU or PyTorch fallback for the B200 path)")
-        _lib = C.CDLL(LIB_PATH)
-        _lib.vpb_last_error.restype = C.c_char_p
-        _lib.vpb_conv_gemm.argtypes = [C.POINTER(ConvArgs), C.c_void_p]
-        _lib.vpb_conv_gemm.restype = C.c_int
+        lib_ = C.CDLL(LIB_PATH)
+        for name, (restype, argtypes) in SIGNATURES.items():
+            fn = getattr(lib_, name)
+            fn.restype, fn.argtypes = restype, argtypes
+        _lib = lib_
     return _lib
 
 

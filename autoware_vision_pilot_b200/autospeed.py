@@ -15,7 +15,7 @@ PREC_16, PREC_SPLIT = 0, 1   # VP_PREC_*
 # dtype name -> (dtype, precision) of vp_autospeed_create_precision; "fp32" (the reference's precision="fp32") is the
 # split-fp16 fp32-grade detector
 PRECISION_BY_DTYPE = {"fp16": (L.VPB_F16, PREC_16), "bf16": (L.VPB_BF16, PREC_16), "fp32": (L.VPB_F16, PREC_SPLIT)}
-_bound = False
+_bind = L.lib   # the name this module had for it before the C-ABI declarations moved to _lib
 
 
 def precision_args(dtype: str):
@@ -23,43 +23,6 @@ def precision_args(dtype: str):
     if dtype not in PRECISION_BY_DTYPE:
         raise ValueError(f"dtype {dtype!r}: one of {sorted(PRECISION_BY_DTYPE)}")
     return PRECISION_BY_DTYPE[dtype]
-
-
-def _bind():
-    global _bound
-    lib = L.lib()
-    if _bound:
-        return lib
-    lib.vp_autospeed_create.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.vp_autospeed_create_batch.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]
-    lib.vp_autospeed_create_precision.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
-                                                  C.POINTER(C.c_void_p)]
-    lib.vp_autospeed_destroy.argtypes = [C.c_void_p]
-    lib.vp_autospeed_destroy.restype = None
-    lib.vp_autospeed_set_thresholds.argtypes = [C.c_void_p, C.c_float, C.c_float]
-    lib.vp_autospeed_infer.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.vp_autospeed_infer_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-    lib.vp_autospeed_infer_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.vp_autospeed_infer_device_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.vp_autospeed_infer_frames.argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int, C.c_int]
-    lib.vp_autospeed_infer_device_frames.argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int]
-    lib.vp_autospeed_infer_frames_fmt.argtypes = [C.c_void_p, C.POINTER(L.FrameFmt), C.c_int, C.c_int]
-    lib.vp_autospeed_infer_device_frames_fmt.argtypes = [C.c_void_p, C.POINTER(L.FrameFmt), C.c_int]
-    lib.vp_autospeed_set_rectify.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    lib.vp_autospeed_sync.argtypes = [C.c_void_p, C.c_int]
-    lib.vp_autospeed_detections.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    lib.vp_autospeed_raw.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
-                                     C.POINTER(C.c_int)]
-    lib.vp_autospeed_detections_at.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_int),
-                                               C.POINTER(C.c_int)]
-    lib.vp_autospeed_raw_at.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_void_p),
-                                        C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    lib.vp_autospeed_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_double)]
-    lib.vp_autospeed_read_tap.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long, C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                          C.POINTER(C.c_int)]
-    lib.vp_autospeed_read_tap.restype = C.c_long
-    _bound = True
-    return lib
 
 
 class AutoSpeedEngine:
@@ -70,7 +33,7 @@ class AutoSpeedEngine:
         frames of one shape (infer_batch / infer_device_batch); sample k's results are detections(k) / raw(k) /
         read_tap("<name>@k")."""
         dt, prec = precision_args(dtype)
-        self._lib = _bind()
+        self._lib = L.lib()
         self._h = C.c_void_p()
         L.check(self._lib.vp_autospeed_create_precision(weights_vpw.encode(), gpu_id, dt, prec, stream, batch,
                                                         C.byref(self._h)), "vp_autospeed_create_precision")

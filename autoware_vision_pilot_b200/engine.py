@@ -7,6 +7,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 from . import _lib as L
+from ._lib import LateralConfig, View
 
 SCENE_SEG, SCENE_3D, DOMAIN_SEG, EGO_LANES = 0, 1, 2, 3
 KIND_BY_NAME = {"scene_seg": SCENE_SEG, "scene_3d": SCENE_3D, "domain_seg": DOMAIN_SEG, "ego_lanes": EGO_LANES}
@@ -15,27 +16,12 @@ CONV_RGB, CONV_BGR_NOSWAP, CONV_BGR_SWAP, CONV_RGB_UNIT = 0, 1, 2, 3
 RESIZE_BY_NAME = {"none": RESIZE_NONE, "pil_bicubic": RESIZE_PIL_BICUBIC, "cv_linear": RESIZE_CV_LINEAR}
 DTYPE_BY_NAME = {"fp16": L.VPB_F16, "bf16": L.VPB_BF16, "fp32": L.VPB_F16}
 PREC_16, PREC_SPLIT = 0, 1
-MAX_BATCH = 8   # VP_MAX_BATCH
+MAX_BATCH = L.MAX_BATCH
 SRC_MASK, SRC_DEPTH, SRC_OVERLAY = 1, 2, 4   # VP_SRC_*
 SRC_BY_NAME = {"mask": SRC_MASK, "depth": SRC_DEPTH, "overlay": SRC_OVERLAY}
-
-
-class _Config(C.Structure):
-    _fields_ = [("gpu_id", C.c_int), ("dtype", C.c_int), ("resize_mode", C.c_int), ("convention", C.c_int),
-                ("n_models", C.c_int), ("kinds", C.c_int * 4), ("weights", C.c_char_p * 4),
-                ("fetch_raw", C.c_int), ("use_graph", C.c_int), ("stream", C.c_void_p),
-                ("single_stream", C.c_int), ("precision", C.c_int), ("batch", C.c_int), ("source_outputs", C.c_int)]
-
-
-class _Output(C.Structure):
-    _fields_ = [("kind", C.c_int), ("channels", C.c_int), ("height", C.c_int), ("width", C.c_int),
-                ("raw_host", C.POINTER(C.c_float)), ("cls_host", C.POINTER(C.c_uint8)),
-                ("raw_dev", C.c_void_p), ("cls_dev", C.c_void_p)]
-
-
-class _SourceOutput(C.Structure):
-    _fields_ = [("kind", C.c_int), ("height", C.c_int), ("width", C.c_int), ("channels", C.c_int), ("pitch", C.c_int),
-                ("is_f32", C.c_int), ("host", C.c_void_p), ("dev", C.c_void_p)]
+# The names this module had before the C-ABI declarations moved to _lib: code written against them keeps working.
+_bind = L.lib
+_Config, _Output, _SourceOutput, _Stats, _TapView = L.EngineConfig, L.Output, L.SourceOutput, L.EngineStats, L.TapView
 
 
 def source_flags(names: Sequence[str]) -> int:
@@ -48,89 +34,6 @@ def source_flags(names: Sequence[str]) -> int:
             raise ValueError(f"unknown source output {n!r} (one of {sorted(SRC_BY_NAME)})")
         flags |= SRC_BY_NAME[n]
     return flags
-
-
-class _Stats(C.Structure):
-    _fields_ = [("n_launches", C.c_int), ("n_gemm_launches", C.c_int), ("gemm_flops", C.c_double),
-                ("total_flops", C.c_double), ("weight_bytes", C.c_size_t), ("act_bytes", C.c_size_t),
-                ("shared_encoders", C.c_int), ("shared_trunks", C.c_int), ("reference_flops", C.c_double)]
-
-
-class LateralConfig(C.Structure):
-    """Mirror of vp_lateral_config (include/vp_b200.h)."""
-
-    _fields_ = [("threshold", C.c_float), ("smoothing", C.c_float), ("homographies", C.POINTER(C.c_double))]
-
-
-class View(C.Structure):
-    """Mirror of vp_view (include/vp_b200.h)."""
-
-    _fields_ = [("convention", C.c_int), ("roi", (C.c_int * 4) * MAX_BATCH)]
-
-
-class _TapView(C.Structure):
-    _fields_ = [("data", C.c_void_p), ("height", C.c_int), ("width", C.c_int), ("channels", C.c_int),
-                ("ld", C.c_int), ("pad", C.c_int), ("dtype", C.c_int)]
-
-
-_bound = False
-
-
-def _bind():
-    global _bound
-    lib = L.lib()
-    if _bound:
-        return lib
-    lib.vp_last_error.restype = C.c_char_p
-    lib.vp_engine_create.argtypes = [C.POINTER(_Config), C.POINTER(C.c_void_p)]
-    lib.vp_engine_destroy.argtypes = [C.c_void_p]
-    lib.vp_engine_destroy.restype = None
-    lib.vp_engine_infer.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-    lib.vp_engine_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-    lib.vp_engine_infer_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-    lib.vp_engine_infer_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.vp_engine_submit_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.vp_engine_infer_device_batch.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.vp_engine_output_at.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(_Output)]
-    lib.vp_engine_sync.argtypes = [C.c_void_p]
-    lib.vp_engine_fetch_raw.argtypes = [C.c_void_p, C.c_int]
-    lib.vp_engine_output.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Output)]
-    lib.vp_engine_num_models.argtypes = [C.c_void_p]
-    lib.vp_engine_pinned_frame.argtypes = [C.c_void_p, C.c_size_t]
-    lib.vp_engine_pinned_frame.restype = C.c_void_p
-    lib.vp_engine_get_stats.argtypes = [C.c_void_p, C.POINTER(_Stats)]
-    lib.vp_engine_profile.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_double),
-                                      C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    lib.vp_engine_read_tap.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long, C.POINTER(C.c_int),
-                                       C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    lib.vp_engine_read_tap.restype = C.c_long
-    lib.vp_engine_read_resized.argtypes = [C.c_void_p, C.c_void_p]
-    lib.vp_engine_read_resized_at.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    for fn in ("vp_engine_infer_frames", "vp_engine_submit_frames", "vp_engine_infer_device_frames"):
-        getattr(lib, fn).argtypes = [C.c_void_p, C.POINTER(L.Frame), C.c_int]
-    for fn in ("vp_engine_infer_frames_fmt", "vp_engine_submit_frames_fmt", "vp_engine_infer_device_frames_fmt"):
-        getattr(lib, fn).argtypes = [C.c_void_p, C.POINTER(L.FrameFmt), C.c_int]
-    lib.vp_engine_tap_dev.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(_TapView)]
-    lib.vp_engine_stream.argtypes = [C.c_void_p]
-    lib.vp_engine_stream.restype = C.c_void_p
-    lib.vp_engine_source_output.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_SourceOutput)]
-    lib.vp_engine_set_rectify.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    lib.vp_engine_time_kind.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_double),
-                                        C.POINTER(C.c_int)]
-    lib.vp_engine_kernel_names.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int)]
-    lib.vp_engine_time_kernel.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_double),
-                                          C.POINTER(C.c_double), C.POINTER(C.c_int)]
-    lib.vp_engine_set_lateral.argtypes = [C.c_void_p, C.c_int, C.POINTER(LateralConfig)]
-    lib.vp_engine_set_steering.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
-    lib.vp_engine_lateral_reset.argtypes = [C.c_void_p, C.c_int]
-    lib.vp_engine_lateral.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.vp_engine_graph_captures.argtypes = [C.c_void_p]
-    lib.vp_engine_set_roi.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.vp_engine_set_detector.argtypes = [C.c_void_p, C.c_void_p]
-    lib.vp_engine_set_view.argtypes = [C.c_void_p, C.c_int, C.POINTER(View)]
-    lib.vp_engine_read_resized_view.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
-    _bound = True
-    return lib
 
 
 class Engine:
@@ -146,8 +49,8 @@ class Engine:
         size (infer_frames / submit_frames / infer_device_frames); sample k's outputs are raw(idx, k) / cls(idx, k).
         source_outputs: any of "mask", "depth", "overlay": every call also makes these results at each camera's own
         resolution (source(idx, kind, k) / source_dev(idx, kind, k)); a kind no model makes is rejected."""
-        self._lib = _bind()
-        cfg = _Config()
+        self._lib = L.lib()
+        cfg = L.EngineConfig()
         cfg.gpu_id, cfg.dtype = gpu_id, DTYPE_BY_NAME[dtype]
         cfg.resize_mode, cfg.convention = resize_mode, convention
         cfg.n_models = len(kinds)
@@ -500,8 +403,8 @@ class Engine:
         return views
 
     # ---- outputs (views into engine-owned host buffers: copy if kept past the next infer)
-    def _out(self, idx: int, sample: int = 0) -> _Output:
-        o = _Output()
+    def _out(self, idx: int, sample: int = 0) -> L.Output:
+        o = L.Output()
         L.check(self._lib.vp_engine_output_at(self._h, idx, sample, C.byref(o)), "vp_engine_output_at")
         return o
 
@@ -519,8 +422,8 @@ class Engine:
         o = self._out(idx, sample)
         return o.raw_dev, o.cls_dev, (o.channels, o.height, o.width)
 
-    def _source(self, idx: int, kind: str, sample: int) -> _SourceOutput:
-        o = _SourceOutput()
+    def _source(self, idx: int, kind: str, sample: int) -> L.SourceOutput:
+        o = L.SourceOutput()
         L.check(self._lib.vp_engine_source_output(self._h, idx, sample, source_flags(kind), C.byref(o)),
                 "vp_engine_source_output")
         return o
@@ -546,9 +449,9 @@ class Engine:
 
     # ---- introspection
     def stats(self) -> dict:
-        s = _Stats()
+        s = L.EngineStats()
         L.check(self._lib.vp_engine_get_stats(self._h, C.byref(s)), "vp_engine_get_stats")
-        return {k: getattr(s, k) for k, _ in _Stats._fields_}
+        return {k: getattr(s, k) for k, _ in L.EngineStats._fields_}
 
     def profile(self) -> List[dict]:
         n = self.stats()["n_launches"] + 4
@@ -584,9 +487,9 @@ class Engine:
 
     def tap_dev(self, name: str) -> dict:
         """Device view of an intermediate tensor (NHWC 16-bit): {data, height, width, channels, ld, pad, dtype}."""
-        v = _TapView()
+        v = L.TapView()
         L.check(self._lib.vp_engine_tap_dev(self._h, name.encode(), C.byref(v)), "vp_engine_tap_dev")
-        return {k: getattr(v, k) for k, _ in _TapView._fields_}
+        return {k: getattr(v, k) for k, _ in L.TapView._fields_}
 
     @property
     def handle(self) -> C.c_void_p:

@@ -18,20 +18,7 @@ import torch
 from . import _lib as L
 
 MAX_CAMERAS = 8   # VP_MAX_BATCH
-
-
-def _bind():
-    lib = L.lib()
-    lib.vpb_lateral_init.argtypes = [C.c_void_p, C.c_void_p]
-    lib.vpb_lateral_update.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                       C.POINTER(C.c_double), C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.vpb_lateral_update_batch.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                             C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p, C.c_void_p,
-                                             C.c_void_p]
-    lib.vpb_lateral_update_cameras.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
-                                               C.POINTER(C.c_int), C.c_float, C.POINTER(C.c_double),
-                                               C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p]
-    return lib
+_bind = L.lib     # the name this module had for it before the C-ABI declarations moved to _lib
 
 
 def _record(raw: bytes) -> dict:
@@ -50,7 +37,7 @@ class LateralPostProcess:
 
     def __init__(self, image_size=(1920, 1080), smoothing_factor: float = 0.5,
                  homography: Optional[Sequence[float]] = None, device: str = "cuda:0"):
-        self._lib = _bind()
+        self._lib = L.lib()
         self.image_size = tuple(image_size)
         self.smoothing = float(smoothing_factor)
         self._hom = (C.c_double * 9)(*homography) if homography is not None else None
@@ -110,7 +97,7 @@ class BatchedLateralPostProcess:
         if not 1 <= cameras <= MAX_CAMERAS:
             raise ValueError(f"{cameras} cameras (1..{MAX_CAMERAS})")
         sizes = _image_sizes(cameras, image_size)
-        self._lib = _bind()
+        self._lib = L.lib()
         self.cameras = cameras
         self.image_sizes = sizes
         self._img_w = (C.c_int * cameras)(*[w for w, _ in sizes])

@@ -85,42 +85,18 @@ def all_gather_cameras(features: torch.Tensor, measurement: torch.Tensor, group=
     return torch.stack(feats), torch.stack(meas)
 
 
-class _View(C.Structure):
-    _fields_ = [("world", C.c_int), ("rank", C.c_int), ("payload_bytes", C.c_size_t),
-                ("gathered_dev", C.c_void_p), ("state_dev", C.c_void_p)]
-
-
 FEAT_BYTES = 10 * 20 * 1456 * 2
 MEAS_BYTES = STATE_DIM * 2 * 8
 PAYLOAD_BYTES = FEAT_BYTES + MEAS_BYTES
 UNIQUE_ID_BYTES = 128
-
-
-def _bind():
-    lib = L.lib()
-    if getattr(lib, "_mc_bound", False):
-        return lib
-    lib.vp_multicam_unique_id.argtypes = [C.c_void_p]
-    lib.vp_multicam_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.vp_multicam_create_local.argtypes = [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.vp_multicam_create_with_comm.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.vp_multicam_destroy.argtypes = [C.c_void_p]
-    lib.vp_multicam_destroy.restype = None
-    lib.vp_multicam_reset.argtypes = [C.c_void_p]
-    lib.vp_multicam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-    lib.vp_multicam_step_engine.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    lib.vp_multicam_sync.argtypes = [C.c_void_p]
-    lib.vp_multicam_get_view.argtypes = [C.c_void_p, C.POINTER(_View)]
-    lib.vp_multicam_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.vp_multicam_time_allgather.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float)]
-    lib._mc_bound = True
-    return lib
+# The names this module had before the C-ABI declarations moved to _lib: code written against them keeps working.
+_bind, _View = L.lib, L.MulticamView
 
 
 def make_unique_id() -> bytes:
     """ncclGetUniqueId through the C-ABI (rank 0); the host distributes the 128 bytes."""
     buf = (C.c_uint8 * UNIQUE_ID_BYTES)()
-    L.check(_bind().vp_multicam_unique_id(buf), "vp_multicam_unique_id")
+    L.check(L.lib().vp_multicam_unique_id(buf), "vp_multicam_unique_id")
     return bytes(buf)
 
 
@@ -139,7 +115,7 @@ class MultiCamera:
     """ctypes face of vp_multicam (include/vp_b200_multicam.h).  No compute in Python."""
 
     def __init__(self, unique_id: bytes, rank: int, world: int, gpu_id: int, stream: Optional[int] = None):
-        self._lib = _bind()
+        self._lib = L.lib()
         self._h = C.c_void_p()
         idb = (C.c_uint8 * UNIQUE_ID_BYTES).from_buffer_copy(unique_id)
         L.check(self._lib.vp_multicam_create(idb, rank, world, gpu_id, stream, C.byref(self._h)), "vp_multicam_create")
@@ -150,7 +126,7 @@ class MultiCamera:
         """n cameras on one GPU, no NCCL (vp_multicam_create_local): step() takes n feature maps back to back and
         [n,14,2] measurements, step_engine() an engine of batch n and the n records of a BatchedLateralPostProcess."""
         self = cls.__new__(cls)
-        self._lib = _bind()
+        self._lib = L.lib()
         self._h = C.c_void_p()
         L.check(self._lib.vp_multicam_create_local(cameras, gpu_id, stream, C.byref(self._h)), "vp_multicam_create_local")
         self.rank, self.world = 0, cameras
@@ -201,9 +177,7 @@ def fuse_measurements(state: torch.Tensor, measurements: torch.Tensor) -> torch.
     state [14,2] fp64 CUDA (updated in place and returned), measurements [n,14,2] fp64 CUDA."""
     if not (state.is_cuda and measurements.is_cuda):
         raise RuntimeError("fuse_measurements runs on the GPU only (no CPU fallback)")
-    lib = L.lib()
-    lib.vpb_bayes_fuse.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     m = measurements.contiguous()
-    L.check(lib.vpb_bayes_fuse(state.data_ptr(), m.data_ptr(), m.shape[0],
+    L.check(L.lib().vpb_bayes_fuse(state.data_ptr(), m.data_ptr(), m.shape[0],
                                torch.cuda.current_stream().cuda_stream), "vpb_bayes_fuse")
     return state

@@ -65,10 +65,6 @@ def main():
     tmp = tempfile.mkdtemp(prefix="vpb_bench_lateral_")
     ego = W.write_vpw(synth.synth_state_dict("ego_lanes"), os.path.join(tmp, "ego_lanes.vpw"))
     lib = L.lib()
-    ip, dp, vp = C.POINTER(C.c_int), C.POINTER(C.c_double), C.c_void_p
-    lib.vpb_lane_masks.argtypes = [vp, C.c_int, C.c_float, vp, vp]
-    lib.vpb_lateral_init.argtypes = [vp, vp]
-    lib.vpb_lateral_update_cameras.argtypes = [vp, C.c_int, C.c_int, C.c_int, ip, ip, C.c_float, dp, dp, vp, vp, vp]
     rec, st = C.sizeof(L.LateralOut), C.sizeof(L.LateralState)
     rows, kernel = [], []
     for name, cams in SETS.items():

@@ -18,7 +18,6 @@ Writes OUT_DIR/bench_mixed_rig.json with the card's name and power limit, read i
     python scripts/bench_mixed_rig.py OUT_DIR [--steps 100] [--rounds 3]
 """
 import argparse
-import ctypes as C
 import json
 import os
 import statistics
@@ -127,7 +126,6 @@ def main():
     seg_w = [W.write_vpw(synth.synth_state_dict(m), os.path.join(tmp, f"{m}.vpw")) for m in models]
     as_w = W.write_vpw(O.synth_state_dict(), os.path.join(tmp, "autospeed.vpw"))
     lib = L.lib()
-    lib.vpb_lane_masks.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     rows = []
     for n in [int(x) for x in args.rigs.split(",")]:
         cams = CAMERAS[n]

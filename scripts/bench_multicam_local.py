@@ -15,7 +15,6 @@ Writes OUT_DIR/bench_multicam_local.json with the card's name and power limit, r
     python scripts/bench_multicam_local.py OUT_DIR [--steps 200] [--rounds 3] [--lateral-reps 2000]
 """
 import argparse
-import ctypes as C
 import json
 import os
 import statistics
@@ -111,7 +110,6 @@ def main():
     torch.cuda.synchronize()
     H, Wd = bench.H_IN, bench.W_IN
     lib = L.lib()
-    lib.vpb_lane_masks.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
 
     rows = []
     for n in batches:

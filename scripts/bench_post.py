@@ -1,7 +1,6 @@
 """Device timings of the widened (SURVEY §8f) output-side ops: the fused mask overlay (HBM-bound) and the
 lateral post-process kernel (latency-bound).  Run on the GPU box: python scripts/bench_post.py
 Inputs are rotated over 24 frame buffers (149 MB > L2) so every overlay launch streams from HBM."""
-import ctypes as C
 import json
 import sys
 
@@ -16,8 +15,6 @@ from oracle import lateral as LT  # noqa: E402
 
 def main():
     lib = L.lib()
-    lib.vpb_visualize_mask.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                       C.c_void_p, C.c_int, C.c_void_p]
     h, w, nbuf = 1080, 1920, 24
     frames = [torch.randint(0, 256, (h, w, 3), dtype=torch.uint8, device="cuda") for _ in range(nbuf)]
     outs = [torch.empty_like(f) for f in frames]

@@ -17,7 +17,6 @@ with the card's name, power limit and SM clocks, read in the same run.
     python scripts/bench_source_outputs.py OUT_DIR [--steps 100] [--rounds 3] [--reps 200]
 """
 import argparse
-import ctypes as C
 import json
 import os
 import statistics
@@ -66,12 +65,6 @@ def main():
     kinds = [E.KIND_BY_NAME[m] for m in models]
     wts = [W.write_vpw(synth.synth_state_dict(m), os.path.join(tmp, f"{m}.vpw")) for m in models]
     lib = L.lib()
-    vp, i_ = C.c_void_p, C.c_int
-    lib.vpb_mask255.argtypes = [vp, i_, i_, i_, vp, vp]
-    lib.vpb_egolanes_ids.argtypes = [vp, i_, i_, i_, vp, vp]
-    lib.vpb_resize_nearest_u8.argtypes = [vp, i_, i_, vp, i_, i_, vp]
-    lib.vpb_resize_linear_f32.argtypes = [vp, i_, i_, vp, i_, i_, vp]
-    lib.vpb_visualize_mask.argtypes = [vp, i_, i_, i_, vp, i_, i_, i_, vp, i_, vp]
     cams = CAMERAS[4]
     n = len(cams)
     frames = camera_frames(torch, synth, cams)

@@ -10,7 +10,7 @@ from autoware_vision_pilot_b200 import autospeed as AS
 
 @pytest.mark.parametrize("batch", [0, -1, AS.MAX_BATCH + 1])
 def test_create_batch_rejects_a_batch_outside_1_to_8(batch):
-    lib = AS._bind()
+    lib = L.lib()
     h = C.c_void_p()
     assert lib.vp_autospeed_create_batch(b"/nonexistent/autospeed.vpw", 0, L.VPB_F16, None, batch, C.byref(h)) == -1
     assert f"batch {batch} out of range" in L.last_error()

@@ -200,7 +200,7 @@ def test_conv_per_image_weights_match_batch1_and_torch():
 def test_batched_engine_rejects_bad_calls(vpw, frames):
     n = 2
     eng = AS.AutoSpeedEngine(vpw, batch=n)
-    lib = AS._bind()
+    lib = L.lib()
     f = frames[0]
     h, w, _ = f.shape
     # single-frame calls on a batched engine

@@ -49,17 +49,7 @@ LEVELS = [(64, 128, 8.0, 0), (32, 64, 16.0, 8192), (16, 32, 32.0, 10240)]     # 
 
 @pytest.fixture(scope="module")
 def lib():
-    lib = L.lib()
-    vp, i, f = C.c_void_p, C.c_int, C.c_float
-    lib.vpb_as_mean_blocks.argtypes = [i]
-    lib.vpb_as_mean.argtypes = [i, vp, i, i, i, vp, vp, i, vp]
-    lib.vpb_as_upsample2.argtypes = [i, vp, i, i, i, i, vp, i, i, vp]
-    lib.vpb_as_maxpool5.argtypes = [i, vp, i, i, i, i, vp, i, vp]
-    lib.vpb_as_split_v.argtypes = [i, vp, i, i, i, i, vp, vp, i, vp]
-    lib.vpb_as_softmax_rows.argtypes = [i, vp, i, i, f, vp, vp]
-    lib.vpb_as_decode.argtypes = [i, vp, i, i, i, f, i, i, vp, i, vp]
-    lib.vpb_as_postprocess.argtypes = [vp, i, i, f, f] + [vp] * 10
-    return lib
+    return L.lib()
 
 
 def sync_cpu(t):

@@ -24,7 +24,7 @@ MISSING = b"/nonexistent/autospeed.vpw"   # the precision checks come first: nei
     (7, AS.PREC_SPLIT, 1, "takes dtype VPB_F16"),
 ])
 def test_create_precision_rejects_before_any_device_work(dtype, precision, batch, msg):
-    lib = AS._bind()
+    lib = L.lib()
     h = C.c_void_p()
     assert lib.vp_autospeed_create_precision(MISSING, 0, dtype, precision, None, batch, C.byref(h)) == VPB_ERR_ARG
     err = L.last_error()
@@ -33,7 +33,7 @@ def test_create_precision_rejects_before_any_device_work(dtype, precision, batch
 
 
 def test_create_precision_checks_the_batch_range_first():
-    lib = AS._bind()
+    lib = L.lib()
     h = C.c_void_p()
     assert lib.vp_autospeed_create_precision(MISSING, 0, L.VPB_F16, AS.PREC_16, None, 9, C.byref(h)) == VPB_ERR_ARG
     assert "batch 9 out of range" in L.last_error()
@@ -49,9 +49,9 @@ def test_python_dtype_mapping():
 
 
 def test_python_engine_raises_value_error_before_the_c_call(monkeypatch):
-    def no_bind():
+    def no_lib():
         raise AssertionError("the library was reached")
-    monkeypatch.setattr(AS, "_bind", no_bind)
+    monkeypatch.setattr(L, "lib", no_lib)
     with pytest.raises(ValueError, match="'fp64'"):
         AS.AutoSpeedEngine("/nonexistent/autospeed.vpw", dtype="fp64")
 
@@ -66,11 +66,6 @@ def test_python_fp32_selects_the_split_mode_through_the_new_call():
 
 def test_split_ops_reject_bad_arguments_without_a_gpu():
     lib = L.lib()
-    vp, i, f = C.c_void_p, C.c_int, C.c_float
-    lib.vpb_as_mean_split.argtypes = [vp, vp, i, i, i, vp, vp, vp]
-    lib.vpb_as_maxpool5_split.argtypes = [vp, vp, i, i, i, i, vp, vp, vp]
-    lib.vpb_as_softmax_rows_split.argtypes = [vp, vp, i, i, f, vp, vp, vp]
-    lib.vpb_as_decode_split.argtypes = [vp, vp, i, i, i, f, i, i, vp, vp]
     buf = (C.c_float * 64)()
     p = (C.addressof(buf) + 15) & ~15   # never dereferenced: every call below must fail validation first
     odd = p + 2

@@ -34,7 +34,7 @@ from oracle import autospeed as O
 from oracle import synth
 from tests.test_autospeed_gpu import _iou
 from tests.test_autospeed_ops_gpu import LEVELS, NA, U, check_mean, decode_ref, pool_ref
-from tests.test_conv_ops_gpu import (AS_IN_PLACE, AS_REWRITTEN, bind_conv_args, expected, operands, outputs,
+from tests.test_conv_ops_gpu import (AS_IN_PLACE, AS_REWRITTEN, expected, operands, outputs,
                                      padded_view, geometry, replay_engine, run)
 from tests.test_encoder_ops_gpu import assert_within, rand, split_residual
 
@@ -64,16 +64,7 @@ def bits(t):
 
 @pytest.fixture(scope="module")
 def lib():
-    lib = L.lib()
-    vp, i, f = C.c_void_p, C.c_int, C.c_float
-    lib.vpb_as_mean_blocks.argtypes = [i]
-    lib.vpb_as_mean_split.argtypes = [vp, vp, i, i, i, vp, vp, vp]
-    lib.vpb_as_maxpool5_split.argtypes = [vp, vp, i, i, i, i, vp, vp, vp]
-    lib.vpb_as_softmax_rows_split.argtypes = [vp, vp, i, i, f, vp, vp, vp]
-    lib.vpb_as_decode_split.argtypes = [vp, vp, i, i, i, f, i, i, vp, vp]
-    lib.vpb_as_upsample2.argtypes = [i, vp, i, i, i, i, vp, i, i, vp]
-    lib.vpb_as_split_v.argtypes = [i, vp, i, i, i, i, vp, vp, i, vp]
-    return lib
+    return L.lib()
 
 
 @pytest.fixture(scope="module")
@@ -246,7 +237,7 @@ def test_split_detector_convolutions(engines):
     es.infer(synth.synth_frame(0))
     n, inplace, rewritten = replay_engine(es.handle, "vp_autospeed_conv_args", es.stats()["n_launches"], "autospeed split")
     assert n > 40 and inplace == AS_IN_PLACE and rewritten == AS_REWRITTEN
-    lib = bind_conv_args()
+    lib = L.lib()
     found = {}
     for i in range(es.stats()["n_launches"]):
         a, name = L.ConvArgs(), C.c_char_p()

@@ -70,8 +70,6 @@ def test_preprocess_fmt_rejects_bad_bayer_and_4_channel_descriptors_without_a_gp
     """Every new check returns VPB_ERR_ARG with a message naming the call and the frame, before any device work (the
     pointers are never dereferenced); format 4 stays unknown."""
     lib = L.lib()
-    lib.vpb_preprocess_fmt.argtypes = [C.POINTER(L.FrameFmt), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                       C.c_void_p]
     buf = (C.c_uint8 * 64)()
     p = C.addressof(buf)
 

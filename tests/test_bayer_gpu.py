@@ -1,7 +1,6 @@
 """Raw Bayer and 4-channel (BGRA, RGBA) camera frames on the GPU: the demosaic and the alpha drop inside the
 pre-process must give, byte for byte, what the packed path gives on cv2.cvtColor of the frame, for the op, both
 engines, every entry point, the graph and the split-fp16 mode."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -86,8 +85,6 @@ def _dev_crop(m, pattern, y0, x0, h, w, pad=29):
 # ------------------------------------------------------------------------------------------------ op level
 def _op(desc, mode, conv, dtype):
     lib = L.lib()
-    lib.vpb_preprocess_fmt.argtypes = [C.POINTER(L.FrameFmt), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                       C.c_void_p]
     out = torch.full((320, 640, 4), 7, dtype=torch.int16, device="cuda")
     u8 = torch.full((320, 640, 3), 77, dtype=torch.uint8, device="cuda")
     L.check(lib.vpb_preprocess_fmt(L.frame_fmt_descs([desc]), mode, conv, dtype, out.data_ptr(), u8.data_ptr(), None),

@@ -1,6 +1,6 @@
-"""CPU-only checks of the shared library: it loads, exports every symbol the headers declare, and
-its host-only pieces (integer resize tables, argument validation, .vpw writer) agree with the
-oracle.  No kernel is launched here."""
+"""CPU-only checks of the shared library: it loads, exports every symbol the headers declare, its ctypes signatures and
+struct mirrors match the headers, and its host-only pieces (integer resize tables, argument validation, .vpw writer)
+agree with the oracle.  No kernel is launched here."""
 import ctypes as C
 import os
 import re
@@ -14,23 +14,61 @@ from autoware_vision_pilot_b200 import weights as W
 from oracle import resize
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADERS = ("vp_b200.h", "vp_b200_ops.h", "vp_b200_autospeed.h", "vp_b200_multicam.h")
 
 
-def _declared_symbols():
-    names = set()
-    for h in ("vp_b200.h", "vp_b200_ops.h", "vp_b200_multicam.h", "vp_b200_autospeed.h"):
+def _prototypes():
+    """{name: (return type, [argument declarations])} of every function the headers declare, in header order"""
+    protos = {}
+    for h in HEADERS:
         src = open(os.path.join(ROOT, "include", h)).read()
         src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-        names |= set(re.findall(r"\b(vpb?_[a-z0-9_]+)\s*\(", src))
-    return sorted(names)
+        src = re.sub(r"^\s*#.*$", "", src, flags=re.M)
+        for decl in src.split(";"):
+            decl = " ".join(re.split(r"[{}]", decl)[-1].split())
+            m = re.fullmatch(r"(.+?)\b(vpb?_\w+)\s*\((.*)\)", decl)
+            if m:
+                args = [a.strip() for a in m.group(3).split(",")]
+                protos[m.group(2)] = (m.group(1).strip(), [] if args == ["void"] else args)
+    return protos
+
+
+def _c_kind(decl):
+    """"pointer", "void" or the scalar type of a C declaration ("const float* w" -> pointer, "long long n" -> long)"""
+    if "*" in decl:
+        return "pointer"
+    words = decl.split()
+    return next(k for k in ("void", "double", "float", "size_t", "long", "int") if k in words)
+
+
+def _ctypes_kind(t):
+    if t is not None and (t in (C.c_void_p, C.c_char_p) or issubclass(t, C._Pointer)):
+        return "pointer"
+    return {None: "void", C.c_int: "int", C.c_float: "float", C.c_double: "double", C.c_size_t: "size_t",
+            C.c_long: "long"}[t]
 
 
 def test_library_exports_every_declared_symbol():
     lib = L.lib()
-    syms = _declared_symbols()
+    syms = sorted(_prototypes())
     assert len(syms) >= 20
     missing = [s for s in syms if not hasattr(lib, s)]
     assert not missing, missing
+
+
+def test_signature_table_matches_the_headers():
+    """_lib.SIGNATURES declares every header function but the variadic vpb_set_error, in header order, each with the
+    header's arity and the header's kind of every argument and of the return value; lib() applies it."""
+    protos = _prototypes()
+    assert list(L.SIGNATURES) == [n for n in protos if n != "vpb_set_error"]
+    for name, (restype, argtypes) in L.SIGNATURES.items():
+        ret, args = protos[name]
+        assert _ctypes_kind(restype) == _c_kind(ret), name
+        assert [_ctypes_kind(t) for t in argtypes] == [_c_kind(a) for a in args], name
+    lib = L.lib()
+    for name, (restype, argtypes) in L.SIGNATURES.items():
+        fn = getattr(lib, name)
+        assert (fn.restype, tuple(fn.argtypes)) == (restype, tuple(argtypes)), name
 
 
 @pytest.mark.parametrize("mode,in_size,out_size", [(1, 1920, 640), (1, 1080, 320), (1, 700, 320), (1, 401, 640),
@@ -39,8 +77,6 @@ def test_resize_tables_match_oracle(mode, in_size, out_size):
     """The C++ host code that builds the kernel's integer coefficient tables reproduces the
     Pillow / OpenCV restatements exactly (which are themselves pinned against the libraries)."""
     lib = L.lib()
-    lib.vpb_resize_tables_host.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                           C.c_int, C.POINTER(C.c_int)]
     bounds = (C.c_int * out_size)()
     cap = out_size * 64
     coeffs = (C.c_int * cap)()
@@ -79,7 +115,6 @@ def test_conv_rejects_bad_arguments_without_a_gpu():
     assert lib.vpb_conv_gemm(C.byref(a), None) == -1 and "upconv" in L.last_error()      # Cout not a multiple of 16
     a.Cout, a.in2, a.w2, a.Cin2, a.ld2, a.taps2 = 32, C.addressof(dummy), C.addressof(dummy), 8, 8, 1
     assert lib.vpb_conv_gemm(C.byref(a), None) == -1 and "upconv" in L.last_error()      # skip taps must be 9
-    lib.vpb_upconv_compose.argtypes = [C.c_void_p] * 6 + [C.c_int] * 4 + [C.c_void_p] * 4
     assert lib.vpb_upconv_compose(None, None, None, None, None, None, 8, 8, 8, 0, None, None, None, None) == -1
 
 
@@ -89,7 +124,6 @@ def test_engine_conv_args_reject_bad_arguments_without_a_gpu():
     lib = L.lib()
     for fn in ("vp_engine_conv_args", "vp_autospeed_conv_args"):
         f = getattr(lib, fn)
-        f.argtypes = [C.c_void_p, C.c_int, C.POINTER(L.ConvArgs), C.POINTER(C.c_char_p)]
         a = L.ConvArgs()
         name = C.c_char_p()
         for op in (0, -1):
@@ -101,15 +135,6 @@ def test_encoder_ops_reject_bad_arguments_without_a_gpu():
     """Every contract violation of the encoder / context op entry points returns VPB_ERR_ARG with a message before
     any device work (so no GPU is needed to see it)."""
     lib = L.lib()
-    vp, i = C.c_void_p, C.c_int
-    lib.vpb_stem_conv_ex.argtypes = [i, vp, vp, i, i, vp, vp, vp, vp, i, vp]
-    lib.vpb_depthwise.argtypes = [i, vp, i, i, i, i, i, vp, vp, vp, vp, vp]
-    lib.vpb_depthwise_ex.argtypes = [i, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp, i, i, vp]
-    lib.vpb_se_scale_ex.argtypes = [i, vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, i, vp]
-    lib.vpb_gap_ex.argtypes = [i, vp, vp, i, i, i, vp, i, vp]
-    lib.vpb_linear_ex.argtypes = [vp, vp, vp, i, i, i, vp, i, vp]
-    lib.vpb_ctx_conv1_ex.argtypes = [i, vp, i, i, vp, vp, i, vp, vp, i, i, i, vp]
-    lib.vpb_fuse_pool_concat_ex.argtypes = [i] + [vp] * 10 + [i, i, vp, vp, i, vp]
     buf = (C.c_float * 64)()
     p = C.addressof(buf)           # never dereferenced: every call below must fail validation first
 
@@ -172,14 +197,6 @@ def test_autospeed_ops_reject_bad_arguments_without_a_gpu():
     """Every contract violation of the AutoSpeed op entry points (the preconditions the SIMT kernels assume) returns
     VPB_ERR_ARG with a message before any device work."""
     lib = L.lib()
-    vp, i, f = C.c_void_p, C.c_int, C.c_float
-    lib.vpb_as_mean.argtypes = [i, vp, i, i, i, vp, vp, i, vp]
-    lib.vpb_as_upsample2.argtypes = [i, vp, i, i, i, i, vp, i, i, vp]
-    lib.vpb_as_maxpool5.argtypes = [i, vp, i, i, i, i, vp, i, vp]
-    lib.vpb_as_split_v.argtypes = [i, vp, i, i, i, i, vp, vp, i, vp]
-    lib.vpb_as_softmax_rows.argtypes = [i, vp, i, i, f, vp, vp]
-    lib.vpb_as_decode.argtypes = [i, vp, i, i, i, f, i, i, vp, i, vp]
-    lib.vpb_as_postprocess.argtypes = [vp, i, i, f, f] + [vp] * 10
     buf = (C.c_float * 64)()
     p = (C.addressof(buf) + 15) & ~15   # never dereferenced: every call below must fail validation first
     odd = p + 2                          # 2-byte aligned, not 16
@@ -239,7 +256,6 @@ def test_autospeed_ops_reject_bad_arguments_without_a_gpu():
     for name, call, msg in cases:
         assert call() == -1, name
         assert msg in L.last_error(), (name, L.last_error())
-    lib.vpb_as_mean_blocks.argtypes = [i]
     assert [lib.vpb_as_mean_blocks(hw) for hw in (1, 63, 64, 128 * 256, 16 * 32)] == [1, 1, 1, 148, 8]
 
 
@@ -317,38 +333,48 @@ def test_engine_create_fails_loudly_without_gpu(tmp_path):
 
 
 def test_ctypes_mirrors_match_the_c_struct_layouts(tmp_path):
-    """The headers are the contract; the ctypes Structures in _lib.py / engine.py are hand-written mirrors.
-    A C program compiled against include/*.h prints sizeof / offsetof of every struct and field, which must
-    equal what ctypes computes — catches a field added on one side only."""
+    """The headers are the contract; the ctypes Structures in _lib.py are hand-written mirrors, each naming its C struct.
+    A C program compiled against include/*.h prints sizeof of every struct and offsetof / sizeof of every field, and
+    the constants the Python side repeats, which must equal what ctypes and Python compute — catches a field added on
+    one side only."""
     import subprocess
     from autoware_vision_pilot_b200 import engine as E
-    from autoware_vision_pilot_b200 import multicam as M
-    mirrors = {
-        "vp_tap_view": (E._TapView, {}),
-        "vp_multicam_view": (M._View, {}),
-        "vpb_conv_args": (L.ConvArgs, {"inp": "in"}),
-        "vpb_lateral_state": (L.LateralState, {}),
-        "vpb_lateral_out": (L.LateralOut, {}),
-        "vp_engine_config": (E._Config, {}),
-        "vp_output": (E._Output, {}),
-        "vp_engine_stats": (E._Stats, {}),
-    }
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "vp_b200.h"', '#include "vp_b200_ops.h"', '#include "vp_b200_multicam.h"',
-             'int main(void) {']
-    for cname, (cls, rename) in mirrors.items():
+    from oracle import yuv as Y
+    mirrors = {}
+    for cls in vars(L).values():
+        if isinstance(cls, type) and issubclass(cls, C.Structure):
+            m = re.match(r"Mirror of (vpb?_\w+)", cls.__doc__ or "")
+            assert m, f"{cls.__name__} does not name the C struct it mirrors"
+            mirrors[m.group(1)] = cls
+    assert set(mirrors) == {"vpb_conv_args", "vpb_frame", "vpb_frame_fmt", "vpb_src_job", "vpb_lateral_state",
+                            "vpb_lateral_out", "vp_engine_config", "vp_output", "vp_source_output", "vp_engine_stats",
+                            "vp_lateral_config", "vp_view", "vp_tap_view", "vp_multicam_view"}
+    consts = {"VP_MAX_BATCH": L.MAX_BATCH, "VP_SRC_MASK": E.SRC_MASK, "VP_SRC_DEPTH": E.SRC_DEPTH,
+              "VP_SRC_OVERLAY": E.SRC_OVERLAY, "VPB_SRC_MASK255": L.SRC_MASK255, "VPB_SRC_IDS": L.SRC_IDS,
+              "VPB_SRC_DEPTH": L.SRC_DEPTH, "VPB_SRC_OVERLAY": L.SRC_OVERLAY, "VPB_PIX_PACKED": L.PIX_PACKED,
+              "VPB_PIX_NV12": L.PIX_NV12, "VPB_PIX_UYVY": L.PIX_UYVY, "VPB_PIX_YUYV": L.PIX_YUYV}
+    lines = ["#include <stdio.h>", "#include <stddef.h>"] + [f'#include "{h}"' for h in HEADERS] + ["int main(void) {"]
+    for cname, cls in mirrors.items():
         lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')
         for fname, _ in cls._fields_:
-            lines.append(f'  printf("{cname}.{fname} %zu\\n", offsetof({cname}, {rename.get(fname, fname)}));')
-    lines += ['  return 0;', '}']
+            cf = "in" if fname == "inp" else fname      # vpb_conv_args.in: a Python keyword
+            lines.append(f'  printf("{cname}.{fname} %zu %zu\\n", offsetof({cname}, {cf}), '
+                         f'sizeof((({cname}*)0)->{cf}));')
+    lines += [f'  printf("{k} %d\\n", {k});' for k in consts] + ["  return 0;", "}"]
     src = tmp_path / "layout.c"
     src.write_text("\n".join(lines))
     exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    out = dict(l.split() for l in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.splitlines())
-    for cname, (cls, _) in mirrors.items():
-        assert int(out[cname]) == C.sizeof(cls), cname
+    subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)],
+                   check=True)
+    out = {k: [int(x) for x in v] for k, *v in
+           (l.split() for l in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.splitlines())}
+    for cname, cls in mirrors.items():
+        assert out[cname] == [C.sizeof(cls)], cname
         for fname, _ in cls._fields_:
-            assert int(out[f"{cname}.{fname}"]) == getattr(cls, fname).offset, f"{cname}.{fname}"
+            field = getattr(cls, fname)
+            assert out[f"{cname}.{fname}"] == [field.offset, field.size], f"{cname}.{fname}"
+    assert {k: out[k][0] for k in consts} == consts
+    assert (Y.PIX_PACKED, Y.PIX_NV12, Y.PIX_UYVY, Y.PIX_YUYV) == (L.PIX_PACKED, L.PIX_NV12, L.PIX_UYVY, L.PIX_YUYV)
 
 
 def test_pillow_bilinear_tables_reproduce_pillow(tmp_path):
@@ -356,8 +382,6 @@ def test_pillow_bilinear_tables_reproduce_pillow(tmp_path):
     run through the kernel's integer arithmetic in numpy, reproduce Image.resize(BILINEAR) bit for bit."""
     from PIL import Image
     lib = L.lib()
-    lib.vpb_resize_tables_host.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                           C.c_int, C.POINTER(C.c_int)]
 
     def tables(in_size, out_size):
         bounds = (C.c_int * out_size)()

@@ -643,14 +643,6 @@ AS_REWRITTEN = {  # op: the later op that rewrites its output or an input
 }
 
 
-def bind_conv_args():
-    lib = L.lib()
-    for fn in ("vp_engine_conv_args", "vp_autospeed_conv_args"):
-        f = getattr(lib, fn)
-        f.argtypes = [C.c_void_p, C.c_int, C.POINTER(L.ConvArgs), C.POINTER(C.c_char_p)]
-    return lib
-
-
 def spans(a):
     """(ptr, nbytes, pitch, width) in bytes of every tensor view op a writes and reads: a view covers width bytes every
     pitch bytes of [ptr, ptr + nbytes)"""
@@ -695,7 +687,7 @@ def overlap(u, v):
 
 
 def replay_engine(handle, fn, n_ops, what):
-    lib = bind_conv_args()
+    lib = L.lib()
     f = getattr(lib, fn)
     convs = []
     for i in range(n_ops):

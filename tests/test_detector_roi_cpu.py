@@ -34,7 +34,7 @@ def test_set_detector_takes_the_detector_type_in_c(tmp_path, std, first):
 
 
 def test_null_engine_is_rejected():
-    lib = E._bind()
+    lib = L.lib()
     assert lib.vp_engine_set_roi(None, 0, 0, 0, 10, 10) == VPB_ERR_ARG
     assert "NULL engine" in L.last_error()
     assert lib.vp_engine_set_detector(None, None) == VPB_ERR_ARG

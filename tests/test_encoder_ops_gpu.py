@@ -47,16 +47,7 @@ ACT_ERR = {NONE: (1.0, 0.0), SILU: (1.1, 6.0), GELU: (1.13, 10.0), SIGMOID: (0.2
 
 @pytest.fixture(scope="module")
 def lib():
-    lib = L.lib()
-    vp, i = C.c_void_p, C.c_int
-    lib.vpb_stem_conv_ex.argtypes = [i, vp, vp, i, i, vp, vp, vp, vp, i, vp]
-    lib.vpb_depthwise_ex.argtypes = [i, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp, i, i, vp]
-    lib.vpb_se_scale_ex.argtypes = [i, vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, i, vp]
-    lib.vpb_gap_ex.argtypes = [i, vp, vp, i, i, i, vp, i, vp]
-    lib.vpb_linear_ex.argtypes = [vp, vp, vp, i, i, i, vp, i, vp]
-    lib.vpb_ctx_conv1_ex.argtypes = [i, vp, i, i, vp, vp, i, vp, vp, i, i, i, vp]
-    lib.vpb_fuse_pool_concat_ex.argtypes = [i] + [vp] * 10 + [i, i, vp, vp, i, vp]
-    return lib
+    return L.lib()
 
 
 # ---------------------------------------------------------------------------------------------------------- helpers

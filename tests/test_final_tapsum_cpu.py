@@ -12,7 +12,6 @@ from autoware_vision_pilot_b200 import _lib as L
 def test_weight_repack_is_the_tap_stacked_matrix(Cout, Cin):
     """[Cout][Cin][3][3] -> [9*Cout][Cin]: row t*Cout + o holds W[o][:][dy][dx], t = 3*dy + dx."""
     lib = L.lib()
-    lib.vpb_final_conv_weights_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     w = np.random.default_rng(Cout * 1000 + Cin).standard_normal((Cout, Cin, 3, 3)).astype(np.float32)
     out = np.full((9 * Cout, Cin), np.nan, dtype=np.float32)
     L.check(lib.vpb_final_conv_weights_host(w.ctypes.data, Cout, Cin, out.ctypes.data), "final_conv_weights")
@@ -26,9 +25,6 @@ def test_weight_repack_is_the_tap_stacked_matrix(Cout, Cin):
 
 def test_tapsum_and_final_gemm_reject_bad_arguments_without_a_gpu():
     lib = L.lib()
-    vp, i = C.c_void_p, C.c_int
-    lib.vpb_final_tapsum.argtypes = [vp, vp, i, i, i, i, vp, vp, i, vp]
-    lib.vpb_final_conv_weights_host.argtypes = [vp, i, i, vp]
     buf = (C.c_float * 64)()
     p = C.addressof(buf)           # never dereferenced: every call below must fail validation first
 

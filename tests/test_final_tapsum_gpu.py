@@ -27,14 +27,6 @@ pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
 
 
-def _lib():
-    lib = L.lib()
-    vp, i = C.c_void_p, C.c_int
-    lib.vpb_final_tapsum.argtypes = [vp, vp, i, i, i, i, vp, vp, i, vp]
-    lib.vpb_final_conv_weights_host.argtypes = [vp, i, i, vp]
-    return lib
-
-
 def _tdt(dtype):
     return torch.bfloat16 if dtype == L.VPB_BF16 else torch.float16
 
@@ -44,13 +36,13 @@ def _weights(w16, dtype):
     Cout, Cin = w16.shape[:2]
     w32 = w16.float().contiguous()
     out = torch.empty(9 * Cout, Cin, dtype=torch.float32)
-    L.check(_lib().vpb_final_conv_weights_host(w32.data_ptr(), Cout, Cin, out.data_ptr()), "final_conv_weights")
+    L.check(L.lib().vpb_final_conv_weights_host(w32.data_ptr(), Cout, Cin, out.data_ptr()), "final_conv_weights")
     return out.to(_tdt(dtype)).cuda()          # exact: the values are 16-bit already
 
 
 def run_pair(xp, wmat, b, Cout, kind, dtype):
     """xp [N][H+2][W+2][Cin] zero-bordered 16-bit -> out fp32 [N][Cout][H][W], cls uint8 [N][H][W] (None for FINAL_NONE)."""
-    lib = _lib()
+    lib = L.lib()
     N, Hp, Wp, Cin = xp.shape
     H, W = Hp - 2, Wp - 2
     P = torch.full((N, 9 * Cout, H, W), float("nan"), device="cuda")

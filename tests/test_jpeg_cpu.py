@@ -112,7 +112,6 @@ def test_stages_pinned():
 # ------------------------------------------------------------------------------------------------ library checks
 def _info(b):
     lib = L.lib()
-    lib.vpb_jpeg_info.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     h, w, s = C.c_int(), C.c_int(), C.c_int()
     rc = lib.vpb_jpeg_info(b, len(b), C.byref(h), C.byref(w), C.byref(s))
     return rc, (h.value, w.value, s.value), L.last_error()
@@ -184,16 +183,11 @@ def test_device_entry_points_reject_jpeg_without_a_device():
     b = encode(natural(16, 16))
     buf = C.create_string_buffer(b, len(b))
     arr = L.frame_fmt_descs([(L.PIX_JPEG, C.addressof(buf), 16, 16, len(b), 0, 0)])
-    lib.vpb_preprocess_fmt.argtypes = [C.POINTER(L.FrameFmt), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                       C.c_void_p]
     assert lib.vpb_preprocess_fmt(arr, 1, 0, 0, C.c_void_p(1), None, None) == VPB_ERR_ARG
     assert "vpb_preprocess_fmt: frame 0: unknown format 11 for a device frame: JPEG frames" in L.last_error()
-    lib.vpb_rectify_frames.argtypes = [C.POINTER(L.FrameFmt), C.POINTER(C.c_void_p), C.c_int, C.c_int,
-                                       C.POINTER(C.c_void_p), C.c_void_p]
     one = (C.c_void_p * 1)(1)
     assert lib.vpb_rectify_frames(arr, one, 1, 0, one, None) == VPB_ERR_ARG
     assert "vpb_rectify_frames: frame 0: unknown format 11 for a device frame: JPEG frames" in L.last_error()
-    lib.vpb_jpeg_decoder_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
     h = C.c_void_p()
     for cap in ((2401, 100, 1), (100, 4801, 1), (100, 100, 9), (0, 100, 1)):
         assert lib.vpb_jpeg_decoder_create(*cap, 0, C.byref(h)) == VPB_ERR_ARG

@@ -110,7 +110,6 @@ def test_runs_on_the_engine_output_without_leaving_the_device(tmp_path):
     assert (c, h, w) == (3, 80, 160)
     masks = torch.empty(3, 80, 160, device="cuda")
     lib = L.lib()
-    lib.vpb_lane_masks.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.check(lib.vpb_lane_masks(ptr, 3 * 80 * 160, 0.0, masks.data_ptr(), None), "vpb_lane_masks")
     post = LateralPostProcess()
     dev = post.update(masks)

@@ -1,15 +1,11 @@
-"""The lateral post-process inside the engine call, without a GPU: the new C symbols exist, the vp_lateral_config
-mirror has the C layout, and the Python engine rejects bad arguments before it calls the library."""
+"""The lateral post-process inside the engine call, without a GPU: the new C symbols exist and the Python engine
+rejects bad arguments before it calls the library."""
 import ctypes as C
-import os
-import subprocess
 
 import pytest
 
 from autoware_vision_pilot_b200 import _lib as L
 from autoware_vision_pilot_b200 import engine as E
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_symbols_exist():
@@ -17,22 +13,6 @@ def test_symbols_exist():
     for sym in ("vp_engine_set_lateral", "vp_engine_set_steering", "vp_engine_lateral_reset", "vp_engine_lateral",
                 "vp_engine_graph_captures", "vpb_lateral_update_logits"):
         getattr(lib, sym)
-
-
-def test_lateral_config_mirror_has_the_c_layout(tmp_path):
-    fields = [f for f, _ in E.LateralConfig._fields_]
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "vp_b200.h"', 'int main(void) {',
-             '  printf("size %zu\\n", sizeof(vp_lateral_config));']
-    lines += [f'  printf("{f} %zu\\n", offsetof(vp_lateral_config, {f}));' for f in fields]
-    lines += ['  return 0;', '}']
-    src = tmp_path / "lat_cfg.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "lat_cfg"
-    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    out = dict(l.split() for l in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.splitlines())
-    assert int(out["size"]) == C.sizeof(E.LateralConfig)
-    for f in fields:
-        assert int(out[f]) == getattr(E.LateralConfig, f).offset, f
 
 
 class _NoCall:

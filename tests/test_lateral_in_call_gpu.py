@@ -30,17 +30,6 @@ H_WIDE = np.array([[1.05, 0.0, -16.0], [0.0, 1.0, 0.0], [0.0, 0.0, 1.0]]) @ H_RE
 ALL_SET = -1e30            # a threshold below every logit: full masks, so PathFinder runs on the synthetic network's output
 
 
-def _lib():
-    lib = L.lib()
-    ip, dp, vp = C.POINTER(C.c_int), C.POINTER(C.c_double), C.c_void_p
-    lib.vpb_lane_masks.argtypes = [vp, C.c_int, C.c_float, vp, vp]
-    lib.vpb_lateral_init.argtypes = [vp, vp]
-    lib.vpb_lateral_update_cameras.argtypes = [vp, C.c_int, C.c_int, C.c_int, ip, ip, C.c_float, dp, dp, vp, vp, vp]
-    lib.vpb_lateral_update_logits.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_float, ip, ip, C.c_float, dp, dp, vp,
-                                              vp, vp]
-    return lib
-
-
 def _sizes(sizes):
     n = len(sizes)
     return (C.c_int * n)(*[w for w, _ in sizes]), (C.c_int * n)(*[h for _, h in sizes])
@@ -58,7 +47,7 @@ class Chain:
     of its own (in place), with the image sizes the caller passes."""
 
     def __init__(self, n, threshold=0.0, smoothing=0.5, homs=None):
-        self.lib, self.n, self.thr, self.sm, self.hom = _lib(), n, threshold, smoothing, _doubles(homs)
+        self.lib, self.n, self.thr, self.sm, self.hom = L.lib(), n, threshold, smoothing, _doubles(homs)
         self.state = torch.zeros(n * ST, dtype=torch.uint8, device="cuda")
         self.out = torch.zeros(n * REC, dtype=torch.uint8, device="cuda")
         self.masks = torch.empty(n * 3 * 80 * 160, dtype=torch.float32, device="cuda")
@@ -114,7 +103,7 @@ def _logits(rng, masks, thr):
 @pytest.mark.parametrize("thr", [0.0, 0.3])
 @pytest.mark.parametrize("n", [1, 3, 8])
 def test_logits_op_equals_lane_masks_then_cameras(n, thr):
-    lib = _lib()
+    lib = L.lib()
     rng = np.random.default_rng(17 * n + int(10 * thr))
     sizes = [(1920, 1080), (1280, 720), (1920, 660), (640, 480), (3840, 2160), (1280, 960), (800, 4320), (577, 321)][:n]
     homs = None if n == 1 else [(H_REF, H_WIDE)[k % 2] for k in range(n)]
@@ -333,7 +322,7 @@ def test_feature_off_keeps_the_launch_list_and_on_adds_one_op(vpws):
 
 
 def test_errors_before_device_work(vpws):
-    lib = E._bind()
+    lib = L.lib()
     two = E.Engine([E.SCENE_SEG, E.EGO_LANES], [vpws["scene_seg"], vpws["ego_lanes"]], resize_mode=E.RESIZE_CV_LINEAR)
     cfg = E.LateralConfig(0.0, 0.5, None)
     assert lib.vp_engine_set_lateral(two.handle, 0, C.byref(cfg)) == VPB_ERR_ARG

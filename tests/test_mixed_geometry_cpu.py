@@ -12,7 +12,7 @@ VPB_ERR_ARG = -1
 
 def _cameras_call(n=2, sizes=((1920, 1080), (1280, 720)), masks=True, states=True, outs=True, null_w=False,
                   null_h=False, smoothing=0.5):
-    lib = LT._bind()
+    lib = L.lib()
     buf = (C.c_double * 64)()
     p = C.addressof(buf)            # never dereferenced: every call below must fail validation first
     ws = (C.c_int * max(len(sizes), 1))(*[s[0] for s in sizes])
@@ -57,7 +57,7 @@ def test_cameras_rejects_an_image_taller_than_4320_naming_the_camera(sizes, cam)
 
 @pytest.mark.parametrize("smoothing", [-0.01, 1.01, float("nan"), float("inf"), float("-inf")])
 def test_every_lateral_call_rejects_smoothing_outside_0_to_1(smoothing):
-    lib = LT._bind()
+    lib = L.lib()
     buf = (C.c_double * 64)()
     p = C.addressof(buf)
     assert _cameras_call(smoothing=smoothing) == VPB_ERR_ARG
@@ -69,7 +69,7 @@ def test_every_lateral_call_rejects_smoothing_outside_0_to_1(smoothing):
 
 
 def test_single_and_batch_calls_reject_an_image_taller_than_4320():
-    lib = LT._bind()
+    lib = L.lib()
     buf = (C.c_double * 64)()
     p = C.addressof(buf)
     assert lib.vpb_lateral_update(p, 128, 256, 7680, 4321, 0.5, None, 0.0, p, p, None) == VPB_ERR_ARG
@@ -79,7 +79,7 @@ def test_single_and_batch_calls_reject_an_image_taller_than_4320():
 
 
 def test_batch_call_names_the_camera_of_a_bad_size_and_keeps_its_message():
-    lib = LT._bind()
+    lib = L.lib()
     buf = (C.c_double * 64)()
     p = C.addressof(buf)
     assert lib.vpb_lateral_update_batch(p, 3, 80, 160, 1920, 0, 0.5, None, None, p, p, None) == VPB_ERR_ARG

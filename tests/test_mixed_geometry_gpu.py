@@ -381,7 +381,7 @@ def test_mixed_rig_local_chain(ckpts, rig):
 
 def test_lateral_cameras_errors_on_device_buffers():
     from autoware_vision_pilot_b200 import lateral as LT
-    lib = LT._bind()
+    lib = L.lib()
     m = torch.zeros(2, 3, 80, 160, device="cuda")
     st = torch.zeros(2 * C.sizeof(L.LateralState), dtype=torch.uint8, device="cuda")
     ws, hs = (C.c_int * 2)(1920, 1280), (C.c_int * 2)(1080, 0)

@@ -13,7 +13,7 @@ VPB_ERR_ARG = -1
 
 
 def _batch_call(masks=True, n=2, H=80, W=160, states=True, outs=True, img=(1920, 1080)):
-    lib = LT._bind()
+    lib = L.lib()
     buf = (C.c_double * 64)()
     p = C.addressof(buf)            # never dereferenced: every call below must fail validation first
     return lib.vpb_lateral_update_batch(p if masks else None, n, H, W, img[0], img[1], 0.5, None, None,
@@ -38,7 +38,7 @@ def test_lateral_batch_rejects_bad_geometry_and_null_pointers(case, kw):
 
 
 def test_lateral_single_camera_keeps_its_message():
-    lib = LT._bind()
+    lib = L.lib()
     assert lib.vpb_lateral_update(None, 80, 160, 1920, 1080, 0.5, None, 0.0, None, None, None) == VPB_ERR_ARG
     assert L.last_error().startswith("lateral: need masks")
 
@@ -51,7 +51,7 @@ def test_batched_lateral_python_rejects_a_camera_count_before_allocating(cameras
 
 @pytest.mark.parametrize("n", [0, -3, 9])
 def test_multicam_local_rejects_a_camera_count_outside_1_to_8(n):
-    lib = MC._bind()
+    lib = L.lib()
     h = C.c_void_p()
     assert lib.vp_multicam_create_local(n, 0, None, C.byref(h)) == VPB_ERR_ARG
     assert f"vp_multicam_create_local: {n} cameras (1..8)" in L.last_error()
@@ -61,6 +61,6 @@ def test_multicam_local_rejects_a_camera_count_outside_1_to_8(n):
 
 
 def test_multicam_local_rejects_a_null_out():
-    lib = MC._bind()
+    lib = L.lib()
     assert lib.vp_multicam_create_local(2, 0, None, None) == VPB_ERR_ARG
     assert "NULL out" in L.last_error()

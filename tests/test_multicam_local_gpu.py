@@ -147,7 +147,6 @@ def ego_vpw(tmp_path_factory):
 def _lane_masks(raw_ptr, n, out, stream):
     from autoware_vision_pilot_b200 import _lib as L
     lib = L.lib()
-    lib.vpb_lane_masks.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.check(lib.vpb_lane_masks(raw_ptr, n * 3 * 80 * 160, 0.0, out.data_ptr(), stream), "vpb_lane_masks")
 
 

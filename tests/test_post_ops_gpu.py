@@ -12,22 +12,9 @@ from oracle import net, post
 pytestmark = pytest.mark.gpu
 
 
-def _lib():
-    lib = L.lib()
-    vp = C.c_void_p
-    lib.vpb_mask255.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp]
-    lib.vpb_egolanes_ids.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp]
-    lib.vpb_lane_masks.argtypes = [vp, C.c_int, C.c_float, vp, vp]
-    lib.vpb_resize_nearest_u8.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp]
-    lib.vpb_resize_linear_f32.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp]
-    lib.vpb_polyfit.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp]
-    lib.vpb_bayes_fuse.argtypes = [vp, vp, C.c_int, vp]
-    return lib
-
-
 @pytest.mark.parametrize("ch", [3, 1])
 def test_mask255_rule(ch):
-    lib = _lib()
+    lib = L.lib()
     g = torch.Generator().manual_seed(ch)
     raw = torch.randn(ch, 320, 640, generator=g)
     raw[:, :4, :8] = 0.25          # exact ties -> first max wins (class 0), not class 1
@@ -38,7 +25,7 @@ def test_mask255_rule(ch):
 
 
 def test_egolanes_ids_and_float_masks():
-    lib = _lib()
+    lib = L.lib()
     raw = torch.randn(3, 80, 160, generator=torch.Generator().manual_seed(3))
     d = raw.cuda()
     ids = torch.empty(80, 160, dtype=torch.uint8, device="cuda")
@@ -51,7 +38,7 @@ def test_egolanes_ids_and_float_masks():
 
 @pytest.mark.parametrize("dh,dw", [(1080, 1920), (720, 1280), (333, 517)])
 def test_resize_back(dh, dw):
-    lib = _lib()
+    lib = L.lib()
     rng = np.random.default_rng(dh)
     m = (rng.integers(0, 2, (320, 640)) * 255).astype(np.uint8)
     dm = torch.from_numpy(m).cuda()
@@ -83,7 +70,7 @@ def _fit(lib, sets, order):
 def test_polyfit_matches_fp64_lstsq(order):
     """Gate 1e-9 relative (SURVEY.md §8d) on the three coordinate regimes of the reference: model
     space y in [40,79], BEV pixels y in [200,640] (cond 2.5e6), BEV metres."""
-    lib = _lib()
+    lib = L.lib()
     rng = np.random.default_rng(order)
     sets = []
     for lo, hi, n in [(40, 79, 40), (40, 79, 200), (200, 640, 90), (0.5, 40.0, 64), (40, 79, 13), (10, 30, 5)]:
@@ -105,7 +92,7 @@ def test_polyfit_matches_fp64_lstsq(order):
 
 def test_bayes_fusion_over_eight_cameras():
     """SURVEY.md §8e: the reference's Estimator::update applied to each camera's measurement."""
-    lib = _lib()
+    lib = L.lib()
     rng = np.random.default_rng(8)
     st = post.initial_state()
     meas = []
@@ -131,8 +118,6 @@ def test_visualize_mask_overlay_is_bit_exact(viz, code, h, w):
     """vpb_visualize_mask (palette + nearest resize + half/half blend in one pass) == the reference's
     three-step composition restated in oracle/post.py (pinned against cv2 on the CPU)."""
     lib = L.lib()
-    lib.vpb_visualize_mask.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                       C.c_void_p, C.c_int, C.c_void_p]
     rng = np.random.default_rng(h + code)
     vals = {"scene": [0, 255], "domain": [0, 255, 9], "egolanes": [0, 1, 2, 255]}[viz]
     mask = rng.choice(vals, size=(320, 640)).astype(np.uint8)
@@ -152,8 +137,6 @@ def test_autosteer_buffer_and_decode():
     import ctypes as C
     from autoware_vision_pilot_b200 import _lib as L
     lib = L.lib()
-    lib.vpb_autosteer_pack.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.vpb_autosteer_decode.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     n = 3 * 80 * 160
     buf = torch.zeros(2, n, device="cuda")
     filled = torch.zeros(1, dtype=torch.int32, device="cuda")

@@ -7,7 +7,6 @@ the converting kernel instantiations.
 
 Device frames sit in buffers padded with 0xff, and outputs are pre-filled with sentinels, so a read of padding or a
 write outside the image shows up as a wrong value."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -117,15 +116,6 @@ class DevFrame:
         self.ptr = buf.data_ptr() + start
 
 
-def _op_bind():
-    lib = L.lib()
-    lib.vpb_preprocess.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
-                                   C.c_void_p, C.c_void_p]
-    lib.vpb_preprocess_fmt.argtypes = [C.POINTER(L.FrameFmt), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                       C.c_void_p]
-    return lib
-
-
 def _outputs():
     out = torch.full((320, 640, 4), OUT_SENTINEL, dtype=torch.int16, device="cuda")
     u8 = torch.full((320, 640, 3), U8_SENTINEL, dtype=torch.uint8, device="cuda")
@@ -135,7 +125,7 @@ def _outputs():
 def run_op(entry, desc, mode, conv, dtype):
     """vpb_preprocess (packed frames) or vpb_preprocess_fmt of one frame -> (uint16 [320, 640, 4], uint8 [320, 640, 3]);
     desc = (format, ptr, h, w, stride, uv_ptr, uv_stride)"""
-    lib = _op_bind()
+    lib = L.lib()
     out, u8 = _outputs()
     if entry == "packed":
         fmt, ptr, h, w, stride, _, _ = desc
@@ -312,7 +302,7 @@ def test_tap_boundary():
     img, small = frame_and_small(5, h, w, E.RESIZE_PIL_BICUBIC)
     df = DevFrame(img)
     check_op(packed_desc(df, h, w), small, E.RESIZE_PIL_BICUBIC, convs=(E.CONV_BGR_SWAP,))
-    lib = _op_bind()
+    lib = L.lib()
     big = DevFrame(np.zeros((2401, 3 * 4801), np.uint8))
     for bh, bw in BICUBIC_REJECTED:
         for entry in ("packed", "fmt"):

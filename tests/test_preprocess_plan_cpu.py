@@ -84,8 +84,6 @@ def letterbox_plan(h, w):
 
 def _ksize(mode, in_size, out_size):
     lib = L.lib()
-    lib.vpb_resize_tables_host.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                           C.c_int, C.POINTER(C.c_int)]
     bounds = (C.c_int * out_size)()
     coeffs = (C.c_int * (out_size * 64))()
     ks = C.c_int()

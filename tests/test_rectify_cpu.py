@@ -172,8 +172,6 @@ def test_oracle_of_a_camera_native_frame_equals_cvtcolor_then_remap(fmt):
 def test_rectify_create_rejects_bad_arguments_without_a_gpu():
     """Every check runs before the device is opened (a machine without a GPU gets the same messages)."""
     lib = L.lib()
-    lib.vpb_rectify_create.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                       C.POINTER(C.c_void_p)]
     m1 = np.zeros((4, 4, 2), np.int16)
     m2 = np.zeros((4, 4), np.uint16)
     out = C.c_void_p(1)

@@ -66,8 +66,6 @@ def _hw(obj):
 # ------------------------------------------------------------------------------------------------ op level
 def _op(objs, maps, bgr):
     lib = L.lib()
-    lib.vpb_rectify_frames.argtypes = [C.POINTER(L.FrameFmt), C.POINTER(C.c_void_p), C.c_int, C.c_int,
-                                       C.POINTER(C.c_void_p), C.c_void_p]
     rects = [L.Rectify(m1, m2, _hw(o)) for o, (m1, m2) in zip(objs, maps)]
     devs = [_dev_frame(o) for o in objs]
     outs = [torch.full((m1.shape[0], m1.shape[1], 3), 77, dtype=torch.uint8, device="cuda") for m1, _ in maps]
@@ -107,8 +105,6 @@ def test_rectify_frames_mixed_batch_of_formats_and_sizes():
 
 def test_rectify_frames_rejects_a_wrong_source_size():
     lib = L.lib()
-    lib.vpb_rectify_frames.argtypes = [C.POINTER(L.FrameFmt), C.POINTER(C.c_void_p), C.c_int, C.c_int,
-                                       C.POINTER(C.c_void_p), C.c_void_p]
     r = L.Rectify(*R.identity_maps(40, 60), (40, 60))
     out = torch.zeros(40, 60, 3, dtype=torch.uint8, device="cuda")
     arr = L.frame_fmt_descs([(L.PIX_PACKED, out.data_ptr(), 40, 61, 183, 0, 0)])

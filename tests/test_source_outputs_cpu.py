@@ -1,6 +1,5 @@
 """Source-resolution outputs without a GPU: the argument checks of vpb_source_outputs and of vp_engine_create's
-source_outputs flags (both before any device work), the ctypes mirrors of the new structs, and the C++ adapter with
-its source-output constructor argument."""
+source_outputs flags (both before any device work), and the C++ adapter with its source-output constructor argument."""
 import ctypes as C
 import os
 import subprocess
@@ -26,7 +25,6 @@ def _job(**kw):
 
 def _call(jobs, n=None):
     lib = L.lib()
-    lib.vpb_source_outputs.argtypes = [C.POINTER(L.SrcJob), C.c_int, C.c_void_p]
     arr = (L.SrcJob * max(len(jobs), 1))(*jobs)
     return lib.vpb_source_outputs(arr, len(jobs) if n is None else n, None)
 
@@ -69,8 +67,8 @@ def test_fields_an_output_kind_does_not_read_are_not_checked():
 
 
 def _create(kinds, flags):
-    lib = E._bind()
-    cfg = E._Config()
+    lib = L.lib()
+    cfg = L.EngineConfig()
     cfg.n_models = len(kinds)
     for i, k in enumerate(kinds):
         cfg.kinds[i] = k
@@ -99,32 +97,6 @@ def test_python_names_map_to_flags():
     assert E.source_flags(()) == 0
     with pytest.raises(ValueError, match="unknown source output 'masks'"):
         E.source_flags(("masks",))
-
-
-def test_ctypes_mirrors_match_the_headers(tmp_path):
-    mirrors = {"vp_engine_config": E._Config, "vp_source_output": E._SourceOutput, "vpb_src_job": L.SrcJob}
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "vp_b200.h"', 'int main(void) {']
-    for cname, cls in mirrors.items():
-        lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')
-        for fname, _ in cls._fields_:
-            lines.append(f'  printf("{cname}.{fname} %zu\\n", offsetof({cname}, {fname}));')
-    lines.append('  printf("flags %d %d %d %d %d %d %d\\n", VP_SRC_MASK, VP_SRC_DEPTH, VP_SRC_OVERLAY, VPB_SRC_MASK255, '
-                 'VPB_SRC_IDS, VPB_SRC_DEPTH, VPB_SRC_OVERLAY);')
-    lines += ['  return 0;', '}']
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    out = {}
-    for line in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.splitlines():
-        k, *v = line.split()
-        out[k] = v
-    for cname, cls in mirrors.items():
-        assert int(out[cname][0]) == C.sizeof(cls), cname
-        for fname, _ in cls._fields_:
-            assert int(out[f"{cname}.{fname}"][0]) == getattr(cls, fname).offset, f"{cname}.{fname}"
-    assert [int(x) for x in out["flags"]] == [E.SRC_MASK, E.SRC_DEPTH, E.SRC_OVERLAY, L.SRC_MASK255, L.SRC_IDS,
-                                              L.SRC_DEPTH, L.SRC_OVERLAY]
 
 
 def build_source_adapter_check(tmpdir) -> str:

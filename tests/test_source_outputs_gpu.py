@@ -20,18 +20,6 @@ VIZ_NAME = {L.VIZ_SCENE: "scene", L.VIZ_DOMAIN: "domain", L.VIZ_EGOLANES: "egola
 VPB_ERR_ARG, VPB_ERR_STATE = -1, -3
 
 
-def _lib():
-    lib = L.lib()
-    vp, i = C.c_void_p, C.c_int
-    lib.vpb_mask255.argtypes = [vp, i, i, i, vp, vp]
-    lib.vpb_egolanes_ids.argtypes = [vp, i, i, i, vp, vp]
-    lib.vpb_resize_nearest_u8.argtypes = [vp, i, i, vp, i, i, vp]
-    lib.vpb_resize_linear_f32.argtypes = [vp, i, i, vp, i, i, vp]
-    lib.vpb_visualize_mask.argtypes = [vp, i, i, i, vp, i, i, i, vp, i, vp]
-    lib.vpb_source_outputs.argtypes = [C.POINTER(L.SrcJob), i, vp]
-    return lib
-
-
 class _CAI:
     def __init__(self, ptr, shape, typestr, strides):
         self.__cuda_array_interface__ = {"data": (ptr, False), "shape": tuple(shape), "typestr": typestr,
@@ -87,7 +75,7 @@ SIZES = [(1080, 1920), (720, 1280), (660, 1920), (333, 517)]
 
 
 def test_one_launch_equals_the_single_op_chains_and_the_oracle():
-    lib = _lib()
+    lib = L.lib()
     g = torch.Generator().manual_seed(5)
     raw3 = torch.randn(3, 320, 640, generator=g)
     raw3[:, :6, :10] = 0.5                                  # exact ties: first max wins (class 0)
@@ -248,7 +236,7 @@ def _host_descs(eng, fr):
 
 
 def test_engine_outputs_equal_single_ops_host_and_device(ckpts, rig):
-    lib = _lib()
+    lib = L.lib()
     eng = _engine(ckpts, 4)
     plain = _engine(ckpts, 4, src=())
     assert eng.stats()["n_launches"] == plain.stats()["n_launches"] + 1
@@ -285,7 +273,7 @@ def test_adapter_source_mask_and_depth_at_frame_size(ckpts, tmp_path):
 
 
 def test_batch1_plain_and_split_engines(ckpts, rig):
-    lib = _lib()
+    lib = L.lib()
     eng = _engine(ckpts, 4)
     plain = _engine(ckpts, 4, src=())
     eng.infer_frames(rig)
@@ -312,7 +300,7 @@ def test_batch1_plain_and_split_engines(ckpts, rig):
 
 
 def test_graph_repoints_the_overlay_at_new_frames_then_recaptures(ckpts, rig):
-    lib = _lib()
+    lib = L.lib()
     eng = _engine(ckpts, 4)
     other = _rig(seed=10)
     overlays = []
@@ -335,9 +323,9 @@ def test_graph_repoints_the_overlay_at_new_frames_then_recaptures(ckpts, rig):
 
 
 def test_accessor_errors(ckpts, rig):
-    lib = E._bind()
+    lib = L.lib()
     eng = _engine(ckpts, 1, src=("depth", "overlay"))
-    o = E._SourceOutput()
+    o = L.SourceOutput()
     assert lib.vp_engine_source_output(eng.handle, 0, 0, E.SRC_OVERLAY, C.byref(o)) == VPB_ERR_STATE
     assert "run one call first" in L.last_error()
     eng.infer(rig[1])

@@ -5,7 +5,6 @@ Three gates: (1) vpb_upconv_compose's weights and 9-class bias against an fp64 c
 layer definitions, (2) the kernel against an fp32 emulation that uses the SAME 16-bit composed operands (tight: only
 summation order and the final 16-bit rounding differ), (3) the kernel against conv_transpose2d + conv2d with the
 original fp32 parameters (what the reference graph computes; the gap is the 16-bit rounding of the composed weights)."""
-import ctypes as C
 
 import pytest
 import torch
@@ -71,7 +70,6 @@ def _compose_dev(wt, bt, w3, b3, ws, bs):
     b9 = torch.full((9, Cout), float("nan"), device="cuda")
     p = lambda t: t.data_ptr() if t is not None else None
     lib = L.lib()
-    lib.vpb_upconv_compose.argtypes = [C.c_void_p] * 6 + [C.c_int] * 4 + [C.c_void_p] * 4
     L.check(lib.vpb_upconv_compose(p(w3_), p(b3_), p(wt_), p(bt_), p(ws_), p(bs_), Cout, Cmid, Cin, C2,
                                    p(wf), p(w2f), p(b9), None), "vpb_upconv_compose")
     torch.cuda.synchronize()
@@ -131,7 +129,6 @@ def test_upconv_matches_two_layer_reference(H, W, Cin, Cmid, Cout, C2, bn, pads,
     s = torch.randn(2 * H, 2 * W, C2, generator=g).to(td).cuda() if C2 else None
     wf16 = torch.empty(16, Cout, Cin, device="cuda", dtype=td)
     lib = L.lib()
-    lib.vpb_f32_to_16.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]
     L.check(lib.vpb_f32_to_16(dtype, wf.data_ptr(), wf16.data_ptr(), wf.numel(), None), "vpb_f32_to_16")
     torch.cuda.synchronize()
     assert torch.equal(wf16, wf.to(td))

@@ -1,6 +1,6 @@
-"""Per-model input views (vp_engine_set_view) without a GPU: the new C symbols exist, vp_view's layout matches its ctypes
-mirror, a C caller compiles against the header with -Werror, the checks that need no engine return VPB_ERR_ARG with
-their message, and the Python engine rejects bad arguments before it calls the library."""
+"""Per-model input views (vp_engine_set_view) without a GPU: the new C symbols exist, a C caller compiles against the
+header with -Werror, the checks that need no engine return VPB_ERR_ARG with their message, and the Python engine rejects
+bad arguments before it calls the library."""
 import ctypes as C
 import os
 import subprocess
@@ -34,22 +34,8 @@ def test_a_c_caller_compiles_with_werror(tmp_path, std):
                     str(src), "-o", str(tmp_path / "view.o")], check=True)
 
 
-def test_view_layout_matches_the_ctypes_mirror(tmp_path):
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "vp_b200.h"\n'
-                   "int main(void) {\n"
-                   '  printf("%zu %zu %zu %zu\\n", sizeof(vp_view), offsetof(vp_view, convention), offsetof(vp_view, roi),\n'
-                   "         sizeof(((vp_view*)0)->roi));\n"
-                   "  return 0;\n}\n")
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-std=c11", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)],
-                   check=True)
-    got = [int(v) for v in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-    assert got == [C.sizeof(E.View), E.View.convention.offset, E.View.roi.offset, C.sizeof(C.c_int) * 4 * E.MAX_BATCH]
-
-
 def test_null_engine_is_rejected():
-    lib = E._bind()
+    lib = L.lib()
     v = E.View()
     assert lib.vp_engine_set_view(None, 0, C.byref(v)) == VPB_ERR_ARG
     assert "vp_engine_set_view: NULL engine" in L.last_error()

@@ -1,7 +1,6 @@
 """Camera-native YUV frames (NV12, UYVY, YUYV) on the GPU: the conversion inside the pre-process must give, byte for
 byte, what the packed path gives on cv2.cvtColor of the frame, for the op, both engines, every entry point, the graph
 and the split-fp16 mode."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -80,7 +79,6 @@ def _resize_u8(img, mode):
 
 def _run_op(desc, mode, conv, dtype):
     lib = L.lib()
-    lib.vpb_preprocess_fmt.argtypes = [C.POINTER(L.FrameFmt), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     out = torch.full((320, 640, 4), 7, dtype=torch.int16, device="cuda")
     u8 = torch.full((320, 640, 3), 77, dtype=torch.uint8, device="cuda")
     arr = L.frame_fmt_descs([desc])
@@ -91,8 +89,6 @@ def _run_op(desc, mode, conv, dtype):
 
 def _run_packed_op(img, mode, conv, dtype):
     lib = L.lib()
-    lib.vpb_preprocess.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
-                                   C.c_void_p, C.c_void_p]
     h, w, _ = img.shape
     t = torch.from_numpy(np.ascontiguousarray(img)).cuda()
     out = torch.full((320, 640, 4), 7, dtype=torch.int16, device="cuda")

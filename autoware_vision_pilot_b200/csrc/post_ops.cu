@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include <cstring>
 #include "ops_internal.h"
+#include <climits>
 #include <cmath>
 #include <algorithm>
 #include <set>
@@ -44,7 +45,7 @@ __global__ void egolanes_ids_kernel(const float* __restrict__ in, uint8_t* __res
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= rows * cols) return;
   if (channels >= 3) {
-    const int HW = rows * cols;
+    const size_t HW = static_cast<size_t>(rows) * cols;
     const bool b0 = in[idx] > 0.f, b1 = in[HW + idx] > 0.f, b2 = in[2 * HW + idx] > 0.f;
     out[idx] = b2 ? 2 : b1 ? 1 : b0 ? 0 : 255;
   } else {
@@ -251,6 +252,62 @@ __global__ void __launch_bounds__(128) source_outputs_kernel(const __grid_consta
 // (SURVEY §8a P9: cond 1e5..2.5e6 in raw pixels), the solution is mapped back to raw-y coefficients.
 // Lanes accumulate the moment sums, a shuffle tree reduces them (fixed order => reproducible),
 // lane 0 solves the (order+1)^2 system with partially pivoted Gaussian elimination.
+// A set with fewer distinct y than unknowns (all points on one or two pixel rows) is rank-deficient: every
+// solution takes the mean x of each distinct row there, and the fit returned is the one of least norm in the raw
+// y basis, which is what cv::solve(DECOMP_SVD) gives (lane_filter.cpp:96-101).
+
+// Minimum-norm c (c[p] multiplies y^p, p <= order) with sum_p c[p] yv[i]^p = mu[i] for the k < order + 1 distinct
+// rows yv[0] < .. < yv[k-1].  The constraints are restated on the divided differences of the rows (row 0, then
+// [y0, y1], [y0, y1, y2]): same solution set, but the basis vectors stay far from parallel for neighbouring rows
+// (V(74) and V(75) are 2e-4 apart in angle; V(74) and V[74, 75] are not), and the k <= 3 of them are orthonormalised by
+// Gram-Schmidt run twice, so the solve loses ~cond(basis) * eps instead of the square of the raw rows' condition.
+__device__ void min_norm_fit(const double* yv, const double* mu, int k, int order, double c[4]) {
+  const int m = order + 1;
+  double pw[3][4];                                       // pw[i][e] = yv[i]^e
+  for (int i = 0; i < 3; ++i) {
+    pw[i][0] = 1.0;
+    for (int e = 1; e < 4; ++e) pw[i][e] = i < k ? pw[i][e - 1] * yv[i] : 0.0;
+  }
+  double b[3][4] = {}, nu[3] = {};
+  for (int p = 0; p < m; ++p) {
+    b[0][p] = pw[0][p];                                  // h_p(y0) = y0^p
+    if (k > 1)                                           // h_{p-1}(y0, y1) = sum_{a+e=p-1} y0^a y1^e
+      for (int a = 0; a < p; ++a) b[1][p] += pw[0][a] * pw[1][p - 1 - a];
+    if (k > 2)                                           // h_{p-2}(y0, y1, y2)
+      for (int a = 0; a + 1 < p; ++a)
+        for (int e = 0; a + e + 1 < p; ++e) b[2][p] += pw[0][a] * pw[1][e] * pw[2][p - 2 - a - e];
+  }
+  nu[0] = mu[0];
+  if (k > 1) nu[1] = (mu[1] - mu[0]) / (yv[1] - yv[0]);
+  if (k > 2) nu[2] = ((mu[2] - mu[1]) / (yv[2] - yv[1]) - nu[1]) / (yv[2] - yv[0]);
+  // basis^T = Q R, then c = Q z with R^T z = nu
+  double q[3][4] = {}, R[3][3] = {}, z[3] = {};
+  for (int i = 0; i < k; ++i) {
+    double v[4];
+    for (int p = 0; p < 4; ++p) v[p] = b[i][p];
+    for (int rep = 0; rep < 2; ++rep)
+      for (int j = 0; j < i; ++j) {
+        double d = 0.0;
+        for (int p = 0; p < m; ++p) d += q[j][p] * v[p];
+        R[j][i] += d;
+        for (int p = 0; p < m; ++p) v[p] -= d * q[j][p];
+      }
+    double nrm = 0.0;
+    for (int p = 0; p < m; ++p) nrm += v[p] * v[p];
+    R[i][i] = sqrt(nrm);
+    for (int p = 0; p < m; ++p) q[i][p] = v[p] / R[i][i];
+  }
+  for (int i = 0; i < k; ++i) {
+    double v = nu[i];
+    for (int j = 0; j < i; ++j) v -= R[j][i] * z[j];
+    z[i] = v / R[i][i];
+  }
+  for (int p = 0; p < 4; ++p) {
+    c[p] = 0.0;
+    for (int i = 0; i < k; ++i) c[p] += z[i] * q[i][p];
+  }
+}
+
 __global__ void __launch_bounds__(128) polyfit_kernel(const float* __restrict__ xs, const float* __restrict__ ys,
                                                        const int* __restrict__ offsets, int n_sets, int order,
                                                        double* __restrict__ coeffs, double* __restrict__ yrange) {
@@ -270,6 +327,59 @@ __global__ void __launch_bounds__(128) polyfit_kernel(const float* __restrict__ 
   if (lane == 0 && yrange) { yrange[2 * set] = ymin; yrange[2 * set + 1] = ymax; }
   if (n <= order) {   // fitPolySimple returns {} (lane_filter.cpp:61); fitQuadPoly returns NaNs (poly_fit.cpp:42-47)
     if (lane == 0) for (int k = 0; k < 4; ++k) out[k] = nan("");
+    return;
+  }
+  // distinct y values, up to m of them: each lane keeps the first m distinct values it reads, a butterfly merges the
+  // lists; afterwards every lane holds min(m, number of distinct values) of them (all of them when there are fewer)
+  float dv[4] = {0.f, 0.f, 0.f, 0.f};
+  int nd = 0;
+  for (int i = beg + lane; i < end && nd < m; i += 32) {
+    const float y = ys[i];
+    bool seen = false;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) seen |= q < nd && dv[q] == y;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) if (!seen && q == nd) dv[q] = y;
+    nd += !seen;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    float pv[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) pv[q] = __shfl_xor_sync(0xffffffffu, dv[q], o);
+    const int pn = __shfl_xor_sync(0xffffffffu, nd, o);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      bool seen = r >= pn || nd >= m;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) seen |= q < nd && dv[q] == pv[r];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) if (!seen && q == nd) dv[q] = pv[r];
+      nd += !seen;
+    }
+  }
+  if (nd < m) {
+    // rank-deficient: the per-row means of x, then the minimum-norm fit through them (min_norm_fit)
+    double yv[3] = {0, 0, 0};
+    for (int q = 0; q < nd; ++q) yv[q] = dv[q];
+    for (int a = 0; a < nd; ++a)                         // ascending rows (nd <= 3)
+      for (int e = a + 1; e < nd; ++e)
+        if (yv[e] < yv[a]) { const double t = yv[a]; yv[a] = yv[e]; yv[e] = t; }
+    double sx[3] = {0, 0, 0}, cn[3] = {0, 0, 0};
+    for (int i = beg + lane; i < end; i += 32) {
+      const double y = ys[i];
+      for (int q = 0; q < nd; ++q)
+        if (y == yv[q]) { sx[q] += xs[i]; cn[q] += 1.0; }
+    }
+    for (int q = 0; q < 3; ++q)
+      for (int o = 16; o > 0; o >>= 1) {
+        sx[q] += __shfl_xor_sync(0xffffffffu, sx[q], o);
+        cn[q] += __shfl_xor_sync(0xffffffffu, cn[q], o);
+      }
+    if (lane != 0) return;
+    double mu[3] = {0, 0, 0}, c[4];
+    for (int q = 0; q < nd; ++q) mu[q] = sx[q] / cn[q];
+    min_norm_fit(yv, mu, nd, order, c);
+    for (int k = 0; k < 4; ++k) out[k] = (k < m) ? c[order - k] : 0.0;
     return;
   }
   const double mid = 0.5 * (ymin + ymax);
@@ -330,7 +440,9 @@ __global__ void bayes_fuse_kernel(double* __restrict__ state, const double* __re
       const double m0 = state[2 * i], v0 = state[2 * i + 1];
       const double m1 = z[2 * i], v1 = z[2 * i + 1];
       if (isnan(m1)) { state[2 * i + 1] = v0 * 1.25; continue; }
-      state[2 * i] = (m0 * v1 + m1 * v0) / (v0 + v1);
+      // (m0*v1 + m1*v0) / (v0 + v1), with the one fused multiply-add spelled out that nvcc's default contraction made of
+      // it, so the rounding is the source's and not the compiler's choice
+      state[2 * i] = fma(m1, v0, m0 * v1) / (v0 + v1);
       state[2 * i + 1] = (v0 * v1) / (v0 + v1);
     }
     for (int r = 0; r < 3; ++r) {
@@ -437,34 +549,57 @@ double source_outputs_bytes(const vpb_src_job* jobs, int n) {
 
 using namespace vpb;
 
+// rows * cols pixels of a mask op as an int (VPB_ERR_ARG, naming the call, outside 1..INT_MAX)
+static int mask_pixels(const char* who, int rows, int cols, int* n) {
+  const long long px = static_cast<long long>(rows) * cols;
+  if (rows <= 0 || cols <= 0 || px > INT_MAX) { vpb_set_error("%s: bad size %d x %d", who, rows, cols); return VPB_ERR_ARG; }
+  *n = static_cast<int>(px);
+  return VPB_OK;
+}
+static int resize_size_ok(const char* who, int sh, int sw, int dh, int dw) {
+  if (sh <= 0 || sw <= 0 || dh <= 0 || dw <= 0 || dh > 65535) {   // dh is the grid's y extent
+    vpb_set_error("%s: bad size %dx%d -> %dx%d", who, sh, sw, dh, dw);
+    return VPB_ERR_ARG;
+  }
+  return VPB_OK;
+}
+static unsigned blocks_of(int n, int per) { return static_cast<unsigned>((static_cast<long long>(n) + per - 1) / per); }
+
 extern "C" int vpb_mask255(const float* raw, int channels, int rows, int cols, uint8_t* out, void* stream) {
-  const int n = rows * cols;
-  mask255_kernel<<<(n + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(raw, out, rows, cols, channels);
+  int n = 0;
+  const int rc = mask_pixels("vpb_mask255", rows, cols, &n);
+  if (rc) return rc;
+  mask255_kernel<<<blocks_of(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(raw, out, rows, cols, channels);
   VPB_CUDA_OK(cudaGetLastError());
   return VPB_OK;
 }
 extern "C" int vpb_egolanes_ids(const float* raw, int channels, int rows, int cols, uint8_t* out, void* stream) {
-  const int n = rows * cols;
-  egolanes_ids_kernel<<<(n + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(raw, out, rows, cols, channels);
+  int n = 0;
+  const int rc = mask_pixels("vpb_egolanes_ids", rows, cols, &n);
+  if (rc) return rc;
+  egolanes_ids_kernel<<<blocks_of(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(raw, out, rows, cols, channels);
   VPB_CUDA_OK(cudaGetLastError());
   return VPB_OK;
 }
 extern "C" int vpb_lane_masks(const float* raw, int n, float threshold, float* out, void* stream) {
-  lane_masks_kernel<<<(n + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(raw, out, n, threshold);
+  if (n <= 0) { vpb_set_error("vpb_lane_masks: n = %d values", n); return VPB_ERR_ARG; }
+  lane_masks_kernel<<<blocks_of(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(raw, out, n, threshold);
   VPB_CUDA_OK(cudaGetLastError());
   return VPB_OK;
 }
 extern "C" int vpb_resize_nearest_u8(const uint8_t* src, int sh, int sw, uint8_t* dst, int dh, int dw, void* stream) {
-  if (sh <= 0 || sw <= 0 || dh <= 0 || dw <= 0) { vpb_set_error("resize: bad size"); return VPB_ERR_ARG; }
+  const int rc = resize_size_ok("vpb_resize_nearest_u8", sh, sw, dh, dw);
+  if (rc) return rc;
   const double ifx = 1.0 / (static_cast<double>(dw) / sw), ify = 1.0 / (static_cast<double>(dh) / sh);
-  dim3 grid((dw + 255) / 256, dh);
+  dim3 grid(blocks_of(dw, 256), dh);
   resize_nearest_u8_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(src, sh, sw, dst, dh, dw, ify, ifx);
   VPB_CUDA_OK(cudaGetLastError());
   return VPB_OK;
 }
 extern "C" int vpb_resize_linear_f32(const float* src, int sh, int sw, float* dst, int dh, int dw, void* stream) {
-  if (sh <= 0 || sw <= 0 || dh <= 0 || dw <= 0) { vpb_set_error("resize: bad size"); return VPB_ERR_ARG; }
-  dim3 grid((dw + 255) / 256, dh);
+  const int rc = resize_size_ok("vpb_resize_linear_f32", sh, sw, dh, dw);
+  if (rc) return rc;
+  dim3 grid(blocks_of(dw, 256), dh);
   resize_linear_f32_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       src, sh, sw, dst, dh, dw, static_cast<double>(sh) / dh, static_cast<double>(sw) / dw);
   VPB_CUDA_OK(cudaGetLastError());
@@ -473,8 +608,9 @@ extern "C" int vpb_resize_linear_f32(const float* src, int sh, int sw, float* ds
 extern "C" int vpb_visualize_mask(const uint8_t* mask, int mh, int mw, int viz_type, const uint8_t* frame_bgr, int h, int w,
                                   int stride, uint8_t* out, int out_stride, void* stream) {
   if (!mask || !frame_bgr || !out || mh <= 0 || mw <= 0 || h <= 0 || w <= 0 || stride < 3 * w || out_stride < 3 * w ||
-      viz_type < VPB_VIZ_SCENE || viz_type > VPB_VIZ_EGOLANES) {
-    vpb_set_error("visualize_mask: bad arguments");
+      h > 65535 || viz_type < VPB_VIZ_SCENE || viz_type > VPB_VIZ_EGOLANES) {   // h is the grid's y extent
+    vpb_set_error("vpb_visualize_mask: bad arguments (%dx%d mask, %dx%d frame, strides %d / %d, viz_type %d)", mh, mw, h,
+                  w, stride, out_stride, viz_type);
     return VPB_ERR_ARG;
   }
   const int rc = vpb::viz_tables_init();
@@ -496,8 +632,12 @@ extern "C" int vpb_source_outputs(const vpb_src_job* jobs, int n, void* stream) 
 }
 extern "C" int vpb_polyfit(const float* xs, const float* ys, const int* offsets, int n_sets, int order,
                            double* coeffs, double* yrange, void* stream) {
-  if (order < 1 || order > 3 || n_sets < 0) { vpb_set_error("polyfit: order must be 1..3"); return VPB_ERR_ARG; }
+  if (order < 1 || order > 3 || n_sets < 0) {
+    vpb_set_error("vpb_polyfit: order %d (1..3), %d sets", order, n_sets);
+    return VPB_ERR_ARG;
+  }
   if (n_sets == 0) return VPB_OK;
+  if (!xs || !ys || !offsets || !coeffs) { vpb_set_error("vpb_polyfit: NULL pointer"); return VPB_ERR_ARG; }
   const int warps_per_block = 4;
   polyfit_kernel<<<(n_sets + warps_per_block - 1) / warps_per_block, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       xs, ys, offsets, n_sets, order, coeffs, yrange);
@@ -505,6 +645,10 @@ extern "C" int vpb_polyfit(const float* xs, const float* ys, const int* offsets,
   return VPB_OK;
 }
 extern "C" int vpb_bayes_fuse(double* state, const double* meas, int n_meas, void* stream) {
+  if (!state || (!meas && n_meas > 0) || n_meas < 0) {
+    vpb_set_error("vpb_bayes_fuse: %s", n_meas < 0 ? "n_meas < 0" : "NULL pointer");
+    return VPB_ERR_ARG;
+  }
   bayes_fuse_kernel<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(state, meas, n_meas);
   VPB_CUDA_OK(cudaGetLastError());
   return VPB_OK;

@@ -10,7 +10,8 @@
   `LaneTracker::fitPoly2ndOrder` (src/lane_tracking/lane_tracking.cpp:350-404),
   `fitQuadPoly` (src/path_planning/poly_fit.cpp:36-75, Eigen colPivHouseholderQr): all three solve
   min || A c - x ||  with A = Vandermonde(y) in fp64; restated with numpy.linalg.lstsq (SVD), pinned
-  against cv2.solve(DECOMP_SVD) on the same matrices.
+  against cv2.solve(DECOMP_SVD) on the same matrices.  polyfit_exact is the same solution in exact rational
+  arithmetic, the minimum-norm one on rank-deficient point sets, as the reference for the kernel's tests.
 * `Estimator::update` (production_release/src/path_planning/estimator.cpp:24-74) with PathFinder's
   fusion groups (path_finder.cpp:24-30) and the measurement construction of
   PathFinder::update (path_finder.cpp:97-157).
@@ -70,6 +71,54 @@ def polyfit(xs, ys, order: int) -> np.ndarray:
         return np.full(order + 1, np.nan)
     A = np.stack([ys ** (order - k) for k in range(order + 1)], axis=1)
     return np.linalg.lstsq(A, xs, rcond=None)[0]
+
+
+def _solve_exact(A, b):
+    """A x = b for a square non-singular Fraction matrix, by Gaussian elimination (exact)."""
+    m = len(A)
+    M = [list(A[i]) + [b[i]] for i in range(m)]
+    for c in range(m):
+        piv = next(i for i in range(c, m) if M[i][c] != 0)
+        M[c], M[piv] = M[piv], M[c]
+        for i in range(m):
+            if i != c and M[i][c] != 0:
+                f = M[i][c] / M[c][c]
+                M[i] = [a - f * p for a, p in zip(M[i], M[c])]
+    return [M[i][m] / M[i][i] for i in range(m)]
+
+
+def polyfit_exact(xs, ys, order: int) -> np.ndarray:
+    """The least-squares solution of polyfit() in exact rational arithmetic, rounded once to fp64 at the end
+    (highest power first; NaNs if n <= order).  The inputs are taken as the exact rationals their float values are.
+
+    Full rank (at least order + 1 distinct y): the normal equations in the raw power basis.  Rank-deficient (fewer
+    distinct y than unknowns, e.g. every point on one or two pixel rows): every solution fits the mean x of each
+    distinct row exactly, and the one of least norm, which cv::solve(DECOMP_SVD) returns, is c = V^T (V V^T)^-1 mu
+    with V the raw-basis rows at the distinct y values and mu the per-row means of x."""
+    from fractions import Fraction
+    xs = [Fraction(float(v)) for v in np.asarray(xs, dtype=np.float64).ravel()]
+    ys = [Fraction(float(v)) for v in np.asarray(ys, dtype=np.float64).ravel()]
+    m = order + 1
+    if len(xs) <= order:
+        return np.full(m, np.nan)
+    rows = sorted(set(ys))
+    if len(rows) >= m:
+        pw = [[y ** p for p in range(2 * order + 1)] for y in ys]
+        s = [sum(p[k] for p in pw) for k in range(2 * order + 1)]
+        r = [sum(x * p[k] for x, p in zip(xs, pw)) for k in range(m)]
+        # unknowns c_0..c_order multiply y^(order-j): (A^T A)_ij = sum y^(2*order-i-j), (A^T x)_i = sum x y^(order-i)
+        G = [[s[2 * order - i - j] for j in range(m)] for i in range(m)]
+        c = _solve_exact(G, [r[order - i] for i in range(m)])
+    else:
+        V = [[y ** (order - j) for j in range(m)] for y in rows]
+        mu = []
+        for y in rows:
+            sel = [x for x, yy in zip(xs, ys) if yy == y]
+            mu.append(sum(sel) / len(sel))
+        G = [[sum(a * b for a, b in zip(V[i], V[j])) for j in range(len(rows))] for i in range(len(rows))]
+        lam = _solve_exact(G, mu)
+        c = [sum(lam[i] * V[i][j] for i in range(len(rows))) for j in range(m)]
+    return np.array([float(v) for v in c])
 
 
 def fit_poly_2nd_order(xs, ys) -> np.ndarray:

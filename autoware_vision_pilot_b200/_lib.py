@@ -346,7 +346,8 @@ class EngineConfig(C.Structure):
     _fields_ = [("gpu_id", C.c_int), ("dtype", C.c_int), ("resize_mode", C.c_int), ("convention", C.c_int),
                 ("n_models", C.c_int), ("kinds", C.c_int * 4), ("weights", C.c_char_p * 4),
                 ("fetch_raw", C.c_int), ("use_graph", C.c_int), ("stream", C.c_void_p),
-                ("single_stream", C.c_int), ("precision", C.c_int), ("batch", C.c_int), ("source_outputs", C.c_int)]
+                ("single_stream", C.c_int), ("precision", C.c_int), ("batch", C.c_int), ("source_outputs", C.c_int),
+                ("cameras", C.c_int * 4)]
 
 
 class Output(C.Structure):
@@ -426,6 +427,7 @@ SIGNATURES = {
     "vp_engine_set_view": (i, [vp, i, P(View)]),
     "vp_engine_read_resized_view": (i, [vp, i, i, vp]),
     "vp_engine_set_detector": (i, [vp, vp]),
+    "vp_engine_set_detector_cameras": (i, [vp, vp, i]),
     "vp_engine_set_lateral": (i, [vp, i, P(LateralConfig)]),
     "vp_engine_set_steering": (i, [vp, vp]),
     "vp_engine_lateral_reset": (i, [vp, i]),

@@ -84,10 +84,12 @@ struct vp_engine : EngineRuntime {
   // SE pooling accumulators of every MBConv block: one arena, one accumulator set per sample of the batch.  Its used
   // extent is what a call zeroes (EngineRuntime::call_zero, call_zero_bytes).
   static constexpr size_t kGapCap = 512 * 1024;  // int64 slots per sample (16 blocks x <=1152 ch x 8 replicas per encoder)
+  // (`batch` is the model's own while a model with a camera set is built; the arena holds the engine's every sample)
   long long* gap_alloc(int C) {
-    if (!call_zero) call_zero = dalloc(kGapCap * batch * 8, false);
+    const size_t cap = kGapCap * std::max(cfg.batch, 1);
+    if (!call_zero) call_zero = dalloc(cap * 8, false);
     const size_t need = static_cast<size_t>(C) * kGapReplicas * batch, used = call_zero_bytes / 8;
-    if (used + need > kGapCap * batch) return nullptr;
+    if (used + need > cap) return nullptr;
     call_zero_bytes += (need + 31) / 32 * 32 * 8;
     return static_cast<long long*>(call_zero) + used;
   }
@@ -125,8 +127,19 @@ struct vp_engine : EngineRuntime {
   struct Input { const void* p = nullptr; const void* lo = nullptr; };
   std::array<Input, VP_MAX_MODELS> input{};
   std::vector<uint64_t> enc_hash;          // [model] hash of its encoder's weights (equal: the encoder is shared)
+  std::vector<int> enc_owner;              // [model] the model that built its encoder (itself, or one it shares with)
+  // Camera sets (vp_engine_config.cameras): [model] bit k = sample k, 0 = every sample.  Model m holds model_batch(m)
+  // samples, slot j = sample camera_sample(cams[m], j).  det_cams: the attached detector's.
+  int cams[VP_MAX_MODELS] = {};
+  int det_cams = 0;
+  int model_batch(int m) const { return cams[m] ? __builtin_popcount(cams[m]) : batch; }
+  // model m makes its network input with an op of its own, "preprocess/<m>": it has a view or a camera set, and it
+  // built its encoder (a model sharing it reads the builder's input)
+  bool own_pre(int m) const { return enc_owner[m] == m && (views[m].on || cams[m]); }
   // A model's own region and convention of every sample's full() frame (vp_engine_set_view): op "preprocess/<m>" before
-  // the model's stem, on its lane, into its own network input and resized image (allocated on the first set, kept).
+  // the model's stem, on its lane, into its own network input and resized image (allocated on the first set, kept).  A
+  // model with a camera set has the op and the buffers without a view too (on = false: it reads every sample's pre() in
+  // the engine's convention).  roi is indexed by sample, plan, geom and the buffers by the model's slot.
   struct View {
     bool on = false;
     int convention = 0;
@@ -474,6 +487,9 @@ static void build_model(vp_engine& e, NetBuilder& b, int idx, int kind) {
   const auto it = e.trunk_cache.find(h_trunk);
   // the model's lane starts after the op producing its input: a shared neck, a shared encoder, or the pre-process (op 0)
   e.begin_lane(idx, it != e.trunk_cache.end() ? e.trunk_last_op[h_trunk] : ie != e.enc_cache.end() ? e.enc_last_op[h_enc] : 0);
+  e.enc_owner.push_back(idx);
+  for (int j = 0; j < idx; ++j)
+    if (e.enc_hash[j] == h_enc) { e.enc_owner.back() = e.enc_owner[j]; break; }
   e.enc_hash.push_back(h_enc);
   e.input[idx] = {e.d_pre, e.d_pre_lo};
   e.tap(tag + "pre", e.taps["pre"].t, 3);
@@ -544,11 +560,11 @@ static int build_source_outputs(vp_engine& e) {
   for (int m = 0; m < static_cast<int>(e.outs.size()); ++m) {
     const ModelOut& mo = e.outs[m];
     const size_t plane = static_cast<size_t>(mo.H) * mo.W;
-    for (int k = 0; k < e.batch; ++k)
+    for (int k = 0; k < e.model_batch(m); ++k)     // slot k of the model
       for (int flag : kFlags) {
         if (!(e.cfg.source_outputs & flag)) continue;
         SrcOut so;
-        so.model = m; so.sample = k; so.flag = flag;
+        so.model = m; so.sample = camera_sample(e.cams[m], k); so.flag = flag;
         vpb_src_job& j = so.job;
         j.sh = mo.H; j.sw = mo.W;
         if (mo.kind == VP_SCENE_3D) {
@@ -598,27 +614,74 @@ static int check_source_flags(const vp_engine_config& c) {
   return VPB_OK;
 }
 
+// The camera sets of c into cams, a set of every sample as 0 (none).  VPB_ERR_ARG naming the model for a bit at or above
+// the batch (host-only, before the device is opened; a batch out of range is reported by the create call).
+static int camera_sets(const vp_engine_config& c, int* cams) {
+  if (c.batch < 0 || c.batch > VP_MAX_BATCH) return VPB_OK;
+  const int nb = c.batch > 1 ? c.batch : 1, all = (1 << nb) - 1;
+  for (int i = 0; i < c.n_models; ++i) {
+    if (c.cameras[i] & ~all) {
+      vpb_set_error("vp_engine_create: model %d: cameras 0x%x has a bit at or above the batch %d", i,
+                    static_cast<unsigned>(c.cameras[i]), nb);
+      return VPB_ERR_ARG;
+    }
+    cams[i] = c.cameras[i] == all ? 0 : c.cameras[i];
+  }
+  return VPB_OK;
+}
+
+// With a camera set: every model's weights into w, before the device is opened, and VPB_ERR_ARG naming both models for
+// two models that share an encoder (byte-identical encoder weights, the rule of build_model and vp_engine_set_view) on
+// different sets.
+static int load_weights_for_sets(const vp_engine_config& c, const int* cams, std::vector<WeightMap>& w) {
+  bool any = false;
+  for (int i = 0; i < c.n_models; ++i) any |= cams[i] != 0;
+  if (!any) return VPB_OK;
+  w.resize(c.n_models);
+  std::vector<uint64_t> h(c.n_models);
+  for (int i = 0; i < c.n_models; ++i) {
+    if (!c.weights[i] || !c.weights[i][0]) {
+      vpb_set_error("No path to checkpoint file provided for model %d", i);
+      return VPB_ERR_ARG;
+    }
+    const int rc = load_vpw(c.weights[i], w[i]);
+    if (rc) return rc;
+    h[i] = hash_prefix(w[i], prefixes_for(c.kinds[i]).enc);
+    for (int j = 0; j < i; ++j)
+      if (h[j] == h[i] && cams[j] != cams[i]) {
+        vpb_set_error("vp_engine_create: model %d shares its encoder with model %d, but its cameras 0x%x differ from "
+                      "model %d's 0x%x (models that share an encoder share their camera set)", i, j,
+                      static_cast<unsigned>(c.cameras[i]), j, static_cast<unsigned>(c.cameras[j]));
+        return VPB_ERR_ARG;
+      }
+  }
+  return VPB_OK;
+}
+
 }  // namespace vpb
 
 // Every frame resizes to the 640 x 320 network input: VPB_ERR_ARG (naming `who` and the frame) if one cannot in the
 // engine's resize mode, or if the engine makes overlays and the frame is not packed (the overlay blends the camera
 // frame's pixels as vpb_src_job reads them; a rectified sample's frame here is the packed rectified frame).  With a
-// detector, its letterboxes of the full frames.  Each view's regions pass region_check and resize likewise (the view
-// geometries of the call).  Host-only: callers run it before any device work.
+// detector, its letterboxes of the full frames of its samples.  Each view's regions pass region_check and resize likewise
+// (the geometries of a model's own pre-process, slot by slot, for the samples of its camera set).  Host-only: callers
+// run it before any device work.
 int vp_engine::geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, const char* who, PreGeom* g) {
   for (int m = 0; m < static_cast<int>(outs.size()); ++m) {
     View& v = views[m];
-    for (int k = 0; k < batch && v.on; ++k) {
-      if (region_check(full[k], v.roi[k], m, who, k)) return VPB_ERR_ARG;
-      const vpb_frame_fmt f = crop_frame(full[k], v.roi[k]);
-      v.geom[k] = PreGeom{};
-      v.geom[k].h = f.h; v.geom[k].w = f.w;
-      const int rc = PreprocessPlan::check(v.geom[k], cfg.resize_mode, who, k);
+    for (int j = 0; j < model_batch(m) && own_pre(m); ++j) {
+      const int k = camera_sample(cams[m], j);
+      if (v.on && region_check(full[k], v.roi[k], m, who, k)) return VPB_ERR_ARG;
+      const vpb_frame_fmt f = v.on ? crop_frame(full[k], v.roi[k]) : frames[k];
+      v.geom[j] = PreGeom{};
+      v.geom[j].h = f.h; v.geom[j].w = f.w;
+      const int rc = PreprocessPlan::check(v.geom[j], cfg.resize_mode, who, k);
       if (rc) return rc;
     }
   }
   for (int k = 0; k < batch; ++k) {
-    const int lat_h = lat_model < 0 ? 0 : views[lat_model].on ? views[lat_model].geom[k].h : frames[k].h;
+    const int lat_slot = lat_model < 0 ? -1 : camera_slot(cams[lat_model], k);
+    const int lat_h = lat_slot < 0 ? 0 : views[lat_model].on ? views[lat_model].geom[lat_slot].h : frames[k].h;
     if (lat_h > kLatMaxImgH) {
       vpb_set_error("%s: frame %d: height %d is above the %d rows the lateral post-process takes", who, k, lat_h,
                     kLatMaxImgH);
@@ -634,7 +697,10 @@ int vp_engine::geoms(const vpb_frame_fmt* frames, const vpb_frame_fmt* full, con
     const int rc = PreprocessPlan::check(g[k], cfg.resize_mode, who, k);
     if (rc) return rc;
   }
-  return det ? autospeed_geoms(det, full, who, det_geom) : VPB_OK;
+  if (!det) return VPB_OK;
+  Frames df{};
+  for (int j = 0; j < autospeed_runtime(det)->batch; ++j) df[j] = full[camera_sample(det_cams, j)];
+  return autospeed_geoms(det, df.data(), who, det_geom);
 }
 
 // Enqueue one call's kernels for the batch frames of the call (graph replay when enabled and the geometries are
@@ -645,17 +711,19 @@ int vp_engine::enqueue(const PreGeom* g) {
   int rc = pre.configure(g, batch, cfg.resize_mode);
   for (int m = 0; m < static_cast<int>(outs.size()) && rc == VPB_OK; ++m) {
     View& v = views[m];
-    if (!v.on) continue;
-    rc = v.plan.configure(v.geom, batch, cfg.resize_mode);
+    if (!own_pre(m)) continue;
+    rc = v.plan.configure(v.geom, model_batch(m), cfg.resize_mode);
     double bytes = 0;   // as "preprocess": frame read + 3 x OH x OW 16-bit written, per sample
-    for (int k = 0; k < batch; ++k) bytes += frame_bytes(input_frame(m, k)) + 2.0 * 3 * v.geom[k].OH * v.geom[k].OW;
+    for (int j = 0; j < model_batch(m); ++j)
+      bytes += frame_bytes(input_frame(m, camera_sample(cams[m], j))) + 2.0 * 3 * v.geom[j].OH * v.geom[j].OW;
     ops[op_index(("preprocess/" + std::to_string(m)).c_str())].bytes = bytes;
   }
   if (rc == VPB_OK && !src_outs.empty()) rc = prepare_source(*this);
   if (rc == VPB_OK && det) {
     rc = autospeed_prepare(det, det_geom, stream);
     double bytes = 0;   // as the detector's own pre-process: frame read + 3 x OH x OW 16-bit written, per sample
-    for (int k = 0; k < batch; ++k) bytes += frame_bytes(chain[k].full()) + 2.0 * 3 * det_geom[k].OH * det_geom[k].OW;
+    for (int j = 0; j < autospeed_runtime(det)->batch; ++j)
+      bytes += frame_bytes(chain[camera_sample(det_cams, j)].full()) + 2.0 * 3 * det_geom[j].OH * det_geom[j].OW;
     ops[op_index("det/letterbox")].bytes = bytes;
   }
   if (rc == VPB_OK) rc = run_call();
@@ -666,7 +734,7 @@ int vp_engine::enqueue(const PreGeom* g) {
 
 // mo's class map, if it has one, and with_raw its raw tensor to the pinned host buffers
 static int fetch_out(const vp_engine& e, const ModelOut& mo, bool with_raw) {
-  const size_t plane = static_cast<size_t>(mo.H) * mo.W * e.batch;
+  const size_t plane = static_cast<size_t>(mo.H) * mo.W * e.model_batch(static_cast<int>(&mo - e.outs.data()));
   if (mo.has_cls) VPB_CUDA_OK(cudaMemcpyAsync(mo.h_cls, mo.d_cls, plane, cudaMemcpyDeviceToHost, e.stream));
   if (with_raw) VPB_CUDA_OK(cudaMemcpyAsync(mo.h_raw, mo.d_raw, plane * mo.C * 4, cudaMemcpyDeviceToHost, e.stream));
   return VPB_OK;
@@ -682,7 +750,8 @@ int vp_engine::fetch(bool raw) {
     VPB_CUDA_OK(cudaMemcpyAsync(so.h, so.d, static_cast<size_t>(so.job.dh) * so.job.dst_pitch, cudaMemcpyDeviceToHost, stream));
   src_host = true;
   if (lat_model >= 0) {
-    VPB_CUDA_OK(cudaMemcpyAsync(h_lat_out, d_lat_out + static_cast<size_t>(lat_cur) * batch, sizeof(vpb_lateral_out) * batch,
+    const int n = model_batch(lat_model);
+    VPB_CUDA_OK(cudaMemcpyAsync(h_lat_out, d_lat_out + static_cast<size_t>(lat_cur) * n, sizeof(vpb_lateral_out) * n,
                                 cudaMemcpyDeviceToHost, stream));
     lat_host = true;
   }
@@ -692,6 +761,11 @@ int vp_engine::fetch(bool raw) {
 // ====================================================================== C-ABI
 extern "C" const char* vp_last_error(void) { return vpb_last_error(); }
 
+// The camera sets of a created engine's models: each model with a set that built its encoder gets its own pre-process
+// op and buffers (route_input), a model sharing that encoder reads them, and the taps of a model with a set take its set.
+// The shared "preprocess" goes when no model reads it.
+static int attach_camera_sets(vp_engine& e);
+
 extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
   if (!cfg || !out || cfg->n_models < 1 || cfg->n_models > VP_MAX_MODELS) {
     vpb_set_error("vp_engine_create: bad config");
@@ -699,6 +773,12 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
   }
   *out = nullptr;
   int rc = check_source_flags(*cfg);
+  if (rc) return rc;
+  int cams[VP_MAX_MODELS] = {};
+  rc = camera_sets(*cfg, cams);
+  if (rc) return rc;
+  std::vector<WeightMap> set_w;            // loaded here only when a model has a camera set
+  rc = load_weights_for_sets(*cfg, cams, set_w);
   if (rc) return rc;
   std::unique_ptr<vp_engine> e(new vp_engine());
   rc = e->open("vp_engine_create", cfg->gpu_id, cfg->stream);
@@ -731,20 +811,30 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
     e->tap("pre", pre, 3);                 // RGB of the [320][640][4] network input
   }
   e->add_preprocess(cfg->convention, e->d_pre, e->d_resized);
+  memcpy(e->cams, cams, sizeof(cams));
+  const int nb = e->batch;
   for (int i = 0; i < cfg->n_models; ++i) {
-    if (!cfg->weights[i] || !cfg->weights[i][0]) {
-      // same condition the reference rejects: scene_seg_infer.py:32-33
-      vpb_set_error("No path to checkpoint file provided for model %d", i);
-      return VPB_ERR_ARG;
-    }
     WeightMap w;
-    rc = load_vpw(cfg->weights[i], w);
-    if (rc) return rc;
+    if (set_w.empty()) {
+      if (!cfg->weights[i] || !cfg->weights[i][0]) {
+        // same condition the reference rejects: scene_seg_infer.py:32-33
+        vpb_set_error("No path to checkpoint file provided for model %d", i);
+        return VPB_ERR_ARG;
+      }
+      rc = load_vpw(cfg->weights[i], w);
+      if (rc) return rc;
+    } else {
+      w.swap(set_w[i]);
+    }
     NetBuilder b{*e, w};
+    e->batch = e->model_batch(i);          // a model with a camera set is built as a batch-m_i network
     build_model(*e, b, i, cfg->kinds[i]);
+    e->batch = nb;
     if (b.status()) return b.status();     // an oom first (VPB_ERR_CUDA), with the failing allocation's message
   }
   if (e->oom) return VPB_ERR_CUDA;
+  rc = attach_camera_sets(*e);
+  if (rc) return rc;
   rc = build_source_outputs(*e);
   if (rc) return rc;
   VPB_CUDA_OK(cudaDeviceSynchronize());
@@ -755,7 +845,14 @@ extern "C" int vp_engine_create(const vp_engine_config* cfg, vp_engine** out) {
 extern "C" void vp_engine_destroy(vp_engine* e) { delete e; }   // ~EngineRuntime switches to the engine's device
 
 extern "C" int vp_engine_num_models(const vp_engine* e) { return e ? static_cast<int>(e->outs.size()) : 0; }
-int vpb_engine_batch(const vp_engine* e) { return e ? e->batch : 0; }
+int vpb_engine_model_samples(const vp_engine* e, int model_idx, int* samples, int* batch) {
+  *batch = e ? e->batch : 0;
+  if (!e) return 0;
+  const bool in = model_idx >= 0 && model_idx < static_cast<int>(e->outs.size());
+  const int cams = in ? e->cams[model_idx] : 0, n = in ? e->model_batch(model_idx) : e->batch;
+  for (int j = 0; j < n; ++j) samples[j] = camera_sample(cams, j);
+  return n;
+}
 
 extern "C" uint8_t* vp_engine_pinned_frame(vp_engine* e, size_t bytes) {
   if (!e) return nullptr;
@@ -851,19 +948,26 @@ extern "C" int vp_engine_set_roi(vp_engine* e, int sample, int x, int y, int w, 
 }
 
 // ---------------------------------------------------------------- per-model input views
-// sample `sample` of the [batch][320][640][3] resized images at src to dst (host), synchronously
-static int read_resized(vp_engine* e, const uint8_t* src, int sample, uint8_t* dst, const char* who) {
+// sample `sample` of the [slot][320][640][3] resized images at src of the camera set cams to dst (host), synchronously
+static int read_resized(vp_engine* e, const uint8_t* src, int sample, uint8_t* dst, const char* who, int cams = 0,
+                        int model = -1) {
   if (sample < 0 || sample >= e->batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch); return VPB_ERR_ARG; }
+  const int slot = camera_slot(cams, sample);
+  if (slot < 0) {
+    vpb_set_error("%s: model %d does not run on sample %d (its cameras 0x%x)", who, model, sample, cams);
+    return VPB_ERR_ARG;
+  }
   DeviceGuard guard(e->gpu_id);
   const size_t bytes = static_cast<size_t>(kNetH) * kNetW * 3;
-  VPB_CUDA_OK(cudaMemcpyAsync(dst, src + bytes * sample, bytes, cudaMemcpyDeviceToHost, e->stream));
+  VPB_CUDA_OK(cudaMemcpyAsync(dst, src + bytes * slot, bytes, cudaMemcpyDeviceToHost, e->stream));
   VPB_CUDA_OK(cudaStreamSynchronize(e->stream));
   return VPB_OK;
 }
 
 static bool reads_bgr(int convention) { return convention == VPB_CONV_BGR_NOSWAP || convention == VPB_CONV_BGR_SWAP; }
 
-// Op "preprocess/<m>": the pre-process of model m's view of every sample's full() frame into the view's buffers
+// Op "preprocess/<m>": the pre-process of what model m reads of each sample of its set (input_frame) into its slots of
+// the view's buffers
 static OpRec view_op(vp_engine& e, int m) {
   OpRec op;
   op.name = "preprocess/" + std::to_string(m); op.kname = "preprocess"; op.lane = m;
@@ -871,24 +975,70 @@ static OpRec view_op(vp_engine& e, int m) {
   op.describe = [ep, m](KernelCall& c) {
     const vp_engine::View& v = ep->views[m];
     Frames f{};
-    for (int k = 0; k < ep->batch; ++k) f[k] = ep->input_frame(m, k);
+    for (int j = 0; j < ep->model_batch(m); ++j) f[j] = ep->input_frame(m, camera_sample(ep->cams[m], j));
     return v.plan.describe(f.data(), v.convention, ep->dtype, v.pre, v.resized, c);
   };
   return op;
 }
 
-// model m's stem, its "<m>/pre" tap and its lane's fork follow its view (on) or the engine's input
-static void route_input(vp_engine& e, int m, bool on) {
+// model m's stem, its "<m>/pre" tap and its lane's fork follow its own pre-process (own_pre) or the engine's input; a
+// model sharing another's encoder reads that model's input
+static void route_input(vp_engine& e, int m) {
   vp_engine::View& v = e.views[m];
-  e.input[m] = on ? vp_engine::Input{v.pre, v.pre_lo} : vp_engine::Input{e.d_pre, e.d_pre_lo};
+  const int owner = e.enc_owner[m];
+  const bool on = e.own_pre(m);
+  e.input[m] = owner != m ? e.input[owner] : on ? vp_engine::Input{v.pre, v.pre_lo} : vp_engine::Input{e.d_pre, e.d_pre_lo};
   Tens t = e.taps["pre"].t;
   t.p = const_cast<void*>(e.input[m].p); t.lo = const_cast<void*>(e.input[m].lo);
-  e.tap(std::to_string(m) + "/pre", t, 3);
-  if (m == 0) return;                      // lane 0 is the engine stream: its ops already follow the front ops
+  const std::string name = std::to_string(m) + "/pre";
+  e.tap(name, t, 3);
+  e.taps[name].cameras = e.cams[m]; e.taps[name].model = m;
+  if (m == 0 || owner != m) return;        // lane 0 is the engine stream: its ops already follow the front ops; a sharing
+                                           // model's lane starts after the shared encoder
   auto& ff = e.front_forks;
   ff.erase(std::remove(ff.begin(), ff.end(), m), ff.end());
   if (on) ff.push_back(m);
-  e.set_lane_dep(m, on ? e.op_index("preprocess") - 1 : e.op_index("preprocess"));
+  e.set_lane_dep(m, on ? e.front_count() - 1 : e.front_count());
+}
+
+// model m's own network input and resized image, one per slot of its set (kept once made)
+static int view_buffers(vp_engine& e, int m) {
+  vp_engine::View& view = e.views[m];
+  if (view.pre) return VPB_OK;
+  const size_t in = static_cast<size_t>(kNetH) * kNetW * 4 * 2 * e.model_batch(m) * (e.split ? 2 : 1),
+               rs = static_cast<size_t>(kNetH) * kNetW * 3 * e.model_batch(m);
+  void* p = nullptr; void* q = nullptr;
+  VPB_CUDA_OK(cudaMalloc(&p, in));
+  e.dev_allocs.push_back(p);
+  VPB_CUDA_OK(cudaMalloc(&q, rs));
+  e.dev_allocs.push_back(q);
+  VPB_CUDA_OK(cudaMemsetAsync(p, 0, in, e.stream));   // the fourth channel stays zero, as d_pre's
+  view.pre = p;
+  if (e.split) view.pre_lo = static_cast<uint8_t*>(p) + static_cast<size_t>(kNetH) * kNetW * 4 * 2;
+  view.plan.out_lo = view.pre_lo;
+  view.resized = static_cast<uint8_t*>(q);
+  return VPB_OK;
+}
+
+static int attach_camera_sets(vp_engine& e) {
+  const int nm = static_cast<int>(e.outs.size());
+  bool shared = false;                     // a model reads the engine's "preprocess"
+  for (int m = 0; m < nm; ++m) shared |= e.cams[m] == 0;
+  if (!shared) e.erase_ops(e.op_index("preprocess"), 1);
+  for (int m = 0; m < nm; ++m) {
+    if (!e.cams[m]) continue;
+    const std::string tag = std::to_string(m) + "/";
+    for (auto& kv : e.taps)
+      if (kv.first.compare(0, tag.size(), tag) == 0) { kv.second.cameras = e.cams[m]; kv.second.model = m; }
+    if (e.enc_owner[m] == m) {
+      const int rc = view_buffers(e, m);
+      if (rc) return rc;
+      e.views[m].convention = e.cfg.convention;
+      e.insert_ops(e.op_index((tag + "stem").c_str()), {view_op(e, m)});
+    }
+    route_input(e, m);
+  }
+  return VPB_OK;
 }
 
 extern "C" int vp_engine_set_view(vp_engine* e, int model_idx, const vp_view* v) {
@@ -925,37 +1075,28 @@ extern "C" int vp_engine_set_view(vp_engine* e, int model_idx, const vp_view* v)
   DeviceGuard guard(e->gpu_id);
   vp_engine::View& view = e->views[model_idx];
   e->n_frames = 0;                         // the last call's frames are not those the model now reads
+  const bool had = e->own_pre(model_idx);
   if (!v) {
     if (!view.on) return VPB_OK;
-    e->erase_ops(e->op_index(("preprocess/" + std::to_string(model_idx)).c_str()), 1);
     view.on = false;
-    route_input(*e, model_idx, false);
-    return VPB_OK;
+    view.convention = e->cfg.convention;   // a model with a camera set keeps its op, on the engine's input
+    memset(view.roi, 0, sizeof(view.roi));
+  } else {
+    const int rc = view_buffers(*e, model_idx);
+    if (rc) return rc;
+    view.convention = v->convention == -1 ? e->cfg.convention : v->convention;
+    for (int k = 0; k < e->batch; ++k) {
+      const int* r = v->roi[k];
+      const bool whole = r[2] == 0 && r[3] == 0;
+      for (int i = 0; i < 4; ++i) view.roi[k][i] = whole ? 0 : r[i];
+    }
+    view.on = true;
   }
-  if (!view.pre) {
-    const size_t in = static_cast<size_t>(kNetH) * kNetW * 4 * 2 * e->batch * (e->split ? 2 : 1),
-                 rs = static_cast<size_t>(kNetH) * kNetW * 3 * e->batch;
-    void* p = nullptr; void* q = nullptr;
-    VPB_CUDA_OK(cudaMalloc(&p, in));
-    e->dev_allocs.push_back(p);
-    VPB_CUDA_OK(cudaMalloc(&q, rs));
-    e->dev_allocs.push_back(q);
-    VPB_CUDA_OK(cudaMemsetAsync(p, 0, in, e->stream));   // the fourth channel stays zero, as d_pre's
-    view.pre = p;
-    if (e->split) view.pre_lo = static_cast<uint8_t*>(p) + static_cast<size_t>(kNetH) * kNetW * 4 * 2;
-    view.plan.out_lo = view.pre_lo;
-    view.resized = static_cast<uint8_t*>(q);
-  }
-  view.convention = v->convention == -1 ? e->cfg.convention : v->convention;
-  for (int k = 0; k < e->batch; ++k) {
-    const int* r = v->roi[k];
-    const bool whole = r[2] == 0 && r[3] == 0;
-    for (int i = 0; i < 4; ++i) view.roi[k][i] = whole ? 0 : r[i];
-  }
-  if (view.on) return VPB_OK;              // a new region or convention: the next call re-points or captures again
-  view.on = true;
-  e->insert_ops(e->op_index((std::to_string(model_idx) + "/stem").c_str()), {view_op(*e, model_idx)});
-  route_input(*e, model_idx, true);
+  if (e->own_pre(model_idx) == had) return VPB_OK;   // a new region or convention: the next call re-points or captures again
+  const std::string name = "preprocess/" + std::to_string(model_idx);
+  if (had) e->erase_ops(e->op_index(name.c_str()), 1);
+  else e->insert_ops(e->op_index((std::to_string(model_idx) + "/stem").c_str()), {view_op(*e, model_idx)});
+  route_input(*e, model_idx);
   return VPB_OK;
 }
 
@@ -966,31 +1107,42 @@ extern "C" int vp_engine_read_resized_view(vp_engine* e, int model_idx, int samp
     vpb_set_error("%s: model %d out of range (the engine has %d models)", who, model_idx, static_cast<int>(e->outs.size()));
     return VPB_ERR_ARG;
   }
-  const vp_engine::View& v = e->views[model_idx];
-  return read_resized(e, v.on ? v.resized : e->d_resized, sample, dst, who);
+  const int owner = e->enc_owner[model_idx];
+  return read_resized(e, e->own_pre(owner) ? e->views[owner].resized : e->d_resized, sample, dst, who,
+                      e->cams[model_idx], model_idx);
 }
 
 // ---------------------------------------------------------------- the detector inside the call
-// Op "det/letterbox": the detector's letterbox of every sample's full() frame, B, G, R under the BGR conventions.
+// Op "det/letterbox": the detector's letterbox of the full() frame of each sample of its set into its slots, B, G, R
+// under the BGR conventions.
 static OpRec letterbox_op(vp_engine& e) {
   OpRec op;
   op.name = "det/letterbox"; op.kname = "preprocess"; op.lane = e.front_lane;
   vp_engine* ep = &e;
   op.describe = [ep](KernelCall& c) {
     Frames f{};
-    for (int k = 0; k < ep->batch; ++k) f[k] = ep->chain[k].full();
+    for (int j = 0; j < autospeed_runtime(ep->det)->batch; ++j) f[j] = ep->chain[camera_sample(ep->det_cams, j)].full();
     return autospeed_letterbox(ep->det, f.data(), ep->rect_bgr, c);
   };
   return op;
 }
 
-extern "C" int vp_engine_set_detector(vp_engine* e, vp_autospeed* det) {
-  const char* who = "vp_engine_set_detector";
+// det on the samples of cameras (0: every sample); who names the call
+static int set_detector(vp_engine* e, vp_autospeed* det, int cameras, const char* who) {
   if (!e) { vpb_set_error("%s: NULL engine", who); return VPB_ERR_ARG; }
+  const int all = (1 << e->batch) - 1;
+  if (cameras & ~all) {
+    vpb_set_error("%s: cameras 0x%x has a bit at or above the batch %d", who, static_cast<unsigned>(cameras), e->batch);
+    return VPB_ERR_ARG;
+  }
+  if (cameras == all) cameras = 0;
   if (det) {
     const EngineRuntime* d = autospeed_runtime(det);
-    if (d->batch != e->batch) {
-      vpb_set_error("%s: the detector has batch %d, the engine batch %d", who, d->batch, e->batch);
+    const int n = cameras ? __builtin_popcount(cameras) : e->batch;
+    if (d->batch != n) {
+      if (cameras) vpb_set_error("%s: the detector has batch %d, the camera set 0x%x has %d samples", who, d->batch,
+                                 static_cast<unsigned>(cameras), n);
+      else vpb_set_error("%s: the detector has batch %d, the engine batch %d", who, d->batch, e->batch);
       return VPB_ERR_ARG;
     }
     if (d->gpu_id != e->gpu_id) {
@@ -1010,9 +1162,11 @@ extern "C" int vp_engine_set_detector(vp_engine* e, vp_autospeed* det) {
     e->front_lane = 0;
   }
   e->det = nullptr;
+  e->det_cams = 0;
   e->n_frames = 0;                         // profiling and timing wait for a call on the new op list
   if (!det) return VPB_OK;
   e->det = det;
+  e->det_cams = cameras;
   e->front_lane = static_cast<int>(e->lane_dep.size());
   e->lane_dep.push_back(-1);
   std::vector<OpRec> add{letterbox_op(*e)};
@@ -1026,38 +1180,63 @@ extern "C" int vp_engine_set_detector(vp_engine* e, vp_autospeed* det) {
   return VPB_OK;
 }
 
+extern "C" int vp_engine_set_detector(vp_engine* e, vp_autospeed* det) {
+  return set_detector(e, det, 0, "vp_engine_set_detector");
+}
+
+extern "C" int vp_engine_set_detector_cameras(vp_engine* e, vp_autospeed* det, int cameras) {
+  return set_detector(e, det, cameras, "vp_engine_set_detector_cameras");
+}
+
 // ---------------------------------------------------------------- the lateral post-process inside the call
 // Op "lateral": the EgoLanes logits of model lat_model, each sample's source size (what its pre-process reads: the
 // frame as given, a JPEG frame's SOF size, a rectified frame's map size), the states of slot lat_cur -> the states and
 // records of slot 1 - lat_cur.
+// On a model with a camera set, camera j of the launch is slot j of the model: its states and records are slot j's, its
+// homography and steering those of sample camera_sample(cams, j).
 static OpRec lateral_op(vp_engine& e) {
   OpRec op;
   op.name = "lateral"; op.kname = "lateral_kernel"; op.lane = e.lat_model;
   const ModelOut& mo = e.outs[e.lat_model];
-  op.bytes = e.batch * (4.0 * 3 * mo.H * mo.W + 2.0 * sizeof(vpb_lateral_state) + sizeof(vpb_lateral_out));
+  op.bytes = e.model_batch(e.lat_model) * (4.0 * 3 * mo.H * mo.W + 2.0 * sizeof(vpb_lateral_state) + sizeof(vpb_lateral_out));
   vp_engine* ep = &e;
   op.describe = [ep](KernelCall& c) {
-    const ModelOut& m = ep->outs[ep->lat_model];
+    const int lm = ep->lat_model, n = ep->model_batch(lm);
+    const ModelOut& m = ep->outs[lm];
     int iw[kMaxBatch], ih[kMaxBatch];
-    for (int k = 0; k < ep->batch; ++k) {
-      const vpb_frame_fmt f = ep->input_frame(ep->lat_model, k);
-      iw[k] = f.w; ih[k] = f.h;
+    double hom[9 * kMaxBatch], steer[kMaxBatch];
+    for (int j = 0; j < n; ++j) {
+      const int k = camera_sample(ep->cams[lm], j);
+      const vpb_frame_fmt f = ep->input_frame(lm, k);
+      iw[j] = f.w; ih[j] = f.h;
+      steer[j] = ep->steering[k];
+      if (!ep->lat_hom.empty()) std::copy_n(ep->lat_hom.data() + 9 * k, 9, hom + 9 * j);
     }
-    const size_t rd = static_cast<size_t>(ep->lat_cur) * ep->batch, wr = static_cast<size_t>(1 - ep->lat_cur) * ep->batch;
-    return lateral_call("lateral", m.d_raw, ep->lat_threshold, ep->batch, m.H, m.W, iw, ih, ep->lat_smoothing,
-                        ep->lat_hom.empty() ? nullptr : ep->lat_hom.data(), ep->steering, ep->d_lat_state + rd,
+    const size_t rd = static_cast<size_t>(ep->lat_cur) * n, wr = static_cast<size_t>(1 - ep->lat_cur) * n;
+    return lateral_call("lateral", m.d_raw, ep->lat_threshold, n, m.H, m.W, iw, ih, ep->lat_smoothing,
+                        ep->lat_hom.empty() ? nullptr : hom, steer, ep->d_lat_state + rd,
                         ep->d_lat_state + wr, ep->d_lat_out + wr, c);
   };
   return op;
 }
 
-// fresh states (vpb_lateral_init) for sample `sample` (-1: every sample) of slot `slot`, on the engine's stream
-static int lateral_init_slot(vp_engine& e, int slot, int sample) {
-  for (int k = sample < 0 ? 0 : sample; k < (sample < 0 ? e.batch : sample + 1); ++k) {
-    const int rc = vpb_lateral_init(e.d_lat_state + static_cast<size_t>(slot) * e.batch + k, e.stream);
+// fresh states (vpb_lateral_init) for slot `j` (-1: every slot) of the lateral model's set, in state slot `slot`, on the
+// engine's stream
+static int lateral_init_slot(vp_engine& e, int slot, int j) {
+  const int n = e.model_batch(e.lat_model);
+  for (int k = j < 0 ? 0 : j; k < (j < 0 ? n : j + 1); ++k) {
+    const int rc = vpb_lateral_init(e.d_lat_state + static_cast<size_t>(slot) * n + k, e.stream);
     if (rc) return rc;
   }
   return VPB_OK;
+}
+
+// the lateral model's slot of sample `sample`; -1 (VPB_ERR_ARG's message set, naming who) outside its camera set
+static int lateral_slot(const vp_engine& e, int sample, const char* who) {
+  const int j = camera_slot(e.cams[e.lat_model], sample);
+  if (j < 0)
+    vpb_set_error("%s: model %d does not run on sample %d (its cameras 0x%x)", who, e.lat_model, sample, e.cams[e.lat_model]);
+  return j;
 }
 
 extern "C" int vp_engine_set_lateral(vp_engine* e, int model_idx, const vp_lateral_config* cfg) {
@@ -1094,9 +1273,9 @@ extern "C" int vp_engine_set_lateral(vp_engine* e, int model_idx, const vp_later
   if (cfg->homographies) e->lat_hom.assign(cfg->homographies, cfg->homographies + 9 * e->batch);
   else e->lat_hom.clear();
   e->lat_cur = 0;
-  int rc = lateral_init_slot(*e, 0, -1);
-  if (rc) return rc;
   e->lat_model = model_idx;
+  const int rc = lateral_init_slot(*e, 0, -1);
+  if (rc) { e->lat_model = -1; return rc; }
   const int last = e->op_index((std::to_string(model_idx) + "/dec8sum").c_str());   // the model's final op
   e->insert_ops(last + 1, {lateral_op(*e)});
   return VPB_OK;
@@ -1113,8 +1292,10 @@ extern "C" int vp_engine_lateral_reset(vp_engine* e, int sample) {
   if (!e) { vpb_set_error("%s: NULL engine", who); return VPB_ERR_ARG; }
   if (sample < -1 || sample >= e->batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch); return VPB_ERR_ARG; }
   if (e->lat_model < 0) { vpb_set_error("%s: the lateral post-process is off (vp_engine_set_lateral)", who); return VPB_ERR_STATE; }
+  const int j = sample < 0 ? -1 : lateral_slot(*e, sample, who);
+  if (sample >= 0 && j < 0) return VPB_ERR_ARG;
   DeviceGuard guard(e->gpu_id);
-  return lateral_init_slot(*e, e->lat_cur, sample);
+  return lateral_init_slot(*e, e->lat_cur, j);
 }
 
 extern "C" int vp_engine_lateral(vp_engine* e, int sample, const vpb_lateral_out** host, const vpb_lateral_out** dev) {
@@ -1122,9 +1303,11 @@ extern "C" int vp_engine_lateral(vp_engine* e, int sample, const vpb_lateral_out
   if (!e) { vpb_set_error("%s: NULL engine", who); return VPB_ERR_ARG; }
   if (sample < 0 || sample >= e->batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch); return VPB_ERR_ARG; }
   if (e->lat_model < 0) { vpb_set_error("%s: the lateral post-process is off (vp_engine_set_lateral)", who); return VPB_ERR_STATE; }
+  const int j = lateral_slot(*e, sample, who);
+  if (j < 0) return VPB_ERR_ARG;
   if (!e->lat_ready) { vpb_set_error("%s: run one call first", who); return VPB_ERR_STATE; }
-  if (host) *host = e->lat_host ? e->h_lat_out + sample : nullptr;
-  if (dev) *dev = e->d_lat_out + static_cast<size_t>(e->lat_cur) * e->batch + sample;
+  if (host) *host = e->lat_host ? e->h_lat_out + j : nullptr;
+  if (dev) *dev = e->d_lat_out + static_cast<size_t>(e->lat_cur) * e->model_batch(e->lat_model) + j;
   return VPB_OK;
 }
 
@@ -1134,7 +1317,7 @@ const vpb_lateral_out* vpb_engine_lateral_records(const vp_engine* e, int model_
     return nullptr;
   }
   if (!e->lat_ready) { vpb_set_error("%s: no call has made lateral records yet", who); return nullptr; }
-  return e->d_lat_out + static_cast<size_t>(e->lat_cur) * e->batch;
+  return e->d_lat_out + static_cast<size_t>(e->lat_cur) * e->model_batch(model_idx);
 }
 
 extern "C" int vp_engine_graph_captures(const vp_engine* e) {
@@ -1154,8 +1337,13 @@ extern "C" int vp_engine_fetch_raw(vp_engine* e, int idx) {
 extern "C" int vp_engine_output_at(vp_engine* e, int idx, int sample, vp_output* o) {
   if (!e || !o || idx < 0 || idx >= static_cast<int>(e->outs.size())) { vpb_set_error("vp_engine_output: bad index"); return VPB_ERR_ARG; }
   if (sample < 0 || sample >= e->batch) { vpb_set_error("vp_engine_output: sample %d of a batch of %d", sample, e->batch); return VPB_ERR_ARG; }
+  const int slot = camera_slot(e->cams[idx], sample);
+  if (slot < 0) {
+    vpb_set_error("vp_engine_output: model %d does not run on sample %d (its cameras 0x%x)", idx, sample, e->cams[idx]);
+    return VPB_ERR_ARG;
+  }
   const auto& mo = e->outs[idx];
-  const size_t plane = static_cast<size_t>(mo.H) * mo.W, raw = plane * mo.C * sample, cls = plane * sample;
+  const size_t plane = static_cast<size_t>(mo.H) * mo.W, raw = plane * mo.C * slot, cls = plane * slot;
   o->kind = mo.kind; o->channels = mo.C; o->height = mo.H; o->width = mo.W;
   o->raw_host = mo.h_raw + raw; o->cls_host = mo.has_cls ? mo.h_cls + cls : nullptr;
   o->raw_dev = mo.d_raw + raw; o->cls_dev = mo.has_cls ? mo.d_cls + cls : nullptr;
@@ -1168,6 +1356,10 @@ extern "C" int vp_engine_source_output(vp_engine* e, int idx, int sample, int ki
   const char* who = "vp_engine_source_output";
   if (!e || !o || idx < 0 || idx >= static_cast<int>(e->outs.size())) { vpb_set_error("%s: bad model index", who); return VPB_ERR_ARG; }
   if (sample < 0 || sample >= e->batch) { vpb_set_error("%s: sample %d of a batch of %d", who, sample, e->batch); return VPB_ERR_ARG; }
+  if (camera_slot(e->cams[idx], sample) < 0) {
+    vpb_set_error("%s: model %d does not run on sample %d (its cameras 0x%x)", who, idx, sample, e->cams[idx]);
+    return VPB_ERR_ARG;
+  }
   const SrcOut* so = nullptr;
   for (const auto& x : e->src_outs)
     if (x.model == idx && x.sample == sample && x.flag == kind) { so = &x; break; }

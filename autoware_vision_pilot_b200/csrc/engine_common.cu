@@ -379,6 +379,12 @@ int EngineRuntime::op_index(const char* name) const {
   return -1;
 }
 
+int EngineRuntime::front_count() const {
+  int n = 0;
+  while (n < static_cast<int>(ops.size()) && (ops[n].name == "rectify" || ops[n].name.compare(0, 5, "jpeg_") == 0)) ++n;
+  return n;
+}
+
 void EngineRuntime::insert_ops(size_t at, std::vector<OpRec> add) {
   frame_graph.invalidate();
   const int m = static_cast<int>(add.size());
@@ -436,7 +442,7 @@ void EngineRuntime::sync_front_ops() {
         rectify_call(f, m, rect_list(*this, f, m, o), rect_bgr, o, c);
         return VPB_OK;
       };
-      insert_ops(op_index("preprocess"), std::move(add));    // after the JPEG decode: rectify reads the decoded frame
+      insert_ops(front_count(), std::move(add));    // after the JPEG decode: rectify reads the decoded frame
     } else {
       erase_ops(op_index("rectify"), 1);
     }
@@ -448,7 +454,7 @@ void EngineRuntime::sync_front_ops() {
     const int n = rect_list(*this, f, m, o);
     ops[op_index("rectify")].bytes = rectify_bytes(f, m, n);
   }
-  const int front = op_index("preprocess") - 1;   // the last front op, -1: none
+  const int front = front_count() - 1;   // the last front op, -1: none
   if (front_lane > 0) set_lane_dep(front_lane, front);
   for (int l : front_forks) set_lane_dep(l, front);
 }
@@ -688,7 +694,8 @@ static int enqueue_frames(EngineRuntime* e, int n, const PreGeom* g) {
   e->sync_front_ops();
   double bytes = 0;
   for (int k = 0; k < n; ++k) bytes += frame_bytes(e->chain[k].pre()) + 2.0 * 3 * g[k].OH * g[k].OW;
-  e->ops[e->op_index("preprocess")].bytes = bytes;
+  const int pre = e->op_index("preprocess");   // an engine whose every model has a camera set has none
+  if (pre >= 0) e->ops[pre].bytes = bytes;
   const int rc = e->enqueue(g);
   if (rc) e->n_frames = 0;
   return rc;
@@ -839,7 +846,12 @@ bool EngineRuntime::find_tap(const char* name, Tap* out) const {
   auto it = taps.find(nm);
   if (it == taps.end()) { vpb_set_error("no tap '%s'", name); return false; }
   *out = it->second;
-  out->t.p = static_cast<uint8_t*>(out->t.p) + out->t.bytes() * k;    // split-fp16 engines (lo != NULL) have batch 1
+  const int slot = camera_slot(out->cameras, k);
+  if (slot < 0) {
+    vpb_set_error("tap '%s': model %d does not run on sample %d (its cameras 0x%x)", name, out->model, k, out->cameras);
+    return false;
+  }
+  out->t.p = static_cast<uint8_t*>(out->t.p) + out->t.bytes() * slot;    // split-fp16 engines (lo != NULL) have batch 1
   return true;
 }
 

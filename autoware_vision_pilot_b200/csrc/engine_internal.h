@@ -68,7 +68,21 @@ struct Tens {
 };
 
 // A named intermediate tensor readable as fp32: the leading `channels` channels of t are reported (the rest is padding).
-struct Tap { Tens t; int channels = 0; };
+// cameras: the samples the tensor holds, bit k = sample k, slot j = the j-th set bit (0: every sample); model: whose.
+struct Tap { Tens t; int channels = 0; int cameras = 0; int model = -1; };
+
+// slot of sample k in the camera set `cameras` (0: every sample, slot k); -1 when k is not in the set
+inline int camera_slot(int cameras, int k) {
+  if (!cameras) return k;
+  return (cameras >> k) & 1 ? __builtin_popcount(cameras & ((1u << k) - 1)) : -1;
+}
+// sample of slot j of the camera set `cameras` (0: every sample, sample j)
+inline int camera_sample(int cameras, int j) {
+  if (!cameras) return j;
+  for (int k = 0; k < 32; ++k)
+    if (((cameras >> k) & 1) && j-- == 0) return k;
+  return -1;
+}
 
 struct OpRec {
   std::string name;
@@ -219,6 +233,9 @@ struct EngineRuntime {
   // map of another GPU; then sync_front_ops.
   int set_rectify(int sample, const vpb_rectify* r, const char* who);
   int op_index(const char* name) const;   // index of the op of that name, -1 if there is none
+  // the number of front ops (the JPEG decode ops, "rectify") at the start of the list: the index of "preprocess" when
+  // the list has it
+  int front_count() const;
   // insert ops at index `at` / erase m ops from `at`: the op events and the lanes' producer indices past `at` follow,
   // and the captured graph is dropped
   void insert_ops(size_t at, std::vector<OpRec> add);
@@ -266,7 +283,8 @@ struct EngineRuntime {
   // describes the device copy of frame k (its uv inside `upload` for NV12).  JPEG frames are staged in `jpeg` instead,
   // to be decoded into chain[k].jpg (grown on demand), and chain[k].given is the frame as given.
   int upload_frames(const vpb_frame_fmt* frames, int n);
-  // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch; false (error set) if there is none.
+  // Tap "<name>[@k]": the tensor of sample k (default 0) of the batch, at its slot of the tap's camera set; false (error
+  // set) if there is none or k is not in the set.
   bool find_tap(const char* name, Tap* out) const;
   // tap `name` (find_tap) as fp32 [channels][H][W] into dst (NULL: size query); element count or < 0
   long read_tap(const char* name, float* dst, long cap, int* c, int* h, int* w);
@@ -356,9 +374,11 @@ int autospeed_fetch_rest(vp_autospeed* d);
 
 }  // namespace vpb
 
-// frames per call of a segmentation engine (engine.cu), for callers that see vp_engine only as an opaque type
+// the samples model model_idx of a segmentation engine (engine.cu) runs on, slot by slot, into samples (VP_MAX_BATCH
+// entries) and the engine's batch into *batch; their count (every sample for a model without a camera set or out of range,
+// whose taps the caller then fails to find).  For callers that see vp_engine only as an opaque type.
 struct vp_engine;
-int vpb_engine_batch(const vp_engine* e);
+int vpb_engine_model_samples(const vp_engine* e, int model_idx, int* samples, int* batch);
 // the device records of e's last call made by its in-call lateral post-process on model model_idx (vp_engine_set_lateral);
 // NULL, with the error set naming who, when that model has none or no call has made them
 const vpb_lateral_out* vpb_engine_lateral_records(const vp_engine* e, int model_idx, const char* who);

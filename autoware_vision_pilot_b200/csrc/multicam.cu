@@ -291,14 +291,18 @@ extern "C" int vp_multicam_step_engine(vp_multicam* mc, vp_engine* e, int model_
                                        int predict) {
   if (!mc || !e) { vpb_set_error("vp_multicam_step_engine: bad arguments"); return VPB_ERR_ARG; }
   if (!lat && !(lat = vpb_engine_lateral_records(e, model_idx, "vp_multicam_step_engine"))) return VPB_ERR_ARG;
-  if (mc->local && vpb_engine_batch(e) != mc->world) {
-    vpb_set_error("vp_multicam_step_engine: engine of batch %d for %d cameras", vpb_engine_batch(e), mc->world);
+  int samples[VP_MAX_BATCH], batch = 0;    // the model's samples, slot by slot (its camera set, or the engine's batch)
+  const int n = vpb_engine_model_samples(e, model_idx, samples, &batch);
+  if (mc->local && n != mc->world) {
+    if (n == batch) vpb_set_error("vp_multicam_step_engine: engine of batch %d for %d cameras", batch, mc->world);
+    else vpb_set_error("vp_multicam_step_engine: model %d runs on %d samples of the engine of batch %d, for %d cameras",
+                       model_idx, n, batch, mc->world);
     return VPB_ERR_ARG;
   }
   PackFeats feats{};
   for (int k = 0; k < (mc->local ? mc->world : 1); ++k) {   // NCCL mode: "<idx>/fused" of the rank's single frame
     char name[32];
-    if (mc->local) snprintf(name, sizeof(name), "%d/fused@%d", model_idx, k);
+    if (mc->local) snprintf(name, sizeof(name), "%d/fused@%d", model_idx, samples[k]);
     else snprintf(name, sizeof(name), "%d/fused", model_idx);
     vp_tap_view tv;
     int rc = vp_engine_tap_dev(e, name, &tv);

@@ -2,7 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -24,6 +24,30 @@ _bind = L.lib
 _Config, _Output, _SourceOutput, _Stats, _TapView = L.EngineConfig, L.Output, L.SourceOutput, L.EngineStats, L.TapView
 
 
+def camera_masks(cameras: Optional[Dict[int, Sequence[int]]], n_models: int, batch: int) -> List[int]:
+    """{model: [samples]} -> one vp_engine_config.cameras bit mask per model (0: every sample); ValueError for a model
+    or sample out of range, or an empty or repeated sample list."""
+    masks = [0] * n_models
+    for m, samples in (cameras or {}).items():
+        if not 0 <= m < n_models:
+            raise ValueError(f"cameras: model {m} out of range (the engine has {n_models} models)")
+        samples = [int(k) for k in samples]
+        if not samples:
+            raise ValueError(f"cameras: model {m} has no sample")
+        for k in samples:
+            if not 0 <= k < batch:
+                raise ValueError(f"cameras: model {m}: sample {k} of a batch of {batch}")
+        if len(set(samples)) != len(samples):
+            raise ValueError(f"cameras: model {m}: sample listed twice in {samples}")
+        masks[m] = sum(1 << k for k in samples)
+    return masks
+
+
+def samples_of(mask: int, batch: int) -> List[int]:
+    """the samples of a camera bit mask in slot order (0: every sample)"""
+    return [k for k in range(batch) if not mask or (mask >> k) & 1]
+
+
 def source_flags(names: Sequence[str]) -> int:
     """("mask", "depth", "overlay") -> VP_SRC_* bitmask; ValueError for an unknown name."""
     if isinstance(names, str):
@@ -42,13 +66,20 @@ class Engine:
     def __init__(self, kinds: Sequence[int], weights: Sequence[str], *, gpu_id: int = 0, dtype: str = "fp16",
                  resize_mode: int = RESIZE_NONE, convention: int = CONV_RGB, fetch_raw: bool = True,
                  use_graph: bool = True, stream: Optional[int] = None, single_stream: bool = False,
-                 precision: Optional[int] = None, batch: int = 1, source_outputs: Sequence[str] = ()):
+                 precision: Optional[int] = None, batch: int = 1, source_outputs: Sequence[str] = (),
+                 cameras: Optional[Dict[int, Sequence[int]]] = None):
         """dtype "fp16" | "bf16": 16-bit operands; dtype "fp32" (the reference's precision="fp32") selects the
         split-fp16 fp32-grade mode (precision=PREC_SPLIT on fp16 pairs).  batch > 1 (16-bit only): every call takes
         exactly `batch` frames, of one geometry (infer_batch / submit_batch / infer_device_batch) or each of its own
         size (infer_frames / submit_frames / infer_device_frames); sample k's outputs are raw(idx, k) / cls(idx, k).
         source_outputs: any of "mask", "depth", "overlay": every call also makes these results at each camera's own
-        resolution (source(idx, kind, k) / source_dev(idx, kind, k)); a kind no model makes is rejected."""
+        resolution (source(idx, kind, k) / source_dev(idx, kind, k)); a kind no model makes is rejected.
+        cameras: model index -> the samples that model runs on (its camera set, fixed for the engine's life; a model not
+        listed runs on every sample).  Every per-sample read (raw, cls, source, read_resized, taps "<m>/<name>@k",
+        lateral) keeps the sample index; a sample outside the model's set fails.  Models that share an encoder must
+        share their set."""
+        nb = max(1, batch)
+        masks = camera_masks(cameras, len(kinds), nb)
         self._lib = L.lib()
         cfg = L.EngineConfig()
         cfg.gpu_id, cfg.dtype = gpu_id, DTYPE_BY_NAME[dtype]
@@ -63,13 +94,17 @@ class Engine:
         cfg.precision = (PREC_SPLIT if dtype == "fp32" else PREC_16) if precision is None else precision
         cfg.batch = batch
         cfg.source_outputs = source_flags(source_outputs)
+        for m, mask in enumerate(masks):
+            cfg.cameras[m] = mask
         self._h = C.c_void_p()
         L.check(self._lib.vp_engine_create(C.byref(cfg), C.byref(self._h)), "vp_engine_create")
         self.kinds = list(kinds)
-        self.batch = max(1, batch)
+        self.batch = nb
+        self.cameras = [samples_of(mask, nb) for mask in masks]   # [model] its samples, slot by slot
         self.convention = convention
         self._rectify = {}
         self._detector = None
+        self._detector_samples = []
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -132,24 +167,51 @@ class Engine:
                 v.roi[k][:] = [x, y, w, h]
         L.check(self._lib.vp_engine_set_view(self._h, model_idx, C.byref(v)), "vp_engine_set_view")
 
-    def set_detector(self, det) -> None:
-        """Run the AutoSpeedEngine det (of this engine's batch and GPU) on every sample's whole frame inside every later
-        call, on a lane of its own (det None: detach).  After a host call det.detections(k) holds sample k's detections;
-        after a submit or device call: sync(), then det.sync().  The engine keeps det alive while it is attached, and
-        det.close() detaches it first."""
+    def set_detector(self, det, cameras: Optional[Sequence[int]] = None) -> None:
+        """Run the AutoSpeedEngine det (of this engine's GPU) on the whole frame of every sample, or of the samples in
+        `cameras`, inside every later call, on a lane of its own (det None: detach).  det's batch is the engine's, or
+        len(cameras): det's slot j holds the j-th of the sorted samples.  After a host call detections(k) /
+        detector_raw(k) hold sample k's results (det.detections(j) those of slot j); after a submit or device call:
+        sync(), then det.sync().  The engine keeps det alive while it is attached, and det.close() detaches it first."""
         from .autospeed import AutoSpeedEngine
+        mask = 0
+        if cameras is not None:
+            mask = camera_masks({0: cameras}, 1, self.batch)[0]
+        samples = samples_of(mask, self.batch)
         if det is not None:
             if not isinstance(det, AutoSpeedEngine):
                 raise TypeError(f"set_detector takes an AutoSpeedEngine or None, not {type(det).__name__}")
-            if det.batch != self.batch:
-                raise ValueError(f"the detector has batch {det.batch}, the engine batch {self.batch}")
-        L.check(self._lib.vp_engine_set_detector(self._h, det.handle if det is not None else None),
-                "vp_engine_set_detector")
+            if det.batch != len(samples):
+                if cameras is None:
+                    raise ValueError(f"the detector has batch {det.batch}, the engine batch {self.batch}")
+                raise ValueError(f"the detector has batch {det.batch}, the camera set {samples} has {len(samples)} "
+                                 f"samples")
+        handle = det.handle if det is not None else None
+        if cameras is None:
+            L.check(self._lib.vp_engine_set_detector(self._h, handle), "vp_engine_set_detector")
+        else:
+            L.check(self._lib.vp_engine_set_detector_cameras(self._h, handle, mask), "vp_engine_set_detector_cameras")
         if self._detector is not None:
             self._detector._engines.discard(self)
         if det is not None:
             det._engines.add(self)
         self._detector = det
+        self._detector_samples = samples
+
+    def _detector_slot(self, sample: int) -> int:
+        if self._detector is None:
+            raise RuntimeError("no detector is attached (set_detector)")
+        if sample not in self._detector_samples:
+            raise ValueError(f"the detector does not run on sample {sample} (its samples {self._detector_samples})")
+        return self._detector_samples.index(sample)
+
+    def detections(self, sample: int = 0) -> np.ndarray:
+        """The attached detector's detections of sample `sample` of the last call (its slot of the detector)."""
+        return self._detector.detections(self._detector_slot(sample))
+
+    def detector_raw(self, sample: int = 0) -> np.ndarray:
+        """The attached detector's raw tensor of sample `sample` of the last call (fetch_raw)."""
+        return self._detector.raw(self._detector_slot(sample))
 
     # ---- the lateral post-process inside the call
     def set_lateral(self, model_idx: Optional[int], threshold: float = 0.0, smoothing: float = 0.5,

@@ -77,7 +77,22 @@ typedef struct {
                                        VP_PREC_SPLIT with batch > 1 fails with VPB_ERR_ARG) */
   int source_outputs;               /* 0 (default) or VP_SRC_* flags: results at each camera's own resolution, made in
                                        the same call (vp_engine_source_output) */
+  int cameras[VP_MAX_MODELS];       /* per model, the samples it runs on (its camera set): bit k = sample k; 0 (default)
+                                       or every bit of the batch = every sample.  See "Camera sets" below. */
 } vp_engine_config;
+
+/* Camera sets (vp_engine_config.cameras), fixed when the engine is created.  Model i with a set runs on m_i =
+ * popcount(cameras[i]) samples: its activations, outputs and launches are those of a batch-m_i engine, and its slot j
+ * holds the sample with the j-th set bit.  Its network input is made by an op of its own, "preprocess/<i>" (the one a
+ * view makes, vp_engine_set_view), from each of its samples' frame after the JPEG decode and rectify, which still run
+ * once for every sample; the engine's shared "preprocess" is left out when every model has a set.  Every read stays
+ * addressed by sample (vp_engine_output_at, vp_engine_source_output, vp_engine_read_resized_view, the taps
+ * "<i>/<name>@k", vp_engine_lateral, vp_engine_lateral_reset): a sample outside the model's set returns VPB_ERR_ARG
+ * naming the model and the sample.  The in-call lateral op on a model with a set keeps one state per sample of the set;
+ * vp_lateral_config.homographies and vp_engine_set_steering stay indexed by sample (values of other samples are not
+ * read).  vp_engine_create returns VPB_ERR_ARG, naming the model, before any device work for a bit at or above the
+ * batch, or for sets that differ between models sharing an encoder (byte-identical encoder weights; DomainSeg also
+ * shares SceneSeg's context and neck). */
 
 /* Source-resolution outputs (vp_engine_config.source_outputs), what each model makes of a flag:
  *   VP_SRC_MASK     SceneSeg / DomainSeg: uint8 mask 255 / 0 (createMaskKernel's rule); EgoLanes: uint8 ids {0,1,2,255}
@@ -221,6 +236,11 @@ int vp_engine_read_resized_view(vp_engine* e, int model_idx, int sample, uint8_t
  * batch 1) attaches to any batch-1 engine, 16-bit or split; its copied ops are its split launches and det/letterbox
  * writes its canvas low half.  VPB_ERR_ARG for a NULL engine, or a detector of another batch or GPU. */
 int vp_engine_set_detector(vp_engine* e, struct vp_autospeed* det);
+/* The same on the samples of the bit mask `cameras` only (0: every sample, exactly vp_engine_set_detector): det's batch
+ * is popcount(cameras), and det/letterbox reads the whole frame of the sample with the j-th set bit into det's slot j,
+ * so vp_autospeed_detections_at(det, j, ...) and _raw_at are slot j.  VPB_ERR_ARG for a NULL engine, a bit at or above
+ * the engine's batch, a detector whose batch is not popcount(cameras) (naming both), or one on another GPU. */
+int vp_engine_set_detector_cameras(vp_engine* e, struct vp_autospeed* det, int cameras);
 
 /* The lateral post-process inside the call (production_release/main.cpp:505-577: EgoLanes -> LaneFilter ->
  * LaneTracker -> PathFinder, per camera).  With it set on EgoLanes model model_idx, every later call of every form

@@ -98,7 +98,8 @@ int vp_autospeed_sync(vp_autospeed* e, int fetch);
 int vp_autospeed_detections(vp_autospeed* e, const float** det, int* n, int* n_candidates);
 /* raw prediction tensor, fp32 planar [channels = 8][anchors = 10752]: cx, cy, w, h (canvas pixels), 4 class scores */
 int vp_autospeed_raw(vp_autospeed* e, const float** raw_host, const float** raw_dev, int* channels, int* anchors);
-/* the same for sample 0..batch-1 (the two calls above return sample 0) */
+/* the same for sample 0..batch-1 (the two calls above return sample 0); for a detector attached to a segmentation
+ * engine with vp_engine_set_detector_cameras, `sample` is the detector's slot j: the engine's sample with the j-th set bit */
 int vp_autospeed_detections_at(vp_autospeed* e, int sample, const float** det, int* n, int* n_candidates);
 int vp_autospeed_raw_at(vp_autospeed* e, int sample, const float** raw_host, const float** raw_dev, int* channels,
                         int* anchors);
